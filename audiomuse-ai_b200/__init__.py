@@ -1,4 +1,4 @@
-"""audiomuse-ai_b200: B200-native (sm_100a) replacement for AudioMuse-AI's CLAP analysis hot
+"""audiomuse-ai_b200: H100-native (sm_90a) replacement for AudioMuse-AI's CLAP analysis hot
 path and its downstream k-NN / k-means, behind the reference's own Python call surface.
 
 Import name: ``audiomuse_ai_b200`` (see the loader stub ``audiomuse_ai_b200.py`` at the repo

@@ -111,10 +111,7 @@ DEBUG_LIB_PATH = os.path.join(_PKG_DIR, "libaudiomuse_b200_debug.so")
 DEBUG_SIGNATURES = {
     "am_selftest_gemm": (_i, [_i, _i, _i, _i, _P(C.c_double)]),
     "am_bench_gemm": (_i, [_i, _i, _i, _i, _P(C.c_double)]),
-    "am_probe_mma": (_i, [_i, _i, _i, _i, _P(C.c_double), _P(C.c_double)]),
-    "am_probe_tmem_ld": (_i, [_i, _i, _i, _i, _i, _P(C.c_double), _P(C.c_double)]),
     "am_probe_pipe": (_i, [_i, _i, _i, _P(C.c_double)]),
-    "am_probe_mn_major": (_i, [C.c_void_p, C.c_void_p, _i, _i, _i, _i, _i, _i, C.c_void_p]),
 }
 
 _lib = None

@@ -1,4 +1,4 @@
-"""Mirror of the MusiCNN spectrogram front end of ``tasks/analysis.py:368-391`` on the B200 mel kernel (SURVEY 8(f)
+"""Mirror of the MusiCNN spectrogram front end of ``tasks/analysis.py:368-391`` on the GPU mel kernel (SURVEY 8(f)
 row 4: a sibling tower sharing K1's machinery).
 
     musicnn_patches(audio, sr=16000) -> float32 (n_patches, 187, 96) | None

@@ -1,4 +1,4 @@
-"""Builds libaudiomuse_b200.so (sm_100a) in-tree with nvcc.  No JIT cache: the .so sits next
+"""Builds libaudiomuse_b200.so (sm_90a) in-tree with nvcc.  No JIT cache: the .so sits next
 to this file so it travels to the GPU box with the repo snapshot."""
 from __future__ import annotations
 
@@ -15,7 +15,7 @@ LIB = os.path.join(PKG_DIR, "libaudiomuse_b200.so")
 DEBUG_LIB = os.path.join(PKG_DIR, "libaudiomuse_b200_debug.so")   # product objects + csrc/debug/*.cu (probes, self tests)
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC,-fvisibility=hidden", "--expt-relaxed-constexpr",
 ]
 
@@ -55,7 +55,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
 
     def compile_one(job):
         src, obj = job
-        # AM_EXTRA_NVCC_FLAGS: debug builds on the GPU box (tools/gpu_trace.sh adds -DAM_FUSED_TRACE_BUILD)
+        # AM_EXTRA_NVCC_FLAGS: extra flags for debug builds (e.g. -DNDEBUG=0 -G)
         cmd = [nvcc, *NVCC_FLAGS, *os.environ.get("AM_EXTRA_NVCC_FLAGS", "").split(), "-c", src, "-o", obj]
         if verbose:
             cmd.insert(1, "-Xptxas=-v")
@@ -74,7 +74,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
         os.remove(os.path.join(BUILD, o))
     for lib, members in ((LIB, objs), (DEBUG_LIB, objs + dbg_objs)):
         if jobs or stale or not os.path.exists(lib):
-            cmd = [nvcc, "-shared", "-o", lib, *members, "-gencode", "arch=compute_100a,code=sm_100a",
+            cmd = [nvcc, "-shared", "-o", lib, *members, "-gencode", "arch=compute_90a,code=sm_90a",
                    "-Xcompiler", "-fPIC"]
             r = subprocess.run(cmd, capture_output=True, text=True)
             if r.returncode != 0:

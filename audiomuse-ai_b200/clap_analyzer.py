@@ -1,4 +1,4 @@
-"""Host-side mirror of the reference's ``tasks/clap_analyzer.py`` audio path on the B200 library.
+"""Host-side mirror of the reference's ``tasks/clap_analyzer.py`` audio path on the GPU library.
 
 Same names, argument meaning and error behaviour as the reference functions they replace:
 
@@ -291,10 +291,10 @@ def _load_audio_model() -> bool:
             return False
         try:
             _audio_session = B200Session.from_file(path)
-            logger.info(f"CLAP audio model loaded on B200 from {path}")
+            logger.info(f"CLAP audio model loaded on the GPU from {path}")
             return True
         except Exception as e:
-            logger.error(f"Failed to load CLAP audio model on B200: {e}")
+            logger.error(f"Failed to load CLAP audio model on the GPU: {e}")
             _audio_session = None
             return False
 

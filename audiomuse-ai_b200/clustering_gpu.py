@@ -1,4 +1,4 @@
-"""Mirror of ``tasks/clustering_gpu.py`` (KMeans rows of SURVEY 8(a)) on the B200 library.
+"""Mirror of ``tasks/clustering_gpu.py`` (KMeans rows of SURVEY 8(a)) on the GPU library.
 
     check_gpu_available()                      tasks/clustering_gpu.py:26-79
     GPUKMeans(n_clusters, init, n_init, random_state).fit_predict(X)   :82-148
@@ -34,7 +34,7 @@ def check_gpu_available() -> bool:
     try:
         return _lib.load().am_init(-1) == _lib.AM_OK
     except Exception as e:
-        logger.info(f"B200 library unavailable: {e}")
+        logger.info(f"GPU library unavailable: {e}")
         return False
 
 
@@ -167,7 +167,7 @@ def pca_fit(X, n_components):
 
 
 class GPUPCA:
-    """tasks/clustering_gpu.py:201-277 (cuml.decomposition.PCA -> the B200 library; float n_components in (0, 1) selects
+    """tasks/clustering_gpu.py:201-277 (cuml.decomposition.PCA -> the GPU library; float n_components in (0, 1) selects
     the smallest number of components explaining that share of the variance, as scikit-learn does)."""
 
     def __init__(self, n_components):

@@ -80,8 +80,8 @@ extern "C" int am_init(int device_ordinal) {
   AM_CUDA(cudaGetDevice(&dev));
   cudaDeviceProp p;
   AM_CUDA(cudaGetDeviceProperties(&p, dev));
-  if (p.major != 10) {
-    set_error("device %d is sm_%d%d; this library is built for sm_100a (B200) only", dev, p.major, p.minor);
+  if (p.major != 9 || p.minor != 0) {
+    set_error("device %d is sm_%d%d; this library is built for sm_90a (H100) only", dev, p.major, p.minor);
     return AM_ERR_NO_DEVICE;
   }
   g_sms = p.multiProcessorCount;

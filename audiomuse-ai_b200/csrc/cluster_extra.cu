@@ -1,7 +1,7 @@
 // PCA and DBSCAN for the clustering task (SURVEY 8(f4); tasks/clustering_gpu.py:151-278: cuml.decomposition.PCA and
 // cuml.cluster.DBSCAN with scikit-learn as the fallback -- scikit-learn's results are the bar).
 //
-// PCA   am_pca_moments: column means + covariance (n - 1 normalisation), accumulated in float64 on the device -- B200 has
+// PCA   am_pca_moments: column means + covariance (n - 1 normalisation), accumulated in float64 on the device -- H100 has
 //       FP64 to spare (N d^2 DFMA: 2.6e10 for 100 k x 512) and the eigenvectors of a float32 covariance would not match
 //       LAPACK's to better than 1e-4.  The d x d eigenproblem stays on the host (numpy / LAPACK, like the reference's
 //       Python); am_pca_project applies (X - mean) W^T on the device.

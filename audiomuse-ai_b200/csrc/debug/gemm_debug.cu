@@ -1,14 +1,14 @@
-// Debug entry points of the tcgen05 GEMM (NOT part of libaudiomuse_b200.so: built into libaudiomuse_b200_debug.so,
+// Debug entry points of the wgmma GEMM (NOT part of libaudiomuse_b200.so: built into libaudiomuse_b200_debug.so,
 // declared in include/audiomuse_b200_debug.h; used by tests/test_gpu_gemm.py and tools/gemm_bench.py).
 #include "../common.cuh"
-#include "../gemm_tcgen05.cuh"
+#include "../gemm_wgmma.cuh"
 #include "../../../include/audiomuse_b200_debug.h"
 
 #include <cmath>
 #include <vector>
 
 // ---------------------------------------------------------------- on-device self test (debug C ABI)
-// Runs the tcgen05 kernel and the SIMT reference on seeded bf16 operands and returns the
+// Runs the wgmma kernel and the SIMT reference on seeded bf16 operands and returns the
 // largest |difference| through *max_abs_diff.  flags: bit0 bias, bit1 relu6, bit2 residual,
 // bit3 fp32 output, bit4 m_fastest, bit5 col_sub with alpha = 2.
 extern "C" AM_API int am_selftest_gemm(int M, int N, int K, int flags, double* max_abs_diff) {

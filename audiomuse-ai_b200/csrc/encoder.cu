@@ -1,4 +1,4 @@
-// K2 + K3: student CLAP audio encoder, batched (sm_100a).
+// K2 + K3: student CLAP audio encoder, batched (sm_90a).
 //
 // Replaces the per-segment onnxruntime call of tasks/clap_analyzer.py:534 and the numpy pooling
 // at :552-562.  Architecture: student_clap/models/student_onnx_model.py (bn0 over mel bins ->
@@ -7,7 +7,7 @@
 //
 // Data layout in HBM: activations are NHWC bf16 [B, H, W, Cp] with Cp = channels rounded up to 16
 // (padded channels are exact zeros: zero weight rows + zero bias), so every 1x1 convolution is
-// one K-major GEMM  D[B*H*W, Cout] = A[B*H*W, Cin] x W[Cout, Cin]^T  on the tcgen05 path
+// one K-major GEMM  D[B*H*W, Cout] = A[B*H*W, Cin] x W[Cout, Cin]^T  on the wgmma path
 // (gemm.cu) with the folded-BatchNorm bias, ReLU6 and the residual add fused in its epilogue.
 // Depthwise 3x3 (+BN+ReLU6) is a bandwidth kernel over 8-channel (16-byte) vectors.  The stem
 // (bn0 + pad + 3x3 stride-2 on the single input channel + 1x1 + BN + ReLU6) reads the fp32
@@ -23,7 +23,7 @@
 
 #include "encoder_generic.cuh"
 #include "fused_block.cuh"
-#include "gemm_tcgen05.cuh"
+#include "gemm_wgmma.cuh"
 #include "model_spec.cuh"
 
 namespace am {
@@ -36,13 +36,10 @@ struct Layer {
   int pad_t = 0, pad_b = 0, pad_l = 0, pad_r = 0;
   int h_is_time = 1, gate_act = 0, cmid = 0;
   DevBuf<__nv_bfloat16> w_bf16;  // pointwise: [cout_p, cin_p]
-  DevBuf<__half> w_f16;          // projection (act == 0) pointwise, same layout: the fused block's MMA2 runs fp16 x fp16
-  DevBuf<uint32_t> tpack;        // depthwise of a block with an expansion conv: fusedt::pack_consts (taps, biases)
-  DevBuf<__nv_bfloat16> w1s;     // stem: [cout_p, 16] rows (s_hi, s_hi, s_lo, t_hi, t_lo, 0 ...), the stem as an expansion GEMM (stem_x0_kernel)
   DevBuf<float> w_f32;           // depthwise: [k*k, c_p]; stem: dw[9]; first conv: [kh*kw, c_p]; squeeze-excite: fc1 [cmid, c]
   DevBuf<float> bias;            // [cout_p]  (squeeze-excite: fc1 bias [cmid])
   DevBuf<float> aux0, aux1, aux2;  // stem / first conv: per-mel scale / shift (+ stem pw scale); squeeze-excite: fc2 [c, cmid], fc2 bias
-  // true for the 3x3 / pad 1 / ReLU6 depthwise the packed-fp16 kernels and the fused block kernel implement
+  // true for the 3x3 / pad 1 / ReLU6 depthwise the packed-fp16 kernels implement
   bool dw_fast() const {
     return type == kDepthwise && kh == 3 && kw == 3 && pad_t == 1 && pad_b == 1 && pad_l == 1 && pad_r == 1 && act == kActRelu6;
   }
@@ -60,7 +57,7 @@ struct HeadOp {
 static inline int pad16(int c) { return (int)round_up((size_t)c, 16); }
 
 // ---------------------------------------------------------------- kernels
-// stem: mel f32 [B, n_mels, T] -> NHWC 16-bit [B, Ho, Wo, Cp];  image H = time, W = mel bin.
+// stem: mel f32 [B, n_mels, T] -> NHWC bf16 [B, Ho, Wo, Cp];  image H = time, W = mel bin.
 // A CTA owns a tile of 32 output rows (time) x 8 output columns (mel) of one window.
 //   phase 1: one thread per pixel computes the single-channel 3x3 stride-2 response; lanes of a warp
 //            walk the TIME axis (contiguous in the mel layout), so each tap is a 256-byte strided read
@@ -69,7 +66,6 @@ static inline int pad16(int c) { return (int)round_up((size_t)c, 16); }
 //            16-byte groups (8 pixels x Cp x 2 B contiguous runs per output row).
 constexpr int kStemTH = 32, kStemTW = 8;
 
-template <bool kHalfOut>
 __global__ void __launch_bounds__(256)
 stem_kernel(const float* __restrict__ mel, int B, int n_mels, int T, int Ho, int Wo, int pad_t, int pad_l,
             const float* __restrict__ bn_scale, const float* __restrict__ bn_shift,
@@ -152,81 +148,13 @@ stem_kernel(const float* __restrict__ mel, int B, int n_mels, int T, int Ho, int
 #pragma unroll
       for (int e = 0; e < 8; ++e) o8[e] = relu6f(fmaf(v, sc[e], sh[e]));
       uint4 pk;
-      if constexpr (kHalfOut) {  // consumed only by the fused first block, whose depthwise runs in fp16
-        __half2 t;
-        t = __floats2half2_rn(o8[0], o8[1]); pk.x = *reinterpret_cast<uint32_t*>(&t);
-        t = __floats2half2_rn(o8[2], o8[3]); pk.y = *reinterpret_cast<uint32_t*>(&t);
-        t = __floats2half2_rn(o8[4], o8[5]); pk.z = *reinterpret_cast<uint32_t*>(&t);
-        t = __floats2half2_rn(o8[6], o8[7]); pk.w = *reinterpret_cast<uint32_t*>(&t);
-      } else {
-        __nv_bfloat162 t;
-        t = __floats2bfloat162_rn(o8[0], o8[1]); pk.x = *reinterpret_cast<uint32_t*>(&t);
-        t = __floats2bfloat162_rn(o8[2], o8[3]); pk.y = *reinterpret_cast<uint32_t*>(&t);
-        t = __floats2bfloat162_rn(o8[4], o8[5]); pk.z = *reinterpret_cast<uint32_t*>(&t);
-        t = __floats2bfloat162_rn(o8[6], o8[7]); pk.w = *reinterpret_cast<uint32_t*>(&t);
-      }
+      __nv_bfloat162 t;
+      t = __floats2bfloat162_rn(o8[0], o8[1]); pk.x = *reinterpret_cast<uint32_t*>(&t);
+      t = __floats2bfloat162_rn(o8[2], o8[3]); pk.y = *reinterpret_cast<uint32_t*>(&t);
+      t = __floats2bfloat162_rn(o8[4], o8[5]); pk.z = *reinterpret_cast<uint32_t*>(&t);
+      t = __floats2bfloat162_rn(o8[6], o8[7]); pk.w = *reinterpret_cast<uint32_t*>(&t);
       const int64_t pix = ((int64_t)b * Ho + ho0 + hl) * Wo + wo0 + wl;
       *reinterpret_cast<uint4*>(out + (pix * groups + g) * 8) = pk;
-      }
-    }
-  }
-}
-
-// stem, first half only: the single-channel 3x3 stride-2 response v per output pixel, written as the 16-column bf16
-// row  (v_hi, v_lo, v_hi, 1, 1, 0 ...)  of a [B, Ho, Wo, 16] tensor.  The channel-per-lane fused block then produces the
-// stem's per-channel affine + ReLU6 as its "expansion" GEMM against rows (s_hi, s_hi, s_lo, t_hi, t_lo, 0 ...):
-// v s + t to fp32-class accuracy on the tensor pipe (split bf16), and the 144-channel stem output never exists in HBM
-// (it was 2.4 GB written + read per 256 windows).  Same tile walk as stem_kernel phase 1.
-__global__ void __launch_bounds__(256)
-stem_x0_kernel(const float* __restrict__ mel, int B, int n_mels, int T, int Ho, int Wo, int pad_t, int pad_l,
-               const float* __restrict__ bn_scale, const float* __restrict__ bn_shift, const float* __restrict__ dw,
-               __nv_bfloat16* __restrict__ out) {
-  __shared__ float s_v[kStemTH * kStemTW];
-  const int tiles_h = (Ho + kStemTH - 1) / kStemTH, tiles_w = (Wo + kStemTW - 1) / kStemTW;
-  const int64_t n_tiles = (int64_t)B * tiles_h * tiles_w;
-  float wdw[9];
-#pragma unroll
-  for (int i = 0; i < 9; ++i) wdw[i] = __ldg(&dw[i]);
-  for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-    const int tw = (int)(tile % tiles_w);
-    const int64_t t1 = tile / tiles_w;
-    const int th = (int)(t1 % tiles_h);
-    const int b = (int)(t1 / tiles_h);
-    const int ho0 = th * kStemTH, wo0 = tw * kStemTW;
-    __syncthreads();
-    {
-      const int hl = threadIdx.x & (kStemTH - 1), wl = threadIdx.x / kStemTH;  // lanes walk the time axis
-      const int ho = ho0 + hl, wo = wo0 + wl;
-      float v = 0.f;
-      if (ho < Ho && wo < Wo) {
-        const float* m = mel + (int64_t)b * n_mels * T;
-#pragma unroll
-        for (int dx = 0; dx < 3; ++dx) {
-          const int w = 2 * wo + dx - pad_l;
-          if (w < 0 || w >= n_mels) continue;
-          const float bsc = __ldg(&bn_scale[w]), bsh = __ldg(&bn_shift[w]);
-#pragma unroll
-          for (int dy = 0; dy < 3; ++dy) {
-            const int h = 2 * ho + dy - pad_t;
-            if (h < 0 || h >= T) continue;
-            v = fmaf(wdw[dy * 3 + dx], fmaf(__ldg(&m[(int64_t)w * T + h]), bsc, bsh), v);
-          }
-        }
-      }
-      s_v[hl * kStemTW + wl] = v;
-    }
-    __syncthreads();
-    {
-      const int hl = threadIdx.x >> 3, wl = threadIdx.x & 7;   // consecutive threads = consecutive pixels of a row: 256 B runs
-      const int ho = ho0 + hl, wo = wo0 + wl;
-      if (ho < Ho && wo < Wo) {
-        const float v = s_v[hl * kStemTW + wl];
-        const __nv_bfloat16 hi = __float2bfloat16_rn(v);
-        const __nv_bfloat16 lo = __float2bfloat16_rn(v - __bfloat162float(hi));
-        const uint32_t uh = (uint32_t)__bfloat16_as_ushort(hi), ul = (uint32_t)__bfloat16_as_ushort(lo);
-        uint4* dst = reinterpret_cast<uint4*>(out + (((int64_t)b * Ho + ho) * Wo + wo) * 16);
-        dst[0] = make_uint4(uh | (ul << 16), uh | (0x3f80u << 16), 0x3f80u, 0u);   // v_hi v_lo | v_hi 1 | 1 0 | 0 0
-        dst[1] = make_uint4(0u, 0u, 0u, 0u);
       }
     }
   }
@@ -271,7 +199,7 @@ depthwise_kernel(const __nv_bfloat16* __restrict__ in, int B, int H, int W, int 
   const int ho0 = strip * kDwRows;
   const int nrows = min(kDwRows, Ho - ho0);
 
-  // packed fp16 arithmetic (HFMA2), like the depthwise stage of the fused blocks: inputs are post-ReLU6
+  // packed fp16 arithmetic (HFMA2): inputs are post-ReLU6
   // (|x| <= 6, bf16 -> fp16 is exact there), 9 taps; half the FMAs and half the weight registers of fp32
   __half2 wt[9][4];
 #pragma unroll
@@ -557,7 +485,7 @@ static int launch_linear(const float* x, int B, int K, const float* W, const flo
 // fp32 -> three bf16 terms so that ONE bf16 tensor-core GEMM over K' = 3*Kp reproduces the fp32 product to ~2^-16:
 //   x = hi + lo (+ 2^-17 x),  A' = [hi | hi | lo],  W' = [hi | lo | hi]  =>  A'.W'^T = hi.hi + hi.lo + lo.hi
 // (the dropped lo.lo term is 2^-18).  The head's three linears are 0.7 GFLOP in total: on CUDA cores they were
-// latency bound at 0.45 ms, as split-bf16 GEMMs on the tcgen05 kernel they are a few microseconds each.
+// latency bound at 0.45 ms, as split-bf16 GEMMs on the wgmma kernel they are a few microseconds each.
 __global__ void __launch_bounds__(256)
 split3_kernel(const float* __restrict__ x, int B, int K, int Kp, int in_act, __nv_bfloat16* __restrict__ out) {
   const int64_t n = (int64_t)B * Kp;
@@ -729,7 +657,7 @@ struct am_model {
   am::DevBuf<__nv_bfloat16> act[3];
   am::DevBuf<float> mel_ws, seg_emb, se_mean, se_gate;
   am::DevBuf<__nv_bfloat16> a3;       // head GEMM operand [n, 3 * Kp] (split3_kernel)
-  am::DevBuf<__nv_bfloat16> late_in;  // [n, H, W, C] output of the early (fused) blocks for all windows of a call
+  am::DevBuf<__nv_bfloat16> late_in;  // [n, H, W, C] output of the early layers for all windows of a call
   int late_sub = 256;                 // windows per pass of the late phase
   size_t act_elems = 0;
   int max_sub = 256;         // windows per pass of the early (chunked) phase (256 measured 1 % faster than 128)
@@ -753,11 +681,7 @@ struct am_model {
   am_mel_plan* host_plan = nullptr;  // mel plan of the host entry point, cached per cfg (building one = host trig
   am_mel_cfg host_plan_cfg{};        // tables + cudaMalloc + upload: ~1 ms, was paid on every call)
   int use_simt_gemm = 0;     // debug: AM_GEMM_IMPL=simt
-  struct Block {             // inverted-residual block = [expand] depthwise project
-    int first = 0, expand = -1, dw = 0, proj = 0;
-  };
-  std::vector<Block> blocks;
-  unsigned fused_mask = 0xffffffffu;   // AM_FUSED_BLOCKS: bit i = fuse block i when it fits on chip
+  int fused_blocks = 1;      // AM_FUSED_BLOCKS=0: every block layer by layer (fused_block.cu otherwise)
   ~am_model() {
     for (int i = 0; i < 2; ++i) {
       if (ev_copied[i]) cudaEventDestroy(ev_copied[i]);
@@ -995,13 +919,6 @@ static int build_model(am_model* m, const ModelSpec& spec) {
       for (int o = 0; o < S.cout; ++o)
         for (int i = 0; i < S.cin; ++i) wb[(size_t)o * L->cin_p + i] = __float2bfloat16_rn(S.w[(size_t)o * S.cin + i]);
       AM_TRY(upload(L->w_bf16, wb));
-      if (S.act == kActNone) {  // fp16 copy, saturated to the fp16 range (folded weights are O(1))
-        std::vector<__half> wh((size_t)L->cout_p * L->cin_p, __float2half_rn(0.f));
-        for (int o = 0; o < S.cout; ++o)
-          for (int i = 0; i < S.cin; ++i)
-            wh[(size_t)o * L->cin_p + i] = __float2half_rn(std::min(65504.f, std::max(-65504.f, S.w[(size_t)o * S.cin + i])));
-        AM_TRY(upload(L->w_f16, wh));
-      }
       AM_TRY(upload(L->bias, padded(S.bias, L->cout_p)));
     } else if (S.type == kDepthwise) {
       const int taps = S.kh * S.kw;
@@ -1097,59 +1014,6 @@ static int build_model(am_model* m, const ModelSpec& spec) {
     set_error("weights: the head must start with the spatial pooling and end with the %d-d embedding", m->emb);
     return AM_ERR_IO;
   }
-  // group layers into inverted-residual blocks for the fused kernel: [1x1 expand + ReLU6] -> 3x3 dw + ReLU6 -> linear 1x1
-  for (size_t i = 1; i < m->layers.size();) {
-    const Layer& l = *m->layers[i];
-    am_model::Block blk;
-    blk.first = (int)i;
-    if (l.type == kPointwise && l.block_start && l.act == kActRelu6 && i + 2 < m->layers.size() + 0 &&
-        m->layers[i + 1]->dw_fast() && m->layers[i + 2]->type == kPointwise && m->layers[i + 2]->act == kActNone) {
-      blk.expand = (int)i;
-      blk.dw = (int)i + 1;
-      blk.proj = (int)i + 2;
-      {  // constants of the channel-per-lane fused kernel (fused_block_t.cu), packed once
-        Layer& dwl = *m->layers[i + 1];
-        AM_TRY(dwl.tpack.alloc(fusedt::consts_words(dwl.cin_p)));
-        AM_TRY(fusedt::pack_consts(dwl.w_f32.p, dwl.bias.p, l.bias.p, dwl.cin_p, dwl.tpack.p, nullptr));
-        AM_CUDA(cudaStreamSynchronize(nullptr));
-      }
-      m->blocks.push_back(blk);
-      i += 3;
-    } else if (l.dw_fast() && l.block_start && i + 1 < m->layers.size() && m->layers[i + 1]->type == kPointwise &&
-               m->layers[i + 1]->act == kActNone) {
-      blk.dw = (int)i;
-      blk.proj = (int)i + 1;
-      if (i == 1 && m->layers[0]->type == kStem) {
-        // block 0 behind the rank-1 stem: the stem's per-channel scale / shift become expansion weights over the
-        // (v_hi, v_lo, v_hi, 1, 1) rows stem_x0_kernel writes, and the block runs on the channel-per-lane kernel
-        Layer& stem = *m->layers[0];
-        Layer& dwl = *m->layers[i];
-        const auto& S0 = spec.layers[0];
-        std::vector<__nv_bfloat16> w1((size_t)stem.cout_p * 16, __float2bfloat16_rn(0.f));
-        for (int c = 0; c < S0.cout; ++c) {
-          const float sc = S0.aux2[(size_t)c], sh = S0.bias[(size_t)c];
-          const __nv_bfloat16 sch = __float2bfloat16_rn(sc), shh = __float2bfloat16_rn(sh);
-          __nv_bfloat16* r = &w1[(size_t)c * 16];
-          r[0] = sch;
-          r[1] = sch;
-          r[2] = __float2bfloat16_rn(sc - __bfloat162float(sch));
-          r[3] = shh;
-          r[4] = __float2bfloat16_rn(sh - __bfloat162float(shh));
-        }
-        AM_TRY(upload(stem.w1s, w1));
-        DevBuf<float> zeros;
-        AM_TRY(zeros.alloc((size_t)dwl.cin_p));
-        AM_CUDA(cudaMemset(zeros.p, 0, (size_t)dwl.cin_p * 4));
-        AM_TRY(dwl.tpack.alloc(fusedt::consts_words(dwl.cin_p)));
-        AM_TRY(fusedt::pack_consts(dwl.w_f32.p, dwl.bias.p, zeros.p, dwl.cin_p, dwl.tpack.p, nullptr));
-        AM_CUDA(cudaStreamSynchronize(nullptr));
-      }
-      m->blocks.push_back(blk);
-      i += 2;
-    } else {
-      ++i;
-    }
-  }
   return AM_OK;
 }
 
@@ -1158,53 +1022,56 @@ static int grid_for(int64_t total_threads) {
   return (int)std::max<int64_t>(1, std::min<int64_t>(blocks, (int64_t)sm_count() * 16));
 }
 
-// fused-kernel description of block `bi` at input shape `s` (plan() decides whether it fits on chip)
-static bool block_desc(const am_model* m, int bi, Shape s, bool stem_fp16, fused::BlockDesc* d, fused::Plan* pl) {
-  if (m->use_simt_gemm || !((m->fused_mask >> bi) & 1u)) return false;
-  const am_model::Block& blk = m->blocks[bi];
-  const Layer& dwl = *m->layers[blk.dw];
-  const Layer& pj = *m->layers[blk.proj];
-  *d = fused::BlockDesc{};
-  d->H = s.H;
-  d->W = s.W;
-  d->cin_p = blk.expand >= 0 ? m->layers[blk.expand]->cin_p : dwl.cin_p;
-  d->cmid_p = dwl.cin_p;
-  d->cout_p = pj.cout_p;
-  d->stride = dwl.stride;
-  d->has_expand = blk.expand >= 0 ? 1 : 0;
-  d->residual = pj.residual;
-  d->x_is_fp16 = (bi == 0 && stem_fp16) ? 1 : 0;
-  return fused::plan(*d, pl);
-}
+// The trunk runs in two phases.  EARLY = stem + the leading layers whose input maps are large (at least
+// kEarlyMinPositions positions per window): processed chunk by chunk, so host->device copies of the next chunk hide
+// under it and one chunk already fills the GPU.  LATE = everything after (small tensors): processed ONCE for all
+// windows of the call, so the deep, narrow layers get full-size grids.  The split falls on a block boundary (a
+// residual add reads its block's input).  late_start() is the first layer of the late phase.
+constexpr int64_t kEarlyMinPositions = 4096;
 
-static int block_index_at(const am_model* m, size_t layer) {
-  for (size_t q = 0; q < m->blocks.size(); ++q)
-    if (m->blocks[q].first == (int)layer) return (int)q;
-  return -1;
-}
-
-// The trunk runs in two phases.  EARLY = stem + the leading run of blocks that execute fused (huge
-// spatial extent): processed chunk by chunk, so host->device copies of the next chunk hide under it.
-// LATE = everything after (small tensors): processed ONCE for all windows of the call, so the deep,
-// narrow layers get full-size grids.  late_start() is the first layer of the late phase.
 static size_t late_start(const am_model* m, int T, Shape* s_split, int* c_split) {
   Shape s = stem_out(*m->layers[0], T, m->n_mels);
   int c = m->layers[0]->cout_p;
   size_t i = 1;
   while (i < m->layers.size()) {
-    const int bi = block_index_at(m, i);
-    if (bi < 0) break;
-    fused::BlockDesc d;
-    fused::Plan pl;
-    // x_is_fp16 does not influence plan(); pass false
-    if (!block_desc(m, bi, s, false, &d, &pl)) break;
-    s = dw_out(*m->layers[m->blocks[bi].dw], s);
-    c = m->layers[m->blocks[bi].proj]->cout_p;
-    i = (size_t)m->blocks[bi].proj + 1;
+    const Layer& l = *m->layers[i];
+    if (l.block_start && (int64_t)s.H * s.W < kEarlyMinPositions) break;
+    s = layer_out(l, s);
+    c = l.cout_p;
+    ++i;
   }
   *s_split = s;
   *c_split = c;
   return i;
+}
+
+// Layers from `i` (a block start) form an inverted-residual block the fused kernel runs: [1x1 expand + ReLU6] ->
+// 3x3 depthwise + ReLU6 -> linear 1x1, all inside [i, hi) and fitting fused::plan at input shape `s`.
+static bool fused_block_at(const am_model* m, size_t i, size_t hi, Shape s, fused::BlockDesc* d, fused::Plan* pl,
+                           int* ex, int* dw, int* pj) {
+  const auto& L = m->layers;
+  if (m->use_simt_gemm || !m->fused_blocks || !L[i]->block_start) return false;
+  int e = -1;
+  size_t k = i;
+  if (L[k]->type == kPointwise && L[k]->act == kActRelu6 && L[k]->stride == 1) e = (int)k++;
+  if (k + 1 >= hi || k + 1 >= L.size()) return false;
+  const Layer& D = *L[k];
+  const Layer& P = *L[k + 1];
+  if (!D.dw_fast() || P.type != kPointwise || P.act != kActNone || P.stride != 1 || P.cin_p != D.cin_p) return false;
+  if (e >= 0 && L[(size_t)e]->cout_p != D.cin_p) return false;
+  *d = fused::BlockDesc{};
+  d->H = s.H;
+  d->W = s.W;
+  d->cin_p = e >= 0 ? L[(size_t)e]->cin_p : D.cin_p;
+  d->cmid_p = D.cin_p;
+  d->cout_p = P.cout_p;
+  d->stride = D.stride;
+  d->has_expand = e >= 0 ? 1 : 0;
+  d->residual = P.residual;
+  *ex = e;
+  *dw = (int)k;
+  *pj = (int)k + 1;
+  return fused::plan(*d, pl);
 }
 
 // Runs layers [lo, hi) on `nb` windows.  lo == 0: starts from the log-mel (stem); else from `in` (shape s_in).
@@ -1222,48 +1089,16 @@ static int run_range(am_model* m, const float* mel_dev, const __nv_bfloat16* in,
     return nullptr;
   };
   size_t i = lo;
-  bool stem_fp16 = false;
-  bool stem_x0 = false;        // the stem was written as its rank-1 factor: block 0 runs it as an expansion GEMM
-  fused::BlockDesc d0{};
-  fusedt::Plan plt0;
   if (lo == 0) {
     const Layer& stem = *m->layers[0];
     s = stem_out(stem, T, m->n_mels);
     AM_CHECK(s.H > 0 && s.W > 0, "encoder: input of %d frames x %d mels is too small", T, m->n_mels);
     __nv_bfloat16* dst = pick_dst(hi == 1);
     if (stem.type == kStem) {
-      // the stem feeds only the first block; when that block runs fused its depthwise wants fp16 input
-      if (!m->blocks.empty() && m->blocks[0].first == 1 && m->blocks[0].expand < 0 && hi > 1) {
-        fused::BlockDesc d;
-        fused::Plan pl;
-        stem_fp16 = block_desc(m, 0, s, false, &d, &pl);
-        // Opt-in (AM_STEM_X0=1): measured on B200 the stem-as-expansion-GEMM route is slower for the shipped student
-        // (144 channels = one full 128-lane chunk + a 16-channel one that costs as much: 11.0 k cycles per tile against
-        // 7.8 k for the pixel-per-lane kernel + the stem kernel's 0.5 ms per 256 windows)
-        static const bool use_x0 = std::getenv("AM_STEM_X0") != nullptr;
-        const am_model::Block& b0 = m->blocks[0];
-        if (stem_fp16 && use_x0 && stem.w1s.p && !m->layers[b0.proj]->residual && (size_t)b0.proj < hi) {
-          d0 = d;
-          d0.cin_p = 16;
-          d0.has_expand = 1;
-          d0.x_is_fp16 = 0;
-          stem_x0 = fusedt::plan(d0, &plt0);
-        }
-      }
       const int64_t n_tiles = (int64_t)nb * ((s.H + kStemTH - 1) / kStemTH) * ((s.W + kStemTW - 1) / kStemTW);
       const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(n_tiles, (int64_t)sm_count() * 8));
-      if (stem_x0) {
-        AM_LAUNCH(stem_x0_kernel, grid, 256, 0, st, mel_dev, nb, m->n_mels, T, s.H, s.W, stem.pad_t, stem.pad_l, stem.aux0.p,
-                  stem.aux1.p, stem.w_f32.p, dst);
-      } else if (stem_fp16) {
-        AM_LAUNCH(stem_kernel<true>, grid, 256, (size_t)stem.cout_p * 8, st, mel_dev, nb, m->n_mels, T, s.H, s.W,
-                  stem.pad_t, stem.pad_l, stem.aux0.p, stem.aux1.p, stem.w_f32.p, stem.aux2.p, stem.bias.p, stem.cout_p,
-                  dst);
-      } else {
-        AM_LAUNCH(stem_kernel<false>, grid, 256, (size_t)stem.cout_p * 8, st, mel_dev, nb, m->n_mels, T, s.H, s.W,
-                  stem.pad_t, stem.pad_l, stem.aux0.p, stem.aux1.p, stem.w_f32.p, stem.aux2.p, stem.bias.p, stem.cout_p,
-                  dst);
-      }
+      AM_LAUNCH(stem_kernel, grid, 256, (size_t)stem.cout_p * 8, st, mel_dev, nb, m->n_mels, T, s.H, s.W, stem.pad_t,
+                stem.pad_l, stem.aux0.p, stem.aux1.p, stem.w_f32.p, stem.aux2.p, stem.bias.p, stem.cout_p, dst);
     } else {
       const size_t smem = (size_t)(stem.kh * stem.kw + 1) * stem.cout_p * sizeof(float);
       AM_CHECK(smem <= 48 * 1024, "encoder: first convolution with %d x %d taps x %d channels does not fit in shared memory",
@@ -1279,32 +1114,22 @@ static int run_range(am_model* m, const float* mel_dev, const __nv_bfloat16* in,
   for (; i < hi; ++i) {
     const Layer& l = *m->layers[i];
     if (l.block_start) {
-      // whole block in one kernel when it fits on chip (fused_block.cu)
-      const int bi = block_index_at(m, i);
+      block_in = cur;
       fused::BlockDesc d;
       fused::Plan pl;
-      if (bi >= 0 && (size_t)m->blocks[bi].proj < hi && block_desc(m, bi, s, stem_fp16, &d, &pl)) {
-        const am_model::Block& blk = m->blocks[bi];
-        const Layer& dwl = *m->layers[blk.dw];
-        const Layer& pj = *m->layers[blk.proj];
-        const Layer* ex = blk.expand >= 0 ? m->layers[blk.expand].get() : nullptr;
-        block_in = cur;
-        __nv_bfloat16* dst = pick_dst((size_t)blk.proj + 1 == hi);
-        fusedt::Plan plt;
-        if (bi == 0 && stem_x0) {            // stem + block 0: the stem's affine is this block's expansion GEMM
-          AM_TRY(fusedt::run(d0, plt0, cur, m->layers[0]->w1s.p, dwl.tpack.p, pj.w_f16.p, pj.bias.p, dst, nb, st));
-        } else if (ex && fusedt::plan(d, &plt)) {   // channel-per-lane kernel: depthwise taps straight from TMEM
-          AM_TRY(fusedt::run(d, plt, cur, ex->w_bf16.p, dwl.tpack.p, pj.w_f16.p, pj.bias.p, dst, nb, st));
-        } else {
-          AM_TRY(fused::run(d, pl, cur, ex ? ex->w_bf16.p : nullptr, ex ? ex->bias.p : nullptr, dwl.w_f32.p,
-                            dwl.bias.p, pj.w_f16.p, pj.bias.p, dst, nb, st));
-        }
-        s = dw_out(dwl, s);
+      int ex, dw, pj;
+      if (fused_block_at(m, i, hi, s, &d, &pl, &ex, &dw, &pj)) {  // the whole block in one kernel (fused_block.cu)
+        const Layer* E = ex >= 0 ? m->layers[(size_t)ex].get() : nullptr;
+        const Layer& D = *m->layers[(size_t)dw];
+        const Layer& P = *m->layers[(size_t)pj];
+        __nv_bfloat16* dst = pick_dst((size_t)pj + 1 == hi);
+        AM_TRY(fused::run(d, pl, cur, E ? E->w_bf16.p : nullptr, E ? E->bias.p : nullptr, D.w_f32.p, D.bias.p,
+                          P.w_bf16.p, P.bias.p, dst, nb, st));
+        s = dw_out(D, s);
         cur = block_in = dst;
-        i = (size_t)blk.proj;
+        i = (size_t)pj;
         continue;
       }
-      block_in = cur;
     }
     __nv_bfloat16* dst = pick_dst(i + 1 == hi);
     if (l.type == kDepthwise && !l.dw_fast()) {
@@ -1480,6 +1305,20 @@ static size_t max_act_range(const am_model* m, int T, size_t lo, size_t hi) {
   return mx;
 }
 
+// windows per pass of the early phase for a call of n windows: at most max_sub, and few enough that one activation
+// buffer stays within kEarlyActBudget elements.  The buffers are sized for every layer output, the expanded tensors
+// included (blocks run layer by layer with AM_FUSED_BLOCKS=0 or when a block does not fit the fused kernel): ~50 MB
+// per 10 s window for the shipped student, so 256 windows would need three 14 GB buffers.
+constexpr size_t kEarlyActBudget = (size_t)1 << 30;  // bf16 elements = 2 GiB per buffer
+
+static int early_sub(const am_model* m, int T, int n) {
+  Shape ss;
+  int cs;
+  const size_t per_win = std::max<size_t>(1, max_act_range(m, T, 0, late_start(m, T, &ss, &cs)));
+  const int cap = (int)std::max<size_t>(1, kEarlyActBudget / per_win);
+  return std::min({std::max(n, 1), m->max_sub, cap});
+}
+
 static int ensure_workspace(am_model* m, int T, int nb, int n_total) {
   Shape ss;
   int cs;
@@ -1518,9 +1357,9 @@ static int finish_load(am_model* m, const am::ModelSpec& spec, am_model** out) {
   const char* impl = std::getenv("AM_GEMM_IMPL");
   m->use_simt_gemm = (impl && std::strcmp(impl, "simt") == 0) ? 1 : 0;
   if (const char* sb = std::getenv("AM_CLAP_SUB_BATCH")) m->max_sub = std::max(1, std::atoi(sb));
-  if (const char* fb = std::getenv("AM_FUSED_BLOCKS")) m->fused_mask = (unsigned)std::strtoul(fb, nullptr, 0);
+  if (const char* fb = std::getenv("AM_FUSED_BLOCKS")) m->fused_blocks = std::atoi(fb) != 0;
   if (!m->use_simt_gemm && !gemm::available()) {
-    set_error("am_clap_load: the tcgen05 GEMM path is unavailable on this device; no fallback is shipped");
+    set_error("am_clap_load: the wgmma GEMM path is unavailable on this device; no fallback is shipped");
     delete m;
     return AM_ERR_NO_DEVICE;
   }
@@ -1682,8 +1521,9 @@ extern "C" double am_clap_flops_per_segment(const am_model* m, int T) {
   return 2.0 * (macs + head_macs(m));
 }
 
-// flops (2 x MAC) of one window of T frames executed by the standalone GEMM kernel and by the fused
-// block kernel (pointwise + depthwise inside fused blocks), following the same plan forward_sub uses
+// flops (2 x MAC) of one window of T frames executed by the GEMM kernel and by the fused block kernel (pointwise +
+// depthwise inside fused blocks), and the fused blocks' algorithmic HBM bytes (block input + output, bf16), following
+// the same plan run_range uses
 extern "C" int am_clap_flops_split(const am_model* m, int T, double* gemm_flops, double* fused_flops,
                                    double* fused_bytes) {
   AM_CHECK(m && gemm_flops && fused_flops && fused_bytes && !m->layers.empty(), "am_clap_flops_split: bad argument");
@@ -1691,26 +1531,21 @@ extern "C" int am_clap_flops_split(const am_model* m, int T, double* gemm_flops,
   double g = 0.0, f = 0.0, fb = 0.0;
   for (size_t i = 1; i < m->layers.size(); ++i) {
     const Layer& l = *m->layers[i];
-    bool fused_here = false;
-    if (l.block_start && !m->use_simt_gemm) {
-      const int q = block_index_at(m, i);
-      fused::BlockDesc d;
-      fused::Plan pl;
-      if (q >= 0 && block_desc(m, q, s, false, &d, &pl)) {
-        const am_model::Block& blk = m->blocks[q];
-        const Layer& dwl = *m->layers[blk.dw];
-        const Layer& pj = *m->layers[blk.proj];
-        const Shape o = dw_out(dwl, s);
-        double macs = (double)o.H * o.W * dwl.cin * 9.0 + (double)o.H * o.W * pj.cin * (double)pj.cout;
-        if (blk.expand >= 0) macs += (double)s.H * s.W * m->layers[blk.expand]->cin * (double)m->layers[blk.expand]->cout;
-        f += 2.0 * macs;
-        fb += 2.0 * ((double)s.H * s.W * d.cin_p + (double)o.H * o.W * d.cout_p);  // X in + Y out, 16-bit
-        s = o;
-        i = (size_t)blk.proj;
-        fused_here = true;
-      }
+    fused::BlockDesc d;
+    fused::Plan pl;
+    int ex, dw, pj;
+    if (fused_block_at(m, i, m->layers.size(), s, &d, &pl, &ex, &dw, &pj)) {
+      const Layer& D = *m->layers[(size_t)dw];
+      const Layer& P = *m->layers[(size_t)pj];
+      const Shape o = dw_out(D, s);
+      double macs = (double)o.H * o.W * D.cin * 9.0 + (double)o.H * o.W * P.cin * (double)P.cout;
+      if (ex >= 0) macs += (double)s.H * s.W * m->layers[(size_t)ex]->cin * (double)m->layers[(size_t)ex]->cout;
+      f += 2.0 * macs;
+      fb += 2.0 * ((double)s.H * s.W * d.cin_p + (double)o.H * o.W * d.cout_p);
+      s = o;
+      i = (size_t)pj;
+      continue;
     }
-    if (fused_here) continue;
     if (l.type == kDepthwise) {
       s = dw_out(l, s);
     } else if (l.type == kPointwise) {
@@ -1727,7 +1562,7 @@ extern "C" int am_clap_embed_dev(am_model* m, const float* mel_dev, int B, int T
   AM_CHECK(m && mel_dev && out_dev, "am_clap_embed_dev: NULL argument");
   AM_CHECK(B >= 0 && T > 0, "am_clap_embed_dev: bad shape B=%d T=%d", B, T);
   cudaStream_t st = (cudaStream_t)stream;
-  const int sub = std::min(std::max(B, 1), m->max_sub);
+  const int sub = early_sub(m, T, B);
   AM_TRY(ensure_workspace(m, T, sub, B));
   for (int b0 = 0; b0 < B; b0 += sub) {
     const int nb = std::min(sub, B - b0);
@@ -1762,7 +1597,7 @@ extern "C" int am_clap_embed_tracks_dev(am_model* m, const am_mel_plan* plan, co
   cudaStream_t st = (cudaStream_t)stream;
   const int hop = mel_plan_hop(plan);
   const int T = 1 + n_samples / hop;
-  const int sub = std::min(std::max(n_segments, 1), m->max_sub);
+  const int sub = early_sub(m, T, n_segments);
   AM_TRY(ensure_workspace(m, T, sub, n_segments));
   AM_TRY(m->mel_ws.ensure((size_t)sub * m->n_mels * T));
   AM_TRY(m->seg_emb.ensure((size_t)std::max(n_segments, 1) * m->emb));
@@ -1824,7 +1659,7 @@ extern "C" int am_clap_embed_tracks_submit(am_model* m, const am_mel_cfg* cfg, c
     if (!m->ev_done[i]) AM_CUDA(cudaEventCreateWithFlags(&m->ev_done[i], cudaEventDisableTiming));
   }
   const int T = 1 + n_samples / cfg->hop;
-  const int sub = std::min(std::max(n_segments, 1), m->max_sub);
+  const int sub = early_sub(m, T, n_segments);
   // (growing a workspace buffer while a batch is in flight is safe: cudaFree waits for the device)
   AM_TRY(ensure_workspace(m, T, sub, n_segments));
   AM_TRY(m->mel_ws.ensure((size_t)sub * m->n_mels * T));

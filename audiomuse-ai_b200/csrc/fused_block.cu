@@ -1,978 +1,315 @@
-// Fused PhiNet inverted-residual block (sm_100a):
+// Fused inverted-residual block on sm_90a: [1x1 expand + ReLU6] -> 3x3 depthwise + ReLU6 -> 1x1 project [+ residual]
+// in one kernel, so the expanded tensor (6x the block width) never goes to HBM.
 //
-//     Y = [X +] project( relu6( dw3x3_s( relu6( expand(X) ) ) ) )        all BatchNorms folded
-//
-// in ONE kernel, so the expanded tensor (up to 5.8x the block input) never touches HBM.
-// Replaces, for the wide early blocks, the three-kernel sequence GEMM -> depthwise -> GEMM of
-// encoder.cu (student_clap/models/student_onnx_model.py:95-148 block shape; micromind PhiNetConvBlock).
-//
-// One CTA (16 compute warps + 1 control warp) owns TH output rows x the full width of one window:
-//   TMA      X halo tile  [(TH-1)s+3 rows x W x Cin]  -> smem, K-major SWIZZLE_128B (zero rows = conv padding)
-//   per 64-channel chunk j of the expanded dimension:
-//     tcgen05.mma   D1[t] = X[t] . W1_j^T            (M1 halo pixels in 128-row tiles, N = 64, TMEM)
-//     epilogue 1    TMEM -> +b1, ReLU6, zero outside the image -> fp16 -> smem E (same swizzled layout)
-//     depthwise     3x3 stride s over E (+bd, ReLU6; HFMA2) -> fp16 -> smem A2, written directly in the
-//                   K-major SWIZZLE_128B operand layout (fence.proxy.async before the MMA reads it)
-//     tcgen05.mma   D2 += A2 . W2_j^T                (M = 128 output pixels, N = Cout, TMEM; fp16 x fp16:
-//                   post-ReLU6 values in [0, 6] keep 3 more mantissa bits than bf16 and skip a conversion)
-//   epilogue 2      TMEM -> +b2 (+ residual read from the X tile in smem) -> bf16 -> global Y
-// Weights stream through 2-stage TMA rings; D1 (two sets when the 512 TMEM columns allow) and A2 are
-// double buffered, so the expansion MMA of chunk j+1 runs under epilogue 1 / depthwise of chunk j.
-// Where the time goes (B200, tools/gpu_trace.sh, profiles/r02_fused_trace.txt; cycles per 64-channel chunk of a
-// 128-pixel tile): the compute warps are the critical path -- depthwise 1400-2100, epilogue 1 700-1100, barrier /
-// mbarrier waits ~600 -- while the tensor pipe is 5-19 % busy (an M128 x N64 x K16 tcgen05.mma costs ~48 cycles when
-// issued straight-line, so the ~25 expansion + 4 projection MMAs of a chunk hide completely).  The depthwise phase is
-// bound by shared-memory wavefronts and per-warp latency (one work item per thread and chunk, 4 warps per
-// scheduler), not by arithmetic: its lane mapping below is chosen for wavefronts, not for FMAs.
-#include <cuda_fp16.h>
-
-#include <algorithm>
-#include <type_traits>
-#include <cstdio>
-#include <cstdlib>
-
+// One warpgroup per 8 x 8 output tile of one window.  The input halo tile (10 x 10 pixels at stride 1, 17 x 17 at
+// stride 2) is loaded once into shared memory as K-major 128-byte-swizzled bf16 tiles.  The expansion channels are
+// then walked in chunks of 64:
+//   expansion   wgmma m64n64k16 over the halo rows, fp32 accumulators in registers -> + bias, ReLU6 -> bf16 halo tile
+//               E [halo pixels x 64] in shared memory (pixels outside the image are zero: the depthwise pads with 0);
+//   depthwise   3 x 3 taps from E in fp32 (a thread = 8 channels of one output pixel) + bias, ReLU6 -> bf16, written
+//               as the K-major swizzled A operand [64 pixels x 64 channels] of
+//   projection  wgmma m64n64k16 into up to four 64-column register accumulator blocks (Cout <= 256), accumulated
+//               over the chunks.
+// Epilogue: + bias (+ the block input for a residual block) -> bf16, straight from the registers.
+// Blocks without an expansion conv read E from the input directly.  Rounding follows the layer-by-layer path: the
+// expansion and the depthwise output are rounded to bf16, every sum is fp32.
 #include "fused_block.cuh"
-#include "gemm_tcgen05.cuh"
-#include "ptx_sm100.cuh"
 
-#ifndef AM_FUSED_BACKOFF
-#define AM_FUSED_BACKOFF 0   // (the nanosleep between polls cost ~1 % on B200: 1.737 -> 1.717 ms for block 0)
-#endif
+#include "ptx_sm90.cuh"
 
 namespace am {
 namespace fused {
 
 using namespace ptx;
 
-constexpr int kComputeWarps = 16;   // + 1 control warp: 96 registers per thread without spills
-constexpr int kComputeThreads = kComputeWarps * 32;   // warps 0..15: epilogues + depthwise
-constexpr int kThreads = kComputeThreads + 32;        // warp 16: control (TMA + MMA issue, one lane)
-constexpr int kGrpWarps = kComputeWarps / 4;          // compute warps sharing one TMEM lane group
-constexpr int kCK = 64;                 // expanded channels per chunk = one 128-byte swizzle row
-constexpr int kTileBytes = 128 * 128;   // one [128 rows x 64 ch] bf16 operand tile
-constexpr int kTmemCols = 512;
-constexpr int kTraceItems = 96;
-constexpr int kMaxKb = 8;               // X k-blocks (Cin <= 512)
+constexpr int kTile = 8;        // output tile edge: 64 pixels = one m64 projection
+constexpr int kChunk = 64;      // expansion channels per pass = one 128-byte swizzle row of projection K
+constexpr int kThreads = 128;   // one warpgroup
+constexpr int kMaxCout = 256;
+constexpr size_t kSmemMax = 232448;
+
+template <int S>
+constexpr int halo() { return (kTile - 1) * S + 3; }
+template <int S>
+constexpr int halo_rows() { return (halo<S>() * halo<S>() + 63) / 64 * 64; }
+
+// byte offset of (row, 16-byte chunk) in a K-major SWIZZLE_128B tile (rows of 64 bf16, 8-row atoms of 1024 bytes)
+__device__ __forceinline__ uint32_t sw128(uint32_t row, uint32_t chunk) {
+  return (row << 7) + (((chunk ^ row) & 7u) << 4);
+}
 
 struct Args {
-  int B, H, W, Ho, Wo, stride;
-  int cin_p, cmid_p, cout_p;
-  int has_expand, residual;
-  int TH, IH, M1, m1_tiles, M2;
-  int kb_in, n_chunks;
-  int tiles_per_window, total_tiles;
-  const float* b1;   // [cmid_p]
-  const float* wd;   // [9, cmid_p]
-  const float* bd;   // [cmid_p]
-  const float* b2;   // [cout_p]
-  __nv_bfloat16* Y;  // [B, Ho, Wo, cout_p]
-  // smem byte offsets (from the 1024-aligned base)
-  uint32_t off_x, off_e, off_a2, off_w1, off_w2, off_small, off_bar;
-  uint32_t w1_stage_bytes, w2_stage_bytes;
-  int a2_bufs;       // 1 or 2 A2 operand buffers (2 lets the depthwise of chunk w+1 overlap MMA2(w))
-  int d1_bufs;       // 1 or 2 D1 accumulator sets in TMEM (2 lets MMA1(w+1) overlap epilogue 1 of chunk w)
-  int x_is_fp16;     // no-expand block: the X tile (stem output) is fp16, read by the depthwise directly
-  uint32_t magic_wo, magic_w;  // ceil(2^16 / Wo), ceil(2^16 / W): n / d == (n * magic) >> 16 for n < 2^12
-  long long* trace;  // debug (AM_FUSED_TRACE=1): [kTraceItems][16] clock64 stamps of CTA 0, else NULL
+  const __nv_bfloat16* X;   // [B, H, W, cin_p]
+  const __nv_bfloat16* W1;  // [cmid_p, cin_p] (has_expand)
+  const float* b1;          // [cmid_p]
+  const float* wd;          // [9, cmid_p]
+  const float* bd;          // [cmid_p]
+  const __nv_bfloat16* W2;  // [cout_p, cmid_p]
+  const float* b2;          // [cout_p]
+  __nv_bfloat16* Y;         // [B, Ho, Wo, cout_p]
+  int H, W, Ho, Wo, tiles_y, tiles_x;
+  int cin_p, cmid_p, cout_p, residual;
 };
 
-__host__ __device__ __forceinline__ uint32_t round_up_dev(uint32_t x, uint32_t m) { return (x + m - 1) / m * m; }
+struct Layout {  // shared-memory carve-up (byte offsets from the 1024-aligned base)
+  uint32_t xs, w1s, w2s, a2, e, total;
+};
 
-__device__ __forceinline__ uint32_t pack2(float a, float b) {
-  __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
-  return *reinterpret_cast<uint32_t*>(&h);
-}
-__device__ __forceinline__ uint32_t pack2h(float a, float b) {  // fp16x2 (the E tile is fp16)
-  __half2 h = __floats2half2_rn(a, b);
-  return *reinterpret_cast<uint32_t*>(&h);
-}
-__device__ __forceinline__ __half2 as_h2(uint32_t u) { return *reinterpret_cast<__half2*>(&u); }
-__device__ __forceinline__ __half2 bf2_to_h2(uint32_t u) {  // bf16x2 -> fp16x2 (exact for |x| in fp16 range)
-  return __float22half2_rn(__bfloat1622float2(*reinterpret_cast<__nv_bfloat162*>(&u)));
-}
-__device__ __forceinline__ uint32_t h2_to_bf2(__half2 h) {
-  const float2 f = __half22float2(h);
-  return pack2(f.x, f.y);
-}
-// explicit shared-space vector accesses (32-bit shared addresses: never the generic path)
-__device__ __forceinline__ uint4 lds128(uint32_t addr) {
-  uint4 v;
-  asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr));
-  return v;
-}
-// predicated forms: ONE instruction each (@p LDS / @p STS), so edge handling never splits a basic block --
-// behind an `if` nvcc emits BSSY / BRA / BSYNC and stops hoisting the following loads above it
-__device__ __forceinline__ uint4 lds128_if(uint32_t addr, bool p) {  // zeros when !p
-  uint4 v = make_uint4(0u, 0u, 0u, 0u);
-  asm volatile(
-      "{\n.reg .pred P;\nsetp.ne.b32 P, %5, 0;\n@P ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];\n}\n"
-      : "+r"(v.x), "+r"(v.y), "+r"(v.z), "+r"(v.w)
-      : "r"(addr), "r"((uint32_t)p));
-  return v;
-}
-__device__ __forceinline__ void sts128_if(uint32_t addr, const uint4& v, bool p) {
-  asm volatile("{\n.reg .pred P;\nsetp.ne.b32 P, %5, 0;\n@P st.shared.v4.b32 [%0], {%1, %2, %3, %4};\n}\n" ::"r"(addr),
-               "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w), "r"((uint32_t)p)
-               : "memory");
-}
-__device__ __forceinline__ void sts128(uint32_t addr, const uint4& v) {
-  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
-}
-// Phase timeline for tools/gpu_trace.sh.  Compiled in only with -DAM_FUSED_TRACE_BUILD: even predicated
-// off, the clock reads and stores of 16 trace points were ~10 % of the instructions the kernel issued.
-#ifdef AM_FUSED_TRACE_BUILD
-#define AM_TRACE(slot_)                                                                              \
-  do {                                                                                               \
-    if (a.trace && blockIdx.x == 0 && lane == 0 && w < kTraceItems && (warp == 0 || warp == kComputeWarps)) \
-      a.trace[w * 16 + (slot_)] = clock64();                                                         \
-  } while (0)
-#else
-#define AM_TRACE(slot_) do { } while (0)
-#endif
-
-// ---- MMA issue, written for the instruction stream of the ONE issuing thread.  That thread shares its
-// scheduler with four busy compute warps, so every dependent instruction between two tcgen05.mma costs
-// ~10 cycles of issue latency (measured: 104 cycles per MMA with a generic descriptor loop vs 48 for the
-// bare instruction, tools/mma_probe.py).  Everything below is therefore straight-line per k-block:
-// descriptors are base + compile-time constants (independent UIADD3s), the k-step and M-tile loops are
-// fully unrolled, and the accumulate flag is a compile-time constant except for the first k-step.
-constexpr uint32_t kDescHi = (1024u >> 4) | (1u << 14) | (2u << 29);  // bits [32,64) of make_smem_desc()
-__device__ __forceinline__ uint32_t desc_lo(uint32_t smem_addr) { return (smem_addr >> 4) & 0x3fffu; }
-
-template <int kTiles>
-__device__ __forceinline__ void issue_expand_mma(uint32_t d_base, uint32_t s_x, uint32_t x_kb_bytes, uint32_t s_w1,
-                                                 int kb_in, int cin_p, uint32_t idesc) {
-  uint32_t da = desc_lo(s_x), db = desc_lo(s_w1);
-  const uint32_t da_step = x_kb_bytes >> 4;  // smem addresses stay below 2^18: the 14-bit field never carries
-#pragma unroll 1
-  for (int kb = 0; kb < kb_in; ++kb, da += da_step, db += (kCK * 128) >> 4) {
-    const int ksteps = min(64, cin_p - kb * 64) >> 4;  // cin_p % 16 == 0
-#pragma unroll
-    for (int ks = 0; ks < 4; ++ks) {
-      if (ks < ksteps) {
-        // k-steps outermost, M-tiles innermost: consecutive MMAs target different accumulators
-#pragma unroll
-        for (int t = 0; t < kTiles; ++t)
-          umma_f16_lo(d_base + (uint32_t)(t * kCK), da + (uint32_t)(t * (kTileBytes >> 4) + ks * 2), db + (uint32_t)(ks * 2),
-                      kDescHi, idesc, ks ? 1u : (kb ? 1u : 0u));
-      }
-    }
-  }
-}
-// (must be inlined into the elected region: out of line, nvcc wraps every MMA in an ELECT loop again)
-__device__ __forceinline__ void issue_expand(int m1_tiles, uint32_t d, uint32_t s_x, uint32_t x_kb_bytes, uint32_t sw,
-                                          int kb_in, int cin_p, uint32_t idesc) {
-  switch (m1_tiles) {
-    case 1: issue_expand_mma<1>(d, s_x, x_kb_bytes, sw, kb_in, cin_p, idesc); break;
-    case 2: issue_expand_mma<2>(d, s_x, x_kb_bytes, sw, kb_in, cin_p, idesc); break;
-    case 3: issue_expand_mma<3>(d, s_x, x_kb_bytes, sw, kb_in, cin_p, idesc); break;
-    case 4: issue_expand_mma<4>(d, s_x, x_kb_bytes, sw, kb_in, cin_p, idesc); break;
-    default:
-      for (int t = 0; t < m1_tiles; ++t)
-        issue_expand_mma<1>(d + (uint32_t)(t * kCK), s_x + (uint32_t)(t * kTileBytes), x_kb_bytes, sw, kb_in, cin_p, idesc);
-  }
-}
-__device__ __forceinline__ void issue_project_mma(uint32_t d, uint32_t s_a2, uint32_t s_w2, int ksteps, uint32_t idesc,
-                                                  bool first_chunk) {
-  const uint32_t da = desc_lo(s_a2), db = desc_lo(s_w2);
-#pragma unroll
-  for (int ks = 0; ks < 4; ++ks)
-    if (ks < ksteps)
-      umma_f16_lo(d, da + (uint32_t)(ks * 2), db + (uint32_t)(ks * 2), kDescHi, idesc, ks ? 1u : (first_chunk ? 0u : 1u));
+__host__ __device__ inline Layout layout(int S, bool has_expand, int cin_p, int cout_p) {
+  const uint32_t hr = (uint32_t)(((S == 1 ? 10 * 10 : 17 * 17) + 63) / 64 * 64);
+  const uint32_t kbx = has_expand ? (uint32_t)((cin_p + 63) / 64) : 0u;
+  const uint32_t n2 = (uint32_t)((cout_p + 63) / 64 * 64);
+  Layout l;
+  l.xs = 0;
+  l.w1s = l.xs + kbx * hr * 128;
+  l.w2s = l.w1s + kbx * kChunk * 128;
+  l.a2 = l.w2s + n2 * 128;
+  l.e = l.a2 + 64 * 128;
+  l.total = l.e + hr * 128;
+  return l;
 }
 
-__device__ __forceinline__ void compute_bar_sync() { named_bar_sync_1<kComputeThreads>(); }
-// compute-warp wait: same parity protocol, but back off between polls so 20 spinning warps do not
-// eat the issue slots the working warps need
-__device__ __forceinline__ void mbar_wait_relaxed(uint64_t* bar, uint32_t parity) {
-  const uint32_t addr = smem_u32(bar);
-  for (;;) {
-    uint32_t done;
-    asm volatile(
-        "{\n.reg .pred P1;\n"
-        "mbarrier.try_wait.parity.shared::cta.b64 P1, [%1], %2;\n"
-        "selp.u32 %0, 1, 0, P1;\n}\n"
-        : "=r"(done)
-        : "r"(addr), "r"(parity)
-        : "memory");
-    if (done) break;
-    if (AM_FUSED_BACKOFF) __nanosleep(32);
-  }
-}
-
-// Barrier protocol (k-th completion <-> parity k & 1; every completion count is a function of the
-// flat work-item index w = (tile, chunk) enumerated in order, so all roles derive parities locally):
-//   bar_xk[kb]  TMA     k-block kb of the X halo tile of a tile landed                 (1 / tile each)
-//   bar_w1[s]   TMA     expansion weights of item w (s = w & 1) landed             (1 / item)
-//   bar_w2[s]   TMA     projection weights of item w landed                        (1 / item)
-//   bar_mma1    commit  D1(w) complete in TMEM                                     (1 / item)
-//   bar_mma2    commit  projection MMA of item w retired (A2, W2 stage free; last chunk: D2 ready)
-//   bar_epi1    16      compute warps finished reading D1(w)   -> control may issue MMA1(w+1)
-//   bar_a2      16      compute warps finished writing A2(w) (and reading E / X k-block) -> MMA2(w)
-//   bar_tile    16      compute warps finished epilogue 2 of a tile -> D2 / X (residual) reusable
-// kExpand / kStride / kFp16Src are template parameters so that each launch runs a loop with ONE depthwise
-// body and no format / stride branches (the generic loop was > 20 KB of code: instruction-fetch stalls).
-template <bool kExpand, int kStride, bool kFp16Src>
-__global__ void __launch_bounds__(kThreads, 1)
-fused_block_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_w1,
-                   const __grid_constant__ CUtensorMap map_w2, const Args a) {
+template <int S, bool kExpand>
+__global__ void __launch_bounds__(kThreads)
+fused_block_kernel(const Args a) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  // keep pointer provenance (shared address space) while aligning to 1024 bytes
-  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  const uint32_t sm = smem_u32(smem);
-  const uint32_t s_x = sm + a.off_x, s_e = sm + a.off_e, s_a2 = sm + a.off_a2;
-  const uint32_t s_w1 = sm + a.off_w1, s_w2 = sm + a.off_w2;
-  const int cmid64 = (a.cmid_p + 63) & ~63;                             // per-chunk vectors padded with zeros
-  float* s_b2 = reinterpret_cast<float*>(smem + a.off_small);            // [cout_p]   projection bias, fp32
-  __half* s_wd = reinterpret_cast<__half*>(s_b2 + a.cout_p);             // [9][cmid64] depthwise weights, fp16
-  __half* s_bd = s_wd + 9 * cmid64;                                      // [cmid64]    depthwise bias, fp16
-  __half* s_b1 = s_bd + cmid64;                                          // [cmid64]    expansion bias, fp16
-  const uint32_t s_wd_u32 = smem_u32(s_wd), s_bd_u32 = smem_u32(s_bd), s_b1_u32 = smem_u32(s_b1);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + a.off_bar);
-  uint64_t* bar_xk = bars;       // [kMaxKb]: one per X k-block (a block without expansion refills them one by one)
-  uint64_t* bar_w1 = bars + 8;   // [2]
-  uint64_t* bar_w2 = bars + 10;  // [2]
-  uint64_t* bar_mma1 = bars + 12;  // [2]: one per D1 accumulator set
-  uint64_t* bar_mma2 = bars + 14;  // [2]: one per A2 buffer
-  uint64_t* bar_epi1 = bars + 16;  // [2]: one per D1 accumulator set
-  uint64_t* bar_a2 = bars + 18;    // [2]: one per A2 buffer (a phase can only advance once per MMA2 of that slot)
-  uint64_t* bar_tile = bars + 20;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 21);
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  constexpr int HALO = halo<S>(), HPX = HALO * HALO, HR = halo_rows<S>();
+  const Layout L = layout(S, kExpand, a.cin_p, a.cout_p);
+  uint8_t* xs = smem + L.xs;
+  uint8_t* w1s = smem + L.w1s;
+  uint8_t* w2s = smem + L.w2s;
+  uint8_t* a2 = smem + L.a2;
+  __nv_bfloat16* e = reinterpret_cast<__nv_bfloat16*>(smem + L.e);  // [HR][64], plain rows of 128 bytes
 
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, quad = lane & 3;
+  const int per_img = a.tiles_y * a.tiles_x;
+  const int b = blockIdx.x / per_img;
+  const int ty = (blockIdx.x % per_img) / a.tiles_x, tx = blockIdx.x % a.tiles_x;
+  const int oy0 = ty * kTile, ox0 = tx * kTile;
+  const int gy0 = oy0 * S - 1, gx0 = ox0 * S - 1;  // image position of halo pixel (0, 0)
+  const __nv_bfloat16* Xb = a.X + (int64_t)b * a.H * a.W * a.cin_p;
+  auto in_image = [&](int hp, int& gy, int& gx) {
+    gy = gy0 + hp / HALO;
+    gx = gx0 + hp % HALO;
+    return hp < HPX && gy >= 0 && gy < a.H && gx >= 0 && gx < a.W;
+  };
+  const uint4 zero4 = make_uint4(0u, 0u, 0u, 0u);
 
-  if (tid == 0) {
-    prefetch_tensormap(&map_x);
-    prefetch_tensormap(&map_w1);
-    prefetch_tensormap(&map_w2);
-    for (int i = 0; i < kMaxKb; ++i) mbar_init(&bar_xk[i], 1);
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&bar_w1[i], 1);
-      mbar_init(&bar_w2[i], 1);
+  const int kbx = (a.cin_p + 63) / 64;
+  if (kExpand) {  // input halo tile, once: [kbx][HR rows][64 channels]
+    for (int it = tid; it < kbx * HR * 8; it += kThreads) {
+      const int c = it & 7, p = (it >> 3) % HR, kb = (it >> 3) / HR;
+      const int ch = kb * 64 + c * 8;
+      int gy, gx;
+      uint4 v = zero4;
+      if (ch < a.cin_p && in_image(p, gy, gx)) v = *reinterpret_cast<const uint4*>(Xb + ((int64_t)gy * a.W + gx) * a.cin_p + ch);
+      *reinterpret_cast<uint4*>(xs + kb * HR * 128 + sw128(p, c)) = v;
     }
-    mbar_init(&bar_mma1[0], 1);
-    mbar_init(&bar_mma1[1], 1);
-    mbar_init(&bar_mma2[0], 1);
-    mbar_init(&bar_mma2[1], 1);
-    mbar_init(&bar_epi1[0], kComputeWarps);
-    mbar_init(&bar_epi1[1], kComputeWarps);
-    mbar_init(&bar_a2[0], kComputeWarps);
-    mbar_init(&bar_a2[1], kComputeWarps);
-    mbar_init(bar_tile, kComputeWarps);
-    fence_barrier_init();
+  }
+
+  const int n2_blocks = (a.cout_p + 63) / 64;
+  float acc2[4][32];
+#pragma unroll
+  for (int nb = 0; nb < 4; ++nb)
+#pragma unroll
+    for (int i = 0; i < 32; ++i) acc2[nb][i] = 0.f;
+
+  for (int c0 = 0; c0 < a.cmid_p; c0 += kChunk) {
+    const int nch = min(kChunk, a.cmid_p - c0);
+    __syncthreads();  // the previous chunk's readers of w1s / w2s / E / A2 are done
+    if (kExpand) {
+      for (int it = tid; it < kbx * kChunk * 8; it += kThreads) {
+        const int c = it & 7, r = (it >> 3) % kChunk, kb = (it >> 3) / kChunk;
+        const int ch = kb * 64 + c * 8;
+        uint4 v = zero4;
+        if (r < nch && ch < a.cin_p) v = *reinterpret_cast<const uint4*>(a.W1 + (int64_t)(c0 + r) * a.cin_p + ch);
+        *reinterpret_cast<uint4*>(w1s + kb * kChunk * 128 + sw128(r, c)) = v;
+      }
+    } else {  // no expansion: E is the input's channel chunk
+      for (int it = tid; it < HR * 8; it += kThreads) {
+        const int c = it & 7, p = it >> 3;
+        int gy, gx;
+        uint4 v = zero4;
+        if (c * 8 < nch && in_image(p, gy, gx))
+          v = *reinterpret_cast<const uint4*>(Xb + ((int64_t)gy * a.W + gx) * a.cin_p + c0 + c * 8);
+        *reinterpret_cast<uint4*>(e + p * 64 + c * 8) = v;
+      }
+    }
+    for (int it = tid; it < n2_blocks * 64 * 8; it += kThreads) {
+      const int c = it & 7, r = it >> 3;
+      uint4 v = zero4;
+      if (r < a.cout_p && c * 8 < nch) v = *reinterpret_cast<const uint4*>(a.W2 + (int64_t)r * a.cmid_p + c0 + c * 8);
+      *reinterpret_cast<uint4*>(w2s + sw128(r, c)) = v;
+    }
+    fence_proxy_async();  // generic-proxy writes -> visible to the wgmma (async proxy) reads
+    __syncthreads();
+
+    if (kExpand) {
+      for (int m = 0; m < HR / 64; ++m) {
+        float acc1[32];
+#pragma unroll
+        for (int i = 0; i < 32; ++i) acc1[i] = 0.f;
+        wgmma_fence();
+        for (int kb = 0; kb < kbx; ++kb) {
+          const uint64_t da = make_smem_desc(smem_u32(xs + kb * HR * 128 + m * 64 * 128));
+          const uint64_t db = make_smem_desc(smem_u32(w1s + kb * kChunk * 128));
+          const int ksteps = min(4, (a.cin_p - kb * 64) / 16);
+          for (int ks = 0; ks < ksteps; ++ks)
+            Wgmma<64>::mma(acc1, da + (uint64_t)(ks * 2), db + (uint64_t)(ks * 2), (kb | ks) ? 1u : 0u);
+        }
+        wgmma_commit();
+        wgmma_wait_all();
+        reg_fence(acc1);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int p = m * 64 + warp * 16 + (lane >> 2) + 8 * h;
+          int gy, gx;
+          const bool inside = in_image(p, gy, gx);
+#pragma unroll
+          for (int j = 0; j < 8; ++j) {
+            const int col = 8 * j + 2 * quad;
+            float f0 = 0.f, f1 = 0.f;
+            if (inside && col < nch) {
+              f0 = relu6f(acc1[4 * j + 2 * h] + __ldg(&a.b1[c0 + col]));
+              f1 = relu6f(acc1[4 * j + 2 * h + 1] + __ldg(&a.b1[c0 + col + 1]));
+            }
+            *reinterpret_cast<__nv_bfloat162*>(e + p * 64 + col) = __floats2bfloat162_rn(f0, f1);
+          }
+        }
+      }
+      __syncthreads();
+    } else {
+      __syncthreads();
+    }
+
+    // depthwise: item = 8 channels of one output pixel
+    for (int it = tid; it < 64 * 8; it += kThreads) {
+      const int g = it & 7, px = it >> 3;
+      const int oy = px >> 3, ox = px & 7;
+      uint4 out = zero4;
+      if (g * 8 < nch) {
+        const int cg = c0 + g * 8;
+        float acc[8];
+#pragma unroll
+        for (int q = 0; q < 8; ++q) acc[q] = __ldg(&a.bd[cg + q]);
+#pragma unroll
+        for (int dy = 0; dy < 3; ++dy)
+#pragma unroll
+          for (int dx = 0; dx < 3; ++dx) {
+            const int hp = (oy * S + dy) * HALO + ox * S + dx;
+            const uint4 v = *reinterpret_cast<const uint4*>(e + hp * 64 + g * 8);
+            const __nv_bfloat162* v2 = reinterpret_cast<const __nv_bfloat162*>(&v);
+            const float* w = a.wd + (dy * 3 + dx) * a.cmid_p + cg;
+#pragma unroll
+            for (int q = 0; q < 4; ++q) {
+              const float2 f = __bfloat1622float2(v2[q]);
+              acc[2 * q] = fmaf(f.x, __ldg(&w[2 * q]), acc[2 * q]);
+              acc[2 * q + 1] = fmaf(f.y, __ldg(&w[2 * q + 1]), acc[2 * q + 1]);
+            }
+          }
+        __nv_bfloat162 o2[4];
+#pragma unroll
+        for (int q = 0; q < 4; ++q) o2[q] = __floats2bfloat162_rn(relu6f(acc[2 * q]), relu6f(acc[2 * q + 1]));
+        out = *reinterpret_cast<const uint4*>(o2);
+      }
+      *reinterpret_cast<uint4*>(a2 + sw128(px, g)) = out;
+    }
     fence_proxy_async();
-  }
-  if (warp == kComputeWarps) tmem_alloc(tmem_ptr, kTmemCols);
-  for (int i = tid; i < a.cout_p; i += kThreads) s_b2[i] = a.b2[i];
-  for (int i = tid; i < 9 * cmid64; i += kThreads) {
-    const int t = i / cmid64, c = i - t * cmid64;
-    s_wd[i] = __float2half_rn(c < a.cmid_p ? a.wd[t * a.cmid_p + c] : 0.f);
-  }
-  for (int i = tid; i < cmid64; i += kThreads) {
-    s_bd[i] = __float2half_rn(i < a.cmid_p ? a.bd[i] : 0.f);
-    s_b1[i] = __float2half_rn((kExpand && i < a.cmid_p) ? a.b1[i] : 0.f);
-  }
-  tcgen05_fence_before();
-  __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
-  const uint32_t d1_cols = (uint32_t)(a.m1_tiles * kCK);                 // TMEM columns of one D1 set
-  const uint32_t tmem_d2 = tmem_base + (kExpand ? (uint32_t)a.d1_bufs * d1_cols : 0u);
+    __syncthreads();
 
-  // smem pitch of one X k-block: only M1 rows are real; the MMA's last 128-row tile may read past them
-  // into whatever follows in shared memory (those accumulator rows are never used)
-  const uint32_t x_kb_bytes = (uint32_t)round_up_dev((uint32_t)a.M1 * 128u, 1024u);
-  const int n_my_tiles = blockIdx.x < a.total_tiles ? (a.total_tiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
-  const int n_items = n_my_tiles * a.n_chunks;
-
-  if (warp == kComputeWarps) {
-    // =========================== control warp ===========================
-    if (elect_one_sync()) {  // one lane; see ptx_sm100.cuh for why not `lane == 0`
-      const uint32_t idesc1 = make_idesc(128, kCK);
-      const uint32_t idesc2 = make_idesc_f16(128, a.cout_p);  // A2 (depthwise output) and W2 are fp16
-      const uint32_t x_box_bytes = (uint32_t)a.M1 * 128u;
-      auto tile_of = [&](int ti) { return (int)blockIdx.x + ti * (int)gridDim.x; };
-      auto load_xk = [&](int ti, int kb) {
-        const int tile = tile_of(ti);
-        const int b = tile / a.tiles_per_window;
-        const int h0 = (tile - b * a.tiles_per_window) * a.TH * kStride - 1;
-        mbar_expect_tx(&bar_xk[kb], x_box_bytes);
-        tma_load_4d(smem + a.off_x + kb * x_kb_bytes, &map_x, &bar_xk[kb], kb * 64, 0, h0, b);
-      };
-      auto load_x = [&](int ti) {
-        for (int kb = 0; kb < a.kb_in; ++kb) load_xk(ti, kb);
-      };
-      auto wait_x = [&](int ti) {
-        for (int kb = 0; kb < a.kb_in; ++kb) mbar_wait(&bar_xk[kb], (uint32_t)ti & 1u);
-      };
-      // (w, jw): item index and its chunk index -- tracked by the caller, no division on this thread
-      auto load_w1 = [&](int w, int jw) {
-        if (!kExpand) return;
-        const int stg = w & 1, j = jw;
-        mbar_expect_tx(&bar_w1[stg], (uint32_t)a.kb_in * kCK * 128u);
-        for (int kb = 0; kb < a.kb_in; ++kb)
-          tma_load_2d(smem + a.off_w1 + stg * a.w1_stage_bytes + kb * (kCK * 128), &map_w1, &bar_w1[stg], kb * 64,
-                      j * kCK);
-      };
-      auto load_w2 = [&](int w, int jw) {
-        const int stg = w & 1, j = jw;
-        mbar_expect_tx(&bar_w2[stg], (uint32_t)a.cout_p * 128u);
-        tma_load_2d(smem + a.off_w2 + stg * a.w2_stage_bytes, &map_w2, &bar_w2[stg], j * kCK, 0);
-      };
-      auto issue_mma1 = [&](int w) {  // D1[t] = X[t] . W1_j^T for every halo M-tile
-        const int stg = w & 1;
-        const int ds = (a.d1_bufs == 2) ? (w & 1) : 0;
-        const uint32_t d = tmem_base + (uint32_t)ds * d1_cols;
-        const uint32_t sw = s_w1 + (uint32_t)(stg * a.w1_stage_bytes);
-        issue_expand(a.m1_tiles, d, s_x, x_kb_bytes, sw, a.kb_in, a.cin_p, idesc1);
-        umma_commit(&bar_mma1[ds]);
-      };
-
-      if (n_items > 0) {
-        load_x(0);
-        load_w1(0, 0);
-        load_w2(0, 0);
-        if (n_items > 1) {
-          load_w1(1, a.n_chunks > 1 ? 1 : 0);
-          load_w2(1, a.n_chunks > 1 ? 1 : 0);
-        }
-        if (kExpand) {
-          wait_x(0);
-          mbar_wait(&bar_w1[0], 0);
-          tcgen05_fence_after();
-          issue_mma1(0);
-        }
-      }
-      int ti = 0, j = 0;
-      for (int w = 0; w < n_items; ++w) {
-        const bool first = (j == 0), last = (j == a.n_chunks - 1);
-        const int j1 = last ? 0 : j + 1, j2 = (j1 == a.n_chunks - 1) ? 0 : j1 + 1;  // chunk index of items w+1, w+2
-        const int slot = (a.a2_bufs == 2) ? (w & 1) : 0;
-        const uint32_t kpar = (uint32_t)((a.a2_bufs == 2) ? (w >> 1) : w) & 1u;
-        AM_TRACE(8);
-        // ---- (A) expansion MMA of the next chunk of the SAME tile.  One D1 set: as soon as epilogue 1 of
-        //      chunk w drained it (runs under the depthwise of chunk w).  Two D1 sets: as soon as epilogue 1
-        //      of chunk w-1 drained the other set (runs under epilogue 1 AND depthwise of chunk w).
-        const int ds = (a.d1_bufs == 2) ? (w & 1) : 0;
-        const uint32_t dpar = (uint32_t)((a.d1_bufs == 2) ? (w >> 1) : w) & 1u;  // parity of item w on its D1 barriers
-        bool x_next_issued = false;
-        if (kExpand) {
-          if (!last) {
-            if (a.d1_bufs == 2) {
-              if (w >= 1) mbar_wait(&bar_epi1[(w + 1) & 1], (uint32_t)((w - 1) >> 1) & 1u);  // epilogue 1 of w-1
-            } else {
-              mbar_wait(&bar_epi1[0], (uint32_t)w & 1u);
-            }
-            AM_TRACE(14);
-            mbar_wait(&bar_w1[(w + 1) & 1], (uint32_t)((w + 1) >> 1) & 1u);
-            AM_TRACE(15);
-            tcgen05_fence_after();
-            issue_mma1(w + 1);
-          } else if (!a.residual && ti + 1 < n_my_tiles) {
-            // last chunk: once its expansion MMA retired nobody reads X any more -> prefetch the next
-            // tile's halo now, under the epilogue 1 / depthwise / projection / epilogue 2 of this tile
-            if (a.d1_bufs == 2) mbar_wait(&bar_mma1[ds], dpar);
-            else mbar_wait(&bar_epi1[0], (uint32_t)w & 1u);
-            load_x(ti + 1);
-            x_next_issued = true;
-          }
-          // two D1 sets: W1 stage w & 1 is free once MMA1(w) retired (its barrier cannot advance before
-          // MMA1(w+2) is issued, in the next iteration) -> refill it a full chunk ahead of its use
-          if (a.d1_bufs == 2 && w + 2 < n_items) {
-            mbar_wait(&bar_mma1[ds], dpar);
-            load_w1(w + 2, j2);
-          }
-        }
-        AM_TRACE(9);
-        // ---- (B) projection MMA of item w
-        mbar_wait(&bar_a2[slot], kpar);
-        AM_TRACE(10);
-        if (!kExpand && ti + 1 < n_my_tiles) load_xk(ti + 1, j);  // depthwise(j) was X k-block j's last reader
-        mbar_wait(&bar_w2[w & 1], (uint32_t)(w >> 1) & 1u);
-        if (first && ti > 0) mbar_wait(bar_tile, (uint32_t)(ti - 1) & 1u);  // D2 drained by epilogue 2
-        tcgen05_fence_after();
-        issue_project_mma(tmem_d2, s_a2 + (uint32_t)slot * kTileBytes, s_w2 + (uint32_t)((w & 1) * a.w2_stage_bytes),
-                          min(64, a.cmid_p - j * kCK + 15) / 16, idesc2, first);
-        umma_commit(&bar_mma2[slot]);
-        AM_TRACE(11);
-        if (last && ti + 1 < n_my_tiles && kExpand) {
-          // ---- (C) residual blocks: epilogue 2 reads the residual from X, so its refill waits for it
-          if (!x_next_issued) {
-            mbar_wait(bar_tile, (uint32_t)ti & 1u);  // epilogue 2 done (implies MMA1(w) retired long ago)
-            load_x(ti + 1);
-          }
-          // ---- (D) first expansion MMA of the next tile: its D1 set must have been drained
-          if (a.d1_bufs == 2) {
-            if (w >= 1) mbar_wait(&bar_epi1[(w + 1) & 1], (uint32_t)((w - 1) >> 1) & 1u);
-          } else {
-            mbar_wait(&bar_epi1[0], (uint32_t)w & 1u);
-          }
-          wait_x(ti + 1);
-          mbar_wait(&bar_w1[(w + 1) & 1], (uint32_t)((w + 1) >> 1) & 1u);
-          tcgen05_fence_after();
-          issue_mma1(w + 1);
-        }
-        AM_TRACE(12);
-        // ---- (E) weights of item w+2 into the stages item w just released.  W1 stage w & 1 is free:
-        //      bar_epi1(w) was observed in (A) or (C), which implies MMA1(w) retired (never re-wait on it
-        //      here: the barrier may already have advanced).
-        if (w + 2 < n_items) {
-          if (kExpand && a.d1_bufs == 1) load_w1(w + 2, j2);
-          mbar_wait(&bar_mma2[slot], kpar);  // MMA2(w) done with W2 stage w & 1
-          load_w2(w + 2, j2);
-        }
-        AM_TRACE(13);
-        if (++j == a.n_chunks) {
-          j = 0;
-          ++ti;
-        }
+    // projection: acc2 += A2 [64 x nch] . W2_chunk [Cout x nch]^T
+    wgmma_fence();
+    const uint64_t da = make_smem_desc(smem_u32(a2));
+#pragma unroll
+    for (int nb = 0; nb < 4; ++nb) {
+      if (nb < n2_blocks) {
+        const uint64_t db = make_smem_desc(smem_u32(w2s + nb * 64 * 128));
+        for (int ks = 0; ks < nch / 16; ++ks)
+          Wgmma<64>::mma(acc2[nb], da + (uint64_t)(ks * 2), db + (uint64_t)(ks * 2), (c0 | ks) ? 1u : 0u);
       }
     }
-  } else {
-    // =========================== compute warps ===========================
-    const int lane_grp = warp & 3;     // TMEM lanes [32*lane_grp, +32)
-    const int grp_rank = warp >> 2;    // 0..3: which of the warps sharing that lane group
+    wgmma_commit();
+    wgmma_wait_all();
+#pragma unroll
+    for (int nb = 0; nb < 4; ++nb) reg_fence(acc2[nb]);
+  }
 
-    // ---- per-thread geometry, computed ONCE.  The thread <-> pixel maps never change (epilogue 1: TMEM lane
-    // -> halo pixel of every M-tile; depthwise: thread -> output pixel pair / channel group), so all the
-    // divisions, swizzle terms and edge tests live in a handful of registers instead of being redone for
-    // every 64-channel chunk (they were ~1/3 of the instructions the compute warps issued).
-    const int quarter = grp_rank;                     // this warp's 16 of the chunk's 64 columns (epilogue 1)
-    const int lgl = lane_grp * 32 + lane;             // TMEM lane == pixel row inside an M-tile
-    const int M1 = a.M1;
-    const int my_tiles = kExpand ? min(a.m1_tiles, (M1 - lane_grp * 32 + 127) >> 7) : 0;  // tiles with a live lane
-    // E address of pixel (tile 0, lgl), 16-byte chunks quarter*2 and quarter*2+1 (p & 7 == lane & 7)
-    const uint32_t e_addr0 = s_e + ((uint32_t)lgl << 7) + ((((uint32_t)(quarter * 2)) ^ ((uint32_t)lane & 7u)) << 4);
-    const uint32_t e_addr1 = s_e + ((uint32_t)lgl << 7) + ((((uint32_t)(quarter * 2 + 1)) ^ ((uint32_t)lane & 7u)) << 4);
-    uint32_t valid_mask = 0;  // bit t: this lane's pixel of tile t exists (p < M1)
-    for (int t = 0; t < my_tiles; ++t)
-      if (t * 128 + lgl < M1) valid_mask |= 1u << t;
-    // depthwise: first (normally only) work item of this thread
-    struct DwGeom {
-      uint32_t col[3];   // byte offsets (from the tile base) of the tap columns of the top tap row, swizzle included
-      uint32_t a2[2];    // byte offsets (from the A2 buffer) of the output pixel(s), swizzle included
-      uint32_t g;        // 8-channel group inside the chunk (the same for every lane of a warp)
-      bool ok_l, ok_r, active, second;
-    };
-    // A thread computes TWO VERTICALLY adjacent outputs of one 8-channel group per work item, so that the input rows
-    // they share are loaded once: stride 1 -> 12 tile loads serve 18 taps, stride 2 -> 15 serve 18.
-    // Lane mapping (the depthwise phase is bound by shared-memory wavefronts, profiles/r02_fused_trace.txt):
-    //   stride 1: the 32 lanes of a warp take 32 horizontally consecutive items of the SAME channel group.  The
-    //             depthwise weights / bias are then warp-uniform loads (one broadcast wavefront instead of four) and
-    //             the tile loads of 8 consecutive pixels hit 8 different 16-byte columns (the 128-byte swizzle).
-    //   stride 2: consecutive outputs read pixels TWO columns apart, which under a uniform channel group folds onto
-    //             four swizzle columns (a measured 2-way bank conflict); there a quarter-warp is one item x the eight
-    //             channel groups, as before.
-    constexpr bool dw_uniform_g = (kStride == 1);
-    const int dw_pixels = ((a.TH + 1) >> 1) * a.Wo;                            // work items per channel group
-    const int dw_blocks = dw_uniform_g ? (dw_pixels + 31) >> 5 : (dw_pixels + 3) >> 2;   // per warp: 32 items x 1 group, or 4 x 8
-    // item `it` of a chunk with `ng` live 8-channel groups (8, or 2 / 4 / 6 in a ragged last chunk)
-    auto make_geom = [&](int it, int ng) {
-      DwGeom q;
-      int pix, gq;
-      if (dw_uniform_g) {
-        const int wi = it >> 5;              // warp-item: (pixel block, channel group)
-        int pb;
-        if (ng == 8) { pb = wi >> 3; gq = wi & 7; }
-        else if (ng == 4) { pb = wi >> 2; gq = wi & 3; }
-        else if (ng == 2) { pb = wi >> 1; gq = wi & 1; }
-        else { pb = (int)(((uint32_t)wi * 43691u) >> 18); gq = wi - 6 * pb; }  // ng == 6
-        pix = pb * 32 + (it & 31);
-      } else {
-        if (ng == 8) { pix = it >> 3; gq = it & 7; }
-        else if (ng == 4) { pix = it >> 2; gq = it & 3; }
-        else if (ng == 2) { pix = it >> 1; gq = it & 1; }
-        else { pix = (int)(((uint32_t)it * 43691u) >> 18); gq = it - 6 * pix; }  // ng == 6, it < 2^15
-      }
-      q.g = (uint32_t)gq;
-      q.active = pix < dw_pixels;
-      const int r2 = (int)(((uint32_t)pix * a.magic_wo) >> 16);
-      const int ow = pix - r2 * a.Wo, oh = 2 * r2;
-      q.second = oh + 1 < a.TH;
-      const int o0 = oh * a.Wo + ow;
-      const int iw0 = ow * kStride - 1;  // leftmost tap column (may be -1)
-      const uint32_t prow = (uint32_t)(oh * kStride * a.W);
+  // epilogue: + bias (+ block input) -> bf16
 #pragma unroll
-      for (int c = 0; c < 3; ++c) {
-        const uint32_t pcol = (uint32_t)(iw0 + c);  // W % 8 == 0: the XOR term depends on the column only
-        q.col[c] = ((prow + pcol) << 7) + ((((uint32_t)gq ^ pcol) & 7u) << 4);
-      }
-      q.ok_l = q.active && iw0 >= 0;
-      q.ok_r = q.active && (iw0 + 2 < a.W);
-      const int o1 = o0 + a.Wo;
-      q.a2[0] = ((uint32_t)o0 << 7) + ((((uint32_t)gq ^ (uint32_t)o0) & 7u) << 4);
-      q.a2[1] = ((uint32_t)o1 << 7) + ((((uint32_t)gq ^ (uint32_t)o1) & 7u) << 4);
-      return q;
-    };
-    const DwGeom geom0 = make_geom(tid, 8);
-    const uint32_t row_pitch = (uint32_t)a.W << 7;  // bytes between vertically adjacent pixels (W % 8 == 0)
-    const uint32_t wd_tap_pitch = (uint32_t)cmid64 * 2u;
-    const __half2 e_one = __floats2half2_rn(1.f, 1.f), h_six = __floats2half2_rn(6.f, 6.f);
-    const __half2 h_zero = __floats2half2_rn(0.f, 0.f);
-
-    int ti = 0, j = 0, b = 0, ho0 = 0, h0 = -1;
-    // ---- epilogue 2: D2 -> +b2 (+ residual from the X tile) -> bf16 -> Y.  For a block WITHOUT expansion it is deferred:
-    // it runs after the depthwise of the next item (first chunk of the next tile), so the tile's last projection MMA
-    // retires under that work instead of being waited for (the control warp does not touch D2 again before bar_tile).
-    // With an expansion conv the next tile's X load waits for this epilogue (residual), so there it stays in place.
-    bool epi_pending = false;
-    int ep_b = 0, ep_ho0 = 0, ep_slot = 0, ep_kuse = 0;
-    auto do_epilogue = [&]() {
-      mbar_wait_relaxed(&bar_mma2[ep_slot], (uint32_t)ep_kuse & 1u);
-      tcgen05_fence_after();
-      const int o = lane_grp * 32 + lane;  // output pixel of this thread's TMEM lane
-      const int oh = (int)(((uint32_t)o * a.magic_wo) >> 16), ow = o - oh * a.Wo;
-      const int ho = ep_ho0 + oh;
-      const bool valid = (o < a.M2) && (ho < a.Ho);
-      const int n_out_items = (a.cout_p + 31) / 32;
-      __nv_bfloat16* yrow = a.Y + (((int64_t)ep_b * a.Ho + ho) * a.Wo + ow) * a.cout_p;
-      const uint32_t pc = (uint32_t)((oh + 1) * a.W + ow);  // centre input pixel (stride-1 residual blocks)
-      for (int it = grp_rank; it < n_out_items; it += kGrpWarps) {
-        const int c0 = it * 32;
-        const int width = min(32, a.cout_p - c0);  // 32 or 16 (cout_p % 16 == 0)
-        uint32_t v[32];
-        if (width == 32) {
-          tmem_ld_x32(tmem_d2 + ((uint32_t)(lane_grp * 32) << 16) + (uint32_t)c0, v);
-        } else {
-          uint32_t lo[16];
-          tmem_ld_x16(tmem_d2 + ((uint32_t)(lane_grp * 32) << 16) + (uint32_t)c0, lo);
+  for (int h = 0; h < 2; ++h) {
+    const int px = warp * 16 + (lane >> 2) + 8 * h;
+    const int oy = oy0 + (px >> 3), ox = ox0 + (px & 7);
+    if (oy >= a.Ho || ox >= a.Wo) continue;
+    const int64_t pix = ((int64_t)b * a.Ho + oy) * a.Wo + ox;
 #pragma unroll
-          for (int e = 0; e < 16; ++e) v[e] = lo[e];
+    for (int nb = 0; nb < 4; ++nb) {
+      if (nb >= n2_blocks) continue;
 #pragma unroll
-          for (int e = 16; e < 32; ++e) v[e] = 0u;
+      for (int j = 0; j < 8; ++j) {
+        const int n = nb * 64 + 8 * j + 2 * quad;
+        if (n >= a.cout_p) continue;
+        float f0 = acc2[nb][4 * j + 2 * h] + __ldg(&a.b2[n]);
+        float f1 = acc2[nb][4 * j + 2 * h + 1] + __ldg(&a.b2[n + 1]);
+        if (a.residual) {  // stride 1, cin_p == cout_p: the block input at the same pixel
+          const float2 r = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(a.X + pix * a.cin_p + n));
+          f0 += r.x;
+          f1 += r.y;
         }
-        tmem_ld_wait();
-        if (valid) {
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            if (q * 8 < width) {
-              float f[8];
-#pragma unroll
-              for (int e = 0; e < 8; ++e) f[e] = __uint_as_float(v[q * 8 + e]) + s_b2[c0 + q * 8 + e];
-              if (a.residual) {
-                const int c = c0 + q * 8;
-                const uint4 raw = lds128(s_x + (uint32_t)(c >> 6) * x_kb_bytes +
-                                         sw128_offset(pc, (uint32_t)((c & 63) >> 3)));
-                const __nv_bfloat162* h2 = reinterpret_cast<const __nv_bfloat162*>(&raw);
-#pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                  const float2 f2 = __bfloat1622float2(h2[e]);
-                  f[2 * e] += f2.x;
-                  f[2 * e + 1] += f2.y;
-                }
-              }
-              uint4 pk;
-              pk.x = pack2(f[0], f[1]);
-              pk.y = pack2(f[2], f[3]);
-              pk.z = pack2(f[4], f[5]);
-              pk.w = pack2(f[6], f[7]);
-              *reinterpret_cast<uint4*>(yrow + c0 + q * 8) = pk;
-            }
-          }
-        }
-      }
-      tcgen05_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_tile);
-      epi_pending = false;
-    };
-    uint32_t inside_mask = 0;  // bit t: this lane's pixel of tile t is a real image row (else: zero padding)
-    uint32_t all_inside_mask = 0;
-    for (int w = 0; w < n_items; ++w) {
-      const bool first = (j == 0), last = (j == a.n_chunks - 1);
-      if (first) {
-        const int tile = (int)blockIdx.x + ti * (int)gridDim.x;
-        b = tile / a.tiles_per_window;
-        ho0 = (tile - b * a.tiles_per_window) * a.TH;
-        h0 = ho0 * kStride - 1;
-        inside_mask = 0;
-        for (int t = 0; t < my_tiles; ++t) {
-          const int ih = (int)(((uint32_t)(t * 128 + lgl) * a.magic_w) >> 16);  // halo row of this lane's pixel
-          if ((uint32_t)(h0 + ih) < (uint32_t)a.H) inside_mask |= 1u << t;
-        }
-        inside_mask &= valid_mask;
-        all_inside_mask = 0;  // bit t: the whole warp is inside for tile t (warp-uniform fast path)
-        for (int t = 0; t < my_tiles; ++t)
-          if (__all_sync(0xffffffffu, (inside_mask >> t) & 1u)) all_inside_mask |= 1u << t;
-      }
-      const int c_base = j * kCK;
-      // ragged last chunk (cmid_p % 64 != 0): channels [c_valid, 64) do not exist.  Their epilogue-1 quarters and
-      // depthwise channel groups are skipped outright -- nothing downstream reads them (the projection MMA of
-      // this chunk runs c_valid / 16 k-steps), and for a 144-channel block they were a quarter of all the work
-      const int c_valid = min(kCK, a.cmid_p - c_base);
-      AM_TRACE(0);
-      if (kExpand) {
-        if (first)
-          for (int kb = 0; kb < a.kb_in; ++kb) mbar_wait_relaxed(&bar_xk[kb], (uint32_t)ti & 1u);
-      } else {
-        mbar_wait_relaxed(&bar_xk[j], (uint32_t)ti & 1u);  // the depthwise of chunk j reads X k-block j
-      }
-
-      // ---- epilogue 1: TMEM -> +b1, ReLU6, zero outside the image -> fp16 -> E (swizzled)
-      uint32_t dw_src = s_x + (uint32_t)j * x_kb_bytes;  // no-expand block: depthwise reads X k-block j
-      if (kExpand) {
-        AM_TRACE(1);
-        const int ds = (a.d1_bufs == 2) ? (w & 1) : 0;
-        const uint32_t d1_base = tmem_base + (uint32_t)ds * d1_cols + ((uint32_t)(lane_grp * 32) << 16) + (uint32_t)(quarter * 16);
-        mbar_wait_relaxed(&bar_mma1[ds], (uint32_t)((a.d1_bufs == 2) ? (w >> 1) : w) & 1u);
-        AM_TRACE(2);
-        tcgen05_fence_after();
-        // items = (M-tile, 16-column quarter).  The four warps of a lane group take one quarter each
-        // (its 16 biases are loaded once per chunk) and walk the M-tiles, two TMEM loads in flight before
-        // each wait.  Tiles whose 32 lanes of this lane group lie beyond the M1 halo pixels are skipped.
-        uint32_t bw[8];
-        {
-          const uint4 b0 = lds128(s_b1_u32 + (uint32_t)(c_base + quarter * 16) * 2u);
-          const uint4 b1v = lds128(s_b1_u32 + (uint32_t)(c_base + quarter * 16 + 8) * 2u);
-          bw[0] = b0.x; bw[1] = b0.y; bw[2] = b0.z; bw[3] = b0.w;
-          bw[4] = b1v.x; bw[5] = b1v.y; bw[6] = b1v.z; bw[7] = b1v.w;
-        }
-        auto epi1_item = [&](int t, const uint32_t (&v)[16]) {
-          // pixel exists (p < M1) and is a real image row; halo rows above / below the image get zeros (the
-          // depthwise zero padding) through a zero multiplier and a zero bias -- branch-free
-          const bool valid = (valid_mask >> t) & 1u, inside = (inside_mask >> t) & 1u;
-          const uint32_t toff = (uint32_t)t * (uint32_t)kTileBytes;
-          const __half2 mul = inside ? e_one : h_zero;
-#pragma unroll
-          for (int hq = 0; hq < 2; ++hq) {  // two 16-byte chunks (8 channels each)
-            uint32_t o[4];
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              __half2 h = __floats2half2_rn(__uint_as_float(v[hq * 8 + 2 * e]), __uint_as_float(v[hq * 8 + 2 * e + 1]));
-              // relu6(h + b1): the add and the lower clamp in one HFMA2.RELU
-              h = __hmul2(__hmin2(__hfma2_relu(h, e_one, as_h2(bw[hq * 4 + e])), h_six), mul);
-              o[e] = *reinterpret_cast<uint32_t*>(&h);
-            }
-            sts128_if((hq ? e_addr1 : e_addr0) + toff, make_uint4(o[0], o[1], o[2], o[3]), valid);
-          }
-        };
-        auto epi1_item_fast = [&](int t, const uint32_t (&v)[16]) {  // every lane valid and inside
-          const uint32_t toff = (uint32_t)t * (uint32_t)kTileBytes;
-#pragma unroll
-          for (int hq = 0; hq < 2; ++hq) {
-            uint32_t o[4];
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              __half2 h = __floats2half2_rn(__uint_as_float(v[hq * 8 + 2 * e]), __uint_as_float(v[hq * 8 + 2 * e + 1]));
-              h = __hmin2(__hfma2_relu(h, e_one, as_h2(bw[hq * 4 + e])), h_six);
-              o[e] = *reinterpret_cast<uint32_t*>(&h);
-            }
-            sts128((hq ? e_addr1 : e_addr0) + toff, make_uint4(o[0], o[1], o[2], o[3]));
-          }
-        };
-        for (int t0 = 0; t0 < ((quarter * 16 < c_valid) ? my_tiles : 0); t0 += 2) {  // warp-uniform skip
-          uint32_t va[16], vb[16];
-          const bool two = t0 + 1 < my_tiles;
-          tmem_ld_x16(d1_base + (uint32_t)(t0 * kCK), va);
-          if (two) tmem_ld_x16(d1_base + (uint32_t)((t0 + 1) * kCK), vb);
-          tmem_ld_wait();
-          if ((all_inside_mask >> t0) & 1u) epi1_item_fast(t0, va);  // warp-uniform
-          else epi1_item(t0, va);
-          if (two) {
-            if ((all_inside_mask >> (t0 + 1)) & 1u) epi1_item_fast(t0 + 1, vb);
-            else epi1_item(t0 + 1, vb);
-          }
-        }
-        tcgen05_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&bar_epi1[ds]);
-        AM_TRACE(3);
-        compute_bar_sync();  // E complete
-        dw_src = s_e;
-      }
-
-      // ---- depthwise 3x3 (+bd, ReLU6) -> A2 in the MMA operand layout
-      // depthwise weights / bias of this thread's channel group come from the CTA-resident fp16 smem copy,
-      // one LDS.128 per tap right where it is used (a thread has one work item per chunk, so preloading
-      // all nine taps bought nothing and cost 36 of the 96 registers); channels beyond cmid_p are zero
-      const int slot = (a.a2_bufs == 2) ? (w & 1) : 0;          // A2 buffer ...
-      const int kuse = (a.a2_bufs == 2) ? (w >> 1) : w;         // ... and how often it was used before
-      AM_TRACE(4);
-      if (kuse > 0) mbar_wait_relaxed(&bar_mma2[slot], (uint32_t)(kuse - 1) & 1u);  // its previous MMA2 released it
-      AM_TRACE(5);
-      const uint32_t a2_dst = s_a2 + (uint32_t)slot * kTileBytes;
-      // tap loads: predicated LDS.128 (zeros beyond the left / right image edge); kFp16 is the tile's format
-      auto load_px = [&](uint32_t addr, bool ok, auto is_fp16, __half2 (&x)[4]) {
-        const uint4 raw = lds128_if(addr, ok);
-        if constexpr (decltype(is_fp16)::value) {
-          x[0] = as_h2(raw.x); x[1] = as_h2(raw.y); x[2] = as_h2(raw.z); x[3] = as_h2(raw.w);
-        } else {  // block without expansion fed by a bf16 tensor
-          x[0] = bf2_to_h2(raw.x); x[1] = bf2_to_h2(raw.y); x[2] = bf2_to_h2(raw.z); x[3] = bf2_to_h2(raw.w);
-        }
-      };
-      auto store_px_if = [&](uint32_t a2_off, const __half2 (&acc)[4], bool ok) {
-        uint4 pk;
-        __half2 t;
-        t = __hmin2(acc[0], h_six); pk.x = *reinterpret_cast<uint32_t*>(&t);
-        t = __hmin2(acc[1], h_six); pk.y = *reinterpret_cast<uint32_t*>(&t);
-        t = __hmin2(acc[2], h_six); pk.z = *reinterpret_cast<uint32_t*>(&t);
-        t = __hmin2(acc[3], h_six); pk.w = *reinterpret_cast<uint32_t*>(&t);
-        sts128_if(a2_dst + a2_off, pk, ok);
-      };
-      auto dw_item = [&](const DwGeom& q, auto is_fp16) {
-        const uint32_t wa0 = s_wd_u32 + (uint32_t)(c_base + (int)q.g * 8) * 2u;   // warp-uniform: broadcast loads
-        __half2 bdv[4];
-        {
-          const uint4 r = lds128(s_bd_u32 + (uint32_t)(c_base + (int)q.g * 8) * 2u);
-          bdv[0] = as_h2(r.x);
-          bdv[1] = as_h2(r.y);
-          bdv[2] = as_h2(r.z);
-          bdv[3] = as_h2(r.w);
-        }
-        __half2 acc0[4], acc1[4];
-#pragma unroll
-        for (int e = 0; e < 4; ++e) acc0[e] = acc1[e] = bdv[e];
-        // input rows 0 .. kStride + 2: rows [0, 3) feed the upper output, [kStride, kStride + 3) the lower one.
-        // Each of the nine weight vectors is loaded ONCE and kept for the second use (36 registers).
-        constexpr int kRows = kStride + 3;
-        uint32_t rb = dw_src;
-        __half2 wk[3][3][4];
-#pragma unroll
-        for (int r = 0; r < kRows; ++r, rb += row_pitch) {
-          __half2 x[3][4];
-          const bool row_ok = (r < 3) || q.second;   // the last kStride rows belong to the lower output only
-          load_px(rb + q.col[0], q.ok_l && row_ok, is_fp16, x[0]);
-          load_px(rb + q.col[1], q.active && row_ok, is_fp16, x[1]);
-          load_px(rb + q.col[2], q.ok_r && row_ok, is_fp16, x[2]);
-          if (r < 3) {  // upper output, tap row r
-#pragma unroll
-            for (int dx = 0; dx < 3; ++dx) {
-              const uint4 wr = lds128(wa0 + (uint32_t)(r * 3 + dx) * wd_tap_pitch);
-              wk[r][dx][0] = as_h2(wr.x); wk[r][dx][1] = as_h2(wr.y); wk[r][dx][2] = as_h2(wr.z); wk[r][dx][3] = as_h2(wr.w);
-#pragma unroll
-              for (int e = 0; e < 4; ++e)
-                acc0[e] = (r == 2 && dx == 2) ? __hfma2_relu(x[dx][e], wk[r][dx][e], acc0[e]) : __hfma2(x[dx][e], wk[r][dx][e], acc0[e]);
-            }
-          }
-          if (r >= kStride) {  // lower output, tap row r - kStride
-#pragma unroll
-            for (int dx = 0; dx < 3; ++dx)
-#pragma unroll
-              for (int e = 0; e < 4; ++e)
-                acc1[e] = (r == kRows - 1 && dx == 2) ? __hfma2_relu(x[dx][e], wk[r - kStride][dx][e], acc1[e])
-                                                      : __hfma2(x[dx][e], wk[r - kStride][dx][e], acc1[e]);
-          }
-        }
-        store_px_if(q.a2[0], acc0, q.active);
-        store_px_if(q.a2[1], acc1, q.active && q.second);
-      };
-      {
-        using SrcFmt = std::integral_constant<bool, kFp16Src>;
-        const int ng = c_valid >> 3;                  // live channel groups: 8 except in a ragged last chunk
-        const int dw_limit = dw_uniform_g ? dw_blocks * 32 * ng : dw_pixels * ng;   // uniform-g: whole warps, tail lanes predicated off
-        DwGeom q = (ng == 8) ? geom0 : make_geom(tid, ng);
-        for (int it = tid; it < dw_limit; it += kComputeThreads) {  // normally one pass
-          dw_item(q, SrcFmt{});
-          if (it + kComputeThreads < dw_limit) q = make_geom(it + kComputeThreads, ng);
-        }
-      }
-      if (!kExpand && epi_pending) do_epilogue();
-      fence_proxy_async();  // generic-proxy smem writes -> visible to the tensor core (async proxy)
-      __syncwarp();
-      AM_TRACE(6);
-      if (lane == 0) mbar_arrive(&bar_a2[slot]);
-      // keep the compute warps in lock step per item: mbarrier arrivals are anonymous, so a warp running
-      // ahead must not arrive for item w+1 inside item w's phase; also: every warp is done reading E
-      // before the next epilogue 1 overwrites it.  A block without expansion and with two A2 buffers needs
-      // neither: there is no E, consecutive items arrive on different barriers, and a warp two items ahead
-      // first waits for MMA2 of this item -- which needs every warp's arrival.  Its warps run free.
-      if (kExpand || a.a2_bufs != 2) compute_bar_sync();
-      AM_TRACE(7);
-
-      // ---- epilogue 2 (last chunk of the tile)
-      if (last) {
-        ep_b = b;
-        ep_ho0 = ho0;
-        ep_slot = slot;
-        ep_kuse = kuse;
-        if (kExpand) do_epilogue();
-        else epi_pending = true;
-      }
-      if (++j == a.n_chunks) {
-        j = 0;
-        ++ti;
+        *reinterpret_cast<__nv_bfloat162*>(a.Y + pix * a.cout_p + n) = __floats2bfloat162_rn(f0, f1);
       }
     }
-    if (epi_pending) do_epilogue();
   }
-  tcgen05_fence_before();
-  __syncthreads();
-  if (warp == kComputeWarps) {
-    tcgen05_fence_after();
-    tmem_dealloc(tmem_base, kTmemCols);
-  }
-}
-
-// ---------------------------------------------------------------- host
-static size_t layout_smem(Args& a) {
-  size_t off = 0;
-  const size_t rows_bytes = round_up_dev((uint32_t)a.M1 * 128u, 1024u);
-  a.off_x = (uint32_t)off;
-  off += (size_t)a.kb_in * rows_bytes;
-  a.off_e = (uint32_t)off;
-  if (a.has_expand) off += rows_bytes;
-  a.off_a2 = (uint32_t)off;
-  off += (size_t)a.a2_bufs * kTileBytes;
-  a.off_w1 = (uint32_t)off;
-  a.w1_stage_bytes = a.has_expand ? (uint32_t)a.kb_in * kCK * 128u : 0u;
-  off += 2 * (size_t)a.w1_stage_bytes;
-  a.off_w2 = (uint32_t)off;
-  a.w2_stage_bytes = (uint32_t)round_up((size_t)a.cout_p * 128u, 1024);
-  off += 2 * (size_t)a.w2_stage_bytes;
-  a.off_small = (uint32_t)off;
-  off += (size_t)a.cout_p * 4;                                   // b2 (fp32)
-  off += (size_t)11 * (((size_t)a.cmid_p + 63) & ~(size_t)63) * 2;  // depthwise weights + bias + b1 (fp16, padded)
-  off = round_up(off, 16);
-  a.off_bar = (uint32_t)off;
-  off += 256;
-  return off + 1024;  // alignment slack
 }
 
 bool plan(const BlockDesc& d, Plan* out) {
-  if (d.cout_p > 256 || d.cout_p % 16 || d.cin_p % 16 || d.cmid_p % 16) return false;
-  if (d.W > 64 || d.W < 8 || d.W % 8) return false;    // swizzle term row independent; 16-bit magic division
-  if (!d.has_expand && (d.cmid_p != d.cin_p || d.stride != 1)) return false;  // kernel variants: see run()
-  if (d.residual && (d.stride != 1 || d.cin_p != d.cout_p || !d.has_expand)) return false;
-  if ((d.cin_p + 63) / 64 > kMaxKb) return false;
-  const int Ho = (d.H + 2 - 3) / d.stride + 1, Wo = (d.W + 2 - 3) / d.stride + 1;
-  const int kb_in = (d.cin_p + 63) / 64;
-  for (int TH = std::min(Ho, 128 / std::max(Wo, 1)); TH >= 1; --TH) {
-    Args a{};
-    a.has_expand = d.has_expand;
-    a.cout_p = d.cout_p;
-    a.cmid_p = d.cmid_p;
-    a.kb_in = kb_in;
-    a.IH = (TH - 1) * d.stride + 3;
-    a.M1 = a.IH * d.W;
-    a.m1_tiles = (a.M1 + 127) / 128;
-    if (a.IH > 256) continue;
-    int d1_bufs = 2;
-    if (!d.has_expand || 2 * a.m1_tiles * kCK + d.cout_p > kTmemCols) d1_bufs = 1;
-    const int tmem = (d.has_expand ? d1_bufs * a.m1_tiles * kCK : 0) + d.cout_p;
-    if (tmem > kTmemCols) continue;
-    a.a2_bufs = 2;
-    size_t smem = layout_smem(a);
-    constexpr size_t kSmemLimit = 232448 - 512;  // sm_100 opt-in maximum per CTA
-    if (smem > kSmemLimit) {
-      a.a2_bufs = 1;
-      smem = layout_smem(a);
-    }
-    if (smem > kSmemLimit) continue;
-    out->TH = TH;
-    out->a2_bufs = a.a2_bufs;
-    out->d1_bufs = d1_bufs;
-    out->smem_bytes = smem;
-    return true;
+  if (d.stride != 1 && d.stride != 2) return false;
+  if (d.cout_p > kMaxCout || d.cout_p % 16 || d.cmid_p % 16 || d.cin_p % 16) return false;
+  if (!d.has_expand && d.cin_p != d.cmid_p) return false;
+  if (d.residual && (d.stride != 1 || d.cin_p != d.cout_p)) return false;
+  const Layout l = layout(d.stride, d.has_expand != 0, d.cin_p, d.cout_p);
+  out->smem_bytes = (size_t)l.total + 1024;
+  return out->smem_bytes <= kSmemMax;
+}
+
+template <int S, bool kExpand>
+static int launch(const Args& a, int B, size_t smem, cudaStream_t st) {
+  static bool attr_set = false;
+  if (!attr_set) {
+    AM_CUDA(cudaFuncSetAttribute(fused_block_kernel<S, kExpand>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemMax));
+    attr_set = true;
   }
-  return false;
+  const int64_t grid = (int64_t)B * a.tiles_y * a.tiles_x;
+  AM_CHECK(grid < ((int64_t)1 << 31), "fused block: %lld tiles is too many for one launch", (long long)grid);
+  AM_LAUNCH((fused_block_kernel<S, kExpand>), (unsigned)grid, kThreads, smem, st, a);
+  return AM_OK;
 }
 
 int run(const BlockDesc& d, const Plan& p, const __nv_bfloat16* X, const __nv_bfloat16* W1, const float* b1,
-        const float* wd, const float* bd, const __half* W2, const float* b2, __nv_bfloat16* Y, int B,
+        const float* wd, const float* bd, const __nv_bfloat16* W2, const float* b2, __nv_bfloat16* Y, int B,
         cudaStream_t st) {
+  AM_CHECK(X && wd && bd && W2 && b2 && Y && (!d.has_expand || (W1 && b1)), "fused block: NULL operand");
   Args a{};
-  a.B = B;
-  a.H = d.H;
-  a.W = d.W;
-  a.stride = d.stride;
-  a.Ho = (d.H + 2 - 3) / d.stride + 1;
-  a.Wo = (d.W + 2 - 3) / d.stride + 1;
-  a.cin_p = d.cin_p;
-  a.cmid_p = d.cmid_p;
-  a.cout_p = d.cout_p;
-  a.has_expand = d.has_expand;
-  a.residual = d.residual;
-  a.TH = p.TH;
-  a.IH = (p.TH - 1) * d.stride + 3;
-  a.M1 = a.IH * d.W;
-  a.m1_tiles = (a.M1 + 127) / 128;
-  a.M2 = p.TH * a.Wo;
-  a.kb_in = (d.cin_p + 63) / 64;
-  a.n_chunks = (d.cmid_p + kCK - 1) / kCK;
-  a.tiles_per_window = (a.Ho + p.TH - 1) / p.TH;
-  a.total_tiles = a.tiles_per_window * B;
+  a.X = X;
+  a.W1 = W1;
   a.b1 = b1;
   a.wd = wd;
   a.bd = bd;
+  a.W2 = W2;
   a.b2 = b2;
   a.Y = Y;
-  a.a2_bufs = p.a2_bufs;
-  a.d1_bufs = p.d1_bufs;
-  a.x_is_fp16 = d.x_is_fp16;
-  a.magic_wo = (65536u + (uint32_t)a.Wo - 1u) / (uint32_t)a.Wo;
-  a.magic_w = (65536u + (uint32_t)a.W - 1u) / (uint32_t)a.W;
-  const size_t smem = layout_smem(a);
-  AM_CHECK(smem == p.smem_bytes, "fused block: plan / launch smem mismatch");
-
-  CUtensorMap mx, mw1, mw2;
-  {
-    const uint64_t dims[4] = {(uint64_t)d.cin_p, (uint64_t)d.W, (uint64_t)d.H, (uint64_t)B};
-    const uint64_t str[3] = {(uint64_t)d.cin_p * 2, (uint64_t)d.W * d.cin_p * 2, (uint64_t)d.H * d.W * d.cin_p * 2};
-    const uint32_t box[4] = {64, (uint32_t)d.W, (uint32_t)a.IH, 1};
-    AM_TRY(gemm::encode_map_bf16(&mx, X, 4, dims, str, box));
-  }
-  if (d.has_expand) {
-    const uint64_t dims[2] = {(uint64_t)d.cin_p, (uint64_t)d.cmid_p};
-    const uint64_t str[1] = {(uint64_t)d.cin_p * 2};
-    const uint32_t box[2] = {64, (uint32_t)kCK};
-    AM_TRY(gemm::encode_map_bf16(&mw1, W1, 2, dims, str, box));
-  } else {
-    mw1 = mx;  // unused
-  }
-  {
-    const uint64_t dims[2] = {(uint64_t)d.cmid_p, (uint64_t)d.cout_p};
-    const uint64_t str[1] = {(uint64_t)d.cmid_p * 2};
-    const uint32_t box[2] = {64, (uint32_t)d.cout_p};
-    // fp16 data through a 16-bit tiled map: TMA only moves the bytes (zero OOB fill is format-agnostic)
-    AM_TRY(gemm::encode_map_bf16(&mw2, W2, 2, dims, str, box));
-  }
-  using KernelFn = void (*)(const __grid_constant__ CUtensorMap, const __grid_constant__ CUtensorMap,
-                            const __grid_constant__ CUtensorMap, const Args);
-  KernelFn fn = nullptr;
-  int variant = 0;
-  const bool fp16_src = d.has_expand || d.x_is_fp16;
-  if (d.has_expand && d.stride == 1) { fn = fused_block_kernel<true, 1, true>; variant = 0; }
-  else if (d.has_expand && d.stride == 2) { fn = fused_block_kernel<true, 2, true>; variant = 1; }
-  else if (!d.has_expand && d.stride == 1 && fp16_src) { fn = fused_block_kernel<false, 1, true>; variant = 2; }
-  else if (!d.has_expand && d.stride == 1) { fn = fused_block_kernel<false, 1, false>; variant = 3; }
-  AM_CHECK(fn != nullptr, "fused block: no kernel variant for expand=%d stride=%d", d.has_expand, d.stride);
-  static size_t attr[4] = {0, 0, 0, 0};
-  if (smem > attr[variant]) {
-    AM_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr[variant] = smem;
-  }
-  const int grid = std::max(1, std::min(a.total_tiles, sm_count()));
-  static const bool trace_on = std::getenv("AM_FUSED_TRACE") != nullptr;
-  DevBuf<long long> tr;
-  if (trace_on) {
-    AM_TRY(tr.alloc((size_t)kTraceItems * 16));
-    AM_CUDA(cudaMemsetAsync(tr.p, 0, (size_t)kTraceItems * 16 * 8, st));
-    a.trace = tr.p;
-  }
-  {
-    auto fused_block_kernel = fn;  // (keeps the profiler's kernel name)
-    AM_LAUNCH(fused_block_kernel, grid, kThreads, smem, st, mx, mw1, mw2, a);
-  }
-  if (trace_on) {
-    std::vector<long long> h((size_t)kTraceItems * 16);
-    AM_CUDA(cudaStreamSynchronize(st));
-    AM_CUDA(cudaMemcpy(h.data(), tr.p, h.size() * 8, cudaMemcpyDeviceToHost));
-    const int n = std::min(kTraceItems, ((a.total_tiles - 1) / grid + 1) * a.n_chunks);
-    std::fprintf(stderr, "[fused trace] H=%d W=%d cin=%d cmid=%d cout=%d s=%d TH=%d m1_tiles=%d chunks=%d a2=%d tiles/CTA=%d\n",
-                 a.H, a.W, a.cin_p, a.cmid_p, a.cout_p, a.stride, a.TH, a.m1_tiles, a.n_chunks, a.a2_bufs * 10 + a.d1_bufs,
-                 (a.total_tiles - 1) / grid + 1);
-    const long long t0 = h[0];
-    for (int w = a.n_chunks; w < std::min(n, 3 * a.n_chunks); ++w) {
-      const long long* e = &h[(size_t)w * 16];
-      std::fprintf(stderr,
-                   "  w=%2d @%7lld | compute: waitX %5lld  waitMMA1 %5lld  epi1 %5lld  bar %5lld  waitMMA2 %5lld  dw %5lld  bar %5lld"
-                   " | control: A %5lld (epi %5lld w1 %5lld rest %5lld) waitA2 %5lld  mma2 %5lld  CD %5lld  E %5lld\n",
-                   w, e[0] - t0, e[1] ? e[1] - e[0] : 0, e[2] - e[1], e[3] - e[2], e[4] - e[3], e[5] - e[4], e[6] - e[5],
-                   e[7] - e[6], e[9] - e[8], e[14] ? e[14] - e[8] : 0, e[15] ? e[15] - e[14] : 0, e[15] ? e[9] - e[15] : 0,
-                   e[10] - e[9], e[11] - e[10], e[12] - e[11], e[13] - e[12]);
-    }
-  }
-  return AM_OK;
+  a.H = d.H;
+  a.W = d.W;
+  a.Ho = (d.H - 1) / d.stride + 1;  // 3 x 3, pad 1
+  a.Wo = (d.W - 1) / d.stride + 1;
+  a.tiles_y = (a.Ho + kTile - 1) / kTile;
+  a.tiles_x = (a.Wo + kTile - 1) / kTile;
+  a.cin_p = d.cin_p;
+  a.cmid_p = d.cmid_p;
+  a.cout_p = d.cout_p;
+  a.residual = d.residual;
+  if (d.stride == 1) return d.has_expand ? launch<1, true>(a, B, p.smem_bytes, st) : launch<1, false>(a, B, p.smem_bytes, st);
+  return d.has_expand ? launch<2, true>(a, B, p.smem_bytes, st) : launch<2, false>(a, B, p.smem_bytes, st);
 }
 
 }  // namespace fused

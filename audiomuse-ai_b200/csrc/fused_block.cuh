@@ -1,5 +1,5 @@
-// Fused inverted-residual block (expand 1x1 -> depthwise 3x3 -> project 1x1 [+ residual]) on
-// tcgen05 / TMEM / TMA: see fused_block.cu.
+// Fused inverted-residual block (expand 1x1 -> depthwise 3x3 -> project 1x1 [+ residual]) on wgmma: see
+// fused_block.cu.
 #pragma once
 
 #include "common.cuh"
@@ -13,46 +13,20 @@ struct BlockDesc {
   int stride;                     // depthwise stride (1 or 2), pad 1
   int has_expand;                 // 0: block without expansion conv (cmid == cin)
   int residual;                   // add the block input (stride 1, cin == cout)
-  int x_is_fp16;                  // no-expand block only: X holds fp16 instead of bf16
 };
 
 struct Plan {
-  int TH = 0;                     // output rows per CTA tile
-  int a2_bufs = 1;                // projection-operand buffers (2 when shared memory allows)
-  int d1_bufs = 1;                // expansion accumulator sets in TMEM (2 when the 512 columns allow)
   size_t smem_bytes = 0;
 };
 
-// false when the block does not fit the kernel's on-chip budget (Cout > 256, TMEM, shared memory)
+// false when the block does not fit the kernel (Cout > 256, shared memory)
 bool plan(const BlockDesc& d, Plan* out);
 
+// W1 [cmid_p, cin_p] bf16, b1 [cmid_p] (NULL without an expansion conv); wd [9, cmid_p], bd [cmid_p];
+// W2 [cout_p, cmid_p] bf16, b2 [cout_p]; X [B, H, W, cin_p] -> Y [B, Ho, Wo, cout_p], NHWC bf16
 int run(const BlockDesc& d, const Plan& p, const __nv_bfloat16* X, const __nv_bfloat16* W1, const float* b1,
-        const float* wd, const float* bd, const __half* W2, const float* b2, __nv_bfloat16* Y, int B,
+        const float* wd, const float* bd, const __nv_bfloat16* W2, const float* b2, __nv_bfloat16* Y, int B,
         cudaStream_t st);
 
 }  // namespace fused
-
-// Channel-per-lane formulation of the same block (fused_block_t.cu): the expansion GEMM is transposed so that the
-// depthwise reads its taps from TMEM instead of shared memory.  Covers blocks WITH an expansion convolution whose
-// width is 16 / 32 / 64; plan() returns false for anything else and the caller uses fused::run.
-namespace fusedt {
-
-struct Plan {
-  int TH = 0;
-  int a2_bufs = 1, d1_bufs = 1;
-  int s1 = 0, s2 = 0;             // W1 / W2 shared-memory ring stages
-  size_t smem_bytes = 0;
-};
-
-bool plan(const fused::BlockDesc& d, Plan* out);
-
-// per-channel constants (depthwise taps [9, cmid_p], depthwise bias, expansion bias) packed for the kernel:
-// out holds consts_words(cmid_p) 32-bit words; built once per block when the model is loaded
-size_t consts_words(int cmid_p);
-int pack_consts(const float* wd, const float* bd, const float* b1, int cmid_p, uint32_t* out, cudaStream_t st);
-
-int run(const fused::BlockDesc& d, const Plan& p, const __nv_bfloat16* X, const __nv_bfloat16* W1, const uint32_t* cpack,
-        const __half* W2, const float* b2, __nv_bfloat16* Y, int B, cudaStream_t st);
-
-}  // namespace fusedt
 }  // namespace am

@@ -1,19 +1,16 @@
-// tcgen05 / TMEM / TMA GEMM for sm_100a (see gemm_tcgen05.cuh for the contract).
+// Warpgroup-MMA / TMA GEMM for sm_90a (see gemm_wgmma.cuh for the contract).
 //
-// Persistent, warp-specialised CTA of 320 threads, one CTA per SM:
-//   warp 0      TMA producer: cp.async.bulk.tensor loads of the A tile [128 x 64] and the
-//               B tile [BLOCK_N x 64] (bf16, 128-byte swizzle) into a 4-stage smem ring;
-//   warp 1      TMEM allocator + MMA issuer: one lane issues tcgen05.mma.cta_group::1.kind::f16
-//               (M = 128, N = BLOCK_N <= 256, K = 16 per instruction), accumulators in TMEM,
-//               double-buffered (2 x BLOCK_N of the 512 columns) so the epilogue of tile i
-//               overlaps the MMAs of tile i+1; tcgen05.commit releases smem stages / signals
-//               the epilogue through mbarriers;
-//   warps 2..9  epilogue: the tile's bias slice is staged once in smem; tcgen05.ld (32 lanes x 32
-//               columns per instruction, two warps per lane group taking alternate chunks) ->
-//               registers -> alpha / bias / ReLU6 / residual -> bf16 or fp32 -> 16-byte global stores.
-// Three mbarrier pipelines: smem full/empty (TMA <-> MMA), TMEM full/empty (MMA <-> epilogue).
-#include "gemm_tcgen05.cuh"
-#include "ptx_sm100.cuh"
+// Persistent CTA of 384 threads (three warpgroups), one CTA per SM, tile = 128 rows x BN columns:
+//   warpgroup 0   TMA producer (one elected lane of warp 0): cp.async.bulk.tensor loads of the A tile [128 x 64]
+//                 and the B tile [BN x 64] (bf16, 128-byte swizzle) into a shared-memory ring of up to 4 stages;
+//   warpgroups 1, 2   consumers, rows [0, 64) and [64, 128) of the tile: wgmma.mma_async m64nBNk16 straight from
+//                 the swizzled tiles into fp32 register accumulators, then the epilogue from registers:
+//                 alpha / bias / ReLU6 / residual -> bf16 or fp32 (+ the k-NN chunk maxima); a bf16 tile goes through
+//                 shared memory so that global stores are whole 16-byte chunks of consecutive columns.
+// Two mbarrier arrays: full (TMA -> consumers, transaction counted) and empty (consumers -> TMA).  While the
+// consumers run an epilogue the producer is already filling the ring with the next tile's first K blocks.
+#include "gemm_wgmma.cuh"
+#include "ptx_sm90.cuh"
 
 #include <mutex>
 
@@ -22,13 +19,12 @@ namespace gemm {
 
 constexpr int kBlockM = 128;
 constexpr int kBlockK = 64;            // 64 bf16 = one 128-byte swizzle row
-constexpr int kStages = 4;             // at most; 3 when a 256-wide B tile and the store staging would not fit
-constexpr int kEpiWarps = 8;           // 2 per TMEM lane group (even / odd 32-column chunks)
-constexpr int kThreads = 64 + kEpiWarps * 32;
+constexpr int kStages = 4;             // at most; fewer when a wide B tile would not fit
+constexpr int kThreads = 384;
+constexpr int kConsumerThreads = 256;
 constexpr int kATileBytes = kBlockM * kBlockK * 2;  // 16 KiB
 constexpr int kMaxBlockN = 256;
-constexpr int kTmemCols = 512;
-constexpr int kStoreStageBytes = 32 * 128;  // per epilogue warp: 32 rows x 128 B (fp32) or 64 B (bf16) for the TMA store
+constexpr size_t kSmemMax = 232448;    // 227 KiB: the opt-in limit of one block on sm_90
 
 using namespace ptx;
 
@@ -41,17 +37,23 @@ struct KernelArgs {
   void* D;
   int64_t ldd;
   int d_is_f32;
+  int d_vec;      // D rows allow 2-element vector stores (even ldd, aligned base)
   float alpha;
   const float* bias;
   const float* col_sub;
   int act;
   const __nv_bfloat16* residual;
   int64_t ld_res;
+  int res_vec;    // residual rows allow 2-element vector loads
   float* chunk_max;  // k-NN: per-32-column maxima beside D (see Epilogue::chunk_max)
   int64_t ld_cm;
-  int stages;     // smem ring depth (3 or 4)
-  int tma_store;  // epilogue writes D through shared memory + TMA tile stores (coalesced, asynchronous)
+  int stages;     // smem ring depth
+  int staged;     // bf16 D leaves through a shared-memory tile as whole 16-byte row chunks (coalesced)
 };
+
+// per consumer warpgroup: 64 rows of the tile, rows padded by 16 bytes so the fragment writes spread over the banks
+template <int BN>
+constexpr int stage_pitch() { return BN * 2 + 16; }
 
 __device__ __forceinline__ void tile_coords(const KernelArgs& a, int tile, int& m_blk, int& n_blk) {
   if (a.m_fastest) {
@@ -63,57 +65,47 @@ __device__ __forceinline__ void tile_coords(const KernelArgs& a, int tile, int& 
   }
 }
 
-__device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
-  __nv_bfloat162 h = __floats2bfloat162_rn(lo, hi);
-  return *reinterpret_cast<uint32_t*>(&h);
+__device__ __forceinline__ float epi_act(float v, int act) {
+  if (act == 1) return relu6f(v);
+  if (act == 2) return fmaxf(v, 0.f);                                         // ReLU
+  if (act == 3) return v * fminf(fmaxf(fmaf(v, 1.0f / 6.0f, 0.5f), 0.f), 1.f);  // HardSwish
+  return v;
 }
 
+template <int BN>
 __global__ void __launch_bounds__(kThreads, 1)
-gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
-                    const __grid_constant__ CUtensorMap map_d, const KernelArgs args) {
+gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
+                  const KernelArgs args) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // 1024-byte alignment for SWIZZLE_128B tiles
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  const int b_tile_bytes = args.block_n * kBlockK * 2;
-  const int stage_bytes = kATileBytes + b_tile_bytes;
+  constexpr int kBTileBytes = BN * kBlockK * 2;
+  constexpr int kStageBytes = kATileBytes + kBTileBytes;
   const int n_stages = args.stages;
-  uint8_t* store_stage = smem + n_stages * stage_bytes;  // [kEpiWarps][kStoreStageBytes], 1024-byte aligned
-  const int store_stage_bytes = args.d_is_f32 ? kStoreStageBytes : kStoreStageBytes / 2;  // per epilogue warp
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(store_stage + (args.tma_store ? kEpiWarps * store_stage_bytes : 0));
+  uint8_t* d_stage = smem + n_stages * kStageBytes;  // [2][64][stage_pitch] when args.staged
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(d_stage + (args.staged ? 2 * 64 * stage_pitch<BN>() : 0));
   uint64_t* empty_bar = full_bar + kStages;
-  uint64_t* tmem_full = empty_bar + kStages;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_empty + 2);
-  float* s_bias = reinterpret_cast<float*>(tmem_ptr + 4);  // [2][kMaxBlockN]: bias - col_sub per column
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int num_tiles = args.tiles_m * args.tiles_n;
   const int num_kb = (args.K + kBlockK - 1) / kBlockK;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     prefetch_tensormap(&map_a);
     prefetch_tensormap(&map_b);
-    if (args.tma_store) prefetch_tensormap(&map_d);
     for (int i = 0; i < n_stages; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full[i], 1);
-      mbar_init(&tmem_empty[i], kEpiWarps);
+      mbar_init(&empty_bar[i], kConsumerThreads);
     }
     fence_barrier_init();
     fence_proxy_async();
   }
-  if (warp == 1) tmem_alloc(tmem_ptr, kTmemCols);
-  tcgen05_fence_before();
   __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
 
-  if (warp == 0) {
+  if (warp < 4) {
+    regs_producer();
     // ===================== TMA producer =====================
-    if (elect_one_sync()) {
+    if (warp == 0 && elect_one_sync()) {
       int stage = 0;
       uint32_t phase = 0;
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
@@ -121,11 +113,11 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_cons
         tile_coords(args, tile, m_blk, n_blk);
         for (int kb = 0; kb < num_kb; ++kb) {
           mbar_wait(&empty_bar[stage], phase ^ 1);
-          uint8_t* sa = smem + stage * stage_bytes;
+          uint8_t* sa = smem + stage * kStageBytes;
           uint8_t* sb = sa + kATileBytes;
-          mbar_expect_tx(&full_bar[stage], (uint32_t)stage_bytes);
+          mbar_expect_tx(&full_bar[stage], (uint32_t)kStageBytes);
           tma_load_2d(sa, &map_a, &full_bar[stage], kb * kBlockK, m_blk * kBlockM);
-          tma_load_2d(sb, &map_b, &full_bar[stage], kb * kBlockK, n_blk * args.block_n);
+          tma_load_2d(sb, &map_b, &full_bar[stage], kb * kBlockK, n_blk * BN);
           if (++stage == n_stages) {
             stage = 0;
             phase ^= 1;
@@ -133,240 +125,165 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_cons
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (elect_one_sync()) {
-      const uint32_t idesc = make_idesc(kBlockM, args.block_n);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-        tcgen05_fence_after();
-        const uint32_t tmem_d = tmem_base + (uint32_t)(acc * args.block_n);
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tcgen05_fence_after();
-          const uint32_t sa = smem_u32(smem + stage * stage_bytes);
-          const uint32_t sb = sa + kATileBytes;
-          const uint64_t da = make_smem_desc(sa), db = make_smem_desc(sb);
-          const int ksteps = min(kBlockK, args.K - kb * kBlockK + 15) / 16;  // skip all-zero K tails
-#pragma unroll 1
-          for (int ks = 0; ks < ksteps; ++ks) {
-            // advance 16 bf16 = 32 bytes along K inside the swizzle atom: +2 in the (>>4) address field
-            umma_f16(tmem_d, da + (uint64_t)(ks * 2), db + (uint64_t)(ks * 2), idesc, (kb | ks) ? 1u : 0u);
-          }
-          umma_commit(&empty_bar[stage]);  // frees the smem stage once these MMAs retire
-          if (++stage == n_stages) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-        umma_commit(&tmem_full[acc]);  // accumulator complete -> epilogue
-        if (++acc == 2) {
-          acc = 0;
-          acc_phase ^= 1;
-        }
-      }
-    }
-  } else {
-    // ===================== epilogue (warps 2..9) =====================
-    const int epi_warp = warp - 2;
-    const int lane_grp = warp & 3;        // TMEM lanes [32*lane_grp, +32) are accessible to this warp
-    const int chunk_par = epi_warp >> 2;  // 0: even 32-column chunks, 1: odd
-    const int epi_tid = threadIdx.x - 64;
-    const bool has_cols = (args.bias != nullptr) || (args.col_sub != nullptr);
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-      int m_blk, n_blk;
-      tile_coords(args, tile, m_blk, n_blk);
-      const int64_t n_base = (int64_t)n_blk * args.block_n;
-      float* sb = s_bias + acc * kMaxBlockN;
-      if (has_cols) {  // stage this tile's per-column constants once (one global round trip per tile)
-        for (int c = epi_tid; c < args.block_n; c += kEpiWarps * 32) {
-          const int64_t n = n_base + c;
-          float v = 0.f;
-          if (n < args.N) {
-            if (args.bias) v += __ldg(&args.bias[n]);
-            if (args.col_sub) v -= __ldg(&args.col_sub[n]);
-          }
-          sb[c] = v;
-        }
-      }
-      named_bar_sync_1<kEpiWarps * 32>();
-      mbar_wait(&tmem_full[acc], acc_phase);
-      tcgen05_fence_after();
-      const int64_t row = (int64_t)m_blk * kBlockM + lane_grp * 32 + lane;
-      const bool row_ok = row < args.M;
-      const uint32_t taddr0 = tmem_base + ((uint32_t)(lane_grp * 32) << 16) + (uint32_t)(acc * args.block_n);
-      for (int c = chunk_par * 32; c < args.block_n; c += 64) {
-        const int width = min(32, args.block_n - c);  // 32, or 16 for the last chunk (block_n % 16 == 0)
-        uint32_t v[32];
-        if (width == 32) {
-          tmem_ld_x32(taddr0 + (uint32_t)c, v);
-        } else {
-          uint32_t lo[16];
-          tmem_ld_x16(taddr0 + (uint32_t)c, lo);
-#pragma unroll
-          for (int j = 0; j < 16; ++j) v[j] = lo[j];
-#pragma unroll
-          for (int j = 16; j < 32; ++j) v[j] = 0u;
-        }
-        // residual for this chunk: issue the loads before waiting on TMEM
-        const int64_t n0 = n_base + c;
-        uint4 rres[4];
-        const bool full_bf16 = !args.d_is_f32 && row_ok && (n0 + width <= args.N);
-        if (args.residual && full_bf16) {
-          const uint4* r = reinterpret_cast<const uint4*>(args.residual + row * args.ld_res + n0);
-#pragma unroll
-          for (int j = 0; j < 4; ++j)
-            if (j * 8 < width) rres[j] = __ldg(r + j);
-        }
-        tmem_ld_wait();
-        // TMA-store path: the whole warp stages its 32 x 32 sub-tile (rows / columns outside D are clipped by
-        // the store), so only warp-uniform conditions may skip; the direct path skips per thread
-        const bool via_tma = args.tma_store && width == 32 && (!args.residual || n0 + 32 <= args.N);
-        if (n0 >= args.N || (via_tma ? (row - lane >= args.M) : !row_ok)) continue;
-        float f[32];
-#pragma unroll
-        for (int j = 0; j < 32; ++j) f[j] = __uint_as_float(v[j]);
-        if (args.alpha != 1.0f) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) f[j] *= args.alpha;
-        }
-        if (has_cols) {
-#pragma unroll
-          for (int j = 0; j < 32; j += 4) {
-            const float4 b4 = *reinterpret_cast<const float4*>(sb + c + j);  // smem broadcast
-            f[j] += b4.x;
-            f[j + 1] += b4.y;
-            f[j + 2] += b4.z;
-            f[j + 3] += b4.w;
-          }
-        }
-        if (args.act == 1) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) f[j] = relu6f(f[j]);
-        } else if (args.act == 2) {  // ReLU
-#pragma unroll
-          for (int j = 0; j < 32; ++j) f[j] = fmaxf(f[j], 0.f);
-        } else if (args.act == 3) {  // HardSwish: x * clamp(x / 6 + 0.5, 0, 1)
-#pragma unroll
-          for (int j = 0; j < 32; ++j) f[j] *= fminf(fmaxf(fmaf(f[j], 1.0f / 6.0f, 0.5f), 0.f), 1.f);
-        }
-        if (args.chunk_max && row_ok) {  // k-NN: the maximum of this 32-column chunk (columns >= N excluded)
-          float m = -INFINITY;
-#pragma unroll
-          for (int j = 0; j < 32; ++j)
-            if (j < width && n0 + j < args.N) m = fmaxf(m, f[j]);
-          args.chunk_max[row * args.ld_cm + (n0 >> 5)] = m;
-        }
-        if (via_tma) {
-          if (args.residual && full_bf16) {
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              const __nv_bfloat162* h2 = reinterpret_cast<const __nv_bfloat162*>(&rres[j]);
-#pragma unroll
-              for (int q = 0; q < 4; ++q) {
-                const float2 rv = __bfloat1622float2(h2[q]);
-                f[j * 8 + 2 * q] += rv.x;
-                f[j * 8 + 2 * q + 1] += rv.y;
-              }
-            }
-          }
-          // the previous store issued from this warp's staging buffer must have read it
-          if (lane == 0) tma_store_wait_read();
-          __syncwarp();
-          const uint32_t stg = smem_u32(store_stage + epi_warp * store_stage_bytes);
-          if (args.d_is_f32) {  // 128-byte rows, SWIZZLE_128B: 16-byte chunk j of row r at (j ^ (r & 7))
-            const uint32_t rowa = stg + ((uint32_t)lane << 7);
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(rowa + ((((uint32_t)j) ^ ((uint32_t)lane & 7u)) << 4)),
-                           "f"(f[4 * j]), "f"(f[4 * j + 1]), "f"(f[4 * j + 2]), "f"(f[4 * j + 3])
-                           : "memory");
-            }
-          } else {  // 64-byte rows, SWIZZLE_64B: chunk j of row r at (j ^ ((r >> 1) & 3))
-            const uint32_t rowa = stg + ((uint32_t)lane << 6);
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(
-                               rowa + ((((uint32_t)j) ^ (((uint32_t)lane >> 1) & 3u)) << 4)),
-                           "r"(pack_bf16x2(f[j * 8 + 0], f[j * 8 + 1])), "r"(pack_bf16x2(f[j * 8 + 2], f[j * 8 + 3])),
-                           "r"(pack_bf16x2(f[j * 8 + 4], f[j * 8 + 5])), "r"(pack_bf16x2(f[j * 8 + 6], f[j * 8 + 7]))
-                           : "memory");
-            }
-          }
-          fence_proxy_async();
-          __syncwarp();
-          if (lane == 0) {
-            tma_store_2d(&map_d, stg, (int)n0, (int)(row));  // row of lane 0 == first row of the sub-tile
-            tma_store_commit();
-          }
-        } else if (full_bf16) {
-          __nv_bfloat16* d = reinterpret_cast<__nv_bfloat16*>(args.D) + row * args.ldd + n0;
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            if (j * 8 < width) {
-              if (args.residual) {
-                const __nv_bfloat162* h2 = reinterpret_cast<const __nv_bfloat162*>(&rres[j]);
-#pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                  const float2 rv = __bfloat1622float2(h2[q]);
-                  f[j * 8 + 2 * q] += rv.x;
-                  f[j * 8 + 2 * q + 1] += rv.y;
-                }
-              }
-              uint4 o;
-              o.x = pack_bf16x2(f[j * 8 + 0], f[j * 8 + 1]);
-              o.y = pack_bf16x2(f[j * 8 + 2], f[j * 8 + 3]);
-              o.z = pack_bf16x2(f[j * 8 + 4], f[j * 8 + 5]);
-              o.w = pack_bf16x2(f[j * 8 + 6], f[j * 8 + 7]);
-              reinterpret_cast<uint4*>(d)[j] = o;
-            }
-          }
-        } else if (args.d_is_f32) {
-          float* d = reinterpret_cast<float*>(args.D) + row * args.ldd + n0;
-          if (n0 + width <= args.N && ((reinterpret_cast<uintptr_t>(d) & 15) == 0)) {
-#pragma unroll
-            for (int j = 0; j < 32; j += 4)
-              if (j < width) *reinterpret_cast<float4*>(d + j) = make_float4(f[j], f[j + 1], f[j + 2], f[j + 3]);
-          } else {
-            const int nvalid = (int)min((int64_t)width, args.N - n0);
-#pragma unroll
-            for (int j = 0; j < 32; ++j)
-              if (j < nvalid) d[j] = f[j];
-          }
-        } else {  // ragged bf16 tail (N not a multiple of 16): scalar, never hit by the encoder
-          __nv_bfloat16* d = reinterpret_cast<__nv_bfloat16*>(args.D) + row * args.ldd + n0;
-          const int nvalid = (int)min((int64_t)width, args.N - n0);
-#pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            if (j < nvalid) {
-              float o = f[j];
-              if (args.residual) o += __bfloat162float(args.residual[row * args.ld_res + n0 + j]);
-              d[j] = __float2bfloat16_rn(o);
-            }
-          }
-        }
-      }
-      tcgen05_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tmem_empty[acc]);
-      if (++acc == 2) {
-        acc = 0;
-        acc_phase ^= 1;
-      }
-    }
+    return;
   }
-  if (args.tma_store && warp >= 2 && lane == 0) tma_store_wait_all();  // this lane issued the warp's tile stores
-  tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tcgen05_fence_after();
-    tmem_dealloc(tmem_base, kTmemCols);
+  regs_consumer();
+  // ===================== consumers: warpgroups 1 and 2 =====================
+  const int wg = (threadIdx.x >> 7) - 1;      // 0: tile rows [0, 64), 1: [64, 128)
+  const int wt = threadIdx.x & 127;
+  const int quad = lane & 3;
+  const bool has_cols = (args.bias != nullptr) || (args.col_sub != nullptr);
+  float acc[BN / 2];
+#pragma unroll
+  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+  int stage = 0;
+  uint32_t phase = 0;
+  for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+    int m_blk, n_blk;
+    tile_coords(args, tile, m_blk, n_blk);
+    for (int kb = 0; kb < num_kb; ++kb) {
+      mbar_wait(&full_bar[stage], phase);
+      const uint32_t sa = smem_u32(smem + stage * kStageBytes) + (uint32_t)(wg * 64 * 128);
+      const uint32_t sb = smem_u32(smem + stage * kStageBytes + kATileBytes);
+      const uint64_t da = make_smem_desc(sa), db = make_smem_desc(sb);
+      const int ksteps = min(kBlockK, args.K - kb * kBlockK + 15) / 16;  // skip all-zero K tails
+      wgmma_fence();
+#pragma unroll 1
+      for (int ks = 0; ks < ksteps; ++ks)
+        Wgmma<BN>::mma(acc, da + (uint64_t)(ks * 2), db + (uint64_t)(ks * 2), (kb | ks) ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait_all();
+      reg_fence(acc);
+      mbar_arrive(&empty_bar[stage]);  // this thread's MMAs have read the stage
+      if (++stage == n_stages) {
+        stage = 0;
+        phase ^= 1;
+      }
+    }
+    // ---- epilogue straight from the accumulator registers
+    const int64_t n_base = (int64_t)n_blk * BN;
+    const int64_t row0 = (int64_t)m_blk * kBlockM + wg * 64 + (wt >> 5) * 16 + (lane >> 2);
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+      const int64_t n = n_base + 8 * j + 2 * quad;  // this thread's two columns: n, n + 1
+      float cb0 = 0.f, cb1 = 0.f;
+      if (has_cols) {
+        if (n < args.N) {
+          if (args.bias) cb0 += __ldg(&args.bias[n]);
+          if (args.col_sub) cb0 -= __ldg(&args.col_sub[n]);
+        }
+        if (n + 1 < args.N) {
+          if (args.bias) cb1 += __ldg(&args.bias[n + 1]);
+          if (args.col_sub) cb1 -= __ldg(&args.col_sub[n + 1]);
+        }
+      }
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        float& f0 = acc[4 * j + 2 * h];
+        float& f1 = acc[4 * j + 2 * h + 1];
+        if (args.alpha != 1.0f) {
+          f0 *= args.alpha;
+          f1 *= args.alpha;
+        }
+        f0 = epi_act(f0 + cb0, args.act);
+        f1 = epi_act(f1 + cb1, args.act);
+      }
+    }
+    if (args.staged) {  // bf16: fragment -> shared tile -> 16-byte row chunks
+      uint8_t* stg = d_stage + wg * 64 * stage_pitch<BN>();
+      const int r_lo = (wt >> 5) * 16 + (lane >> 2);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int64_t row = row0 + 8 * h;
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+          const int64_t n = n_base + 8 * j + 2 * quad;
+          float f0 = acc[4 * j + 2 * h], f1 = acc[4 * j + 2 * h + 1];
+          if (args.residual && row < args.M && n < args.N) {  // N % 8 == 0 here: both columns exist
+            const float2 rv = __bfloat1622float2(
+                *reinterpret_cast<const __nv_bfloat162*>(args.residual + row * args.ld_res + n));
+            f0 += rv.x;
+            f1 += rv.y;
+          }
+          *reinterpret_cast<__nv_bfloat162*>(stg + (r_lo + 8 * h) * stage_pitch<BN>() + (8 * j + 2 * quad) * 2) =
+              __floats2bfloat162_rn(f0, f1);
+        }
+      }
+      asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
+      const int64_t tile_row0 = (int64_t)m_blk * kBlockM + wg * 64;
+      for (int idx = wt; idx < 64 * (BN / 8); idx += 128) {
+        const int r = idx / (BN / 8), c8 = idx - r * (BN / 8);
+        const int64_t row = tile_row0 + r, n = n_base + 8 * c8;
+        if (row < args.M && n < args.N)
+          *reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(args.D) + row * args.ldd + n) =
+              *reinterpret_cast<const uint4*>(stg + r * stage_pitch<BN>() + c8 * 16);
+      }
+      asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");  // the tile is read before the next one is staged
+      continue;
+    }
+    if (args.chunk_max) {  // k-NN: the maximum of every 32-column chunk (columns >= N excluded); BN % 32 == 0 here
+#pragma unroll
+      for (int c = 0; c < BN / 32; ++c) {
+        float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+        for (int j = 4 * c; j < 4 * c + 4; ++j) {
+          const int64_t n = n_base + 8 * j + 2 * quad;
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            if (n < args.N) mx[h] = fmaxf(mx[h], acc[4 * j + 2 * h]);
+            if (n + 1 < args.N) mx[h] = fmaxf(mx[h], acc[4 * j + 2 * h + 1]);
+          }
+        }
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 1));
+          mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 2));
+          const int64_t row = row0 + 8 * h;
+          const int64_t n0 = n_base + 32 * c;
+          if (quad == 0 && row < args.M && n0 < args.N) args.chunk_max[row * args.ld_cm + (n0 >> 5)] = mx[h];
+        }
+      }
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int64_t row = row0 + 8 * h;
+      if (row >= args.M) continue;
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        const int64_t n = n_base + 8 * j + 2 * quad;
+        if (n >= args.N) continue;
+        const bool pair = n + 1 < args.N;
+        float f0 = acc[4 * j + 2 * h], f1 = acc[4 * j + 2 * h + 1];
+        if (args.d_is_f32) {
+          float* d = reinterpret_cast<float*>(args.D) + row * args.ldd + n;
+          if (pair && args.d_vec) {
+            *reinterpret_cast<float2*>(d) = make_float2(f0, f1);
+          } else {
+            d[0] = f0;
+            if (pair) d[1] = f1;
+          }
+        } else {
+          if (args.residual) {
+            const __nv_bfloat16* r = args.residual + row * args.ld_res + n;
+            if (pair && args.res_vec) {
+              const float2 rv = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(r));
+              f0 += rv.x;
+              f1 += rv.y;
+            } else {
+              f0 += __bfloat162float(r[0]);
+              if (pair) f1 += __bfloat162float(r[1]);
+            }
+          }
+          __nv_bfloat16* d = reinterpret_cast<__nv_bfloat16*>(args.D) + row * args.ldd + n;
+          if (pair && args.d_vec) {
+            *reinterpret_cast<__nv_bfloat162*>(d) = __floats2bfloat162_rn(f0, f1);
+          } else {
+            d[0] = __float2bfloat16_rn(f0);
+            if (pair) d[1] = __float2bfloat16_rn(f1);
+          }
+        }
+      }
+    }
   }
 }
 
@@ -400,7 +317,6 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t,
 
 static EncodeTiledFn g_encode = nullptr;
 static std::once_flag g_encode_once;
-static bool g_attr_set = false;
 static std::mutex g_attr_mu;
 
 static EncodeTiledFn get_encode() {
@@ -414,7 +330,7 @@ static EncodeTiledFn get_encode() {
   return g_encode;
 }
 
-bool available() { return ensure_init() == AM_OK && device_cc() / 10 == 10 && get_encode() != nullptr; }
+bool available() { return ensure_init() == AM_OK && device_cc() == 90 && get_encode() != nullptr; }
 
 static int make_map(CUtensorMap* map, const void* base, int64_t rows, int64_t ld_elems, int K, int box_rows) {
   const cuuint64_t dims[2] = {(cuuint64_t)K, (cuuint64_t)rows};
@@ -432,7 +348,7 @@ static int make_map(CUtensorMap* map, const void* base, int64_t rows, int64_t ld
   return AM_OK;
 }
 
-// generic bf16 tiled tensor map (rank <= 4), SWIZZLE_128B, zero OOB fill (used by fused_block.cu)
+// generic bf16 tiled tensor map (rank <= 4), SWIZZLE_128B, zero OOB fill (used by kmeans_tc.cu)
 int encode_map_bf16(void* map_out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
                     const uint32_t* box) {
   AM_CHECK(get_encode() != nullptr, "cuTensorMapEncodeTiled unavailable");
@@ -454,11 +370,30 @@ int encode_map_bf16(void* map_out, const void* base, int rank, const uint64_t* d
   return AM_OK;
 }
 
-static int pick_block_n(int64_t N) {
+// tile widths gemm_wgmma_kernel is instantiated for (the switch in gemm_bf16)
+static bool gemm_has_n(int n) {
+  return n == 16 || n == 32 || n == 48 || n == 64 || n == 80 || n == 96 || n == 112 || n == 128 || n == 160 ||
+         n == 192 || n == 224 || n == 256;
+}
+
+// the smallest instantiated tile width >= n (n <= kMaxBlockN)
+int tile_n_for(int n) {
+  for (int c = 16; c <= kMaxBlockN; c += 16)
+    if (c >= n && gemm_has_n(c)) return c;
+  return kMaxBlockN;
+}
+
+static int pick_block_n(int64_t N, bool chunk_max) {
   const int64_t n16 = (int64_t)round_up((size_t)N, 16);
-  if (n16 <= kMaxBlockN) return (int)n16;
-  const int64_t tiles = (n16 + kMaxBlockN - 1) / kMaxBlockN;
-  return (int)round_up((size_t)((n16 + tiles - 1) / tiles), 16);
+  int bn;
+  if (n16 <= kMaxBlockN) {
+    bn = (int)n16;
+  } else {
+    const int64_t tiles = (n16 + kMaxBlockN - 1) / kMaxBlockN;
+    bn = (int)round_up((size_t)((n16 + tiles - 1) / tiles), 16);
+  }
+  if (chunk_max) bn = std::min(kMaxBlockN, (int)round_up((size_t)bn, 32));  // chunk c <-> columns [32c, 32c + 32)
+  return tile_n_for(bn);
 }
 
 static KernelArgs make_args(int64_t M, int64_t N, int K, void* D, int64_t ldd, bool d_is_f32, const Epilogue& ep,
@@ -467,14 +402,14 @@ static KernelArgs make_args(int64_t M, int64_t N, int K, void* D, int64_t ldd, b
   a.M = M;
   a.N = N;
   a.K = K;
-  a.block_n = pick_block_n(N);
-  if (ep.chunk_max) a.block_n = std::min(kMaxBlockN, (int)round_up((size_t)a.block_n, 32));  // chunk c <-> columns [32c, 32c + 32)
+  a.block_n = pick_block_n(N, ep.chunk_max != nullptr);
   a.tiles_m = (int)((M + kBlockM - 1) / kBlockM);
   a.tiles_n = (int)((N + a.block_n - 1) / a.block_n);
   a.m_fastest = m_fastest ? 1 : 0;
   a.D = D;
   a.ldd = ldd;
   a.d_is_f32 = d_is_f32 ? 1 : 0;
+  a.d_vec = (ldd % 2 == 0 && (reinterpret_cast<uintptr_t>(D) & (d_is_f32 ? 7 : 3)) == 0) ? 1 : 0;
   a.alpha = ep.alpha;
   a.bias = ep.bias;
   a.col_sub = ep.col_sub;
@@ -483,7 +418,30 @@ static KernelArgs make_args(int64_t M, int64_t N, int K, void* D, int64_t ldd, b
   a.ld_cm = ep.ld_cm;
   a.residual = ep.residual;
   a.ld_res = ep.ld_res;
+  a.res_vec = (ep.ld_res % 2 == 0 && (reinterpret_cast<uintptr_t>(ep.residual) & 3) == 0) ? 1 : 0;
+  a.staged = (!d_is_f32 && !ep.chunk_max && N % 8 == 0 && ldd % 8 == 0 && (reinterpret_cast<uintptr_t>(D) & 15) == 0 &&
+              (!ep.residual || (ep.ld_res % 2 == 0 && (reinterpret_cast<uintptr_t>(ep.residual) & 3) == 0))) ? 1 : 0;
   return a;
+}
+
+template <int BN>
+static int launch_bn(const CUtensorMap& map_a, const CUtensorMap& map_b, KernelArgs& args, cudaStream_t st) {
+  static bool attr_set = false;
+  {
+    std::lock_guard<std::mutex> lk(g_attr_mu);
+    if (!attr_set) {
+      AM_CUDA(cudaFuncSetAttribute(gemm_wgmma_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemMax));
+      attr_set = true;
+    }
+  }
+  const size_t stage_bytes = (size_t)kATileBytes + (size_t)BN * kBlockK * 2;
+  const size_t tail = 1024 + 2 * kStages * sizeof(uint64_t) + (args.staged ? 2 * 64 * stage_pitch<BN>() : 0);
+  args.stages = (int)std::min<size_t>(kStages, (kSmemMax - tail) / stage_bytes);
+  const size_t smem = (size_t)args.stages * stage_bytes + tail;
+  const int tiles = args.tiles_m * args.tiles_n;
+  const int grid = std::max(1, std::min(tiles, sm_count()));
+  AM_LAUNCH(gemm_wgmma_kernel<BN>, grid, kThreads, smem, st, map_a, map_b, args);
+  return AM_OK;
 }
 
 int gemm_bf16(const __nv_bfloat16* A, int64_t M, int64_t lda, const __nv_bfloat16* B, int64_t N, int64_t ldb, int K,
@@ -493,45 +451,27 @@ int gemm_bf16(const __nv_bfloat16* A, int64_t M, int64_t lda, const __nv_bfloat1
   AM_CHECK(lda % 8 == 0 && ldb % 8 == 0, "gemm: lda/ldb must be multiples of 8 elements (TMA 16-byte pitch)");
   AM_CHECK((reinterpret_cast<uintptr_t>(A) & 15) == 0 && (reinterpret_cast<uintptr_t>(B) & 15) == 0,
            "gemm: operands must be 16-byte aligned");
-  AM_CHECK(available(), "gemm: tcgen05 path unavailable (needs sm_100 and cuTensorMapEncodeTiled)");
+  AM_CHECK(available(), "gemm: wgmma path unavailable (needs sm_90 and cuTensorMapEncodeTiled)");
   KernelArgs args = make_args(M, N, K, D, ldd, d_is_f32, ep, m_fastest);
-  CUtensorMap map_a, map_b, map_d;
+  CUtensorMap map_a, map_b;
   AM_TRY(make_map(&map_a, A, M, lda, K, kBlockM));
   AM_TRY(make_map(&map_b, B, N, ldb, K, args.block_n));
-  // D through TMA tile stores when its pitch / base allow a tensor map (16-byte multiples)
-  const size_t esz = d_is_f32 ? 4 : 2;
-  static const bool no_tma_store = std::getenv("AM_GEMM_NO_TMA_STORE") != nullptr;
-  args.tma_store = (!no_tma_store && (ldd * esz) % 16 == 0 && (reinterpret_cast<uintptr_t>(D) & 15) == 0 &&
-                    M < (int64_t)1 << 31 && N < (int64_t)1 << 31) ? 1 : 0;
-  if (args.tma_store) {
-    const cuuint64_t dims[2] = {(cuuint64_t)N, (cuuint64_t)M};
-    const cuuint64_t strides[1] = {(cuuint64_t)ldd * esz};
-    const cuuint32_t box[2] = {32, 32};
-    const cuuint32_t estr[2] = {1, 1};
-    CUresult r = get_encode()(&map_d, d_is_f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, D,
-                              dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                              d_is_f32 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
-                              CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) args.tma_store = 0;  // odd pitch etc.: the direct-store epilogue handles it
+  switch (args.block_n) {
+    case 16: return launch_bn<16>(map_a, map_b, args, st);
+    case 32: return launch_bn<32>(map_a, map_b, args, st);
+    case 48: return launch_bn<48>(map_a, map_b, args, st);
+    case 64: return launch_bn<64>(map_a, map_b, args, st);
+    case 80: return launch_bn<80>(map_a, map_b, args, st);
+    case 96: return launch_bn<96>(map_a, map_b, args, st);
+    case 112: return launch_bn<112>(map_a, map_b, args, st);
+    case 128: return launch_bn<128>(map_a, map_b, args, st);
+    case 160: return launch_bn<160>(map_a, map_b, args, st);
+    case 192: return launch_bn<192>(map_a, map_b, args, st);
+    case 224: return launch_bn<224>(map_a, map_b, args, st);
+    case 256: return launch_bn<256>(map_a, map_b, args, st);
   }
-  if (!args.tma_store) map_d = map_a;
-  const size_t stage_bytes = (size_t)kATileBytes + (size_t)args.block_n * kBlockK * 2;
-  const size_t tail = (args.tma_store ? (size_t)kEpiWarps * (d_is_f32 ? kStoreStageBytes : kStoreStageBytes / 2) : 0) +
-                      1024 + 256 + 2 * kMaxBlockN * 4;
-  constexpr size_t kSmemMax = 232448;
-  args.stages = (kStages * stage_bytes + tail <= kSmemMax) ? kStages : kStages - 1;
-  const size_t smem = (size_t)args.stages * stage_bytes + tail;
-  {
-    std::lock_guard<std::mutex> lk(g_attr_mu);
-    if (!g_attr_set) {
-      AM_CUDA(cudaFuncSetAttribute(gemm_tcgen05_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemMax));
-      g_attr_set = true;
-    }
-  }
-  const int tiles = args.tiles_m * args.tiles_n;
-  const int grid = std::max(1, std::min(tiles, sm_count()));
-  AM_LAUNCH(gemm_tcgen05_kernel, grid, kThreads, smem, st, map_a, map_b, map_d, args);
-  return AM_OK;
+  set_error("gemm: no kernel for a %d-column tile", args.block_n);
+  return AM_ERR_INVALID;
 }
 
 int gemm_bf16_simt(const __nv_bfloat16* A, int64_t M, int64_t lda, const __nv_bfloat16* B, int64_t N, int64_t ldb,

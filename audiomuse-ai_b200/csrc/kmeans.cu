@@ -1,7 +1,7 @@
-// K5: Lloyd k-means (sm_100a).  Replaces cuml.cluster.KMeans(...).fit_predict as called by
+// K5: Lloyd k-means (sm_90a).  Replaces cuml.cluster.KMeans(...).fit_predict as called by
 // tasks/clustering_gpu.py:100-123 (k-means++ init, n_init restarts, labels + cluster_centers_).
 //
-// Per Lloyd iteration, k <= 128 (kmeans_tc.cu): the assignment is a split-bf16 tcgen05 GEMM with a fused argmin
+// Per Lloyd iteration, k <= 128 (kmeans_tc.cu): the assignment is a split-bf16 wgmma GEMM with a fused argmin
 // epilogue (+ an exact fp32 recheck of near-ties), the partial sums a sort-by-label pass that reads every row
 // once -- two passes over the data per iteration, HBM-bound.  This file keeps the driver (k-means++ seeding,
 // sklearn's tolerance / empty-cluster rules, restarts) and the CUDA-core kernels that serve k > 128 and small

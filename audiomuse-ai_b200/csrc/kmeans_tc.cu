@@ -1,4 +1,4 @@
-// K5 on the tensor cores: one Lloyd E-step + M-step partial sums for k <= 128 clusters (sm_100a).
+// K5 on the tensor cores: one Lloyd E-step + M-step partial sums for k <= 128 clusters (sm_90a).
 //
 // Replaces cuml.cluster.KMeans's assignment GEMM (tasks/clustering_gpu.py:100-123; SURVEY 2.4 K5).
 //
@@ -7,15 +7,16 @@
 //   per iteration
 //     centre prep               C f32 [k, d] -> Cs bf16 [2*kp, dp] = rows [0, kp): hi, [kp, 2kp): lo;  cn[j] = ||c_j||^2
 //                               (+inf for the padded rows j >= k), cmax = max ||c_j||.
-//     assign_tc_kernel          persistent warp-specialised CTAs, a tile = 128 points:
-//                                 warp 0   TMA: per 64-wide K chunk the A_hi, A_lo [128 x 64] and B [2kp x 64] tiles
-//                                          (SWIZZLE_128B) into a 3-stage mbarrier ring;
-//                                 warp 1   one elected thread issues tcgen05.mma.kind::f16 (M128, N = kp, K16):
-//                                          D += A_hi.B_hi + A_lo.B_hi + A_hi.B_lo   -- an fp32-class dot product
-//                                          (dropped term lo.lo <= 2^-18 |x||c|), accumulators double-buffered in TMEM;
-//                                 warps 2-5 FUSED ARGMIN EPILOGUE: thread = point; tcgen05.ld 32 columns at a time,
-//                                          v_j = cn_j - 2 D_j, running best / second best; writes label and distance,
-//                                          nothing else -- the [N, k] score matrix never exists in memory.
+//     assign_tc_kernel          persistent warp-specialised CTAs of three warpgroups, a tile = 128 points:
+//                                 warpgroup 0     TMA: per 64-wide K chunk the A_hi, A_lo [128 x 64] and B [2kp x 64]
+//                                                 tiles (SWIZZLE_128B) into a 3-stage mbarrier ring;
+//                                 warpgroups 1-2  64 points each: wgmma.mma_async m64n{kp}k16 into fp32 registers,
+//                                                 D += A_hi.B_hi + A_lo.B_hi + A_hi.B_lo   -- an fp32-class dot product
+//                                                 (dropped term lo.lo <= 2^-18 |x||c|); then the FUSED ARGMIN
+//                                                 EPILOGUE from the registers: v_j = cn_j - 2 D_j, running best /
+//                                                 second best per thread, merged over the 4 threads of a row; writes
+//                                                 label and distance, nothing else -- the [N, k] score matrix never
+//                                                 exists in memory.
 //                               A point whose runner-up is within the proven error band of the best
 //                               (2^-11 ||x|| max||c||) is appended to a recheck list.
 //     recheck_kernel            exact fp32 argmin (the CUDA-core arithmetic of kmeans.cu's assign_kernel) for the
@@ -29,8 +30,8 @@
 // HBM traffic per iteration: Xs once (assign) + X once (accumulate) = 2 * N * d * 4 bytes.
 #include "kmeans_tc.cuh"
 
-#include "gemm_tcgen05.cuh"
-#include "ptx_sm100.cuh"
+#include "gemm_wgmma.cuh"
+#include "ptx_sm90.cuh"
 
 #include <algorithm>
 #include <cmath>
@@ -42,7 +43,8 @@ using namespace ptx;
 
 constexpr int kTileM = 128;
 constexpr int kChunkK = 64;
-constexpr int kThreads = 64 + 4 * 32;  // TMA warp, MMA warp, 4 epilogue warps
+constexpr int kThreads = 384;         // producer warpgroup (one TMA lane) + two consumer warpgroups
+constexpr int kConsumerThreads = 256;
 constexpr int kATile = kTileM * kChunkK * 2;  // 16 KiB
 constexpr int kSlabMax = 4096;                // most points one accumulate CTA sorts at a time
 
@@ -106,46 +108,49 @@ struct AssignArgs {
   float band_scale;       // 2^-11
 };
 
+constexpr int kStages = 3;
+
+// (best, index, runner-up) of two disjoint candidate sets; equal scores keep the lower centre index
+__device__ __forceinline__ void merge_best(float& best, int& best_j, float& second, float b2, int j2, float s2) {
+  if (b2 < best || (b2 == best && j2 < best_j)) {
+    second = fminf(s2, best);
+    best = b2;
+    best_j = j2;
+  } else {
+    second = fminf(second, b2);
+  }
+}
+
+template <int KP>
 __global__ void __launch_bounds__(kThreads, 1)
 assign_tc_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_c, const AssignArgs args) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  constexpr int kStages = 3;
-  const int b_bytes = 2 * args.kp * kChunkK * 2;  // hi rows then lo rows
-  const int stage_bytes = 2 * kATile + b_bytes;
+  constexpr int b_bytes = 2 * KP * kChunkK * 2;  // hi rows then lo rows
+  constexpr int stage_bytes = 2 * kATile + b_bytes;
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kStages * stage_bytes);
   uint64_t* empty_bar = full_bar + kStages;
-  uint64_t* tmem_full = empty_bar + kStages;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_empty + 2);
-  float* s_cn = reinterpret_cast<float*>(tmem_ptr + 4);  // [kp]
+  float* s_cn = reinterpret_cast<float*>(empty_bar + kStages);  // [KP]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int num_kb = args.dp / kChunkK;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     prefetch_tensormap(&map_x);
     prefetch_tensormap(&map_c);
     for (int i = 0; i < kStages; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full[i], 1);
-      mbar_init(&tmem_empty[i], 4);
+      mbar_init(&empty_bar[i], kConsumerThreads);
     }
     fence_barrier_init();
     fence_proxy_async();
   }
-  if (warp == 1) tmem_alloc(tmem_ptr, 256);
-  for (int i = threadIdx.x; i < args.kp; i += kThreads) s_cn[i] = args.cn[i];
-  tcgen05_fence_before();
+  for (int i = threadIdx.x; i < KP; i += kThreads) s_cn[i] = args.cn[i];
   __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
 
-  if (warp == 0) {
-    if (elect_one_sync()) {
+  if (warp < 4) {
+    regs_producer();
+    if (warp == 0 && elect_one_sync()) {
       int stage = 0;
       uint32_t phase = 0;
       for (int tile = blockIdx.x; tile < args.tiles; tile += gridDim.x) {
@@ -163,91 +168,74 @@ assign_tc_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constan
         }
       }
     }
-  } else if (warp == 1) {
-    if (elect_one_sync()) {
-      const uint32_t idesc = make_idesc(kTileM, args.kp);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int tile = blockIdx.x; tile < args.tiles; tile += gridDim.x) {
-        mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-        tcgen05_fence_after();
-        const uint32_t tmem_d = tmem_base + (uint32_t)(acc * 128);
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tcgen05_fence_after();
-          const uint32_t sa = smem_u32(smem + stage * stage_bytes);
-          const uint64_t d_ahi = make_smem_desc(sa), d_alo = make_smem_desc(sa + kATile);
-          const uint64_t d_bhi = make_smem_desc(sa + 2 * kATile);
-          const uint64_t d_blo = make_smem_desc(sa + 2 * kATile + (uint32_t)args.kp * 128u);
+    return;
+  }
+  regs_consumer();
+  // ===================== consumers: warpgroup g owns tile rows [64 g, 64 g + 64) =====================
+  const int wg = (threadIdx.x >> 7) - 1;
+  const int quad = lane & 3;
+  const float cmax = sqrtf(__int_as_float(*args.cmax2_bits));
+  float acc[KP / 2];
 #pragma unroll
-          for (int ks = 0; ks < kChunkK / 16; ++ks) {
-            const uint64_t o = (uint64_t)(ks * 2);  // 16 bf16 = 32 bytes along K inside the swizzle atom
-            umma_f16(tmem_d, d_ahi + o, d_bhi + o, idesc, (kb | ks) ? 1u : 0u);
-            umma_f16(tmem_d, d_alo + o, d_bhi + o, idesc, 1u);
-            umma_f16(tmem_d, d_ahi + o, d_blo + o, idesc, 1u);
-          }
-          umma_commit(&empty_bar[stage]);
-          if (++stage == kStages) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-        umma_commit(&tmem_full[acc]);
-        if (++acc == 2) {
-          acc = 0;
-          acc_phase ^= 1;
-        }
+  for (int i = 0; i < KP / 2; ++i) acc[i] = 0.f;
+  int stage = 0;
+  uint32_t phase = 0;
+  for (int tile = blockIdx.x; tile < args.tiles; tile += gridDim.x) {
+    for (int kb = 0; kb < num_kb; ++kb) {
+      mbar_wait(&full_bar[stage], phase);
+      const uint32_t sa = smem_u32(smem + stage * stage_bytes);
+      const uint32_t rows = (uint32_t)(wg * 64 * 128);
+      const uint64_t d_ahi = make_smem_desc(sa + rows), d_alo = make_smem_desc(sa + kATile + rows);
+      const uint64_t d_bhi = make_smem_desc(sa + 2 * kATile);
+      const uint64_t d_blo = make_smem_desc(sa + 2 * kATile + (uint32_t)KP * 128u);
+      wgmma_fence();
+#pragma unroll
+      for (int ks = 0; ks < kChunkK / 16; ++ks) {
+        const uint64_t o = (uint64_t)(ks * 2);  // 16 bf16 = 32 bytes along K inside the swizzle atom
+        Wgmma<KP>::mma(acc, d_ahi + o, d_bhi + o, (kb | ks) ? 1u : 0u);
+        Wgmma<KP>::mma(acc, d_alo + o, d_bhi + o, 1u);
+        Wgmma<KP>::mma(acc, d_ahi + o, d_blo + o, 1u);
+      }
+      wgmma_commit();
+      wgmma_wait_all();
+      reg_fence(acc);
+      mbar_arrive(&empty_bar[stage]);
+      if (++stage == kStages) {
+        stage = 0;
+        phase ^= 1;
       }
     }
-  } else {
-    // ===================== fused argmin epilogue: thread = point =====================
-    const int lane_grp = warp & 3;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    const float cmax = sqrtf(__int_as_float(*args.cmax2_bits));
-    for (int tile = blockIdx.x; tile < args.tiles; tile += gridDim.x) {
-      const int64_t row = (int64_t)tile * kTileM + lane_grp * 32 + lane;
-      const bool row_ok = row < args.N;
-      const float xn = row_ok ? __ldg(&args.xn[row]) : 0.f;
-      mbar_wait(&tmem_full[acc], acc_phase);
-      tcgen05_fence_after();
-      const uint32_t taddr0 = tmem_base + ((uint32_t)(lane_grp * 32) << 16) + (uint32_t)(acc * 128);
+    // ===================== fused argmin epilogue: a quad of threads = two points =====================
+    const int64_t row0 = (int64_t)tile * kTileM + wg * 64 + ((threadIdx.x & 127) >> 5) * 16 + (lane >> 2);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int64_t row = row0 + 8 * h;
       float best = INFINITY, second = INFINITY;
-      int best_j = 0;
-      for (int c = 0; c < args.kp; c += 32) {
-        uint32_t v[32];
-        if (args.kp - c >= 32) {
-          tmem_ld_x32(taddr0 + (uint32_t)c, v);
-        } else {
-          uint32_t lo[16];
-          tmem_ld_x16(taddr0 + (uint32_t)c, lo);
+      int best_j = 0;  // a label in range even for a row whose scores are all NaN / +inf
 #pragma unroll
-          for (int j = 0; j < 16; ++j) v[j] = lo[j];
+      for (int j = 0; j < KP / 8; ++j) {  // this thread's columns in increasing order
 #pragma unroll
-          for (int j = 16; j < 32; ++j) v[j] = 0u;
-        }
-        tmem_ld_wait();
-#pragma unroll
-        for (int j = 0; j < 32; ++j) {
-          if (c + j < args.kp) {
-            const float s = fmaf(-2.0f, __uint_as_float(v[j]), s_cn[c + j]);  // +inf for padded centres
-            if (s < best) {
-              second = best;
-              best = s;
-              best_j = c + j;
-            } else if (s < second) {
-              second = s;
-            }
+        for (int e = 0; e < 2; ++e) {
+          const int c = 8 * j + 2 * quad + e;
+          const float s = fmaf(-2.0f, acc[4 * j + 2 * h + e], s_cn[c]);  // +inf for padded centres
+          if (s < best) {
+            second = best;
+            best = s;
+            best_j = c;
+          } else if (s < second) {
+            second = s;
           }
         }
       }
-      // release the accumulator before the global writes
-      tcgen05_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tmem_empty[acc]);
-      if (row_ok) {
+#pragma unroll
+      for (int o = 1; o <= 2; o <<= 1) {
+        const float b2 = __shfl_xor_sync(0xffffffffu, best, o);
+        const int j2 = __shfl_xor_sync(0xffffffffu, best_j, o);
+        const float s2 = __shfl_xor_sync(0xffffffffu, second, o);
+        merge_best(best, best_j, second, b2, j2, s2);
+      }
+      if (quad == 0 && row < args.N) {
+        const float xn = __ldg(&args.xn[row]);
         args.labels[row] = best_j;
         if (args.dist) args.dist[row] = fmaxf(best + xn, 0.f);
         // |v~ - v| <= 2^-13 ||x|| max||c|| per centre (split-bf16 residuals + fp32 accumulation over dp terms);
@@ -258,17 +246,7 @@ assign_tc_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constan
           args.recheck[slot] = (int32_t)row;
         }
       }
-      if (++acc == 2) {
-        acc = 0;
-        acc_phase ^= 1;
-      }
     }
-  }
-  tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tcgen05_fence_after();
-    tmem_dealloc(tmem_base, 256);
   }
 }
 
@@ -514,6 +492,20 @@ int Plan::launch_accumulate(float* sums, float* counts, double* inertia_dev, con
   return AM_OK;
 }
 
+template <int KP>
+static int launch_assign(const Plan& p, const AssignArgs& a, cudaStream_t st) {
+  const size_t smem = 1024 + kStages * (size_t)(2 * kATile + 2 * KP * kChunkK * 2) + 2 * kStages * 8 + (size_t)KP * 4;
+  static bool attr_set = false;
+  if (!attr_set) {
+    AM_CUDA(cudaFuncSetAttribute(assign_tc_kernel<KP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    attr_set = true;
+  }
+  const int grid = std::min(a.tiles, sm_count());
+  AM_LAUNCH(assign_tc_kernel<KP>, grid, kThreads, smem, st, *reinterpret_cast<const CUtensorMap*>(p.map_x),
+            *reinterpret_cast<const CUtensorMap*>(p.map_c), a);
+  return AM_OK;
+}
+
 int Plan::step(const float* C_dev, int32_t* labels, float* sums, float* counts, double* inertia_dev, float* dist,
                cudaStream_t st) {
   AM_CUDA(cudaMemsetAsync(scal.p, 0, 2 * sizeof(int), st));
@@ -532,15 +524,19 @@ int Plan::step(const float* C_dev, int32_t* labels, float* sums, float* counts, 
   a.n_recheck = scal.p + 1;
   a.recheck = recheck.p;
   a.band_scale = 1.0f / 2048.0f;
-  const size_t smem = 1024 + 3 * (size_t)(2 * kATile + 2 * kp * kChunkK * 2) + 256 + (size_t)kp * 4;
-  static size_t attr = 0;
-  if (smem > attr) {
-    AM_CUDA(cudaFuncSetAttribute(assign_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr = smem;
+  switch (kp) {
+    case 16: AM_TRY(launch_assign<16>(*this, a, st)); break;
+    case 32: AM_TRY(launch_assign<32>(*this, a, st)); break;
+    case 48: AM_TRY(launch_assign<48>(*this, a, st)); break;
+    case 64: AM_TRY(launch_assign<64>(*this, a, st)); break;
+    case 80: AM_TRY(launch_assign<80>(*this, a, st)); break;
+    case 96: AM_TRY(launch_assign<96>(*this, a, st)); break;
+    case 112: AM_TRY(launch_assign<112>(*this, a, st)); break;
+    case 128: AM_TRY(launch_assign<128>(*this, a, st)); break;
+    default:
+      set_error("kmeans: no assignment kernel for %d centres", kp);
+      return AM_ERR_INVALID;
   }
-  const int grid = std::min(a.tiles, sm_count());
-  AM_LAUNCH(assign_tc_kernel, grid, kThreads, smem, st, *reinterpret_cast<const CUtensorMap*>(map_x),
-            *reinterpret_cast<const CUtensorMap*>(map_c), a);
   AM_LAUNCH(recheck_kernel, sm_count() * 8, 256, 0, st, X, d, C_dev, cn.p, k, scal.p + 1, recheck.p, labels, dist);
   if (sums) {
     AM_CUDA(cudaMemsetAsync(sums, 0, (size_t)k * d * 4, st));

@@ -6,7 +6,7 @@
 namespace am {
 namespace kmtc {
 
-// true when the tcgen05 path can serve this problem (k <= 128; sm_100; AM_KMEANS_SIMT unset)
+// true when the wgmma path can serve this problem (k <= 128; sm_90; AM_KMEANS_SIMT unset)
 bool usable(int64_t N, int d, int k);
 
 struct Plan {

@@ -1,10 +1,10 @@
-// K4: exact brute-force k-NN index (sm_100a).  Replaces the voyager.Index object
+// K4: exact brute-force k-NN index (sm_90a).  Replaces the voyager.Index object
 // (tasks/voyager_manager.py:183,1397,1447,1580,1681; tasks/clap_text_search.py:173,263,493).
 //
 // Exactness by construction ("filter with a proven bound, then re-rank in float64"):
 //   1. approximate scores s~[q, j] for every stored row, with |s~ - s| <= eps
 //      (fp32 SIMT pass: eps from the fp32 dot-product error bound;
-//       bf16 tensor-core pass (gemm_tcgen05.cuh): eps from the bf16 rounding residual norms);
+//       bf16 tensor-core pass (gemm_wgmma.cuh): eps from the bf16 rounding residual norms);
 //   2. per query: T = k-th largest s~ (radix select).  Every exact top-k row satisfies
 //      s~ >= T - 2*eps, so {j : s~_j >= T - 2 eps} is a superset of the answer;
 //   3. the superset (k + a handful) is re-scored with float64 accumulation from the stored
@@ -18,7 +18,7 @@
 #include <cmath>
 #include <mutex>
 
-#include "gemm_tcgen05.cuh"
+#include "gemm_wgmma.cuh"
 
 namespace am {
 
@@ -1193,7 +1193,7 @@ static int knn_query_impl(const am_index* idx, const float* Q_dev, int nq, int k
         }
 #undef AM_SMALL_LAUNCH
       } else if (fused) {
-        // S[q, j] = Qb[q,:] . Xb[j,:] (bf16 x bf16 -> fp32 in TMEM, euclidean fix-up in the epilogue) + per-32 maxima
+        // S[q, j] = Qb[q,:] . Xb[j,:] (bf16 x bf16 -> fp32 in registers, euclidean fix-up in the epilogue) + per-32 maxima
         p.CM = CM.p;
         p.ldCM = ldCM;
         p.n_chunks = n_chunks;

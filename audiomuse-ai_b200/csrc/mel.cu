@@ -1,4 +1,4 @@
-// K1: fused  frame -> Hann window -> rFFT-2048 -> |.|^2 -> sparse mel -> 10*log10  (sm_100a)
+// K1: fused  frame -> Hann window -> rFFT-2048 -> |.|^2 -> sparse mel -> 10*log10  (sm_90a)
 //
 // Replaces librosa.feature.melspectrogram + power_to_db as called from
 // tasks/clap_analyzer.py:438-454.  One HBM pass: PCM in (int16 or f32), log-mel out.

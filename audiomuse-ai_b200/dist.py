@@ -1,4 +1,4 @@
-"""One process per GPU over torch.distributed (NCCL on the B200 box, gloo in CPU tests).
+"""One process per GPU over torch.distributed (NCCL on GPU machines, gloo in CPU tests).
 
 SURVEY 8(e): tracks are independent, so analysis shards a contiguous block of the sorted track
 list per rank with NO data-path collective; afterwards ONE all-gather of the f32[N/W, 512]

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py -- tracks/sec analysed (10 s @ 48 kHz) + k-NN queries/sec over 100 k embeddings.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 One "step" = one pass of the analysis hot path (PCM16 windows -> log-mel -> student CLAP encoder ->
@@ -13,12 +13,14 @@ Reported (ONE JSON line on rank 0):
   e2e       the same metric through the public host API: pinned host PCM16 -> H2D -> kernels -> D2H embeddings,
             all inside the timed region.  value = B200Session.embed_tracks_stream (bulk analysis: two batches in
             flight), sync_call_value = one blocking B200Session.embed_tracks call per step
-  roofline  dominant kernel (the tcgen05 pointwise-conv GEMM), tensor bound, from per-launch CUDA
+  roofline  dominant kernel (the wgmma pointwise-conv GEMM), tensor bound, from per-launch CUDA
             events recorded by the library inside the timed region; roofline_mel = the fused mel kernel
   knn       k-NN queries/s over 100 000 x 512 (BASELINE.json configs[2]) at batch 4096 / 256 / 1
   cpu_baseline   the oracle (CPU restatement of librosa + onnxruntime, reference libs are not
             installable) timed on this box's host cores on a bounded sample
 `--impl reference` times that CPU restatement as the arm itself (rank 0 only).
+`--dump-outputs DIR` writes what the last timed step computed (the per-track embeddings, float32) as DIR/<name>.npy;
+inputs are seeded, so two builds run with the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -45,27 +47,14 @@ WEIGHT_SEED = 0
 
 
 def _peaks():
-    try:
-        with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
-            p = json.load(f)
-        return {"hbm_gbs": float(p["hbm_gbs"]), "bf16_tflops": float(p["bf16_tflops"]),
-                "bf16_tflops_sustained": float(p.get("bf16_tflops_sustained", p["bf16_tflops"])),
-                "source": "MEASURED_PEAKS.json"}
-    except Exception:
-        return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "source": "fallback"}
-
-
-def _traffic(name):
-    """DRAM bytes per launch from the committed ncu --set full capture (profiles/*.json), or None."""
-    try:
-        with open(os.path.join(ROOT, "profiles", "roofline_traffic.json")) as f:
-            return json.load(f).get(name)
-    except Exception:
-        return None
+    """H100 SXM data-sheet peaks (a card allowed 700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense bf16.  Reference points
+    for the roofline fractions, not rates this code has reached; a power-limited card clocks lower."""
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0,
+            "source": "H100 SXM data sheet (700 W)"}
 
 
 class ClockSampler:
-    """SM clock / throttle reasons sampled DURING the timed region (B200_PROFILING.md).  NVML is queried in-process
+    """SM clock / throttle reasons sampled DURING the timed region.  NVML is queried in-process
     (nvidia_ml_py): spawning `nvidia-smi` every 100 ms re-initialises the driver interface for every GPU of the box and
     was seen to stall kernel launches by ~10-20 ms per call (a 12 ms step measured as 13.8 ms); nvidia-smi remains the
     fallback when the module is missing."""
@@ -354,14 +343,13 @@ def run_scale_sections(args, sess, plan, pcm_dev, offs_dev, dev, rank, world, ba
 def run_b200(args):
     import torch
 
-    import __graft_entry__ as ge
     from audiomuse_ai_b200 import _lib, clap_analyzer as ca, corpus, dist as amdist, voyager_compat as vc, weights
 
     rank, local_rank, world = amdist.init_process_group()
     if not torch.cuda.is_available():
         raise SystemExit("bench.py: no CUDA device; this framework has no CPU path (use --impl reference)")
     if not os.path.exists(_lib.LIB_PATH):
-        ge.build()
+        raise SystemExit(f"bench.py: {_lib.LIB_PATH} is missing; run build() (python __graft_entry__.py) first")
     dev = torch.device("cuda", local_rank)
     torch.cuda.set_device(dev)
     numa_node = amdist.bind_to_gpu_numa_node(local_rank) if world > 1 else None   # before the pinned buffers exist
@@ -396,7 +384,7 @@ def run_b200(args):
         step_device()
     barrier()
 
-    # ---- timed region: K steps, device-resident inputs (246 MB of PCM16 per step > 126 MB L2)
+    # ---- timed region: K steps, device-resident inputs (246 MB of PCM16 per step > 50 MB L2)
     sampler = ClockSampler(local_rank) if rank == 0 else None
     if sampler:
         sampler.start()
@@ -417,6 +405,10 @@ def run_b200(args):
     clocks = sampler.stop() if sampler else None
     ms = amdist.max_over_ranks(ms, dev)
     value = world * n_tracks * args.steps / (ms / 1000.0)
+    if args.dump_outputs and rank == 0:  # the last timed step's result, as the caller of step_device receives it
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        emb = (gathered if world > 1 else out_dev).cpu().numpy().astype(np.float32)
+        np.save(os.path.join(args.dump_outputs, "embeddings.npy"), emb)
 
     # ---- end to end through the host API (pinned host PCM -> H2D -> kernels -> D2H)
     pcm_np, offs_np = pcm_host.numpy(), offs_host.numpy()
@@ -453,48 +445,34 @@ def run_b200(args):
     if rank != 0:
         return
     # ---- rooflines from the per-launch events recorded inside the timed region
-    gemm_fl, fused_fl, fused_by = sess.flops_split(T_FRAMES)
+    gemm_fl, _, _ = sess.flops_split(T_FRAMES)
     def kernel_rec(substr):
         ms = sum(v["ms"] for k, v in prof.items() if substr in k)
         cnt = sum(v["count"] for k, v in prof.items() if substr in k)
         return {"ms": ms, "count": cnt}
 
-    gemm = kernel_rec("gemm_tcgen05_kernel")
-    # the inverted-residual blocks that run fused: channel-per-lane kernel (blocks with an expansion conv) and the
-    # pixel-per-lane kernel (block 0, no expansion); flops_split() counts both as "fused"
-    fusedk = kernel_rec("fused_block")
-    fused_parts = {k.split("(")[0].split("::")[-1].split("<")[0]: round(v["ms"] / max(args.steps, 1), 4)
-                   for k, v in prof.items() if "fused_block" in k}
+    gemm = kernel_rec("gemm_wgmma_kernel")
     peak_tf = peaks["bf16_tflops_sustained"]
 
     def tensor_roofline(name, rec, flops_per_window, note):
         tf = flops_per_window * n_tracks * args.steps / (rec["ms"] / 1000.0) / 1e12 if rec["ms"] > 0 else 0.0
         return {"kernel": f"{name} ({note})", "bound": "tensor", "achieved": tf, "peak": peak_tf,
-                "unit": "TFLOP/s", "frac": tf / peak_tf, "traffic": _traffic(name), "launches": rec["count"],
+                "unit": "TFLOP/s", "frac": tf / peak_tf, "launches": rec["count"],
                 "share_of_step": rec["ms"] / (ms if ms > 0 else 1.0), "flops_per_window": flops_per_window,
-                "peak_source": peaks["source"] + " bf16_tflops_sustained (kernel timed inside a long step)"}
+                "peak_source": peaks["source"]}
 
-    r_gemm = tensor_roofline("gemm_tcgen05_kernel", gemm, gemm_fl, "unfused pointwise convs, bf16 -> fp32 TMEM")
-    r_fused = tensor_roofline("fused_block_t_kernel + fused_block_kernel", fusedk, fused_fl,
-                              "expand + depthwise + project per block, tcgen05 + CUDA cores")
-    r_fused["ms_per_step_by_kernel"] = fused_parts
-    if fusedk["ms"] > 0:  # the same kernel against the HBM roofline (block input + output only)
-        gbs = fused_by * n_tracks * args.steps / (fusedk["ms"] / 1000.0) / 1e9
-        r_fused["hbm_view"] = {"achieved": gbs, "peak": peaks["hbm_gbs"], "unit": "GB/s", "frac": gbs / peaks["hbm_gbs"],
-                               "algorithmic_bytes_per_window": fused_by}
-    roofline = r_fused if fusedk["ms"] >= gemm["ms"] else r_gemm
-    roofline_other = r_gemm if roofline is r_fused else r_fused
+    roofline = tensor_roofline("gemm_wgmma_kernel", gemm, gemm_fl, "pointwise convs, bf16 -> fp32 registers")
     mel = kernel_rec("mel_kernel")
     mel_bytes = (N_SAMPLES * 2 + 128 * T_FRAMES * 4) * n_tracks * args.steps
     mel_gbs = mel_bytes / (mel["ms"] / 1000.0) / 1e9 if mel["ms"] > 0 else 0.0
     roofline_mel = {"kernel": "mel_kernel<int16>", "bound": "hbm", "achieved": mel_gbs, "peak": peaks["hbm_gbs"],
-                    "unit": "GB/s", "frac": mel_gbs / peaks["hbm_gbs"], "traffic": _traffic("mel_kernel"),
+                    "unit": "GB/s", "frac": mel_gbs / peaks["hbm_gbs"],
                     "launches": mel["count"], "share_of_step": mel["ms"] / (ms if ms > 0 else 1.0),
                     "algorithmic_bytes_per_window": N_SAMPLES * 2 + 128 * T_FRAMES * 4}
     # the same kernel against the fp32 FMA peak: 1001 frames x (5 N log2 N / 2 real-FFT flops + power + sparse mel + log),
-    # SURVEY 8(d); peak = SMs x 128 FMA lanes x 2 flop x max SM clock (nominal: no measured fp32 figure in MEASURED_PEAKS.json)
+    # SURVEY 8(d); peak = SMs x 128 FMA lanes x 2 flop x max SM clock (nominal)
     mel_flops = T_FRAMES * (56320 + 3 * 1025 + 2 * 1176 + 128)
-    sm_mhz = (clocks or {}).get("sm_max_mhz") or 1965.0
+    sm_mhz = (clocks or {}).get("sm_max_mhz") or 1980.0
     fp32_peak = torch.cuda.get_device_properties(dev).multi_processor_count * 128 * 2 * sm_mhz * 1e6 / 1e12
     mel_tf = mel_flops * n_tracks * args.steps / (mel["ms"] / 1000.0) / 1e12 if mel["ms"] > 0 else 0.0
     roofline_mel["compute_view"] = {"achieved": mel_tf, "peak": fp32_peak, "unit": "TFLOP/s (fp32)", "frac": mel_tf / fp32_peak,
@@ -539,7 +517,7 @@ def run_b200(args):
         s1_ms = sum(v for k, v in k1.items() if "score" in k)
         if g_ms > 0:
             tf = 2.0 * 4096 * 100_000 * 512 / (g_ms * 1e-3) / 1e12
-            knn["roofline_batch4096"] = {"kernel": "gemm_tcgen05_kernel (bf16 scores + per-32 maxima)", "bound": "tensor",
+            knn["roofline_batch4096"] = {"kernel": "gemm_wgmma_kernel (bf16 scores + per-32 maxima)", "bound": "tensor",
                                           "achieved": tf, "peak": peaks["bf16_tflops_sustained"], "unit": "TFLOP/s",
                                           "frac": tf / peaks["bf16_tflops_sustained"],
                                           "selection_ms": sum(v for k, v in k4.items() if "select" in k),
@@ -568,13 +546,13 @@ def run_b200(args):
         "config": {"workload": f"configs[1]: batch={n_tracks} synthetic 10s@48kHz tracks per GPU -> mel + CLAP embed",
                    "tracks_per_gpu": n_tracks, "numa_node_of_rank0": numa_node, "window_samples": N_SAMPLES, "encoder": "PhiNet student "
                    "alpha=3.0 beta=0.75 t0=6 N=8 (8.3 M params, random init seed 0)",
-                   "l2": "inputs larger than L2 (245.8 MB PCM16 per step vs 126 MB)",
+                   "l2": "inputs larger than L2 (245.8 MB PCM16 per step vs 50 MB)",
                    "parallelism": f"dp{world} (tracks sharded, one all-gather of embeddings per step)"},
         "e2e": {"value": e2e_value, "unit": UNIT, "api": "B200Session.embed_tracks_stream (pipelined, 2 batches in flight)",
                 "sync_call_value": e2e_sync, "h2d_bytes_per_step": int(pcm_np.nbytes + offs_np.nbytes),
                 "d2h_bytes_per_step": int(n_tracks * sess.embedding_dim * 4)},
         "gpu_launches": int(launches),
-        "roofline": roofline, "roofline_2nd": roofline_other, "roofline_mel": roofline_mel,
+        "roofline": roofline, "roofline_mel": roofline_mel,
         "kernel_ms_per_step": kernel_ms,
         "knn": knn, "clocks": clocks, "cpu_baseline": cpu,
     }
@@ -597,8 +575,12 @@ def main():
     ap.add_argument("--library-tracks", type=int, default=100_000, help="fixed library size of the strong-scaling section")
     ap.add_argument("--kmeans-rows", type=int, default=1_000_000)
     ap.add_argument("--profile-mode", action="store_true",
-                    help="for runs under ncu: honour --warmup < 3; the printed numbers are NOT bench values")
+                    help="for profiling runs: honour --warmup < 3; the printed numbers are NOT bench values")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's embeddings (float32) to DIR/embeddings.npy")
     args = ap.parse_args()
+    if args.dump_outputs and args.impl == "reference":
+        ap.error("--dump-outputs writes the GPU path's embeddings; the reference arm computes none to dump")
     if args.impl == "reference":
         run_reference(args)
     else:

@@ -1,5 +1,5 @@
 /*
- * audiomuse_b200.h -- C ABI of libaudiomuse_b200.so (sm_100a).
+ * audiomuse_b200.h -- C ABI of libaudiomuse_b200.so (sm_90a).
  *
  * The reference (NeptuneHub/AudioMuse-AI) has no FFI of its own: the hot path is Python
  * calling third-party wheels (librosa, onnxruntime, voyager, cuML).  Each entry point below
@@ -38,7 +38,7 @@ typedef enum am_status {
   AM_ERR_INVALID = -1,     /* bad argument / unsupported configuration */
   AM_ERR_CUDA = -2,        /* CUDA runtime error (message has the cudaError string) */
   AM_ERR_OOM = -3,         /* allocation failed: message contains "out of memory" */
-  AM_ERR_NO_DEVICE = -4,   /* no sm_100 device visible */
+  AM_ERR_NO_DEVICE = -4,   /* no sm_90 device visible */
   AM_ERR_IO = -5,          /* weight file unreadable / malformed */
   AM_ERR_RECALL = -6       /* fewer than k neighbours exist (voyager.RecallError) */
 } am_status;
@@ -165,8 +165,8 @@ AM_API int am_clap_n_mels(const am_model* m);
 /* 2 * multiply-accumulates of one segment of T frames (for tensor-roofline accounting) */
 AM_API double am_clap_flops_per_segment(const am_model* m, int T);
 
-/* flops of one window executed by the standalone GEMM kernel vs inside the fused block kernel, and the
- * algorithmic HBM bytes (block input + output) of the fused blocks */
+/* flops of one window executed by the GEMM kernel; the fused-block share (flops, and the algorithmic HBM
+ * bytes of fused blocks) is 0 on sm_90, where every block runs layer by layer */
 AM_API int am_clap_flops_split(const am_model* m, int T, double* gemm_flops, double* fused_flops,
                                double* fused_bytes);
 

@@ -11,27 +11,11 @@
 extern "C" {
 #endif
 
-/* debug: tcgen05 GEMM vs a CUDA-core reference on seeded operands (tests/test_gpu_gemm.py) */
+/* debug: wgmma GEMM vs a CUDA-core reference on seeded operands (tests/test_gpu_gemm.py) */
 AM_API int am_selftest_gemm(int M, int N, int K, int flags, double* max_abs_diff);
-/* debug: device time (CUDA events, mean of `iters` launches after one warm-up) of the tcgen05 GEMM
+/* debug: device time (CUDA events, mean of `iters` launches after one warm-up) of the wgmma GEMM
  * on seeded bf16 operands, bf16 output, no epilogue terms: the tensor-pipe ceiling of this kernel */
 AM_API int am_bench_gemm(int M, int N, int K, int iters, double* ms_per_launch);
-/* debug: cycles per tcgen05.mma (M128 x N x K16, SWIZZLE_128B smem operands) on every SM: issue-side
- * and issue-to-commit, cycling over d_tiles accumulators; traffic 0 = idle CTA, 1 = 16 warps of LDS.128,
- * 2 = LDS.128 + STS.128 beside it */
-AM_API int am_probe_mma(int N, int iters, int d_tiles, int traffic, double* issue_cycles, double* total_cycles);
-/* debug: TMEM read bandwidth per SM (bytes / cycle) with `warps` warps issuing tcgen05.ld.32x32b.x{cols},
- * `depth` loads in flight per wait; n_mma > 0 adds a 17th warp streaming that many M128 x N64 MMAs beside
- * the loads (warps must be 16) and reports their cost */
-AM_API int am_probe_tmem_ld(int warps, int cols, int depth, int iters, int n_mma, double* bytes_per_cycle,
-                            double* cycles_per_mma);
-
-/* debug: one M128 x N x K tcgen05.mma chain with an MN-major SWIZZLE_128B A operand (fp16 [m_rows x K] row-major
- * in, laid out by threads with M-atom stride lbo_bytes and K-group stride sbo_bytes; swap exchanges the two
- * descriptor fields) and a K-major B (fp16 [N x K]); d_out f32 [128 x N] */
-AM_API int am_probe_mn_major(const uint16_t* a_f16, const uint16_t* b_f16, int N, int K, int lbo_bytes, int sbo_bytes,
-                             int m_rows, int swap, float* d_out);
-
 /* debug: issue rate of one fp16x2 / pack / permute instruction kind (op 0 HFMA2, 1 HFMA2 immediate, 2 HFMA2.SAT,
  * 3 HMNMX2 pair, 4 PRMT, 5 F2FP pack + add, 6 HFMA2 + PRMT) with `warps` warps per SM: cycles per warp-instruction
  * per SM sub-partition */

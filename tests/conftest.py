@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
     # the in-tree library is a build artefact (git-ignored): build it when a fresh checkout has none.  A failing
     # build is reported as such -- there is no fallback for the tests to hide behind.
     lib = os.path.join(ROOT, "audiomuse-ai_b200", "libaudiomuse_b200.so")

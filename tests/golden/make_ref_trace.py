@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""Golden "call traces" of the reference's own query functions, for the GPU box (which has no /root/reference).
+"""Golden "call traces" of the reference's own query functions, so that the GPU tests need no reference checkout.
 
-    python tests/golden/make_ref_trace.py          # needs /root/reference; writes tests/golden/ref_trace.npz
+    AUDIOMUSE_REFERENCE=<checkout of AudioMuse-AI> python tests/golden/make_ref_trace.py   # writes tests/golden/ref_trace.npz
 
 Runs, UNMODIFIED and over a recording brute-force index (tests/ref_harness.RecordingIndex = the reference tests'
 DummyVoyagerIndex contract with float64 ranking and lower-id ties),
@@ -15,7 +15,7 @@ DummyVoyagerIndex contract with float64 ranking and lower-id ties),
 
 on seeded libraries (3000 x 200 "music_library", 2000 x 512 CLAP) with an in-memory metadata table, and stores every
 index call they made (query vector, k -> ids, distances; get_vector id -> vector) together with each function's final
-answer.  tests/test_gpu_ref_trace.py replays the calls against audiomuse_ai_b200.voyager_compat.Index on the B200: if
+answer.  tests/test_gpu_ref_trace.py replays the calls against audiomuse_ai_b200.voyager_compat.Index on the GPU: if
 every call returns what the recording index returned, the reference functions -- deterministic given those returns --
 produce the recorded answers over the shim as well.
 """

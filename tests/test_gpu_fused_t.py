@@ -1,6 +1,6 @@
-"""The channel-per-lane fused block (csrc/fused_block_t.cu) against the unfused layer-by-layer path and against the
-pixel-per-lane kernel it replaces, plus the tcgen05 operand layout it relies on (MN-major A, checked against numpy).
-The kernel choice is read from the environment when the library initialises, so every variant runs in its own process."""
+"""The fused inverted-residual block kernel (csrc/fused_block.cu) against the layer-by-layer path (AM_FUSED_BLOCKS=0:
+expansion GEMM, depthwise kernel, projection GEMM).  The choice is read from the environment when the model is
+loaded, so every variant runs in its own process."""
 import os
 import subprocess
 import sys
@@ -19,7 +19,10 @@ sess = ca.B200Session.from_state_dict(weights.random_state_dict(0))
 rng = np.random.default_rng(0)
 mel = (rng.standard_normal((3, 1, 128, %d)) * 12 - 30).astype(np.float32)
 mel[1, :, :, :] = -100.0                      # digital silence: every bin on the floor
+from audiomuse_ai_b200 import _lib
+_lib.profile_enable(True)
 np.save(sys.argv[1], sess.run(None, {"mel_spectrogram": mel})[0])
+open(sys.argv[1] + ".kernels", "w").write("\n".join(_lib.profile_report()))
 """
 
 
@@ -28,6 +31,8 @@ def _embed(tmp_path, name, env, T=1001):
     r = subprocess.run([sys.executable, "-c", CHILD % (ROOT, T), out], env=dict(os.environ, **env), capture_output=True,
                        text=True, timeout=600)
     assert r.returncode == 0, r.stderr[-3000:]
+    fused_ran = any("fused_block_kernel" in k for k in open(out + ".kernels").read().splitlines())
+    assert fused_ran == (env.get("AM_FUSED_BLOCKS") != "0"), f"{name}: fused kernel ran = {fused_ran}"
     return np.load(out)
 
 
@@ -35,42 +40,20 @@ def _cos(a, b):
     return np.array([float(np.dot(x, y) / (np.linalg.norm(x) * np.linalg.norm(y))) for x, y in zip(a, b)])
 
 
-def test_channel_per_lane_kernel_matches_the_unfused_path_and_the_old_kernel(tmp_path):
-    ref = _embed(tmp_path, "unfused", {"AM_FUSED_BLOCKS": "0"})
-    new = _embed(tmp_path, "fused_t", {})
-    old = _embed(tmp_path, "fused_v1", {"AM_FUSED_V1": "1"})
-    small = _embed(tmp_path, "fused_t_small_tiles", {"AM_FUSEDT_SMALL_TILES": "1"})
-    x0 = _embed(tmp_path, "stem_x0", {"AM_STEM_X0": "1"})
-    for name, got in (("channel-per-lane", new), ("pixel-per-lane", old), ("small tiles", small), ("stem as GEMM", x0)):
-        c = _cos(got, ref)
-        print(f"{name}: min cosine vs unfused {c.min():.7f}, max |diff| {np.abs(got - ref).max():.2e}")
-        assert c.min() > 1 - 1e-4, (name, c)   # (the silent window is the worst: ~6e-5)
-        assert np.abs(got - ref).max() < 2e-3, name
-    # the two fused kernels round the same way up to the activation's clamp: they agree closer than either does with the
-    # unfused path (which keeps the expanded tensor in bf16, the fused kernels in fp16)
-    assert np.abs(new - old).max() < 1.5e-3
+def test_fused_block_kernel_matches_the_layer_by_layer_path(tmp_path):
+    ref = _embed(tmp_path, "layer_by_layer", {"AM_FUSED_BLOCKS": "0"})
+    got = _embed(tmp_path, "fused", {})
+    c = _cos(got, ref)
+    print(f"fused: min cosine vs layer by layer {c.min():.7f}, max |diff| {np.abs(got - ref).max():.2e}")
+    # both round the expanded tensor and the depthwise output to bf16; the depthwise sums in fp32 here, in fp16 pairs
+    # on the layer path
+    assert c.min() > 1 - 1e-4, c
+    assert np.abs(got - ref).max() < 2e-3
 
 
 def test_short_window_runs_through_the_partial_tiles(tmp_path):
-    """T = 333 frames: spatial sizes that are no multiple of the tile heights (last tile of every block is partial)."""
-    ref = _embed(tmp_path, "unfused_s", {"AM_FUSED_BLOCKS": "0"}, T=333)
-    new = _embed(tmp_path, "fused_t_s", {}, T=333)
+    """T = 333 frames: spatial sizes that are no multiple of the 8 x 8 tile (the last tiles of every block are partial)."""
+    ref = _embed(tmp_path, "layer_by_layer_s", {"AM_FUSED_BLOCKS": "0"}, T=333)
+    new = _embed(tmp_path, "fused_s", {}, T=333)
     assert _cos(new, ref).min() > 1 - 1e-4
     assert np.abs(new - ref).max() < 2e-3
-
-
-@pytest.mark.parametrize("N,K,lbo,sbo,rows", [(80, 128, 16384, 1024, 128), (144, 64, 1024, 2048, 128), (80, 128, 0, 1024, 64)])
-def test_mn_major_a_operand_layout(N, K, lbo, sbo, rows):
-    """tcgen05.mma with an MN-major SWIZZLE_128B A operand laid out the way the depthwise warps store it: atoms of
-    64 pixels x 8 channels, LBO between pixel atoms, SBO between channel groups (LBO = 0: the second atom aliases the first)."""
-    from audiomuse_ai_b200 import _lib
-    lib = _lib.load_debug()
-    rng = np.random.default_rng(N + K)
-    a = rng.standard_normal((rows, K)).astype(np.float16)
-    b = rng.standard_normal((N, K)).astype(np.float16)
-    d = np.zeros((128, N), dtype=np.float32)
-    _lib.check_debug(lib.am_probe_mn_major(a.ctypes.data, b.ctypes.data, N, K, lbo, sbo, rows, 0, d.ctypes.data))
-    want = a.astype(np.float32) @ b.astype(np.float32).T
-    if rows == 64:
-        want = np.concatenate([want, want], 0)
-    assert np.abs(d - want).max() < 1e-3 * max(1.0, np.abs(want).max())

@@ -1,4 +1,4 @@
-"""tcgen05/TMA GEMM vs the SIMT reference kernel, on device (am_selftest_gemm).  Each case runs in
+"""wgmma/TMA GEMM vs the SIMT reference kernel, on device (am_selftest_gemm).  Each case runs in
 a subprocess under a timeout so a pipeline hang cannot wedge the test session."""
 import subprocess
 import sys
@@ -12,6 +12,8 @@ CASES = [
     (128, 64, 64, 0), (128, 256, 64, 0), (256, 80, 144, 3), (1000, 432, 80, 3), (4096, 80, 432, 5),
     (333, 2592, 576, 3), (512, 576, 2592, 5), (130, 1360, 288, 3), (128, 5000, 512, 8 | 16),
     (256, 4100, 256, 8 | 16 | 32), (64, 48, 16, 1),
+    # the remaining tile widths: 16, 32, 96, 112 (+ N % 8 != 0 with a residual: the unstaged bf16 epilogue), 128, 160
+    (256, 16, 64, 1), (300, 24, 48, 3), (512, 96, 96, 5), (200, 100, 64, 4 | 1), (333, 128, 144, 3), (257, 136, 80, 5),
 ]
 
 SCRIPT = r"""
@@ -37,4 +39,4 @@ def test_tcgen05_gemm_matches_simt(M, N, K, flags):
     assert int(st) == 0, msg
     # both sides accumulate bf16 products in fp32; only summation order and one bf16 rounding differ
     tol = 0.08 if not (flags & 8) else 2e-3
-    assert float(diff) <= tol, f"max |tcgen05 - simt| = {diff}"
+    assert float(diff) <= tol, f"max |wgmma - simt| = {diff}"

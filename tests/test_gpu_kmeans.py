@@ -133,7 +133,7 @@ def test_config4_scale_properties():
 @pytest.mark.parametrize("n,d,k,kind", [(60000, 512, 128, "clustered"), (40000, 200, 100, "clustered"),
                                         (30000, 58, 40, "uniform"), (20000, 96, 7, "uniform")])
 def test_tensor_core_step_equals_exact_path(n, d, k, kind):
-    """am_kmeans_plan_step (split-bf16 tcgen05 GEMM + fused argmin + exact recheck of near-ties) returns the SAME
+    """am_kmeans_plan_step (split-bf16 wgmma GEMM + fused argmin + exact recheck of near-ties) returns the SAME
     labels as the exact fp32 CUDA-core path (AM_KMEANS_SIMT=1) -- on clustered data and on structureless data, where
     a large share of the points is a near-tie -- and matching counts / sums / inertia.  d = 58, 200 and k in [40, 100]
     are the reference's shapes (clustering_helper.py), 512 / 128 is config 4."""

@@ -19,9 +19,8 @@ def _windows():
 
 
 def _check(got_db, want_db, want_pow, tag=""):
-    """Bounds set from tools/mel_error_report.py on the B200 (profiles/r02_mel_error_report.txt): the kernel's worst
-    error over ALL bins of the corpus is 7.6e-5 dB except under the full-scale sine, whose side bins sit 80-100+ dB
-    below the frame peak (2.7e-4 dB at >= 1e-8 of the peak, 4.6e-3 dB at >= 1e-10).  Asserted:
+    """Bounds for the kernel's fp32 error (tools/mel_error_report.py prints it per bin): bins far below their frame's
+    peak -- the side bins of a full-scale sine sit 80-100+ dB down -- carry the largest error in dB.  Asserted:
       * <= 1e-3 dB on every bin within 80 dB of its frame's strongest bin (SURVEY 7 step 2);
       * everywhere (no mask): |P_got - P_want| <= 1e-3 * P_want + 1e-9 * frame peak -- a bin 80 dB down may be off
         by at most 10 %, one 60 dB down by 0.1 % (the round-1 bound allowed 2e-6 * peak: 100 % at -57 dB)."""

@@ -10,7 +10,7 @@
             style (get_vector + k cycling 101 / 10 / 30 / 100 / 300 / 1000): p50 / p99 latency, queries/s;
             and the same mix in batches of 256
 
-Prints ONE JSON object; `python tools/bench_scale.py > profiles/<tag>_scale.json`.  The oracle is used here only
+Prints ONE JSON object; `python tools/bench_scale.py > scale.json`.  The oracle is used here only
 as the checker of ids / inertia, never as the thing measured.
 """
 import json

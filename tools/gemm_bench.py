@@ -1,4 +1,4 @@
-"""Device-time sweep of the tcgen05 GEMM (am_bench_gemm): TFLOP/s by shape.  GPU box only."""
+"""Device-time sweep of the wgmma GEMM (am_bench_gemm): TFLOP/s by shape.  Needs an H100."""
 import ctypes as C
 import sys
 

@@ -1,4 +1,4 @@
-"""Config 4 (BASELINE.json configs[3]): Lloyd iterations on 1 M x 512 f32 rows, k = 128, one B200.
+"""Config 4 (BASELINE.json configs[3]): Lloyd iterations on 1 M x 512 f32 rows, k = 128, one GPU.
 Times `iters` am_kmeans_plan_step calls (assignment GEMM with fused argmin + recheck + partial sums) with CUDA events,
 checks the labels of the tensor-core path against the exact CUDA-core path (AM_KMEANS_SIMT=1), and prints one JSON line.
     python tools/kmeans_bench.py [--n 1000000] [--iters 20]"""
