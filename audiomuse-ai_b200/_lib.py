@@ -98,6 +98,7 @@ SIGNATURES = {
     "am_pca_moments": (_i, [_vp, _i64, _i, _vp, _vp]),
     "am_pca_project": (_i, [_vp, _i64, _i, _vp, _vp, _i, _vp]),
     "am_dbscan": (_i, [_vp, _i64, _i, _f, _i, _vp, _P(_i)]),
+    "am_cluster_scores": (_i, [_vp, _i64, _i, _vp, _i, _i, _vp, _vp]),
     "am_kmeans_assign_dev": (_i, [_vp, _i64, _i, _vp, _i, _vp, _vp, _vp, _vp, _vp]),
     "am_kmeans_plan_create": (_i, [_vp, _i64, _i, _i, _vp, _P(_vp)]),
     "am_kmeans_plan_step": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),

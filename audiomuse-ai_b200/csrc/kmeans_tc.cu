@@ -32,6 +32,7 @@
 
 #include "gemm_wgmma.cuh"
 #include "ptx_sm90.cuh"
+#include "split_bf16.cuh"
 
 #include <algorithm>
 #include <cmath>
@@ -49,28 +50,7 @@ constexpr int kATile = kTileM * kChunkK * 2;  // 16 KiB
 constexpr int kSlabMax = 4096;                // most points one accumulate CTA sorts at a time
 
 // ---------------------------------------------------------------- split passes
-// one warp per row: Xs[row] = [hi | lo], xn[row] = ||x||^2 (fp32)
-__global__ void __launch_bounds__(256)
-split_rows_kernel(const float* __restrict__ X, int64_t N, int d, int dp, __nv_bfloat16* __restrict__ Xs,
-                  float* __restrict__ xn) {
-  const int lane = threadIdx.x & 31;
-  const int64_t warps = (int64_t)gridDim.x * (blockDim.x >> 5);
-  for (int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); row < N; row += warps) {
-    const float* x = X + row * d;
-    __nv_bfloat16* o = Xs + row * 2 * dp;
-    float acc = 0.f;
-    for (int i = lane; i < dp; i += 32) {
-      const float v = i < d ? x[i] : 0.f;
-      acc = fmaf(v, v, acc);
-      const __nv_bfloat16 hi = __float2bfloat16_rn(v);
-      o[i] = hi;
-      o[dp + i] = __float2bfloat16_rn(v - __bfloat162float(hi));
-    }
-    acc = warp_sum(acc);
-    if (lane == 0 && xn) xn[row] = acc;
-  }
-}
-
+// the rows: split_rows_kernel (split_bf16.cuh, shared with the silhouette kernel)
 // one warp per centre row (incl. the padded rows): Cs, cn, and the max norm (as int bits of a non-negative float)
 __global__ void __launch_bounds__(256)
 split_centers_kernel(const float* __restrict__ C, int k, int d, int kp, int dp, __nv_bfloat16* __restrict__ Cs,

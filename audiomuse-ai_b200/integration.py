@@ -47,11 +47,17 @@ def make_filter_by_distance(vm):
     return _filter_by_distance_b200
 
 
-def apply(clap=None, voyager_manager=None, clustering=None, allow_sklearn_fallback: bool = True) -> None:
-    """clap / voyager_manager / clustering: the reference's already imported tasks.* modules (pass only the ones to
-    patch).  allow_sklearn_fallback keeps the reference's contract that a failing GPU k-means silently falls back to
-    scikit-learn (tasks/clustering_gpu.py:130-148); this repository's own tests run with it off so a missing CUDA
-    library can never pass as the GPU path."""
+METRIC_NAMES = ("silhouette_score", "davies_bouldin_score", "calinski_harabasz_score")
+
+
+def apply(clap=None, voyager_manager=None, clustering=None, allow_sklearn_fallback: bool = True,
+          clustering_helper=None) -> None:
+    """clap / voyager_manager / clustering / clustering_helper: the reference's already imported tasks.* modules (pass
+    only the ones to patch).  allow_sklearn_fallback keeps the reference's contract that a failing GPU k-means silently
+    falls back to scikit-learn (tasks/clustering_gpu.py:130-148); this repository's own tests run with it off so a
+    missing CUDA library can never pass as the GPU path.  clustering_helper imports the three scores by name at module
+    level (tasks/clustering_helper.py:16) and looks them up at call time (:462-470), so replacing the module attributes
+    moves the fitness scoring to the GPU."""
     if clap is not None:
         from . import clap_analyzer as b200_clap
 
@@ -66,5 +72,10 @@ def apply(clap=None, voyager_manager=None, clustering=None, allow_sklearn_fallba
         clustering.GPUDBSCAN = b200_cg.GPUDBSCAN   # get_clustering_model / get_pca_model look the classes up at call time
         clustering.GPUPCA = b200_cg.GPUPCA
         clustering.check_gpu_available = b200_cg.check_gpu_available
-        if allow_sklearn_fallback:
-            os.environ.setdefault("B200_ALLOW_SKLEARN_FALLBACK", "1")
+    if clustering_helper is not None:
+        from . import cluster_metrics as b200_cm
+
+        for name in METRIC_NAMES:
+            setattr(clustering_helper, name, getattr(b200_cm, name))
+    if (clustering is not None or clustering_helper is not None) and allow_sklearn_fallback:
+        os.environ.setdefault("B200_ALLOW_SKLEARN_FALLBACK", "1")

@@ -248,6 +248,16 @@ AM_API int am_pca_project(const float* X, int64_t N, int d, const float* mean, c
  * sklearn.cluster.DBSCAN (clusters in order of their lowest core index, border points take the smallest label among
  * their core neighbours, noise -1).  N <= 2^20 (the neighbourhood bit matrix is N^2 / 8 bytes). */
 AM_API int am_dbscan(const float* X, int64_t N, int d, float eps, int min_samples, int32_t* labels, int* n_clusters);
+/* Clustering scores of tasks/clustering_helper.py:462-470 (sklearn.metrics silhouette_score, davies_bouldin_score,
+ * calinski_harabasz_score; euclidean).  X f32[N, d] (1 <= d <= 8192); labels i32[N] in [0, n_labels), every label
+ * present, 2 <= n_labels <= N - 1 (scikit-learn's LabelEncoder output: DBSCAN's -1 is an ordinary label there);
+ * which = bit 0 silhouette, bit 1 Davies-Bouldin, bit 2 Calinski-Harabasz; scores f64[3] in that order (entries not
+ * asked for are left alone); samples f32[N] optional: the per-row silhouette, caller's row order.  Silhouette runs
+ * as split-bf16 tensor-core distance tiles reduced per cluster in the epilogue (only f64[N, n_labels] is stored);
+ * DB / CH accumulate in float64.  Limits: N <= 2^31 - 129 (int32 permutation), and N * n_labels <= 2^31 when bit 0 is
+ * set; AM_ERR_INVALID beyond them. */
+AM_API int am_cluster_scores(const float* X, int64_t N, int d, const int32_t* labels, int n_labels, int which,
+                             double* scores, float* samples);
 
 /* Iterative form for Lloyd loops on device data (multi-GPU: one plan per rank over its row shard, the host all-reduces
  * sums / counts between steps; tasks/clustering_gpu.py:108-124 is the call this serves).  The plan keeps a split-bf16
