@@ -15,13 +15,18 @@ so a missing CUDA library can never masquerade as the GPU path).
         host + am_pca_project; sets components_, explained_variance_ratio_, n_components_ like sklearn's PCA
     get_pca_model(n_components, use_gpu)                               :407-421
 
-GMM / spectral clustering have no GPU implementation in the reference either (:280-335, scikit-learn always).
+    GPUSpectralClustering(n_clusters, ..., n_neighbors, random_state, n_init).fit_predict(X)   :312-335 -> the reference
+        wraps sklearn.cluster.SpectralClustering; here spectral_embedding (k-NN graph + Chebyshev-filtered subspace
+        iteration, csrc/spectral.cu) + kmeans_fit on the embedding.  Sets labels_, using_gpu; no cluster_centers_.
+
+GMM has no GPU implementation in the reference either (:280-310, scikit-learn always).
 """
 from __future__ import annotations
 
 import ctypes as C
 import logging
 import os
+import time
 
 import numpy as np
 
@@ -239,16 +244,227 @@ class GPUPCA:
         return (np.asarray(X, dtype=np.float64) @ self.components_ + self.mean_).astype(np.float32)
 
 
+# Chebyshev filter of the spectral eigensolver: a degree is chosen so that the filter amplifies by at most _CHEB_AMP
+# (the Gram matrix of the filtered block then has a condition number of about _CHEB_AMP^2, far from float64's limit),
+# and never above _CHEB_MAX_DEGREE SpMMs per outer iteration.
+_CHEB_AMP = 1e4
+_CHEB_MAX_DEGREE = 200
+
+
+def _spectral_block(n_components, N):
+    """b: the wanted vectors + a guard of half as many (at least 16), rounded up to whole 32-column warps (the padding
+    is computed anyway).  The guard vectors widen the gap the filter works against: the convergence rate of the k-th
+    pair is set by lambda_k against lambda_{b+1}, not lambda_{k+1}."""
+    return min(N, -(-(n_components + max(16, n_components // 2)) // 32) * 32)
+
+
+def _cheb_degree(cut):
+    t0 = (3.0 - cut) / (1.0 + cut)                  # where x = 1 lands once [-1, cut] is mapped onto [-1, 1]
+    return int(np.clip(np.floor(np.arccosh(_CHEB_AMP) / np.arccosh(t0)), 1, _CHEB_MAX_DEGREE))
+
+
+def _rayleigh_ritz(G, H):
+    """Ritz pairs of S in the span of V from G = V^T V and H = V^T S V: theta descending, Q with Q^T G Q = I.  G is
+    Jacobi-scaled and whitened through its eigendecomposition (not one Cholesky factor), which stays accurate when a
+    strong filter has left G ill-conditioned."""
+    G = 0.5 * (G + G.T)
+    H = 0.5 * (H + H.T)
+    s = np.sqrt(np.diag(G))
+    if not np.all(s > 0):
+        raise RuntimeError("spectral eigensolver: a block vector vanished")
+    Gs, Hs = G / np.outer(s, s), H / np.outer(s, s)
+    mu, U = np.linalg.eigh(Gs)
+    if mu[0] <= mu[-1] * 1e-14:
+        raise RuntimeError(f"spectral eigensolver: the block lost rank (Gram eigenvalues {mu[0]:.3g} .. {mu[-1]:.3g})")
+    B = U / np.sqrt(mu)
+    T = B.T @ Hs @ B
+    th, Z = np.linalg.eigh(0.5 * (T + T.T))
+    th, Z = th[::-1], Z[:, ::-1]
+    return th.copy(), np.ascontiguousarray((B @ Z) / s[:, None])
+
+
+def spectral_embedding(X, n_components, n_neighbors=10, seed=0, tol=1e-8, max_iter=300, details=None):
+    """-> (embedding f64[N, n_components], eigenvalues of L_sym ascending) with sklearn.manifold.spectral_embedding's
+    meaning for affinity='nearest_neighbors' as SpectralClustering builds it (0.5 (C + C^T) of
+    kneighbors_graph(include_self=True), normed Laplacian, drop_first=False): the eigenvectors of the smallest
+    eigenvalues of L_sym = I - D^-1/2 W D^-1/2, each divided by sqrt(deg) and sign-flipped so that its largest-magnitude
+    entry is positive.
+
+    Chebyshev-filtered subspace iteration on S = I - L_sym (csrc/spectral.cu): filter the block, Rayleigh-Ritz on the
+    host, rotate, repeat until every wanted Ritz pair has ||S u - theta u|| <= tol with ||u|| = 1 (measured on the
+    device).  RuntimeError after max_iter outer iterations: unconverged vectors are never returned.  details (a dict,
+    optional) receives the graph (affinity: W as a scipy CSR matrix without diagonal; dd = sqrt(deg)), the final
+    residuals and the stage counts and times."""
+    X = _check_spectral_input(X)
+    N, d = X.shape
+    k = int(n_components)
+    if not 1 <= k <= N:
+        raise ValueError(f"n_components={n_components} must be between 1 and n_samples={N}")
+    if not 2 <= int(n_neighbors) <= N:
+        raise ValueError(f"n_neighbors={n_neighbors} must be between 2 and n_samples={N}")
+    lib = _lib.load()
+    b = _spectral_block(k, N)
+    plan = C.c_void_p()
+    _lib.check(lib.am_spectral_plan_create(_lib.ptr(X), N, d, int(n_neighbors), b, int(seed) & 0xFFFFFFFFFFFFFFFF,
+                                           C.byref(plan)))
+    try:
+        t0 = time.perf_counter()
+        G, H = np.empty((b, b)), np.empty((b, b))
+        res = np.full(k, np.inf)
+        Q, cut, it = None, None, 0
+        while True:
+            if it == max_iter:
+                raise RuntimeError(f"spectral eigensolver did not converge in {max_iter} iterations "
+                                   f"(largest residual {res.max():.3g} > tol {tol:g})")
+            degree = 0 if cut is None else _cheb_degree(cut)
+            _lib.check(lib.am_spectral_plan_iterate(plan, None if Q is None else _lib.ptr(Q), degree,
+                                                    0.0 if cut is None else cut, _lib.ptr(G), _lib.ptr(H)))
+            it += 1
+            theta, Q = _rayleigh_ritz(G, H)
+            Qk, thk = np.ascontiguousarray(Q[:, :k]), np.ascontiguousarray(theta[:k])
+            _lib.check(lib.am_spectral_plan_residuals(plan, _lib.ptr(Qk), _lib.ptr(thk), k, _lib.ptr(res), None))
+            if np.all(res <= tol):
+                break
+            cut = float(np.clip(theta[-1], -1.0 + 1e-12, 1.0 - 1e-12))   # damp everything below the block
+        emb = np.empty((N, k), dtype=np.float64)
+        _lib.check(lib.am_spectral_plan_embed(plan, _lib.ptr(Qk), k, _lib.ptr(emb)))
+        eig_s = time.perf_counter() - t0
+        if details is not None:
+            nnz, blk, n_spmm = C.c_int64(0), C.c_int(0), C.c_int64(0)
+            knn_ms, graph_ms = C.c_float(0), C.c_float(0)
+            _lib.check(lib.am_spectral_plan_info(plan, C.byref(nnz), C.byref(blk), C.byref(n_spmm), C.byref(knn_ms),
+                                                 C.byref(graph_ms)))
+            details.update(block=int(blk.value), nnz=int(nnz.value), n_spmm=int(n_spmm.value), outer_iterations=it,
+                           knn_ms=float(knn_ms.value), graph_ms=float(graph_ms.value), eigensolver_ms=1e3 * eig_s,
+                           residuals=res.copy())
+            details["affinity"], details["dd"] = _spectral_graph(lib, plan, N, int(nnz.value))
+    finally:
+        lib.am_spectral_plan_free(plan)
+    # sklearn.utils.extmath._deterministic_vector_sign_flip on the (n_components, N) layout
+    top = np.argmax(np.abs(emb), axis=0)
+    signs = np.sign(emb[top, np.arange(k)])
+    signs[signs == 0] = 1.0
+    emb *= signs[None, :]
+    return emb, 1.0 - thk
+
+
+def spectral_graph(X, n_neighbors=10):
+    """-> (W, dd): the affinity graph spectral_embedding works on, built on the device -- W = 0.5 (C + C^T) of
+    kneighbors_graph(X, n_neighbors, include_self=True) without its diagonal, as a scipy CSR matrix (float32 values 0.5
+    or 1, sorted column indices) -- and dd = sqrt(row sums of W), float64."""
+    X = _check_spectral_input(X)
+    N, d = X.shape
+    if not 2 <= int(n_neighbors) <= N:
+        raise ValueError(f"n_neighbors={n_neighbors} must be between 2 and n_samples={N}")
+    lib = _lib.load()
+    plan = C.c_void_p()
+    _lib.check(lib.am_spectral_plan_create(_lib.ptr(X), N, d, int(n_neighbors), 1, 0, C.byref(plan)))
+    try:
+        nnz = C.c_int64(0)
+        _lib.check(lib.am_spectral_plan_info(plan, C.byref(nnz), None, None, None, None))
+        return _spectral_graph(lib, plan, N, int(nnz.value))
+    finally:
+        lib.am_spectral_plan_free(plan)
+
+
+def _spectral_graph(lib, plan, N, nnz):
+    import scipy.sparse as sp
+    indptr, indices = np.empty(N + 1, np.int64), np.empty(max(nnz, 1), np.int32)
+    data, dd = np.empty(max(nnz, 1), np.float32), np.empty(N, np.float64)
+    _lib.check(lib.am_spectral_plan_graph(plan, _lib.ptr(indptr), _lib.ptr(indices), _lib.ptr(data), _lib.ptr(dd)))
+    return sp.csr_matrix((data[:nnz], indices[:nnz], indptr), shape=(N, N)), dd
+
+
+def _check_spectral_input(X):
+    X = np.asarray(X)
+    if X.ndim != 2:
+        raise ValueError(f"Expected 2D array, got {X.ndim}D array instead")
+    if X.shape[0] < 2 or X.shape[1] < 1:
+        raise ValueError(f"Found array with shape {X.shape}: need at least 2 samples and 1 feature")
+    X32 = np.ascontiguousarray(X, dtype=np.float32)
+    if not (np.isfinite(X).all() and np.isfinite(X32).all()):
+        raise ValueError("Input X contains NaN or infinity.")
+    return X32
+
+
+class GPUSpectralClustering:
+    """tasks/clustering_gpu.py:312-335 (sklearn.cluster.SpectralClustering there) on the device: the k-NN affinity
+    graph and the Laplacian eigenvectors come from spectral_embedding, the labels from kmeans_fit on the embedding with
+    n_init restarts.  Sets labels_ and using_gpu.  It sets no cluster_centers_ / means_, so the clustering task takes
+    the per-label means of the data as the centres (clustering_helper.py:320-333), as it does for scikit-learn's
+    class."""
+
+    def __init__(self, n_clusters, assign_labels="kmeans", affinity="nearest_neighbors", n_neighbors=10,
+                 random_state=None, n_init=10, verbose=False):
+        self.n_clusters = n_clusters
+        self.assign_labels = assign_labels
+        self.affinity = affinity
+        self.n_neighbors = n_neighbors
+        self.random_state = random_state
+        self.n_init = n_init
+        self.verbose = verbose
+        self.model = None
+        self.labels_ = None
+        self.using_gpu = False
+
+    def _validate(self, X):
+        if self.affinity != "nearest_neighbors":
+            raise ValueError(f"affinity={self.affinity!r} is not supported on the GPU (only 'nearest_neighbors')")
+        if self.assign_labels != "kmeans":
+            raise ValueError(f"assign_labels={self.assign_labels!r} is not supported on the GPU (only 'kmeans')")
+        X = _check_spectral_input(X)
+        N = X.shape[0]
+        if not 2 <= int(self.n_clusters) <= N - 1:
+            raise ValueError(f"n_clusters={self.n_clusters} must be between 2 and n_samples - 1 = {N - 1}")
+        if not 2 <= int(self.n_neighbors) <= N:
+            raise ValueError(f"n_neighbors={self.n_neighbors} must be between 2 and n_samples = {N}")
+        return X
+
+    def fit_predict(self, X):
+        X32 = self._validate(X)
+        try:
+            seed = 0 if self.random_state is None else int(self.random_state)
+            emb, _ = spectral_embedding(X32, int(self.n_clusters), n_neighbors=int(self.n_neighbors), seed=seed)
+            _, labels, _, _ = kmeans_fit(emb.astype(np.float32), int(self.n_clusters), n_init=int(self.n_init),
+                                         seed=seed)
+            self.labels_, self.using_gpu = labels, True
+            logger.debug(f"GPU SpectralClustering completed: {self.n_clusters} clusters")
+            return labels
+        except Exception as e:
+            if os.environ.get("B200_ALLOW_SKLEARN_FALLBACK", "0") != "1":
+                raise
+            logger.warning(f"GPU SpectralClustering failed, falling back to CPU: {e}")
+        from sklearn.cluster import SpectralClustering
+        self.model = SpectralClustering(n_clusters=self.n_clusters, assign_labels=self.assign_labels,
+                                        affinity=self.affinity, n_neighbors=self.n_neighbors,
+                                        random_state=self.random_state, n_init=self.n_init, verbose=self.verbose)
+        self.labels_ = self.model.fit_predict(X)
+        self.using_gpu = False
+        return self.labels_
+
+    def fit(self, X):
+        self.fit_predict(X)
+        return self
+
+
 def get_clustering_model(method, params, use_gpu=False):
     if use_gpu and method == "kmeans":
         return GPUKMeans(n_clusters=params["n_clusters"], init="k-means++", n_init=10)
     if use_gpu and method == "dbscan":
         return GPUDBSCAN(eps=params["eps"], min_samples=params["min_samples"])
-    from sklearn.cluster import DBSCAN, KMeans
+    if use_gpu and method == "spectral":
+        return GPUSpectralClustering(n_clusters=params["n_clusters"], assign_labels="kmeans",
+                                     affinity="nearest_neighbors", n_neighbors=params.get("n_neighbors", 20),
+                                     random_state=params.get("random_state"), n_init=10, verbose=False)
+    from sklearn.cluster import DBSCAN, KMeans, SpectralClustering
     if method == "kmeans":
         return KMeans(n_clusters=params["n_clusters"], init="k-means++", n_init=10)
     if method == "dbscan":
         return DBSCAN(eps=params["eps"], min_samples=params["min_samples"])
+    if method == "spectral":
+        return SpectralClustering(n_clusters=params["n_clusters"], assign_labels="kmeans", affinity="nearest_neighbors",
+                                  n_neighbors=params.get("n_neighbors", 20), random_state=params.get("random_state"),
+                                  n_init=10, verbose=False)
     raise ValueError(f"Unsupported clustering method: {method}")
 
 

@@ -71,6 +71,7 @@ def apply(clap=None, voyager_manager=None, clustering=None, allow_sklearn_fallba
         clustering.GPUKMeans = b200_cg.GPUKMeans
         clustering.GPUDBSCAN = b200_cg.GPUDBSCAN   # get_clustering_model / get_pca_model look the classes up at call time
         clustering.GPUPCA = b200_cg.GPUPCA
+        clustering.GPUSpectralClustering = b200_cg.GPUSpectralClustering
         clustering.check_gpu_available = b200_cg.check_gpu_available
     if clustering_helper is not None:
         from . import cluster_metrics as b200_cm

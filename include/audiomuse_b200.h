@@ -274,6 +274,36 @@ AM_API int am_kmeans_plan_uses_tensor_cores(const am_kmeans_plan* plan);
 AM_API int am_kmeans_plan_last_recheck(am_kmeans_plan* plan, void* stream, int* n_rows);
 AM_API void am_kmeans_plan_free(am_kmeans_plan* plan);
 
+/* ------------------------------------------------------------------ spectral clustering (graph + eigensolver)
+ * Replaces sklearn.cluster.SpectralClustering(affinity='nearest_neighbors') behind GPUSpectralClustering
+ * (tasks/clustering_gpu.py:312-335).  The plan holds, on the device, X's k-NN graph W = 0.5 (C + C^T) without its
+ * diagonal (C = kneighbors_graph(X, n_neighbors, include_self=True): exact euclidean lists of am_knn_query), dd =
+ * sqrt(row sums of W) and S = D^-1/2 W D^-1/2 in float64, and a block V f64[N, block] seeded from `seed`.  The
+ * host runs the subspace iteration (audiomuse-ai_b200/clustering_gpu.py, spectral_embedding): it only sees block x block
+ * matrices and length-block vectors.  Every call is synchronous; a plan is used by one thread at a time.
+ *   _create      X f32[N, d] (host), 2 <= n_neighbors <= N, 1 <= block <= N, N < 2^31
+ *   _info        nnz of W, the block width, SpMMs run so far, device ms of the k-NN stage and of the CSR build
+ *   _graph       W as CSR: indptr i64[N + 1], indices i32[nnz] (ascending per row), data f32[nnz] (0.5 or 1), and
+ *                dd f64[N]; each pointer optional
+ *   _iterate     Q f64[block, block] (row-major, optional): V <- V Q first.  Then V <- p(S) V, p the scaled Chebyshev
+ *                polynomial of `degree` that damps [-1, cut] and is 1 at 1 (degree 0: no filter).  Returns
+ *                G = V^T V and H = V^T S V, f64[block, block]
+ *   _residuals   Q f64[block, ncols], theta f64[ncols]: res[c] = ||S V q_c - theta_c V q_c|| / ||V q_c|| and, optional,
+ *                norms[c] = ||V q_c||, for the V of the last _iterate
+ *   _embed       out f64[N, ncols] = (V Q)[i, c] / dd[i], Q f64[block, ncols] */
+typedef struct am_spectral_plan am_spectral_plan;
+AM_API int am_spectral_plan_create(const float* X, int64_t N, int d, int n_neighbors, int block, uint64_t seed,
+                                   am_spectral_plan** out);
+AM_API int am_spectral_plan_info(const am_spectral_plan* plan, int64_t* nnz, int* block, int64_t* n_spmm,
+                                 float* knn_ms, float* graph_ms);
+AM_API int am_spectral_plan_graph(am_spectral_plan* plan, int64_t* indptr, int32_t* indices, float* data, double* dd);
+AM_API int am_spectral_plan_iterate(am_spectral_plan* plan, const double* Q, int degree, double cut, double* G,
+                                    double* H);
+AM_API int am_spectral_plan_residuals(am_spectral_plan* plan, const double* Q, const double* theta, int ncols,
+                                      double* res, double* norms);
+AM_API int am_spectral_plan_embed(am_spectral_plan* plan, const double* Q, int ncols, double* out);
+AM_API void am_spectral_plan_free(am_spectral_plan* plan);
+
 #ifdef __cplusplus
 }
 #endif
