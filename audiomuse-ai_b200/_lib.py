@@ -97,7 +97,7 @@ SIGNATURES = {
     "am_kmeans_fit": (_i, [_vp, _i64, _i, _i, _i, _i, _f, _u64, _vp, _vp, _vp, _P(_f), _P(_i)]),
     "am_pca_moments": (_i, [_vp, _i64, _i, _vp, _vp]),
     "am_pca_project": (_i, [_vp, _i64, _i, _vp, _vp, _i, _vp]),
-    "am_dbscan": (_i, [_vp, _i64, _i, _f, _i, _vp, _P(_i)]),
+    "am_dbscan": (_i, [_vp, _i64, _i, C.c_double, _i, _vp, _P(_i)]),
     "am_cluster_scores": (_i, [_vp, _i64, _i, _vp, _i, _i, _vp, _vp]),
     "am_kmeans_assign_dev": (_i, [_vp, _i64, _i, _vp, _i, _vp, _vp, _vp, _vp, _vp]),
     "am_kmeans_plan_create": (_i, [_vp, _i64, _i, _i, _vp, _P(_vp)]),

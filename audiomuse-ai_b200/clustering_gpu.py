@@ -114,6 +114,20 @@ class GPUKMeans:
         return d2.argmin(1).astype(np.int32)
 
 
+def _finite_f32(X):
+    """X as C-contiguous float32 [N, d]; ValueError (scikit-learn's) for another rank or for NaN / inf, also after the
+    cast to float32, before any device work.  A non-finite row is adjacent to nothing in the distance kernels, so without
+    this check DBSCAN would call it noise and PCA would feed NaN to eigh."""
+    X = np.asarray(X)
+    if X.ndim != 2:
+        raise ValueError(f"Expected 2D array, got {X.ndim}D array instead")
+    with np.errstate(over="ignore"):   # a float64 value beyond float32's range becomes inf here and is reported below
+        X32 = np.ascontiguousarray(X, dtype=np.float32)
+    if not (np.isfinite(X).all() and np.isfinite(X32).all()):
+        raise ValueError("Input X contains NaN or infinity.")
+    return X32
+
+
 class GPUDBSCAN:
     """tasks/clustering_gpu.py:151-199.  labels_ are sklearn.cluster.DBSCAN's (same numbering), computed on the device."""
 
@@ -126,10 +140,8 @@ class GPUDBSCAN:
         self.using_gpu = False
 
     def fit_predict(self, X):
+        X = _finite_f32(X)
         try:
-            X = np.ascontiguousarray(X, dtype=np.float32)
-            if X.ndim != 2:
-                raise ValueError("X must be [N, d]")
             labels = np.empty((X.shape[0],), dtype=np.int32)
             n = C.c_int(0)
             _lib.check(_lib.load().am_dbscan(_lib.ptr(X), X.shape[0], X.shape[1], float(self.eps), int(self.min_samples),
@@ -186,8 +198,8 @@ class GPUPCA:
         self.using_gpu = False
 
     def fit_transform(self, X):
+        X32 = _finite_f32(X)
         try:
-            X32 = np.ascontiguousarray(X, dtype=np.float32)
             N, d = X32.shape
             kmax = min(N, d)
             if isinstance(self.n_components, float) and 0 < self.n_components < 1:
@@ -201,8 +213,8 @@ class GPUPCA:
                     raise ValueError(f"n_components={self.n_components} must be between 1 and min(n_samples, n_features)={kmax}")
                 mean, comps, ev, total = pca_fit(X32, k)
             Y = np.empty((N, k), dtype=np.float32)
-            m32, c32 = mean.astype(np.float32), np.ascontiguousarray(comps, dtype=np.float32)
-            _lib.check(_lib.load().am_pca_project(_lib.ptr(X32), N, d, _lib.ptr(m32), _lib.ptr(c32), k, _lib.ptr(Y)))
+            c32 = np.ascontiguousarray(comps, dtype=np.float32)
+            _lib.check(_lib.load().am_pca_project(_lib.ptr(X32), N, d, _lib.ptr(mean), _lib.ptr(c32), k, _lib.ptr(Y)))
             self.mean_, self.components_ = mean, comps
             self.explained_variance_, self.explained_variance_ratio_ = ev, ev / total
             self.n_components_, self.using_gpu = k, True
@@ -229,10 +241,11 @@ class GPUPCA:
             raise ValueError("Model must be fitted before transform")
         if not self.using_gpu:
             return self.model.transform(X)
-        X32 = np.ascontiguousarray(X, dtype=np.float32)
+        X32 = _finite_f32(X)
         Y = np.empty((X32.shape[0], self.n_components_), dtype=np.float32)
-        m32, c32 = self.mean_.astype(np.float32), np.ascontiguousarray(self.components_, dtype=np.float32)
-        _lib.check(_lib.load().am_pca_project(_lib.ptr(X32), X32.shape[0], X32.shape[1], _lib.ptr(m32), _lib.ptr(c32),
+        m64 = np.ascontiguousarray(self.mean_, dtype=np.float64)
+        c32 = np.ascontiguousarray(self.components_, dtype=np.float32)
+        _lib.check(_lib.load().am_pca_project(_lib.ptr(X32), X32.shape[0], X32.shape[1], _lib.ptr(m64), _lib.ptr(c32),
                                               int(self.n_components_), _lib.ptr(Y)))
         return Y
 
@@ -376,14 +389,9 @@ def _spectral_graph(lib, plan, N, nnz):
 
 
 def _check_spectral_input(X):
-    X = np.asarray(X)
-    if X.ndim != 2:
-        raise ValueError(f"Expected 2D array, got {X.ndim}D array instead")
-    if X.shape[0] < 2 or X.shape[1] < 1:
-        raise ValueError(f"Found array with shape {X.shape}: need at least 2 samples and 1 feature")
-    X32 = np.ascontiguousarray(X, dtype=np.float32)
-    if not (np.isfinite(X).all() and np.isfinite(X32).all()):
-        raise ValueError("Input X contains NaN or infinity.")
+    X32 = _finite_f32(X)
+    if X32.shape[0] < 2 or X32.shape[1] < 1:
+        raise ValueError(f"Found array with shape {X32.shape}: need at least 2 samples and 1 feature")
     return X32
 
 

@@ -4,13 +4,17 @@
 // PCA   am_pca_moments: column means + covariance (n - 1 normalisation), accumulated in float64 on the device -- H100 has
 //       FP64 to spare (N d^2 DFMA: 2.6e10 for 100 k x 512) and the eigenvectors of a float32 covariance would not match
 //       LAPACK's to better than 1e-4.  The d x d eigenproblem stays on the host (numpy / LAPACK, like the reference's
-//       Python); am_pca_project applies (X - mean) W^T on the device.
+//       Python); am_pca_project applies (X - mean) W^T on the device, centring against the float64 mean in float64 (a
+//       float32 mean would cost |mean| * 2^-24 per coordinate, which is large next to a small spread).
 // DBSCAN brute force, exact: one pass of tiled squared distances (fp32 differences, float64 re-check inside a relative
-//       1e-5 band around eps^2) writes the eps-neighbourhood relation as an N x N bit matrix (1.25 GB at 100 k rows) and the
-//       neighbour counts; core points = count >= min_samples (the point itself included, as scikit-learn); clusters =
-//       connected components of the core-core relation (min-index label propagation with pointer jumping over the bit
-//       rows); a border point takes the SMALLEST label among its core neighbours -- which is what scikit-learn's
-//       index-ordered depth-first expansion produces, clusters being numbered by their lowest core index.
+//       1e-5 band around eps^2, against eps^2 formed in float64 from the caller's double eps) writes the eps-neighbourhood
+//       relation as an N x N bit matrix (1.25 GB at 100 k rows) and the neighbour counts; core points = count >=
+//       min_samples (the point itself included, as scikit-learn); clusters = connected components of the core-core
+//       relation, found in one pass by lock-free union-find (each edge hooks the larger root under the smaller with
+//       atomicCAS, then a compress pass), so the work does not depend on the index order of the points and no iteration
+//       cap can cut a component short; every root is the lowest core index of its component; a border point takes the
+//       SMALLEST root among its core neighbours -- which is what scikit-learn's index-ordered depth-first expansion
+//       produces, clusters being numbered by their lowest core index.
 #include "common.cuh"
 
 #include <algorithm>
@@ -82,15 +86,16 @@ __global__ void cov_finish_kernel(double* __restrict__ Cov, int d, double inv) {
   if ((j / kCovTile) > (i / kCovTile)) Cov[(int64_t)j * d + i] = v;
 }
 
-// Y[r, c] = sum_i (X[r, i] - mu_i) W[c, i]  (float64 accumulation); one warp per row, components in shared memory chunks
+// Y[r, c] = sum_i (X[r, i] - mu_i) W[c, i]  (centring and accumulation in float64); one warp per row, the centred row in
+// shared memory (rounded to float once, after the float64 subtraction)
 __global__ void __launch_bounds__(256)
-pca_project_kernel(const float* __restrict__ X, int64_t N, int d, const float* __restrict__ mean, const float* __restrict__ W,
+pca_project_kernel(const float* __restrict__ X, int64_t N, int d, const double* __restrict__ mean, const float* __restrict__ W,
                    int k, float* __restrict__ Y) {
   extern __shared__ float s_row[];   // [8 warps][d]
   const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
   float* xr = s_row + (size_t)wib * d;
   for (int64_t r = (int64_t)blockIdx.x * 8 + wib; r < N; r += (int64_t)gridDim.x * 8) {
-    for (int i = lane; i < d; i += 32) xr[i] = X[r * d + i] - mean[i];
+    for (int i = lane; i < d; i += 32) xr[i] = (float)((double)X[r * d + i] - mean[i]);
     __syncwarp();
     for (int c = 0; c < k; ++c) {
       double acc = 0.0;
@@ -108,8 +113,8 @@ pca_project_kernel(const float* __restrict__ X, int64_t N, int d, const float* _
 // adjacency bits + neighbour counts.  Tile: 64 rows (i) x 64 rows (j); thread (ty, tx) owns a 4 x 4 block of pairs.
 constexpr int kDbTile = 64, kDbK = 32;
 __global__ void __launch_bounds__(256)
-dbscan_adj_kernel(const float* __restrict__ X, int N, int d, float eps2, uint32_t* __restrict__ adj, int words,
-                  int* __restrict__ count) {
+dbscan_adj_kernel(const float* __restrict__ X, int N, int d, float eps2, double eps2_exact, uint32_t* __restrict__ adj,
+                  int words, int* __restrict__ count) {
   __shared__ float sa[kDbK][kDbTile + 1], sb[kDbK][kDbTile + 1];
   __shared__ uint32_t sbits[kDbTile][2];
   const int i0 = blockIdx.y * kDbTile, j0 = blockIdx.x * kDbTile;
@@ -158,7 +163,7 @@ dbscan_adj_kernel(const float* __restrict__ X, int N, int d, float eps2, uint32_
           const double t = (double)X[(int64_t)i * d + k] - (double)X[(int64_t)j * d + k];
           s = fma(t, t, s);
         }
-        in = s <= (double)eps2;
+        in = s <= eps2_exact;
       }
       if (in) bits |= 1u << (tx * 4 + v & 31);
     }
@@ -175,7 +180,7 @@ dbscan_adj_kernel(const float* __restrict__ X, int N, int d, float eps2, uint32_
   }
 }
 
-// label[i] = i for core points, INT_MAX otherwise
+// label[i] = i for core points (a forest of singletons), INT_MAX otherwise
 __global__ void dbscan_init_kernel(const int* __restrict__ count, int N, int min_samples, int* __restrict__ label,
                                    unsigned char* __restrict__ core) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -185,38 +190,66 @@ __global__ void dbscan_init_kernel(const int* __restrict__ count, int N, int min
   label[i] = c ? i : 0x7fffffff;
 }
 
-// one propagation round over the core-core relation: label[i] = min(label[i], min_j label[j]), then pointer jumping.
-// One warp per row; *changed is set when any label moved.
+// Union-find forest over the core points, stored in label[]: label[x] == x for a root, label[x] < x otherwise.  A root
+// only stops being one by a successful atomicCAS that hangs it under a smaller index, and every other write stores an
+// ancestor, so a parent read at any time is an ancestor, and the root of a tree is its smallest index.
+__device__ __forceinline__ int uf_find(int* parent, int x) {
+  for (;;) {   // path halving; terminates because a parent is always smaller than its child
+    const int p = __ldcg(parent + x);
+    if (p == x) return x;
+    const int gp = __ldcg(parent + p);
+    if (gp == p) return p;
+    // x is not a root, so no atomicCAS targets it.  The store may overwrite a nearer ancestor written meanwhile by
+    // another thread; any ancestor is a valid parent while hooking, but not as a final label (see the compress kernel).
+    parent[x] = gp;
+    x = gp;
+  }
+}
+
+// hooking: the larger root goes under the smaller; a failed atomicCAS means that root was just hooked elsewhere, so
+// continue from its new root.  Each failure moves one of the two to a smaller index, so the loop ends.
+__device__ __forceinline__ void uf_union(int* parent, int a, int b) {
+  a = uf_find(parent, a);
+  b = uf_find(parent, b);
+  while (a != b) {
+    if (a > b) {
+      const int t = a;
+      a = b;
+      b = t;
+    }
+    const int old = atomicCAS(parent + b, b, a);
+    if (old == b) return;
+    b = uf_find(parent, old);
+  }
+}
+
+// every core-core edge of row i is hooked once from each end; one warp per row, one pass over the bit matrix
 __global__ void __launch_bounds__(256)
-dbscan_propagate_kernel(const uint32_t* __restrict__ adj, int words, int N, const unsigned char* __restrict__ core,
-                        int* __restrict__ label, int* __restrict__ changed) {
+dbscan_hook_kernel(const uint32_t* __restrict__ adj, int words, int N, const unsigned char* __restrict__ core,
+                   int* __restrict__ label) {
   const int lane = threadIdx.x & 31;
   const int i = blockIdx.x * 8 + (threadIdx.x >> 5);
   if (i >= N || !core[i]) return;
-  int best = label[i];
   const uint32_t* row = adj + (int64_t)i * words;
   for (int w = lane; w < words; w += 32) {
     uint32_t b = row[w];
     while (b) {
       const int j = w * 32 + __ffs(b) - 1;
       b &= b - 1;
-      if (core[j]) best = min(best, label[j]);
+      if (j != i && core[j]) uf_union(label, i, j);
     }
   }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) best = min(best, __shfl_xor_sync(0xffffffffu, best, o));
-  if (lane == 0) {
-    int root = best;
-    for (int hop = 0; hop < 8; ++hop) {   // pointer jumping: labels are indices of core points with smaller labels
-      const int up = label[root];
-      if (up >= root) break;
-      root = up;
-    }
-    if (root < label[i]) {
-      atomicMin(&label[i], root);
-      *changed = 1;
-    }
-  }
+}
+
+// after every hook: each core point takes its root, the lowest core index of its component.  The walk writes nothing
+// but label[i] itself: a path-halving store from another thread could land after label[i] = root and put a
+// non-root ancestor back.
+__global__ void dbscan_compress_kernel(int N, const unsigned char* __restrict__ core, int* __restrict__ label) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= N || !core[i]) return;
+  int r = i;
+  for (int p = __ldcg(label + r); p != r; p = __ldcg(label + r)) r = p;
+  label[i] = r;
 }
 
 // border points: the smallest component label among core neighbours (noise: none)
@@ -277,19 +310,20 @@ extern "C" int am_pca_moments(const float* X, int64_t N, int d, double* mean, do
   return AM_OK;
 }
 
-extern "C" int am_pca_project(const float* X, int64_t N, int d, const float* mean, const float* components, int k,
+extern "C" int am_pca_project(const float* X, int64_t N, int d, const double* mean, const float* components, int k,
                               float* Y) {
   AM_CHECK(X && mean && components && Y && N >= 1 && d >= 1 && k >= 1 && d <= 8192, "am_pca_project: bad argument");
   AM_TRY(ensure_init());
   Stream st;
   AM_TRY(st.create());
-  DevBuf<float> dX, dM, dW, dY;
+  DevBuf<float> dX, dW, dY;
+  DevBuf<double> dM;
   AM_TRY(dX.alloc((size_t)N * d));
   AM_TRY(dM.alloc((size_t)d));
   AM_TRY(dW.alloc((size_t)k * d));
   AM_TRY(dY.alloc((size_t)N * k));
   AM_CUDA(cudaMemcpyAsync(dX.p, X, (size_t)N * d * 4, cudaMemcpyHostToDevice, st.s));
-  AM_CUDA(cudaMemcpyAsync(dM.p, mean, (size_t)d * 4, cudaMemcpyHostToDevice, st.s));
+  AM_CUDA(cudaMemcpyAsync(dM.p, mean, (size_t)d * 8, cudaMemcpyHostToDevice, st.s));
   AM_CUDA(cudaMemcpyAsync(dW.p, components, (size_t)k * d * 4, cudaMemcpyHostToDevice, st.s));
   const size_t smem = (size_t)8 * d * 4;
   AM_CHECK(smem <= 200 * 1024, "am_pca_project: %d features do not fit the row buffer", d);
@@ -305,38 +339,32 @@ extern "C" int am_pca_project(const float* X, int64_t N, int d, const float* mea
   return AM_OK;
 }
 
-extern "C" int am_dbscan(const float* X, int64_t N64, int d, float eps, int min_samples, int32_t* labels, int* n_clusters) {
-  AM_CHECK(X && labels && N64 >= 1 && N64 <= (1 << 20) && d >= 1 && eps > 0.f && min_samples >= 1,
-           "am_dbscan: bad argument (1 <= N <= 2^20, eps > 0, min_samples >= 1)");
+extern "C" int am_dbscan(const float* X, int64_t N64, int d, double eps, int min_samples, int32_t* labels, int* n_clusters) {
+  AM_CHECK(X && labels && N64 >= 1 && N64 <= (1 << 20) && d >= 1 && eps > 0.0 && eps * eps <= 3.0e38 && min_samples >= 1,
+           "am_dbscan: bad argument (1 <= N <= 2^20, 0 < eps, eps^2 finite in float, min_samples >= 1)");
   AM_TRY(ensure_init());
   const int N = (int)N64, words = (N + 31) / 32;
   Stream st;
   AM_TRY(st.create());
   DevBuf<float> dX;
   DevBuf<uint32_t> adj;
-  DevBuf<int> count, label, out, changed;
+  DevBuf<int> count, label, out;
   DevBuf<unsigned char> core;
   AM_TRY(dX.alloc((size_t)N * d));
   AM_TRY(adj.alloc((size_t)N * words));
   AM_TRY(count.alloc((size_t)N));
   AM_TRY(label.alloc((size_t)N));
   AM_TRY(out.alloc((size_t)N));
-  AM_TRY(changed.alloc(1));
   AM_TRY(core.alloc((size_t)N));
   AM_CUDA(cudaMemcpyAsync(dX.p, X, (size_t)N * d * 4, cudaMemcpyHostToDevice, st.s));
   AM_CUDA(cudaMemsetAsync(count.p, 0, (size_t)N * 4, st.s));
   AM_CUDA(cudaMemsetAsync(adj.p, 0, (size_t)N * words * 4, st.s));
   const unsigned tiles = (unsigned)ceil_div(N, kDbTile);
-  AM_LAUNCH(dbscan_adj_kernel, dim3(tiles, tiles), 256, 0, st.s, dX.p, N, d, eps * eps, adj.p, words, count.p);
+  const double eps2 = eps * eps;
+  AM_LAUNCH(dbscan_adj_kernel, dim3(tiles, tiles), 256, 0, st.s, dX.p, N, d, (float)eps2, eps2, adj.p, words, count.p);
   AM_LAUNCH(dbscan_init_kernel, (unsigned)ceil_div(N, 256), 256, 0, st.s, count.p, N, min_samples, label.p, core.p);
-  for (int round = 0; round < 4096; ++round) {
-    AM_CUDA(cudaMemsetAsync(changed.p, 0, 4, st.s));
-    AM_LAUNCH(dbscan_propagate_kernel, (unsigned)ceil_div(N, 8), 256, 0, st.s, adj.p, words, N, core.p, label.p, changed.p);
-    int h = 0;
-    AM_CUDA(cudaMemcpyAsync(&h, changed.p, 4, cudaMemcpyDeviceToHost, st.s));
-    AM_CUDA(cudaStreamSynchronize(st.s));
-    if (!h) break;
-  }
+  AM_LAUNCH(dbscan_hook_kernel, (unsigned)ceil_div(N, 8), 256, 0, st.s, adj.p, words, N, core.p, label.p);
+  AM_LAUNCH(dbscan_compress_kernel, (unsigned)ceil_div(N, 256), 256, 0, st.s, N, core.p, label.p);
   AM_LAUNCH(dbscan_border_kernel, (unsigned)ceil_div(N, 8), 256, 0, st.s, adj.p, words, N, core.p, label.p, out.p);
   std::vector<int> h((size_t)N);
   AM_CUDA(cudaMemcpyAsync(h.data(), out.p, (size_t)N * 4, cudaMemcpyDeviceToHost, st.s));

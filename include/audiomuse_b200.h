@@ -241,13 +241,15 @@ AM_API int am_kmeans_assign_dev(const float* X_dev, int64_t N, int d, const floa
  * Replace cuml.decomposition.PCA / cuml.cluster.DBSCAN behind GPUPCA / GPUDBSCAN (tasks/clustering_gpu.py:151-278);
  * scikit-learn's results are the bar (its CPU classes are the reference's own fallback).
  * am_pca_moments: column means f64[d] and the covariance f64[d, d] (n - 1 normalisation), float64 accumulation on the
- * device; the d x d eigenproblem is the host's (LAPACK).  am_pca_project: Y f32[N, k] = (X - mean) components^T. */
+ * device; the d x d eigenproblem is the host's (LAPACK).  am_pca_project: Y f32[N, k] = (X - mean) components^T, the
+ * centring done in float64 against the float64 mean. */
 AM_API int am_pca_moments(const float* X, int64_t N, int d, double* mean, double* cov);
-AM_API int am_pca_project(const float* X, int64_t N, int d, const float* mean, const float* components, int k, float* Y);
+AM_API int am_pca_project(const float* X, int64_t N, int d, const double* mean, const float* components, int k, float* Y);
 /* Exact brute-force DBSCAN (euclidean, eps-neighbourhood includes the point itself): labels i32[N] numbered like
  * sklearn.cluster.DBSCAN (clusters in order of their lowest core index, border points take the smallest label among
- * their core neighbours, noise -1).  N <= 2^20 (the neighbourhood bit matrix is N^2 / 8 bytes). */
-AM_API int am_dbscan(const float* X, int64_t N, int d, float eps, int min_samples, int32_t* labels, int* n_clusters);
+ * their core neighbours, noise -1).  A pair is a neighbour pair when its float64 squared distance is <= eps * eps in
+ * float64, as in scikit-learn on the float64 copy of X.  N <= 2^20 (the neighbourhood bit matrix is N^2 / 8 bytes). */
+AM_API int am_dbscan(const float* X, int64_t N, int d, double eps, int min_samples, int32_t* labels, int* n_clusters);
 /* Clustering scores of tasks/clustering_helper.py:462-470 (sklearn.metrics silhouette_score, davies_bouldin_score,
  * calinski_harabasz_score; euclidean).  X f32[N, d] (1 <= d <= 8192); labels i32[N] in [0, n_labels), every label
  * present, 2 <= n_labels <= N - 1 (scikit-learn's LabelEncoder output: DBSCAN's -1 is an ordinary label there);
