@@ -28,8 +28,8 @@
 //   seg_dist_kernel           per-label sums of ||x - c|| and ||x - c||^2
 //   host                      the L x L centroid step and scikit-learn's special cases.
 #include "gemm_wgmma.cuh"
-#include "ptx_sm90.cuh"
 #include "split_bf16.cuh"
+#include "tma_pipeline.cuh"
 
 #include <algorithm>
 #include <cmath>
@@ -39,15 +39,15 @@ namespace am {
 namespace cm {
 
 using namespace ptx;
+using pipe::kChunkK;
+using pipe::kThreads;
 
 constexpr int kTile = 128;   // rows of a CTA tile = columns of a column block
-constexpr int kChunkK = 64;
 constexpr int kStages = 3;
-constexpr int kThreads = 384;  // producer warpgroup + two consumer warpgroups
-constexpr int kConsumerThreads = 256;
 constexpr int kOpTile = kTile * kChunkK * 2;  // one bf16 128 x 64 operand tile: 16 KiB
 constexpr int kStageBytes = 4 * kOpTile;      // A_hi, A_lo, B_hi, B_lo
-constexpr size_t kSmem = 1024 + (size_t)kStages * kStageBytes + 2 * kStages * 8;
+using Ring = pipe::Ring<kStages>;
+constexpr size_t kSmem = Ring::smem_bytes(kStageBytes, kStages, 0);
 
 // one warp per row: Xp[i] = X[perm[i]]
 __global__ void __launch_bounds__(256)
@@ -79,9 +79,7 @@ template <bool kDiag>
 __global__ void __launch_bounds__(kThreads, 1)
 silhouette_tc_kernel(const __grid_constant__ CUtensorMap map_x, const SilArgs a) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kStages * kStageBytes);
-  uint64_t* empty_bar = full_bar + kStages;
+  Ring ring(smem_raw, kStageBytes, kStages, 0);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int num_kb = a.dp / kChunkK;
@@ -91,33 +89,20 @@ silhouette_tc_kernel(const __grid_constant__ CUtensorMap map_x, const SilArgs a)
 
   if (threadIdx.x == 0) {
     prefetch_tensormap(&map_x);
-    for (int i = 0; i < kStages; ++i) {
-      mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], kConsumerThreads);
-    }
-    fence_barrier_init();
-    fence_proxy_async();
+    ring.init();
   }
   __syncthreads();
 
   if (warp < 4) {
     regs_producer();
     if (warp == 0 && elect_one_sync()) {
-      int stage = 0;
-      uint32_t phase = 0;
       for (int b = b_begin; b < b_end; ++b) {
         for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          uint8_t* s = smem + stage * kStageBytes;
-          mbar_expect_tx(&full_bar[stage], (uint32_t)kStageBytes);
-          tma_load_2d(s, &map_x, &full_bar[stage], kb * kChunkK, tile * kTile);                             // A hi
-          tma_load_2d(s + kOpTile, &map_x, &full_bar[stage], a.dp + kb * kChunkK, tile * kTile);            // A lo
-          tma_load_2d(s + 2 * kOpTile, &map_x, &full_bar[stage], kb * kChunkK, b * kTile);                  // B hi
-          tma_load_2d(s + 3 * kOpTile, &map_x, &full_bar[stage], a.dp + kb * kChunkK, b * kTile);           // B lo
-          if (++stage == kStages) {
-            stage = 0;
-            phase ^= 1;
-          }
+          const Ring::Slot s = ring.acquire();
+          tma_load_2d(s.smem, &map_x, s.bar, kb * kChunkK, tile * kTile);                    // A hi
+          tma_load_2d(s.smem + kOpTile, &map_x, s.bar, a.dp + kb * kChunkK, tile * kTile);   // A lo
+          tma_load_2d(s.smem + 2 * kOpTile, &map_x, s.bar, kb * kChunkK, b * kTile);         // B hi
+          tma_load_2d(s.smem + 3 * kOpTile, &map_x, s.bar, a.dp + kb * kChunkK, b * kTile);  // B lo
         }
       }
     }
@@ -138,32 +123,12 @@ silhouette_tc_kernel(const __grid_constant__ CUtensorMap map_x, const SilArgs a)
   float acc[64];
 #pragma unroll
   for (int i = 0; i < 64; ++i) acc[i] = 0.f;
-  int stage = 0;
-  uint32_t phase = 0;
   for (int b = b_begin; b < b_end; ++b) {
     for (int kb = 0; kb < num_kb; ++kb) {
-      mbar_wait(&full_bar[stage], phase);
-      const uint32_t sa = smem_u32(smem + stage * kStageBytes);
+      const uint32_t s = ring.wait();
       const uint32_t rows = (uint32_t)(wg * 64 * 128);
-      const uint64_t d_ahi = make_smem_desc(sa + rows), d_alo = make_smem_desc(sa + kOpTile + rows);
-      const uint64_t d_bhi = make_smem_desc(sa + 2 * kOpTile), d_blo = make_smem_desc(sa + 3 * kOpTile);
-      wgmma_fence();
-#pragma unroll
-      for (int ks = 0; ks < kChunkK / 16; ++ks) {
-        const uint64_t o = (uint64_t)(ks * 2);  // 16 bf16 = 32 bytes along K inside the swizzle atom
-        Wgmma<128>::mma(acc, d_ahi + o, d_bhi + o, (kb | ks) ? 1u : 0u);
-        Wgmma<128>::mma(acc, d_alo + o, d_bhi + o, 1u);
-        Wgmma<128>::mma(acc, d_ahi + o, d_blo + o, 1u);
-        Wgmma<128>::mma(acc, d_alo + o, d_blo + o, 1u);
-      }
-      wgmma_commit();
-      wgmma_wait_all();
-      reg_fence(acc);
-      mbar_arrive(&empty_bar[stage]);
-      if (++stage == kStages) {
-        stage = 0;
-        phase ^= 1;
-      }
+      pipe::mma_chunk_split<128, true>(acc, s + rows, s + kOpTile + rows, s + 2 * kOpTile, s + 3 * kOpTile, kb);
+      ring.release();
     }
     const int64_t c0 = (int64_t)b * kTile;
     if constexpr (kDiag) {
@@ -398,11 +363,8 @@ extern "C" int am_cluster_scores(const float* X, int64_t N, int d, const int32_t
     AM_CUDA(cudaMemsetAsync(S.p, 0, (size_t)N * L * 8, st.s));
     AM_CUDA(cudaMemsetAsync(total.p, 0, 8, st.s));
     AM_LAUNCH(split_rows_kernel, row_grid, 256, 0, st.s, dXp.p, N, d, dp, Xs.p, nullptr);
-    alignas(64) unsigned char map_x[128];
-    const uint64_t dims[2] = {(uint64_t)(2 * dp), (uint64_t)N};
-    const uint64_t strides[1] = {(uint64_t)(2 * dp) * 2};
-    const uint32_t box[2] = {(uint32_t)kChunkK, (uint32_t)kTile};
-    AM_TRY(gemm::encode_map_bf16(map_x, Xs.p, 2, dims, strides, box));
+    CUtensorMap map;
+    AM_TRY(gemm::encode_map_bf16(&map, Xs.p, 2 * dp, N, 2 * dp, kTile));
     SilArgs a{};
     a.N = N;
     a.dp = dp;
@@ -417,13 +379,8 @@ extern "C" int am_cluster_scores(const float* X, int64_t N, int d, const int32_t
     a.seg = dSeg.p;
     a.off = dOff.p;
     a.S = S.p;
-    static bool attr_set = false;
-    if (!attr_set) {
-      AM_CUDA(cudaFuncSetAttribute(silhouette_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmem));
-      AM_CUDA(cudaFuncSetAttribute(silhouette_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmem));
-      attr_set = true;
-    }
-    const CUtensorMap& map = *reinterpret_cast<const CUtensorMap*>(map_x);
+    AM_TRY(allow_dynamic_smem<silhouette_tc_kernel<true>>(kSmem));
+    AM_TRY(allow_dynamic_smem<silhouette_tc_kernel<false>>(kSmem));
     AM_LAUNCH(silhouette_tc_kernel<true>, dim3((unsigned)tiles, 1u), kThreads, kSmem, st.s, map, a);
     AM_LAUNCH(silhouette_tc_kernel<false>, dim3((unsigned)tiles, (unsigned)splits), kThreads, kSmem, st.s, map, a);
     AM_LAUNCH(silhouette_finish_kernel, row_grid, 256, 0, st.s, S.p, N, L, dSeg.p, dOff.p, dPerm.p, dSamples.p,

@@ -63,6 +63,15 @@ int mel_plan_hop(const am_mel_plan* plan);  // mel.cu
 int sm_count();             // SMs of the active device
 int device_cc();            // major*10+minor
 
+// Lets kKernel launch with up to `bytes` of dynamic shared memory.  The attribute is set by the first call for each
+// kernel (the static's initialisation is thread safe, so concurrent first launches set it once and all wait for it);
+// every call passes that kernel's same constant limit.
+template <auto kKernel>
+int allow_dynamic_smem(size_t bytes) {
+  static const cudaError_t e = cudaFuncSetAttribute(kKernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+  return e == cudaSuccess ? AM_OK : cuda_fail(e, "cudaFuncSetAttribute(MaxDynamicSharedMemorySize)", __FILE__, __LINE__);
+}
+
 // ---------------------------------------------------------------- RAII device / pinned buffers
 template <typename T>
 struct DevBuf {

@@ -274,11 +274,7 @@ bool plan(const BlockDesc& d, Plan* out) {
 
 template <int S, bool kExpand>
 static int launch(const Args& a, int B, size_t smem, cudaStream_t st) {
-  static bool attr_set = false;
-  if (!attr_set) {
-    AM_CUDA(cudaFuncSetAttribute(fused_block_kernel<S, kExpand>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemMax));
-    attr_set = true;
-  }
+  AM_TRY((allow_dynamic_smem<fused_block_kernel<S, kExpand>>(kSmemMax)));
   const int64_t grid = (int64_t)B * a.tiles_y * a.tiles_x;
   AM_CHECK(grid < ((int64_t)1 << 31), "fused block: %lld tiles is too many for one launch", (long long)grid);
   AM_LAUNCH((fused_block_kernel<S, kExpand>), (unsigned)grid, kThreads, smem, st, a);

@@ -7,24 +7,25 @@
 //                 the swizzled tiles into fp32 register accumulators, then the epilogue from registers:
 //                 alpha / bias / ReLU6 / residual -> bf16 or fp32 (+ the k-NN chunk maxima); a bf16 tile goes through
 //                 shared memory so that global stores are whole 16-byte chunks of consecutive columns.
-// Two mbarrier arrays: full (TMA -> consumers, transaction counted) and empty (consumers -> TMA).  While the
-// consumers run an epilogue the producer is already filling the ring with the next tile's first K blocks.
+// The ring and its barriers are tma_pipeline.cuh's.  While the consumers run an epilogue the producer is already
+// filling the ring with the next tile's first K blocks.
 #include "gemm_wgmma.cuh"
-#include "ptx_sm90.cuh"
+#include "tma_pipeline.cuh"
 
 #include <mutex>
 
 namespace am {
 namespace gemm {
 
+using pipe::kChunkK;
+using pipe::kThreads;
+
 constexpr int kBlockM = 128;
-constexpr int kBlockK = 64;            // 64 bf16 = one 128-byte swizzle row
 constexpr int kStages = 4;             // at most; fewer when a wide B tile would not fit
-constexpr int kThreads = 384;
-constexpr int kConsumerThreads = 256;
-constexpr int kATileBytes = kBlockM * kBlockK * 2;  // 16 KiB
+constexpr int kATileBytes = kBlockM * kChunkK * 2;  // 16 KiB
 constexpr int kMaxBlockN = 256;
 constexpr size_t kSmemMax = 232448;    // 227 KiB: the opt-in limit of one block on sm_90
+using Ring = pipe::Ring<kStages>;
 
 using namespace ptx;
 
@@ -77,28 +78,17 @@ __global__ void __launch_bounds__(kThreads, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
                   const KernelArgs args) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  // 1024-byte alignment for SWIZZLE_128B tiles
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  constexpr int kBTileBytes = BN * kBlockK * 2;
-  constexpr int kStageBytes = kATileBytes + kBTileBytes;
-  const int n_stages = args.stages;
-  uint8_t* d_stage = smem + n_stages * kStageBytes;  // [2][64][stage_pitch] when args.staged
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(d_stage + (args.staged ? 2 * 64 * stage_pitch<BN>() : 0));
-  uint64_t* empty_bar = full_bar + kStages;
+  // after the ring: [2][64][stage_pitch] bf16 output tiles when args.staged
+  Ring ring(smem_raw, kATileBytes + BN * kChunkK * 2, args.stages, args.staged ? 2 * 64 * stage_pitch<BN>() : 0);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int num_tiles = args.tiles_m * args.tiles_n;
-  const int num_kb = (args.K + kBlockK - 1) / kBlockK;
+  const int num_kb = (args.K + kChunkK - 1) / kChunkK;
 
   if (threadIdx.x == 0) {
     prefetch_tensormap(&map_a);
     prefetch_tensormap(&map_b);
-    for (int i = 0; i < n_stages; ++i) {
-      mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], kConsumerThreads);
-    }
-    fence_barrier_init();
-    fence_proxy_async();
+    ring.init();
   }
   __syncthreads();
 
@@ -106,22 +96,13 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
     regs_producer();
     // ===================== TMA producer =====================
     if (warp == 0 && elect_one_sync()) {
-      int stage = 0;
-      uint32_t phase = 0;
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
         int m_blk, n_blk;
         tile_coords(args, tile, m_blk, n_blk);
         for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          uint8_t* sa = smem + stage * kStageBytes;
-          uint8_t* sb = sa + kATileBytes;
-          mbar_expect_tx(&full_bar[stage], (uint32_t)kStageBytes);
-          tma_load_2d(sa, &map_a, &full_bar[stage], kb * kBlockK, m_blk * kBlockM);
-          tma_load_2d(sb, &map_b, &full_bar[stage], kb * kBlockK, n_blk * BN);
-          if (++stage == n_stages) {
-            stage = 0;
-            phase ^= 1;
-          }
+          const Ring::Slot s = ring.acquire();
+          tma_load_2d(s.smem, &map_a, s.bar, kb * kChunkK, m_blk * kBlockM);
+          tma_load_2d(s.smem + kATileBytes, &map_b, s.bar, kb * kChunkK, n_blk * BN);
         }
       }
     }
@@ -136,29 +117,14 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
   float acc[BN / 2];
 #pragma unroll
   for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-  int stage = 0;
-  uint32_t phase = 0;
   for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
     int m_blk, n_blk;
     tile_coords(args, tile, m_blk, n_blk);
     for (int kb = 0; kb < num_kb; ++kb) {
-      mbar_wait(&full_bar[stage], phase);
-      const uint32_t sa = smem_u32(smem + stage * kStageBytes) + (uint32_t)(wg * 64 * 128);
-      const uint32_t sb = smem_u32(smem + stage * kStageBytes + kATileBytes);
-      const uint64_t da = make_smem_desc(sa), db = make_smem_desc(sb);
-      const int ksteps = min(kBlockK, args.K - kb * kBlockK + 15) / 16;  // skip all-zero K tails
-      wgmma_fence();
-#pragma unroll 1
-      for (int ks = 0; ks < ksteps; ++ks)
-        Wgmma<BN>::mma(acc, da + (uint64_t)(ks * 2), db + (uint64_t)(ks * 2), (kb | ks) ? 1u : 0u);
-      wgmma_commit();
-      wgmma_wait_all();
-      reg_fence(acc);
-      mbar_arrive(&empty_bar[stage]);  // this thread's MMAs have read the stage
-      if (++stage == n_stages) {
-        stage = 0;
-        phase ^= 1;
-      }
+      const uint32_t s = ring.wait();
+      const int ksteps = min(kChunkK, args.K - kb * kChunkK + 15) / 16;  // skip all-zero K tails
+      pipe::mma_chunk<BN>(acc, s + (uint32_t)(wg * 64 * 128), s + kATileBytes, ksteps, kb);
+      ring.release();
     }
     // ---- epilogue straight from the accumulator registers
     const int64_t n_base = (int64_t)n_blk * BN;
@@ -190,7 +156,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
       }
     }
     if (args.staged) {  // bf16: fragment -> shared tile -> 16-byte row chunks
-      uint8_t* stg = d_stage + wg * 64 * stage_pitch<BN>();
+      uint8_t* stg = ring.extra() + wg * 64 * stage_pitch<BN>();
       const int r_lo = (wt >> 5) * 16 + (lane >> 2);
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
@@ -317,7 +283,6 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t,
 
 static EncodeTiledFn g_encode = nullptr;
 static std::once_flag g_encode_once;
-static std::mutex g_attr_mu;
 
 static EncodeTiledFn get_encode() {
   std::call_once(g_encode_once, [] {
@@ -332,39 +297,19 @@ static EncodeTiledFn get_encode() {
 
 bool available() { return ensure_init() == AM_OK && device_cc() == 90 && get_encode() != nullptr; }
 
-static int make_map(CUtensorMap* map, const void* base, int64_t rows, int64_t ld_elems, int K, int box_rows) {
-  const cuuint64_t dims[2] = {(cuuint64_t)K, (cuuint64_t)rows};
-  const cuuint64_t strides[1] = {(cuuint64_t)ld_elems * 2};
-  const cuuint32_t box[2] = {(cuuint32_t)kBlockK, (cuuint32_t)box_rows};
-  const cuuint32_t estr[2] = {1, 1};
-  CUresult r = get_encode()(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box,
-                            estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                            CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    set_error("cuTensorMapEncodeTiled failed (%d) rows=%lld ld=%lld K=%d box_rows=%d", (int)r, (long long)rows,
-              (long long)ld_elems, K, box_rows);
-    return AM_ERR_CUDA;
-  }
-  return AM_OK;
-}
-
-// generic bf16 tiled tensor map (rank <= 4), SWIZZLE_128B, zero OOB fill (used by kmeans_tc.cu)
-int encode_map_bf16(void* map_out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
-                    const uint32_t* box) {
+int encode_map_bf16(void* map_out, const void* base, int64_t inner, int64_t rows, int64_t pitch_elems, int box_rows) {
   AM_CHECK(get_encode() != nullptr, "cuTensorMapEncodeTiled unavailable");
-  cuuint64_t d[4], st[3];
-  cuuint32_t b[4], es[4] = {1, 1, 1, 1};
-  for (int i = 0; i < rank; ++i) {
-    d[i] = dims[i];
-    b[i] = box[i];
-  }
-  for (int i = 0; i + 1 < rank; ++i) st[i] = strides_bytes[i];
-  CUresult r = get_encode()(reinterpret_cast<CUtensorMap*>(map_out), CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, rank,
-                            const_cast<void*>(base), d, st, b, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
+  const cuuint64_t dims[2] = {(cuuint64_t)inner, (cuuint64_t)rows};
+  const cuuint64_t strides[1] = {(cuuint64_t)pitch_elems * 2};
+  const cuuint32_t box[2] = {(cuuint32_t)kChunkK, (cuuint32_t)box_rows};
+  const cuuint32_t estr[2] = {1, 1};
+  CUresult r = get_encode()(reinterpret_cast<CUtensorMap*>(map_out), CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2,
+                            const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                             CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
-    set_error("cuTensorMapEncodeTiled(rank %d) failed (%d)", rank, (int)r);
+    set_error("cuTensorMapEncodeTiled failed (%d) inner=%lld rows=%lld pitch=%lld box_rows=%d", (int)r,
+              (long long)inner, (long long)rows, (long long)pitch_elems, box_rows);
     return AM_ERR_CUDA;
   }
   return AM_OK;
@@ -377,7 +322,7 @@ static bool gemm_has_n(int n) {
 }
 
 // the smallest instantiated tile width >= n (n <= kMaxBlockN)
-int tile_n_for(int n) {
+static int tile_n_for(int n) {
   for (int c = 16; c <= kMaxBlockN; c += 16)
     if (c >= n && gemm_has_n(c)) return c;
   return kMaxBlockN;
@@ -426,18 +371,11 @@ static KernelArgs make_args(int64_t M, int64_t N, int K, void* D, int64_t ldd, b
 
 template <int BN>
 static int launch_bn(const CUtensorMap& map_a, const CUtensorMap& map_b, KernelArgs& args, cudaStream_t st) {
-  static bool attr_set = false;
-  {
-    std::lock_guard<std::mutex> lk(g_attr_mu);
-    if (!attr_set) {
-      AM_CUDA(cudaFuncSetAttribute(gemm_wgmma_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemMax));
-      attr_set = true;
-    }
-  }
-  const size_t stage_bytes = (size_t)kATileBytes + (size_t)BN * kBlockK * 2;
-  const size_t tail = 1024 + 2 * kStages * sizeof(uint64_t) + (args.staged ? 2 * 64 * stage_pitch<BN>() : 0);
-  args.stages = (int)std::min<size_t>(kStages, (kSmemMax - tail) / stage_bytes);
-  const size_t smem = (size_t)args.stages * stage_bytes + tail;
+  AM_TRY(allow_dynamic_smem<gemm_wgmma_kernel<BN>>(kSmemMax));
+  const size_t stage_bytes = (size_t)kATileBytes + (size_t)BN * kChunkK * 2;
+  const size_t extra = args.staged ? 2 * 64 * stage_pitch<BN>() : 0;
+  args.stages = (int)std::min<size_t>(kStages, (kSmemMax - Ring::smem_bytes(0, 0, extra)) / stage_bytes);
+  const size_t smem = Ring::smem_bytes(stage_bytes, args.stages, extra);
   const int tiles = args.tiles_m * args.tiles_n;
   const int grid = std::max(1, std::min(tiles, sm_count()));
   AM_LAUNCH(gemm_wgmma_kernel<BN>, grid, kThreads, smem, st, map_a, map_b, args);
@@ -454,8 +392,8 @@ int gemm_bf16(const __nv_bfloat16* A, int64_t M, int64_t lda, const __nv_bfloat1
   AM_CHECK(available(), "gemm: wgmma path unavailable (needs sm_90 and cuTensorMapEncodeTiled)");
   KernelArgs args = make_args(M, N, K, D, ldd, d_is_f32, ep, m_fastest);
   CUtensorMap map_a, map_b;
-  AM_TRY(make_map(&map_a, A, M, lda, K, kBlockM));
-  AM_TRY(make_map(&map_b, B, N, ldb, K, args.block_n));
+  AM_TRY(encode_map_bf16(&map_a, A, K, M, lda, kBlockM));
+  AM_TRY(encode_map_bf16(&map_b, B, K, N, ldb, args.block_n));
   switch (args.block_n) {
     case 16: return launch_bn<16>(map_a, map_b, args, st);
     case 32: return launch_bn<32>(map_a, map_b, args, st);

@@ -31,9 +31,6 @@ struct Epilogue {
 // cuTensorMapEncodeTiled
 bool available();
 
-// the smallest tile width >= n (n <= 256) the wgmma kernels are instantiated for
-int tile_n_for(int n);
-
 // lda/ldb in elements, multiples of 8 (16-byte TMA row pitch).  ldd in elements of D.
 // m_fastest: enumerate tiles with the M index fastest (B tile shared by consecutive CTAs;
 // right when A is small, e.g. k-NN queries); otherwise N fastest (A tile shared).
@@ -41,9 +38,10 @@ int gemm_bf16(const __nv_bfloat16* A, int64_t M, int64_t lda, const __nv_bfloat1
               int64_t ldb, int K, void* D, int64_t ldd, bool d_is_f32, const Epilogue& ep,
               bool m_fastest, cudaStream_t st);
 
-// bf16 tiled tensor map, rank <= 4, SWIZZLE_128B, zero OOB fill.  map_out: 128-byte CUtensorMap.
-int encode_map_bf16(void* map_out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
-                    const uint32_t* box);
+// The TMA map of the wgmma kernels' K-major operands: a 2-D bf16 matrix of `rows` rows of `inner` elements,
+// `pitch_elems` apart (a multiple of 8), loaded in 64 x box_rows boxes with SWIZZLE_128B, zero fill outside.
+// map_out: 128-byte CUtensorMap.
+int encode_map_bf16(void* map_out, const void* base, int64_t inner, int64_t rows, int64_t pitch_elems, int box_rows);
 
 // reference implementation on CUDA cores (slow; used only by the on-device self test)
 int gemm_bf16_simt(const __nv_bfloat16* A, int64_t M, int64_t lda, const __nv_bfloat16* B, int64_t N,

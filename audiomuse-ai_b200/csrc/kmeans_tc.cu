@@ -31,8 +31,8 @@
 #include "kmeans_tc.cuh"
 
 #include "gemm_wgmma.cuh"
-#include "ptx_sm90.cuh"
 #include "split_bf16.cuh"
+#include "tma_pipeline.cuh"
 
 #include <algorithm>
 #include <cmath>
@@ -41,11 +41,10 @@ namespace am {
 namespace kmtc {
 
 using namespace ptx;
+using pipe::kChunkK;
+using pipe::kThreads;
 
 constexpr int kTileM = 128;
-constexpr int kChunkK = 64;
-constexpr int kThreads = 384;         // producer warpgroup (one TMA lane) + two consumer warpgroups
-constexpr int kConsumerThreads = 256;
 constexpr int kATile = kTileM * kChunkK * 2;  // 16 KiB
 constexpr int kSlabMax = 4096;                // most points one accumulate CTA sorts at a time
 
@@ -89,6 +88,11 @@ struct AssignArgs {
 };
 
 constexpr int kStages = 3;
+using Ring = pipe::Ring<kStages>;
+
+// per stage: A_hi, A_lo [128 x 64], then B [2 KP x 64] = centres hi rows, lo rows
+template <int KP>
+constexpr int stage_bytes() { return 2 * kATile + 2 * KP * kChunkK * 2; }
 
 // (best, index, runner-up) of two disjoint candidate sets; equal scores keep the lower centre index
 __device__ __forceinline__ void merge_best(float& best, int& best_j, float& second, float b2, int j2, float s2) {
@@ -105,12 +109,8 @@ template <int KP>
 __global__ void __launch_bounds__(kThreads, 1)
 assign_tc_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_c, const AssignArgs args) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  constexpr int b_bytes = 2 * KP * kChunkK * 2;  // hi rows then lo rows
-  constexpr int stage_bytes = 2 * kATile + b_bytes;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kStages * stage_bytes);
-  uint64_t* empty_bar = full_bar + kStages;
-  float* s_cn = reinterpret_cast<float*>(empty_bar + kStages);  // [KP]
+  Ring ring(smem_raw, stage_bytes<KP>(), kStages, KP * sizeof(float));
+  float* s_cn = reinterpret_cast<float*>(ring.extra());  // [KP]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int num_kb = args.dp / kChunkK;
@@ -118,12 +118,7 @@ assign_tc_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constan
   if (threadIdx.x == 0) {
     prefetch_tensormap(&map_x);
     prefetch_tensormap(&map_c);
-    for (int i = 0; i < kStages; ++i) {
-      mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], kConsumerThreads);
-    }
-    fence_barrier_init();
-    fence_proxy_async();
+    ring.init();
   }
   for (int i = threadIdx.x; i < KP; i += kThreads) s_cn[i] = args.cn[i];
   __syncthreads();
@@ -131,20 +126,12 @@ assign_tc_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constan
   if (warp < 4) {
     regs_producer();
     if (warp == 0 && elect_one_sync()) {
-      int stage = 0;
-      uint32_t phase = 0;
       for (int tile = blockIdx.x; tile < args.tiles; tile += gridDim.x) {
         for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          uint8_t* sa = smem + stage * stage_bytes;
-          mbar_expect_tx(&full_bar[stage], (uint32_t)stage_bytes);
-          tma_load_2d(sa, &map_x, &full_bar[stage], kb * kChunkK, tile * kTileM);                    // hi
-          tma_load_2d(sa + kATile, &map_x, &full_bar[stage], args.dp + kb * kChunkK, tile * kTileM);  // lo
-          tma_load_2d(sa + 2 * kATile, &map_c, &full_bar[stage], kb * kChunkK, 0);                    // centres hi | lo
-          if (++stage == kStages) {
-            stage = 0;
-            phase ^= 1;
-          }
+          const Ring::Slot s = ring.acquire();
+          tma_load_2d(s.smem, &map_x, s.bar, kb * kChunkK, tile * kTileM);                    // hi
+          tma_load_2d(s.smem + kATile, &map_x, s.bar, args.dp + kb * kChunkK, tile * kTileM);  // lo
+          tma_load_2d(s.smem + 2 * kATile, &map_c, s.bar, kb * kChunkK, 0);                    // centres hi | lo
         }
       }
     }
@@ -158,32 +145,13 @@ assign_tc_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constan
   float acc[KP / 2];
 #pragma unroll
   for (int i = 0; i < KP / 2; ++i) acc[i] = 0.f;
-  int stage = 0;
-  uint32_t phase = 0;
   for (int tile = blockIdx.x; tile < args.tiles; tile += gridDim.x) {
     for (int kb = 0; kb < num_kb; ++kb) {
-      mbar_wait(&full_bar[stage], phase);
-      const uint32_t sa = smem_u32(smem + stage * stage_bytes);
+      const uint32_t s = ring.wait();
       const uint32_t rows = (uint32_t)(wg * 64 * 128);
-      const uint64_t d_ahi = make_smem_desc(sa + rows), d_alo = make_smem_desc(sa + kATile + rows);
-      const uint64_t d_bhi = make_smem_desc(sa + 2 * kATile);
-      const uint64_t d_blo = make_smem_desc(sa + 2 * kATile + (uint32_t)KP * 128u);
-      wgmma_fence();
-#pragma unroll
-      for (int ks = 0; ks < kChunkK / 16; ++ks) {
-        const uint64_t o = (uint64_t)(ks * 2);  // 16 bf16 = 32 bytes along K inside the swizzle atom
-        Wgmma<KP>::mma(acc, d_ahi + o, d_bhi + o, (kb | ks) ? 1u : 0u);
-        Wgmma<KP>::mma(acc, d_alo + o, d_bhi + o, 1u);
-        Wgmma<KP>::mma(acc, d_ahi + o, d_blo + o, 1u);
-      }
-      wgmma_commit();
-      wgmma_wait_all();
-      reg_fence(acc);
-      mbar_arrive(&empty_bar[stage]);
-      if (++stage == kStages) {
-        stage = 0;
-        phase ^= 1;
-      }
+      pipe::mma_chunk_split<KP, false>(acc, s + rows, s + kATile + rows, s + 2 * kATile,
+                                       s + 2 * kATile + (uint32_t)KP * 128u, kb);
+      ring.release();
     }
     // ===================== fused argmin epilogue: a quad of threads = two points =====================
     const int64_t row0 = (int64_t)tile * kTileM + wg * 64 + ((threadIdx.x & 127) >> 5) * 16 + (lane >> 2);
@@ -441,18 +409,8 @@ int Plan::create(const float* X_dev, int64_t N_, int d_, int k_, cudaStream_t st
   AM_TRY(inertia64.alloc(1));
   const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((N + 7) / 8, (int64_t)sm_count() * 16));
   AM_LAUNCH(split_rows_kernel, grid, 256, 0, st, X, N, d, dp, Xs.p, xn.p);
-  {
-    const uint64_t dims[2] = {(uint64_t)(2 * dp), (uint64_t)N};
-    const uint64_t strides[1] = {(uint64_t)(2 * dp) * 2};
-    const uint32_t box[2] = {(uint32_t)kChunkK, (uint32_t)kTileM};
-    AM_TRY(gemm::encode_map_bf16(map_x, Xs.p, 2, dims, strides, box));
-  }
-  {
-    const uint64_t dims[2] = {(uint64_t)dp, (uint64_t)(2 * kp)};
-    const uint64_t strides[1] = {(uint64_t)dp * 2};
-    const uint32_t box[2] = {(uint32_t)kChunkK, (uint32_t)(2 * kp)};
-    AM_TRY(gemm::encode_map_bf16(map_c, Cs.p, 2, dims, strides, box));
-  }
+  AM_TRY(gemm::encode_map_bf16(map_x, Xs.p, 2 * dp, N, 2 * dp, kTileM));
+  AM_TRY(gemm::encode_map_bf16(map_c, Cs.p, dp, 2 * kp, dp, 2 * kp));
   return AM_OK;
 }
 
@@ -474,12 +432,8 @@ int Plan::launch_accumulate(float* sums, float* counts, double* inertia_dev, con
 
 template <int KP>
 static int launch_assign(const Plan& p, const AssignArgs& a, cudaStream_t st) {
-  const size_t smem = 1024 + kStages * (size_t)(2 * kATile + 2 * KP * kChunkK * 2) + 2 * kStages * 8 + (size_t)KP * 4;
-  static bool attr_set = false;
-  if (!attr_set) {
-    AM_CUDA(cudaFuncSetAttribute(assign_tc_kernel<KP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr_set = true;
-  }
+  const size_t smem = Ring::smem_bytes(stage_bytes<KP>(), kStages, KP * sizeof(float));
+  AM_TRY(allow_dynamic_smem<assign_tc_kernel<KP>>(smem));
   const int grid = std::min(a.tiles, sm_count());
   AM_LAUNCH(assign_tc_kernel<KP>, grid, kThreads, smem, st, *reinterpret_cast<const CUtensorMap*>(p.map_x),
             *reinterpret_cast<const CUtensorMap*>(p.map_c), a);

@@ -1,0 +1,128 @@
+// The warp-specialised TMA -> wgmma main loop shared by gemm_wgmma_kernel (gemm.cu), assign_tc_kernel (kmeans_tc.cu)
+// and silhouette_tc_kernel (cluster_metrics.cu).
+//
+// A CTA of three warpgroups: warpgroup 0 is the producer (one elected lane of warp 0 issues the TMA loads), warpgroups
+// 1 and 2 are consumers (64 rows of the 128-row tile each).  Operand tiles travel through a ring of shared-memory
+// stages guarded by two mbarrier arrays: `full` (TMA -> consumers, transaction counted) and `empty` (consumers ->
+// TMA, one arrival per consumer thread).  Every thread that takes part keeps its own stage / phase position.
+//
+// Dynamic shared memory: [alignment slack][stages x stage_bytes][extra_bytes of the kernel's own][full][empty].
+#pragma once
+
+#include "ptx_sm90.cuh"
+
+namespace am {
+namespace pipe {
+
+constexpr int kThreads = 384;          // producer warpgroup + two consumer warpgroups
+constexpr int kConsumerThreads = 256;
+constexpr int kChunkK = 64;            // K per stage: 64 bf16 = one 128-byte swizzle row
+
+// kMaxStages barrier pairs are reserved whatever the run-time stage count (the GEMM picks it per tile width).
+template <int kMaxStages>
+struct Ring {
+  // the dynamic shared memory a launch requests for this layout; 1024 bytes of slack for the SWIZZLE_128B alignment
+  __host__ __device__ static constexpr size_t smem_bytes(size_t stage_bytes, int stages, size_t extra_bytes) {
+    return 1024 + (size_t)stages * stage_bytes + extra_bytes + 2 * kMaxStages * sizeof(uint64_t);
+  }
+
+  uint8_t* base;  // stage i at base + i * stage_bytes, 1024-byte aligned
+  uint64_t* full;
+  uint64_t* empty;
+  uint32_t stage_bytes;
+  int stages;
+  int stage = 0;
+  uint32_t phase = 0;
+
+  __device__ __forceinline__ Ring(uint8_t* smem_raw, uint32_t stage_bytes_, int stages_, uint32_t extra_bytes)
+      : base(reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023)),
+        full(reinterpret_cast<uint64_t*>(base + stages_ * stage_bytes_ + extra_bytes)),
+        empty(full + kMaxStages),
+        stage_bytes(stage_bytes_),
+        stages(stages_) {}
+
+  // the kernel's own region after the ring
+  __device__ __forceinline__ uint8_t* extra() const { return base + stages * stage_bytes; }
+
+  // thread 0, before the CTA's first __syncthreads
+  __device__ __forceinline__ void init() const {
+    for (int i = 0; i < stages; ++i) {
+      ptx::mbar_init(&full[i], 1);
+      ptx::mbar_init(&empty[i], kConsumerThreads);
+    }
+    ptx::fence_barrier_init();
+    ptx::fence_proxy_async();
+  }
+
+  // producer: waits until the consumers have freed the next stage and arms its `full` barrier for a whole stage of
+  // TMA bytes; the caller issues the loads of the stage into `smem`, completing on `bar`
+  struct Slot {
+    uint8_t* smem;
+    uint64_t* bar;
+  };
+  __device__ __forceinline__ Slot acquire() {
+    ptx::mbar_wait(&empty[stage], phase ^ 1);
+    ptx::mbar_expect_tx(&full[stage], stage_bytes);
+    const Slot s{base + stage * stage_bytes, &full[stage]};
+    advance();
+    return s;
+  }
+
+  // consumer: waits until the next stage has landed and returns its shared-memory address ...
+  __device__ __forceinline__ uint32_t wait() const {
+    ptx::mbar_wait(&full[stage], phase);
+    return ptx::smem_u32(base + stage * stage_bytes);
+  }
+  // ... and hands it back to the producer once this thread's MMAs have read it
+  __device__ __forceinline__ void release() {
+    ptx::mbar_arrive(&empty[stage]);
+    advance();
+  }
+
+ private:
+  __device__ __forceinline__ void advance() {
+    if (++stage == stages) {
+      stage = 0;
+      phase ^= 1;
+    }
+  }
+};
+
+// D[64 x N] (+)= A[64 x 64] . B[N x 64]^T for one K chunk of K-major SWIZZLE_128B tiles at shared addresses a, b:
+// `ksteps` 16-wide steps (fewer than 4 skips an all-zero K tail); chunk kb == 0 overwrites D.  Returns with the MMAs
+// complete.
+template <int N>
+__device__ __forceinline__ void mma_chunk(float (&acc)[N / 2], uint32_t a, uint32_t b, int ksteps, int kb) {
+  const uint64_t da = ptx::make_smem_desc(a), db = ptx::make_smem_desc(b);
+  ptx::wgmma_fence();
+#pragma unroll 1
+  for (int ks = 0; ks < ksteps; ++ks)
+    ptx::Wgmma<N>::mma(acc, da + (uint64_t)(ks * 2), db + (uint64_t)(ks * 2), (kb | ks) ? 1u : 0u);
+  ptx::wgmma_commit();
+  ptx::wgmma_wait_all();
+  ptx::reg_fence(acc);
+}
+
+// The split-bf16 form, x = hi + lo: D (+)= A_hi.B_hi + A_lo.B_hi + A_hi.B_lo (+ A_lo.B_lo when kLoLo), in that order
+// per 16-wide K step, over a whole 64-wide chunk.
+template <int N, bool kLoLo>
+__device__ __forceinline__ void mma_chunk_split(float (&acc)[N / 2], uint32_t a_hi, uint32_t a_lo, uint32_t b_hi,
+                                                uint32_t b_lo, int kb) {
+  const uint64_t d_ahi = ptx::make_smem_desc(a_hi), d_alo = ptx::make_smem_desc(a_lo);
+  const uint64_t d_bhi = ptx::make_smem_desc(b_hi), d_blo = ptx::make_smem_desc(b_lo);
+  ptx::wgmma_fence();
+#pragma unroll
+  for (int ks = 0; ks < kChunkK / 16; ++ks) {
+    const uint64_t o = (uint64_t)(ks * 2);  // 16 bf16 = 32 bytes along K inside the swizzle atom
+    ptx::Wgmma<N>::mma(acc, d_ahi + o, d_bhi + o, (kb | ks) ? 1u : 0u);
+    ptx::Wgmma<N>::mma(acc, d_alo + o, d_bhi + o, 1u);
+    ptx::Wgmma<N>::mma(acc, d_ahi + o, d_blo + o, 1u);
+    if constexpr (kLoLo) ptx::Wgmma<N>::mma(acc, d_alo + o, d_blo + o, 1u);
+  }
+  ptx::wgmma_commit();
+  ptx::wgmma_wait_all();
+  ptx::reg_fence(acc);
+}
+
+}  // namespace pipe
+}  // namespace am

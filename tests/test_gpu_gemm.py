@@ -28,7 +28,7 @@ print("RESULT", st, d.value, lib.am_last_error().decode() if st else "")
 
 
 @pytest.mark.parametrize("M,N,K,flags", CASES)
-def test_tcgen05_gemm_matches_simt(M, N, K, flags):
+def test_wgmma_gemm_matches_simt(M, N, K, flags):
     import os
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     r = subprocess.run([sys.executable, "-c", SCRIPT % (root, M, N, K, flags)], capture_output=True, text=True,
