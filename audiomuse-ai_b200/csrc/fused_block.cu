@@ -1,21 +1,29 @@
 // Fused inverted-residual block on sm_90a: [1x1 expand + ReLU6] -> 3x3 depthwise + ReLU6 -> 1x1 project [+ residual]
 // in one kernel, so the expanded tensor (6x the block width) never goes to HBM.
 //
-// One warpgroup per 8 x 8 output tile of one window.  The input halo tile (10 x 10 pixels at stride 1, 17 x 17 at
-// stride 2) is loaded once into shared memory as K-major 128-byte-swizzled bf16 tiles.  The expansion channels are
-// then walked in chunks of 64:
-//   expansion   wgmma m64n64k16 over the halo rows, fp32 accumulators in registers -> + bias, ReLU6 -> bf16 halo tile
-//               E [halo pixels x 64] in shared memory (pixels outside the image are zero: the depthwise pads with 0);
-//   depthwise   3 x 3 taps from E in fp32 (a thread = 8 channels of one output pixel) + bias, ReLU6 -> bf16, written
-//               as the K-major swizzled A operand [64 pixels x 64 channels] of
-//   projection  wgmma m64n64k16 into up to four 64-column register accumulator blocks (Cout <= 256), accumulated
-//               over the chunks.
+// Persistent, warp-specialised CTA of three warpgroups (tma_pipeline.cuh), each CTA looping over 8 x 8 output tiles:
+//   warpgroup 0   TMA producer (one elected lane): per tile the input halo (10 x 10 pixels at stride 1, 17 x 17 at
+//                 stride 2) through a 4-D NHWC tensor map as K-major 128-byte-swizzled bf16 rows, zero filled outside
+//                 the image and past cin_p; per 64-channel chunk of the expansion, into a two-stage ring: the W1 and
+//                 W2 chunks (2-D maps, zero filled past cmid_p / cout_p), the depthwise weights and biases and the
+//                 expansion bias (bulk copies), or, without an expansion conv, the input's channel chunk itself.
+//                 The next tile's halo and first chunks load while the consumers finish the current tile.
+//   warpgroups 1, 2   consumers, sharing one tile; per chunk:
+//     expansion   wgmma m64n64k16 over the halo rows (m blocks split between the warpgroups), fp32 accumulators ->
+//                 + bias, ReLU6 -> bf16 halo tile E [halo pixels x 64] (pixels outside the image are zero: the
+//                 depthwise pads with 0, and relu6(bias) need not be);
+//     depthwise   3 x 3 taps from E in fp32 (a thread = 8 channels of one output pixel) + bias, ReLU6 -> bf16, written
+//                 as the K-major swizzled A operand [64 pixels x 64 channels] of
+//     projection  wgmma m64n64k16 into register accumulators, 64-column blocks split between the warpgroups (Cout <=
+//                 256), accumulated over the chunks in ascending order.
+//   Two named barriers per chunk order E and the A operand between the consumer warpgroups.
 // Epilogue: + bias (+ the block input for a residual block) -> bf16, straight from the registers.
-// Blocks without an expansion conv read E from the input directly.  Rounding follows the layer-by-layer path: the
-// expansion and the depthwise output are rounded to bf16, every sum is fp32.
+// Rounding follows the layer-by-layer path: the expansion and the depthwise output are rounded to bf16, every sum is
+// fp32.
 #include "fused_block.cuh"
 
-#include "ptx_sm90.cuh"
+#include "gemm_wgmma.cuh"
+#include "tma_pipeline.cuh"
 
 namespace am {
 namespace fused {
@@ -24,242 +32,297 @@ using namespace ptx;
 
 constexpr int kTile = 8;        // output tile edge: 64 pixels = one m64 projection
 constexpr int kChunk = 64;      // expansion channels per pass = one 128-byte swizzle row of projection K
-constexpr int kThreads = 128;   // one warpgroup
 constexpr int kMaxCout = 256;
+constexpr int kMaxStages = 2;
 constexpr size_t kSmemMax = 232448;
+constexpr uint32_t kConsumerBar = 1;  // named barrier of the two consumer warpgroups
+// per stage after W1 / W2: depthwise weights [9][64], depthwise bias [64], expansion bias [64], fp32
+constexpr uint32_t kDwBytes = (9 + 1 + 1) * kChunk * 4;
+using Ring = pipe::Ring<kMaxStages>;
 
-template <int S>
-constexpr int halo() { return (kTile - 1) * S + 3; }
-template <int S>
-constexpr int halo_rows() { return (halo<S>() * halo<S>() + 63) / 64 * 64; }
+__host__ __device__ constexpr int halo(int S) { return (kTile - 1) * S + 3; }
+__host__ __device__ constexpr int halo_px(int S) { return halo(S) * halo(S); }
+__host__ __device__ constexpr int halo_rows(int S) { return (halo_px(S) + 63) / 64 * 64; }
+
+constexpr uint32_t round1k(uint32_t v) { return (v + 1023u) & ~1023u; }
 
 // byte offset of (row, 16-byte chunk) in a K-major SWIZZLE_128B tile (rows of 64 bf16, 8-row atoms of 1024 bytes)
 __device__ __forceinline__ uint32_t sw128(uint32_t row, uint32_t chunk) {
   return (row << 7) + (((chunk ^ row) & 7u) << 4);
 }
 
-struct Args {
-  const __nv_bfloat16* X;   // [B, H, W, cin_p]
-  const __nv_bfloat16* W1;  // [cmid_p, cin_p] (has_expand)
-  const float* b1;          // [cmid_p]
-  const float* wd;          // [9, cmid_p]
-  const float* bd;          // [cmid_p]
-  const __nv_bfloat16* W2;  // [cout_p, cmid_p]
-  const float* b2;          // [cout_p]
-  __nv_bfloat16* Y;         // [B, Ho, Wo, cout_p]
-  int H, W, Ho, Wo, tiles_y, tiles_x;
-  int cin_p, cmid_p, cout_p, residual;
+// Shared memory: the ring of per-chunk stages, then the kernel's own region (offsets from its start).
+//   stage (expand):     [W1 chunk: kbx x 64 rows x 128 B][W2 chunk: n2 rows x 128 B][depthwise params]
+//   stage (no expand):  [input chunk: halo pixels x 128 B][W2 chunk][depthwise params]
+//   own region:         [input halo: kbx x HR rows x 128 B][projection A: 64 x 128 B][E: halo pixels x 128 B][2 barriers]
+struct Layout {
+  uint32_t stage, w2, dw;     // stage bytes, offsets of W2 and the depthwise params inside a stage
+  uint32_t xs, a2, e, bars, extra;
+  int stages;
+  size_t smem;
 };
 
-struct Layout {  // shared-memory carve-up (byte offsets from the 1024-aligned base)
-  uint32_t xs, w1s, w2s, a2, e, total;
-};
-
-__host__ __device__ inline Layout layout(int S, bool has_expand, int cin_p, int cout_p) {
-  const uint32_t hr = (uint32_t)(((S == 1 ? 10 * 10 : 17 * 17) + 63) / 64 * 64);
+static Layout layout(int S, bool has_expand, int cin_p, int cout_p, int stages) {
+  const uint32_t hr = (uint32_t)halo_rows(S), hpx = (uint32_t)halo_px(S);
   const uint32_t kbx = has_expand ? (uint32_t)((cin_p + 63) / 64) : 0u;
   const uint32_t n2 = (uint32_t)((cout_p + 63) / 64 * 64);
   Layout l;
+  l.w2 = has_expand ? kbx * kChunk * 128 : round1k(hpx * 128);
+  l.dw = l.w2 + n2 * 128;
+  l.stage = round1k(l.dw + kDwBytes);
   l.xs = 0;
-  l.w1s = l.xs + kbx * hr * 128;
-  l.w2s = l.w1s + kbx * kChunk * 128;
-  l.a2 = l.w2s + n2 * 128;
-  l.e = l.a2 + 64 * 128;
-  l.total = l.e + hr * 128;
+  l.a2 = l.xs + kbx * hr * 128;
+  l.e = l.a2 + kTile * kTile * 128;
+  l.bars = l.e + (has_expand ? hpx * 128 : 0u);
+  l.extra = l.bars + 2 * sizeof(uint64_t);
+  l.stages = stages;
+  l.smem = Ring::smem_bytes(l.stage, stages, l.extra);
   return l;
 }
 
-template <int S, bool kExpand>
-__global__ void __launch_bounds__(kThreads)
-fused_block_kernel(const Args a) {
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  constexpr int HALO = halo<S>(), HPX = HALO * HALO, HR = halo_rows<S>();
-  const Layout L = layout(S, kExpand, a.cin_p, a.cout_p);
-  uint8_t* xs = smem + L.xs;
-  uint8_t* w1s = smem + L.w1s;
-  uint8_t* w2s = smem + L.w2s;
-  uint8_t* a2 = smem + L.a2;
-  __nv_bfloat16* e = reinterpret_cast<__nv_bfloat16*>(smem + L.e);  // [HR][64], plain rows of 128 bytes
+struct Args {
+  const __nv_bfloat16* X;   // [B, H, W, cin_p] (the residual)
+  const float* wd;          // [9, cmid_p]
+  const float* bd;          // [cmid_p]
+  const float* b1;          // [cmid_p] (has_expand)
+  const float* b2;          // [cout_p]
+  __nv_bfloat16* Y;         // [B, Ho, Wo, cout_p]
+  int H, W, Ho, Wo, tiles_y, tiles_x, num_tiles;
+  int cin_p, cmid_p, cout_p, residual;
+  Layout l;
+};
 
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, quad = lane & 3;
+template <int S, bool kExpand>
+__global__ void __launch_bounds__(pipe::kThreads, 1)
+fused_block_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_w1,
+                   const __grid_constant__ CUtensorMap map_w2, const Args a) {
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  constexpr int HALO = halo(S), HPX = halo_px(S), HR = halo_rows(S);
+  Ring ring(smem_raw, a.l.stage, a.l.stages, a.l.extra);
+  uint8_t* own = ring.extra();
+  uint8_t* xs = own + a.l.xs;
+  uint8_t* a2 = own + a.l.a2;
+  uint64_t* xs_full = reinterpret_cast<uint64_t*>(own + a.l.bars);  // halo landed (TMA -> consumers)
+  uint64_t* xs_empty = xs_full + 1;                                 // last expansion of the tile done (consumers -> TMA)
+
   const int per_img = a.tiles_y * a.tiles_x;
-  const int b = blockIdx.x / per_img;
-  const int ty = (blockIdx.x % per_img) / a.tiles_x, tx = blockIdx.x % a.tiles_x;
-  const int oy0 = ty * kTile, ox0 = tx * kTile;
-  const int gy0 = oy0 * S - 1, gx0 = ox0 * S - 1;  // image position of halo pixel (0, 0)
-  const __nv_bfloat16* Xb = a.X + (int64_t)b * a.H * a.W * a.cin_p;
-  auto in_image = [&](int hp, int& gy, int& gx) {
-    gy = gy0 + hp / HALO;
-    gx = gx0 + hp % HALO;
-    return hp < HPX && gy >= 0 && gy < a.H && gx >= 0 && gx < a.W;
-  };
+  const int kbx = (a.cin_p + 63) / 64;
+  const int n2_blocks = (a.cout_p + 63) / 64;
+
+  if (threadIdx.x == 0) {
+    prefetch_tensormap(&map_x);
+    if (kExpand) prefetch_tensormap(&map_w1);
+    prefetch_tensormap(&map_w2);
+    mbar_init(xs_full, 1);
+    mbar_init(xs_empty, pipe::kConsumerThreads);
+    ring.init();  // fences the barrier initialisations above too
+  }
+  __syncthreads();
+
+  if (threadIdx.x < 128) {
+    regs_producer();
+    // ===================== TMA producer =====================
+    if (threadIdx.x < 32 && elect_one_sync()) {
+      uint32_t xs_phase = 0;
+      for (int tile = blockIdx.x; tile < a.num_tiles; tile += gridDim.x) {
+        const int b = tile / per_img, ty = (tile % per_img) / a.tiles_x, tx = tile % a.tiles_x;
+        const int gy0 = ty * kTile * S - 1, gx0 = tx * kTile * S - 1;  // image position of halo pixel (0, 0)
+        if (kExpand) {
+          mbar_wait(xs_empty, xs_phase ^ 1);
+          mbar_expect_tx(xs_full, (uint32_t)(kbx * HPX * 128));
+          for (int kb = 0; kb < kbx; ++kb) tma_load_4d(xs + kb * HR * 128, &map_x, xs_full, kb * 64, gx0, gy0, b);
+          xs_phase ^= 1;
+        }
+        for (int c0 = 0; c0 < a.cmid_p; c0 += kChunk) {
+          const uint32_t nb = (uint32_t)min(kChunk, a.cmid_p - c0) * 4;  // bytes of one row of depthwise params
+          const uint32_t tx_bytes = (kExpand ? (uint32_t)kbx * kChunk * 128 : (uint32_t)HPX * 128) +
+                                    (uint32_t)n2_blocks * 64 * 128 + (kExpand ? 11u : 10u) * nb;
+          const Ring::Slot s = ring.acquire(tx_bytes);
+          if (kExpand) {
+            for (int kb = 0; kb < kbx; ++kb) tma_load_2d(s.smem + kb * kChunk * 128, &map_w1, s.bar, kb * 64, c0);
+          } else {
+            tma_load_4d(s.smem, &map_x, s.bar, c0, gx0, gy0, b);
+          }
+          tma_load_2d(s.smem + a.l.w2, &map_w2, s.bar, c0, 0);
+          float* dw = reinterpret_cast<float*>(s.smem + a.l.dw);
+          for (int t = 0; t < 9; ++t) bulk_load(dw + t * kChunk, a.wd + (int64_t)t * a.cmid_p + c0, nb, s.bar);
+          bulk_load(dw + 9 * kChunk, a.bd + c0, nb, s.bar);
+          if (kExpand) bulk_load(dw + 10 * kChunk, a.b1 + c0, nb, s.bar);
+        }
+      }
+    }
+    return;
+  }
+  regs_consumer();
+  // ===================== consumers: warpgroups 1 and 2 =====================
+  const int ct = threadIdx.x - 128;          // 0 .. 255
+  // warp-uniform by construction (a shuffle result), so branches on it keep the wgmmas on a converged path
+  const int wg = __shfl_sync(0xffffffffu, ct >> 7, 0), wt = ct & 127;
+  const int warp = wt >> 5, lane = wt & 31, quad = lane & 3;
+  __nv_bfloat16* e_own = reinterpret_cast<__nv_bfloat16*>(own + a.l.e);  // [HPX][64], plain rows of 128 bytes
   const uint4 zero4 = make_uint4(0u, 0u, 0u, 0u);
 
-  const int kbx = (a.cin_p + 63) / 64;
-  if (kExpand) {  // input halo tile, once: [kbx][HR rows][64 channels]
-    for (int it = tid; it < kbx * HR * 8; it += kThreads) {
-      const int c = it & 7, p = (it >> 3) % HR, kb = (it >> 3) / HR;
-      const int ch = kb * 64 + c * 8;
-      int gy, gx;
-      uint4 v = zero4;
-      if (ch < a.cin_p && in_image(p, gy, gx)) v = *reinterpret_cast<const uint4*>(Xb + ((int64_t)gy * a.W + gx) * a.cin_p + ch);
-      *reinterpret_cast<uint4*>(xs + kb * HR * 128 + sw128(p, c)) = v;
-    }
-  }
-
-  const int n2_blocks = (a.cout_p + 63) / 64;
-  float acc2[4][32];
+  // the first MMA of every expansion m block and of every tile's projection overwrites (scale_d = 0)
+  float acc1[32];     // expansion
+  float acc2[2][32];  // projection column blocks nb = wg and wg + 2
 #pragma unroll
-  for (int nb = 0; nb < 4; ++nb)
+  for (int i = 0; i < 32; ++i) acc1[i] = 0.f;
 #pragma unroll
-    for (int i = 0; i < 32; ++i) acc2[nb][i] = 0.f;
+  for (int j = 0; j < 2; ++j)
+#pragma unroll
+    for (int i = 0; i < 32; ++i) acc2[j][i] = 0.f;
 
-  for (int c0 = 0; c0 < a.cmid_p; c0 += kChunk) {
-    const int nch = min(kChunk, a.cmid_p - c0);
-    __syncthreads();  // the previous chunk's readers of w1s / w2s / E / A2 are done
+  uint32_t xs_phase = 0;
+  for (int tile = blockIdx.x; tile < a.num_tiles; tile += gridDim.x) {
+    const int b = tile / per_img, ty = (tile % per_img) / a.tiles_x, tx = tile % a.tiles_x;
+    const int oy0 = ty * kTile, ox0 = tx * kTile;
+    const int gy0 = oy0 * S - 1, gx0 = ox0 * S - 1;
     if (kExpand) {
-      for (int it = tid; it < kbx * kChunk * 8; it += kThreads) {
-        const int c = it & 7, r = (it >> 3) % kChunk, kb = (it >> 3) / kChunk;
-        const int ch = kb * 64 + c * 8;
-        uint4 v = zero4;
-        if (r < nch && ch < a.cin_p) v = *reinterpret_cast<const uint4*>(a.W1 + (int64_t)(c0 + r) * a.cin_p + ch);
-        *reinterpret_cast<uint4*>(w1s + kb * kChunk * 128 + sw128(r, c)) = v;
-      }
-    } else {  // no expansion: E is the input's channel chunk
-      for (int it = tid; it < HR * 8; it += kThreads) {
-        const int c = it & 7, p = it >> 3;
-        int gy, gx;
-        uint4 v = zero4;
-        if (c * 8 < nch && in_image(p, gy, gx))
-          v = *reinterpret_cast<const uint4*>(Xb + ((int64_t)gy * a.W + gx) * a.cin_p + c0 + c * 8);
-        *reinterpret_cast<uint4*>(e + p * 64 + c * 8) = v;
-      }
+      mbar_wait(xs_full, xs_phase);
+      xs_phase ^= 1;
     }
-    for (int it = tid; it < n2_blocks * 64 * 8; it += kThreads) {
-      const int c = it & 7, r = it >> 3;
-      uint4 v = zero4;
-      if (r < a.cout_p && c * 8 < nch) v = *reinterpret_cast<const uint4*>(a.W2 + (int64_t)r * a.cmid_p + c0 + c * 8);
-      *reinterpret_cast<uint4*>(w2s + sw128(r, c)) = v;
-    }
-    fence_proxy_async();  // generic-proxy writes -> visible to the wgmma (async proxy) reads
-    __syncthreads();
 
-    if (kExpand) {
-      for (int m = 0; m < HR / 64; ++m) {
-        float acc1[32];
-#pragma unroll
-        for (int i = 0; i < 32; ++i) acc1[i] = 0.f;
-        wgmma_fence();
-        for (int kb = 0; kb < kbx; ++kb) {
-          const uint64_t da = make_smem_desc(smem_u32(xs + kb * HR * 128 + m * 64 * 128));
-          const uint64_t db = make_smem_desc(smem_u32(w1s + kb * kChunk * 128));
-          const int ksteps = min(4, (a.cin_p - kb * 64) / 16);
-          for (int ks = 0; ks < ksteps; ++ks)
-            Wgmma<64>::mma(acc1, da + (uint64_t)(ks * 2), db + (uint64_t)(ks * 2), (kb | ks) ? 1u : 0u);
-        }
-        wgmma_commit();
-        wgmma_wait_all();
-        reg_fence(acc1);
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int p = m * 64 + warp * 16 + (lane >> 2) + 8 * h;
-          int gy, gx;
-          const bool inside = in_image(p, gy, gx);
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const int col = 8 * j + 2 * quad;
-            float f0 = 0.f, f1 = 0.f;
-            if (inside && col < nch) {
-              f0 = relu6f(acc1[4 * j + 2 * h] + __ldg(&a.b1[c0 + col]));
-              f1 = relu6f(acc1[4 * j + 2 * h + 1] + __ldg(&a.b1[c0 + col + 1]));
-            }
-            *reinterpret_cast<__nv_bfloat162*>(e + p * 64 + col) = __floats2bfloat162_rn(f0, f1);
+    for (int c0 = 0; c0 < a.cmid_p; c0 += kChunk) {
+      const int nch = min(kChunk, a.cmid_p - c0);
+      uint8_t* sp = ring.wait_ptr();
+      const uint32_t st = smem_u32(sp);
+      const float* dwp = reinterpret_cast<const float*>(sp + a.l.dw);
+      const __nv_bfloat16* e = kExpand ? e_own : reinterpret_cast<const __nv_bfloat16*>(sp);
+
+      if (kExpand) {
+        for (int m = wg; m < HR / 64; m += 2) {
+          wgmma_fence();
+          for (int kb = 0; kb < kbx; ++kb) {
+            const uint64_t da = make_smem_desc(smem_u32(xs + kb * HR * 128 + m * 64 * 128));
+            const uint64_t db = make_smem_desc(st + (uint32_t)(kb * kChunk * 128));
+            const int ksteps = min(4, (a.cin_p - kb * 64) / 16);
+            for (int ks = 0; ks < ksteps; ++ks)
+              Wgmma<64>::mma(acc1, da + (uint64_t)(ks * 2), db + (uint64_t)(ks * 2), (kb | ks) ? 1u : 0u);
           }
-        }
-      }
-      __syncthreads();
-    } else {
-      __syncthreads();
-    }
-
-    // depthwise: item = 8 channels of one output pixel
-    for (int it = tid; it < 64 * 8; it += kThreads) {
-      const int g = it & 7, px = it >> 3;
-      const int oy = px >> 3, ox = px & 7;
-      uint4 out = zero4;
-      if (g * 8 < nch) {
-        const int cg = c0 + g * 8;
-        float acc[8];
+          wgmma_commit();
+          wgmma_wait_all();
+          reg_fence(acc1);
 #pragma unroll
-        for (int q = 0; q < 8; ++q) acc[q] = __ldg(&a.bd[cg + q]);
+          for (int h = 0; h < 2; ++h) {
+            const int p = m * 64 + warp * 16 + (lane >> 2) + 8 * h;
+            if (p >= HPX) continue;
+            const int gy = gy0 + p / HALO, gx = gx0 + p % HALO;
+            const bool inside = gy >= 0 && gy < a.H && gx >= 0 && gx < a.W;
 #pragma unroll
-        for (int dy = 0; dy < 3; ++dy)
-#pragma unroll
-          for (int dx = 0; dx < 3; ++dx) {
-            const int hp = (oy * S + dy) * HALO + ox * S + dx;
-            const uint4 v = *reinterpret_cast<const uint4*>(e + hp * 64 + g * 8);
-            const __nv_bfloat162* v2 = reinterpret_cast<const __nv_bfloat162*>(&v);
-            const float* w = a.wd + (dy * 3 + dx) * a.cmid_p + cg;
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {
-              const float2 f = __bfloat1622float2(v2[q]);
-              acc[2 * q] = fmaf(f.x, __ldg(&w[2 * q]), acc[2 * q]);
-              acc[2 * q + 1] = fmaf(f.y, __ldg(&w[2 * q + 1]), acc[2 * q + 1]);
+            for (int j = 0; j < 8; ++j) {
+              const int col = 8 * j + 2 * quad;
+              float f0 = 0.f, f1 = 0.f;
+              if (inside && col < nch) {
+                f0 = relu6f(acc1[4 * j + 2 * h] + dwp[10 * kChunk + col]);
+                f1 = relu6f(acc1[4 * j + 2 * h + 1] + dwp[10 * kChunk + col + 1]);
+              }
+              *reinterpret_cast<__nv_bfloat162*>(e_own + p * 64 + col) = __floats2bfloat162_rn(f0, f1);
             }
           }
+        }
+        if (c0 + kChunk >= a.cmid_p) mbar_arrive(xs_empty);  // this thread's reads of the halo are complete
+      }
+      // E is complete, and both warpgroups' previous projection has finished reading A
+      named_bar_sync(kConsumerBar, pipe::kConsumerThreads);
+
+      // depthwise: item = 8 channels of one output pixel
+      for (int it = ct; it < 64 * 8; it += pipe::kConsumerThreads) {
+        const int g = it & 7, px = it >> 3;
+        const int oy = px >> 3, ox = px & 7;
+        uint4 out = zero4;
+        if (g * 8 < nch) {
+          const float* bias = dwp + 9 * kChunk + g * 8;
+          float acc[8];
+#pragma unroll
+          for (int q = 0; q < 8; ++q) acc[q] = bias[q];
+#pragma unroll
+          for (int dy = 0; dy < 3; ++dy)
+#pragma unroll
+            for (int dx = 0; dx < 3; ++dx) {
+              const int hp = (oy * S + dy) * HALO + ox * S + dx;
+              const uint4 v = *reinterpret_cast<const uint4*>(e + hp * 64 + g * 8);
+              const __nv_bfloat162* v2 = reinterpret_cast<const __nv_bfloat162*>(&v);
+              const float4* w4 = reinterpret_cast<const float4*>(dwp + (dy * 3 + dx) * kChunk + g * 8);
+              const float4 wa = w4[0], wb = w4[1];
+              const float w[8] = {wa.x, wa.y, wa.z, wa.w, wb.x, wb.y, wb.z, wb.w};
+#pragma unroll
+              for (int q = 0; q < 4; ++q) {
+                const float2 f = __bfloat1622float2(v2[q]);
+                acc[2 * q] = fmaf(f.x, w[2 * q], acc[2 * q]);
+                acc[2 * q + 1] = fmaf(f.y, w[2 * q + 1], acc[2 * q + 1]);
+              }
+            }
         __nv_bfloat162 o2[4];
 #pragma unroll
-        for (int q = 0; q < 4; ++q) o2[q] = __floats2bfloat162_rn(relu6f(acc[2 * q]), relu6f(acc[2 * q + 1]));
-        out = *reinterpret_cast<const uint4*>(o2);
-      }
-      *reinterpret_cast<uint4*>(a2 + sw128(px, g)) = out;
-    }
-    fence_proxy_async();
-    __syncthreads();
-
-    // projection: acc2 += A2 [64 x nch] . W2_chunk [Cout x nch]^T
-    wgmma_fence();
-    const uint64_t da = make_smem_desc(smem_u32(a2));
-#pragma unroll
-    for (int nb = 0; nb < 4; ++nb) {
-      if (nb < n2_blocks) {
-        const uint64_t db = make_smem_desc(smem_u32(w2s + nb * 64 * 128));
-        for (int ks = 0; ks < nch / 16; ++ks)
-          Wgmma<64>::mma(acc2[nb], da + (uint64_t)(ks * 2), db + (uint64_t)(ks * 2), (c0 | ks) ? 1u : 0u);
-      }
-    }
-    wgmma_commit();
-    wgmma_wait_all();
-#pragma unroll
-    for (int nb = 0; nb < 4; ++nb) reg_fence(acc2[nb]);
-  }
-
-  // epilogue: + bias (+ block input) -> bf16
-#pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    const int px = warp * 16 + (lane >> 2) + 8 * h;
-    const int oy = oy0 + (px >> 3), ox = ox0 + (px & 7);
-    if (oy >= a.Ho || ox >= a.Wo) continue;
-    const int64_t pix = ((int64_t)b * a.Ho + oy) * a.Wo + ox;
-#pragma unroll
-    for (int nb = 0; nb < 4; ++nb) {
-      if (nb >= n2_blocks) continue;
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const int n = nb * 64 + 8 * j + 2 * quad;
-        if (n >= a.cout_p) continue;
-        float f0 = acc2[nb][4 * j + 2 * h] + __ldg(&a.b2[n]);
-        float f1 = acc2[nb][4 * j + 2 * h + 1] + __ldg(&a.b2[n + 1]);
-        if (a.residual) {  // stride 1, cin_p == cout_p: the block input at the same pixel
-          const float2 r = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(a.X + pix * a.cin_p + n));
-          f0 += r.x;
-          f1 += r.y;
+          for (int q = 0; q < 4; ++q) o2[q] = __floats2bfloat162_rn(relu6f(acc[2 * q]), relu6f(acc[2 * q + 1]));
+          out = *reinterpret_cast<const uint4*>(o2);
         }
-        *reinterpret_cast<__nv_bfloat162*>(a.Y + pix * a.cout_p + n) = __floats2bfloat162_rn(f0, f1);
+        *reinterpret_cast<uint4*>(a2 + sw128(px, g)) = out;
+      }
+      fence_proxy_async();  // generic-proxy writes of A -> visible to the wgmma (async proxy) reads
+      // A is complete, and both warpgroups are done reading E
+      named_bar_sync(kConsumerBar, pipe::kConsumerThreads);
+
+      // projection: acc2 += A2 [64 x nch] . W2_chunk [Cout x nch]^T
+      wgmma_fence();
+      const uint64_t da = make_smem_desc(smem_u32(a2));
+#pragma unroll
+      for (int j = 0; j < 2; ++j) {
+        const int nb = wg + 2 * j;
+        if (nb < n2_blocks) {
+          const uint64_t db = make_smem_desc(st + a.l.w2 + (uint32_t)(nb * 64 * 128));
+          for (int ks = 0; ks < nch / 16; ++ks)
+            Wgmma<64>::mma(acc2[j], da + (uint64_t)(ks * 2), db + (uint64_t)(ks * 2), (c0 | ks) ? 1u : 0u);
+        }
+      }
+      wgmma_commit();
+      wgmma_wait_all();
+#pragma unroll
+      for (int j = 0; j < 2; ++j) reg_fence(acc2[j]);
+      ring.release();
+    }
+
+    // epilogue: + bias (+ block input) -> bf16
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int px = warp * 16 + (lane >> 2) + 8 * h;
+      const int oy = oy0 + (px >> 3), ox = ox0 + (px & 7);
+      if (oy >= a.Ho || ox >= a.Wo) continue;
+      const int64_t pix = ((int64_t)b * a.Ho + oy) * a.Wo + ox;
+#pragma unroll
+      for (int jb = 0; jb < 2; ++jb) {
+        const int nb = wg + 2 * jb;
+        if (nb >= n2_blocks) continue;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const int n = nb * 64 + 8 * j + 2 * quad;
+          if (n >= a.cout_p) continue;
+          float f0 = acc2[jb][4 * j + 2 * h] + __ldg(&a.b2[n]);
+          float f1 = acc2[jb][4 * j + 2 * h + 1] + __ldg(&a.b2[n + 1]);
+          if (a.residual) {  // stride 1, cin_p == cout_p: the block input at the same pixel
+            const float2 r = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(a.X + pix * a.cin_p + n));
+            f0 += r.x;
+            f1 += r.y;
+          }
+          *reinterpret_cast<__nv_bfloat162*>(a.Y + pix * a.cout_p + n) = __floats2bfloat162_rn(f0, f1);
+        }
       }
     }
   }
+}
+
+// The shapes the fused path takes: those whose single-buffered tile working set (input halo, one W1 and W2 chunk,
+// the projection A operand and E, all at whole 64-row granularity) fits in shared memory.  This is the rule of the
+// earlier single-warpgroup kernel, kept so that exactly the same blocks fuse (the rest run layer by layer) rather
+// than the set drifting with this kernel's layout.  Every such shape fits that layout with at least one stage: a
+// one-stage layout is never larger for blocks with an expansion (E holds only the halo pixels, not 64-row blocks), and
+// at most 48 bytes larger for the no-expansion blocks, whose working set is far below the limit.
+static bool fits(const BlockDesc& d) {
+  const size_t hr = (size_t)halo_rows(d.stride);
+  const size_t kbx = d.has_expand ? (size_t)((d.cin_p + 63) / 64) : 0;
+  const size_t n2 = (size_t)((d.cout_p + 63) / 64 * 64);
+  const size_t set = kbx * hr * 128 + kbx * kChunk * 128 + n2 * 128 + 64 * 128 + hr * 128;
+  return set + 1024 <= kSmemMax;
 }
 
 bool plan(const BlockDesc& d, Plan* out) {
@@ -267,17 +330,20 @@ bool plan(const BlockDesc& d, Plan* out) {
   if (d.cout_p > kMaxCout || d.cout_p % 16 || d.cmid_p % 16 || d.cin_p % 16) return false;
   if (!d.has_expand && d.cin_p != d.cmid_p) return false;
   if (d.residual && (d.stride != 1 || d.cin_p != d.cout_p)) return false;
-  const Layout l = layout(d.stride, d.has_expand != 0, d.cin_p, d.cout_p);
-  out->smem_bytes = (size_t)l.total + 1024;
+  if (!fits(d)) return false;
+  Layout l = layout(d.stride, d.has_expand != 0, d.cin_p, d.cout_p, kMaxStages);
+  if (l.smem > kSmemMax) l = layout(d.stride, d.has_expand != 0, d.cin_p, d.cout_p, 1);
+  out->stages = l.stages;
+  out->smem_bytes = l.smem;
   return out->smem_bytes <= kSmemMax;
 }
 
 template <int S, bool kExpand>
-static int launch(const Args& a, int B, size_t smem, cudaStream_t st) {
+static int launch(const CUtensorMap& mx, const CUtensorMap& m1, const CUtensorMap& m2, const Args& a, size_t smem,
+                  cudaStream_t st) {
   AM_TRY((allow_dynamic_smem<fused_block_kernel<S, kExpand>>(kSmemMax)));
-  const int64_t grid = (int64_t)B * a.tiles_y * a.tiles_x;
-  AM_CHECK(grid < ((int64_t)1 << 31), "fused block: %lld tiles is too many for one launch", (long long)grid);
-  AM_LAUNCH((fused_block_kernel<S, kExpand>), (unsigned)grid, kThreads, smem, st, a);
+  const int grid = std::max(1, std::min(a.num_tiles, sm_count()));
+  AM_LAUNCH((fused_block_kernel<S, kExpand>), grid, pipe::kThreads, smem, st, mx, m1, m2, a);
   return AM_OK;
 }
 
@@ -285,13 +351,14 @@ int run(const BlockDesc& d, const Plan& p, const __nv_bfloat16* X, const __nv_bf
         const float* wd, const float* bd, const __nv_bfloat16* W2, const float* b2, __nv_bfloat16* Y, int B,
         cudaStream_t st) {
   AM_CHECK(X && wd && bd && W2 && b2 && Y && (!d.has_expand || (W1 && b1)), "fused block: NULL operand");
+  auto aligned16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
+  AM_CHECK(aligned16(X) && aligned16(W2) && aligned16(wd) && aligned16(bd) && (!d.has_expand || (aligned16(W1) && aligned16(b1))),
+           "fused block: operands must be 16-byte aligned (TMA)");
   Args a{};
   a.X = X;
-  a.W1 = W1;
-  a.b1 = b1;
   a.wd = wd;
   a.bd = bd;
-  a.W2 = W2;
+  a.b1 = b1;
   a.b2 = b2;
   a.Y = Y;
   a.H = d.H;
@@ -300,12 +367,25 @@ int run(const BlockDesc& d, const Plan& p, const __nv_bfloat16* X, const __nv_bf
   a.Wo = (d.W - 1) / d.stride + 1;
   a.tiles_y = (a.Ho + kTile - 1) / kTile;
   a.tiles_x = (a.Wo + kTile - 1) / kTile;
+  const int64_t tiles = (int64_t)B * a.tiles_y * a.tiles_x;
+  AM_CHECK(tiles < ((int64_t)1 << 31), "fused block: %lld tiles is too many for one launch", (long long)tiles);
+  a.num_tiles = (int)tiles;
   a.cin_p = d.cin_p;
   a.cmid_p = d.cmid_p;
   a.cout_p = d.cout_p;
   a.residual = d.residual;
-  if (d.stride == 1) return d.has_expand ? launch<1, true>(a, B, p.smem_bytes, st) : launch<1, false>(a, B, p.smem_bytes, st);
-  return d.has_expand ? launch<2, true>(a, B, p.smem_bytes, st) : launch<2, false>(a, B, p.smem_bytes, st);
+  const Layout l = layout(d.stride, d.has_expand != 0, d.cin_p, d.cout_p, p.stages);
+  AM_CHECK(l.smem == p.smem_bytes, "fused block: plan does not match the block");
+  a.l = l;
+
+  CUtensorMap mx, m1, m2;
+  const int hl = halo(d.stride);
+  AM_TRY(gemm::encode_map_nhwc_bf16(&mx, X, B, d.H, d.W, d.cin_p, hl, hl, d.has_expand != 0));
+  AM_TRY(gemm::encode_map_bf16(&m2, W2, d.cmid_p, d.cout_p, d.cmid_p, (d.cout_p + 63) / 64 * 64));
+  if (d.has_expand) AM_TRY(gemm::encode_map_bf16(&m1, W1, d.cin_p, d.cmid_p, d.cin_p, kChunk));
+  else m1 = m2;  // unused
+  if (d.stride == 1) return d.has_expand ? launch<1, true>(mx, m1, m2, a, l.smem, st) : launch<1, false>(mx, m1, m2, a, l.smem, st);
+  return d.has_expand ? launch<2, true>(mx, m1, m2, a, l.smem, st) : launch<2, false>(mx, m1, m2, a, l.smem, st);
 }
 
 }  // namespace fused

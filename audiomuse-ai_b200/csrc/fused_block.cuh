@@ -17,6 +17,7 @@ struct BlockDesc {
 
 struct Plan {
   size_t smem_bytes = 0;
+  int stages = 1;  // depth of the per-chunk weight ring (2 unless only 1 fits)
 };
 
 // false when the block does not fit the kernel (Cout > 256, shared memory)

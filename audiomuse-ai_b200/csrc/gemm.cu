@@ -315,6 +315,25 @@ int encode_map_bf16(void* map_out, const void* base, int64_t inner, int64_t rows
   return AM_OK;
 }
 
+int encode_map_nhwc_bf16(void* map_out, const void* base, int64_t n, int64_t h, int64_t w, int64_t c, int box_w,
+                         int box_h, bool swizzle) {
+  AM_CHECK(get_encode() != nullptr, "cuTensorMapEncodeTiled unavailable");
+  const cuuint64_t dims[4] = {(cuuint64_t)c, (cuuint64_t)w, (cuuint64_t)h, (cuuint64_t)n};
+  const cuuint64_t strides[3] = {(cuuint64_t)(c * 2), (cuuint64_t)(w * c * 2), (cuuint64_t)(h * w * c * 2)};
+  const cuuint32_t box[4] = {(cuuint32_t)kChunkK, (cuuint32_t)box_w, (cuuint32_t)box_h, 1};
+  const cuuint32_t estr[4] = {1, 1, 1, 1};
+  CUresult r = get_encode()(reinterpret_cast<CUtensorMap*>(map_out), CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4,
+                            const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                            swizzle ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE,
+                            CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    set_error("cuTensorMapEncodeTiled failed (%d) nhwc=[%lld, %lld, %lld, %lld] box=%dx%d", (int)r, (long long)n,
+              (long long)h, (long long)w, (long long)c, box_w, box_h);
+    return AM_ERR_CUDA;
+  }
+  return AM_OK;
+}
+
 // tile widths gemm_wgmma_kernel is instantiated for (the switch in gemm_bf16)
 static bool gemm_has_n(int n) {
   return n == 16 || n == 32 || n == 48 || n == 64 || n == 80 || n == 96 || n == 112 || n == 128 || n == 160 ||

@@ -43,6 +43,12 @@ int gemm_bf16(const __nv_bfloat16* A, int64_t M, int64_t lda, const __nv_bfloat1
 // map_out: 128-byte CUtensorMap.
 int encode_map_bf16(void* map_out, const void* base, int64_t inner, int64_t rows, int64_t pitch_elems, int box_rows);
 
+// The TMA map of a dense NHWC bf16 activation [n, h, w, c] (c a multiple of 8), loaded in boxes of 64 channels x
+// box_w x box_h pixels of one image, zero fill outside (negative coordinates included): with `swizzle` as K-major
+// SWIZZLE_128B rows (one row per pixel, x fastest), without as plain 128-byte rows.
+int encode_map_nhwc_bf16(void* map_out, const void* base, int64_t n, int64_t h, int64_t w, int64_t c, int box_w,
+                         int box_h, bool swizzle);
+
 // reference implementation on CUDA cores (slow; used only by the on-device self test)
 int gemm_bf16_simt(const __nv_bfloat16* A, int64_t M, int64_t lda, const __nv_bfloat16* B, int64_t N,
                    int64_t ldb, int K, void* D, int64_t ldd, bool d_is_f32, const Epilogue& ep,

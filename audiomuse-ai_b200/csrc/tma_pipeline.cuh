@@ -1,5 +1,5 @@
-// The warp-specialised TMA -> wgmma main loop shared by gemm_wgmma_kernel (gemm.cu), assign_tc_kernel (kmeans_tc.cu)
-// and silhouette_tc_kernel (cluster_metrics.cu).
+// The warp-specialised TMA -> wgmma main loop shared by gemm_wgmma_kernel (gemm.cu), assign_tc_kernel (kmeans_tc.cu),
+// silhouette_tc_kernel (cluster_metrics.cu) and fused_block_kernel (fused_block.cu).
 //
 // A CTA of three warpgroups: warpgroup 0 is the producer (one elected lane of warp 0 issues the TMA loads), warpgroups
 // 1 and 2 are consumers (64 rows of the 128-row tile each).  Operand tiles travel through a ring of shared-memory
@@ -60,18 +60,22 @@ struct Ring {
     uint8_t* smem;
     uint64_t* bar;
   };
-  __device__ __forceinline__ Slot acquire() {
+  __device__ __forceinline__ Slot acquire() { return acquire(stage_bytes); }
+  // ... or for `tx_bytes`, when the loads of a stage do not fill it
+  __device__ __forceinline__ Slot acquire(uint32_t tx_bytes) {
     ptx::mbar_wait(&empty[stage], phase ^ 1);
-    ptx::mbar_expect_tx(&full[stage], stage_bytes);
+    ptx::mbar_expect_tx(&full[stage], tx_bytes);
     const Slot s{base + stage * stage_bytes, &full[stage]};
     advance();
     return s;
   }
 
   // consumer: waits until the next stage has landed and returns its shared-memory address ...
-  __device__ __forceinline__ uint32_t wait() const {
+  __device__ __forceinline__ uint32_t wait() const { return ptx::smem_u32(wait_ptr()); }
+  // ... or its generic address, for ordinary loads from the stage
+  __device__ __forceinline__ uint8_t* wait_ptr() const {
     ptx::mbar_wait(&full[stage], phase);
-    return ptx::smem_u32(base + stage * stage_bytes);
+    return base + stage * stage_bytes;
   }
   // ... and hands it back to the producer once this thread's MMAs have read it
   __device__ __forceinline__ void release() {
