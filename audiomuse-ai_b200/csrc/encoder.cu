@@ -39,6 +39,7 @@ struct Layer {
   DevBuf<float> w_f32;           // depthwise: [k*k, c_p]; stem: dw[9]; first conv: [kh*kw, c_p]; squeeze-excite: fc1 [cmid, c]
   DevBuf<float> bias;            // [cout_p]  (squeeze-excite: fc1 bias [cmid])
   DevBuf<float> aux0, aux1, aux2;  // stem / first conv: per-mel scale / shift (+ stem pw scale); squeeze-excite: fc2 [c, cmid], fc2 bias
+  DevBuf<float> fused_params;    // 3x3 depthwise: its weights, bias and the preceding pointwise layer's bias per 64-channel chunk (fused::pack_params)
   // true for the 3x3 / pad 1 / ReLU6 depthwise the packed-fp16 kernels implement
   bool dw_fast() const {
     return type == kDepthwise && kh == 3 && kw == 3 && pad_t == 1 && pad_b == 1 && pad_l == 1 && pad_r == 1 && act == kActRelu6;
@@ -931,6 +932,11 @@ static int build_model(am_model* m, const ModelSpec& spec) {
         for (int t = 0; t < taps; ++t) wt[(size_t)t * L->cin_p + ch] = S.w[(size_t)ch * taps + t];
       AM_TRY(upload(L->w_f32, wt));
       AM_TRY(upload(L->bias, padded(S.bias, L->cin_p)));
+      if (L->dw_fast()) {  // the fused kernel's parameters; the expansion bias matters only when fused_block_at fuses it
+        const LayerSpec* E = li > 0 && spec.layers[li - 1].type == kPointwise ? &spec.layers[li - 1] : nullptr;
+        const std::vector<float> b1 = E ? padded(E->bias, L->cin_p) : std::vector<float>();
+        AM_TRY(upload(L->fused_params, fused::pack_params(wt, padded(S.bias, L->cin_p), E ? &b1 : nullptr, L->cin_p)));
+      }
     } else if (S.type == kSqueezeExcite) {
       if (S.w.size() != (size_t)S.cmid * S.cin || S.bias.size() != (size_t)S.cmid || S.aux0.size() != (size_t)S.cin * S.cmid ||
           S.aux1.size() != (size_t)S.cin) {
@@ -1123,8 +1129,7 @@ static int run_range(am_model* m, const float* mel_dev, const __nv_bfloat16* in,
         const Layer& D = *m->layers[(size_t)dw];
         const Layer& P = *m->layers[(size_t)pj];
         __nv_bfloat16* dst = pick_dst((size_t)pj + 1 == hi);
-        AM_TRY(fused::run(d, pl, cur, E ? E->w_bf16.p : nullptr, E ? E->bias.p : nullptr, D.w_f32.p, D.bias.p,
-                          P.w_bf16.p, P.bias.p, dst, nb, st));
+        AM_TRY(fused::run(d, pl, cur, E ? E->w_bf16.p : nullptr, D.fused_params.p, P.w_bf16.p, P.bias.p, dst, nb, st));
         s = dw_out(D, s);
         cur = block_in = dst;
         i = (size_t)pj;

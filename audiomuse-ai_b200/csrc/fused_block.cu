@@ -4,22 +4,27 @@
 // Persistent, warp-specialised CTA of three warpgroups (tma_pipeline.cuh), each CTA looping over 8 x 8 output tiles:
 //   warpgroup 0   TMA producer (one elected lane): per tile the input halo (10 x 10 pixels at stride 1, 17 x 17 at
 //                 stride 2) through a 4-D NHWC tensor map as K-major 128-byte-swizzled bf16 rows, zero filled outside
-//                 the image and past cin_p; per 64-channel chunk of the expansion, into a two-stage ring: the W1 and
-//                 W2 chunks (2-D maps, zero filled past cmid_p / cout_p), the depthwise weights and biases and the
-//                 expansion bias (bulk copies), or, without an expansion conv, the input's channel chunk itself.
-//                 The next tile's halo and first chunks load while the consumers finish the current tile.
+//                 the image and past cin_p; per 64-channel chunk of the expansion, into a ring of as many stages as fit
+//                 (up to 4): the W1 and W2 chunks (2-D maps, zero filled past cmid_p / cout_p) or, without an expansion
+//                 conv, the input's channel chunk itself, and the chunk's depthwise weights and biases and expansion
+//                 bias in one bulk copy (packed per chunk at model load, pack_params).  The next tile's halo and first
+//                 chunks load while the consumers finish the current tile.
 //   warpgroups 1, 2   consumers, sharing one tile; per chunk:
-//     expansion   wgmma m64n64k16 over the halo rows (m blocks split between the warpgroups), fp32 accumulators ->
-//                 + bias, ReLU6 -> bf16 halo tile E [halo pixels x 64] (pixels outside the image are zero: the
-//                 depthwise pads with 0, and relu6(bias) need not be);
-//     depthwise   3 x 3 taps from E in fp32 (a thread = 8 channels of one output pixel) + bias, ReLU6 -> bf16, written
-//                 as the K-major swizzled A operand [64 pixels x 64 channels] of
+//     expansion   at stride 1 wgmma m64n64k16, one of the 2 halo m blocks per warpgroup; at stride 2 m64n32k16 over
+//                 all 5 m blocks, one 32-column half of the chunk per warpgroup; fp32 accumulators -> + bias, ReLU6
+//                 -> bf16 halo tile E [halo pixels x 64, 16-byte groups XOR-swizzled by pixel] (pixels outside the
+//                 image are zero: the depthwise pads with 0, and relu6(bias) need not be);
+//     depthwise   3 x 3 taps from E in fp32 (a thread = 8 channels of two adjacent output pixels) + bias, ReLU6 ->
+//                 bf16, written as the K-major swizzled A operand [64 pixels x 64 channels] of
 //     projection  wgmma m64n64k16 into register accumulators, 64-column blocks split between the warpgroups (Cout <=
 //                 256), accumulated over the chunks in ascending order.
-//   Two named barriers per chunk order E and the A operand between the consumer warpgroups.
+//   With two or more stages the chunks overlap: chunk c + 1's expansion MMAs are issued before chunk c's depthwise and
+//   run under it (they write only registers), and its epilogue refills E after chunk c's projection.  Two named
+//   barriers per chunk order E and the A operand between the consumer warpgroups; both retire their projection before
+//   the first, so one A buffer serves.
 // Epilogue: + bias (+ the block input for a residual block) -> bf16, straight from the registers.
 // Rounding follows the layer-by-layer path: the expansion and the depthwise output are rounded to bf16, every sum is
-// fp32.
+// fp32, in the same order for every element.
 #include "fused_block.cuh"
 
 #include "gemm_wgmma.cuh"
@@ -33,11 +38,13 @@ using namespace ptx;
 constexpr int kTile = 8;        // output tile edge: 64 pixels = one m64 projection
 constexpr int kChunk = 64;      // expansion channels per pass = one 128-byte swizzle row of projection K
 constexpr int kMaxCout = 256;
-constexpr int kMaxStages = 2;
+constexpr int kMaxStages = 4;
 constexpr size_t kSmemMax = 232448;
 constexpr uint32_t kConsumerBar = 1;  // named barrier of the two consumer warpgroups
-// per stage after W1 / W2: depthwise weights [9][64], depthwise bias [64], expansion bias [64], fp32
-constexpr uint32_t kDwBytes = (9 + 1 + 1) * kChunk * 4;
+// per stage after W1 / W2, and per chunk in pack_params: depthwise weights [9][64], depthwise bias [64], expansion
+// bias [64], fp32
+constexpr int kParamRows = 9 + 1 + 1;
+constexpr uint32_t kDwBytes = kParamRows * kChunk * 4;
 using Ring = pipe::Ring<kMaxStages>;
 
 __host__ __device__ constexpr int halo(int S) { return (kTile - 1) * S + 3; }
@@ -45,6 +52,10 @@ __host__ __device__ constexpr int halo_px(int S) { return halo(S) * halo(S); }
 __host__ __device__ constexpr int halo_rows(int S) { return (halo_px(S) + 63) / 64 * 64; }
 
 constexpr uint32_t round1k(uint32_t v) { return (v + 1023u) & ~1023u; }
+
+// element offset of channel group g (8 channels) of pixel p in E: rows of 64 bf16, the 16-byte groups XOR-swizzled
+// by the pixel so that the expansion epilogue's stores (8 pixels of one group per warp) hit distinct banks
+__device__ __forceinline__ int e_off(int p, int g) { return p * 64 + ((g ^ (p & 7)) << 3); }
 
 // byte offset of (row, 16-byte chunk) in a K-major SWIZZLE_128B tile (rows of 64 bf16, 8-row atoms of 1024 bytes)
 __device__ __forceinline__ uint32_t sw128(uint32_t row, uint32_t chunk) {
@@ -82,9 +93,7 @@ static Layout layout(int S, bool has_expand, int cin_p, int cout_p, int stages) 
 
 struct Args {
   const __nv_bfloat16* X;   // [B, H, W, cin_p] (the residual)
-  const float* wd;          // [9, cmid_p]
-  const float* bd;          // [cmid_p]
-  const float* b1;          // [cmid_p] (has_expand)
+  const float* params;      // [cmid_p / 64 rounded up][kParamRows][64] (pack_params)
   const float* b2;          // [cout_p]
   __nv_bfloat16* Y;         // [B, Ho, Wo, cout_p]
   int H, W, Ho, Wo, tiles_y, tiles_x, num_tiles;
@@ -92,12 +101,45 @@ struct Args {
   Layout l;
 };
 
+// Per-phase cycle counters of a measurement build (-DAM_FUSED_PHASES, tools/fused_block_phases.py): one thread of each
+// warpgroup sums clock64 deltas per phase and adds them, per CTA, to g_phase_cycles[warpgroup]; run() prints the sums
+// of every launch to stderr.  A default build compiles PhaseClock to nothing.
+enum Phase { kRingWait, kHaloWait, kExpandMma, kExpandEpi, kDepthwise, kProjectMma, kBarrier, kEpilogue, kIssue, kNumPhases };
+#ifdef AM_FUSED_PHASES
+static const char* const kPhaseNames[kNumPhases] = {"ring_wait", "halo_wait", "expand_mma", "expand_epi", "depthwise",
+                                                     "project_mma", "barrier", "epilogue", "issue"};
+__device__ unsigned long long g_phase_cycles[3][kNumPhases];
+__device__ __forceinline__ long long clock_now() {
+  long long v;
+  asm volatile("mov.u64 %0, %%clock64;" : "=l"(v));
+  return v;
+}
+struct PhaseClock {
+  uint32_t acc[kNumPhases];  // 32 bits: a CTA's cycles in one phase of one launch stay far below 2^32
+  long long t;
+  __device__ __forceinline__ PhaseClock() : acc{}, t(clock_now()) {}
+  __device__ __forceinline__ void lap(Phase p) {
+    const long long n = clock_now();
+    acc[p] += (uint32_t)(n - t);
+    t = n;
+  }
+  __device__ __forceinline__ void flush(int wg) {
+    for (int p = 0; p < kNumPhases; ++p) atomicAdd(&g_phase_cycles[wg][p], (unsigned long long)acc[p]);
+  }
+};
+#else
+struct PhaseClock {
+  __device__ __forceinline__ void lap(Phase) {}
+  __device__ __forceinline__ void flush(int) {}
+};
+#endif
+
 template <int S, bool kExpand>
 __global__ void __launch_bounds__(pipe::kThreads, 1)
 fused_block_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_w1,
                    const __grid_constant__ CUtensorMap map_w2, const Args a) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  constexpr int HALO = halo(S), HPX = halo_px(S), HR = halo_rows(S);
+  constexpr int HALO = halo(S), HPX = halo_px(S), HR = halo_rows(S), MB = HR / 64;
   Ring ring(smem_raw, a.l.stage, a.l.stages, a.l.extra);
   uint8_t* own = ring.extra();
   uint8_t* xs = own + a.l.xs;
@@ -123,33 +165,36 @@ fused_block_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_const
     regs_producer();
     // ===================== TMA producer =====================
     if (threadIdx.x < 32 && elect_one_sync()) {
+      PhaseClock clk;
       uint32_t xs_phase = 0;
       for (int tile = blockIdx.x; tile < a.num_tiles; tile += gridDim.x) {
         const int b = tile / per_img, ty = (tile % per_img) / a.tiles_x, tx = tile % a.tiles_x;
         const int gy0 = ty * kTile * S - 1, gx0 = tx * kTile * S - 1;  // image position of halo pixel (0, 0)
         if (kExpand) {
+          clk.lap(kIssue);
           mbar_wait(xs_empty, xs_phase ^ 1);
+          clk.lap(kHaloWait);
           mbar_expect_tx(xs_full, (uint32_t)(kbx * HPX * 128));
           for (int kb = 0; kb < kbx; ++kb) tma_load_4d(xs + kb * HR * 128, &map_x, xs_full, kb * 64, gx0, gy0, b);
           xs_phase ^= 1;
         }
         for (int c0 = 0; c0 < a.cmid_p; c0 += kChunk) {
-          const uint32_t nb = (uint32_t)min(kChunk, a.cmid_p - c0) * 4;  // bytes of one row of depthwise params
           const uint32_t tx_bytes = (kExpand ? (uint32_t)kbx * kChunk * 128 : (uint32_t)HPX * 128) +
-                                    (uint32_t)n2_blocks * 64 * 128 + (kExpand ? 11u : 10u) * nb;
+                                    (uint32_t)n2_blocks * 64 * 128 + kDwBytes;
+          clk.lap(kIssue);
           const Ring::Slot s = ring.acquire(tx_bytes);
+          clk.lap(kRingWait);
           if (kExpand) {
             for (int kb = 0; kb < kbx; ++kb) tma_load_2d(s.smem + kb * kChunk * 128, &map_w1, s.bar, kb * 64, c0);
           } else {
             tma_load_4d(s.smem, &map_x, s.bar, c0, gx0, gy0, b);
           }
           tma_load_2d(s.smem + a.l.w2, &map_w2, s.bar, c0, 0);
-          float* dw = reinterpret_cast<float*>(s.smem + a.l.dw);
-          for (int t = 0; t < 9; ++t) bulk_load(dw + t * kChunk, a.wd + (int64_t)t * a.cmid_p + c0, nb, s.bar);
-          bulk_load(dw + 9 * kChunk, a.bd + c0, nb, s.bar);
-          if (kExpand) bulk_load(dw + 10 * kChunk, a.b1 + c0, nb, s.bar);
+          bulk_load(s.smem + a.l.dw, a.params + (int64_t)c0 * kParamRows, kDwBytes, s.bar);
         }
       }
+      clk.lap(kIssue);
+      clk.flush(0);
     }
     return;
   }
@@ -161,17 +206,71 @@ fused_block_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_const
   const int warp = wt >> 5, lane = wt & 31, quad = lane & 3;
   __nv_bfloat16* e_own = reinterpret_cast<__nv_bfloat16*>(own + a.l.e);  // [HPX][64], plain rows of 128 bytes
   const uint4 zero4 = make_uint4(0u, 0u, 0u, 0u);
+  const int nchunks = (a.cmid_p + kChunk - 1) / kChunk;
+  // With two or more stages chunk c + 1's expansion reads its stage while chunk c's is still held; a one-stage ring
+  // cannot hold both, so there the expansion waits for chunk c's projection and the stage it frees.
+  const bool ahead = a.l.stages > 1;
 
-  // the first MMA of every expansion m block and of every tile's projection overwrites (scale_d = 0)
-  float acc1[32];     // expansion
-  float acc2[2][32];  // projection column blocks nb = wg and wg + 2
+  // How the warpgroups share the expansion: at stride 1 (2 m blocks) one m block each over all 64 columns, at stride 2
+  // (5 m blocks, which do not split evenly) every m block over one 32-column half each.
+  constexpr bool kSplitN = MB % 2 != 0;
+  constexpr int kEM = kSplitN ? MB : MB / 2, kEN = kSplitN ? 32 : 64;  // m blocks and columns per warpgroup
+  const int m0 = kSplitN ? 0 : wg, n0 = kSplitN ? 32 * wg : 0;        // first m block and column of this warpgroup
+
+  // the first MMA of every expansion and of every tile's projection overwrites (scale_d = 0)
+  float acc1[kEM][kEN / 2];  // expansion: m block m0 + m, columns n0 .. n0 + kEN - 1 of the chunk
+  float acc2[2][32];         // projection column blocks nb = wg and wg + 2
 #pragma unroll
-  for (int i = 0; i < 32; ++i) acc1[i] = 0.f;
+  for (int m = 0; m < kEM; ++m)
+#pragma unroll
+    for (int i = 0; i < kEN / 2; ++i) acc1[m][i] = 0.f;
 #pragma unroll
   for (int j = 0; j < 2; ++j)
 #pragma unroll
     for (int i = 0; i < 32; ++i) acc2[j][i] = 0.f;
 
+  // acc1 = this warpgroup's halo rows . W1 chunk columns [n0, n0 + kEN)^T, issued and committed, not waited for
+  auto expand_issue = [&](const uint8_t* stage) {
+    const uint32_t w1 = smem_u32(stage) + (uint32_t)(n0 * 128);
+    wgmma_fence();
+#pragma unroll
+    for (int m = 0; m < kEM; ++m)
+      for (int kb = 0; kb < kbx; ++kb) {
+        const uint64_t da = make_smem_desc(smem_u32(xs + (kb * HR + (m0 + m) * 64) * 128));
+        const uint64_t db = make_smem_desc(w1 + (uint32_t)(kb * kChunk * 128));
+        const int ksteps = min(4, (a.cin_p - kb * 64) / 16);
+        for (int ks = 0; ks < ksteps; ++ks)
+          Wgmma<kEN>::mma(acc1[m], da + (uint64_t)(ks * 2), db + (uint64_t)(ks * 2), (kb | ks) ? 1u : 0u);
+      }
+    wgmma_commit();
+  };
+  // E columns of this warpgroup = relu6(acc1 + b1), zero outside the image and past the chunk's channels
+  auto expand_epilogue = [&](const uint8_t* stage, int nch, int gy0, int gx0) {
+#pragma unroll
+    for (int m = 0; m < kEM; ++m) reg_fence(acc1[m]);
+    const float* b1 = reinterpret_cast<const float*>(stage + a.l.dw) + 10 * kChunk;
+#pragma unroll
+    for (int m = 0; m < kEM; ++m)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int p = (m0 + m) * 64 + warp * 16 + (lane >> 2) + 8 * h;
+        if (p >= HPX) continue;
+        const int gy = gy0 + p / HALO, gx = gx0 + p % HALO;
+        const bool inside = gy >= 0 && gy < a.H && gx >= 0 && gx < a.W;
+#pragma unroll
+        for (int j = 0; j < kEN / 8; ++j) {
+          const int col = n0 + 8 * j + 2 * quad;
+          float f0 = 0.f, f1 = 0.f;
+          if (inside && col < nch) {
+            f0 = relu6f(acc1[m][4 * j + 2 * h] + b1[col]);
+            f1 = relu6f(acc1[m][4 * j + 2 * h + 1] + b1[col + 1]);
+          }
+          *reinterpret_cast<__nv_bfloat162*>(e_own + e_off(p, n0 / 8 + j) + 2 * quad) = __floats2bfloat162_rn(f0, f1);
+        }
+      }
+  };
+
+  PhaseClock clk;
   uint32_t xs_phase = 0;
   for (int tile = blockIdx.x; tile < a.num_tiles; tile += gridDim.x) {
     const int b = tile / per_img, ty = (tile % per_img) / a.tiles_x, tx = tile % a.tiles_x;
@@ -180,88 +279,83 @@ fused_block_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_const
     if (kExpand) {
       mbar_wait(xs_full, xs_phase);
       xs_phase ^= 1;
+      clk.lap(kHaloWait);
+      const uint8_t* s0 = ring.wait_ptr();
+      clk.lap(kRingWait);
+      expand_issue(s0);
+      wgmma_wait<0>();
+      clk.lap(kExpandMma);
+      expand_epilogue(s0, min(kChunk, a.cmid_p), gy0, gx0);
+      if (nchunks == 1) mbar_arrive(xs_empty);  // this thread's reads of the halo are complete
+      clk.lap(kExpandEpi);
     }
 
-    for (int c0 = 0; c0 < a.cmid_p; c0 += kChunk) {
-      const int nch = min(kChunk, a.cmid_p - c0);
-      uint8_t* sp = ring.wait_ptr();
-      const uint32_t st = smem_u32(sp);
+    for (int c = 0; c < nchunks; ++c) {
+      const int c0 = c * kChunk, nch = min(kChunk, a.cmid_p - c0);
+      const bool next = kExpand && c + 1 < nchunks;  // chunk c + 1's expansion runs in this iteration
+      uint8_t* sp = ring.wait_ptr();  // returns at once when the expansion already waited for it
+      clk.lap(kRingWait);
       const float* dwp = reinterpret_cast<const float*>(sp + a.l.dw);
       const __nv_bfloat16* e = kExpand ? e_own : reinterpret_cast<const __nv_bfloat16*>(sp);
-
-      if (kExpand) {
-        for (int m = wg; m < HR / 64; m += 2) {
-          wgmma_fence();
-          for (int kb = 0; kb < kbx; ++kb) {
-            const uint64_t da = make_smem_desc(smem_u32(xs + kb * HR * 128 + m * 64 * 128));
-            const uint64_t db = make_smem_desc(st + (uint32_t)(kb * kChunk * 128));
-            const int ksteps = min(4, (a.cin_p - kb * 64) / 16);
-            for (int ks = 0; ks < ksteps; ++ks)
-              Wgmma<64>::mma(acc1, da + (uint64_t)(ks * 2), db + (uint64_t)(ks * 2), (kb | ks) ? 1u : 0u);
-          }
-          wgmma_commit();
-          wgmma_wait_all();
-          reg_fence(acc1);
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            const int p = m * 64 + warp * 16 + (lane >> 2) + 8 * h;
-            if (p >= HPX) continue;
-            const int gy = gy0 + p / HALO, gx = gx0 + p % HALO;
-            const bool inside = gy >= 0 && gy < a.H && gx >= 0 && gx < a.W;
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              const int col = 8 * j + 2 * quad;
-              float f0 = 0.f, f1 = 0.f;
-              if (inside && col < nch) {
-                f0 = relu6f(acc1[4 * j + 2 * h] + dwp[10 * kChunk + col]);
-                f1 = relu6f(acc1[4 * j + 2 * h + 1] + dwp[10 * kChunk + col + 1]);
-              }
-              *reinterpret_cast<__nv_bfloat162*>(e_own + p * 64 + col) = __floats2bfloat162_rn(f0, f1);
-            }
-          }
-        }
-        if (c0 + kChunk >= a.cmid_p) mbar_arrive(xs_empty);  // this thread's reads of the halo are complete
-      }
       // E is complete, and both warpgroups' previous projection has finished reading A
       named_bar_sync(kConsumerBar, pipe::kConsumerThreads);
+      clk.lap(kBarrier);
+      const uint8_t* sn = nullptr;  // chunk c + 1's stage
+      if (next && ahead) {
+        sn = ring.wait_ahead_ptr();
+        clk.lap(kRingWait);
+        expand_issue(sn);
+        clk.lap(kExpandMma);
+      }
 
-      // depthwise: item = 8 channels of one output pixel
-      for (int it = ct; it < 64 * 8; it += pipe::kConsumerThreads) {
-        const int g = it & 7, px = it >> 3;
+      // depthwise: a thread = 8 channels (group g) of two horizontally adjacent output pixels, so each tap's weights
+      // are loaded once for both
+      {
+        const int g = ct & 7, px = (ct >> 3) * 2;
         const int oy = px >> 3, ox = px & 7;
-        uint4 out = zero4;
+        uint4 out[2] = {zero4, zero4};
         if (g * 8 < nch) {
           const float* bias = dwp + 9 * kChunk + g * 8;
-          float acc[8];
+          float acc[2][8];
 #pragma unroll
-          for (int q = 0; q < 8; ++q) acc[q] = bias[q];
+          for (int q = 0; q < 8; ++q) acc[0][q] = acc[1][q] = bias[q];
 #pragma unroll
           for (int dy = 0; dy < 3; ++dy)
 #pragma unroll
             for (int dx = 0; dx < 3; ++dx) {
-              const int hp = (oy * S + dy) * HALO + ox * S + dx;
-              const uint4 v = *reinterpret_cast<const uint4*>(e + hp * 64 + g * 8);
-              const __nv_bfloat162* v2 = reinterpret_cast<const __nv_bfloat162*>(&v);
               const float4* w4 = reinterpret_cast<const float4*>(dwp + (dy * 3 + dx) * kChunk + g * 8);
               const float4 wa = w4[0], wb = w4[1];
               const float w[8] = {wa.x, wa.y, wa.z, wa.w, wb.x, wb.y, wb.z, wb.w};
 #pragma unroll
-              for (int q = 0; q < 4; ++q) {
-                const float2 f = __bfloat1622float2(v2[q]);
-                acc[2 * q] = fmaf(f.x, w[2 * q], acc[2 * q]);
-                acc[2 * q + 1] = fmaf(f.y, w[2 * q + 1], acc[2 * q + 1]);
+              for (int i = 0; i < 2; ++i) {
+                const int hp = (oy * S + dy) * HALO + (ox + i) * S + dx;
+                const uint4 v = *reinterpret_cast<const uint4*>(e + e_off(hp, g));
+                const __nv_bfloat162* v2 = reinterpret_cast<const __nv_bfloat162*>(&v);
+#pragma unroll
+                for (int q = 0; q < 4; ++q) {
+                  const float2 f = __bfloat1622float2(v2[q]);
+                  acc[i][2 * q] = fmaf(f.x, w[2 * q], acc[i][2 * q]);
+                  acc[i][2 * q + 1] = fmaf(f.y, w[2 * q + 1], acc[i][2 * q + 1]);
+                }
               }
             }
-        __nv_bfloat162 o2[4];
 #pragma unroll
-          for (int q = 0; q < 4; ++q) o2[q] = __floats2bfloat162_rn(relu6f(acc[2 * q]), relu6f(acc[2 * q + 1]));
-          out = *reinterpret_cast<const uint4*>(o2);
+          for (int i = 0; i < 2; ++i) {
+            __nv_bfloat162 o2[4];
+#pragma unroll
+            for (int q = 0; q < 4; ++q)
+              o2[q] = __floats2bfloat162_rn(relu6f(acc[i][2 * q]), relu6f(acc[i][2 * q + 1]));
+            out[i] = *reinterpret_cast<const uint4*>(o2);
+          }
         }
-        *reinterpret_cast<uint4*>(a2 + sw128(px, g)) = out;
+#pragma unroll
+        for (int i = 0; i < 2; ++i) *reinterpret_cast<uint4*>(a2 + sw128(px + i, g)) = out[i];
       }
       fence_proxy_async();  // generic-proxy writes of A -> visible to the wgmma (async proxy) reads
+      clk.lap(kDepthwise);
       // A is complete, and both warpgroups are done reading E
       named_bar_sync(kConsumerBar, pipe::kConsumerThreads);
+      clk.lap(kBarrier);
 
       // projection: acc2 += A2 [64 x nch] . W2_chunk [Cout x nch]^T
       wgmma_fence();
@@ -270,16 +364,33 @@ fused_block_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_const
       for (int j = 0; j < 2; ++j) {
         const int nb = wg + 2 * j;
         if (nb < n2_blocks) {
-          const uint64_t db = make_smem_desc(st + a.l.w2 + (uint32_t)(nb * 64 * 128));
+          const uint64_t db = make_smem_desc(smem_u32(sp) + a.l.w2 + (uint32_t)(nb * 64 * 128));
           for (int ks = 0; ks < nch / 16; ++ks)
             Wgmma<64>::mma(acc2[j], da + (uint64_t)(ks * 2), db + (uint64_t)(ks * 2), (c0 | ks) ? 1u : 0u);
         }
       }
       wgmma_commit();
-      wgmma_wait_all();
+      clk.lap(kProjectMma);
+
+      if (next && !ahead) {  // one stage: chunk c + 1 lands only once chunk c's stage is free
+        wgmma_wait<0>();
+        ring.release();
+        sn = ring.wait_ptr();
+        clk.lap(kRingWait);
+        expand_issue(sn);
+      }
+      // Retires chunk c + 1's expansion too.  Waiting for it alone (wait_group 1) and running its epilogue under the
+      // projection makes ptxas serialise the wgmmas (C7514), so the two retire together.
+      wgmma_wait<0>();
 #pragma unroll
       for (int j = 0; j < 2; ++j) reg_fence(acc2[j]);
-      ring.release();
+      if (!next || ahead) ring.release();
+      clk.lap(kProjectMma);
+      if (next) {
+        expand_epilogue(sn, min(kChunk, a.cmid_p - c0 - kChunk), gy0, gx0);
+        if (c + 2 == nchunks) mbar_arrive(xs_empty);  // this thread's reads of the halo are complete
+        clk.lap(kExpandEpi);
+      }
     }
 
     // epilogue: + bias (+ block input) -> bf16
@@ -308,7 +419,9 @@ fused_block_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_const
         }
       }
     }
+    clk.lap(kEpilogue);
   }
+  if (wt == 0) clk.flush(1 + wg);
 }
 
 // The shapes the fused path takes: those whose single-buffered tile working set (input halo, one W1 and W2 chunk,
@@ -332,7 +445,7 @@ bool plan(const BlockDesc& d, Plan* out) {
   if (d.residual && (d.stride != 1 || d.cin_p != d.cout_p)) return false;
   if (!fits(d)) return false;
   Layout l = layout(d.stride, d.has_expand != 0, d.cin_p, d.cout_p, kMaxStages);
-  if (l.smem > kSmemMax) l = layout(d.stride, d.has_expand != 0, d.cin_p, d.cout_p, 1);
+  for (int s = kMaxStages - 1; s >= 1 && l.smem > kSmemMax; --s) l = layout(d.stride, d.has_expand != 0, d.cin_p, d.cout_p, s);
   out->stages = l.stages;
   out->smem_bytes = l.smem;
   return out->smem_bytes <= kSmemMax;
@@ -343,22 +456,47 @@ static int launch(const CUtensorMap& mx, const CUtensorMap& m1, const CUtensorMa
                   cudaStream_t st) {
   AM_TRY((allow_dynamic_smem<fused_block_kernel<S, kExpand>>(kSmemMax)));
   const int grid = std::max(1, std::min(a.num_tiles, sm_count()));
+#ifdef AM_FUSED_PHASES
+  void* counters = nullptr;
+  AM_CUDA(cudaGetSymbolAddress(&counters, g_phase_cycles));
+  AM_CUDA(cudaMemsetAsync(counters, 0, sizeof(g_phase_cycles), st));
+#endif
   AM_LAUNCH((fused_block_kernel<S, kExpand>), grid, pipe::kThreads, smem, st, mx, m1, m2, a);
+#ifdef AM_FUSED_PHASES
+  unsigned long long c[3][kNumPhases];
+  AM_CUDA(cudaStreamSynchronize(st));
+  AM_CUDA(cudaMemcpyFromSymbol(c, g_phase_cycles, sizeof(c)));
+  std::fprintf(stderr, "fused_phases H=%d W=%d cin=%d cmid=%d cout=%d S=%d stages=%d grid=%d tiles=%d", a.H, a.W,
+               a.cin_p, a.cmid_p, a.cout_p, S, a.l.stages, grid, a.num_tiles);
+  for (int w = 0; w < 3; ++w)
+    for (int p = 0; p < kNumPhases; ++p) std::fprintf(stderr, " wg%d.%s=%llu", w, kPhaseNames[p], c[w][p]);
+  std::fprintf(stderr, "\n");
+#endif
   return AM_OK;
 }
 
-int run(const BlockDesc& d, const Plan& p, const __nv_bfloat16* X, const __nv_bfloat16* W1, const float* b1,
-        const float* wd, const float* bd, const __nv_bfloat16* W2, const float* b2, __nv_bfloat16* Y, int B,
-        cudaStream_t st) {
-  AM_CHECK(X && wd && bd && W2 && b2 && Y && (!d.has_expand || (W1 && b1)), "fused block: NULL operand");
+std::vector<float> pack_params(const std::vector<float>& wd, const std::vector<float>& bd, const std::vector<float>* b1,
+                               int c_p) {
+  const int chunks = (c_p + kChunk - 1) / kChunk;
+  std::vector<float> out((size_t)chunks * kParamRows * kChunk, 0.f);
+  for (int c = 0; c < c_p; ++c) {
+    float* q = &out[((size_t)(c / kChunk) * kParamRows) * kChunk + c % kChunk];
+    for (int t = 0; t < 9; ++t) q[t * kChunk] = wd[(size_t)t * c_p + c];
+    q[9 * kChunk] = bd[c];
+    if (b1) q[10 * kChunk] = (*b1)[c];
+  }
+  return out;
+}
+
+int run(const BlockDesc& d, const Plan& p, const __nv_bfloat16* X, const __nv_bfloat16* W1, const float* params,
+        const __nv_bfloat16* W2, const float* b2, __nv_bfloat16* Y, int B, cudaStream_t st) {
+  AM_CHECK(X && params && W2 && b2 && Y && (!d.has_expand || W1), "fused block: NULL operand");
   auto aligned16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
-  AM_CHECK(aligned16(X) && aligned16(W2) && aligned16(wd) && aligned16(bd) && (!d.has_expand || (aligned16(W1) && aligned16(b1))),
+  AM_CHECK(aligned16(X) && aligned16(W2) && aligned16(params) && (!d.has_expand || aligned16(W1)),
            "fused block: operands must be 16-byte aligned (TMA)");
   Args a{};
   a.X = X;
-  a.wd = wd;
-  a.bd = bd;
-  a.b1 = b1;
+  a.params = params;
   a.b2 = b2;
   a.Y = Y;
   a.H = d.H;
@@ -380,7 +518,7 @@ int run(const BlockDesc& d, const Plan& p, const __nv_bfloat16* X, const __nv_bf
 
   CUtensorMap mx, m1, m2;
   const int hl = halo(d.stride);
-  AM_TRY(gemm::encode_map_nhwc_bf16(&mx, X, B, d.H, d.W, d.cin_p, hl, hl, d.has_expand != 0));
+  AM_TRY(gemm::encode_map_nhwc_bf16(&mx, X, B, d.H, d.W, d.cin_p, hl, hl, true));
   AM_TRY(gemm::encode_map_bf16(&m2, W2, d.cmid_p, d.cout_p, d.cmid_p, (d.cout_p + 63) / 64 * 64));
   if (d.has_expand) AM_TRY(gemm::encode_map_bf16(&m1, W1, d.cin_p, d.cmid_p, d.cin_p, kChunk));
   else m1 = m2;  // unused

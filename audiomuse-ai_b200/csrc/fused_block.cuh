@@ -17,17 +17,22 @@ struct BlockDesc {
 
 struct Plan {
   size_t smem_bytes = 0;
-  int stages = 1;  // depth of the per-chunk weight ring (2 unless only 1 fits)
+  int stages = 1;  // depth of the per-chunk weight ring: as many stages as fit, up to 4
 };
 
 // false when the block does not fit the kernel (Cout > 256, shared memory)
 bool plan(const BlockDesc& d, Plan* out);
 
-// W1 [cmid_p, cin_p] bf16, b1 [cmid_p] (NULL without an expansion conv); wd [9, cmid_p], bd [cmid_p];
+// The kernel's per-chunk parameters of a 3x3 depthwise layer of c_p channels: for every 64 channels, one contiguous
+// [11][64] fp32 block of the 9 tap weights (wd [9, c_p]), the bias (bd [c_p]) and the preceding expansion's bias (b1
+// [c_p]; zeros when NULL), zero past c_p, so that one bulk copy loads a chunk's parameters.
+std::vector<float> pack_params(const std::vector<float>& wd, const std::vector<float>& bd, const std::vector<float>* b1,
+                               int c_p);
+
+// W1 [cmid_p, cin_p] bf16 (NULL without an expansion conv); params = pack_params(depthwise, expansion bias);
 // W2 [cout_p, cmid_p] bf16, b2 [cout_p]; X [B, H, W, cin_p] -> Y [B, Ho, Wo, cout_p], NHWC bf16
-int run(const BlockDesc& d, const Plan& p, const __nv_bfloat16* X, const __nv_bfloat16* W1, const float* b1,
-        const float* wd, const float* bd, const __nv_bfloat16* W2, const float* b2, __nv_bfloat16* Y, int B,
-        cudaStream_t st);
+int run(const BlockDesc& d, const Plan& p, const __nv_bfloat16* X, const __nv_bfloat16* W1, const float* params,
+        const __nv_bfloat16* W2, const float* b2, __nv_bfloat16* Y, int B, cudaStream_t st);
 
 }  // namespace fused
 }  // namespace am

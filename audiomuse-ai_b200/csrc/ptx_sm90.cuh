@@ -98,6 +98,9 @@ __device__ __forceinline__ void regs_consumer() { asm volatile("setmaxnreg.inc.s
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// waits until at most N committed groups of this warpgroup are pending (groups retire in commit order)
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 // keeps the accumulator registers live across the asynchronous MMAs (they are read only after wgmma_wait_all)
 template <int R>
 __device__ __forceinline__ void reg_fence(float (&d)[R]) {

@@ -35,7 +35,9 @@ struct Ring {
   uint32_t phase = 0;
 
   __device__ __forceinline__ Ring(uint8_t* smem_raw, uint32_t stage_bytes_, int stages_, uint32_t extra_bytes)
-      : base(reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023)),
+      // an offset from smem_raw rather than an integer round trip, so that the compiler still knows every pointer
+      // into the ring is shared memory and emits LDS / STS for the kernels' own accesses instead of generic LD / ST
+      : base(smem_raw + ((1024u - (ptx::smem_u32(smem_raw) & 1023u)) & 1023u)),
         full(reinterpret_cast<uint64_t*>(base + stages_ * stage_bytes_ + extra_bytes)),
         empty(full + kMaxStages),
         stage_bytes(stage_bytes_),
@@ -76,6 +78,12 @@ struct Ring {
   __device__ __forceinline__ uint8_t* wait_ptr() const {
     ptx::mbar_wait(&full[stage], phase);
     return base + stage * stage_bytes;
+  }
+  // ... or, still holding that stage, waits for the one after it without advancing (needs stages > 1)
+  __device__ __forceinline__ uint8_t* wait_ahead_ptr() const {
+    const int next = stage + 1 == stages ? 0 : stage + 1;
+    ptx::mbar_wait(&full[next], next == 0 ? phase ^ 1 : phase);
+    return base + next * stage_bytes;
   }
   // ... and hands it back to the producer once this thread's MMAs have read it
   __device__ __forceinline__ void release() {
