@@ -96,7 +96,9 @@ int build_filterbank(const am_mel_cfg& c, std::vector<float>& w /* [n_mels * bin
 }
 
 // ---------------------------------------------------------------- device: 32-point FFT
-__device__ __forceinline__ float cos32(int i) {  // cos(2*pi*i/32), i in [0,16)
+// Only ever called with compile-time indices (fft32_stage's template arguments and unrolled loop counters), so every
+// call folds to a constant.
+__host__ __device__ constexpr float cos32(int i) {  // cos(2*pi*i/32), i in [0,16)
   switch (i) {
     case 0: return 1.0f;
     case 1: return 0.98078528040323044913f;
@@ -117,52 +119,59 @@ __device__ __forceinline__ float cos32(int i) {  // cos(2*pi*i/32), i in [0,16)
   }
 }
 // sin(2*pi*i/32) for i in [0,16): sin(x) = cos(x - pi/2) -> index i-8; cos is even.
-__device__ __forceinline__ float sin32i(int i) {
-  int j = i - 8;
-  if (j < 0) j = -j;
-  return cos32(j);
-}
+__host__ __device__ constexpr float sin32i(int i) { return cos32(i >= 8 ? i - 8 : 8 - i); }
 
 __host__ __device__ constexpr int rev5(int i) {
   return ((i & 1) << 4) | ((i & 2) << 2) | (i & 4) | ((i & 8) >> 2) | ((i & 16) >> 4);
 }
 
-// In-place radix-2 decimation-in-frequency, forward (e^{-i...}).  Input natural order,
-// output bit-reversed: X[k] is left in element rev5(k).  Fully unrolled; all indices and
-// twiddles are compile-time, trivial twiddles cost no multiplies.
-__device__ __forceinline__ void fft32(float (&re)[32], float (&im)[32]) {
+// One radix-2 decimation-in-frequency stage of butterfly span kHalf.  The stage is a template argument so that
+// every index and twiddle is a compile-time constant: with a runtime `half` loop nvcc kept the stage loop rolled,
+// put re/im in local memory and looked the twiddles up through an indirect branch.  Products that feed a later
+// addition are rounded on their own (__fmul_rn): straight-line code would otherwise let nvcc contract them into
+// FMAs and change the result in the last bits.
+template <int kHalf>
+__device__ __forceinline__ void fft32_stage(float (&re)[32], float (&im)[32]) {
 #pragma unroll
-  for (int half = 16; half >= 1; half >>= 1) {
+  for (int base = 0; base < 32; base += 2 * kHalf) {
 #pragma unroll
-    for (int base = 0; base < 32; base += 2 * half) {
-#pragma unroll
-      for (int j = 0; j < half; ++j) {
-        const int a = base + j, b = a + half;
-        const float ar = re[a], ai = im[a], br = re[b], bi = im[b];
-        re[a] = ar + br;
-        im[a] = ai + bi;
-        const float dr = ar - br, di = ai - bi;
-        const int idx = j * (16 / half);  // twiddle W_32^idx = cos - i sin
-        if (idx == 0) {
-          re[b] = dr;
-          im[b] = di;
-        } else if (idx == 8) {  // * (-i)
-          re[b] = di;
-          im[b] = -dr;
-        } else if (idx == 4) {  // * (1 - i)/sqrt2
-          re[b] = (dr + di) * 0.70710678118654752440f;
-          im[b] = (di - dr) * 0.70710678118654752440f;
-        } else if (idx == 12) {  // * (-1 - i)/sqrt2
-          re[b] = (di - dr) * 0.70710678118654752440f;
-          im[b] = -(dr + di) * 0.70710678118654752440f;
-        } else {
-          const float c = cos32(idx), s = sin32i(idx);
-          re[b] = fmaf(dr, c, di * s);
-          im[b] = fmaf(di, c, -dr * s);
-        }
+    for (int j = 0; j < kHalf; ++j) {
+      const int a = base + j, b = a + kHalf;
+      const float ar = re[a], ai = im[a], br = re[b], bi = im[b];
+      re[a] = ar + br;
+      im[a] = ai + bi;
+      const float dr = ar - br, di = ai - bi;
+      const int idx = j * (16 / kHalf);  // twiddle W_32^idx = cos - i sin
+      if (idx == 0) {
+        re[b] = dr;
+        im[b] = di;
+      } else if (idx == 8) {  // * (-i)
+        re[b] = di;
+        im[b] = -dr;
+      } else if (idx == 4) {  // * (1 - i)/sqrt2
+        re[b] = __fmul_rn(dr + di, 0.70710678118654752440f);
+        im[b] = __fmul_rn(di - dr, 0.70710678118654752440f);
+      } else if (idx == 12) {  // * (-1 - i)/sqrt2
+        re[b] = __fmul_rn(di - dr, 0.70710678118654752440f);
+        im[b] = __fmul_rn(-(dr + di), 0.70710678118654752440f);
+      } else {
+        const float c = cos32(idx), s = sin32i(idx);
+        re[b] = fmaf(dr, c, di * s);
+        im[b] = fmaf(di, c, -dr * s);
       }
     }
   }
+}
+
+// In-place radix-2 decimation-in-frequency, forward (e^{-i...}).  Input natural order,
+// output bit-reversed: X[k] is left in element rev5(k).  Straight-line code; trivial
+// twiddles cost no multiplies.
+__device__ __forceinline__ void fft32(float (&re)[32], float (&im)[32]) {
+  fft32_stage<16>(re, im);
+  fft32_stage<8>(re, im);
+  fft32_stage<4>(re, im);
+  fft32_stage<2>(re, im);
+  fft32_stage<1>(re, im);
 }
 
 // ---------------------------------------------------------------- device: kernel
@@ -293,8 +302,8 @@ mel_kernel(const void* __restrict__ pcm, int n_samples, int hop, int T, int n_me
     for (int n1 = 0; n1 < 32; ++n1) {
       const float2 x = xf[32 * n1 + lane];
       const float2 w = wf[32 * n1 + lane];
-      re[n1] = x.x * w.x;
-      im[n1] = x.y * w.y;
+      re[n1] = __fmul_rn(x.x, w.x);  // not contracted into the first butterflies
+      im[n1] = __fmul_rn(x.y, w.y);
     }
     fft32(re, im);  // element i = Y[k1 = rev5(i)] for this n2
     // ---- twiddle W_1024^(n2*k1) and transpose to lane = k1, element = n2

@@ -38,13 +38,14 @@ LINE = re.compile(r"fused_phases H=(\d+) W=(\d+) cin=(\d+) cmid=(\d+) cout=(\d+)
                   r"tiles=(\d+)(.*)")
 
 
-def build_copy(tree, dst):
-    """The package and its import stub from `tree`, built into `dst` with the phase counters compiled in."""
+def build_copy(tree, dst, nvcc_flags="-DAM_FUSED_PHASES"):
+    """The package and its import stub from `tree`, built into `dst` with `nvcc_flags` (by default the phase
+    counters compiled in)."""
     for name in ("audiomuse-ai_b200", "include"):
         shutil.copytree(os.path.join(tree, name), os.path.join(dst, name), dirs_exist_ok=True,
                         ignore=shutil.ignore_patterns("*.so", "build", "__pycache__"))
     shutil.copy(os.path.join(tree, "audiomuse_ai_b200.py"), dst)
-    env = dict(os.environ, AM_EXTRA_NVCC_FLAGS="-DAM_FUSED_PHASES")
+    env = dict(os.environ, AM_EXTRA_NVCC_FLAGS=nvcc_flags)
     subprocess.run([sys.executable, os.path.join(dst, "audiomuse-ai_b200", "build_native.py")], env=env, check=True,
                    stdout=subprocess.DEVNULL)
 
