@@ -120,6 +120,7 @@ DEBUG_SIGNATURES = {
     "am_selftest_gemm": (_i, [_i, _i, _i, _i, _P(C.c_double)]),
     "am_bench_gemm": (_i, [_i, _i, _i, _i, _P(C.c_double)]),
     "am_probe_pipe": (_i, [_i, _i, _i, _P(C.c_double)]),
+    "am_debug_block": (_i, [_i] * 10 + [_vp] * 10 + [_P(_i)]),
 }
 
 _lib = None

@@ -21,6 +21,7 @@
 #include <cstdio>
 #include <memory>
 
+#include "depthwise.cuh"
 #include "encoder_generic.cuh"
 #include "fused_block.cuh"
 #include "gemm_wgmma.cuh"
@@ -40,7 +41,8 @@ struct Layer {
   DevBuf<float> bias;            // [cout_p]  (squeeze-excite: fc1 bias [cmid])
   DevBuf<float> aux0, aux1, aux2;  // stem / first conv: per-mel scale / shift (+ stem pw scale); squeeze-excite: fc2 [c, cmid], fc2 bias
   DevBuf<float> fused_params;    // 3x3 depthwise: its weights, bias and the preceding pointwise layer's bias per 64-channel chunk (fused::pack_params)
-  // true for the 3x3 / pad 1 / ReLU6 depthwise the packed-fp16 kernels implement
+  bool dw_fp16 = false;          // 3x3 depthwise: layer by layer, the packed-fp16 kernels cannot overflow on it (dw3x3_fp16_safe)
+  // true for the 3x3 / pad 1 / ReLU6 depthwise the packed-fp16 kernels and the fused block kernel implement
   bool dw_fast() const {
     return type == kDepthwise && kh == 3 && kw == 3 && pad_t == 1 && pad_b == 1 && pad_l == 1 && pad_r == 1 && act == kActRelu6;
   }
@@ -933,7 +935,10 @@ static int build_model(am_model* m, const ModelSpec& spec) {
       AM_TRY(upload(L->w_f32, wt));
       AM_TRY(upload(L->bias, padded(S.bias, L->cin_p)));
       if (L->dw_fast()) {  // the fused kernel's parameters; the expansion bias matters only when fused_block_at fuses it
-        const LayerSpec* E = li > 0 && spec.layers[li - 1].type == kPointwise ? &spec.layers[li - 1] : nullptr;
+        const LayerSpec& prev = spec.layers[li - 1];  // li > 0: the first layer is a stem or first convolution
+        const bool relu6_in = prev.act == kActRelu6 && (prev.type == kStem || prev.type == kConvFirst || prev.type == kPointwise);
+        L->dw_fp16 = dw3x3_fp16_safe(wt, padded(S.bias, L->cin_p), L->cin_p, relu6_in);
+        const LayerSpec* E = prev.type == kPointwise ? &prev : nullptr;
         const std::vector<float> b1 = E ? padded(E->bias, L->cin_p) : std::vector<float>();
         AM_TRY(upload(L->fused_params, fused::pack_params(wt, padded(S.bias, L->cin_p), E ? &b1 : nullptr, L->cin_p)));
       }
@@ -1026,6 +1031,53 @@ static int build_model(am_model* m, const ModelSpec& spec) {
 static int grid_for(int64_t total_threads) {
   const int64_t blocks = (total_threads + 255) / 256;
   return (int)std::max<int64_t>(1, std::min<int64_t>(blocks, (int64_t)sm_count() * 16));
+}
+
+bool dw3x3_fp16_safe(const std::vector<float>& w, const std::vector<float>& bias, int cp, bool relu6_input) {
+  if (!relu6_input) return false;
+  for (int c = 0; c < cp; ++c) {
+    double m = std::fabs((double)bias[(size_t)c]);
+    for (int t = 0; t < 9; ++t) m += 6.0 * std::fabs((double)w[(size_t)t * cp + c]);
+    if (!(m < 32768.0)) return false;  // NaN weights are not safe either
+  }
+  return true;
+}
+
+int dw3x3(const __nv_bfloat16* in, int B, int H, int W, int cp, int stride, const float* w, const float* bias, bool fp16,
+          __nv_bfloat16* out, cudaStream_t st, int* kernel) {
+  AM_CHECK(stride == 1 || stride == 2, "depthwise: stride %d", stride);
+  const int Ho = (H - 1) / stride + 1, Wo = (W - 1) / stride + 1;
+  AM_CHECK(B > 0 && H > 0 && W > 0 && cp % 8 == 0, "depthwise: empty input or channels not a multiple of 8");
+  if (!fp16) {
+    if (kernel) *kernel = kDwGeneric;
+    AM_LAUNCH(depthwise_generic_kernel, grid_for((int64_t)B * Ho * Wo * (cp / 8)), 256, 0, st, in, B, H, W, cp, Ho, Wo,
+              3, stride, 1, 1, w, bias, (int)kActRelu6, out);
+    return AM_OK;
+  }
+  const int strips = (Ho + kDwRows - 1) / kDwRows;
+  const int64_t total = (int64_t)B * strips * Wo * (cp / 8);
+  const unsigned grid = (unsigned)((total + kDwThreads - 1) / kDwThreads);
+  static const bool no_row = std::getenv("AM_DW_NO_ROW") != nullptr;
+  const int rstrips = (Ho + kDwRowR - 1) / kDwRowR;
+  const int64_t rtotal = (int64_t)B * rstrips * (cp / 8);
+  if (!no_row && W <= 16 && rtotal >= (int64_t)sm_count() * 8 * kDwThreads) {
+    // narrow late maps with enough (window, strip, channel group) work items to fill the GPU
+    if (kernel) *kernel = kDwRow;
+    const unsigned rgrid = (unsigned)((rtotal + kDwThreads - 1) / kDwThreads);
+    if (stride == 1) {
+      AM_LAUNCH(depthwise_row_kernel<1>, rgrid, kDwThreads, 0, st, in, B, H, W, cp, Ho, Wo, w, bias, out);
+    } else {
+      AM_LAUNCH(depthwise_row_kernel<2>, rgrid, kDwThreads, 0, st, in, B, H, W, cp, Ho, Wo, w, bias, out);
+    }
+  } else {
+    if (kernel) *kernel = kDwStrip;
+    if (stride == 1) {
+      AM_LAUNCH(depthwise_kernel<1>, grid, kDwThreads, 0, st, in, B, H, W, cp, Ho, Wo, w, bias, out);
+    } else {
+      AM_LAUNCH(depthwise_kernel<2>, grid, kDwThreads, 0, st, in, B, H, W, cp, Ho, Wo, w, bias, out);
+    }
+  }
+  return AM_OK;
 }
 
 // The trunk runs in two phases.  EARLY = stem + the leading layers whose input maps are large (at least
@@ -1145,31 +1197,8 @@ static int run_range(am_model* m, const float* mel_dev, const __nv_bfloat16* in,
                 l.pad_l, l.w_f32.p, l.bias.p, l.act, dst);
       s = o;
     } else if (l.type == kDepthwise) {
-      const Shape o = dw_out(l, s);
-      const int strips = (o.H + kDwRows - 1) / kDwRows;
-      const int64_t total = (int64_t)nb * strips * o.W * (l.cout_p / 8);
-      const unsigned grid = (unsigned)((total + kDwThreads - 1) / kDwThreads);
-      static const bool no_row = std::getenv("AM_DW_NO_ROW") != nullptr;
-      const int rstrips = (o.H + kDwRowR - 1) / kDwRowR;
-      const int64_t rtotal = (int64_t)nb * rstrips * (l.cout_p / 8);
-      if (!no_row && s.W <= 16 && rtotal >= (int64_t)sm_count() * 8 * kDwThreads) {
-        // narrow late maps with enough (window, strip, channel group) work items to fill the GPU
-        const unsigned rgrid = (unsigned)((rtotal + kDwThreads - 1) / kDwThreads);
-        if (l.stride == 1) {
-          AM_LAUNCH(depthwise_row_kernel<1>, rgrid, kDwThreads, 0, st, cur, nb, s.H, s.W, l.cin_p, o.H, o.W, l.w_f32.p,
-                    l.bias.p, dst);
-        } else {
-          AM_LAUNCH(depthwise_row_kernel<2>, rgrid, kDwThreads, 0, st, cur, nb, s.H, s.W, l.cin_p, o.H, o.W, l.w_f32.p,
-                    l.bias.p, dst);
-        }
-      } else if (l.stride == 1) {
-        AM_LAUNCH(depthwise_kernel<1>, grid, kDwThreads, 0, st, cur, nb, s.H, s.W, l.cin_p, o.H, o.W, l.w_f32.p,
-                  l.bias.p, dst);
-      } else {
-        AM_LAUNCH(depthwise_kernel<2>, grid, kDwThreads, 0, st, cur, nb, s.H, s.W, l.cin_p, o.H, o.W, l.w_f32.p,
-                  l.bias.p, dst);
-      }
-      s = o;
+      AM_TRY(dw3x3(cur, nb, s.H, s.W, l.cin_p, l.stride, l.w_f32.p, l.bias.p, l.dw_fp16, dst, st, nullptr));
+      s = dw_out(l, s);
     } else if (l.type == kSqueezeExcite) {
       const int HW = s.H * s.W;
       AM_TRY(m->se_mean.ensure((size_t)nb * l.cin));

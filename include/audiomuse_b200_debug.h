@@ -20,6 +20,19 @@ AM_API int am_bench_gemm(int M, int N, int K, int iters, double* ms_per_launch);
  * 3 HMNMX2 pair, 4 PRMT, 5 F2FP pack + add, 6 HFMA2 + PRMT) with `warps` warps per SM: cycles per warp-instruction
  * per SM sub-partition */
 AM_API int am_probe_pipe(int op, int warps, int iters, double* cycles_per_warp_instr_per_smsp);
+/* debug: one inverted-residual block [1x1 expand + bias + ReLU6] -> 3x3 depthwise (pad 1, stride) + bias + ReLU6 ->
+ * 1x1 project + bias [+ X], on host operands (bf16 as raw uint16, NHWC activations): X [B, H, W, cin_p],
+ * W1 [cmid_p, cin_p] + b1 [cmid_p] (NULL without an expansion, then cin_p == cmid_p), wd [9, cmid_p] + bd [cmid_p],
+ * W2 [cout_p, cmid_p] + b2 [cout_p] -> Y [B, Ho, Wo, cout_p].  Allocates, uploads, runs, synchronises, downloads.
+ *   path 0: the fused kernel as the encoder plans it; a block it rejects is an error and launches nothing.
+ *           *info = the ring depth of the plan.
+ *   path 1: layer by layer through the encoder's GEMM and depthwise dispatch; *info = the depthwise kernel (0 strip,
+ *           1 row, 2 fp32 generic).  E_out [B, H, W, cmid_p] and D_out [B, Ho, Wo, cmid_p] (may be NULL) receive the
+ *           expanded and depthwise tensors. */
+AM_API int am_debug_block(int path, int B, int H, int W, int cin_p, int cmid_p, int cout_p, int stride, int has_expand,
+                          int residual, const uint16_t* X, const uint16_t* W1, const float* b1, const float* wd,
+                          const float* bd, const uint16_t* W2, const float* b2, uint16_t* Y, uint16_t* E_out,
+                          uint16_t* D_out, int* info);
 
 #ifdef __cplusplus
 }
