@@ -112,6 +112,12 @@ SIGNATURES = {
     "am_spectral_plan_residuals": (_i, [_vp, _vp, _vp, _i, _vp, _vp]),
     "am_spectral_plan_embed": (_i, [_vp, _vp, _i, _vp]),
     "am_spectral_plan_free": (None, [_vp]),
+    "am_spectral_plan_create_csr": (_i, [_vp, _vp, _vp, _i64, _i, _u64, _P(_vp)]),
+    "am_umap_plan_create": (_i, [_vp, _i64, _i, _i, _i, _P(_vp)]),
+    "am_umap_plan_info": (_i, [_vp, _P(_i64), _P(_i), _P(_i), _P(_f), _P(_f), _P(_f)]),
+    "am_umap_plan_graph": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "am_umap_plan_layout": (_i, [_vp, _vp, _i, C.c_double, C.c_double, C.c_double, C.c_double, C.c_double, _u64]),
+    "am_umap_plan_free": (None, [_vp]),
 }
 
 # include/audiomuse_b200_debug.h: probes and self tests, in libaudiomuse_b200_debug.so only

@@ -322,25 +322,7 @@ def spectral_embedding(X, n_components, n_neighbors=10, seed=0, tol=1e-8, max_it
                                            C.byref(plan)))
     try:
         t0 = time.perf_counter()
-        G, H = np.empty((b, b)), np.empty((b, b))
-        res = np.full(k, np.inf)
-        Q, cut, it = None, None, 0
-        while True:
-            if it == max_iter:
-                raise RuntimeError(f"spectral eigensolver did not converge in {max_iter} iterations "
-                                   f"(largest residual {res.max():.3g} > tol {tol:g})")
-            degree = 0 if cut is None else _cheb_degree(cut)
-            _lib.check(lib.am_spectral_plan_iterate(plan, None if Q is None else _lib.ptr(Q), degree,
-                                                    0.0 if cut is None else cut, _lib.ptr(G), _lib.ptr(H)))
-            it += 1
-            theta, Q = _rayleigh_ritz(G, H)
-            Qk, thk = np.ascontiguousarray(Q[:, :k]), np.ascontiguousarray(theta[:k])
-            _lib.check(lib.am_spectral_plan_residuals(plan, _lib.ptr(Qk), _lib.ptr(thk), k, _lib.ptr(res), None))
-            if np.all(res <= tol):
-                break
-            cut = float(np.clip(theta[-1], -1.0 + 1e-12, 1.0 - 1e-12))   # damp everything below the block
-        emb = np.empty((N, k), dtype=np.float64)
-        _lib.check(lib.am_spectral_plan_embed(plan, _lib.ptr(Qk), k, _lib.ptr(emb)))
+        emb, thk, res, it = _solve_plan(lib, plan, N, b, k, tol, max_iter)
         eig_s = time.perf_counter() - t0
         if details is not None:
             nnz, blk, n_spmm = C.c_int64(0), C.c_int(0), C.c_int64(0)
@@ -353,12 +335,72 @@ def spectral_embedding(X, n_components, n_neighbors=10, seed=0, tol=1e-8, max_it
             details["affinity"], details["dd"] = _spectral_graph(lib, plan, N, int(nnz.value))
     finally:
         lib.am_spectral_plan_free(plan)
-    # sklearn.utils.extmath._deterministic_vector_sign_flip on the (n_components, N) layout
+    return _sign_flip(emb), 1.0 - thk
+
+
+def spectral_embedding_csr(W, n_components, seed=0, tol=1e-8, max_iter=300, details=None):
+    """spectral_embedding's eigensolver on a given graph: W a symmetric scipy sparse matrix with positive weights and
+    no empty row (float64 on the device).  -> (embedding f64[N, n_components], eigenvalues of L_sym ascending), the
+    embedding divided by sqrt(deg) and sign-flipped as spectral_embedding's.  details (optional) receives the outer
+    iterations, the residuals and the solver time."""
+    import scipy.sparse as sp
+    W = sp.csr_matrix(W, dtype=np.float64)
+    W.sort_indices()
+    N = W.shape[0]
+    k = int(n_components)
+    if W.shape != (N, N) or not 1 <= k <= N:
+        raise ValueError(f"need a square graph and 1 <= n_components <= N (got {W.shape}, {n_components})")
+    indptr = np.ascontiguousarray(W.indptr, dtype=np.int64)
+    indices = np.ascontiguousarray(W.indices, dtype=np.int32)
+    data = np.ascontiguousarray(W.data, dtype=np.float64)
+    lib = _lib.load()
+    b = _spectral_block(k, N)
+    plan = C.c_void_p()
+    _lib.check(lib.am_spectral_plan_create_csr(_lib.ptr(indptr), _lib.ptr(indices), _lib.ptr(data), N, b,
+                                               int(seed) & 0xFFFFFFFFFFFFFFFF, C.byref(plan)))
+    try:
+        t0 = time.perf_counter()
+        emb, thk, res, it = _solve_plan(lib, plan, N, b, k, tol, max_iter)
+        if details is not None:
+            details.update(block=b, outer_iterations=it, residuals=res.copy(),
+                           eigensolver_ms=1e3 * (time.perf_counter() - t0))
+    finally:
+        lib.am_spectral_plan_free(plan)
+    return _sign_flip(emb), 1.0 - thk
+
+
+def _solve_plan(lib, plan, N, b, k, tol, max_iter):
+    """The outer loop shared by both plan kinds: filter, Rayleigh-Ritz on the host, rotate, until every wanted Ritz
+    pair has a residual <= tol.  -> (V Q / dd f64[N, k], theta descending f64[k], residuals, outer iterations)"""
+    G, H = np.empty((b, b)), np.empty((b, b))
+    res = np.full(k, np.inf)
+    Q, cut, it = None, None, 0
+    while True:
+        if it == max_iter:
+            raise RuntimeError(f"spectral eigensolver did not converge in {max_iter} iterations "
+                               f"(largest residual {res.max():.3g} > tol {tol:g})")
+        degree = 0 if cut is None else _cheb_degree(cut)
+        _lib.check(lib.am_spectral_plan_iterate(plan, None if Q is None else _lib.ptr(Q), degree,
+                                                0.0 if cut is None else cut, _lib.ptr(G), _lib.ptr(H)))
+        it += 1
+        theta, Q = _rayleigh_ritz(G, H)
+        Qk, thk = np.ascontiguousarray(Q[:, :k]), np.ascontiguousarray(theta[:k])
+        _lib.check(lib.am_spectral_plan_residuals(plan, _lib.ptr(Qk), _lib.ptr(thk), k, _lib.ptr(res), None))
+        if np.all(res <= tol):
+            break
+        cut = float(np.clip(theta[-1], -1.0 + 1e-12, 1.0 - 1e-12))   # damp everything below the block
+    emb = np.empty((N, k), dtype=np.float64)
+    _lib.check(lib.am_spectral_plan_embed(plan, _lib.ptr(Qk), k, _lib.ptr(emb)))
+    return emb, thk, res, it
+
+
+def _sign_flip(emb):
+    """sklearn.utils.extmath._deterministic_vector_sign_flip on the (n_components, N) layout"""
     top = np.argmax(np.abs(emb), axis=0)
-    signs = np.sign(emb[top, np.arange(k)])
+    signs = np.sign(emb[top, np.arange(emb.shape[1])])
     signs[signs == 0] = 1.0
     emb *= signs[None, :]
-    return emb, 1.0 - thk
+    return emb
 
 
 def spectral_graph(X, n_neighbors=10):

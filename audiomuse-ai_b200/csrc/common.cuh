@@ -166,6 +166,16 @@ struct Stream {
 inline size_t round_up(size_t x, size_t m) { return (x + m - 1) / m * m; }
 inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 
+// ---------------------------------------------------------------- symmetrised k-NN graphs (spectral.cu)
+// CSR of k-NN lists ids i64[N, k] (device; a row's own id and ids outside [0, N) are skipped), columns ascending per
+// row.  memb == nullptr: the affinity 0.5 (C + C^T) into w32 (0.5 or 1) and dd = sqrt(row sums).  memb f64[N, k] (a
+// value per list entry): the fuzzy union A + A^T - A o A^T into w64.  Allocates the outputs; synchronises.
+int knn_csr_build(const int64_t* ids, const double* memb, int64_t N, int k, cudaStream_t st, DevBuf<int64_t>& indptr,
+                  DevBuf<int32_t>& indices, DevBuf<float>* w32, DevBuf<double>* dd, DevBuf<double>* w64,
+                  int64_t* nnz);
+// exclusive scan of cnt i32[N] into off i64[N + 1] (off[N] = the total), stream-ordered
+int csr_scan(const int* cnt, int64_t N, int64_t* off, cudaStream_t st);
+
 // ---------------------------------------------------------------- device helpers
 #ifdef __CUDACC__
 __device__ __forceinline__ float warp_sum(float v) {

@@ -13,6 +13,8 @@
 //                            is an edge in both lists (weight 1), once an edge in one list (weight 0.5)
 //   compact_rows_kernel      merge -> CSR indices i32 / weights f32, deg and dd in float64
 //   normalise_kernel         s_ij = w_ij / dd_j / dd_i (scipy's order), float64: the values of S = D^-1/2 W D^-1/2
+// The same count / scan / scatter / sort / compact steps build UMAP's fuzzy union (knn_csr_build with memberships,
+// called from umap.cu); am_spectral_plan_create_csr starts from a given float64 graph (degree_kernel for dd).
 //
 // Eigensolver steps, float64 throughout (the wanted eigenvalues can be packed 1e-3 apart, so the block is never
 // rounded to fp32):
@@ -87,21 +89,26 @@ __global__ void __launch_bounds__(1024) scan_kernel(const int* __restrict__ cnt,
   }
 }
 
+// memb (optional): a value per list entry, carried with both directions into raw_v
 __global__ void scatter_edges_kernel(const int64_t* __restrict__ ids, int64_t N, int k, const int64_t* __restrict__ off,
-                                     int* __restrict__ cursor, int32_t* __restrict__ raw) {
+                                     int* __restrict__ cursor, int32_t* __restrict__ raw, const double* __restrict__ memb,
+                                     double* __restrict__ raw_v) {
   const int64_t total = N * k;
   for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (int64_t)gridDim.x * blockDim.x) {
     const int64_t i = e / k, j = ids[e];
     if (j == i || j < 0 || j >= N) continue;
-    raw[off[i] + atomicAdd(&cursor[i], 1)] = (int32_t)j;
-    raw[off[j] + atomicAdd(&cursor[j], 1)] = (int32_t)i;
+    const int64_t pi = off[i] + atomicAdd(&cursor[i], 1), pj = off[j] + atomicAdd(&cursor[j], 1);
+    raw[pi] = (int32_t)j;
+    raw[pj] = (int32_t)i;
+    if (memb) raw_v[pi] = raw_v[pj] = memb[e];
   }
 }
 
-// one warp per row: rank sort of the row's columns (ties by position) into `sorted`, and the number of distinct columns
+// one warp per row: rank sort of the row's columns (ties by position) into `sorted` (and raw_v's values, when given,
+// into sorted_v), and the number of distinct columns
 __global__ void __launch_bounds__(256)
 sort_rows_kernel(const int64_t* __restrict__ off, int64_t N, const int32_t* __restrict__ raw, int32_t* __restrict__ sorted,
-                 int* __restrict__ ucnt) {
+                 int* __restrict__ ucnt, const double* __restrict__ raw_v, double* __restrict__ sorted_v) {
   const int lane = threadIdx.x & 31;
   const int64_t warps = (int64_t)gridDim.x * (blockDim.x >> 5);
   for (int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); row < N; row += warps) {
@@ -117,6 +124,7 @@ sort_rows_kernel(const int64_t* __restrict__ off, int64_t N, const int32_t* __re
         rank += (y < x) || (y == x && q < p);
       }
       o[rank] = x;
+      if (raw_v) sorted_v[base + rank] = raw_v[base + p];
     }
     __syncwarp();
     int u = 0;
@@ -127,12 +135,15 @@ sort_rows_kernel(const int64_t* __restrict__ off, int64_t N, const int32_t* __re
   }
 }
 
-// one warp per row: distinct columns -> CSR, weight 1 for a column present twice (i in j's list and j in i's), 0.5
-// otherwise; deg = the row sum (exact: multiples of 0.5), dd = sqrt(deg)
+// one warp per row: distinct columns -> CSR.  Affinity (kFuzzy false): weight 1 for a column present twice (i in j's
+// list and j in i's), 0.5 otherwise; deg = the row sum (exact: multiples of 0.5), dd = sqrt(deg).  Fuzzy union (kFuzzy
+// true, UMAP's W = A + A^T - A o A^T): from the carried memberships, a + b - a b for a column present twice (the same
+// value in either order), a for one present once, into w64; w and dd are not written.
+template <bool kFuzzy>
 __global__ void __launch_bounds__(256)
 compact_rows_kernel(const int64_t* __restrict__ off, int64_t N, const int32_t* __restrict__ sorted,
                     const int64_t* __restrict__ indptr, int32_t* __restrict__ indices, float* __restrict__ w,
-                    double* __restrict__ dd) {
+                    double* __restrict__ dd, const double* __restrict__ sorted_v, double* __restrict__ w64) {
   const int lane = threadIdx.x & 31;
   const int64_t warps = (int64_t)gridDim.x * (blockDim.x >> 5);
   for (int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); row < N; row += warps) {
@@ -148,22 +159,43 @@ compact_rows_kernel(const int64_t* __restrict__ off, int64_t N, const int32_t* _
       const bool first = valid && (p == 0 || s[p - 1] != x);
       const unsigned m = __ballot_sync(0xffffffffu, first);
       if (first) {
-        const float wt = (p + 1 < L && s[p + 1] == x) ? 1.0f : 0.5f;
+        const bool twice = p + 1 < L && s[p + 1] == x;
         const int64_t pos = out + __popc(m & ((1u << lane) - 1u));
         indices[pos] = x;
-        w[pos] = wt;
-        deg += wt;
+        if (kFuzzy) {
+          const double a = sorted_v[base + p], b = twice ? sorted_v[base + p + 1] : 0.0;
+          w64[pos] = twice ? a + b - a * b : a;
+        } else {
+          const float wt = twice ? 1.0f : 0.5f;
+          w[pos] = wt;
+          deg += wt;
+        }
       }
       out += __popc(m);
     }
+    if (kFuzzy) continue;
     deg = warp_sum(deg);
     if (lane == 0) dd[row] = sqrt(deg);
   }
 }
 
+// one warp per row: deg = the row sum of a float64 W (lanes strided over the row, then a fixed shuffle tree), dd = sqrt
+__global__ void __launch_bounds__(256)
+degree_kernel(const int64_t* __restrict__ indptr, int64_t N, const double* __restrict__ w, double* __restrict__ dd) {
+  const int lane = threadIdx.x & 31;
+  const int64_t warps = (int64_t)gridDim.x * (blockDim.x >> 5);
+  for (int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); row < N; row += warps) {
+    double deg = 0.0;
+    for (int64_t p = indptr[row] + lane; p < indptr[row + 1]; p += 32) deg += w[p];
+    deg = warp_sum(deg);
+    if (lane == 0) dd[row] = sqrt(deg);
+  }
+}
+
+template <typename T>
 __global__ void __launch_bounds__(256)
 normalise_kernel(const int64_t* __restrict__ indptr, int64_t N, const int32_t* __restrict__ indices,
-                 const float* __restrict__ w, const double* __restrict__ dd, double* __restrict__ s) {
+                 const T* __restrict__ w, const double* __restrict__ dd, double* __restrict__ s) {
   const int lane = threadIdx.x & 31;
   const int64_t warps = (int64_t)gridDim.x * (blockDim.x >> 5);
   for (int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); row < N; row += warps) {
@@ -397,11 +429,75 @@ int upload_q(am_spectral_plan* p, const double* Q, int ncols) {
   return AM_OK;
 }
 
+// the block buffers and the seeded start block V (synchronises)
+int init_block(am_spectral_plan* p, uint64_t seed) {
+  const size_t blk = (size_t)p->N * p->ld;
+  AM_TRY(p->V.alloc(blk));
+  AM_TRY(p->Y.alloc(blk));
+  AM_TRY(p->SV.alloc(blk));
+  AM_TRY(p->red.alloc((size_t)2 * p->b * p->b));
+  AM_LAUNCH(init_block_kernel, flat_grid((int64_t)blk), 256, 0, p->st.s, p->V.p, p->N, p->b, p->ld, seed);
+  AM_CUDA(cudaStreamSynchronize(p->st.s));
+  return AM_OK;
+}
+
 dim3 rowmul_grid(const am_spectral_plan* p, int ncols) {
   return dim3((unsigned)((p->N + kRotRows - 1) / kRotRows), (unsigned)ceil_div(ncols, 32));
 }
 
 }  // namespace sp
+
+int csr_scan(const int* cnt, int64_t N, int64_t* off, cudaStream_t st) {
+  AM_LAUNCH(sp::scan_kernel, 1, 1024, 0, st, cnt, N, off);
+  return AM_OK;
+}
+
+int knn_csr_build(const int64_t* ids, const double* memb, int64_t N, int k, cudaStream_t st, DevBuf<int64_t>& indptr,
+                  DevBuf<int32_t>& indices, DevBuf<float>* w32, DevBuf<double>* dd, DevBuf<double>* w64, int64_t* nnz) {
+  const bool fuzzy = memb != nullptr;
+  DevBuf<int64_t> off;
+  DevBuf<int> cnt, cursor;
+  DevBuf<int32_t> raw, sorted;
+  DevBuf<double> raw_v, sorted_v;
+  AM_TRY(cnt.alloc((size_t)N));
+  AM_TRY(cursor.alloc((size_t)N));
+  AM_TRY(off.alloc((size_t)N + 1));
+  AM_TRY(indptr.alloc((size_t)N + 1));
+  if (!fuzzy) AM_TRY(dd->alloc((size_t)N));
+  AM_CUDA(cudaMemsetAsync(cnt.p, 0, (size_t)N * 4, st));
+  AM_CUDA(cudaMemsetAsync(cursor.p, 0, (size_t)N * 4, st));
+  const int eg = sp::flat_grid(N * k), rg = sp::row_grid(N);
+  AM_LAUNCH(sp::count_edges_kernel, eg, 256, 0, st, ids, N, k, cnt.p);
+  AM_LAUNCH(sp::scan_kernel, 1, 1024, 0, st, cnt.p, N, off.p);
+  int64_t raw_nnz = 0;
+  AM_CUDA(cudaMemcpyAsync(&raw_nnz, off.p + N, 8, cudaMemcpyDeviceToHost, st));
+  AM_CUDA(cudaStreamSynchronize(st));
+  AM_TRY(raw.alloc((size_t)std::max<int64_t>(1, raw_nnz)));
+  AM_TRY(sorted.alloc((size_t)std::max<int64_t>(1, raw_nnz)));
+  if (fuzzy) {
+    AM_TRY(raw_v.alloc((size_t)std::max<int64_t>(1, raw_nnz)));
+    AM_TRY(sorted_v.alloc((size_t)std::max<int64_t>(1, raw_nnz)));
+  }
+  AM_LAUNCH(sp::scatter_edges_kernel, eg, 256, 0, st, ids, N, k, off.p, cursor.p, raw.p, memb, raw_v.p);
+  AM_LAUNCH(sp::sort_rows_kernel, rg, 256, 0, st, off.p, N, raw.p, sorted.p, cnt.p, raw_v.p, sorted_v.p);
+  AM_LAUNCH(sp::scan_kernel, 1, 1024, 0, st, cnt.p, N, indptr.p);
+  AM_CUDA(cudaMemcpyAsync(nnz, indptr.p + N, 8, cudaMemcpyDeviceToHost, st));
+  AM_CUDA(cudaStreamSynchronize(st));
+  AM_TRY(indices.alloc((size_t)std::max<int64_t>(1, *nnz)));
+  if (fuzzy) {
+    AM_TRY(w64->alloc((size_t)std::max<int64_t>(1, *nnz)));
+    AM_LAUNCH(sp::compact_rows_kernel<true>, rg, 256, 0, st, off.p, N, sorted.p, indptr.p, indices.p, nullptr, nullptr,
+              sorted_v.p, w64->p);
+  } else {
+    AM_TRY(w32->alloc((size_t)std::max<int64_t>(1, *nnz)));
+    AM_LAUNCH(sp::compact_rows_kernel<false>, rg, 256, 0, st, off.p, N, sorted.p, indptr.p, indices.p, w32->p, dd->p,
+              nullptr, nullptr);
+  }
+  // the scratch buffers are freed on return: finish with them first
+  AM_CUDA(cudaStreamSynchronize(st));
+  return AM_OK;
+}
+
 }  // namespace am
 
 using namespace am;
@@ -439,9 +535,7 @@ extern "C" int am_spectral_plan_create(const float* X, int64_t N, int d, int n_n
   }
   auto body = [&]() -> int {
     DevBuf<float> dX, dist;
-    DevBuf<int64_t> ids, off;
-    DevBuf<int> cnt, cursor;
-    DevBuf<int32_t> raw, sorted;
+    DevBuf<int64_t> ids;
     AM_TRY(dX.alloc((size_t)N * d));
     AM_CUDA(cudaMemcpyAsync(dX.p, X, (size_t)N * d * 4, cudaMemcpyHostToDevice, st));
     AM_TRY(ids.alloc((size_t)N * n_neighbors));
@@ -455,39 +549,12 @@ extern "C" int am_spectral_plan_create(const float* X, int64_t N, int d, int n_n
       AM_TRY(qs);
     }
     AM_CUDA(cudaEventRecord(ev[1], st));
-    AM_TRY(cnt.alloc((size_t)N));
-    AM_TRY(cursor.alloc((size_t)N));
-    AM_TRY(off.alloc((size_t)N + 1));
-    AM_TRY(p->indptr.alloc((size_t)N + 1));
-    AM_TRY(p->dd.alloc((size_t)N));
-    AM_CUDA(cudaMemsetAsync(cnt.p, 0, (size_t)N * 4, st));
-    AM_CUDA(cudaMemsetAsync(cursor.p, 0, (size_t)N * 4, st));
-    const int eg = sp::flat_grid(N * n_neighbors), rg = sp::row_grid(N);
-    AM_LAUNCH(sp::count_edges_kernel, eg, 256, 0, st, ids.p, N, n_neighbors, cnt.p);
-    AM_LAUNCH(sp::scan_kernel, 1, 1024, 0, st, cnt.p, N, off.p);
-    int64_t raw_nnz = 0;
-    AM_CUDA(cudaMemcpyAsync(&raw_nnz, off.p + N, 8, cudaMemcpyDeviceToHost, st));
-    AM_CUDA(cudaStreamSynchronize(st));
-    AM_TRY(raw.alloc((size_t)std::max<int64_t>(1, raw_nnz)));
-    AM_TRY(sorted.alloc((size_t)std::max<int64_t>(1, raw_nnz)));
-    AM_LAUNCH(sp::scatter_edges_kernel, eg, 256, 0, st, ids.p, N, n_neighbors, off.p, cursor.p, raw.p);
-    AM_LAUNCH(sp::sort_rows_kernel, rg, 256, 0, st, off.p, N, raw.p, sorted.p, cnt.p);
-    AM_LAUNCH(sp::scan_kernel, 1, 1024, 0, st, cnt.p, N, p->indptr.p);
-    AM_CUDA(cudaMemcpyAsync(&p->nnz, p->indptr.p + N, 8, cudaMemcpyDeviceToHost, st));
-    AM_CUDA(cudaStreamSynchronize(st));
-    AM_TRY(p->indices.alloc((size_t)std::max<int64_t>(1, p->nnz)));
-    AM_TRY(p->w.alloc((size_t)std::max<int64_t>(1, p->nnz)));
+    AM_TRY(knn_csr_build(ids.p, nullptr, N, n_neighbors, st, p->indptr, p->indices, &p->w, &p->dd, nullptr, &p->nnz));
     AM_TRY(p->s.alloc((size_t)std::max<int64_t>(1, p->nnz)));
-    AM_LAUNCH(sp::compact_rows_kernel, rg, 256, 0, st, off.p, N, sorted.p, p->indptr.p, p->indices.p, p->w.p, p->dd.p);
-    AM_LAUNCH(sp::normalise_kernel, rg, 256, 0, st, p->indptr.p, N, p->indices.p, p->w.p, p->dd.p, p->s.p);
+    AM_LAUNCH(sp::normalise_kernel<float>, sp::row_grid(N), 256, 0, st, p->indptr.p, N, p->indices.p, p->w.p, p->dd.p,
+              p->s.p);
     AM_CUDA(cudaEventRecord(ev[2], st));
-    const size_t blk = (size_t)N * p->ld;
-    AM_TRY(p->V.alloc(blk));
-    AM_TRY(p->Y.alloc(blk));
-    AM_TRY(p->SV.alloc(blk));
-    AM_TRY(p->red.alloc((size_t)2 * p->b * p->b));
-    AM_LAUNCH(sp::init_block_kernel, sp::flat_grid((int64_t)blk), 256, 0, st, p->V.p, N, p->b, p->ld, seed);
-    AM_CUDA(cudaStreamSynchronize(st));
+    AM_TRY(sp::init_block(p, seed));
     AM_CUDA(cudaEventElapsedTime(&p->knn_ms, ev[0], ev[1]));
     AM_CUDA(cudaEventElapsedTime(&p->graph_ms, ev[1], ev[2]));
     return AM_OK;
@@ -495,6 +562,54 @@ extern "C" int am_spectral_plan_create(const float* X, int64_t N, int d, int n_n
   s = body();
   for (auto& e : ev) cudaEventDestroy(e);
   if (s != AM_OK) return fail(s);
+  *out = p;
+  return AM_OK;
+}
+
+extern "C" int am_spectral_plan_create_csr(const int64_t* indptr, const int32_t* indices, const double* weights,
+                                           int64_t N, int block, uint64_t seed, am_spectral_plan** out) {
+  AM_CHECK(indptr && out && N >= 1, "am_spectral_plan_create_csr: bad argument (need indptr, out, N >= 1)");
+  AM_CHECK(N <= (int64_t)INT32_MAX, "am_spectral_plan_create_csr: N = %lld exceeds 2^31 - 1", (long long)N);
+  AM_CHECK(block >= 1 && block <= N, "am_spectral_plan_create_csr: block = %d outside [1, N = %lld]", block,
+           (long long)N);
+  const int64_t nnz = indptr[N];
+  AM_CHECK(indptr[0] == 0 && nnz >= 0 && (nnz == 0 || (indices && weights)),
+           "am_spectral_plan_create_csr: bad CSR (indptr[0] must be 0; indices and weights needed when nnz > 0)");
+  for (int64_t i = 0; i < N; ++i)
+    AM_CHECK(indptr[i + 1] > indptr[i], "am_spectral_plan_create_csr: row %lld is empty (zero degree)", (long long)i);
+  for (int64_t e = 0; e < nnz; ++e)
+    AM_CHECK(indices[e] >= 0 && indices[e] < N && weights[e] > 0.0 && std::isfinite(weights[e]),
+             "am_spectral_plan_create_csr: entry %lld has a column outside [0, N) or a weight that is not finite and "
+             "positive", (long long)e);
+  *out = nullptr;
+  AM_TRY(ensure_init());
+  auto* p = new am_spectral_plan();
+  p->N = N;
+  p->b = block;
+  p->ld = (int)round_up((size_t)block, 32);
+  p->nnz = nnz;
+  auto body = [&]() -> int {
+    AM_TRY(p->st.create());
+    cudaStream_t st = p->st.s;
+    DevBuf<double> w;
+    AM_TRY(p->indptr.alloc((size_t)N + 1));
+    AM_TRY(p->indices.alloc((size_t)nnz));
+    AM_TRY(w.alloc((size_t)nnz));
+    AM_TRY(p->s.alloc((size_t)nnz));
+    AM_TRY(p->dd.alloc((size_t)N));
+    AM_CUDA(cudaMemcpyAsync(p->indptr.p, indptr, ((size_t)N + 1) * 8, cudaMemcpyHostToDevice, st));
+    AM_CUDA(cudaMemcpyAsync(p->indices.p, indices, (size_t)nnz * 4, cudaMemcpyHostToDevice, st));
+    AM_CUDA(cudaMemcpyAsync(w.p, weights, (size_t)nnz * 8, cudaMemcpyHostToDevice, st));
+    AM_LAUNCH(sp::degree_kernel, sp::row_grid(N), 256, 0, st, p->indptr.p, N, w.p, p->dd.p);
+    AM_LAUNCH(sp::normalise_kernel<double>, sp::row_grid(N), 256, 0, st, p->indptr.p, N, p->indices.p, w.p, p->dd.p,
+              p->s.p);
+    return sp::init_block(p, seed);  // synchronises before w is freed
+  };
+  const int s = body();
+  if (s != AM_OK) {
+    delete p;
+    return s;
+  }
   *out = p;
   return AM_OK;
 }
@@ -512,6 +627,7 @@ extern "C" int am_spectral_plan_info(const am_spectral_plan* p, int64_t* nnz, in
 
 extern "C" int am_spectral_plan_graph(am_spectral_plan* p, int64_t* indptr, int32_t* indices, float* data, double* dd) {
   AM_CHECK(p, "am_spectral_plan_graph: NULL plan");
+  AM_CHECK(!data || !p->nnz || p->w.p, "am_spectral_plan_graph: a plan made from a CSR keeps no float32 W");
   cudaStream_t st = p->st.s;
   if (indptr) AM_CUDA(cudaMemcpyAsync(indptr, p->indptr.p, ((size_t)p->N + 1) * 8, cudaMemcpyDeviceToHost, st));
   if (indices && p->nnz) AM_CUDA(cudaMemcpyAsync(indices, p->indices.p, (size_t)p->nnz * 4, cudaMemcpyDeviceToHost, st));

@@ -51,13 +51,15 @@ METRIC_NAMES = ("silhouette_score", "davies_bouldin_score", "calinski_harabasz_s
 
 
 def apply(clap=None, voyager_manager=None, clustering=None, allow_sklearn_fallback: bool = True,
-          clustering_helper=None) -> None:
+          clustering_helper=None, song_alchemy=None, app_map=None) -> None:
     """clap / voyager_manager / clustering / clustering_helper: the reference's already imported tasks.* modules (pass
     only the ones to patch).  allow_sklearn_fallback keeps the reference's contract that a failing GPU k-means silently
     falls back to scikit-learn (tasks/clustering_gpu.py:130-148); this repository's own tests run with it off so a
     missing CUDA library can never pass as the GPU path.  clustering_helper imports the three scores by name at module
     level (tasks/clustering_helper.py:16) and looks them up at call time (:462-470), so replacing the module attributes
-    moves the fitness scoring to the GPU."""
+    moves the fitness scoring to the GPU.  song_alchemy / app_map get the GPU UMAP projection as _project_with_umap:
+    app_helper imports it from tasks.song_alchemy at call time (app_helper.py:1320, 1437), app_map binds it when it is
+    imported (app_map.py:13), so both modules are patched."""
     if clap is not None:
         from . import clap_analyzer as b200_clap
 
@@ -78,5 +80,10 @@ def apply(clap=None, voyager_manager=None, clustering=None, allow_sklearn_fallba
 
         for name in METRIC_NAMES:
             setattr(clustering_helper, name, getattr(b200_cm, name))
+    for mod in (song_alchemy, app_map):
+        if mod is not None:
+            from . import projection
+
+            mod._project_with_umap = projection.project_with_umap
     if (clustering is not None or clustering_helper is not None) and allow_sklearn_fallback:
         os.environ.setdefault("B200_ALLOW_SKLEARN_FALLBACK", "1")

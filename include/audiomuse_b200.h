@@ -305,6 +305,38 @@ AM_API int am_spectral_plan_residuals(am_spectral_plan* plan, const double* Q, c
                                       double* res, double* norms);
 AM_API int am_spectral_plan_embed(am_spectral_plan* plan, const double* Q, int ncols, double* out);
 AM_API void am_spectral_plan_free(am_spectral_plan* plan);
+/* A plan over a given symmetric graph instead of a k-NN graph: indptr i64[N + 1], indices i32[nnz], weights f64[nnz]
+ * (host; every row non-empty, every weight finite and > 0, the matrix symmetric).  dd = sqrt(row sums) and S are
+ * computed in float64; _iterate / _residuals / _embed work as above (_info reports no k-NN or CSR time, and _graph
+ * copies no data: the caller owns the graph).  Serves UMAP's spectral initialisation. */
+AM_API int am_spectral_plan_create_csr(const int64_t* indptr, const int32_t* indices, const double* weights, int64_t N,
+                                       int block, uint64_t seed, am_spectral_plan** out);
+
+/* ------------------------------------------------------------------ UMAP graph + layout
+ * Replaces umap.UMAP(n_components=2).fit_transform behind tasks/song_alchemy._project_with_umap (:272-287).  The plan
+ * holds umap-learn 0.5's fuzzy simplicial set of X, pruned for n_epochs, and runs the SGD layout; the host fits a, b and
+ * computes the spectral initialisation (audiomuse-ai_b200/projection.py).  Every call is synchronous; a plan is used by
+ * one thread at a time.
+ *   _create      X f32[N, d] (host), N >= 2, 1 <= n_neighbors <= N (the row itself counts as its first neighbour),
+ *                n_epochs >= 1 (no seed: nothing in the graph is random; _layout takes it).  k-NN: exact euclidean (am_knn_query), distances recomputed in float64.  rho, sigma:
+ *                smooth_knn_dist (local_connectivity 1); W = A + A^T - A o A^T; entries with w < max(w) / n_epochs
+ *                dropped; epochs_per_sample = n_epochs / (n_epochs w / max(w))
+ *   _info        nnz of the pruned W, n_neighbors, n_epochs, device ms of the k-NN, the graph and the last layout
+ *   _graph       the pruned W as CSR (indptr i64[N + 1], indices i32[nnz] ascending per row, weights f64[nnz]), rho and
+ *                sigma f64[N], epochs_per_sample f64[nnz]; each pointer optional
+ *   _layout      emb f32[N, 2] in/out: the first `epochs` epochs (0 <= epochs <= n_epochs) of the n_epochs schedule,
+ *                learning rate alpha0 (1 - n / n_epochs), curve a, b, repulsion gamma, neg_rate negative samples per
+ *                sample.  Per-vertex updates from the previous epoch's embedding, negative samples from a hash of
+ *                (seed, epoch, entry, sample): one seed gives bit-identical output on every call */
+typedef struct am_umap_plan am_umap_plan;
+AM_API int am_umap_plan_create(const float* X, int64_t N, int d, int n_neighbors, int n_epochs, am_umap_plan** out);
+AM_API int am_umap_plan_info(const am_umap_plan* plan, int64_t* nnz, int* n_neighbors, int* n_epochs, float* knn_ms,
+                             float* graph_ms, float* layout_ms);
+AM_API int am_umap_plan_graph(am_umap_plan* plan, int64_t* indptr, int32_t* indices, double* weights, double* rho,
+                              double* sigma, double* epochs_per_sample);
+AM_API int am_umap_plan_layout(am_umap_plan* plan, float* emb, int epochs, double a, double b, double gamma,
+                               double alpha0, double neg_rate, uint64_t seed);
+AM_API void am_umap_plan_free(am_umap_plan* plan);
 
 #ifdef __cplusplus
 }
