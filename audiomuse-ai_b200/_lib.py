@@ -118,6 +118,8 @@ SIGNATURES = {
     "am_umap_plan_graph": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "am_umap_plan_layout": (_i, [_vp, _vp, _i, C.c_double, C.c_double, C.c_double, C.c_double, C.c_double, _u64]),
     "am_umap_plan_free": (None, [_vp]),
+    "am_artist_gmm_fit": (_i, [_vp, _i64, _i, _vp, _i, _vp, _vp, _i, _i, C.c_double, C.c_double, _vp, _i64]
+                          + [_vp] * 12),
 }
 
 # include/audiomuse_b200_debug.h: probes and self tests, in libaudiomuse_b200_debug.so only

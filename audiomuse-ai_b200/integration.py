@@ -51,7 +51,7 @@ METRIC_NAMES = ("silhouette_score", "davies_bouldin_score", "calinski_harabasz_s
 
 
 def apply(clap=None, voyager_manager=None, clustering=None, allow_sklearn_fallback: bool = True,
-          clustering_helper=None, song_alchemy=None, app_map=None) -> None:
+          clustering_helper=None, song_alchemy=None, app_map=None, artist_gmm_manager=None) -> None:
     """clap / voyager_manager / clustering / clustering_helper: the reference's already imported tasks.* modules (pass
     only the ones to patch).  allow_sklearn_fallback keeps the reference's contract that a failing GPU k-means silently
     falls back to scikit-learn (tasks/clustering_gpu.py:130-148); this repository's own tests run with it off so a
@@ -59,7 +59,11 @@ def apply(clap=None, voyager_manager=None, clustering=None, allow_sklearn_fallba
     level (tasks/clustering_helper.py:16) and looks them up at call time (:462-470), so replacing the module attributes
     moves the fitness scoring to the GPU.  song_alchemy / app_map get the GPU UMAP projection as _project_with_umap:
     app_helper imports it from tasks.song_alchemy at call time (app_helper.py:1320, 1437), app_map binds it when it is
-    imported (app_map.py:13), so both modules are patched."""
+    imported (app_map.py:13), so both modules are patched.  artist_gmm_manager gets the GPU fit_artist_gmm and
+    select_optimal_gmm_components; build_and_store_artist_index looks both up at call time (:556, :185), and the
+    reference's own functions are kept for the B200_ALLOW_SKLEARN_FALLBACK=1 path.  That module runs `import voyager`
+    when it is imported, so install_voyager_shim() must come before `import tasks.artist_gmm_manager` and before
+    `import tasks.analysis`, which imports it."""
     if clap is not None:
         from . import clap_analyzer as b200_clap
 
@@ -85,5 +89,12 @@ def apply(clap=None, voyager_manager=None, clustering=None, allow_sklearn_fallba
             from . import projection
 
             mod._project_with_umap = projection.project_with_umap
-    if (clustering is not None or clustering_helper is not None) and allow_sklearn_fallback:
+    if artist_gmm_manager is not None:
+        from . import artist_gmm
+
+        artist_gmm.capture_originals(artist_gmm_manager)
+        artist_gmm_manager.fit_artist_gmm = artist_gmm.fit_artist_gmm
+        artist_gmm_manager.select_optimal_gmm_components = artist_gmm.select_optimal_gmm_components
+    if (clustering is not None or clustering_helper is not None or artist_gmm_manager is not None) \
+            and allow_sklearn_fallback:
         os.environ.setdefault("B200_ALLOW_SKLEARN_FALLBACK", "1")

@@ -338,6 +338,34 @@ AM_API int am_umap_plan_layout(am_umap_plan* plan, float* emb, int epochs, doubl
                                double alpha0, double neg_rate, uint64_t seed);
 AM_API void am_umap_plan_free(am_umap_plan* plan);
 
+/* ------------------------------------------------------------------ artist-similarity GMM sweep
+ * Replaces tasks/artist_gmm_manager.select_optimal_gmm_components (:63-126), which fit_artist_gmm (:129-216) calls:
+ * for every artist and every K of its range, GaussianMixture(K, covariance_type='diag', max_iter, n_init,
+ * random_state=42).fit and bic, float64 arithmetic on float32 rows (oracle/artist_gmm.py states it).  Synchronous.
+ *   rows         f32[n_rows, d], the artists' rows one after the other; offsets i64[n_artists + 1] (0 .. n_rows, every
+ *                artist >= 1 row); 1 <= d <= AM_ARTIST_GMM_MAX_D; every value finite
+ *   k_lo, k_hi   i32[n_artists]: the K tried, 1 <= k_lo, k_hi <= AM_ARTIST_GMM_MAX_K (k_hi < k_lo: none); a K above
+ *                the artist's row count fails, as scikit-learn's fit raises
+ *   draws        f64[n_draws]: MT19937(seed).random_sample() in order; init i of a K-fit uses the
+ *                1 + (K - 1)(2 + floor(ln K)) doubles from i times that count (at least n_init times it for the
+ *                largest K)
+ *   per artist   chosen_k i32 (0: every K failed), bic f64[16] and failed u8[16] per K (bic NaN where failed or not
+ *                tried), lower_bound f64, n_iter i32, converged u8 [16, n_init] per (K, init) (NaN / 0 for an init
+ *                that never ran), and the chosen fit's weights f32[16], means and covariances f32[16, d] (first K rows)
+ *   kpp          optional i32[n_artists, 16, n_init, 16]: the k-means++ centre rows (within the artist)
+ *   labels       optional i32[16, n_init, n_rows]: the k-means labels each (K, init) starts EM from
+ *   phase_ms     optional f32[2]: device ms of the fits and of the selection, from CUDA events
+ * Rows are staged in shared memory when n d 4 <= AM_ARTIST_GMM_SMEM_BYTES. */
+#define AM_ARTIST_GMM_MAX_K 16
+#define AM_ARTIST_GMM_MAX_D 1024
+#define AM_ARTIST_GMM_SMEM_BYTES 98304
+AM_API int am_artist_gmm_fit(const float* rows, int64_t n_rows, int d, const int64_t* offsets, int n_artists,
+                             const int32_t* k_lo, const int32_t* k_hi, int n_init, int max_iter, double tol,
+                             double reg_covar, const double* draws, int64_t n_draws, int32_t* chosen_k, double* bic,
+                             uint8_t* failed, double* lower_bound, int32_t* n_iter, uint8_t* converged,
+                             float* weights, float* means, float* covariances, int32_t* kpp, int32_t* labels,
+                             float* phase_ms);
+
 #ifdef __cplusplus
 }
 #endif
