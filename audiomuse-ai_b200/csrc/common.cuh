@@ -165,6 +165,11 @@ struct Stream {
 
 inline size_t round_up(size_t x, size_t m) { return (x + m - 1) / m * m; }
 inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
+// blocks of 256 threads for a grid-stride kernel over `total_threads` items: at most 16 per SM
+inline int grid_for(int64_t total_threads) {
+  const int64_t blocks = (total_threads + 255) / 256;
+  return (int)(blocks < 1 ? 1 : (blocks < (int64_t)sm_count() * 16 ? blocks : (int64_t)sm_count() * 16));
+}
 
 // ---------------------------------------------------------------- symmetrised k-NN graphs (spectral.cu)
 // CSR of k-NN lists ids i64[N, k] (device; a row's own id and ids outside [0, N) are skipped), columns ascending per

@@ -1,7 +1,7 @@
 // Debug entry point of the inverted-residual block (NOT part of libaudiomuse_b200.so: built into
 // libaudiomuse_b200_debug.so, declared in include/audiomuse_b200_debug.h; used by tests/test_gpu_block_exact.py).
 // Runs one block on host operands either fused (fused_block.cu) or layer by layer, through the same calls the
-// encoder's run_range makes for it.
+// encoder's run_steps makes for it.
 #include "../common.cuh"
 #include "../depthwise.cuh"
 #include "../fused_block.cuh"

@@ -1,4 +1,4 @@
-// The 3x3 / pad 1 / ReLU6 depthwise of the layer-by-layer path (kernels in encoder.cu), shared by the encoder and the
+// The 3x3 / pad 1 / ReLU6 depthwise of the layer-by-layer path (depthwise.cu), shared by the encoder and the
 // block debug entry (debug/block_debug.cu) so that both pick the same kernel for the same shape.
 #pragma once
 

@@ -9,12 +9,10 @@
 // (padded channels are exact zeros: zero weight rows + zero bias), so every 1x1 convolution is
 // one K-major GEMM  D[B*H*W, Cout] = A[B*H*W, Cin] x W[Cout, Cin]^T  on the wgmma path
 // (gemm.cu) with the folded-BatchNorm bias, ReLU6 and the residual add fused in its epilogue.
-// Depthwise 3x3 (+BN+ReLU6) is a bandwidth kernel over 8-channel (16-byte) vectors.  The stem
+// Depthwise 3x3 (+BN+ReLU6) is a bandwidth kernel over 8-channel (16-byte) vectors (depthwise.cu).  The stem
 // (bn0 + pad + 3x3 stride-2 on the single input channel + 1x1 + BN + ReLU6) reads the fp32
 // log-mel directly and is computed in fp32.  The head (<= 2.5 MMAC per window) runs in fp32.
 #include "common.cuh"
-
-#include <cuda_fp16.h>
 
 #include <algorithm>
 #include <cmath>
@@ -52,7 +50,7 @@ struct Layer {
 struct HeadOp {
   int kind = 0, a = -1, b = -1, dst = -1, K = 0, N = 0, act = 0, stride = 1;
   float eps = 0.f, eps2 = 0.f;
-  DevBuf<float> w, bias;          // fp32 weights (SIMT path, LayerNorm gain / shift, affine scale / shift)
+  DevBuf<float> w, bias;          // LayerNorm gain / shift, affine scale / shift; kVecLinear: bias
   DevBuf<__nv_bfloat16> w3;       // kVecLinear: bf16 [N, 3*Kp] = [hi | lo | hi] (see split3_kernel)
   bool has_w = false, has_bias = false;
 };
@@ -163,242 +161,6 @@ stem_kernel(const float* __restrict__ mel, int B, int n_mels, int T, int Ho, int
   }
 }
 
-// depthwise 3x3, pad 1, stride s, folded BN, ReLU6.  NHWC bf16.
-// A thread owns 8 channels (one 16-byte vector) of a vertical strip of kDwRows output rows at one
-// output column: the 9 x 8 folded weights live in registers, each input row (3 taps) is loaded once
-// and scattered into the (up to three) output rows it feeds, so the input is read ~(s*R+2)/R times
-// from L1/L2 instead of 9.  Consecutive threads = consecutive channel groups (coalesced 16 B).
-constexpr int kDwRows = 4;
-constexpr int kDwThreads = 128;
-
-__device__ __forceinline__ void dw_load_row(const __nv_bfloat16* base, int h, int H, int W, int cp, int x0,
-                                            uint4 (&raw)[3]) {
-#pragma unroll
-  for (int dx = 0; dx < 3; ++dx) {
-    const int x = x0 + dx;
-    raw[dx] = make_uint4(0u, 0u, 0u, 0u);
-    if (h >= 0 && h < H && x >= 0 && x < W)
-      raw[dx] = __ldg(reinterpret_cast<const uint4*>(base + ((int64_t)h * W + x) * cp));
-  }
-}
-
-template <int kStride>
-__global__ void __launch_bounds__(kDwThreads, 3)
-depthwise_kernel(const __nv_bfloat16* __restrict__ in, int B, int H, int W, int cp, int Ho, int Wo,
-                 const float* __restrict__ w /* [9, cp] */, const float* __restrict__ bias,
-                 __nv_bfloat16* __restrict__ out) {
-  const int groups = cp >> 3;
-  const int strips = (Ho + kDwRows - 1) / kDwRows;
-  const int64_t total = (int64_t)B * strips * Wo * groups;
-  const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= total) return;
-  const int g = (int)(idx % groups);
-  int64_t r = idx / groups;
-  const int wo = (int)(r % Wo);
-  r /= Wo;
-  const int strip = (int)(r % strips);
-  const int b = (int)(r / strips);
-  const int c0 = g * 8;
-  const int ho0 = strip * kDwRows;
-  const int nrows = min(kDwRows, Ho - ho0);
-
-  // packed fp16 arithmetic (HFMA2): inputs are post-ReLU6
-  // (|x| <= 6, bf16 -> fp16 is exact there), 9 taps; half the FMAs and half the weight registers of fp32
-  __half2 wt[9][4];
-#pragma unroll
-  for (int t = 0; t < 9; ++t) {
-    const float4 w0 = __ldg(reinterpret_cast<const float4*>(w + t * cp + c0));
-    const float4 w1 = __ldg(reinterpret_cast<const float4*>(w + t * cp + c0 + 4));
-    wt[t][0] = __floats2half2_rn(w0.x, w0.y);
-    wt[t][1] = __floats2half2_rn(w0.z, w0.w);
-    wt[t][2] = __floats2half2_rn(w1.x, w1.y);
-    wt[t][3] = __floats2half2_rn(w1.z, w1.w);
-  }
-  __half2 acc[kDwRows][4];
-  {
-    const float4 b0 = __ldg(reinterpret_cast<const float4*>(bias + c0));
-    const float4 b1 = __ldg(reinterpret_cast<const float4*>(bias + c0 + 4));
-#pragma unroll
-    for (int i = 0; i < kDwRows; ++i) {
-      acc[i][0] = __floats2half2_rn(b0.x, b0.y);
-      acc[i][1] = __floats2half2_rn(b0.z, b0.w);
-      acc[i][2] = __floats2half2_rn(b1.x, b1.y);
-      acc[i][3] = __floats2half2_rn(b1.z, b1.w);
-    }
-  }
-  const int x0 = wo * kStride - 1;
-  const int h_first = ho0 * kStride - 1;
-  constexpr int kInRows = (kDwRows - 1) * kStride + 3;
-  const __nv_bfloat16* base = in + ((int64_t)b * H) * W * cp + c0;
-  // software pipeline: the loads of input row ir+1 are in flight while row ir is consumed
-  uint4 cur[3], nxt[3];
-  dw_load_row(base, h_first, H, W, cp, x0, cur);
-#pragma unroll
-  for (int ir = 0; ir < kInRows; ++ir) {
-    if (ir + 1 < kInRows) dw_load_row(base, h_first + ir + 1, H, W, cp, x0, nxt);
-    __half2 px[3][4];
-#pragma unroll
-    for (int dx = 0; dx < 3; ++dx) {
-      const __nv_bfloat162* h2 = reinterpret_cast<const __nv_bfloat162*>(&cur[dx]);
-#pragma unroll
-      for (int q = 0; q < 4; ++q) px[dx][q] = __float22half2_rn(__bfloat1622float2(h2[q]));
-    }
-    // input row ir feeds output row o with kernel row dy = ir - o*stride, 0 <= dy < 3
-#pragma unroll
-    for (int dy = 0; dy < 3; ++dy) {
-      const int num = ir - dy;
-      if (num < 0 || (num % kStride) != 0) continue;
-      const int o = num / kStride;
-      if (o >= kDwRows) continue;
-#pragma unroll
-      for (int dx = 0; dx < 3; ++dx)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) acc[o][j] = __hfma2(px[dx][j], wt[dy * 3 + dx][j], acc[o][j]);
-    }
-#pragma unroll
-    for (int dx = 0; dx < 3; ++dx) cur[dx] = nxt[dx];
-  }
-  const __half2 h_zero = __floats2half2_rn(0.f, 0.f), h_six = __floats2half2_rn(6.f, 6.f);
-#pragma unroll
-  for (int o = 0; o < kDwRows; ++o) {
-    if (o < nrows) {
-      uint4 pk;
-      uint32_t* pw = reinterpret_cast<uint32_t*>(&pk);
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const float2 f = __half22float2(__hmin2(__hmax2(acc[o][j], h_zero), h_six));
-        const __nv_bfloat162 t = __floats2bfloat162_rn(f.x, f.y);
-        pw[j] = *reinterpret_cast<const uint32_t*>(&t);
-      }
-      *reinterpret_cast<uint4*>(out + ((((int64_t)b * Ho + ho0 + o) * Wo + wo) * cp) + c0) = pk;
-    }
-  }
-}
-
-// Row-sliding depthwise 3x3 for the NARROW late maps (W <= 16: blocks 6-9).  A thread owns 8 channels of a strip
-// of 2 output rows and walks the output columns, keeping a 3-column window of the input rows in registers: every
-// input pixel is loaded ONCE (the strip kernel above loads it from three threads -- in three different CTAs once
-// the channel count exceeds the CTA size -- and those re-reads went to L2).  Packed fp16 arithmetic as above.
-constexpr int kDwRowR = 2;
-
-template <int kStride>
-__global__ void __launch_bounds__(kDwThreads, 3)
-depthwise_row_kernel(const __nv_bfloat16* __restrict__ in, int B, int H, int W, int cp, int Ho, int Wo,
-                     const float* __restrict__ w /* [9, cp] */, const float* __restrict__ bias,
-                     __nv_bfloat16* __restrict__ out) {
-  constexpr int IR = (kDwRowR - 1) * kStride + 3;  // input rows feeding the strip
-  const int groups = cp >> 3;
-  const int strips = (Ho + kDwRowR - 1) / kDwRowR;
-  const int64_t total = (int64_t)B * strips * groups;
-  const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= total) return;
-  const int g = (int)(idx % groups);
-  const int64_t r = idx / groups;
-  const int strip = (int)(r % strips);
-  const int b = (int)(r / strips);
-  const int c0 = g * 8;
-  const int ho0 = strip * kDwRowR;
-  __half2 wt[9][4], bv[4];
-#pragma unroll
-  for (int t = 0; t < 9; ++t) {
-    const float4 w0 = __ldg(reinterpret_cast<const float4*>(w + t * cp + c0));
-    const float4 w1 = __ldg(reinterpret_cast<const float4*>(w + t * cp + c0 + 4));
-    wt[t][0] = __floats2half2_rn(w0.x, w0.y);
-    wt[t][1] = __floats2half2_rn(w0.z, w0.w);
-    wt[t][2] = __floats2half2_rn(w1.x, w1.y);
-    wt[t][3] = __floats2half2_rn(w1.z, w1.w);
-  }
-  {
-    const float4 b0 = __ldg(reinterpret_cast<const float4*>(bias + c0));
-    const float4 b1 = __ldg(reinterpret_cast<const float4*>(bias + c0 + 4));
-    bv[0] = __floats2half2_rn(b0.x, b0.y);
-    bv[1] = __floats2half2_rn(b0.z, b0.w);
-    bv[2] = __floats2half2_rn(b1.x, b1.y);
-    bv[3] = __floats2half2_rn(b1.z, b1.w);
-  }
-  const int h_first = ho0 * kStride - 1;
-  const __nv_bfloat16* base = in + ((int64_t)b * H) * W * cp + c0;
-  auto load_raw = [&](int x, uint4 (&raw)[IR]) {
-#pragma unroll
-    for (int ir = 0; ir < IR; ++ir) {
-      const int h = h_first + ir;
-      raw[ir] = make_uint4(0u, 0u, 0u, 0u);
-      if (h >= 0 && h < H && x >= 0 && x < W) raw[ir] = __ldg(reinterpret_cast<const uint4*>(base + ((int64_t)h * W + x) * cp));
-    }
-  };
-  auto unpack = [&](const uint4 (&raw)[IR], __half2 (&col)[IR][4]) {
-#pragma unroll
-    for (int ir = 0; ir < IR; ++ir) {
-      const __nv_bfloat162* h2 = reinterpret_cast<const __nv_bfloat162*>(&raw[ir]);
-#pragma unroll
-      for (int q = 0; q < 4; ++q) col[ir][q] = __float22half2_rn(__bfloat1622float2(h2[q]));
-    }
-  };
-  const __half2 h_zero = __floats2half2_rn(0.f, 0.f), h_six = __floats2half2_rn(6.f, 6.f);
-  __half2 ca[IR][4], cb[IR][4], cc[IR][4];  // input columns x-1, x, x+1 of the current output column
-  uint4 raw[IR], raw2[IR];
-  load_raw(-1, raw);
-  unpack(raw, ca);
-  if (kStride == 1) {
-    load_raw(0, raw);
-    unpack(raw, cb);
-  }
-  load_raw(kStride == 1 ? 1 : 0, raw);  // prefetch for the first column
-  if (kStride == 2) load_raw(1, raw2);
-  for (int wo = 0; wo < Wo; ++wo) {
-    if (kStride == 1) {
-      unpack(raw, cc);
-      if (wo + 1 < Wo) load_raw(wo + 2, raw);  // next column's loads fly under this column's arithmetic
-    } else {
-      unpack(raw, cb);
-      unpack(raw2, cc);
-      if (wo + 1 < Wo) {
-        load_raw(2 * wo + 2, raw);
-        load_raw(2 * wo + 3, raw2);
-      }
-    }
-#pragma unroll
-    for (int o = 0; o < kDwRowR; ++o) {
-      if (ho0 + o < Ho) {
-        __half2 acc[4];
-#pragma unroll
-        for (int j = 0; j < 4; ++j) acc[j] = bv[j];
-#pragma unroll
-        for (int dy = 0; dy < 3; ++dy) {
-          const int ir = o * kStride + dy;
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            acc[j] = __hfma2(ca[ir][j], wt[dy * 3 + 0][j], acc[j]);
-            acc[j] = __hfma2(cb[ir][j], wt[dy * 3 + 1][j], acc[j]);
-            acc[j] = __hfma2(cc[ir][j], wt[dy * 3 + 2][j], acc[j]);
-          }
-        }
-        uint4 pk;
-        uint32_t* pw = reinterpret_cast<uint32_t*>(&pk);
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const float2 f = __half22float2(__hmin2(__hmax2(acc[j], h_zero), h_six));
-          const __nv_bfloat162 t = __floats2bfloat162_rn(f.x, f.y);
-          pw[j] = *reinterpret_cast<const uint32_t*>(&t);
-        }
-        *reinterpret_cast<uint4*>(out + ((((int64_t)b * Ho + ho0 + o) * Wo + wo) * cp) + c0) = pk;
-      }
-    }
-    // slide the window
-#pragma unroll
-    for (int ir = 0; ir < IR; ++ir)
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        if (kStride == 1) {
-          ca[ir][j] = cb[ir][j];
-          cb[ir][j] = cc[ir][j];
-        } else {
-          ca[ir][j] = cc[ir][j];
-        }
-      }
-  }
-}
-
 // head step 1: mean over the positions a 1x1 stride-s conv visits -> f32 [B, C]
 __global__ void strided_mean_kernel(const __nv_bfloat16* __restrict__ in, int H, int W, int cp, int C, int stride,
                                     float* __restrict__ out) {
@@ -411,78 +173,6 @@ __global__ void strided_mean_kernel(const __nv_bfloat16* __restrict__ in, int H,
       for (int w = 0; w < W; w += stride) acc += __bfloat162float(in[(((int64_t)b * H + h) * W + w) * cp + c]);
     out[(int64_t)b * C + c] = acc * inv;
   }
-}
-
-// y[b, n] = bias[n] + sum_k f(x[b, k]) * W[n, k]   (f = identity or exact GELU), fp32.
-// Shared-memory tiled SGEMM: kTR (batch rows) x 64 (outputs) per CTA, 16-wide K steps, 256 threads with a
-// (kTR / 16) x 4 register micro-tile each.  kTR = 16 keeps the head's small problems (256 rows) on every
-// SM: with 64-row tiles linear1 ran on 32 CTAs and took 0.2 ms for 0.3 GFLOP.
-template <int kTR>
-__global__ void __launch_bounds__(256)
-linear_f32_kernel(const float* __restrict__ x, int B, int K, const float* __restrict__ W,
-                  const float* __restrict__ bias, int N, float* __restrict__ y, int in_act) {
-  constexpr int kMR = kTR / 16;
-  __shared__ float s_x[16][kTR + 4];  // [k][row]
-  __shared__ float s_w[16][64 + 4];   // [k][col]
-  const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
-  const int row0 = blockIdx.y * kTR, col0 = blockIdx.x * 64;
-  float acc[kMR][4];
-#pragma unroll
-  for (int i = 0; i < kMR; ++i)
-#pragma unroll
-    for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
-  for (int k0 = 0; k0 < K; k0 += 16) {
-    // k fastest for coalesced global reads (16 consecutive floats per row)
-    for (int i = threadIdx.x; i < 64 * 16; i += 256) {
-      const int r = i >> 4, kk = i & 15;
-      const int k = k0 + kk;
-      float wv = 0.f;
-      if (k < K && col0 + r < N) wv = __ldg(&W[(int64_t)(col0 + r) * K + k]);
-      s_w[kk][r] = wv;
-      if (r < kTR) {
-        float xv = 0.f;
-        if (k < K && row0 + r < B) {
-          xv = apply_act(in_act, x[(int64_t)(row0 + r) * K + k]);
-        }
-        s_x[kk][r] = xv;
-      }
-    }
-    __syncthreads();
-#pragma unroll
-    for (int kk = 0; kk < 16; ++kk) {
-      float a[kMR], bq[4];
-#pragma unroll
-      for (int i = 0; i < kMR; ++i) a[i] = s_x[kk][ty * kMR + i];
-#pragma unroll
-      for (int j = 0; j < 4; ++j) bq[j] = s_w[kk][tx * 4 + j];
-#pragma unroll
-      for (int i = 0; i < kMR; ++i)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(a[i], bq[j], acc[i][j]);
-    }
-    __syncthreads();
-  }
-#pragma unroll
-  for (int i = 0; i < kMR; ++i) {
-    const int r = row0 + ty * kMR + i;
-    if (r >= B) continue;
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const int c = col0 + tx * 4 + j;
-      if (c < N) y[(int64_t)r * N + c] = acc[i][j] + (bias ? bias[c] : 0.f);
-    }
-  }
-}
-
-static int launch_linear(const float* x, int B, int K, const float* W, const float* bias, int N, float* y, int in_act,
-                         cudaStream_t st) {
-  // 64-row tiles only when they still give every SM two CTAs
-  if ((int64_t)ceil_div(N, 64) * ceil_div(B, 64) >= 2 * (int64_t)sm_count()) {
-    AM_LAUNCH((linear_f32_kernel<64>), dim3(ceil_div(N, 64), ceil_div(B, 64)), 256, 0, st, x, B, K, W, bias, N, y, in_act);
-  } else {
-    AM_LAUNCH((linear_f32_kernel<16>), dim3(ceil_div(N, 64), ceil_div(B, 16)), 256, 0, st, x, B, K, W, bias, N, y, in_act);
-  }
-  return AM_OK;
 }
 
 // fp32 -> three bf16 terms so that ONE bf16 tensor-core GEMM over K' = 3*Kp reproduces the fp32 product to ~2^-16:
@@ -603,36 +293,6 @@ track_pool_kernel(const float* __restrict__ seg_emb, const int32_t* __restrict__
     for (int i = tid; i < E; i += blockDim.x) out[(int64_t)t * E + i] /= s_norm;
 }
 
-// ---------------------------------------------------------------- blob reader
-struct Reader {
-  const uint8_t* p;
-  const uint8_t* end;
-  bool ok = true;
-  template <typename T>
-  T get() {
-    T v{};
-    if (p + sizeof(T) > end) {
-      ok = false;
-      return v;
-    }
-    std::memcpy(&v, p, sizeof(T));
-    p += sizeof(T);
-    return v;
-  }
-  std::vector<float> floats() {
-    const uint64_t n = get<uint64_t>();
-    std::vector<float> v;
-    if (!ok || n > (uint64_t)(end - p) / 4) {
-      ok = false;
-      return v;
-    }
-    v.resize(n);
-    std::memcpy(v.data(), p, n * 4);
-    p += n * 4;
-    return v;
-  }
-};
-
 template <typename T>
 static int upload(DevBuf<T>& dst, const std::vector<T>& src) {
   AM_TRY(dst.alloc(std::max<size_t>(src.size(), 1)));
@@ -645,6 +305,36 @@ static std::vector<float> padded(const std::vector<float>& v, size_t n) {
   std::copy(v.begin(), v.begin() + std::min(n, v.size()), o.begin());
   return o;
 }
+
+struct Shape {
+  int H, W;
+};
+
+// One launch group of the trunk.
+enum StepKind { kStepStem, kStepConvFirst, kStepFused, kStepPointwise, kStepDw3x3, kStepDwGeneric, kStepSqueezeExcite };
+
+struct Step {
+  int kind = 0;
+  size_t first = 0, last = 0;  // layers [first, last] it runs; kStepFused: [expansion,] depthwise, projection
+  Shape in{0, 0}, out{0, 0};
+  int cout_p = 0;              // padded channels of its output
+  bool starts_block = false;   // its input is the residual source until the next such step
+  fused::BlockDesc desc{};     // kStepFused
+  fused::Plan plan;
+};
+
+// What runs for windows of T frames: every decision that depends on the shapes is taken here, once.  run_steps, the
+// workspace sizes and the flop counts of am_clap_flops_* all read it.
+struct ForwardPlan {
+  int T = 0;  // 0: not built
+  std::vector<Step> steps;
+  size_t late_step = 0;  // steps [0, late_step) are the early phase
+  Shape split{0, 0};     // input of the late phase: shape and padded channels
+  int split_c = 0;
+  // per-window elements of the largest layer output of each phase, the expanded tensors included (blocks run layer by
+  // layer with AM_FUSED_BLOCKS=0 or when a block does not fit the fused kernel)
+  size_t early_act = 0, late_act = 0;
+};
 
 }  // namespace am
 
@@ -663,7 +353,7 @@ struct am_model {
   am::DevBuf<__nv_bfloat16> late_in;  // [n, H, W, C] output of the early layers for all windows of a call
   int late_sub = 256;                 // windows per pass of the late phase
   size_t act_elems = 0;
-  int max_sub = 256;         // windows per pass of the early (chunked) phase (256 measured 1 % faster than 128)
+  am::ForwardPlan plan;               // of the window length of the latest call (plan_for)
   am::Stream stream;         // compute stream of the host-pointer entry points
   am::Stream copy_stream;    // H2D staging stream (host API): copies of chunk i+1 overlap compute of chunk i
   am::DevBuf<int16_t> pcm_stage[2];
@@ -683,7 +373,6 @@ struct am_model {
   bool slot_used[2] = {false, false};
   am_mel_plan* host_plan = nullptr;  // mel plan of the host entry point, cached per cfg (building one = host trig
   am_mel_cfg host_plan_cfg{};        // tables + cudaMalloc + upload: ~1 ms, was paid on every call)
-  int use_simt_gemm = 0;     // debug: AM_GEMM_IMPL=simt
   int fused_blocks = 1;      // AM_FUSED_BLOCKS=0: every block layer by layer (fused_block.cu otherwise)
   ~am_model() {
     for (int i = 0; i < 2; ++i) {
@@ -698,157 +387,11 @@ struct am_model {
 
 namespace am {
 
-struct Shape {
-  int H, W;
-};
-
 // output extent of a spatial layer (first conv / stem / depthwise); 1x1 layers keep the shape
 static Shape layer_out(const Layer& l, Shape s) {
   if (l.type == kDepthwise || l.type == kConvFirst || l.type == kStem)
     return {(s.H + l.pad_t + l.pad_b - l.kh) / l.stride + 1, (s.W + l.pad_l + l.pad_r - l.kw) / l.stride + 1};
   return s;
-}
-static Shape stem_out(const Layer& l, int T, int n_mels) {
-  return layer_out(l, l.h_is_time ? Shape{T, n_mels} : Shape{n_mels, T});
-}
-static Shape dw_out(const Layer& l, Shape s) { return layer_out(l, s); }
-
-// AMW1 blob (audiomuse-ai_b200/weights.py) -> ModelSpec
-static int parse_blob(const void* blob, size_t nbytes, ModelSpec* spec) {
-  Reader r{(const uint8_t*)blob, (const uint8_t*)blob + nbytes};
-  char magic[4];
-  for (int i = 0; i < 4; ++i) magic[i] = (char)r.get<uint8_t>();
-  if (!r.ok || std::memcmp(magic, "AMW1", 4) != 0) {
-    set_error("weights: bad magic (expected AMW1 or an ONNX ModelProto)");
-    return AM_ERR_IO;
-  }
-  const uint32_t version = r.get<uint32_t>();
-  spec->n_mels = (int)r.get<uint32_t>();
-  spec->emb = (int)r.get<uint32_t>();
-  spec->source = "AMW1";
-  const uint32_t n_layers = r.get<uint32_t>();
-  if (!r.ok || version != 1 || n_layers == 0 || n_layers > 4096) {
-    set_error("weights: bad header (version %u, %u layers)", version, n_layers);
-    return AM_ERR_IO;
-  }
-  for (uint32_t li = 0; li < n_layers; ++li) {
-    const uint32_t type = r.get<uint32_t>();
-    int32_t prm[8];
-    for (int i = 0; i < 8; ++i) prm[i] = r.get<int32_t>();
-    if (!r.ok) break;
-    if (type == kHead) {  // pn_block (1x1 stride s) -> mean -> Projection -> LayerNorm -> L2 as a row program
-      const int cin = prm[0], trunk = prm[1], emb = prm[2], stride = prm[3];
-      float ln_eps;
-      std::memcpy(&ln_eps, &prm[4], 4);
-      auto pn_w = r.floats(), pn_b = r.floats(), l1 = r.floats(), l2 = r.floats(), g = r.floats(), b = r.floats();
-      if (!r.ok || pn_w.size() != (size_t)trunk * cin || pn_b.size() != (size_t)trunk || l1.size() != (size_t)emb * trunk ||
-          l2.size() != (size_t)emb * emb || g.size() != (size_t)emb || b.size() != (size_t)emb) {
-        set_error("weights: malformed head record");
-        return AM_ERR_IO;
-      }
-      auto reg = [&](int dim) {
-        spec->reg_dim.push_back(dim);
-        return spec->n_regs++;
-      };
-      VecOp pool;
-      pool.kind = kVecPool;
-      pool.stride = stride;
-      pool.N = cin;
-      pool.dst = reg(cin);
-      VecOp pn;
-      pn.kind = kVecLinear;
-      pn.a = pool.dst;
-      pn.K = cin;
-      pn.N = trunk;
-      pn.w = pn_w;
-      pn.bias = pn_b;
-      pn.dst = reg(trunk);
-      VecOp e1;
-      e1.kind = kVecLinear;
-      e1.a = pn.dst;
-      e1.K = trunk;
-      e1.N = emb;
-      e1.w = l1;
-      e1.dst = reg(emb);
-      VecOp e2;
-      e2.kind = kVecLinear;
-      e2.a = e1.dst;
-      e2.K = emb;
-      e2.N = emb;
-      e2.act = kActGelu;
-      e2.w = l2;
-      e2.dst = reg(emb);
-      VecOp fin;
-      fin.kind = kVecAddLnL2;
-      fin.a = e1.dst;
-      fin.b = e2.dst;
-      fin.N = emb;
-      fin.eps = ln_eps;
-      fin.eps2 = 1e-12f;
-      fin.w = g;
-      fin.bias = b;
-      fin.dst = reg(emb);
-      spec->head = {pool, pn, e1, e2, fin};
-      continue;
-    }
-    LayerSpec L;
-    L.type = (int)type;
-    if (type == kStem) {
-      L.cin = 1;
-      L.cout = prm[0];
-      L.kh = L.kw = 3;
-      L.stride = 2;
-      L.act = kActRelu6;
-      L.pad_t = prm[1];
-      L.pad_b = prm[2];
-      L.pad_l = prm[3];
-      L.pad_r = prm[4];
-      L.aux0 = r.floats();
-      L.aux1 = r.floats();
-      L.w = r.floats();
-      L.aux2 = r.floats();
-      L.bias = r.floats();
-      if (!r.ok || L.aux0.size() != (size_t)spec->n_mels || L.aux1.size() != (size_t)spec->n_mels || L.w.size() != 9 ||
-          L.aux2.size() != (size_t)L.cout || L.bias.size() != (size_t)L.cout) {
-        set_error("weights: malformed stem record");
-        return AM_ERR_IO;
-      }
-    } else if (type == kPointwise) {
-      L.cin = prm[0];
-      L.cout = prm[1];
-      L.act = prm[2];
-      L.residual = prm[3];
-      L.block_start = prm[4];
-      L.w = r.floats();
-      L.bias = r.floats();
-      if (!r.ok || L.w.size() != (size_t)L.cin * L.cout || L.bias.size() != (size_t)L.cout) {
-        set_error("weights: malformed pointwise record (layer %u)", li);
-        return AM_ERR_IO;
-      }
-    } else if (type == kDepthwise) {
-      L.cin = L.cout = prm[0];
-      L.stride = prm[1];
-      L.block_start = prm[4];
-      L.kh = L.kw = 3;
-      L.pad_t = L.pad_b = L.pad_l = L.pad_r = 1;
-      L.act = kActRelu6;
-      L.w = r.floats();
-      L.bias = r.floats();  // w: [c, 9]
-      if (!r.ok || L.w.size() != (size_t)L.cin * 9 || L.bias.size() != (size_t)L.cin || (L.stride != 1 && L.stride != 2)) {
-        set_error("weights: malformed depthwise record (layer %u)", li);
-        return AM_ERR_IO;
-      }
-    } else {
-      set_error("weights: unknown layer type %u", type);
-      return AM_ERR_IO;
-    }
-    spec->layers.push_back(std::move(L));
-  }
-  if (!r.ok) {
-    set_error("weights: truncated blob");
-    return AM_ERR_IO;
-  }
-  return AM_OK;
 }
 
 // ModelSpec -> device model: pads channels to 16, converts weights to the kernels' layouts, validates the chain
@@ -996,7 +539,6 @@ static int build_model(am_model* m, const ModelSpec& spec) {
         set_error("weights: malformed linear in the head (op %zu)", q);
         return AM_ERR_IO;
       }
-      AM_TRY(upload(H->w, S.w));
       AM_TRY(upload_split3(H->w3, S.w, S.N, S.K));
       H->has_w = true;
       if (!S.bias.empty()) {
@@ -1028,87 +570,18 @@ static int build_model(am_model* m, const ModelSpec& spec) {
   return AM_OK;
 }
 
-static int grid_for(int64_t total_threads) {
-  const int64_t blocks = (total_threads + 255) / 256;
-  return (int)std::max<int64_t>(1, std::min<int64_t>(blocks, (int64_t)sm_count() * 16));
-}
-
-bool dw3x3_fp16_safe(const std::vector<float>& w, const std::vector<float>& bias, int cp, bool relu6_input) {
-  if (!relu6_input) return false;
-  for (int c = 0; c < cp; ++c) {
-    double m = std::fabs((double)bias[(size_t)c]);
-    for (int t = 0; t < 9; ++t) m += 6.0 * std::fabs((double)w[(size_t)t * cp + c]);
-    if (!(m < 32768.0)) return false;  // NaN weights are not safe either
-  }
-  return true;
-}
-
-int dw3x3(const __nv_bfloat16* in, int B, int H, int W, int cp, int stride, const float* w, const float* bias, bool fp16,
-          __nv_bfloat16* out, cudaStream_t st, int* kernel) {
-  AM_CHECK(stride == 1 || stride == 2, "depthwise: stride %d", stride);
-  const int Ho = (H - 1) / stride + 1, Wo = (W - 1) / stride + 1;
-  AM_CHECK(B > 0 && H > 0 && W > 0 && cp % 8 == 0, "depthwise: empty input or channels not a multiple of 8");
-  if (!fp16) {
-    if (kernel) *kernel = kDwGeneric;
-    AM_LAUNCH(depthwise_generic_kernel, grid_for((int64_t)B * Ho * Wo * (cp / 8)), 256, 0, st, in, B, H, W, cp, Ho, Wo,
-              3, stride, 1, 1, w, bias, (int)kActRelu6, out);
-    return AM_OK;
-  }
-  const int strips = (Ho + kDwRows - 1) / kDwRows;
-  const int64_t total = (int64_t)B * strips * Wo * (cp / 8);
-  const unsigned grid = (unsigned)((total + kDwThreads - 1) / kDwThreads);
-  static const bool no_row = std::getenv("AM_DW_NO_ROW") != nullptr;
-  const int rstrips = (Ho + kDwRowR - 1) / kDwRowR;
-  const int64_t rtotal = (int64_t)B * rstrips * (cp / 8);
-  if (!no_row && W <= 16 && rtotal >= (int64_t)sm_count() * 8 * kDwThreads) {
-    // narrow late maps with enough (window, strip, channel group) work items to fill the GPU
-    if (kernel) *kernel = kDwRow;
-    const unsigned rgrid = (unsigned)((rtotal + kDwThreads - 1) / kDwThreads);
-    if (stride == 1) {
-      AM_LAUNCH(depthwise_row_kernel<1>, rgrid, kDwThreads, 0, st, in, B, H, W, cp, Ho, Wo, w, bias, out);
-    } else {
-      AM_LAUNCH(depthwise_row_kernel<2>, rgrid, kDwThreads, 0, st, in, B, H, W, cp, Ho, Wo, w, bias, out);
-    }
-  } else {
-    if (kernel) *kernel = kDwStrip;
-    if (stride == 1) {
-      AM_LAUNCH(depthwise_kernel<1>, grid, kDwThreads, 0, st, in, B, H, W, cp, Ho, Wo, w, bias, out);
-    } else {
-      AM_LAUNCH(depthwise_kernel<2>, grid, kDwThreads, 0, st, in, B, H, W, cp, Ho, Wo, w, bias, out);
-    }
-  }
-  return AM_OK;
-}
-
 // The trunk runs in two phases.  EARLY = stem + the leading layers whose input maps are large (at least
 // kEarlyMinPositions positions per window): processed chunk by chunk, so host->device copies of the next chunk hide
 // under it and one chunk already fills the GPU.  LATE = everything after (small tensors): processed ONCE for all
 // windows of the call, so the deep, narrow layers get full-size grids.  The split falls on a block boundary (a
-// residual add reads its block's input).  late_start() is the first layer of the late phase.
+// residual add reads its block's input).
 constexpr int64_t kEarlyMinPositions = 4096;
-
-static size_t late_start(const am_model* m, int T, Shape* s_split, int* c_split) {
-  Shape s = stem_out(*m->layers[0], T, m->n_mels);
-  int c = m->layers[0]->cout_p;
-  size_t i = 1;
-  while (i < m->layers.size()) {
-    const Layer& l = *m->layers[i];
-    if (l.block_start && (int64_t)s.H * s.W < kEarlyMinPositions) break;
-    s = layer_out(l, s);
-    c = l.cout_p;
-    ++i;
-  }
-  *s_split = s;
-  *c_split = c;
-  return i;
-}
 
 // Layers from `i` (a block start) form an inverted-residual block the fused kernel runs: [1x1 expand + ReLU6] ->
 // 3x3 depthwise + ReLU6 -> linear 1x1, all inside [i, hi) and fitting fused::plan at input shape `s`.
-static bool fused_block_at(const am_model* m, size_t i, size_t hi, Shape s, fused::BlockDesc* d, fused::Plan* pl,
-                           int* ex, int* dw, int* pj) {
+static bool fused_block_at(const am_model* m, size_t i, size_t hi, Shape s, Step* st) {
   const auto& L = m->layers;
-  if (m->use_simt_gemm || !m->fused_blocks || !L[i]->block_start) return false;
+  if (!m->fused_blocks || !L[i]->block_start) return false;
   int e = -1;
   size_t k = i;
   if (L[k]->type == kPointwise && L[k]->act == kActRelu6 && L[k]->stride == 1) e = (int)k++;
@@ -1117,157 +590,178 @@ static bool fused_block_at(const am_model* m, size_t i, size_t hi, Shape s, fuse
   const Layer& P = *L[k + 1];
   if (!D.dw_fast() || P.type != kPointwise || P.act != kActNone || P.stride != 1 || P.cin_p != D.cin_p) return false;
   if (e >= 0 && L[(size_t)e]->cout_p != D.cin_p) return false;
-  *d = fused::BlockDesc{};
-  d->H = s.H;
-  d->W = s.W;
-  d->cin_p = e >= 0 ? L[(size_t)e]->cin_p : D.cin_p;
-  d->cmid_p = D.cin_p;
-  d->cout_p = P.cout_p;
-  d->stride = D.stride;
-  d->has_expand = e >= 0 ? 1 : 0;
-  d->residual = P.residual;
-  *ex = e;
-  *dw = (int)k;
-  *pj = (int)k + 1;
-  return fused::plan(*d, pl);
+  fused::BlockDesc& d = st->desc;
+  d = fused::BlockDesc{};
+  d.H = s.H;
+  d.W = s.W;
+  d.cin_p = e >= 0 ? L[(size_t)e]->cin_p : D.cin_p;
+  d.cmid_p = D.cin_p;
+  d.cout_p = P.cout_p;
+  d.stride = D.stride;
+  d.has_expand = e >= 0 ? 1 : 0;
+  d.residual = P.residual;
+  st->first = i;
+  st->last = k + 1;
+  return fused::plan(d, &st->plan);
 }
 
-// Runs layers [lo, hi) on `nb` windows.  lo == 0: starts from the log-mel (stem); else from `in` (shape s_in).
-// The last operation writes to `final_out` when given, else to a workspace buffer; *out / *s_out describe it.
-static int run_range(am_model* m, const float* mel_dev, const __nv_bfloat16* in, Shape s_in, size_t lo, size_t hi,
-                     int nb, int T, __nv_bfloat16* final_out, const __nv_bfloat16** out, Shape* s_out,
-                     cudaStream_t st) {
-  Shape s = s_in;
+static int build_plan(const am_model* m, int T, ForwardPlan* p) {
+  const auto& L = m->layers;
+  *p = ForwardPlan{};
+  const Layer& stem = *L[0];
+  Shape s = layer_out(stem, stem.h_is_time ? Shape{T, m->n_mels} : Shape{m->n_mels, T});
+  AM_CHECK(s.H > 0 && s.W > 0, "encoder: input of %d frames x %d mels is too small", T, m->n_mels);
+  AM_CHECK(stem.type == kStem || (size_t)(stem.kh * stem.kw + 1) * stem.cout_p * sizeof(float) <= 48 * 1024,
+           "encoder: first convolution with %d x %d taps x %d channels does not fit in shared memory", stem.kh, stem.kw,
+           stem.cout_p);
+  // first layer of the late phase
+  size_t split = 1;
+  for (Shape w = s; split < L.size(); ++split) {
+    if (L[split]->block_start && (int64_t)w.H * w.W < kEarlyMinPositions) break;
+    w = layer_out(*L[split], w);
+  }
+  Step st;
+  st.kind = stem.type == kStem ? kStepStem : kStepConvFirst;
+  st.in = st.out = s;
+  st.cout_p = stem.cout_p;
+  p->steps.push_back(st);
+  p->late_step = 1;
+  p->early_act = (size_t)s.H * s.W * stem.cout_p;
+  for (size_t i = 1; i < L.size();) {
+    const bool late = i >= split;
+    const int prev = p->steps.back().kind;
+    st = Step{};
+    st.in = s;
+    st.starts_block = L[i]->block_start || i == split || prev == kStepStem || prev == kStepConvFirst || prev == kStepFused;
+    if (fused_block_at(m, i, late ? L.size() : split, s, &st)) {
+      st.kind = kStepFused;
+    } else {
+      const Layer& l = *L[i];
+      st.first = st.last = i;
+      switch (l.type) {
+        case kPointwise: st.kind = kStepPointwise; break;
+        case kDepthwise: st.kind = l.dw_fast() ? kStepDw3x3 : kStepDwGeneric; break;
+        case kSqueezeExcite: st.kind = kStepSqueezeExcite; break;
+        default: set_error("encoder: layer %zu of type %d cannot run here", i, l.type); return AM_ERR_INVALID;
+      }
+      AM_CHECK(l.type != kSqueezeExcite || (size_t)(l.cin + l.cmid) * sizeof(float) <= 48 * 1024,
+               "encoder: squeeze-excite over %d channels does not fit in shared memory", l.cin);
+    }
+    size_t& act = late ? p->late_act : p->early_act;
+    for (i = st.first; i <= st.last; ++i) {
+      s = layer_out(*L[i], s);
+      AM_CHECK(s.H > 0 && s.W > 0, "encoder: depthwise layer %zu has an empty output", i);
+      act = std::max(act, (size_t)s.H * s.W * L[i]->cout_p);
+    }
+    st.out = s;
+    st.cout_p = L[st.last]->cout_p;
+    p->steps.push_back(st);
+    if (!late) p->late_step = p->steps.size();
+  }
+  p->split = p->steps[p->late_step - 1].out;
+  p->split_c = p->steps[p->late_step - 1].cout_p;
+  p->T = T;
+  return AM_OK;
+}
+
+// the model's plan for windows of T frames: rebuilt when T changes (a session runs one window length)
+static int plan_for(am_model* m, int T, const ForwardPlan** out) {
+  if (m->plan.T != T) AM_TRY(build_plan(m, T, &m->plan));
+  *out = &m->plan;
+  return AM_OK;
+}
+
+// Launches steps [lo, hi) of the plan on `nb` windows.  lo == 0: starts from the log-mel (stem); else from `in`.
+// The last step writes to `final_out` when given, else to a workspace buffer; *out is what it wrote.
+static int run_steps(am_model* m, const ForwardPlan& p, const float* mel_dev, const __nv_bfloat16* in, size_t lo, size_t hi,
+                     int nb, __nv_bfloat16* final_out, const __nv_bfloat16** out, cudaStream_t st) {
   const __nv_bfloat16* cur = in;
   const __nv_bfloat16* block_in = in;
-  auto pick_dst = [&](bool is_last) -> __nv_bfloat16* {
-    if (is_last && final_out) return final_out;
+  for (size_t q = lo; q < hi; ++q) {
+    const Step& t = p.steps[q];
+    const Layer& l = *m->layers[t.last];
+    if (t.starts_block) block_in = cur;
+    __nv_bfloat16* dst = q + 1 == hi ? final_out : nullptr;
     for (auto& b : m->act)
-      if (b.p != cur && b.p != block_in) return b.p;
-    return nullptr;
-  };
-  size_t i = lo;
-  if (lo == 0) {
-    const Layer& stem = *m->layers[0];
-    s = stem_out(stem, T, m->n_mels);
-    AM_CHECK(s.H > 0 && s.W > 0, "encoder: input of %d frames x %d mels is too small", T, m->n_mels);
-    __nv_bfloat16* dst = pick_dst(hi == 1);
-    if (stem.type == kStem) {
-      const int64_t n_tiles = (int64_t)nb * ((s.H + kStemTH - 1) / kStemTH) * ((s.W + kStemTW - 1) / kStemTW);
-      const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(n_tiles, (int64_t)sm_count() * 8));
-      AM_LAUNCH(stem_kernel, grid, 256, (size_t)stem.cout_p * 8, st, mel_dev, nb, m->n_mels, T, s.H, s.W, stem.pad_t,
-                stem.pad_l, stem.aux0.p, stem.aux1.p, stem.w_f32.p, stem.aux2.p, stem.bias.p, stem.cout_p, dst);
-    } else {
-      const size_t smem = (size_t)(stem.kh * stem.kw + 1) * stem.cout_p * sizeof(float);
-      AM_CHECK(smem <= 48 * 1024, "encoder: first convolution with %d x %d taps x %d channels does not fit in shared memory",
-               stem.kh, stem.kw, stem.cout_p);
-      const int grid = grid_for((int64_t)nb * s.H * s.W * (stem.cout_p / 8));
-      AM_LAUNCH(conv_first_kernel, grid, 256, smem, st, mel_dev, nb, m->n_mels, T, s.H, s.W, stem.kh, stem.kw, stem.stride,
-                stem.pad_t, stem.pad_l, stem.h_is_time, stem.aux0.p, stem.aux1.p, stem.w_f32.p, stem.bias.p, stem.cout_p,
-                stem.act, dst);
-    }
-    cur = block_in = dst;
-    i = 1;
-  }
-  for (; i < hi; ++i) {
-    const Layer& l = *m->layers[i];
-    if (l.block_start) {
-      block_in = cur;
-      fused::BlockDesc d;
-      fused::Plan pl;
-      int ex, dw, pj;
-      if (fused_block_at(m, i, hi, s, &d, &pl, &ex, &dw, &pj)) {  // the whole block in one kernel (fused_block.cu)
-        const Layer* E = ex >= 0 ? m->layers[(size_t)ex].get() : nullptr;
-        const Layer& D = *m->layers[(size_t)dw];
-        const Layer& P = *m->layers[(size_t)pj];
-        __nv_bfloat16* dst = pick_dst((size_t)pj + 1 == hi);
-        AM_TRY(fused::run(d, pl, cur, E ? E->w_bf16.p : nullptr, D.fused_params.p, P.w_bf16.p, P.bias.p, dst, nb, st));
-        s = dw_out(D, s);
-        cur = block_in = dst;
-        i = (size_t)pj;
-        continue;
+      if (!dst && b.p != cur && b.p != block_in) dst = b.p;
+    const Shape s = t.in, o = t.out;
+    switch (t.kind) {
+      case kStepStem: {
+        const int64_t n_tiles = (int64_t)nb * ((o.H + kStemTH - 1) / kStemTH) * ((o.W + kStemTW - 1) / kStemTW);
+        const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(n_tiles, (int64_t)sm_count() * 8));
+        AM_LAUNCH(stem_kernel, grid, 256, (size_t)l.cout_p * 8, st, mel_dev, nb, m->n_mels, p.T, o.H, o.W, l.pad_t, l.pad_l,
+                  l.aux0.p, l.aux1.p, l.w_f32.p, l.aux2.p, l.bias.p, l.cout_p, dst);
+        break;
       }
-    }
-    __nv_bfloat16* dst = pick_dst(i + 1 == hi);
-    if (l.type == kDepthwise && !l.dw_fast()) {
-      const Shape o = dw_out(l, s);
-      AM_CHECK(o.H > 0 && o.W > 0, "encoder: depthwise layer %zu has an empty output", i);
-      const int grid = grid_for((int64_t)nb * o.H * o.W * (l.cout_p / 8));
-      AM_LAUNCH(depthwise_generic_kernel, grid, 256, 0, st, cur, nb, s.H, s.W, l.cin_p, o.H, o.W, l.kh, l.stride, l.pad_t,
-                l.pad_l, l.w_f32.p, l.bias.p, l.act, dst);
-      s = o;
-    } else if (l.type == kDepthwise) {
-      AM_TRY(dw3x3(cur, nb, s.H, s.W, l.cin_p, l.stride, l.w_f32.p, l.bias.p, l.dw_fp16, dst, st, nullptr));
-      s = dw_out(l, s);
-    } else if (l.type == kSqueezeExcite) {
-      const int HW = s.H * s.W;
-      AM_TRY(m->se_mean.ensure((size_t)nb * l.cin));
-      AM_TRY(m->se_gate.ensure((size_t)nb * l.cin));
-      AM_LAUNCH(channel_mean_kernel, dim3((unsigned)ceil_div(l.cin, 64), (unsigned)nb), 256, 0, st, cur, HW, l.cin_p, l.cin,
-                m->se_mean.p);
-      const size_t smem = (size_t)(l.cin + l.cmid) * sizeof(float);
-      AM_CHECK(smem <= 48 * 1024, "encoder: squeeze-excite over %d channels does not fit in shared memory", l.cin);
-      AM_LAUNCH(se_gate_kernel, nb, 256, smem, st, m->se_mean.p, l.cin, l.cmid, l.w_f32.p, l.bias.p, l.aux0.p, l.aux1.p, l.act,
-                l.gate_act, m->se_gate.p);
-      AM_LAUNCH(se_scale_kernel, grid_for((int64_t)nb * HW * (l.cin_p / 8)), 256, 0, st, cur, (int64_t)HW, l.cin_p, l.cin,
-                m->se_gate.p, nb, dst);
-    } else if (l.type == kPointwise) {
-      const int64_t M = (int64_t)nb * s.H * s.W;
-      gemm::Epilogue ep;
-      ep.bias = l.bias.p;
-      ep.act = l.act;
-      if (l.residual) {
-        ep.residual = block_in;
-        ep.ld_res = l.cout_p;
+      case kStepConvFirst: {
+        const size_t smem = (size_t)(l.kh * l.kw + 1) * l.cout_p * sizeof(float);
+        const int grid = grid_for((int64_t)nb * o.H * o.W * (l.cout_p / 8));
+        AM_LAUNCH(conv_first_kernel, grid, 256, smem, st, mel_dev, nb, m->n_mels, p.T, o.H, o.W, l.kh, l.kw, l.stride, l.pad_t,
+                  l.pad_l, l.h_is_time, l.aux0.p, l.aux1.p, l.w_f32.p, l.bias.p, l.cout_p, l.act, dst);
+        break;
       }
-      if (m->use_simt_gemm) {
-        for (int64_t m0 = 0; m0 < M; m0 += 32768) {
-          const int64_t mm = std::min<int64_t>(32768, M - m0);
-          gemm::Epilogue e2 = ep;
-          if (e2.residual) e2.residual += m0 * l.cout_p;
-          AM_TRY(gemm::gemm_bf16_simt(cur + m0 * l.cin_p, mm, l.cin_p, l.w_bf16.p, l.cout_p, l.cin_p, l.cin_p,
-                                      dst + m0 * l.cout_p, l.cout_p, false, e2, st));
+      case kStepFused: {  // the whole block in one kernel (fused_block.cu)
+        const Layer& D = *m->layers[t.last - 1];
+        AM_TRY(fused::run(t.desc, t.plan, cur, t.desc.has_expand ? m->layers[t.first]->w_bf16.p : nullptr, D.fused_params.p,
+                          l.w_bf16.p, l.bias.p, dst, nb, st));
+        break;
+      }
+      case kStepDwGeneric:
+        AM_LAUNCH(depthwise_generic_kernel, grid_for((int64_t)nb * o.H * o.W * (l.cout_p / 8)), 256, 0, st, cur, nb, s.H, s.W,
+                  l.cin_p, o.H, o.W, l.kh, l.stride, l.pad_t, l.pad_l, l.w_f32.p, l.bias.p, l.act, dst);
+        break;
+      case kStepDw3x3:
+        AM_TRY(dw3x3(cur, nb, s.H, s.W, l.cin_p, l.stride, l.w_f32.p, l.bias.p, l.dw_fp16, dst, st, nullptr));
+        break;
+      case kStepSqueezeExcite: {
+        const int HW = s.H * s.W;
+        AM_TRY(m->se_mean.ensure((size_t)nb * l.cin));
+        AM_TRY(m->se_gate.ensure((size_t)nb * l.cin));
+        AM_LAUNCH(channel_mean_kernel, dim3((unsigned)ceil_div(l.cin, 64), (unsigned)nb), 256, 0, st, cur, HW, l.cin_p, l.cin,
+                  m->se_mean.p);
+        const size_t smem = (size_t)(l.cin + l.cmid) * sizeof(float);
+        AM_LAUNCH(se_gate_kernel, nb, 256, smem, st, m->se_mean.p, l.cin, l.cmid, l.w_f32.p, l.bias.p, l.aux0.p, l.aux1.p, l.act,
+                  l.gate_act, m->se_gate.p);
+        AM_LAUNCH(se_scale_kernel, grid_for((int64_t)nb * HW * (l.cin_p / 8)), 256, 0, st, cur, (int64_t)HW, l.cin_p, l.cin,
+                  m->se_gate.p, nb, dst);
+        break;
+      }
+      case kStepPointwise: {
+        gemm::Epilogue ep;
+        ep.bias = l.bias.p;
+        ep.act = l.act;
+        if (l.residual) {
+          ep.residual = block_in;
+          ep.ld_res = l.cout_p;
         }
-      } else {
-        AM_TRY(gemm::gemm_bf16(cur, M, l.cin_p, l.w_bf16.p, l.cout_p, l.cin_p, l.cin_p, dst, l.cout_p, false, ep,
-                               /*m_fastest=*/false, st));
+        AM_TRY(gemm::gemm_bf16(cur, (int64_t)nb * s.H * s.W, l.cin_p, l.w_bf16.p, l.cout_p, l.cin_p, l.cin_p, dst, l.cout_p, false,
+                               ep, /*m_fastest=*/false, st));
+        break;
       }
-    } else {
-      set_error("encoder: layer %zu of type %d cannot run here", i, l.type);
-      return AM_ERR_INVALID;
     }
     cur = dst;
   }
   *out = cur;
-  *s_out = s;
   return AM_OK;
 }
 
 // EARLY phase of `nb` windows (log-mel at mel_dev): result appended to m->late_in at window offset b0
-static int forward_early(am_model* m, const float* mel_dev, int nb, int b0, int T, cudaStream_t st) {
-  Shape ss;
-  int cs;
-  const size_t split = late_start(m, T, &ss, &cs);
-  const size_t per_win = (size_t)ss.H * ss.W * cs;
+static int forward_early(am_model* m, const ForwardPlan& p, const float* mel_dev, int nb, int b0, cudaStream_t st) {
+  const size_t per_win = (size_t)p.split.H * p.split.W * p.split_c;
   const __nv_bfloat16* o;
-  Shape so;
-  return run_range(m, mel_dev, nullptr, Shape{0, 0}, 0, split, nb, T, m->late_in.p + (size_t)b0 * per_win, &o, &so, st);
+  return run_steps(m, p, mel_dev, nullptr, 0, p.late_step, nb, m->late_in.p + (size_t)b0 * per_win, &o, st);
 }
 
 // LATE phase for all `n` windows + the head program's pooling (for a 1x1 stride-s conv in front of the mean, the
 // mean over the positions the conv visits commutes with it: the conv runs on the pooled rows)
-static int forward_late(am_model* m, int n, int T, cudaStream_t st) {
-  Shape ss;
-  int cs;
-  const size_t split = late_start(m, T, &ss, &cs);
-  const size_t per_win = (size_t)ss.H * ss.W * cs;
+static int forward_late(am_model* m, const ForwardPlan& p, int n, cudaStream_t st) {
+  const size_t per_win = (size_t)p.split.H * p.split.W * p.split_c;
+  const Shape so = p.steps.back().out;
   const HeadOp& pool = *m->head[0];
   for (int b0 = 0; b0 < n; b0 += m->late_sub) {
     const int nb = std::min(m->late_sub, n - b0);
     const __nv_bfloat16* o = m->late_in.p + (size_t)b0 * per_win;
-    Shape so = ss;
-    if (split < m->layers.size())
-      AM_TRY(run_range(m, nullptr, o, ss, split, m->layers.size(), nb, T, nullptr, &o, &so, st));
+    AM_TRY(run_steps(m, p, nullptr, o, p.late_step, p.steps.size(), nb, nullptr, &o, st));
     AM_LAUNCH(strided_mean_kernel, nb, 256, 0, st, o, so.H, so.W, m->head_cin_p, m->head_cin, pool.stride,
               m->regs[(size_t)pool.dst]->p + (size_t)b0 * m->head_cin);
   }
@@ -1288,16 +782,12 @@ static int head_forward(am_model* m, int n, float* out_dev, cudaStream_t st) {
     const int egrid = grid_for(rows * dim);
     switch (h.kind) {
       case kVecLinear: {
-        if (m->use_simt_gemm) {  // AM_GEMM_IMPL=simt: everything on CUDA cores (debug)
-          AM_TRY(launch_linear(a, n, h.K, h.w.p, h.has_bias ? h.bias.p : nullptr, h.N, dst, h.act, st));
-        } else {
-          const int Kp = (int)round_up((size_t)h.K, 8);
-          const int grid = (int)std::min<int64_t>(((int64_t)n * Kp + 255) / 256, (int64_t)sm_count() * 8);
-          AM_LAUNCH(split3_kernel, grid, 256, 0, st, a, n, h.K, Kp, h.act, m->a3.p);
-          gemm::Epilogue ep;
-          ep.bias = h.has_bias ? h.bias.p : nullptr;
-          AM_TRY(gemm::gemm_bf16(m->a3.p, n, 3 * Kp, h.w3.p, h.N, 3 * Kp, 3 * Kp, dst, h.N, /*d_is_f32=*/true, ep, false, st));
-        }
+        const int Kp = (int)round_up((size_t)h.K, 8);
+        const int grid = (int)std::min<int64_t>(((int64_t)n * Kp + 255) / 256, (int64_t)sm_count() * 8);
+        AM_LAUNCH(split3_kernel, grid, 256, 0, st, a, n, h.K, Kp, h.act, m->a3.p);
+        gemm::Epilogue ep;
+        ep.bias = h.has_bias ? h.bias.p : nullptr;
+        AM_TRY(gemm::gemm_bf16(m->a3.p, n, 3 * Kp, h.w3.p, h.N, 3 * Kp, 3 * Kp, dst, h.N, /*d_is_f32=*/true, ep, false, st));
         break;
       }
       case kVecUnary:
@@ -1327,47 +817,27 @@ static int head_forward(am_model* m, int n, float* out_dev, cudaStream_t st) {
   return AM_OK;
 }
 
-// per-window elements of the largest activation written by layers [lo, hi) (lo == 0 includes the stem)
-static size_t max_act_range(const am_model* m, int T, size_t lo, size_t hi) {
-  Shape s = stem_out(*m->layers[0], T, m->n_mels);
-  size_t mx = lo == 0 ? (size_t)s.H * s.W * m->layers[0]->cout_p : 0;
-  for (size_t i = 1; i < hi && i < m->layers.size(); ++i) {
-    const Layer& l = *m->layers[i];
-    s = layer_out(l, s);
-    if (i >= lo) mx = std::max(mx, (size_t)std::max(s.H, 0) * std::max(s.W, 0) * l.cout_p);
-  }
-  return mx;
-}
-
-// windows per pass of the early phase for a call of n windows: at most max_sub, and few enough that one activation
-// buffer stays within kEarlyActBudget elements.  The buffers are sized for every layer output, the expanded tensors
-// included (blocks run layer by layer with AM_FUSED_BLOCKS=0 or when a block does not fit the fused kernel): ~50 MB
-// per 10 s window for the shipped student, so 256 windows would need three 14 GB buffers.
+// Windows per pass: the early phase takes at most kMaxSub (256 measured 1 % faster than 128), and few enough that one
+// activation buffer stays within kEarlyActBudget elements (the buffers hold every layer output, ~50 MB per 10 s window
+// for the shipped student, so 256 windows would need three 14 GB buffers); the late phase takes at most kLateSub.
+constexpr int kMaxSub = 256, kLateSub = 256;
 constexpr size_t kEarlyActBudget = (size_t)1 << 30;  // bf16 elements = 2 GiB per buffer
 
-static int early_sub(const am_model* m, int T, int n) {
-  Shape ss;
-  int cs;
-  const size_t per_win = std::max<size_t>(1, max_act_range(m, T, 0, late_start(m, T, &ss, &cs)));
-  const int cap = (int)std::max<size_t>(1, kEarlyActBudget / per_win);
-  return std::min({std::max(n, 1), m->max_sub, cap});
+static int early_sub(const ForwardPlan& p, int n) {
+  const int cap = (int)std::max<size_t>(1, kEarlyActBudget / std::max<size_t>(1, p.early_act));
+  return std::min({std::max(n, 1), kMaxSub, cap});
 }
 
-static int ensure_workspace(am_model* m, int T, int nb, int n_total) {
-  Shape ss;
-  int cs;
-  const size_t split = late_start(m, T, &ss, &cs);
+static int ensure_workspace(am_model* m, const ForwardPlan& p, int nb, int n_total) {
   const size_t nt = (size_t)std::max(n_total, 1);
-  static const int late_cap = std::getenv("AM_CLAP_LATE_SUB") ? std::max(1, std::atoi(std::getenv("AM_CLAP_LATE_SUB"))) : 256;
-  m->late_sub = (int)std::min<size_t>(nt, (size_t)late_cap);
-  const size_t need = std::max(max_act_range(m, T, 0, split) * (size_t)nb,
-                               max_act_range(m, T, split, m->layers.size()) * (size_t)m->late_sub);
+  m->late_sub = (int)std::min<size_t>(nt, (size_t)kLateSub);
+  const size_t need = std::max(p.early_act * (size_t)nb, p.late_act * (size_t)m->late_sub);
   if (need > m->act_elems) {
     for (auto& b : m->act) b.release();
     for (auto& b : m->act) AM_TRY(b.alloc(std::max<size_t>(need, 16)));
     m->act_elems = need;
   }
-  AM_TRY(m->late_in.ensure(nt * (size_t)std::max(ss.H, 1) * std::max(ss.W, 1) * cs));
+  AM_TRY(m->late_in.ensure(nt * (size_t)p.split.H * p.split.W * p.split_c));
   size_t kmax = 8;
   for (size_t r = 0; r < m->regs.size(); ++r) {
     AM_TRY(m->regs[r]->ensure(nt * (size_t)m->reg_dim[r]));
@@ -1388,11 +858,8 @@ static int finish_load(am_model* m, const am::ModelSpec& spec, am_model** out) {
     delete m;
     return s;
   }
-  const char* impl = std::getenv("AM_GEMM_IMPL");
-  m->use_simt_gemm = (impl && std::strcmp(impl, "simt") == 0) ? 1 : 0;
-  if (const char* sb = std::getenv("AM_CLAP_SUB_BATCH")) m->max_sub = std::max(1, std::atoi(sb));
   if (const char* fb = std::getenv("AM_FUSED_BLOCKS")) m->fused_blocks = std::atoi(fb) != 0;
-  if (!m->use_simt_gemm && !gemm::available()) {
+  if (!gemm::available()) {
     set_error("am_clap_load: the wgmma GEMM path is unavailable on this device; no fallback is shipped");
     delete m;
     return AM_ERR_NO_DEVICE;
@@ -1404,7 +871,7 @@ static int finish_load(am_model* m, const am::ModelSpec& spec, am_model** out) {
 // `path` (may be NULL) locates external tensor data of an ONNX model (model.onnx.data next to the model file)
 static int load_any(const void* blob, size_t nbytes, const char* path, am::ModelSpec* spec) {
   if (looks_like_onnx(blob, nbytes)) return load_onnx_spec(blob, nbytes, path, spec);
-  return parse_blob(blob, nbytes, spec);
+  return load_amw1_spec(blob, nbytes, spec);
 }
 
 extern "C" int am_clap_load_mem(const void* blob, size_t nbytes, am_model** out) {
@@ -1536,54 +1003,53 @@ static double head_macs(const am_model* m) {
   return macs;
 }
 
-extern "C" double am_clap_flops_per_segment(const am_model* m, int T) {
-  if (!m || m->layers.empty()) return 0.0;
-  Shape s = stem_out(*m->layers[0], T, m->n_mels);
-  const Layer& f = *m->layers[0];
-  double macs = f.type == kStem ? (double)s.H * s.W * (9.0 + f.cout) : (double)s.H * s.W * f.kh * f.kw * f.cout;
-  for (size_t i = 1; i < m->layers.size(); ++i) {
+// MACs of one window in the step's 1x1 convolutions and in its other layers
+static void step_macs(const am_model* m, const Step& t, double* pointwise, double* other) {
+  *pointwise = *other = 0.0;
+  Shape s = t.in;
+  for (size_t i = t.first; i <= t.last; ++i) {
     const Layer& l = *m->layers[i];
-    if (l.type == kDepthwise) {
-      s = dw_out(l, s);
-      macs += (double)s.H * s.W * l.cin * l.kh * l.kw;
-    } else if (l.type == kPointwise) {
-      macs += (double)s.H * s.W * l.cin * (double)l.cout;
-    } else if (l.type == kSqueezeExcite) {
-      macs += 2.0 * l.cin * l.cmid;
+    if (l.type == kPointwise) {
+      *pointwise += (double)s.H * s.W * l.cin * (double)l.cout;
+      continue;
     }
+    s = t.out;
+    if (l.type == kStem) *other += (double)s.H * s.W * (9.0 + l.cout);
+    if (l.type == kConvFirst) *other += (double)s.H * s.W * l.kh * l.kw * l.cout;
+    if (l.type == kDepthwise) *other += (double)s.H * s.W * l.cin * l.kh * l.kw;
+    if (l.type == kSqueezeExcite) *other += 2.0 * l.cin * l.cmid;
   }
-  return 2.0 * (macs + head_macs(m));
+}
+
+extern "C" double am_clap_flops_per_segment(const am_model* m, int T) {
+  ForwardPlan p;
+  if (!m || m->layers.empty() || build_plan(m, T, &p) != AM_OK) return 0.0;
+  double macs = head_macs(m);
+  for (const Step& t : p.steps) {
+    double pw, other;
+    step_macs(m, t, &pw, &other);
+    macs += pw + other;
+  }
+  return 2.0 * macs;
 }
 
 // flops (2 x MAC) of one window of T frames executed by the GEMM kernel and by the fused block kernel (pointwise +
-// depthwise inside fused blocks), and the fused blocks' algorithmic HBM bytes (block input + output, bf16), following
-// the same plan run_range uses
+// depthwise inside fused blocks), and the fused blocks' algorithmic HBM bytes (block input + output, bf16): sums over
+// the steps run_steps launches
 extern "C" int am_clap_flops_split(const am_model* m, int T, double* gemm_flops, double* fused_flops,
                                    double* fused_bytes) {
   AM_CHECK(m && gemm_flops && fused_flops && fused_bytes && !m->layers.empty(), "am_clap_flops_split: bad argument");
-  Shape s = stem_out(*m->layers[0], T, m->n_mels);
+  ForwardPlan p;
+  AM_TRY(build_plan(m, T, &p));
   double g = 0.0, f = 0.0, fb = 0.0;
-  for (size_t i = 1; i < m->layers.size(); ++i) {
-    const Layer& l = *m->layers[i];
-    fused::BlockDesc d;
-    fused::Plan pl;
-    int ex, dw, pj;
-    if (fused_block_at(m, i, m->layers.size(), s, &d, &pl, &ex, &dw, &pj)) {
-      const Layer& D = *m->layers[(size_t)dw];
-      const Layer& P = *m->layers[(size_t)pj];
-      const Shape o = dw_out(D, s);
-      double macs = (double)o.H * o.W * D.cin * 9.0 + (double)o.H * o.W * P.cin * (double)P.cout;
-      if (ex >= 0) macs += (double)s.H * s.W * m->layers[(size_t)ex]->cin * (double)m->layers[(size_t)ex]->cout;
-      f += 2.0 * macs;
-      fb += 2.0 * ((double)s.H * s.W * d.cin_p + (double)o.H * o.W * d.cout_p);
-      s = o;
-      i = (size_t)pj;
-      continue;
-    }
-    if (l.type == kDepthwise) {
-      s = dw_out(l, s);
-    } else if (l.type == kPointwise) {
-      g += 2.0 * (double)s.H * s.W * l.cin * (double)l.cout;
+  for (const Step& t : p.steps) {
+    double pw, other;
+    step_macs(m, t, &pw, &other);
+    if (t.kind == kStepFused) {
+      f += 2.0 * (pw + other);
+      fb += 2.0 * ((double)t.in.H * t.in.W * t.desc.cin_p + (double)t.out.H * t.out.W * t.desc.cout_p);
+    } else if (t.kind == kStepPointwise) {
+      g += 2.0 * pw;
     }
   }
   *gemm_flops = g;
@@ -1596,13 +1062,15 @@ extern "C" int am_clap_embed_dev(am_model* m, const float* mel_dev, int B, int T
   AM_CHECK(m && mel_dev && out_dev, "am_clap_embed_dev: NULL argument");
   AM_CHECK(B >= 0 && T > 0, "am_clap_embed_dev: bad shape B=%d T=%d", B, T);
   cudaStream_t st = (cudaStream_t)stream;
-  const int sub = early_sub(m, T, B);
-  AM_TRY(ensure_workspace(m, T, sub, B));
+  const ForwardPlan* p;
+  AM_TRY(plan_for(m, T, &p));
+  const int sub = early_sub(*p, B);
+  AM_TRY(ensure_workspace(m, *p, sub, B));
   for (int b0 = 0; b0 < B; b0 += sub) {
     const int nb = std::min(sub, B - b0);
-    AM_TRY(forward_early(m, mel_dev + (size_t)b0 * m->n_mels * T, nb, b0, T, st));
+    AM_TRY(forward_early(m, *p, mel_dev + (size_t)b0 * m->n_mels * T, nb, b0, st));
   }
-  AM_TRY(forward_late(m, B, T, st));
+  AM_TRY(forward_late(m, *p, B, st));
   return head_forward(m, B, out_dev, st);
 }
 
@@ -1631,16 +1099,18 @@ extern "C" int am_clap_embed_tracks_dev(am_model* m, const am_mel_plan* plan, co
   cudaStream_t st = (cudaStream_t)stream;
   const int hop = mel_plan_hop(plan);
   const int T = 1 + n_samples / hop;
-  const int sub = early_sub(m, T, n_segments);
-  AM_TRY(ensure_workspace(m, T, sub, n_segments));
+  const ForwardPlan* p;
+  AM_TRY(plan_for(m, T, &p));
+  const int sub = early_sub(*p, n_segments);
+  AM_TRY(ensure_workspace(m, *p, sub, n_segments));
   AM_TRY(m->mel_ws.ensure((size_t)sub * m->n_mels * T));
   AM_TRY(m->seg_emb.ensure((size_t)std::max(n_segments, 1) * m->emb));
   for (int b0 = 0; b0 < n_segments; b0 += sub) {
     const int nb = std::min(sub, n_segments - b0);
     AM_TRY(am_mel_batch_dev(plan, pcm_dev + (size_t)b0 * n_samples, 1, nb, n_samples, m->mel_ws.p, st));
-    AM_TRY(forward_early(m, m->mel_ws.p, nb, b0, T, st));
+    AM_TRY(forward_early(m, *p, m->mel_ws.p, nb, b0, st));
   }
-  AM_TRY(forward_late(m, n_segments, T, st));
+  AM_TRY(forward_late(m, *p, n_segments, st));
   AM_TRY(head_forward(m, n_segments, m->seg_emb.p, st));
   AM_LAUNCH(track_pool_kernel, n_tracks, 256, 0, st, m->seg_emb.p, seg_offsets_dev, m->emb, out_dev);
   return AM_OK;
@@ -1693,9 +1163,11 @@ extern "C" int am_clap_embed_tracks_submit(am_model* m, const am_mel_cfg* cfg, c
     if (!m->ev_done[i]) AM_CUDA(cudaEventCreateWithFlags(&m->ev_done[i], cudaEventDisableTiming));
   }
   const int T = 1 + n_samples / cfg->hop;
-  const int sub = early_sub(m, T, n_segments);
+  const ForwardPlan* p;
+  AM_TRY(plan_for(m, T, &p));
+  const int sub = early_sub(*p, n_segments);
   // (growing a workspace buffer while a batch is in flight is safe: cudaFree waits for the device)
-  AM_TRY(ensure_workspace(m, T, sub, n_segments));
+  AM_TRY(ensure_workspace(m, *p, sub, n_segments));
   AM_TRY(m->mel_ws.ensure((size_t)sub * m->n_mels * T));
   AM_TRY(m->seg_emb.ensure((size_t)std::max(n_segments, 1) * m->emb));
   for (auto& b : m->pcm_stage) AM_TRY(b.ensure((size_t)sub * n_samples));
@@ -1729,10 +1201,10 @@ extern "C" int am_clap_embed_tracks_submit(am_model* m, const am_mel_cfg* cfg, c
       AM_CUDA(cudaStreamWaitEvent(st, m->ev_copied[slot], 0));
       AM_TRY(am_mel_batch_dev(plan, m->pcm_stage[slot].p, 1, nb, n_samples, m->mel_ws.p, st));
       AM_CUDA(cudaEventRecord(m->ev_done[slot], st));  // the mel kernel was the staging slot's only reader
-      AM_TRY(forward_early(m, m->mel_ws.p, nb, b0, T, st));
+      AM_TRY(forward_early(m, *p, m->mel_ws.p, nb, b0, st));
       b0 += nb;
     }
-    AM_TRY(forward_late(m, n_segments, T, st));
+    AM_TRY(forward_late(m, *p, n_segments, st));
     AM_TRY(head_forward(m, n_segments, m->seg_emb.p, st));
     AM_LAUNCH(track_pool_kernel, n_tracks, 256, 0, st, m->seg_emb.p, m->off_stage.p, m->emb, m->out_stage.p);
     AM_CUDA(cudaMemcpyAsync(tk.stage.p, m->out_stage.p, out_count * 4, cudaMemcpyDeviceToHost, st));

@@ -1,6 +1,6 @@
 // Kernels of the graph-driven encoder path that are NOT part of the PhiNet fast path: first convolution with
 // an arbitrary small kernel, depthwise K x K with any activation, squeeze-excite, and the head's row program.
-// Included by encoder.cu only.  Layout conventions as in encoder.cu (NHWC bf16, channels padded to 16).
+// Included by encoder.cu and depthwise.cu (hence static kernels).  Layout conventions as in encoder.cu (NHWC bf16, channels padded to 16).
 #pragma once
 
 #include "common.cuh"
@@ -35,7 +35,7 @@ __device__ __forceinline__ uint4 pack8_bf16(const float (&o)[8]) {
 // h_is_time: image (H, W) = (time, mel) (PhiNet view) else (mel, time) (plain NCHW view of the input).
 // Per-mel affine (bn0) applied to in-range samples; padding contributes exact zeros.
 // One thread = one output pixel x one 8-channel group; weights [kh*kw, Cp] + bias staged in shared memory.
-__global__ void __launch_bounds__(256)
+static __global__ void __launch_bounds__(256)
 conv_first_kernel(const float* __restrict__ mel, int B, int n_mels, int T, int Ho, int Wo, int kh, int kw, int stride,
                   int pad_t, int pad_l, int h_is_time, const float* __restrict__ sc, const float* __restrict__ sh,
                   const float* __restrict__ w /* [kh*kw, cp] */, const float* __restrict__ bias, int cp, int act,
@@ -80,7 +80,7 @@ conv_first_kernel(const float* __restrict__ mel, int B, int n_mels, int T, int H
 
 // Depthwise K x K (K odd, <= 7), stride 1 / 2, arbitrary zero padding, folded BN bias, any trunk activation.
 // fp32 accumulation.  One thread = one output pixel x one 8-channel group (coalesced 16-byte accesses).
-__global__ void __launch_bounds__(256)
+static __global__ void __launch_bounds__(256)
 depthwise_generic_kernel(const __nv_bfloat16* __restrict__ in, int B, int H, int W, int cp, int Ho, int Wo, int k,
                          int stride, int pad_t, int pad_l, const float* __restrict__ w /* [k*k, cp] */,
                          const float* __restrict__ bias, int act, __nv_bfloat16* __restrict__ out) {
@@ -123,7 +123,7 @@ depthwise_generic_kernel(const __nv_bfloat16* __restrict__ in, int B, int H, int
 }
 
 // squeeze: mean over (H, W) of NHWC bf16 -> f32 [B, C].  grid (ceil(C / 64), B), 256 threads: 64 channels x 4 pixel lanes.
-__global__ void __launch_bounds__(256)
+static __global__ void __launch_bounds__(256)
 channel_mean_kernel(const __nv_bfloat16* __restrict__ in, int HW, int cp, int C, float* __restrict__ out) {
   __shared__ float s_part[4][64];
   const int c = blockIdx.x * 64 + (threadIdx.x & 63), lane = threadIdx.x >> 6, b = blockIdx.y;
@@ -138,7 +138,7 @@ channel_mean_kernel(const __nv_bfloat16* __restrict__ in, int HW, int cp, int C,
 
 // the two tiny fully connected layers of a squeeze-excite gate, one CTA per window:
 // gate[b, c] = gate_act( W2 . inner_act( W1 . mean[b] + b1 ) + b2 )
-__global__ void __launch_bounds__(256)
+static __global__ void __launch_bounds__(256)
 se_gate_kernel(const float* __restrict__ mean, int C, int Cm, const float* __restrict__ w1, const float* __restrict__ b1,
                const float* __restrict__ w2, const float* __restrict__ b2, int inner_act, int gate_act,
                float* __restrict__ gate) {
@@ -164,7 +164,7 @@ se_gate_kernel(const float* __restrict__ mean, int C, int Cm, const float* __res
 }
 
 // excite: y[b, p, c] = x[b, p, c] * gate[b, c]   (8 channels per thread)
-__global__ void __launch_bounds__(256)
+static __global__ void __launch_bounds__(256)
 se_scale_kernel(const __nv_bfloat16* __restrict__ in, int64_t HW, int cp, int C, const float* __restrict__ gate, int B,
                 __nv_bfloat16* __restrict__ out) {
   const int groups = cp >> 3;
@@ -188,14 +188,14 @@ se_scale_kernel(const __nv_bfloat16* __restrict__ in, int64_t HW, int cp, int C,
 }
 
 // ---------------------------------------------------------------- head row program (f32 [n, dim])
-__global__ void vec_unary_kernel(const float* __restrict__ x, int64_t n, int act, float* __restrict__ y) {
+static __global__ void vec_unary_kernel(const float* __restrict__ x, int64_t n, int act, float* __restrict__ y) {
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
     y[i] = apply_act(act, x[i]);
 }
-__global__ void vec_add_kernel(const float* __restrict__ a, const float* __restrict__ b, int64_t n, float* __restrict__ y) {
+static __global__ void vec_add_kernel(const float* __restrict__ a, const float* __restrict__ b, int64_t n, float* __restrict__ y) {
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) y[i] = a[i] + b[i];
 }
-__global__ void vec_affine_kernel(const float* __restrict__ x, int64_t n, int dim, const float* __restrict__ scale,
+static __global__ void vec_affine_kernel(const float* __restrict__ x, int64_t n, int dim, const float* __restrict__ scale,
                                   const float* __restrict__ shift, float* __restrict__ y) {
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
     const int c = (int)(i % dim);
@@ -223,7 +223,7 @@ __device__ __forceinline__ float block_sum_256(float v, float* s_red, float* s_o
 }
 
 // one CTA per row: y = (x - mean) * rsqrt(var + eps) * g + b
-__global__ void __launch_bounds__(256)
+static __global__ void __launch_bounds__(256)
 vec_layernorm_kernel(const float* __restrict__ x, int E, const float* __restrict__ g, const float* __restrict__ bt, float eps,
                      float* __restrict__ y) {
   __shared__ float s_red[32];
@@ -242,7 +242,7 @@ vec_layernorm_kernel(const float* __restrict__ x, int E, const float* __restrict
 }
 
 // one CTA per row: y = x / max(||x||, eps)
-__global__ void __launch_bounds__(256)
+static __global__ void __launch_bounds__(256)
 vec_l2norm_kernel(const float* __restrict__ x, int E, float eps, float* __restrict__ y) {
   __shared__ float s_red[32];
   __shared__ float s_out;

@@ -1,4 +1,4 @@
-// Host-side description of an audio encoder, produced by a loader (AMW1 blob reader in encoder.cu, ONNX graph
+// Host-side description of an audio encoder, produced by a loader (AMW1 blob reader in amw1_model.cu, ONNX graph
 // lowering in onnx_model.cu) and consumed by encoder.cu's build_model(): folded fp32 weights + the layer program.
 //
 // The trunk is a chain of NHWC layers (one live residual source at a time: the input of the latest
@@ -66,5 +66,7 @@ struct ModelSpec {
 // Returns AM_OK or an am_status with am_last_error() naming the unsupported node / pattern.
 int load_onnx_spec(const void* data, size_t nbytes, const char* path, ModelSpec* out);
 bool looks_like_onnx(const void* data, size_t nbytes);
+// amw1_model.cu: reads an AMW1 blob (audiomuse-ai_b200/weights.py).  AM_OK, or AM_ERR_IO with am_last_error() set.
+int load_amw1_spec(const void* blob, size_t nbytes, ModelSpec* spec);
 
 }  // namespace am

@@ -51,6 +51,25 @@ def test_fused_block_kernel_matches_the_layer_by_layer_path(tmp_path):
     assert np.abs(got - ref).max() < 2e-3
 
 
+def test_one_model_follows_a_changing_window_length():
+    """The execution plan is kept per window length: 1001, 333 and again 1001 frames on one model give what a fresh
+    model gives for each length, also after the workspace was released."""
+    from audiomuse_ai_b200 import clap_analyzer as ca, weights
+
+    def embed(sess, T):
+        mel = (np.random.default_rng(T).standard_normal((3, 1, 128, T)) * 12 - 30).astype(np.float32)
+        return sess.run(None, {"mel_spectrogram": mel})[0]
+
+    blob = weights.export_blob(weights.random_state_dict(0))
+    fresh = {T: embed(ca.B200Session(blob), T) for T in (1001, 333)}
+    sess = ca.B200Session(blob)
+    for T in (1001, 333, 1001):
+        np.testing.assert_array_equal(embed(sess, T), fresh[T])
+    sess.release_workspace()
+    for T in (333, 1001):
+        np.testing.assert_array_equal(embed(sess, T), fresh[T])
+
+
 def test_short_window_runs_through_the_partial_tiles(tmp_path):
     """T = 333 frames: spatial sizes that are no multiple of the 8 x 8 tile (the last tiles of every block are partial)."""
     ref = _embed(tmp_path, "layer_by_layer_s", {"AM_FUSED_BLOCKS": "0"}, T=333)
