@@ -14,8 +14,8 @@
 //                 all 5 m blocks, one 32-column half of the chunk per warpgroup; fp32 accumulators -> + bias, ReLU6
 //                 -> bf16 halo tile E [halo pixels x 64, 16-byte groups XOR-swizzled by pixel] (pixels outside the
 //                 image are zero: the depthwise pads with 0, and relu6(bias) need not be);
-//     depthwise   3 x 3 taps from E in fp32 (a thread = 8 channels of two adjacent output pixels) + bias, ReLU6 ->
-//                 bf16, written as the K-major swizzled A operand [64 pixels x 64 channels] of
+//     depthwise   3 x 3 taps from E in fp32 (a thread = 2 channels of one output column, walking its input rows) +
+//                 bias, ReLU6 -> bf16, written as the K-major swizzled A operand [64 pixels x 64 channels] of
 //     projection  wgmma m64n64k16 into register accumulators, 64-column blocks split between the warpgroups (Cout <=
 //                 256), accumulated over the chunks in ascending order.
 //   With two or more stages the chunks overlap: chunk c + 1's expansion MMAs are issued before chunk c's depthwise and
@@ -205,7 +205,6 @@ fused_block_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_const
   const int wg = __shfl_sync(0xffffffffu, ct >> 7, 0), wt = ct & 127;
   const int warp = wt >> 5, lane = wt & 31, quad = lane & 3;
   __nv_bfloat16* e_own = reinterpret_cast<__nv_bfloat16*>(own + a.l.e);  // [HPX][64], plain rows of 128 bytes
-  const uint4 zero4 = make_uint4(0u, 0u, 0u, 0u);
   const int nchunks = (a.cmid_p + kChunk - 1) / kChunk;
   // With two or more stages chunk c + 1's expansion reads its stage while chunk c's is still held; a one-stage ring
   // cannot hold both, so there the expansion waits for chunk c's projection and the stage it frees.
@@ -244,11 +243,16 @@ fused_block_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_const
       }
     wgmma_commit();
   };
-  // E columns of this warpgroup = relu6(acc1 + b1), zero outside the image and past the chunk's channels
+  // E columns of this warpgroup = relu6(acc1 + b1), zero outside the image and past the chunk's channels.  The bias
+  // columns are read into registers before the first store into E (the compiler cannot move shared-memory loads above
+  // stores that may alias them), and the zero cases are selects, so each bf16 pair is a short branch-free chain.
   auto expand_epilogue = [&](const uint8_t* stage, int nch, int gy0, int gx0) {
 #pragma unroll
     for (int m = 0; m < kEM; ++m) reg_fence(acc1[m]);
     const float* b1 = reinterpret_cast<const float*>(stage + a.l.dw) + 10 * kChunk;
+    float2 bias[kEN / 8];  // columns n0 + 8 j + 2 quad and the one after
+#pragma unroll
+    for (int j = 0; j < kEN / 8; ++j) bias[j] = *reinterpret_cast<const float2*>(b1 + n0 + 8 * j + 2 * quad);
 #pragma unroll
     for (int m = 0; m < kEM; ++m)
 #pragma unroll
@@ -259,12 +263,9 @@ fused_block_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_const
         const bool inside = gy >= 0 && gy < a.H && gx >= 0 && gx < a.W;
 #pragma unroll
         for (int j = 0; j < kEN / 8; ++j) {
-          const int col = n0 + 8 * j + 2 * quad;
-          float f0 = 0.f, f1 = 0.f;
-          if (inside && col < nch) {
-            f0 = relu6f(acc1[m][4 * j + 2 * h] + b1[col]);
-            f1 = relu6f(acc1[m][4 * j + 2 * h + 1] + b1[col + 1]);
-          }
+          const bool keep = inside && n0 + 8 * j + 2 * quad < nch;
+          const float f0 = keep ? relu6f(acc1[m][4 * j + 2 * h] + bias[j].x) : 0.f;
+          const float f1 = keep ? relu6f(acc1[m][4 * j + 2 * h + 1] + bias[j].y) : 0.f;
           *reinterpret_cast<__nv_bfloat162*>(e_own + e_off(p, n0 / 8 + j) + 2 * quad) = __floats2bfloat162_rn(f0, f1);
         }
       }
@@ -308,48 +309,54 @@ fused_block_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_const
         clk.lap(kExpandMma);
       }
 
-      // depthwise: a thread = 8 channels (group g) of two horizontally adjacent output pixels, so each tap's weights
-      // are loaded once for both
+      // depthwise: a thread = one channel pair (2 cp, 2 cp + 1) of one output column ox, a warp = all 64 channels of
+      // that column, so every E load and A store of a warp is one 128-byte pixel row (conflict-free under the XOR
+      // swizzles).  The thread walks the column's HALO input rows top to bottom, converts each of the row's 3 taps once
+      // and adds it into every output row that uses it; per output the order stays bias, then dy and dx ascending.
       {
-        const int g = ct & 7, px = (ct >> 3) * 2;
-        const int oy = px >> 3, ox = px & 7;
-        uint4 out[2] = {zero4, zero4};
-        if (g * 8 < nch) {
-          const float* bias = dwp + 9 * kChunk + g * 8;
-          float acc[2][8];
+        const int ox = ct >> 5, cp = lane, g = cp >> 2;
+        uint32_t out[kTile] = {};  // bf16 pairs of output rows 0 .. 7; lanes past the chunk's channels write zeros
+        if (2 * cp < nch) {
+          float2 w[9];
 #pragma unroll
-          for (int q = 0; q < 8; ++q) acc[0][q] = acc[1][q] = bias[q];
+          for (int t = 0; t < 9; ++t) w[t] = *reinterpret_cast<const float2*>(dwp + t * kChunk + 2 * cp);
+          const float2 bias = *reinterpret_cast<const float2*>(dwp + 9 * kChunk + 2 * cp);
+          float2 acc[kTile];
 #pragma unroll
-          for (int dy = 0; dy < 3; ++dy)
+          for (int oy = 0; oy < kTile; ++oy) acc[oy] = bias;
+          // halo pixel ox * S + d (d = iy * HALO + dx) is at col[d & 7] + 64 d: its swizzle depends on d only mod 8
+          const __nv_bfloat16* col[8];
+#pragma unroll
+          for (int k = 0; k < 8; ++k) col[k] = e + ox * S * 64 + ((g ^ ((ox * S + k) & 7)) << 3) + 2 * (cp & 3);
+#pragma unroll
+          for (int iy = 0; iy < HALO; ++iy) {
+            float2 v[3];
 #pragma unroll
             for (int dx = 0; dx < 3; ++dx) {
-              const float4* w4 = reinterpret_cast<const float4*>(dwp + (dy * 3 + dx) * kChunk + g * 8);
-              const float4 wa = w4[0], wb = w4[1];
-              const float w[8] = {wa.x, wa.y, wa.z, wa.w, wb.x, wb.y, wb.z, wb.w};
-#pragma unroll
-              for (int i = 0; i < 2; ++i) {
-                const int hp = (oy * S + dy) * HALO + (ox + i) * S + dx;
-                const uint4 v = *reinterpret_cast<const uint4*>(e + e_off(hp, g));
-                const __nv_bfloat162* v2 = reinterpret_cast<const __nv_bfloat162*>(&v);
-#pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                  const float2 f = __bfloat1622float2(v2[q]);
-                  acc[i][2 * q] = fmaf(f.x, w[2 * q], acc[i][2 * q]);
-                  acc[i][2 * q + 1] = fmaf(f.y, w[2 * q + 1], acc[i][2 * q + 1]);
-                }
-              }
+              const int d = iy * HALO + dx;
+              v[dx] = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(col[d & 7] + d * 64));
             }
 #pragma unroll
-          for (int i = 0; i < 2; ++i) {
-            __nv_bfloat162 o2[4];
+            for (int dy = 0; dy < 3; ++dy) {  // output row oy takes input row iy as its tap row dy
+              if (iy < dy || (iy - dy) % S != 0 || (iy - dy) / S >= kTile) continue;
+              const int oy = (iy - dy) / S;
 #pragma unroll
-            for (int q = 0; q < 4; ++q)
-              o2[q] = __floats2bfloat162_rn(relu6f(acc[i][2 * q]), relu6f(acc[i][2 * q + 1]));
-            out[i] = *reinterpret_cast<const uint4*>(o2);
+              for (int dx = 0; dx < 3; ++dx) {
+                acc[oy].x = fmaf(v[dx].x, w[dy * 3 + dx].x, acc[oy].x);
+                acc[oy].y = fmaf(v[dx].y, w[dy * 3 + dx].y, acc[oy].y);
+              }
+            }
+          }
+#pragma unroll
+          for (int oy = 0; oy < kTile; ++oy) {
+            const __nv_bfloat162 o = __floats2bfloat162_rn(relu6f(acc[oy].x), relu6f(acc[oy].y));
+            out[oy] = *reinterpret_cast<const uint32_t*>(&o);
           }
         }
+        // A row 8 oy + ox: its swizzle depends on ox only (sw128 takes the row mod 8)
+        uint8_t* arow = a2 + sw128(ox, g) + 4 * (cp & 3);
 #pragma unroll
-        for (int i = 0; i < 2; ++i) *reinterpret_cast<uint4*>(a2 + sw128(px + i, g)) = out[i];
+        for (int oy = 0; oy < kTile; ++oy) *reinterpret_cast<uint32_t*>(arow + oy * kTile * 128) = out[oy];
       }
       fence_proxy_async();  // generic-proxy writes of A -> visible to the wgmma (async proxy) reads
       clk.lap(kDepthwise);
