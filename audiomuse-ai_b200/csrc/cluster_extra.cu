@@ -327,11 +327,7 @@ extern "C" int am_pca_project(const float* X, int64_t N, int d, const double* me
   AM_CUDA(cudaMemcpyAsync(dW.p, components, (size_t)k * d * 4, cudaMemcpyHostToDevice, st.s));
   const size_t smem = (size_t)8 * d * 4;
   AM_CHECK(smem <= 200 * 1024, "am_pca_project: %d features do not fit the row buffer", d);
-  static size_t attr = 0;
-  if (smem > 48 * 1024 && smem > attr) {
-    AM_CUDA(cudaFuncSetAttribute(pca_project_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr = smem;
-  }
+  AM_TRY(allow_dynamic_smem<pca_project_kernel>(200 * 1024));
   const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((N + 7) / 8, (int64_t)sm_count() * 8));
   AM_LAUNCH(pca_project_kernel, grid, 256, smem, st.s, dX.p, N, d, dM.p, dW.p, k, dY.p);
   AM_CUDA(cudaMemcpyAsync(Y, dY.p, (size_t)N * k * 4, cudaMemcpyDeviceToHost, st.s));

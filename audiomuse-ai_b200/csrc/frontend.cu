@@ -361,12 +361,8 @@ extern "C" int64_t am_resample_out_len(const am_resample_plan* p, int64_t n_in) 
 extern "C" int am_resample_dev(const am_resample_plan* p, const float* x_dev, int64_t n_in, float* y_dev, void* stream) {
   AM_CHECK(p && x_dev && y_dev && n_in > 0, "am_resample_dev: bad argument");
   const int64_t n_out = am_resample_out_len(p, n_in);
-  const size_t smem = p->host.poly.size() * 4;
-  static size_t attr = 0;
-  if (smem > 48 * 1024 && smem > attr) {
-    AM_CUDA(cudaFuncSetAttribute(resample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr = smem;
-  }
+  const size_t smem = p->host.poly.size() * 4;  // <= 200 KiB (am_resample_plan_create)
+  AM_TRY(allow_dynamic_smem<resample_kernel>(200 * 1024));
   const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((n_out + 255) / 256, (int64_t)sm_count() * 8));
   AM_LAUNCH(resample_kernel, grid, 256, smem, (cudaStream_t)stream, x_dev, n_in, p->poly_dev.p, p->host.up, p->host.down,
             p->host.taps, p->host.n_pre_remove, y_dev, n_out);

@@ -54,24 +54,15 @@ int gemm_bf16_simt(const __nv_bfloat16* A, int64_t M, int64_t lda, const __nv_bf
                    int64_t ldb, int K, void* D, int64_t ldd, bool d_is_f32, const Epilogue& ep,
                    cudaStream_t st);
 
-// S[q, j] = Qb[q, :] . Xb[j, :]  (2*dot - xnorm2[j] when xnorm2 != NULL), fp32 out.
-// Qb has `qrows` rows (multiple of 128, zero padded).
-inline int scores_bf16(const __nv_bfloat16* Qb, int qrows, const __nv_bfloat16* Xb, int64_t N, int dpad,
-                       float* S, int64_t ldS, const float* xnorm2, cudaStream_t st) {
-  Epilogue ep;
-  ep.alpha = xnorm2 ? 2.0f : 1.0f;
-  ep.col_sub = xnorm2;
-  return gemm_bf16(Qb, qrows, dpad, Xb, N, dpad, dpad, S, ldS, true, ep, /*m_fastest=*/true, st);
-}
-
-// same scores + the maximum of every 32 consecutive ones: CM[q, j / 32]
-inline int scores_chunkmax_bf16(const __nv_bfloat16* Qb, int qrows, const __nv_bfloat16* Xb, int64_t N, int dpad,
-                                float* S, int64_t ldS, float* CM, int64_t ldCM, const float* xnorm2, cudaStream_t st) {
+// S[q, j] = Qb[q, :] . Xb[j, :]  (2*dot - xnorm2[j] when xnorm2 != NULL), fp32 out; CM != NULL: also the maximum of
+// every 32 consecutive scores, CM[q, j / 32].  Qb has `qrows` rows (multiple of 128, zero padded).
+inline int scores_bf16(const __nv_bfloat16* Qb, int qrows, const __nv_bfloat16* Xb, int64_t N, int dpad, float* S,
+                       int64_t ldS, float* CM, int64_t ldCM, const float* xnorm2, cudaStream_t st) {
   Epilogue ep;
   ep.alpha = xnorm2 ? 2.0f : 1.0f;
   ep.col_sub = xnorm2;
   ep.chunk_max = CM;
-  ep.ld_cm = ldCM;
+  ep.ld_cm = CM ? ldCM : 0;
   return gemm_bf16(Qb, qrows, dpad, Xb, N, dpad, dpad, S, ldS, true, ep, /*m_fastest=*/true, st);
 }
 

@@ -257,11 +257,7 @@ static int launch_accumulate(const float* X, int64_t N, int d, const int32_t* la
   const int W = accumulate_width(k);
   const size_t smem = (size_t)k * W * 4;
   AM_CHECK(smem <= 200 * 1024, "kmeans: k=%d too large for the shared-memory accumulation slab", k);
-  static size_t attr_smem = 0;
-  if (smem > attr_smem) {
-    AM_CUDA(cudaFuncSetAttribute(accumulate_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr_smem = smem;
-  }
+  AM_TRY(allow_dynamic_smem<accumulate_kernel>(200 * 1024));
   const int ppc = 4096;
   dim3 grid((unsigned)((N + ppc - 1) / ppc), (unsigned)ceil_div(d, W));
   AM_LAUNCH(accumulate_kernel, grid, 256, smem, st, X, N, d, labels, k, W, ppc, sums);

@@ -16,7 +16,7 @@
 
 #include <algorithm>
 #include <cmath>
-#include <mutex>
+#include <memory>
 
 #include "gemm_wgmma.cuh"
 
@@ -42,8 +42,6 @@ struct am_index {
   int dpad = 0;
   float max_norm = 1.0f;      // max ||x|| over stored rows
   float xres_max = 0.0f;      // max ||x - bf16(x)|| over stored rows
-  std::vector<float> host;    // lazy host mirror for get_vector
-  std::mutex host_mu;
 };
 
 namespace am {
@@ -487,6 +485,21 @@ __device__ __forceinline__ float score_eps(const SelectParams& p, int q) {
   return eps;
 }
 
+// one compare-exchange of a bitonic network sorting by (distance asc, id asc): the pair (lo, hi) is put in ascending
+// order when `up`, in descending order otherwise
+template <class I>
+__device__ __forceinline__ void bitonic_exchange(double* dist, int* ids, I lo, I hi, bool up) {
+  const double dl = dist[lo], dh = dist[hi];
+  const int il = ids[lo], ih = ids[hi];
+  const bool gt = (dl > dh) || (dl == dh && il > ih);
+  if (gt == up) {
+    dist[lo] = dh;
+    dist[hi] = dl;
+    ids[lo] = ih;
+    ids[hi] = il;
+  }
+}
+
 // exact float64 distances of the `count` candidate rows in c_id (one warp per candidate), bitonic sort by
 // (distance asc, id asc), first k written out.  All threads of the CTA; c_id / c_dist hold kCandCap entries.
 __device__ void rerank_sort_emit(const SelectParams& p, int q, unsigned count, double* c_dist, int* c_id) {
@@ -507,17 +520,7 @@ __device__ void rerank_sort_emit(const SelectParams& p, int q, unsigned count, d
     for (unsigned stride = size >> 1; stride > 0; stride >>= 1) {
       for (unsigned t = tid; t < n2 / 2; t += kSelThreads) {
         const unsigned lo = 2 * t - (t & (stride - 1));
-        const unsigned hi = lo + stride;
-        const bool up = ((lo & size) == 0);
-        const double dl = c_dist[lo], dh = c_dist[hi];
-        const int il = c_id[lo], ih = c_id[hi];
-        const bool gt = (dl > dh) || (dl == dh && il > ih);
-        if (gt == up) {
-          c_dist[lo] = dh;
-          c_dist[hi] = dl;
-          c_id[lo] = ih;
-          c_id[hi] = il;
-        }
+        bitonic_exchange(c_dist, c_id, lo, lo + stride, (lo & size) == 0);
       }
       __syncthreads();
     }
@@ -746,17 +749,7 @@ __global__ void bitonic_step_kernel(double* __restrict__ dist, int* __restrict__
   const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (t >= npad / 2) return;
   const int64_t lo = 2 * t - (t & (int64_t)(stride - 1));
-  const int64_t hi = lo + stride;
-  const bool up = ((lo & size) == 0);
-  const double dl = dist[lo], dh = dist[hi];
-  const int il = ids[lo], ih = ids[hi];
-  const bool gt = (dl > dh) || (dl == dh && il > ih);
-  if (gt == up) {
-    dist[lo] = dh;
-    dist[hi] = dl;
-    ids[lo] = ih;
-    ids[hi] = il;
-  }
+  bitonic_exchange(dist, ids, lo, lo + (int64_t)stride, (lo & size) == 0);
 }
 
 __global__ void emit_topk_kernel(const double* __restrict__ dist, const int* __restrict__ ids, int k,
@@ -812,6 +805,27 @@ static float reduce_max_host(const float* dev, int64_t n, cudaStream_t st, int* 
 constexpr int kFilterThreads = 256;
 constexpr int kFilterCap = 4096;  // items per list
 
+// get_direct_distance (voyager_manager.py:99-140) between stored rows a and b, one warp, float64 accumulation:
+// euclidean ||a - b||, otherwise 1 - cos (+inf when either row is zero)
+__device__ __forceinline__ double direct_distance(const float* a, const float* b, int d, int metric, int lane) {
+  double dot = 0.0, na = 0.0, nb = 0.0, d2 = 0.0;
+  for (int t = lane; t < d; t += 32) {
+    const double av = (double)__ldg(&a[t]), bv = (double)__ldg(&b[t]);
+    dot = fma(av, bv, dot);
+    na = fma(av, av, na);
+    nb = fma(bv, bv, nb);
+    const double df = av - bv;
+    d2 = fma(df, df, d2);
+  }
+  dot = warp_sum(dot);
+  na = warp_sum(na);
+  nb = warp_sum(nb);
+  d2 = warp_sum(d2);
+  if (metric == kMetricL2) return sqrt(d2);
+  const double den = sqrt(na) * sqrt(nb);
+  return den == 0.0 ? INFINITY : 1.0 - fmin(1.0, fmax(-1.0, dot / den));
+}
+
 __global__ void __launch_bounds__(kFilterThreads)
 filter_by_distance_kernel(const float* __restrict__ X, int64_t N, int d, int metric, const int64_t* __restrict__ ids,
                           int n, double threshold, int lookback, int batch, unsigned char* __restrict__ keep) {
@@ -832,27 +846,7 @@ filter_by_distance_kernel(const float* __restrict__ X, int64_t N, int d, int met
       const int start = max(0, (batched ? base : kept) - lookback);
       const float* a = X + row * d;
       for (int j = start + warp; j < kept; j += warps) {
-        const float* b = X + (int64_t)s_kept[j] * d;
-        double dot = 0.0, na = 0.0, nb = 0.0, d2 = 0.0;
-        for (int t = lane; t < d; t += 32) {
-          const double av = (double)__ldg(&a[t]), bv = (double)__ldg(&b[t]);
-          dot = fma(av, bv, dot);
-          na = fma(av, av, na);
-          nb = fma(bv, bv, nb);
-          const double df = av - bv;
-          d2 = fma(df, df, d2);
-        }
-        dot = warp_sum(dot);
-        na = warp_sum(na);
-        nb = warp_sum(nb);
-        d2 = warp_sum(d2);
-        double dist;
-        if (metric == kMetricL2) {
-          dist = sqrt(d2);
-        } else {
-          const double den = sqrt(na) * sqrt(nb);
-          dist = den == 0.0 ? INFINITY : 1.0 - fmin(1.0, fmax(-1.0, dot / den));
-        }
+        const double dist = direct_distance(a, X + (int64_t)s_kept[j] * d, d, metric, lane);
         if (lane == 0 && dist < threshold) s_close = 1;
       }
     }
@@ -886,29 +880,7 @@ pairwise_direct_kernel(const float* __restrict__ X, int64_t N, int d, int metric
     const int j = i + (int)(pidx - ((int64_t)i * n - (int64_t)i * (i - 1) / 2));
     const int64_t ra = ids[i], rb = ids[j];
     float res = INFINITY;  // a missing vector: the reference returns +inf
-    if (ra >= 0 && ra < N && rb >= 0 && rb < N) {
-      const float* a = X + ra * d;
-      const float* b = X + rb * d;
-      double dot = 0.0, na = 0.0, nb = 0.0, d2 = 0.0;
-      for (int t = lane; t < d; t += 32) {
-        const double av = (double)__ldg(&a[t]), bv = (double)__ldg(&b[t]);
-        dot = fma(av, bv, dot);
-        na = fma(av, av, na);
-        nb = fma(bv, bv, nb);
-        const double df = av - bv;
-        d2 = fma(df, df, d2);
-      }
-      dot = warp_sum(dot);
-      na = warp_sum(na);
-      nb = warp_sum(nb);
-      d2 = warp_sum(d2);
-      if (metric == kMetricL2) {
-        res = (float)sqrt(d2);
-      } else {
-        const double den = sqrt(na) * sqrt(nb);
-        res = den == 0.0 ? INFINITY : (float)(1.0 - fmin(1.0, fmax(-1.0, dot / den)));
-      }
-    }
+    if (ra >= 0 && ra < N && rb >= 0 && rb < N) res = (float)direct_distance(X + ra * d, X + rb * d, d, metric, lane);
     if (lane == 0) {
       out[(int64_t)i * n + j] = res;
       out[(int64_t)j * n + i] = res;
@@ -931,13 +903,31 @@ __global__ void gather_rows_kernel(const float* __restrict__ X, int64_t N, int d
 
 using namespace am;
 
-static int finish_build(am_index* idx, cudaStream_t st) {
-  const int64_t N = idx->N;
-  const int d = idx->d;
+// the body of am_knn_build (X in host memory, kind = cudaMemcpyHostToDevice, on a stream of its own) and
+// am_knn_build_dev (X in device memory, kind = cudaMemcpyDeviceToDevice, on the caller's stream `st`)
+static int build_index(const char* fn, const float* X, int64_t N, int d, int metric, cudaMemcpyKind kind, cudaStream_t st,
+                       am_index** out) {
+  AM_CHECK(out != nullptr, "%s: out is NULL", fn);
+  *out = nullptr;
+  AM_CHECK(N >= 0 && d > 0 && (X != nullptr || N == 0), "%s: bad shape N=%lld d=%d", fn, (long long)N, d);
+  AM_CHECK(metric >= 0 && metric <= 2, "%s: metric must be 0 (cosine), 1 (euclidean) or 2 (ip)", fn);
+  AM_CHECK(N < (int64_t)0x7fffffff, "%s: at most 2^31-2 rows", fn);  // row ids are int, 0x7fffffff marks padding
+  AM_TRY(ensure_init());
+  Stream own;
+  if (kind == cudaMemcpyHostToDevice) {
+    AM_TRY(own.create());
+    st = own.s;
+  }
+  std::unique_ptr<am_index> idx(new am_index());
+  idx->N = N;
+  idx->d = d;
+  idx->metric = metric;
+  AM_TRY(idx->X.alloc(std::max<size_t>((size_t)N * d, 1)));
   AM_TRY(idx->xnorm2.alloc(std::max<int64_t>(N, 1)));
   if (N > 0) {
-    AM_LAUNCH(row_prepare_kernel, (unsigned)((N + 7) / 8), 256, 0, st, idx->X.p, N, d,
-              idx->metric == kMetricCos ? 1 : 0, idx->xnorm2.p);
+    AM_CUDA(cudaMemcpyAsync(idx->X.p, X, (size_t)N * d * 4, kind, st));
+    AM_LAUNCH(row_prepare_kernel, (unsigned)((N + 7) / 8), 256, 0, st, idx->X.p, N, d, metric == kMetricCos ? 1 : 0,
+              idx->xnorm2.p);
     int s;
     const float m2 = reduce_max_host(idx->xnorm2.p, N, st, &s);
     AM_TRY(s);
@@ -946,94 +936,30 @@ static int finish_build(am_index* idx, cudaStream_t st) {
     idx->dpad = (int)round_up(d, 64);
     AM_TRY(idx->Xb.alloc((size_t)N * idx->dpad));
     AM_TRY(idx->xres.alloc(N));
-    AM_LAUNCH(row_to_bf16_kernel, (unsigned)((N + 7) / 8), 256, 0, st, idx->X.p, N, d, idx->dpad,
-              idx->Xb.p, idx->xres.p);
+    AM_LAUNCH(row_to_bf16_kernel, (unsigned)((N + 7) / 8), 256, 0, st, idx->X.p, N, d, idx->dpad, idx->Xb.p, idx->xres.p);
     idx->xres_max = reduce_max_host(idx->xres.p, N, st, &s);
     AM_TRY(s);
   }
+  *out = idx.release();
   return AM_OK;
 }
 
 extern "C" int am_knn_build(const float* X, int64_t N, int d, int metric, am_index** out) {
-  AM_CHECK(out != nullptr, "am_knn_build: out is NULL");
-  *out = nullptr;
-  AM_CHECK(N >= 0 && d > 0 && (X != nullptr || N == 0), "am_knn_build: bad shape N=%lld d=%d", (long long)N, d);
-  AM_CHECK(metric >= 0 && metric <= 2, "am_knn_build: metric must be 0 (cosine), 1 (euclidean) or 2 (ip)");
-  AM_CHECK(N < (int64_t)0x7fffffff, "am_knn_build: at most 2^31-1 rows");
-  AM_TRY(ensure_init());
-  auto* idx = new am_index();
-  idx->N = N;
-  idx->d = d;
-  idx->metric = metric;
-  Stream st;
-  int s = st.create();
-  if (s == AM_OK) s = idx->X.alloc(std::max<size_t>((size_t)N * d, 1));
-  if (s == AM_OK && N > 0) {
-    cudaError_t e = cudaMemcpyAsync(idx->X.p, X, (size_t)N * d * 4, cudaMemcpyHostToDevice, st.s);
-    if (e != cudaSuccess) s = cuda_fail(e, "H2D index rows", __FILE__, __LINE__);
-  }
-  if (s == AM_OK) s = finish_build(idx, st.s);
-  if (s != AM_OK) {
-    delete idx;
-    return s;
-  }
-  *out = idx;
-  return AM_OK;
+  return build_index("am_knn_build", X, N, d, metric, cudaMemcpyHostToDevice, nullptr, out);
 }
 
-extern "C" int am_knn_build_dev(const float* X_dev, int64_t N, int d, int metric, void* stream,
-                                am_index** out) {
-  AM_CHECK(out != nullptr, "am_knn_build_dev: out is NULL");
-  *out = nullptr;
-  AM_CHECK(N >= 0 && d > 0 && (X_dev != nullptr || N == 0), "am_knn_build_dev: bad shape");
-  AM_CHECK(metric >= 0 && metric <= 2, "am_knn_build_dev: bad metric");
-  AM_TRY(ensure_init());
-  auto* idx = new am_index();
-  idx->N = N;
-  idx->d = d;
-  idx->metric = metric;
-  cudaStream_t st = (cudaStream_t)stream;
-  int s = idx->X.alloc(std::max<size_t>((size_t)N * d, 1));
-  if (s == AM_OK && N > 0) {
-    cudaError_t e = cudaMemcpyAsync(idx->X.p, X_dev, (size_t)N * d * 4, cudaMemcpyDeviceToDevice, st);
-    if (e != cudaSuccess) s = cuda_fail(e, "D2D index rows", __FILE__, __LINE__);
-  }
-  if (s == AM_OK) s = finish_build(idx, st);
-  if (s != AM_OK) {
-    delete idx;
-    return s;
-  }
-  *out = idx;
-  return AM_OK;
+extern "C" int am_knn_build_dev(const float* X_dev, int64_t N, int d, int metric, void* stream, am_index** out) {
+  return build_index("am_knn_build_dev", X_dev, N, d, metric, cudaMemcpyDeviceToDevice, (cudaStream_t)stream, out);
 }
 
 extern "C" void am_knn_free(am_index* idx) { delete idx; }
 extern "C" int64_t am_knn_size(const am_index* idx) { return idx ? idx->N : 0; }
 extern "C" int am_knn_dim(const am_index* idx) { return idx ? idx->d : 0; }
 
-extern "C" int am_knn_get_vector(const am_index* cidx, int64_t id, float* out) {
-  am_index* idx = const_cast<am_index*>(cidx);
-  AM_CHECK(idx && out, "am_knn_get_vector: NULL argument");
-  AM_CHECK(id >= 0 && id < idx->N, "am_knn_get_vector: id %lld out of range [0, %lld)", (long long)id,
-           (long long)idx->N);
-  {
-    std::lock_guard<std::mutex> lk(idx->host_mu);
-    if (idx->host.empty()) {
-      idx->host.resize((size_t)idx->N * idx->d);
-      cudaError_t e = cudaMemcpy(idx->host.data(), idx->X.p, idx->host.size() * 4, cudaMemcpyDeviceToHost);
-      if (e != cudaSuccess) {
-        idx->host.clear();
-        return cuda_fail(e, "D2H index mirror", __FILE__, __LINE__);
-      }
-    }
-  }
-  std::memcpy(out, idx->host.data() + (size_t)id * idx->d, (size_t)idx->d * 4);
-  return AM_OK;
+extern "C" int am_knn_get_vector(const am_index* idx, int64_t id, float* out) {
+  return am_knn_get_vectors(idx, &id, 1, out);
 }
 
-// device-pointer query; scratch is allocated per call so the entry point is re-entrant.  host_ids / host_dist (optional):
-// the host entry point's destinations -- results are copied there in the same stream round trip as the overflow flags
-// (one synchronisation per query chunk instead of two; a single query is latency bound on exactly these).
 // one stream-ordered allocation carved into the temporaries of a query call (a call used to make nine cudaMallocAsync /
 // cudaFreeAsync pairs: ~20 us of the ~110 us a single query took through the host API)
 struct Arena {
@@ -1050,10 +976,6 @@ struct Arena {
     off += pad(count * sizeof(T));
     return r;
   }
-};
-template <class T>
-struct View {
-  T* p = nullptr;
 };
 // pinned host staging of the calling thread (query in, [ids | dist | overflow] out in ONE copy each way)
 struct HostStage {
@@ -1074,159 +996,204 @@ struct HostStage {
   }
 };
 
-static int knn_query_impl(const am_index* idx, const float* Q_dev, int nq, int k, int mode, int64_t* ids_dev, float* dist_dev,
-                          void* stream, int64_t* host_ids, float* host_dist, int* overflow_dev = nullptr,
-                          HostStage* merged = nullptr) {
-  // merged != NULL: the caller laid out [ids | dist | overflow] contiguously from ids_dev (256-byte padded parts) and
-  // owns a pinned staging buffer of that size: results and flags travel in one device-to-host copy
-  AM_CHECK(idx && Q_dev && ids_dev && dist_dev, "am_knn_query_dev: NULL argument");
-  AM_CHECK(nq >= 0 && k >= 0, "am_knn_query_dev: negative size");
-  if (k > idx->N) {
-    set_error("am_knn_query: k=%d exceeds the %lld stored vectors (voyager.RecallError)", k, (long long)idx->N);
-    return AM_ERR_RECALL;
-  }
-  if (nq == 0 || k == 0) return AM_OK;
-  cudaStream_t st = (cudaStream_t)stream;
+// ---------------------------------------------------------------- query plan
+// Everything about a query call that follows from (index, nq, k, mode), decided before anything is launched.
+enum class Scorer {
+  None,       // the full sort computes every distance itself
+  F32,        // score_f32_kernel over the fp32 rows (+ chunk_max_rows_kernel for the chunk-max selection)
+  Bf16Small,  // score_bf16_small_kernel: one pass over the bf16 rows per 1-4 queries, which also prepares the queries
+              // and writes the chunk maxima
+  Bf16Gemm,   // the wgmma GEMM over the bf16 rows, chunk maxima from its epilogue for the chunk-max selection
+};
+enum class Selection { ChunkMax, Rows, FullSort };  // select_cm_kernel, select_rerank_kernel, full_sort_query
+
+struct QueryPlan {
+  Scorer scorer;
+  Selection select;
+  int per_pass;      // queries per pass
+  int qrows;         // rows of the per-pass query buffers (the GEMM's A operand: a multiple of 128, zero padded)
+  SelectParams sel;  // shapes, error bound and index rows of the selection; the run adds the per-pass pointers
+  size_t n_cm, n_s, n_qs, n_qb, n_qres;  // elements of the scratch buffers (qnorm and the overflow flags: qrows each)
+};
+
+static int plan_query(const am_index* idx, int nq, int k, int mode, QueryPlan* pl) {
   const int64_t N = idx->N;
   const int d = idx->d;
   const bool want_tensor = (mode == 2) || (mode == 0 && nq >= 16 && N >= 4096);
   const bool use_tensor = want_tensor && gemm::available();
   AM_CHECK(!(mode == 2 && !use_tensor), "am_knn_query: tensor-core filter unavailable on this device");
-
-  // chunk-max selection for batches on the tensor-core path (AM_KNN_NO_CHUNKMAX=1: stream the score rows instead)
-  const bool no_cm = std::getenv("AM_KNN_NO_CHUNKMAX") != nullptr;
-  const int64_t n_chunks = (N + kCmChunk - 1) / kCmChunk;
-  const bool fused = !no_cm && k <= kCmMaxK && n_chunks >= 4 * (int64_t)k;
-  const int64_t ldCM = round_up(n_chunks, 8);
-  // chunk queries so the score matrix stays under ~1.5 GiB
-  const int64_t ldS = round_up(N, 4);
-  int chunk = (int)std::max<int64_t>(1, std::min<int64_t>(nq, (int64_t)(3ll << 28) / ldS));
-  if (use_tensor) chunk = std::max(128, chunk / 128 * 128);
-  // a handful of queries: one pass over the bf16 copy (scores + chunk maxima) instead of the fp32 rows + a second kernel
-  static const bool no_small = std::getenv("AM_KNN_NO_SMALL_BF16") != nullptr;
-  const bool small_bf16 = !use_tensor && mode == 0 && fused && !no_small && idx->Xb.p != nullptr &&
-                          (idx->dpad == 256 || idx->dpad == 512 || idx->dpad == 1024);
-  View<float> S, Qs, qres, CM;
-  View<double> qnorm;
-  View<__nv_bfloat16> Qb;
-  View<int> overflow;
-  const int qrows = use_tensor ? (int)round_up(std::min(nq, chunk), 128) : std::min(nq, chunk);
-  Arena arena;
-  {
-    const size_t n_cm = fused ? (size_t)qrows * ldCM : 0, n_s = (size_t)qrows * ldS, n_qs = small_bf16 ? 0 : (size_t)qrows * d;
-    const size_t n_qb = use_tensor ? (size_t)qrows * idx->dpad : 0, n_qres = (use_tensor || small_bf16) ? (size_t)qrows : 0;
-    AM_TRY(arena.reserve(Arena::pad(n_cm * 4) + Arena::pad(n_s * 4) + Arena::pad(n_qs * 4) + Arena::pad((size_t)qrows * 8) +
-                             Arena::pad((size_t)qrows * 4) + Arena::pad(n_qb * 2) + Arena::pad(n_qres * 4),
-                         st));
-    CM.p = arena.take<float>(n_cm);
-    S.p = arena.take<float>(n_s);
-    Qs.p = arena.take<float>(n_qs);
-    qnorm.p = arena.take<double>((size_t)qrows);
-    overflow.p = overflow_dev ? overflow_dev : arena.take<int>((size_t)qrows);
-    Qb.p = arena.take<__nv_bfloat16>(n_qb);
-    qres.p = arena.take<float>(n_qres);
-  }
-  static std::once_flag attr_once;
-  static cudaError_t attr_err = cudaSuccess;
-  const size_t sel_smem = (size_t)kCandCap * (sizeof(double) + sizeof(int));
-  std::call_once(attr_once, [&] {
-    attr_err = cudaFuncSetAttribute(select_rerank_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                    (int)sel_smem);
-    if (attr_err == cudaSuccess)
-      attr_err = cudaFuncSetAttribute(select_cm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sel_smem);
-  });
-  if (attr_err != cudaSuccess) return cuda_fail(attr_err, "cudaFuncSetAttribute(select)", __FILE__, __LINE__);
-  std::vector<int> h_overflow;
-  for (int q0 = 0; q0 < nq; q0 += chunk) {
-    const int nc = std::min(chunk, nq - q0);
-    const float* Qc = Q_dev + (int64_t)q0 * d;
+  SelectParams& p = pl->sel;
+  p = SelectParams{};
+  p.N = N;
+  p.d = d;
+  p.metric = idx->metric;
+  p.k = k;
+  p.X = idx->X.p;
+  p.xnorm2 = idx->xnorm2.p;
+  p.xnorm_max = idx->max_norm;
+  p.ldS = round_up(N, 4);
+  p.n_chunks = (N + kCmChunk - 1) / kCmChunk;
+  p.ldCM = round_up(p.n_chunks, 8);
+  // chunk-max selection when the k-th largest chunk maximum leaves enough chunks beside the k winners
+  const bool chunk_max = k <= kCmMaxK && p.n_chunks >= 4 * (int64_t)k;
+  if (k > kCandCap - 64) {
+    pl->select = Selection::FullSort;
+    pl->scorer = Scorer::None;
+  } else {
+    pl->select = chunk_max ? Selection::ChunkMax : Selection::Rows;
     if (use_tensor)
-      AM_CUDA(cudaMemsetAsync(Qb.p, 0, (size_t)qrows * idx->dpad * sizeof(__nv_bfloat16), st));
-    if (!small_bf16)   // (the small-batch scoring kernel prepares its queries itself)
-      AM_LAUNCH(query_prepare_kernel, ceil_div(nc, 8), 256, 0, st, Qc, nc, d, idx->dpad, idx->metric, Qs.p, qnorm.p,
-                use_tensor ? Qb.p : nullptr, use_tensor ? qres.p : nullptr);
-    SelectParams p{};
-    p.S = S.p;
-    p.ldS = ldS;
-    p.N = N;
-    p.d = d;
-    p.metric = idx->metric;
-    p.k = k;
-    p.X = idx->X.p;
-    p.xnorm2 = idx->xnorm2.p;
-    p.Q = Qc;
-    p.qnorm = qnorm.p;
+      pl->scorer = Scorer::Bf16Gemm;
+    else if (mode == 0 && chunk_max && (idx->dpad == 256 || idx->dpad == 512 || idx->dpad == 1024))
+      pl->scorer = Scorer::Bf16Small;
+    else
+      pl->scorer = Scorer::F32;
+  }
+  const bool gemm = pl->scorer == Scorer::Bf16Gemm, small = pl->scorer == Scorer::Bf16Small;
+  // passes of at most 3 << 28 scores (3 GiB)
+  pl->per_pass = (int)std::max<int64_t>(1, std::min<int64_t>(nq, (int64_t)(3ll << 28) / p.ldS));
+  if (gemm) pl->per_pass = std::max(128, pl->per_pass / 128 * 128);
+  pl->qrows = gemm ? (int)round_up(std::min(nq, pl->per_pass), 128) : std::min(nq, pl->per_pass);
+  const size_t qrows = (size_t)pl->qrows;
+  pl->n_cm = pl->select == Selection::ChunkMax ? qrows * p.ldCM : 0;
+  pl->n_s = pl->scorer == Scorer::None ? 0 : qrows * p.ldS;
+  pl->n_qs = small ? 0 : qrows * d;
+  pl->n_qb = gemm ? qrows * idx->dpad : 0;
+  pl->n_qres = (gemm || small) ? qrows : 0;
+  // fp32 accumulation error: <= (d * 2^-24 * 1.01) * ||q|| ||x||  (any summation order).  It scales with ||q|| ||x||:
+  // cosine queries are unit vectors; for inner product / euclidean the kernel multiplies by the query's own norm
+  // (score_eps), so a query far larger than the stored rows is covered
+  const float fp32_rel = (float)d * 6.1e-8f;
+  p.eps_scales_with_q = idx->metric == kMetricCos ? 0 : 1;
+  if (gemm || small) {  // bf16 products: the rounding residuals of both sides enter the bound (score_eps)
+    p.xres = idx->xres.p;
+    p.xres_max = idx->xres_max;
+    p.eps_abs = fp32_rel * idx->max_norm;
+  } else {  // fp32 pass: |s~ - s| <= d 2^-24 ||q|| ||x|| per dot product (x2 for the euclidean score 2 q.x - ||x||^2,
+            // plus the rounding of the stored fp32 ||x||^2)
+    p.eps_abs = fp32_rel * idx->max_norm * (idx->metric == kMetricL2 ? 2.0f : 1.0f) +
+                (idx->metric == kMetricL2 ? 1.2e-7f * idx->max_norm * idx->max_norm : 0.0f);
+  }
+  return AM_OK;
+}
+
+struct QueryBufs {
+  float *CM, *S, *Qs;
+  double* qnorm;
+  int* overflow;
+  __nv_bfloat16* Qb;
+  float* qres;
+};
+
+template <int kQ, int kSegs>
+static int score_small_launch(const am_index* idx, const QueryPlan& pl, const QueryBufs& b, const float* Qc, int nc, int t0,
+                              int grid, cudaStream_t st) {
+  AM_LAUNCH((score_bf16_small_kernel<kQ, kSegs>), grid, 256, 0, st, idx->Xb.p, idx->xnorm2.p, idx->N, idx->d, idx->dpad, Qc,
+            nc, t0, idx->metric, b.S, pl.sel.ldS, b.CM, pl.sel.ldCM, pl.sel.n_chunks, b.qnorm, b.qres);
+  return AM_OK;
+}
+
+// the pass's queries four, two or one per launch
+template <int kSegs>
+static int score_small(const am_index* idx, const QueryPlan& pl, const QueryBufs& b, const float* Qc, int nc,
+                       cudaStream_t st) {
+  const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((pl.sel.n_chunks + 7) / 8, (int64_t)sm_count() * 8));
+  for (int t0 = 0; t0 < nc;) {
+    const int kq = nc - t0 >= 4 ? 4 : (nc - t0 >= 2 ? 2 : 1);
+    if (kq == 4) AM_TRY((score_small_launch<4, kSegs>(idx, pl, b, Qc, nc, t0, grid, st)));
+    else if (kq == 2) AM_TRY((score_small_launch<2, kSegs>(idx, pl, b, Qc, nc, t0, grid, st)));
+    else AM_TRY((score_small_launch<1, kSegs>(idx, pl, b, Qc, nc, t0, grid, st)));
+    t0 += kq;
+  }
+  return AM_OK;
+}
+
+// Runs a checked query (1 <= k <= N, nq >= 1) on device pointers.  host_ids / host_dist (optional): the host entry point's
+// destinations -- results are copied there in the same stream round trip as the overflow flags (one synchronisation per
+// pass instead of two; a single query is latency bound on exactly these).  merged != NULL: the caller laid out
+// [ids | dist | overflow] contiguously from ids_dev (256-byte padded parts) and owns a pinned staging buffer of that size:
+// results and flags travel in one device-to-host copy.  Scratch is allocated per call so the entry points are re-entrant.
+static int knn_query_impl(const am_index* idx, const float* Q_dev, int nq, int k, int mode, int64_t* ids_dev, float* dist_dev,
+                          cudaStream_t st, int64_t* host_ids, float* host_dist, int* overflow_dev = nullptr,
+                          HostStage* merged = nullptr) {
+  QueryPlan pl;
+  AM_TRY(plan_query(idx, nq, k, mode, &pl));
+  const int64_t N = idx->N;
+  const int d = idx->d;
+  const bool gemm = pl.scorer == Scorer::Bf16Gemm, small = pl.scorer == Scorer::Bf16Small;
+  Arena arena;
+  AM_TRY(arena.reserve(Arena::pad(pl.n_cm * 4) + Arena::pad(pl.n_s * 4) + Arena::pad(pl.n_qs * 4) +
+                           Arena::pad((size_t)pl.qrows * 8) + Arena::pad((size_t)pl.qrows * 4) + Arena::pad(pl.n_qb * 2) +
+                           Arena::pad(pl.n_qres * 4),
+                       st));
+  QueryBufs b;
+  b.CM = arena.take<float>(pl.n_cm);
+  b.S = arena.take<float>(pl.n_s);
+  b.Qs = arena.take<float>(pl.n_qs);
+  b.qnorm = arena.take<double>((size_t)pl.qrows);
+  b.overflow = overflow_dev ? overflow_dev : arena.take<int>((size_t)pl.qrows);
+  b.Qb = arena.take<__nv_bfloat16>(pl.n_qb);
+  b.qres = arena.take<float>(pl.n_qres);
+  SelectParams p = pl.sel;
+  p.S = b.S;
+  p.CM = b.CM;
+  p.qnorm = b.qnorm;
+  p.qres = (gemm || small) ? b.qres : nullptr;
+  p.overflow = b.overflow;
+  const size_t sel_smem = (size_t)kCandCap * (sizeof(double) + sizeof(int));
+  std::vector<int> h_overflow;
+  for (int q0 = 0; q0 < nq; q0 += pl.per_pass) {
+    const int nc = std::min(pl.per_pass, nq - q0);
+    p.Q = Q_dev + (int64_t)q0 * d;
     p.ids = ids_dev + (int64_t)q0 * k;
     p.dist = dist_dev + (int64_t)q0 * k;
-    p.overflow = overflow.p;
-    p.xnorm_max = idx->max_norm;
-    // fp32 accumulation error: <= (d * 2^-24 * 1.01) * ||q|| ||x||  (any summation order)
-    const float fp32_rel = (float)d * 6.1e-8f;
-    if (use_tensor || small_bf16) {
-      p.qres = qres.p;
-      p.xres = idx->xres.p;
-      p.xres_max = idx->xres_max;
-      // the accumulation term scales with ||q|| ||x||: cosine queries are unit vectors; for inner product / euclidean
-      // the kernel multiplies by the query's own norm (score_eps), so a query far larger than the stored rows is covered
-      p.eps_abs = fp32_rel * idx->max_norm;
-      p.eps_scales_with_q = idx->metric == kMetricCos ? 0 : 1;
-      if (small_bf16) {
-        p.CM = CM.p;
-        p.ldCM = ldCM;
-        p.n_chunks = n_chunks;
-        const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((n_chunks + 7) / 8, (int64_t)sm_count() * 8));
-        const float* xn2 = idx->xnorm2.p;
-#define AM_SMALL_LAUNCH(Q_, SG_)                                                                                        \
-  AM_LAUNCH((score_bf16_small_kernel<Q_, SG_>), grid, 256, 0, st, idx->Xb.p, xn2, N, d, idx->dpad, Qc, nc, t0, idx->metric, \
-            S.p, ldS, CM.p, ldCM, n_chunks, qnorm.p, qres.p)
-        for (int t0 = 0; t0 < nc;) {
-          const int left = nc - t0;
-          const int kq = left >= 4 ? 4 : (left >= 2 ? 2 : 1);
-          if (idx->dpad == 256) {
-            if (kq == 4) AM_SMALL_LAUNCH(4, 1); else if (kq == 2) AM_SMALL_LAUNCH(2, 1); else AM_SMALL_LAUNCH(1, 1);
-          } else if (idx->dpad == 512) {
-            if (kq == 4) AM_SMALL_LAUNCH(4, 2); else if (kq == 2) AM_SMALL_LAUNCH(2, 2); else AM_SMALL_LAUNCH(1, 2);
-          } else {
-            if (kq == 4) AM_SMALL_LAUNCH(4, 4); else if (kq == 2) AM_SMALL_LAUNCH(2, 4); else AM_SMALL_LAUNCH(1, 4);
-          }
-          t0 += kq;
+    // 1. queries: norms, normalised fp32 copy, bf16 copy + residual norm
+    if (gemm) AM_CUDA(cudaMemsetAsync(b.Qb, 0, (size_t)pl.qrows * idx->dpad * sizeof(__nv_bfloat16), st));
+    if (!small)
+      AM_LAUNCH(query_prepare_kernel, ceil_div(nc, 8), 256, 0, st, p.Q, nc, d, idx->dpad, idx->metric, b.Qs, b.qnorm,
+                gemm ? b.Qb : nullptr, gemm ? b.qres : nullptr);
+    // 2. approximate scores, and their per-32 maxima for the chunk-max selection
+    switch (pl.scorer) {
+      case Scorer::None:
+        break;
+      case Scorer::F32: {
+        const int grid = std::max(1, std::min<int>((int)((N + 7) / 8), sm_count() * 8));
+        for (int t0 = 0; t0 < nc; t0 += kQT)
+          AM_LAUNCH(score_f32_kernel, grid, 256, (size_t)kQT * d * 4, st, idx->X.p, idx->xnorm2.p, N, d, b.Qs, nc, t0,
+                    idx->metric, b.S, p.ldS);
+        if (pl.select == Selection::ChunkMax) {
+          const int64_t warps = (int64_t)nc * p.n_chunks;
+          AM_LAUNCH(chunk_max_rows_kernel, (unsigned)std::min<int64_t>((warps + 7) / 8, (int64_t)sm_count() * 16), 256, 0,
+                    st, b.S, p.ldS, N, nc, p.n_chunks, b.CM, p.ldCM);
         }
-#undef AM_SMALL_LAUNCH
-      } else if (fused) {
-        // S[q, j] = Qb[q,:] . Xb[j,:] (bf16 x bf16 -> fp32 in registers, euclidean fix-up in the epilogue) + per-32 maxima
-        p.CM = CM.p;
-        p.ldCM = ldCM;
-        p.n_chunks = n_chunks;
-        AM_TRY(gemm::scores_chunkmax_bf16(Qb.p, qrows, idx->Xb.p, N, idx->dpad, S.p, ldS, CM.p, ldCM,
-                                          idx->metric == kMetricL2 ? idx->xnorm2.p : nullptr, st));
-      } else {
-        AM_TRY(gemm::scores_bf16(Qb.p, qrows, idx->Xb.p, N, idx->dpad, S.p, ldS,
+        break;
+      }
+      case Scorer::Bf16Small:
+        if (idx->dpad == 256) AM_TRY(score_small<1>(idx, pl, b, p.Q, nc, st));
+        else if (idx->dpad == 512) AM_TRY(score_small<2>(idx, pl, b, p.Q, nc, st));
+        else AM_TRY(score_small<4>(idx, pl, b, p.Q, nc, st));
+        break;
+      case Scorer::Bf16Gemm:  // bf16 x bf16 -> fp32 in registers, euclidean fix-up in the epilogue
+        AM_TRY(gemm::scores_bf16(b.Qb, pl.qrows, idx->Xb.p, N, idx->dpad, b.S, p.ldS,
+                                 pl.select == Selection::ChunkMax ? b.CM : nullptr, p.ldCM,
                                  idx->metric == kMetricL2 ? idx->xnorm2.p : nullptr, st));
-      }
-    } else {
-      const int grid = std::max(1, std::min<int>((int)((N + 7) / 8), sm_count() * 8));
-      for (int t0 = 0; t0 < nc; t0 += kQT)
-        AM_LAUNCH(score_f32_kernel, grid, 256, (size_t)kQT * d * 4, st, idx->X.p, idx->xnorm2.p, N, d, Qs.p,
-                  nc, t0, idx->metric, S.p, ldS);
-      // fp32 pass: |s~ - s| <= d 2^-24 ||q|| ||x|| per dot product (x2 for the euclidean score 2 q.x - ||x||^2, plus the
-      // rounding of the stored fp32 ||x||^2); ||q|| enters per query inside the kernel (score_eps)
-      p.eps_abs = fp32_rel * idx->max_norm * (idx->metric == kMetricL2 ? 2.0f : 1.0f) +
-                  (idx->metric == kMetricL2 ? 1.2e-7f * idx->max_norm * idx->max_norm : 0.0f);
-      p.eps_scales_with_q = idx->metric == kMetricCos ? 0 : 1;
-      if (fused) {
-        p.CM = CM.p;
-        p.ldCM = ldCM;
-        p.n_chunks = n_chunks;
-        const int64_t warps = (int64_t)nc * n_chunks;
-        AM_LAUNCH(chunk_max_rows_kernel, (unsigned)std::min<int64_t>((warps + 7) / 8, (int64_t)sm_count() * 16), 256, 0, st, S.p,
-                  ldS, N, nc, n_chunks, CM.p, ldCM);
-      }
+        break;
     }
-    bool big_k = k > kCandCap - 64;
-    if (!big_k) {
-      if (fused) AM_LAUNCH(select_cm_kernel, nc, kSelThreads, sel_smem, st, p);
-      else AM_LAUNCH(select_rerank_kernel, nc, kSelThreads, sel_smem, st, p);
-      h_overflow.resize(nc);
+    // 3. selection + exact re-rank; a query whose candidates do not fit on chip raises its overflow flag
+    switch (pl.select) {
+      case Selection::ChunkMax:
+        AM_TRY(allow_dynamic_smem<select_cm_kernel>(sel_smem));
+        AM_LAUNCH(select_cm_kernel, nc, kSelThreads, sel_smem, st, p);
+        break;
+      case Selection::Rows:
+        AM_TRY(allow_dynamic_smem<select_rerank_kernel>(sel_smem));
+        AM_LAUNCH(select_rerank_kernel, nc, kSelThreads, sel_smem, st, p);
+        break;
+      case Selection::FullSort:
+        break;
+    }
+    // 4. results and overflow flags to the host; flagged queries (all of them for the full sort) answered by the full sort
+    h_overflow.assign(nc, 1);
+    if (pl.select != Selection::FullSort) {
       if (merged && host_ids && nc == nq) {
         const size_t o_dist = Arena::pad((size_t)nq * k * 8), o_ovf = o_dist + Arena::pad((size_t)nq * k * 4);
         const size_t bytes = o_ovf + (size_t)nq * sizeof(int);
@@ -1237,15 +1204,13 @@ static int knn_query_impl(const am_index* idx, const float* Q_dev, int nq, int k
         std::memcpy(host_dist, h + o_dist, (size_t)nq * k * 4);
         std::memcpy(h_overflow.data(), h + o_ovf, (size_t)nq * sizeof(int));
       } else {
-        AM_CUDA(cudaMemcpyAsync(h_overflow.data(), overflow.p, nc * sizeof(int), cudaMemcpyDeviceToHost, st));
+        AM_CUDA(cudaMemcpyAsync(h_overflow.data(), b.overflow, nc * sizeof(int), cudaMemcpyDeviceToHost, st));
         if (host_ids) {
           AM_CUDA(cudaMemcpyAsync(host_ids + (int64_t)q0 * k, p.ids, (size_t)nc * k * 8, cudaMemcpyDeviceToHost, st));
           AM_CUDA(cudaMemcpyAsync(host_dist + (int64_t)q0 * k, p.dist, (size_t)nc * k * 4, cudaMemcpyDeviceToHost, st));
         }
         AM_CUDA(cudaStreamSynchronize(st));
       }
-    } else {
-      h_overflow.assign(nc, 1);
     }
     bool any = false;
     for (int q = 0; q < nc; ++q)
@@ -1253,7 +1218,7 @@ static int knn_query_impl(const am_index* idx, const float* Q_dev, int nq, int k
         AM_TRY(full_sort_query(p, q, st));
         any = true;
       }
-    if (any && host_ids) {  // rare: rows answered by the exact full sort are copied again
+    if (any && host_ids) {  // rows answered by the exact full sort are copied again
       AM_CUDA(cudaMemcpyAsync(host_ids + (int64_t)q0 * k, p.ids, (size_t)nc * k * 8, cudaMemcpyDeviceToHost, st));
       AM_CUDA(cudaMemcpyAsync(host_dist + (int64_t)q0 * k, p.dist, (size_t)nc * k * 4, cudaMemcpyDeviceToHost, st));
       AM_CUDA(cudaStreamSynchronize(st));
@@ -1262,20 +1227,29 @@ static int knn_query_impl(const am_index* idx, const float* Q_dev, int nq, int k
   return AM_OK;
 }
 
+// the size checks of both query entry points
+static int check_query(const am_index* idx, int nq, int k) {
+  AM_CHECK(nq >= 0 && k >= 0, "am_knn_query: negative size");
+  if (k > idx->N) {
+    set_error("am_knn_query: k=%d exceeds the %lld stored vectors (voyager.RecallError)", k, (long long)idx->N);
+    return AM_ERR_RECALL;
+  }
+  return AM_OK;
+}
+
 extern "C" int am_knn_query_dev(const am_index* idx, const float* Q_dev, int nq, int k, int mode, int64_t* ids_dev,
                                 float* dist_dev, void* stream) {
-  return knn_query_impl(idx, Q_dev, nq, k, mode, ids_dev, dist_dev, stream, nullptr, nullptr);
+  AM_CHECK(idx && Q_dev && ids_dev && dist_dev, "am_knn_query_dev: NULL argument");
+  AM_TRY(check_query(idx, nq, k));
+  if (nq == 0 || k == 0) return AM_OK;
+  return knn_query_impl(idx, Q_dev, nq, k, mode, ids_dev, dist_dev, (cudaStream_t)stream, nullptr, nullptr);
 }
 
 extern "C" int am_knn_query_ex(const am_index* idx, const float* Q, int nq, int k, int mode, int64_t* ids,
                                float* dist) {
   AM_CHECK(idx && (Q || nq == 0) && (ids || nq * (int64_t)k == 0) && (dist || nq * (int64_t)k == 0),
            "am_knn_query: NULL argument");
-  AM_CHECK(nq >= 0 && k >= 0, "am_knn_query: negative size");
-  if (k > idx->N) {
-    set_error("am_knn_query: k=%d exceeds the %lld stored vectors (voyager.RecallError)", k, (long long)idx->N);
-    return AM_ERR_RECALL;
-  }
+  AM_TRY(check_query(idx, nq, k));
   if (nq == 0 || k == 0) return AM_OK;
   AM_TRY(ensure_init());
   static thread_local Stream st;  // one stream per calling thread (Flask gthread x4): re-entrant

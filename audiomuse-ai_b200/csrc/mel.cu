@@ -387,6 +387,9 @@ mel_kernel(const void* __restrict__ pcm, int n_samples, int hop, int T, int n_me
   }
 }
 
+// sm_90's opt-in maximum of dynamic shared memory per block: every mel_kernel instantiation may launch with up to this
+constexpr size_t kMelSmemMax = 227 * 1024;
+
 static size_t mel_smem_bytes(int hop, int n_mels, int nnz) {
   const int n_stage = (kFramesPerCta - 1) * hop + kNfft;
   size_t floats = ((n_stage + 3) & ~3) + kNfft + 2 * 32 * 32 + (size_t)kWarps * 32 * kTrStride +
@@ -448,6 +451,13 @@ extern "C" int am_mel_plan_create(const am_mel_cfg* cfg, am_mel_plan** out) {
     for (int k = 0; k < len[m]; ++k) wts.push_back(fb[(size_t)m * bins + st[m] + k]);
     if (hi > max_bin) max_bin = hi;
   }
+  const size_t smem = mel_smem_bytes(cfg->hop, nm, (int)wts.size());
+  AM_CHECK(smem <= kMelSmemMax, "mel: hop %d with %d mel bands needs %zu bytes of shared memory, above %zu", cfg->hop, nm,
+           smem, kMelSmemMax);
+  AM_TRY((allow_dynamic_smem<mel_kernel<true, 19>>(kMelSmemMax)));
+  AM_TRY((allow_dynamic_smem<mel_kernel<false, 19>>(kMelSmemMax)));
+  AM_TRY((allow_dynamic_smem<mel_kernel<true, 32>>(kMelSmemMax)));
+  AM_TRY((allow_dynamic_smem<mel_kernel<false, 32>>(kMelSmemMax)));
   // periodic Hann of the frame length; zero beyond it (frames shorter than 2048 are zero-padded transforms)
   std::vector<float> win(kNfft, 0.0f);
   for (int n = 0; n < cfg->n_fft; ++n) win[n] = (float)(0.5 - 0.5 * std::cos(2.0 * M_PI * n / cfg->n_fft));
@@ -496,18 +506,6 @@ extern "C" int am_mel_plan_create(const am_mel_cfg* cfg, am_mel_plan** out) {
   plan->t.band_len = reinterpret_cast<int*>(base + o_len);
   plan->t.band_off = reinterpret_cast<int*>(base + o_off);
   plan->t.weights = reinterpret_cast<float*>(base + o_w);
-  const size_t smem = mel_smem_bytes(cfg->hop, cfg->n_mels, plan->nnz);
-  e = cudaFuncSetAttribute(mel_kernel<true, 19>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (e == cudaSuccess)
-    e = cudaFuncSetAttribute(mel_kernel<false, 19>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (e == cudaSuccess)
-    e = cudaFuncSetAttribute(mel_kernel<true, 32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (e == cudaSuccess)
-    e = cudaFuncSetAttribute(mel_kernel<false, 32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (e != cudaSuccess) {
-    delete plan;
-    return cuda_fail(e, "cudaFuncSetAttribute(mel)", __FILE__, __LINE__);
-  }
   *out = plan;
   return AM_OK;
 }

@@ -1,4 +1,6 @@
 """K4 parity: exact GPU index vs the float64 oracle -- identical ids (bit-exact index work)."""
+import ctypes
+import functools
 import os
 
 import numpy as np
@@ -174,6 +176,11 @@ def test_pairwise_and_get_vectors(space_name, golden_dir):
     ids = [int(i) for i in rng.choice(500, 37, replace=False)]
     stored = idx.get_vectors(ids)
     np.testing.assert_array_equal(stored, np.stack([idx.get_vector(i) for i in ids]))
+    from audiomuse_ai_b200 import _lib
+    one = np.empty(200, np.float32)
+    for j, i in enumerate(ids):   # the one-row C entry point
+        _lib.check(_lib.load().am_knn_get_vector(idx._ensure_built(), ctypes.c_int64(idx._row_of(i)), _lib.ptr(one)))
+        np.testing.assert_array_equal(one, stored[j])
     dm = idx.pairwise_distances(ids + [10_000])
     assert dm.shape == (38, 38) and np.isinf(dm[-1, :-1]).all() and np.isinf(dm[:-1, -1]).all()
     fn = oknn.direct_euclidean_distance if space_name == "Euclidean" else oknn.direct_cosine_distance
@@ -219,32 +226,39 @@ def test_queries_are_reentrant_across_threads():
         np.testing.assert_array_equal(got_single[i][0], want_single[i][0])
 
 
-@pytest.mark.parametrize("k", [1, 50, 500])
-@pytest.mark.parametrize("space_name", ["Cosine", "Euclidean"])
-def test_chunk_max_selection_equals_row_streaming_selection(k, space_name):
-    """Batches on the tensor-core path: the GEMM epilogue also writes the maximum of every 32 scores, and the selection
-    kernel works from those maxima (threshold + the few chunks that can hold answers) instead of streaming each
-    query's whole row of scores twice.  The answers are identical, id for id and distance for distance, to the
-    row-streaming kernel (AM_KNN_NO_CHUNKMAX=1) and to the float64 oracle, at config-3 size with a ragged N, incl.
-    k = 500 (the reference's n + 4n expansion), for cosine and euclidean spaces."""
+CHUNK_MAX_KS = (1, 50, 500, 600)
+
+
+@functools.lru_cache(maxsize=None)
+def _config3_ragged(space_name):
+    """Config-3 size with a ragged N (100 003 x 512, 640 queries): the index and the oracle's top max(CHUNK_MAX_KS) of
+    the rows as stored (cosine: unit-normalised), whose prefixes are the top k for every smaller k (the order is total:
+    distance, then id)."""
     from audiomuse_ai_b200 import corpus, voyager_compat as vc
     x, _ = _lib_data(100_003, 512, 1234)
     q = corpus.knn_queries(x, 600, 40, 99)
-    space = getattr(vc.Space, space_name)
     if space_name == "Euclidean":
         x = x * np.random.default_rng(3).uniform(0.5, 2.0, (len(x), 1)).astype(np.float32)
-    idx = _index(x, space)
-    ids, dist = idx.query(q, k, mode=2)
-    os.environ["AM_KNN_NO_CHUNKMAX"] = "1"
-    try:
-        ids0, dist0 = idx.query(q, k, mode=2)
-    finally:
-        del os.environ["AM_KNN_NO_CHUNKMAX"]
-    np.testing.assert_array_equal(ids, ids0)
-    np.testing.assert_array_equal(dist, dist0)
-    sel = [0, 321, 639]
     metric = oknn.EUCLIDEAN if space_name == "Euclidean" else oknn.COSINE
-    np.testing.assert_array_equal(ids[sel].astype(np.int64), oknn.topk(x, q[sel], k, metric)[0])
+    idx = _index(x, getattr(vc.Space, space_name))
+    return idx, q, oknn.topk(idx.get_vectors(range(len(x))), q, max(CHUNK_MAX_KS), metric)
+
+
+@pytest.mark.parametrize("k", CHUNK_MAX_KS)
+@pytest.mark.parametrize("space_name", ["Cosine", "Euclidean"])
+def test_chunk_max_selection_equals_row_streaming_selection(k, space_name):
+    """Batches on the tensor-core path: for k <= 512 the GEMM epilogue also writes the maximum of every 32 scores, and
+    the selection kernel works from those maxima (threshold + the few chunks that can hold answers) instead of
+    streaming each query's whole row of scores twice; k = 600 streams the rows.  Every query's answer is the float64
+    oracle's, id for id, at config-3 size with a ragged N, incl. k = 500 (the reference's n + 4n expansion), for
+    cosine and euclidean spaces; and identical, id for id and distance for distance, to the fp32 scoring pass."""
+    idx, q, (want_ids, want_dist) = _config3_ragged(space_name)
+    ids, dist = idx.query(q, k, mode=2)
+    np.testing.assert_array_equal(ids.astype(np.int64), want_ids[:, :k])
+    np.testing.assert_allclose(dist, want_dist[:, :k], rtol=1e-6, atol=2e-7)
+    ids1, dist1 = idx.query(q, k, mode=1)
+    np.testing.assert_array_equal(ids1, ids)
+    np.testing.assert_array_equal(dist1, dist)
 
 
 @pytest.mark.parametrize("space_name", ["Euclidean", "InnerProduct"])

@@ -157,3 +157,37 @@ def test_musicnn_front_end_matches_oracle(seconds):
     print(f"[musicnn mel] {got.shape[0]} patches, max |err| = {err.max():.2e} (values up to {want.max():.2f})")
     assert err.max() <= 2e-4                       # log10(1 + 1e4 x): absolute, values in [0, ~8]
     assert af.musicnn_patches(x[: 187 * 256]) is None and omel.musicnn_patches(x[: 187 * 256]) is None   # one frame short
+
+
+def test_plans_of_different_sizes_run_side_by_side():
+    """A plan's shared-memory need grows with its mel bands.  A 128-band plan created before a 64-band one still runs
+    once the smaller plan exists, and each gives exactly what it gives when it is the only plan."""
+    import torch
+    from audiomuse_ai_b200 import clap_analyzer as ca
+    wins = np.ascontiguousarray(_windows()[:3], dtype=np.float32)
+    pcm = torch.from_numpy(wins).cuda()
+
+    def cfg(n_mels):
+        c = ca._mel_cfg(transpose=False)
+        c.n_mels = n_mels
+        return c
+
+    def run(plan):
+        out = torch.empty((len(wins), plan.cfg.n_mels, 1 + wins.shape[1] // plan.cfg.hop), device="cuda")
+        plan.mel_dev(pcm.data_ptr(), False, len(wins), wins.shape[1], out.data_ptr())
+        torch.cuda.synchronize()
+        return out.cpu().numpy()
+
+    alone = {}
+    for n_mels in (128, 64):
+        plan = ca.MelPlan(cfg(n_mels))
+        alone[n_mels] = run(plan)
+        plan.close()
+    big, small = ca.MelPlan(cfg(128)), ca.MelPlan(cfg(64))
+    try:
+        np.testing.assert_array_equal(run(big), alone[128])
+        np.testing.assert_array_equal(run(small), alone[64])
+        np.testing.assert_array_equal(run(big), alone[128])
+    finally:
+        big.close()
+        small.close()

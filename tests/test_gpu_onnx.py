@@ -174,10 +174,11 @@ def test_out_of_memory_convention_and_retry(tmp_path, monkeypatch, caplog):
     import ctypes as C
     from audiomuse_ai_b200 import _lib, clap_analyzer as ca, corpus, weights
     lib = _lib.load()
-    # 1. a REAL allocation failure: an index of 2^31 x 512 floats (4 TiB) cannot be allocated
+    # 1. a REAL allocation failure: an index of 2^31 - 2 x 512 floats (4 TiB; the most rows an index takes) cannot be
+    # allocated
     x = torch.zeros(512, device="cuda")
     h = C.c_void_p()
-    st = lib.am_knn_build_dev(C.c_void_p(x.data_ptr()), 1 << 31, 512, 0, None, C.byref(h))
+    st = lib.am_knn_build_dev(C.c_void_p(x.data_ptr()), (1 << 31) - 2, 512, 0, None, C.byref(h))
     assert st == _lib.AM_ERR_OOM and "out of memory" in _lib.last_error()
     with pytest.raises(_lib.B200OutOfMemory) as e:
         _lib.check(st)
