@@ -120,6 +120,7 @@ SIGNATURES = {
     "am_umap_plan_free": (None, [_vp]),
     "am_artist_gmm_fit": (_i, [_vp, _i64, _i, _vp, _i, _vp, _vp, _i, _i, C.c_double, C.c_double, _vp, _i64]
                           + [_vp] * 12),
+    "am_gmm_full_fit": (_i, [_vp, _i64, _i, _i, _i, _i, C.c_double, C.c_double, _vp, _i64] + [_vp] * 15),
 }
 
 # include/audiomuse_b200_debug.h: probes and self tests, in libaudiomuse_b200_debug.so only

@@ -60,10 +60,23 @@ def draws_per_init(K: int) -> int:
     return 1 + (K - 1) * n_local_trials(K)
 
 
+def kpp_draws(random_state, K: int, n_init: int) -> np.ndarray:
+    """every double the k-means++ inits of a GaussianMixture(K, n_init, init_params='k-means++').fit draw from
+    check_random_state(random_state), in order: None is numpy's global RandomState, an int seeds a new one, an instance
+    is used as is and is left in the state scikit-learn's fit leaves it in"""
+    if random_state is None:
+        rs = np.random.mtrand._rand
+    elif isinstance(random_state, np.random.RandomState):
+        rs = random_state
+    else:
+        rs = np.random.RandomState(random_state)
+    return rs.random_sample(n_init * draws_per_init(K))
+
+
 @functools.lru_cache(maxsize=4)
 def draw_table(k_max: int = MAX_K, n_init: int = GMM_N_INIT, seed: int = GMM_SEED) -> np.ndarray:
     """every double the k-means++ inits of a GaussianMixture(K <= k_max, n_init, random_state=seed).fit draw, in order"""
-    t = np.random.RandomState(seed).random_sample(n_init * draws_per_init(k_max))
+    t = kpp_draws(seed, k_max, n_init)
     t.flags.writeable = False
     return t
 

@@ -19,7 +19,11 @@ so a missing CUDA library can never masquerade as the GPU path).
         wraps sklearn.cluster.SpectralClustering; here spectral_embedding (k-NN graph + Chebyshev-filtered subspace
         iteration, csrc/spectral.cu) + kmeans_fit on the embedding.  Sets labels_, using_gpu; no cluster_centers_.
 
-GMM has no GPU implementation in the reference either (:280-310, scikit-learn always).
+    GPUGaussianMixture(n_components, covariance_type='full', init_params='k-means++', n_init, random_state,
+        reg_covar).fit_predict(X)   :284-309 -> the reference wraps sklearn.mixture.GaussianMixture; here gmm_fit
+        (am_gmm_full_fit, csrc/gmm.cu): scikit-learn's k-means++ initialisation on the generator's own draws and float64
+        EM on the tensor cores.  Sets means_, weights_, covariances_, precisions_cholesky_, lower_bound_,
+        lower_bounds_, n_iter_, converged_, labels_, using_gpu.  Only covariance_type='full' runs on the device.
 """
 from __future__ import annotations
 
@@ -27,10 +31,14 @@ import ctypes as C
 import logging
 import os
 import time
+import warnings
+from dataclasses import dataclass
+from typing import Optional
 
 import numpy as np
 
 from . import _lib
+from .artist_gmm import draws_per_init, kpp_draws
 
 logger = logging.getLogger("tasks.clustering_gpu")
 
@@ -497,6 +505,191 @@ class GPUSpectralClustering:
         return self
 
 
+GMM_MAX_D = 256             # AM_GMM_MAX_D
+GMM_MAX_K = 512             # AM_GMM_MAX_K
+GMM_MAX_COMPONENTS = 65535  # AM_GMM_MAX_COMPONENTS: n_init n_components
+GMM_COVARIANCE_TYPE = "full"
+_ILL_DEFINED = ("Fitting the mixture model failed because some components have ill-defined empirical covariance (for "
+                "instance caused by singleton or collapsed samples). Try to decrease the number of components, increase "
+                "reg_covar, or scale the input data.")
+
+
+@dataclass
+class GmmFit:
+    """One GaussianMixture fit: the best init's parameters (float64), its bounds and the labels of one more E-step.
+    With intermediates=True also kpp i32[n_init, K] (the k-means++ rows) and, per init, lower_bounds
+    f64[n_init, max_iter] (NaN after its n_iter), n_iter and converged."""
+    weights: np.ndarray
+    means: np.ndarray
+    covariances: np.ndarray
+    precisions_cholesky: np.ndarray
+    lower_bound: float
+    lower_bounds: list
+    n_iter: int
+    converged: bool
+    best_init: int
+    labels: np.ndarray
+    phase_ms: dict
+    kpp: Optional[np.ndarray] = None
+    init_lower_bounds: Optional[np.ndarray] = None
+    init_n_iter: Optional[np.ndarray] = None
+    init_converged: Optional[np.ndarray] = None
+
+
+def _check_gmm_input(X, n_components):
+    """X as C-contiguous float64 [N, d] with scikit-learn's ValueErrors, before any device work"""
+    X = np.asarray(X)
+    if X.ndim != 2:
+        raise ValueError(f"Expected 2D array, got {X.ndim}D array instead")
+    if X.shape[0] < 2:
+        raise ValueError(f"Found array with {X.shape[0]} sample(s) (shape={X.shape}) while a minimum of 2 is required.")
+    X64 = np.ascontiguousarray(X, dtype=np.float64)
+    if not np.isfinite(X64).all():
+        raise ValueError("Input X contains NaN or infinity.")
+    N, d = X64.shape
+    if N < n_components:
+        raise ValueError(f"Expected n_samples >= n_components but got n_components = {n_components}, n_samples = {N}")
+    if d > GMM_MAX_D:
+        raise ValueError(f"n_features = {d} exceeds {GMM_MAX_D}, the most the GPU mixture supports")
+    return X64
+
+
+def _check_gmm_params(n_components, n_init, max_iter, tol, reg_covar):
+    if not (isinstance(n_components, (int, np.integer)) and n_components >= 1):
+        raise ValueError(f"n_components must be an int >= 1, got {n_components!r}")
+    if n_components > GMM_MAX_K:
+        raise ValueError(f"n_components = {n_components} exceeds {GMM_MAX_K}, the most the GPU mixture supports")
+    if not (isinstance(n_init, (int, np.integer)) and n_init >= 1):
+        raise ValueError(f"n_init must be an int >= 1, got {n_init!r}")
+    if n_init * n_components > GMM_MAX_COMPONENTS:
+        raise ValueError(f"n_init * n_components = {n_init * n_components} exceeds {GMM_MAX_COMPONENTS}, the most the "
+                         "GPU mixture supports")
+    if not (isinstance(max_iter, (int, np.integer)) and max_iter >= 1):
+        raise ValueError(f"max_iter must be an int >= 1, got {max_iter!r}")
+    if not tol >= 0:
+        raise ValueError(f"tol must be >= 0, got {tol!r}")
+    if not reg_covar >= 0:
+        raise ValueError(f"reg_covar must be >= 0, got {reg_covar!r}")
+
+
+def gmm_fit(X, n_components, n_init=10, max_iter=100, tol=1e-3, reg_covar=1e-4, random_state=None,
+            intermediates=False) -> GmmFit:
+    """GaussianMixture(n_components, covariance_type='full', init_params='k-means++', n_init, max_iter, tol,
+    reg_covar, random_state).fit_predict(X) on the device, in float64 whatever X's dtype.  The k-means++ draws come
+    from check_random_state(random_state) on the host, so the generator ends where scikit-learn's fit leaves it.
+    ValueError for invalid input (before any device work) and for an ill-defined covariance; B200Error when the
+    device fails."""
+    _check_gmm_params(n_components, n_init, max_iter, tol, reg_covar)
+    X = _check_gmm_input(X, int(n_components))
+    N, d = X.shape
+    K, n_init, max_iter = int(n_components), int(n_init), int(max_iter)
+    lib = _lib.load()
+    draws = np.ascontiguousarray(kpp_draws(random_state, K, n_init))
+    w = np.empty(K)
+    m = np.empty((K, d))
+    cv = np.empty((K, d, d))
+    pc = np.empty((K, d, d))
+    lbs = np.empty(max_iter)
+    it, conv, best, bad = C.c_int32(0), C.c_int32(0), C.c_int32(0), C.c_int32(0)
+    labels = np.empty(N, np.int64)
+    ms = np.zeros(5, np.float32)
+    kpp = np.empty((n_init, K), np.int32) if intermediates else None
+    ilb = np.empty((n_init, max_iter)) if intermediates else None
+    iit = np.empty(n_init, np.int32) if intermediates else None
+    iconv = np.empty(n_init, np.int32) if intermediates else None
+    opt = lambda a: None if a is None else _lib.ptr(a)   # noqa: E731
+    _lib.check(lib.am_gmm_full_fit(
+        _lib.ptr(X), N, d, K, n_init, max_iter, float(tol), float(reg_covar), _lib.ptr(draws), len(draws),
+        _lib.ptr(w), _lib.ptr(m), _lib.ptr(cv), _lib.ptr(pc), _lib.ptr(lbs), C.byref(it), C.byref(conv), C.byref(best),
+        _lib.ptr(labels), C.byref(bad), opt(kpp), opt(ilb), opt(iit), opt(iconv), _lib.ptr(ms)))
+    if bad.value:
+        raise ValueError(_ILL_DEFINED)
+    n = int(it.value)
+    return GmmFit(weights=w, means=m, covariances=cv, precisions_cholesky=pc, lower_bound=float(lbs[n - 1]),
+                  lower_bounds=[float(v) for v in lbs[:n]], n_iter=n, converged=bool(conv.value),
+                  best_init=int(best.value), labels=labels,
+                  phase_ms=dict(zip(("seeding", "estep", "normalise", "mstep", "cholesky"), map(float, ms))),
+                  kpp=kpp, init_lower_bounds=ilb, init_n_iter=iit, init_converged=None if iconv is None else iconv > 0)
+
+
+class GPUGaussianMixture:
+    """tasks/clustering_gpu.py:284-309 (sklearn.mixture.GaussianMixture there) on the device through gmm_fit, for
+    covariance_type='full' and init_params='k-means++'; other values are refused with ValueError.  max_iter and tol
+    are scikit-learn's defaults.  The clustering task reads means_ for the centres (clustering_helper.py:324-325)."""
+
+    def __init__(self, n_components, covariance_type="full", init_params="k-means++", n_init=10, random_state=None,
+                 reg_covar=1e-4, max_iter=100, tol=1e-3):
+        self.n_components = n_components
+        self.covariance_type = covariance_type
+        self.init_params = init_params
+        self.n_init = n_init
+        self.random_state = random_state
+        self.reg_covar = reg_covar
+        self.max_iter = max_iter
+        self.tol = tol
+        self.model = None
+        self.means_ = None
+        self.weights_ = None
+        self.covariances_ = None
+        self.precisions_cholesky_ = None
+        self.lower_bound_ = None
+        self.lower_bounds_ = None
+        self.n_iter_ = None
+        self.converged_ = None
+        self.labels_ = None
+        self.using_gpu = False
+
+    def _validate(self, X):
+        if self.covariance_type != "full":
+            raise ValueError(f"covariance_type={self.covariance_type!r} is not supported on the GPU (only 'full')")
+        if self.init_params != "k-means++":
+            raise ValueError(f"init_params={self.init_params!r} is not supported on the GPU (only 'k-means++')")
+        _check_gmm_params(self.n_components, self.n_init, self.max_iter, self.tol, self.reg_covar)
+        return _check_gmm_input(X, int(self.n_components))
+
+    def fit_predict(self, X):
+        X64 = self._validate(X)
+        rs = self.random_state
+        if rs is None:
+            rs = np.random.mtrand._rand
+        state = rs.get_state() if isinstance(rs, np.random.RandomState) else None
+        try:
+            f = gmm_fit(X64, int(self.n_components), n_init=int(self.n_init), max_iter=int(self.max_iter),
+                        tol=self.tol, reg_covar=self.reg_covar, random_state=rs)
+            dt = X.dtype if isinstance(X, np.ndarray) and X.dtype in (np.float32, np.float64) else np.float64
+            self.weights_, self.means_ = f.weights.astype(dt), f.means.astype(dt)
+            self.covariances_, self.precisions_cholesky_ = f.covariances.astype(dt), f.precisions_cholesky.astype(dt)
+            self.lower_bound_, self.lower_bounds_ = f.lower_bound, f.lower_bounds
+            self.n_iter_, self.converged_, self.labels_ = f.n_iter, f.converged, f.labels
+            self.using_gpu = True
+            if not f.converged:
+                from sklearn.exceptions import ConvergenceWarning
+                warnings.warn("Best performing initialization did not converge. Try different init parameters, or "
+                              "increase max_iter, tol, or check for degenerate data.", ConvergenceWarning)
+            logger.debug(f"GPU GaussianMixture completed: {self.n_components} components, {f.n_iter} iterations")
+            return f.labels
+        except _lib.B200Error as e:
+            if os.environ.get("B200_ALLOW_SKLEARN_FALLBACK", "0") != "1":
+                raise
+            logger.warning(f"GPU GaussianMixture failed, falling back to CPU: {e}")
+        if state is not None:
+            rs.set_state(state)                     # the fallback draws what the device fit would have drawn
+        from sklearn.mixture import GaussianMixture
+        self.model = GaussianMixture(n_components=self.n_components, covariance_type=self.covariance_type,
+                                     init_params=self.init_params, n_init=self.n_init, random_state=rs,
+                                     reg_covar=self.reg_covar, max_iter=self.max_iter, tol=self.tol)
+        self.labels_ = self.model.fit_predict(X)
+        for n in ("means_", "weights_", "covariances_", "precisions_cholesky_", "lower_bound_", "lower_bounds_",
+                  "n_iter_", "converged_"):
+            setattr(self, n, getattr(self.model, n))
+        self.using_gpu = False
+        return self.labels_
+
+    def fit(self, X):
+        self.fit_predict(X)
+        return self
+
+
 def get_clustering_model(method, params, use_gpu=False):
     if use_gpu and method == "kmeans":
         return GPUKMeans(n_clusters=params["n_clusters"], init="k-means++", n_init=10)
@@ -506,6 +699,9 @@ def get_clustering_model(method, params, use_gpu=False):
         return GPUSpectralClustering(n_clusters=params["n_clusters"], assign_labels="kmeans",
                                      affinity="nearest_neighbors", n_neighbors=params.get("n_neighbors", 20),
                                      random_state=params.get("random_state"), n_init=10, verbose=False)
+    if use_gpu and method == "gmm":
+        return GPUGaussianMixture(n_components=params["n_components"], covariance_type=GMM_COVARIANCE_TYPE,
+                                  init_params="k-means++", n_init=10, random_state=None, reg_covar=1e-4)
     from sklearn.cluster import DBSCAN, KMeans, SpectralClustering
     if method == "kmeans":
         return KMeans(n_clusters=params["n_clusters"], init="k-means++", n_init=10)
@@ -515,6 +711,10 @@ def get_clustering_model(method, params, use_gpu=False):
         return SpectralClustering(n_clusters=params["n_clusters"], assign_labels="kmeans", affinity="nearest_neighbors",
                                   n_neighbors=params.get("n_neighbors", 20), random_state=params.get("random_state"),
                                   n_init=10, verbose=False)
+    if method == "gmm":
+        from sklearn.mixture import GaussianMixture
+        return GaussianMixture(n_components=params["n_components"], covariance_type=GMM_COVARIANCE_TYPE,
+                               init_params="k-means++", n_init=10, random_state=None, reg_covar=1e-4)
     raise ValueError(f"Unsupported clustering method: {method}")
 
 

@@ -51,7 +51,8 @@ METRIC_NAMES = ("silhouette_score", "davies_bouldin_score", "calinski_harabasz_s
 
 
 def apply(clap=None, voyager_manager=None, clustering=None, allow_sklearn_fallback: bool = True,
-          clustering_helper=None, song_alchemy=None, app_map=None, artist_gmm_manager=None) -> None:
+          clustering_helper=None, song_alchemy=None, app_map=None, artist_gmm_manager=None,
+          gaussian_mixture=None) -> None:
     """clap / voyager_manager / clustering / clustering_helper: the reference's already imported tasks.* modules (pass
     only the ones to patch).  allow_sklearn_fallback keeps the reference's contract that a failing GPU k-means silently
     falls back to scikit-learn (tasks/clustering_gpu.py:130-148); this repository's own tests run with it off so a
@@ -63,7 +64,9 @@ def apply(clap=None, voyager_manager=None, clustering=None, allow_sklearn_fallba
     select_optimal_gmm_components; build_and_store_artist_index looks both up at call time (:556, :185), and the
     reference's own functions are kept for the B200_ALLOW_SKLEARN_FALLBACK=1 path.  That module runs `import voyager`
     when it is imported, so install_voyager_shim() must come before `import tasks.artist_gmm_manager` and before
-    `import tasks.analysis`, which imports it."""
+    `import tasks.analysis`, which imports it.  gaussian_mixture (the reference's tasks.clustering_gpu again) gets the
+    GPU GPUGaussianMixture; get_clustering_model looks the class up at call time (:385).  clustering= alone leaves
+    that class to the reference."""
     if clap is not None:
         from . import clap_analyzer as b200_clap
 
@@ -79,6 +82,10 @@ def apply(clap=None, voyager_manager=None, clustering=None, allow_sklearn_fallba
         clustering.GPUPCA = b200_cg.GPUPCA
         clustering.GPUSpectralClustering = b200_cg.GPUSpectralClustering
         clustering.check_gpu_available = b200_cg.check_gpu_available
+    if gaussian_mixture is not None:
+        from . import clustering_gpu as b200_cg
+
+        gaussian_mixture.GPUGaussianMixture = b200_cg.GPUGaussianMixture
     if clustering_helper is not None:
         from . import cluster_metrics as b200_cm
 
@@ -95,6 +102,6 @@ def apply(clap=None, voyager_manager=None, clustering=None, allow_sklearn_fallba
         artist_gmm.capture_originals(artist_gmm_manager)
         artist_gmm_manager.fit_artist_gmm = artist_gmm.fit_artist_gmm
         artist_gmm_manager.select_optimal_gmm_components = artist_gmm.select_optimal_gmm_components
-    if (clustering is not None or clustering_helper is not None or artist_gmm_manager is not None) \
-            and allow_sklearn_fallback:
+    if (clustering is not None or clustering_helper is not None or artist_gmm_manager is not None
+            or gaussian_mixture is not None) and allow_sklearn_fallback:
         os.environ.setdefault("B200_ALLOW_SKLEARN_FALLBACK", "1")

@@ -366,6 +366,31 @@ AM_API int am_artist_gmm_fit(const float* rows, int64_t n_rows, int d, const int
                              float* weights, float* means, float* covariances, int32_t* kpp, int32_t* labels,
                              float* phase_ms);
 
+/* ------------------------------------------------------------------ clustering-task Gaussian mixture, full covariance
+ * GaussianMixture(K, covariance_type='full', init_params='k-means++', n_init, max_iter, tol, reg_covar).fit_predict
+ * (tasks/clustering_helper._apply_clustering_model, method 'gmm') in float64.  Synchronous.
+ *   X            f64[N, d], K <= N, 1 <= d <= AM_GMM_MAX_D, 1 <= K <= AM_GMM_MAX_K,
+ *                n_init K <= AM_GMM_MAX_COMPONENTS (the components of all inits are one launch dimension)
+ *   draws        f64[n_draws]: the generator's random_sample() in order; init i uses the 1 + (K - 1)(2 + floor(ln K))
+ *                doubles from i times that count (at least n_init times it)
+ *   outputs      the best init's (first strictly greatest final lower bound) weights f64[K], means f64[K, d],
+ *                covariances and precisions_cholesky f64[K, d, d], lower_bounds f64[max_iter] (NaN after n_iter),
+ *                n_iter, converged, best_init, labels i64[N] (argmax of one more E-step)
+ *   ill_defined  1 when a Cholesky pivot of any init was <= 0 or not finite (scikit-learn's ValueError); the other
+ *                outputs are then not written
+ *   optional     kpp i32[n_init, K] (k-means++ rows), init_lower_bounds f64[n_init, max_iter], init_n_iter and
+ *                init_converged i32[n_init], phase_ms f32[5] (device ms of seeding, E-step, normaliser, M-step,
+ *                Cholesky and inverse, from CUDA events)
+ * The workspace (about n_init K (N + 3 d^2) doubles) is allocated per call on the call's own stream. */
+#define AM_GMM_MAX_D 256
+#define AM_GMM_MAX_K 512
+#define AM_GMM_MAX_COMPONENTS 65535
+AM_API int am_gmm_full_fit(const double* X, int64_t N, int d, int K, int n_init, int max_iter, double tol,
+                           double reg_covar, const double* draws, int64_t n_draws, double* weights, double* means,
+                           double* covariances, double* precisions_cholesky, double* lower_bounds, int32_t* n_iter,
+                           int32_t* converged, int32_t* best_init, int64_t* labels, int32_t* ill_defined, int32_t* kpp,
+                           double* init_lower_bounds, int32_t* init_n_iter, int32_t* init_converged, float* phase_ms);
+
 #ifdef __cplusplus
 }
 #endif
