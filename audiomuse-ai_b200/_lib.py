@@ -130,6 +130,7 @@ DEBUG_SIGNATURES = {
     "am_bench_gemm": (_i, [_i, _i, _i, _i, _P(C.c_double)]),
     "am_probe_pipe": (_i, [_i, _i, _i, _P(C.c_double)]),
     "am_debug_block": (_i, [_i] * 10 + [_vp] * 10 + [_P(_i)]),
+    "am_debug_kmeans_step": (_i, [_i, _vp, _i64, _i, _i] + [_vp] * 7),
 }
 
 _lib = None

@@ -6,18 +6,18 @@
 // once -- two passes over the data per iteration, HBM-bound.  This file keeps the driver (k-means++ seeding,
 // sklearn's tolerance / empty-cluster rules, restarts) and the CUDA-core kernels that serve k > 128 and small
 // problems:
-//   assign   one warp per point; centres streamed through L1/L2; argmin_c (||c||^2 - 2 x.c)
-//            with fp32 FMAs, lowest index wins ties; inertia accumulated in float64  (compute-bound on CUDA cores);
+//   assign   one warp per point; centres streamed through L1/L2; argmin_c (||c||^2 - 2 x.c) by exact_argmin
+//            (kmeans_tc.cuh), lowest index wins ties; inertia accumulated in float64  (compute-bound on CUDA cores);
 //   update   label-segmented column sums in shared memory ([k, W] slab per CTA, W columns),
 //            flushed with one global atomicAdd per (centre, column) per CTA.
 // Multi-GPU (dist.py): rows stay sharded; am_kmeans_plan_step / am_kmeans_assign_dev produce per-rank partial
 // sums / counts which the host all-reduces (NCCL) before dividing.
 #include "common.cuh"
+#include "gemm_wgmma.cuh"
 #include "kmeans_tc.cuh"
 
 #include <algorithm>
 #include <cmath>
-#include <memory>
 
 namespace am {
 
@@ -47,17 +47,7 @@ assign_kernel(const float* __restrict__ X, int64_t N, int d, const float* __rest
     float xn = 0.f;
     for (int i = lane; i < d; i += 32) xn = fmaf(x[i], x[i], xn);
     xn = warp_sum(xn);
-    for (int j = 0; j < k; ++j) {
-      const float* c = C + (int64_t)j * d;
-      float acc = 0.f;
-      for (int i = lane; i < d; i += 32) acc = fmaf(__ldg(&x[i]), __ldg(&c[i]), acc);
-      acc = warp_sum(acc);
-      const float v = cn[j] - 2.0f * acc;
-      if (v < best) {
-        best = v;
-        best_j = j;
-      }
-    }
+    for (int j = 0; j < k; ++j) exact_argmin<1, 1>(x, d, C, cn, k, lane, j, best, best_j);
     if (lane == 0) {
       labels[row] = best_j;
       if (counts) atomicAdd(&counts[best_j], 1.0f);
@@ -250,11 +240,9 @@ struct SplitMix {
   double uniform() { return (double)(next() >> 11) * (1.0 / 9007199254740992.0); }
 };
 
-static int accumulate_width(int k) { return k <= 128 ? 128 : (k <= 256 ? 64 : 32); }
-
 static int launch_accumulate(const float* X, int64_t N, int d, const int32_t* labels, int k, float* sums,
                              cudaStream_t st) {
-  const int W = accumulate_width(k);
+  const int W = k <= 128 ? 128 : (k <= 256 ? 64 : 32);
   const size_t smem = (size_t)k * W * 4;
   AM_CHECK(smem <= 200 * 1024, "kmeans: k=%d too large for the shared-memory accumulation slab", k);
   AM_TRY(allow_dynamic_smem<accumulate_kernel>(200 * 1024));
@@ -264,13 +252,42 @@ static int launch_accumulate(const float* X, int64_t N, int d, const int32_t* la
   return AM_OK;
 }
 
-static int assign_pass(const float* X, int64_t N, int d, const float* C, float* cn, int k, int32_t* labels,
-                       float* sums, float* counts, double* inertia, cudaStream_t st, float* dist = nullptr) {
-  AM_LAUNCH(center_norms_kernel, ceil_div(k, 8), 256, 0, st, C, k, d, cn);
+__global__ void f64_to_f32_kernel(const double* in, float* out) { out[0] = (float)in[0]; }
+
+// The one choice between the two Lloyd steps.  The tensor-core step (kmeans_tc.cu) is eligible when
+// gemm::available(), 1 <= k <= 128 (the widest assign_tc_kernel), 1 <= d <= 4096 (the recheck band assumes fp32
+// accumulation over at most 4096 terms) and 1 <= N < 2^31 (int32 row lists).  It first builds a split-bf16 copy of
+// the rows, so it serves
+//   KMeansUse::kPlan     every eligible shape: a plan is made to be stepped many times;
+//   KMeansUse::kFit      an eligible shape with N k d >= 5e7 (a whole am_kmeans_fit);
+//   KMeansUse::kAssign   an eligible shape with N k d >= 2e9 (one am_kmeans_assign_dev step pays for the copy alone).
+// Everything else runs on CUDA cores, the only path for k > 128 or d > 4096.
+bool kmeans_use_tensor_cores(int64_t N, int d, int k, KMeansUse use) {
+  if (!gemm::available() || k < 1 || k > 128 || d < 1 || d > 4096 || N < 1 || N >= ((int64_t)1 << 31)) return false;
+  const double work = (double)N * k * d;
+  return use == KMeansUse::kPlan || (use == KMeansUse::kFit && work >= 5e7) ||
+         (use == KMeansUse::kAssign && work >= 2e9);
+}
+
+}  // namespace am
+
+using namespace am;
+
+int am_kmeans_plan::create(bool tensor_cores, cudaStream_t st) {
+  AM_TRY(inert.alloc(1));
+  if (!tensor_cores) return cn.alloc(k);
+  tc.reset(new kmtc::Plan{X, N, d, k});
+  return tc->create(st);
+}
+
+int am_kmeans_plan::step(const float* C, int32_t* labels, float* sums, float* counts, double* inertia, float* dist,
+                         cudaStream_t st) {
+  if (tc) return tc->step(C, labels, sums, counts, inertia, dist, st);
+  AM_LAUNCH(center_norms_kernel, ceil_div(k, 8), 256, 0, st, C, k, d, cn.p);
   if (counts) AM_CUDA(cudaMemsetAsync(counts, 0, (size_t)k * 4, st));
   if (inertia) AM_CUDA(cudaMemsetAsync(inertia, 0, 8, st));
   const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((N + 7) / 8, (int64_t)sm_count() * 8));
-  AM_LAUNCH(assign_kernel, grid, 256, 0, st, X, N, d, C, cn, k, labels, counts, inertia, dist);
+  AM_LAUNCH(assign_kernel, grid, 256, 0, st, X, N, d, C, cn.p, k, labels, counts, inertia, dist);
   if (sums) {
     AM_CUDA(cudaMemsetAsync(sums, 0, (size_t)k * d * 4, st));
     AM_TRY(launch_accumulate(X, N, d, labels, k, sums, st));
@@ -278,63 +295,27 @@ static int assign_pass(const float* X, int64_t N, int d, const float* C, float* 
   return AM_OK;
 }
 
-__global__ void f64_to_f32_kernel(const double* in, float* out) { out[0] = (float)in[0]; }
-
-}  // namespace am
-
-using namespace am;
-
 extern "C" int am_kmeans_assign_dev(const float* X_dev, int64_t N, int d, const float* centers_dev, int k,
                                     int32_t* labels_dev, float* sums_dev, float* counts_dev, float* inertia_dev,
                                     void* stream) {
   AM_CHECK(X_dev && centers_dev && labels_dev, "am_kmeans_assign_dev: NULL argument");
   AM_CHECK(N > 0 && d > 0 && k > 0, "am_kmeans_assign_dev: bad shape");
   AM_TRY(ensure_init());
-  cudaStream_t st = (cudaStream_t)stream;
-  DevBuf<float> cn;
-  DevBuf<double> inert;
-  AM_TRY(cn.alloc(k));
-  AM_TRY(inert.alloc(1));
-  if (kmtc::usable(N, d, k) && (double)N * k * d >= 2e9) {  // big one-shot call: the split pass pays for itself
-    kmtc::Plan plan;
-    AM_TRY(plan.create(X_dev, N, d, k, st));
-    AM_TRY(plan.step(centers_dev, labels_dev, sums_dev, counts_dev, inertia_dev ? inert.p : nullptr, nullptr, st));
-    if (inertia_dev) AM_LAUNCH(f64_to_f32_kernel, 1, 1, 0, st, inert.p, inertia_dev);
-    AM_CUDA(cudaStreamSynchronize(st));
-    return AM_OK;
-  }
-  AM_TRY(assign_pass(X_dev, N, d, centers_dev, cn.p, k, labels_dev, sums_dev, counts_dev,
-                     inertia_dev ? inert.p : nullptr, st));
-  if (inertia_dev) AM_LAUNCH(f64_to_f32_kernel, 1, 1, 0, st, inert.p, inertia_dev);
-  AM_CUDA(cudaStreamSynchronize(st));  // scratch is freed on return
+  am_kmeans_plan p{X_dev, N, d, k};
+  AM_TRY(p.create(kmeans_use_tensor_cores(N, d, k, KMeansUse::kAssign), (cudaStream_t)stream));
+  AM_TRY(am_kmeans_plan_step(&p, centers_dev, labels_dev, sums_dev, counts_dev, inertia_dev, nullptr, stream));
+  AM_CUDA(cudaStreamSynchronize((cudaStream_t)stream));  // the step's scratch is freed on return
   return AM_OK;
 }
 
 // ---- iterative device API: the split-bf16 copy of the rows is built once and reused by every Lloyd step
-struct am_kmeans_plan {
-  kmtc::Plan tc;
-  bool use_tc = false;
-  const float* X = nullptr;
-  int64_t N = 0;
-  int d = 0, k = 0;
-  DevBuf<float> cn;
-  DevBuf<double> inert;
-};
-
 extern "C" int am_kmeans_plan_create(const float* X_dev, int64_t N, int d, int k, void* stream, am_kmeans_plan** out) {
   AM_CHECK(out != nullptr, "am_kmeans_plan_create: out is NULL");
   *out = nullptr;
   AM_CHECK(X_dev && N > 0 && d > 0 && k > 0, "am_kmeans_plan_create: bad argument");
   AM_TRY(ensure_init());
-  auto p = std::make_unique<am_kmeans_plan>();
-  p->X = X_dev;
-  p->N = N;
-  p->d = d;
-  p->k = k;
-  AM_TRY(p->cn.alloc(k));
-  AM_TRY(p->inert.alloc(1));
-  p->use_tc = kmtc::usable(N, d, k);
-  if (p->use_tc) AM_TRY(p->tc.create(X_dev, N, d, k, (cudaStream_t)stream));
+  std::unique_ptr<am_kmeans_plan> p(new am_kmeans_plan{X_dev, N, d, k});
+  AM_TRY(p->create(kmeans_use_tensor_cores(N, d, k, KMeansUse::kPlan), (cudaStream_t)stream));
   *out = p.release();
   return AM_OK;
 }
@@ -348,24 +329,144 @@ extern "C" void am_kmeans_plan_free(am_kmeans_plan* p) {
 extern "C" int am_kmeans_plan_last_recheck(am_kmeans_plan* p, void* stream, int* n_rows) {
   AM_CHECK(p && n_rows, "am_kmeans_plan_last_recheck: NULL argument");
   *n_rows = 0;
-  if (!p->use_tc) return AM_OK;
-  return p->tc.last_recheck_count((cudaStream_t)stream, n_rows);
+  if (!p->tc) return AM_OK;
+  AM_CUDA(cudaMemcpyAsync(n_rows, p->tc->scal.p + 1, sizeof(int), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
+  AM_CUDA(cudaStreamSynchronize((cudaStream_t)stream));
+  return AM_OK;
 }
 
-extern "C" int am_kmeans_plan_uses_tensor_cores(const am_kmeans_plan* p) { return p && p->use_tc ? 1 : 0; }
+extern "C" int am_kmeans_plan_uses_tensor_cores(const am_kmeans_plan* p) { return p && p->tc ? 1 : 0; }
 
 extern "C" int am_kmeans_plan_step(am_kmeans_plan* p, const float* centers_dev, int32_t* labels_dev, float* sums_dev,
                                    float* counts_dev, float* inertia_dev, float* dist_dev, void* stream) {
   AM_CHECK(p && centers_dev && labels_dev, "am_kmeans_plan_step: NULL argument");
   cudaStream_t st = (cudaStream_t)stream;
-  if (p->use_tc) {
-    AM_TRY(p->tc.step(centers_dev, labels_dev, sums_dev, counts_dev, inertia_dev ? p->inert.p : nullptr, dist_dev, st));
-  } else {
-    AM_TRY(assign_pass(p->X, p->N, p->d, centers_dev, p->cn.p, p->k, labels_dev, sums_dev, counts_dev,
-                       inertia_dev ? p->inert.p : nullptr, st, dist_dev));
-  }
+  AM_TRY(p->step(centers_dev, labels_dev, sums_dev, counts_dev, inertia_dev ? p->inert.p : nullptr, dist_dev, st));
   if (inertia_dev) AM_LAUNCH(f64_to_f32_kernel, 1, 1, 0, st, p->inert.p, inertia_dev);
   return AM_OK;  // stream-ordered: no synchronisation
+}
+
+// sklearn: tol_ = mean(var(X, axis=0)) * tol
+static int scaled_tolerance(const float* X, int64_t N, int d, float tol, cudaStream_t st, double* tol_abs) {
+  DevBuf<double> mom;
+  AM_TRY(mom.alloc((size_t)2 * d));
+  AM_CUDA(cudaMemsetAsync(mom.p, 0, (size_t)2 * d * 8, st));
+  dim3 grid(ceil_div(d, 128), (unsigned)std::max<int64_t>(1, std::min<int64_t>(256, N / 1024)));
+  AM_LAUNCH(column_moments_kernel, grid, 128, 0, st, X, N, d, mom.p, mom.p + d);
+  std::vector<double> hm((size_t)2 * d);
+  AM_CUDA(cudaMemcpyAsync(hm.data(), mom.p, hm.size() * 8, cudaMemcpyDeviceToHost, st));
+  AM_CUDA(cudaStreamSynchronize(st));
+  double var_mean = 0.0;
+  for (int c = 0; c < d; ++c) {
+    const double mu = hm[c] / N;
+    var_mean += hm[d + c] / N - mu * mu;
+  }
+  *tol_abs = var_mean / d * tol;
+  return AM_OK;
+}
+
+// greedy k-means++ into C [k, d] (D^2 sampling with 2 + ln k local trials, as sklearn / cuML do), on the device scratch
+// mind2 f32[N], bsum f64[nblk], cand f32[kMaxTrials, d], bpot f64[nblk, kMaxTrials] (nblk 1024-row blocks)
+static int kmeanspp_seed(const float* X, int64_t N, int d, int k, SplitMix& rng, float* C, float* mind2,
+                         double* bsum, float* cand, double* bpot, cudaStream_t st) {
+  const int64_t nblk = (N + 1023) / 1024;
+  std::vector<double> hbs(nblk), hpot((size_t)nblk * kMaxTrials);
+  std::vector<float> hblock(1024);
+  const int L = std::min(kMaxTrials, 2 + (int)std::log((double)k));
+  int64_t pick = std::min<int64_t>((int64_t)(rng.uniform() * N), N - 1);
+  AM_CUDA(cudaMemcpyAsync(C, X + (size_t)pick * d, (size_t)d * 4, cudaMemcpyDeviceToDevice, st));
+  AM_LAUNCH(pp_update_kernel, (unsigned)nblk, 256, 0, st, X, N, d, C, 1, mind2, bsum);
+  for (int j = 1; j < k; ++j) {
+    AM_CUDA(cudaMemcpyAsync(hbs.data(), bsum, nblk * 8, cudaMemcpyDeviceToHost, st));
+    AM_CUDA(cudaStreamSynchronize(st));
+    double total = 0.0;
+    for (double v : hbs) total += v;
+    int64_t cand_row[kMaxTrials];
+    for (int l = 0; l < L; ++l) {
+      double r = rng.uniform() * total;
+      int64_t b = 0;
+      for (; b < nblk - 1; ++b) {
+        if (r < hbs[b]) break;
+        r -= hbs[b];
+      }
+      const int64_t b0 = b * 1024, cnt = std::min<int64_t>(1024, N - b0);
+      AM_CUDA(cudaMemcpyAsync(hblock.data(), mind2 + b0, cnt * 4, cudaMemcpyDeviceToHost, st));
+      AM_CUDA(cudaStreamSynchronize(st));
+      int64_t o = 0;
+      for (; o < cnt - 1; ++o) {
+        if (r < hblock[o]) break;
+        r -= hblock[o];
+      }
+      cand_row[l] = b0 + o;
+      AM_CUDA(cudaMemcpyAsync(cand + (size_t)l * d, X + (size_t)cand_row[l] * d, (size_t)d * 4,
+                              cudaMemcpyDeviceToDevice, st));
+    }
+    AM_LAUNCH(pp_trial_kernel, (unsigned)nblk, 256, 0, st, X, N, d, cand, L, mind2, bpot);
+    AM_CUDA(cudaMemcpyAsync(hpot.data(), bpot, (size_t)nblk * kMaxTrials * 8, cudaMemcpyDeviceToHost, st));
+    AM_CUDA(cudaStreamSynchronize(st));
+    int best = 0;
+    double best_pot = INFINITY;
+    for (int l = 0; l < L; ++l) {
+      double pot = 0.0;
+      for (int64_t b = 0; b < nblk; ++b) pot += hpot[(size_t)b * kMaxTrials + l];
+      if (pot < best_pot) {
+        best_pot = pot;
+        best = l;
+      }
+    }
+    AM_CUDA(cudaMemcpyAsync(C + (size_t)j * d, cand + (size_t)best * d, (size_t)d * 4, cudaMemcpyDeviceToDevice,
+                            st));
+    if (j < k - 1)
+      AM_LAUNCH(pp_update_kernel, (unsigned)nblk, 256, 0, st, X, N, d, C + (size_t)j * d, 0, mind2, bsum);
+  }
+  return AM_OK;
+}
+
+// sklearn's Lloyd from the centres in C, at most max_iter steps: after each E-step, empty clusters are relocated as
+// sklearn does it, then the centres move; stops once the squared shift is <= tol_abs.  *n_iter = the steps run.
+static int lloyd(am_kmeans_plan& step, int max_iter, double tol_abs, float* C, int32_t* labels, float* sums,
+                 float* counts, float* dist, double* shift2_dev, cudaStream_t st, int* n_iter) {
+  const int64_t N = step.N;
+  const int d = step.d, k = step.k;
+  std::vector<float> hcounts((size_t)k), hdist;
+  DevBuf<int64_t> far_dev;
+  DevBuf<int32_t> empty_dev;
+  int it = 0;
+  for (it = 1; it <= max_iter; ++it) {
+    AM_TRY(step.step(C, labels, sums, counts, nullptr, dist, st));
+    // empty clusters are relocated the way sklearn's Lloyd does it (rare: costs one [k] read-back per
+    // iteration, and the [N] distances only when a cluster actually emptied)
+    AM_CUDA(cudaMemcpyAsync(hcounts.data(), counts, (size_t)k * 4, cudaMemcpyDeviceToHost, st));
+    AM_CUDA(cudaStreamSynchronize(st));
+    std::vector<int32_t> empty;
+    for (int j = 0; j < k; ++j)
+      if (hcounts[j] == 0.f) empty.push_back(j);
+    if (!empty.empty() && (int64_t)empty.size() < N) {
+      hdist.resize((size_t)N);
+      AM_CUDA(cudaMemcpyAsync(hdist.data(), dist, (size_t)N * 4, cudaMemcpyDeviceToHost, st));
+      AM_CUDA(cudaStreamSynchronize(st));
+      std::vector<int64_t> order((size_t)N);
+      for (int64_t i = 0; i < N; ++i) order[(size_t)i] = i;
+      std::partial_sort(order.begin(), order.begin() + (int64_t)empty.size(), order.end(), [&](int64_t a, int64_t b) {
+        return hdist[(size_t)a] > hdist[(size_t)b] || (hdist[(size_t)a] == hdist[(size_t)b] && a < b);
+      });
+      AM_TRY(far_dev.alloc(empty.size()));
+      AM_TRY(empty_dev.alloc(empty.size()));
+      AM_CUDA(cudaMemcpyAsync(far_dev.p, order.data(), empty.size() * 8, cudaMemcpyHostToDevice, st));
+      AM_CUDA(cudaMemcpyAsync(empty_dev.p, empty.data(), empty.size() * 4, cudaMemcpyHostToDevice, st));
+      AM_LAUNCH(relocate_empty_kernel, 1, 256, 0, st, step.X, d, labels, far_dev.p, empty_dev.p, (int)empty.size(), sums,
+                counts);
+      AM_CUDA(cudaStreamSynchronize(st));  // far_dev / empty_dev are reused next time
+    }
+    AM_CUDA(cudaMemsetAsync(shift2_dev, 0, 8, st));
+    AM_LAUNCH(update_centers_kernel, k, 128, 0, st, sums, counts, k, d, C, shift2_dev);
+    double shift2 = 0.0;
+    AM_CUDA(cudaMemcpyAsync(&shift2, shift2_dev, 8, cudaMemcpyDeviceToHost, st));
+    AM_CUDA(cudaStreamSynchronize(st));
+    if (shift2 <= tol_abs) break;
+  }
+  *n_iter = std::min(it, max_iter);
+  return AM_OK;
 }
 
 extern "C" int am_kmeans_fit(const float* X, int64_t N, int d, int k, int n_init, int max_iter, float tol,
@@ -377,161 +478,45 @@ extern "C" int am_kmeans_fit(const float* X, int64_t N, int d, int k, int n_init
   AM_TRY(ensure_init());
   Stream st;
   AM_TRY(st.create());
-  DevBuf<float> dX, dC, dBestC, cn, sums, counts, mind2;
+  DevBuf<float> dX, dC, dBestC, sums, counts, dist, mind2, cand;
   DevBuf<int32_t> dL, dBestL;
-  DevBuf<double> scal, bsum, mom;
+  DevBuf<double> scal, bsum, bpot;
   AM_TRY(dX.alloc((size_t)N * d));
   AM_TRY(dC.alloc((size_t)k * d));
   AM_TRY(dBestC.alloc((size_t)k * d));
-  AM_TRY(cn.alloc(k));
   AM_TRY(sums.alloc((size_t)k * d));
   AM_TRY(counts.alloc(k));
+  AM_TRY(dist.alloc((size_t)N));
   AM_TRY(dL.alloc(N));
   AM_TRY(dBestL.alloc(N));
   AM_TRY(scal.alloc(2));  // [0] inertia, [1] shift2
-  AM_TRY(mom.alloc((size_t)2 * d));
   AM_CUDA(cudaMemcpyAsync(dX.p, X, (size_t)N * d * 4, cudaMemcpyHostToDevice, st.s));
-  std::unique_ptr<kmtc::Plan> plan;
-  if (kmtc::usable(N, d, k) && (double)N * k * d >= 5e7) {
-    plan = std::make_unique<kmtc::Plan>();
-    AM_TRY(plan->create(dX.p, N, d, k, st.s));
-  }
-
-  // sklearn: tol_ = mean(var(X, axis=0)) * tol
-  AM_CUDA(cudaMemsetAsync(mom.p, 0, (size_t)2 * d * 8, st.s));
-  {
-    dim3 grid(ceil_div(d, 128), (unsigned)std::max<int64_t>(1, std::min<int64_t>(256, N / 1024)));
-    AM_LAUNCH(column_moments_kernel, grid, 128, 0, st.s, dX.p, N, d, mom.p, mom.p + d);
-  }
-  std::vector<double> hm((size_t)2 * d);
-  AM_CUDA(cudaMemcpyAsync(hm.data(), mom.p, hm.size() * 8, cudaMemcpyDeviceToHost, st.s));
-  AM_CUDA(cudaStreamSynchronize(st.s));
-  double var_mean = 0.0;
-  for (int c = 0; c < d; ++c) {
-    const double mu = hm[c] / N;
-    var_mean += hm[d + c] / N - mu * mu;
-  }
-  var_mean /= d;
-  const double tol_abs = var_mean * tol;
+  am_kmeans_plan step{dX.p, N, d, k};
+  AM_TRY(step.create(kmeans_use_tensor_cores(N, d, k, KMeansUse::kFit), st.s));
+  double tol_abs = 0.0;
+  AM_TRY(scaled_tolerance(dX.p, N, d, tol, st.s, &tol_abs));
 
   SplitMix rng{seed ^ 0x5851f42d4c957f2dull};
-  double best_inertia = INFINITY;
-  int best_iters = 0;
-  const int restarts = init_centers ? 1 : n_init;
   const int64_t nblk = (N + 1023) / 1024;
-  DevBuf<float> cand;
-  DevBuf<double> bpot;
   if (!init_centers) {
     AM_TRY(mind2.alloc(N));
     AM_TRY(bsum.alloc(nblk));
     AM_TRY(cand.alloc((size_t)kMaxTrials * d));
     AM_TRY(bpot.alloc((size_t)nblk * kMaxTrials));
   }
-  std::vector<double> hbs(nblk), hpot((size_t)nblk * kMaxTrials);
-  std::vector<float> hcounts((size_t)k), hdist;
-  DevBuf<float> pdist;
-  DevBuf<int64_t> far_dev;
-  DevBuf<int32_t> empty_dev;
-  AM_TRY(pdist.alloc((size_t)N));
-  std::vector<float> hblock(1024);
-
-  for (int run = 0; run < restarts; ++run) {
-    if (init_centers) {
-      AM_CUDA(cudaMemcpyAsync(dC.p, init_centers, (size_t)k * d * 4, cudaMemcpyHostToDevice, st.s));
-    } else {
-      // greedy k-means++ (D^2 sampling with 2 + ln k local trials, as sklearn / cuML do)
-      const int L = std::min(kMaxTrials, 2 + (int)std::log((double)k));
-      int64_t pick = std::min<int64_t>((int64_t)(rng.uniform() * N), N - 1);
-      AM_CUDA(cudaMemcpyAsync(dC.p, dX.p + (size_t)pick * d, (size_t)d * 4, cudaMemcpyDeviceToDevice, st.s));
-      AM_LAUNCH(pp_update_kernel, (unsigned)nblk, 256, 0, st.s, dX.p, N, d, dC.p, 1, mind2.p, bsum.p);
-      for (int j = 1; j < k; ++j) {
-        AM_CUDA(cudaMemcpyAsync(hbs.data(), bsum.p, nblk * 8, cudaMemcpyDeviceToHost, st.s));
-        AM_CUDA(cudaStreamSynchronize(st.s));
-        double total = 0.0;
-        for (double v : hbs) total += v;
-        int64_t cand_row[kMaxTrials];
-        for (int l = 0; l < L; ++l) {
-          double r = rng.uniform() * total;
-          int64_t b = 0;
-          for (; b < nblk - 1; ++b) {
-            if (r < hbs[b]) break;
-            r -= hbs[b];
-          }
-          const int64_t b0 = b * 1024, cnt = std::min<int64_t>(1024, N - b0);
-          AM_CUDA(cudaMemcpyAsync(hblock.data(), mind2.p + b0, cnt * 4, cudaMemcpyDeviceToHost, st.s));
-          AM_CUDA(cudaStreamSynchronize(st.s));
-          int64_t o = 0;
-          for (; o < cnt - 1; ++o) {
-            if (r < hblock[o]) break;
-            r -= hblock[o];
-          }
-          cand_row[l] = b0 + o;
-          AM_CUDA(cudaMemcpyAsync(cand.p + (size_t)l * d, dX.p + (size_t)cand_row[l] * d, (size_t)d * 4,
-                                  cudaMemcpyDeviceToDevice, st.s));
-        }
-        AM_LAUNCH(pp_trial_kernel, (unsigned)nblk, 256, 0, st.s, dX.p, N, d, cand.p, L, mind2.p, bpot.p);
-        AM_CUDA(cudaMemcpyAsync(hpot.data(), bpot.p, (size_t)nblk * kMaxTrials * 8, cudaMemcpyDeviceToHost, st.s));
-        AM_CUDA(cudaStreamSynchronize(st.s));
-        int best = 0;
-        double best_pot = INFINITY;
-        for (int l = 0; l < L; ++l) {
-          double pot = 0.0;
-          for (int64_t b = 0; b < nblk; ++b) pot += hpot[(size_t)b * kMaxTrials + l];
-          if (pot < best_pot) {
-            best_pot = pot;
-            best = l;
-          }
-        }
-        AM_CUDA(cudaMemcpyAsync(dC.p + (size_t)j * d, cand.p + (size_t)best * d, (size_t)d * 4,
-                                cudaMemcpyDeviceToDevice, st.s));
-        if (j < k - 1)
-          AM_LAUNCH(pp_update_kernel, (unsigned)nblk, 256, 0, st.s, dX.p, N, d, dC.p + (size_t)j * d, 0, mind2.p,
-                    bsum.p);
-      }
-    }
+  double best_inertia = INFINITY;
+  int best_iters = 0;
+  for (int run = 0; run < (init_centers ? 1 : n_init); ++run) {
+    if (init_centers) AM_CUDA(cudaMemcpyAsync(dC.p, init_centers, (size_t)k * d * 4, cudaMemcpyHostToDevice, st.s));
+    else AM_TRY(kmeanspp_seed(dX.p, N, d, k, rng, dC.p, mind2.p, bsum.p, cand.p, bpot.p, st.s));
     int it = 0;
-    for (it = 1; it <= max_iter; ++it) {
-      if (plan) AM_TRY(plan->step(dC.p, dL.p, sums.p, counts.p, nullptr, pdist.p, st.s));
-      else AM_TRY(assign_pass(dX.p, N, d, dC.p, cn.p, k, dL.p, sums.p, counts.p, nullptr, st.s, pdist.p));
-      // empty clusters are relocated the way sklearn's Lloyd does it (rare: costs one [k] read-back per
-      // iteration, and the [N] distances only when a cluster actually emptied)
-      AM_CUDA(cudaMemcpyAsync(hcounts.data(), counts.p, (size_t)k * 4, cudaMemcpyDeviceToHost, st.s));
-      AM_CUDA(cudaStreamSynchronize(st.s));
-      std::vector<int32_t> empty;
-      for (int j = 0; j < k; ++j)
-        if (hcounts[j] == 0.f) empty.push_back(j);
-      if (!empty.empty() && (int64_t)empty.size() < N) {
-        hdist.resize((size_t)N);
-        AM_CUDA(cudaMemcpyAsync(hdist.data(), pdist.p, (size_t)N * 4, cudaMemcpyDeviceToHost, st.s));
-        AM_CUDA(cudaStreamSynchronize(st.s));
-        std::vector<int64_t> order((size_t)N);
-        for (int64_t i = 0; i < N; ++i) order[(size_t)i] = i;
-        std::partial_sort(order.begin(), order.begin() + (int64_t)empty.size(), order.end(), [&](int64_t a, int64_t b) {
-          return hdist[(size_t)a] > hdist[(size_t)b] || (hdist[(size_t)a] == hdist[(size_t)b] && a < b);
-        });
-        AM_TRY(far_dev.alloc(empty.size()));
-        AM_TRY(empty_dev.alloc(empty.size()));
-        AM_CUDA(cudaMemcpyAsync(far_dev.p, order.data(), empty.size() * 8, cudaMemcpyHostToDevice, st.s));
-        AM_CUDA(cudaMemcpyAsync(empty_dev.p, empty.data(), empty.size() * 4, cudaMemcpyHostToDevice, st.s));
-        AM_LAUNCH(relocate_empty_kernel, 1, 256, 0, st.s, dX.p, d, dL.p, far_dev.p, empty_dev.p, (int)empty.size(), sums.p,
-                  counts.p);
-        AM_CUDA(cudaStreamSynchronize(st.s));  // far_dev / empty_dev are reused next time
-      }
-      AM_CUDA(cudaMemsetAsync(scal.p + 1, 0, 8, st.s));
-      AM_LAUNCH(update_centers_kernel, k, 128, 0, st.s, sums.p, counts.p, k, d, dC.p, scal.p + 1);
-      double shift2 = 0.0;
-      AM_CUDA(cudaMemcpyAsync(&shift2, scal.p + 1, 8, cudaMemcpyDeviceToHost, st.s));
-      AM_CUDA(cudaStreamSynchronize(st.s));
-      if (shift2 <= tol_abs) break;
-    }
-    it = std::min(it, max_iter);
+    AM_TRY(lloyd(step, max_iter, tol_abs, dC.p, dL.p, sums.p, counts.p, dist.p, scal.p + 1, st.s, &it));
     // final E-step: labels and inertia consistent with the returned centres
-    if (plan) AM_TRY(plan->step(dC.p, dL.p, nullptr, nullptr, scal.p, nullptr, st.s));
-    else AM_TRY(assign_pass(dX.p, N, d, dC.p, cn.p, k, dL.p, nullptr, nullptr, scal.p, st.s));
+    AM_TRY(step.step(dC.p, dL.p, nullptr, nullptr, scal.p, nullptr, st.s));
     double inert = 0.0;
     AM_CUDA(cudaMemcpyAsync(&inert, scal.p, 8, cudaMemcpyDeviceToHost, st.s));
     AM_CUDA(cudaStreamSynchronize(st.s));
-    if (inert < best_inertia) {
+    if (inert < best_inertia) {  // keep the best restart
       best_inertia = inert;
       best_iters = it;
       AM_CUDA(cudaMemcpyAsync(dBestC.p, dC.p, (size_t)k * d * 4, cudaMemcpyDeviceToDevice, st.s));

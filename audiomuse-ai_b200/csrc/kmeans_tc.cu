@@ -19,7 +19,7 @@
 //                                                 exists in memory.
 //                               A point whose runner-up is within the proven error band of the best
 //                               (2^-11 ||x|| max||c||) is appended to a recheck list.
-//     recheck_kernel            exact fp32 argmin (the CUDA-core arithmetic of kmeans.cu's assign_kernel) for the
+//     recheck_kernel            exact fp32 argmin (exact_argmin, shared with kmeans.cu's assign_kernel) for the
 //                               listed points only: labels equal the exact-arithmetic labels for EVERY point.
 //     accumulate_sorted_kernel  M-step partial sums: a CTA counting-sorts the labels of its 2048-point slab in
 //                               shared memory, then each warp walks one label segment: rows are read once, as whole
@@ -198,10 +198,9 @@ assign_tc_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constan
   }
 }
 
-// exact fp32 argmin for the listed rows, the arithmetic of kmeans.cu's assign_kernel (v_j = cn_j - 2 x.c_j with
-// lane-strided fp32 FMAs + a shuffle tree; strict "<" in index order, so the lowest index wins ties).  One CTA per
-// row, the centres dealt round-robin to its 8 warps (a single warp walking all k centres took ~0.3 ms per row, and
-// a kernel is as slow as its slowest row); each warp keeps four dot products in flight.
+// exact fp32 argmin for the listed rows (exact_argmin, kmeans_tc.cuh, as assign_kernel decides).  One CTA per row,
+// the centres dealt round-robin to its 8 warps (a single warp walking all k centres took ~0.3 ms per row, and a
+// kernel is as slow as its slowest row); each warp keeps four dot products in flight, centres j0 + 8 u (u < 4).
 __global__ void __launch_bounds__(256)
 recheck_kernel(const float* __restrict__ X, int d, const float* __restrict__ C, const float* __restrict__ cn, int k,
                const int* __restrict__ n_recheck, const int32_t* __restrict__ recheck, int32_t* __restrict__ labels,
@@ -218,29 +217,7 @@ recheck_kernel(const float* __restrict__ X, int d, const float* __restrict__ C, 
     xn = warp_sum(xn);
     float best = INFINITY;
     int best_j = 0x7fffffff;
-    for (int j0 = warp; j0 < k; j0 += 32) {  // centres j0, j0 + 8, j0 + 16, j0 + 24 together
-      float acc[4] = {0.f, 0.f, 0.f, 0.f};
-      for (int i = lane; i < d; i += 32) {
-        const float xv = __ldg(&x[i]);
-#pragma unroll
-        for (int u = 0; u < 4; ++u) {
-          const int j = j0 + 8 * u;
-          if (j < k) acc[u] = fmaf(xv, __ldg(&C[(int64_t)j * d + i]), acc[u]);
-        }
-      }
-#pragma unroll
-      for (int u = 0; u < 4; ++u) {
-        const int j = j0 + 8 * u;
-        const float a = warp_sum(acc[u]);
-        if (j < k) {
-          const float v = cn[j] - 2.0f * a;
-          if (v < best) {  // j increases inside a warp: ties keep the lower index
-            best = v;
-            best_j = j;
-          }
-        }
-      }
-    }
+    for (int j0 = warp; j0 < k; j0 += 32) exact_argmin<4, 8>(x, d, C, cn, k, lane, j0, best, best_j);
     if (lane == 0) {
       s_best[warp] = best;
       s_idx[warp] = best_j;
@@ -388,16 +365,7 @@ accumulate_sorted_kernel(const float* __restrict__ X, int64_t N, int d, const in
 }
 
 // ---------------------------------------------------------------- host
-bool usable(int64_t N, int d, int k) {
-  return gemm::available() && k >= 1 && k <= 128 && d >= 1 && d <= 4096 && N >= 1 && N < ((int64_t)1 << 31) &&
-         std::getenv("AM_KMEANS_SIMT") == nullptr;
-}
-
-int Plan::create(const float* X_dev, int64_t N_, int d_, int k_, cudaStream_t st) {
-  N = N_;
-  d = d_;
-  k = k_;
-  X = X_dev;
+int Plan::create(cudaStream_t st) {
   dp = (int)round_up((size_t)d, 64);
   kp = (int)round_up((size_t)k, 16);
   AM_TRY(Xs.alloc((size_t)N * 2 * dp));
@@ -406,7 +374,6 @@ int Plan::create(const float* X_dev, int64_t N_, int d_, int k_, cudaStream_t st
   AM_TRY(cn.alloc((size_t)kp));
   AM_TRY(scal.alloc(2));  // [0] max ||c||^2 bits, [1] recheck counter
   AM_TRY(recheck.alloc((size_t)N));
-  AM_TRY(inertia64.alloc(1));
   const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((N + 7) / 8, (int64_t)sm_count() * 16));
   AM_LAUNCH(split_rows_kernel, grid, 256, 0, st, X, N, d, dp, Xs.p, xn.p);
   AM_TRY(gemm::encode_map_bf16(map_x, Xs.p, 2 * dp, N, 2 * dp, kTileM));
@@ -483,12 +450,6 @@ int Plan::step(const float* C_dev, int32_t* labels, float* sums, float* counts, 
     AM_CUDA(cudaMemsetAsync(scratch_sums.p, 0, (size_t)k * d * 4, st));
     AM_TRY(launch_accumulate(scratch_sums.p, nullptr, inertia_dev, C_dev, labels, st));
   }
-  return AM_OK;
-}
-
-int Plan::last_recheck_count(cudaStream_t st, int* out) {
-  AM_CUDA(cudaMemcpyAsync(out, scal.p + 1, sizeof(int), cudaMemcpyDeviceToHost, st));
-  AM_CUDA(cudaStreamSynchronize(st));
   return AM_OK;
 }
 

@@ -263,8 +263,8 @@ AM_API int am_cluster_scores(const float* X, int64_t N, int d, const int32_t* la
 
 /* Iterative form for Lloyd loops on device data (multi-GPU: one plan per rank over its row shard, the host all-reduces
  * sums / counts between steps; tasks/clustering_gpu.py:108-124 is the call this serves).  The plan keeps a split-bf16
- * copy of the rows so each step is one tensor-core assignment pass + one partial-sum pass (k <= 128; larger k runs on
- * CUDA cores).  X_dev must stay valid while the plan lives.  am_kmeans_plan_step is stream-ordered (no sync):
+ * copy of the rows so each step is one tensor-core assignment pass + one partial-sum pass when the shape allows it
+ * (kmeans_use_tensor_cores in csrc/kmeans.cu; k > 128 or d > 4096 runs on CUDA cores).  X_dev must stay valid while the plan lives.  am_kmeans_plan_step is stream-ordered (no sync):
  * labels i32[N]; sums f32[k,d], counts f32[k], inertia f32[1] (each optional) are OVERWRITTEN; dist f32[N] (optional)
  * receives the squared distance of every row to its centre. */
 typedef struct am_kmeans_plan am_kmeans_plan;

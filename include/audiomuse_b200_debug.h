@@ -33,6 +33,13 @@ AM_API int am_debug_block(int path, int B, int H, int W, int cin_p, int cmid_p, 
                           int residual, const uint16_t* X, const uint16_t* W1, const float* b1, const float* wd,
                           const float* bd, const uint16_t* W2, const float* b2, uint16_t* Y, uint16_t* E_out,
                           uint16_t* D_out, int* info);
+/* debug: one k-means Lloyd step on a named path, with the operands of am_kmeans_plan_step plus the rows X_dev [N, d]
+ * and k; synchronises before it returns.
+ *   path 0: the tensor-core step; a shape it does not take is an error.
+ *   path 1: the exact CUDA-core step. */
+AM_API int am_debug_kmeans_step(int path, const float* X_dev, int64_t N, int d, int k, const float* centers_dev,
+                                int32_t* labels_dev, float* sums_dev, float* counts_dev, float* inertia_dev,
+                                float* dist_dev, void* stream);
 
 #ifdef __cplusplus
 }

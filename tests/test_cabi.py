@@ -35,13 +35,14 @@ def test_library_exports_every_declared_symbol(lib):
     assert set(_lib.SIGNATURES) == set(names), set(_lib.SIGNATURES) ^ set(names)
 
 
-def test_product_library_ships_no_debug_probes(lib):
-    """The probes / self tests (include/audiomuse_b200_debug.h) live in libaudiomuse_b200_debug.so only."""
+def test_product_library_ships_no_debug_entry_points(lib):
+    """The probes, self tests and debug entry points (include/audiomuse_b200_debug.h, am_debug_kmeans_step among
+    them) live in libaudiomuse_b200_debug.so only."""
     from audiomuse_ai_b200 import _lib
     txt = open(os.path.join(ROOT, "include", "audiomuse_b200_debug.h")).read()
     dbg_names = sorted(set(re.findall(r"AM_API\s+[\w\s\*]+?\b(am_\w+)\s*\(", txt)))
     assert set(dbg_names) == set(_lib.DEBUG_SIGNATURES) == {"am_selftest_gemm", "am_bench_gemm", "am_probe_pipe",
-                                                            "am_debug_block"}
+                                                            "am_debug_block", "am_debug_kmeans_step"}
     dbg = _lib.load_debug()
     for n in dbg_names:
         assert hasattr(dbg, n)

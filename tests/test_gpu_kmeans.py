@@ -132,14 +132,16 @@ def test_config4_scale_properties():
 
 @pytest.mark.parametrize("n,d,k,kind", [(60000, 512, 128, "clustered"), (40000, 200, 100, "clustered"),
                                         (30000, 58, 40, "uniform"), (20000, 96, 7, "uniform")])
-def test_tensor_core_step_equals_exact_path(n, d, k, kind):
+def test_tensor_core_step_equals_debug_exact_step(n, d, k, kind):
     """am_kmeans_plan_step (split-bf16 wgmma GEMM + fused argmin + exact recheck of near-ties) returns the SAME
-    labels as the exact fp32 CUDA-core path (AM_KMEANS_SIMT=1) -- on clustered data and on structureless data, where
-    a large share of the points is a near-tie -- and matching counts / sums / inertia.  d = 58, 200 and k in [40, 100]
-    are the reference's shapes (clustering_helper.py), 512 / 128 is config 4."""
-    import os
+    labels as the exact fp32 CUDA-core step that am_debug_kmeans_step path 1 runs on the same shape -- on clustered
+    data and on structureless data, where a large share of the points is a near-tie -- and matching counts / sums /
+    inertia.  d = 58, 200 and k in [40, 100] are the reference's shapes (clustering_helper.py), 512 / 128 is
+    config 4."""
+    import ctypes as C
+    import json
     import torch
-    from audiomuse_ai_b200 import dist as amdist
+    from audiomuse_ai_b200 import _lib, dist as amdist
     if kind == "clustered":
         x, _, cen = _data(n, d, k, 5)
         centers = cen + 0.02 * np.random.default_rng(0).standard_normal(cen.shape).astype(np.float32)
@@ -149,20 +151,30 @@ def test_tensor_core_step_equals_exact_path(n, d, k, kind):
     xd, cd = torch.from_numpy(x).cuda(), torch.from_numpy(centers).cuda()
     out = {}
     for mode in ("tc", "simt"):
-        if mode == "simt":
-            os.environ["AM_KMEANS_SIMT"] = "1"
-        try:
-            plan = amdist.KMeansPlan(xd, k)
-        finally:
-            os.environ.pop("AM_KMEANS_SIMT", None)
-        assert plan.uses_tensor_cores == (mode == "tc")
         lab = torch.empty(n, dtype=torch.int32, device="cuda")
         sums = torch.empty(k, d, device="cuda"); cnt = torch.empty(k, device="cuda"); inert = torch.zeros(1, device="cuda")
         dist = torch.empty(n, device="cuda")
-        plan.step(cd, lab, sums, cnt, inert, dist)
-        torch.cuda.synchronize()
+        if mode == "tc":
+            plan = amdist.KMeansPlan(xd, k)
+            assert plan.uses_tensor_cores
+            plan.step(cd, lab, sums, cnt, inert, dist)
+            torch.cuda.synchronize()
+            plan.close()
+        else:
+            p = lambda t: C.c_void_p(t.data_ptr())  # noqa: E731
+            dbg = _lib.load_debug()
+            dbg.am_profile_enable(1)
+            _lib.check_debug(dbg.am_debug_kmeans_step(
+                1, p(xd), n, d, k, p(cd), p(lab), p(sums), p(cnt), p(inert), p(dist),
+                C.c_void_p(torch.cuda.current_stream().cuda_stream)))
+            size = dbg.am_profile_report(None, 0)
+            buf = C.create_string_buffer(size + 16)
+            dbg.am_profile_report(buf, size + 16)
+            dbg.am_profile_enable(0)
+            kernels = json.loads(buf.value.decode() or "{}")
+            # the exact side ran on CUDA cores: assign_kernel, no tensor-core assignment
+            assert "assign_kernel" in kernels and not any(kk.startswith("assign_tc_kernel") for kk in kernels), kernels
         out[mode] = (lab.cpu().numpy(), sums.cpu().numpy(), cnt.cpu().numpy(), float(inert.item()), dist.cpu().numpy())
-        plan.close()
     np.testing.assert_array_equal(out["tc"][0], out["simt"][0])
     np.testing.assert_array_equal(out["tc"][2], out["simt"][2])
     np.testing.assert_allclose(out["tc"][1], out["simt"][1], rtol=2e-5, atol=2e-3)
@@ -170,3 +182,15 @@ def test_tensor_core_step_equals_exact_path(n, d, k, kind):
     np.testing.assert_allclose(out["tc"][4], out["simt"][4], rtol=0, atol=2e-3 * max(1.0, float(out["simt"][4].max())))
     want_lab, want_inertia = okm.assign(x[:4000], centers)
     assert (out["tc"][0][:4000] == want_lab).mean() > 0.999       # float64 oracle (ties aside)
+
+
+def test_plan_path_follows_the_shape():
+    """A plan takes the tensor-core step for every shape it can serve (k <= 128, d <= 4096) and the CUDA-core step
+    beyond either limit (kmeans_use_tensor_cores in kmeans.cu)."""
+    import torch
+    from audiomuse_ai_b200 import dist as amdist
+    x = torch.zeros(300, 4097, device="cuda")
+    for k, d, want in ((128, 512, True), (129, 512, False), (40, 4097, False)):
+        plan = amdist.KMeansPlan(x[:, :d].contiguous(), k)
+        assert plan.uses_tensor_cores == want, (k, d)
+        plan.close()

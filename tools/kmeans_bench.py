@@ -1,8 +1,10 @@
 """Config 4 (BASELINE.json configs[3]): Lloyd iterations on 1 M x 512 f32 rows, k = 128, one GPU.
 Times `iters` am_kmeans_plan_step calls (assignment GEMM with fused argmin + recheck + partial sums) with CUDA events,
-checks the labels of the tensor-core path against the exact CUDA-core path (AM_KMEANS_SIMT=1), and prints one JSON line.
+checks the labels of the tensor-core path against the exact CUDA-core path (am_debug_kmeans_step in the debug
+library), and prints one JSON line.
     python tools/kmeans_bench.py [--n 1000000] [--iters 20]"""
 import argparse
+import ctypes as C
 import json
 import os
 import sys
@@ -66,13 +68,10 @@ out = {"config": f"{a.n} x {d} f32, k={k}", "tensor_cores": plan.uses_tensor_cor
 if a.check:
     plan.step(centers, labels, sums, counts, inertia)
     torch.cuda.synchronize()
-    os.environ["AM_KMEANS_SIMT"] = "1"
-    exact = amdist.KMeansPlan(xd, k)
-    assert not exact.uses_tensor_cores
     l2 = torch.empty_like(labels); s2 = torch.empty_like(sums); c2 = torch.empty_like(counts); i2 = torch.zeros(1, device="cuda")
-    exact.step(centers, l2, s2, c2, i2)
-    torch.cuda.synchronize()
-    del os.environ["AM_KMEANS_SIMT"]
+    p = lambda t: C.c_void_p(t.data_ptr())  # noqa: E731
+    _lib.check_debug(_lib.load_debug().am_debug_kmeans_step(1, p(xd), a.n, d, k, p(centers), p(l2), p(s2), p(c2), p(i2),
+                                                            None, C.c_void_p(torch.cuda.current_stream().cuda_stream)))
     out["labels_equal_exact_path"] = bool((labels == l2).all().item())
     out["label_mismatches"] = int((labels != l2).sum().item())
     out["counts_equal"] = bool((counts == c2).all().item())
