@@ -10,14 +10,15 @@
 //                 bias in one bulk copy (packed per chunk at model load, pack_params).  The next tile's halo and first
 //                 chunks load while the consumers finish the current tile.
 //   warpgroups 1, 2   consumers, sharing one tile; per chunk:
-//     expansion   at stride 1 wgmma m64n64k16, one of the 2 halo m blocks per warpgroup; at stride 2 m64n32k16 over
-//                 all 5 m blocks, one 32-column half of the chunk per warpgroup; fp32 accumulators -> + bias, ReLU6
-//                 -> bf16 halo tile E [halo pixels x 64, 16-byte groups XOR-swizzled by pixel] (pixels outside the
-//                 image are zero: the depthwise pads with 0, and relu6(bias) need not be);
+//     expansion   transposed, E^T = W1 chunk . halo^T, so the halo pixels are the MMA's N: each warpgroup one
+//                 contiguous run of 8-pixel atoms (wgmma m64n152k16 / m64n144k16 at stride 2, m64n56k16 / m64n48k16
+//                 at stride 1); fp32 accumulators -> + bias, ReLU6 -> bf16, stored back pixel-major by stmatrix
+//                 .trans into the halo tile E [halo pixels x 64, 16-byte groups XOR-swizzled by pixel] (pixels
+//                 outside the image are zero: the depthwise pads with 0, and relu6(bias) need not be);
 //     depthwise   3 x 3 taps from E in fp32 (a thread = 2 channels of one output column, walking its input rows) +
 //                 bias, ReLU6 -> bf16, written as the K-major swizzled A operand [64 pixels x 64 channels] of
-//     projection  wgmma m64n64k16 into register accumulators, 64-column blocks split between the warpgroups (Cout <=
-//                 256), accumulated over the chunks in ascending order.
+//     projection  wgmma m64n(Cout / 2)k16 into register accumulators, one half of the output columns per warpgroup
+//                 (Cout <= 256), accumulated over the chunks in ascending order.
 //   With two or more stages the chunks overlap: chunk c + 1's expansion MMAs are issued before chunk c's depthwise and
 //   run under it (they write only registers), and its epilogue refills E after chunk c's projection.  Two named
 //   barriers per chunk order E and the A operand between the consumer warpgroups; both retire their projection before
@@ -26,6 +27,8 @@
 // Rounding follows the layer-by-layer path: the expansion and the depthwise output are rounded to bf16, every sum is
 // fp32, in the same order for every element.
 #include "fused_block.cuh"
+
+#include <type_traits>
 
 #include "gemm_wgmma.cuh"
 #include "tma_pipeline.cuh"
@@ -139,7 +142,7 @@ __global__ void __launch_bounds__(pipe::kThreads, 1)
 fused_block_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_w1,
                    const __grid_constant__ CUtensorMap map_w2, const Args a) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  constexpr int HALO = halo(S), HPX = halo_px(S), HR = halo_rows(S), MB = HR / 64;
+  constexpr int HALO = halo(S), HPX = halo_px(S), HR = halo_rows(S);
   Ring ring(smem_raw, a.l.stage, a.l.stages, a.l.extra);
   uint8_t* own = ring.extra();
   uint8_t* xs = own + a.l.xs;
@@ -210,65 +213,114 @@ fused_block_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_const
   // cannot hold both, so there the expansion waits for chunk c's projection and the stage it frees.
   const bool ahead = a.l.stages > 1;
 
-  // How the warpgroups share the expansion: at stride 1 (2 m blocks) one m block each over all 64 columns, at stride 2
-  // (5 m blocks, which do not split evenly) every m block over one 32-column half each.
-  constexpr bool kSplitN = MB % 2 != 0;
-  constexpr int kEM = kSplitN ? MB : MB / 2, kEN = kSplitN ? 32 : 64;  // m blocks and columns per warpgroup
-  const int m0 = kSplitN ? 0 : wg, n0 = kSplitN ? 32 * wg : 0;        // first m block and column of this warpgroup
+  // The expansion runs transposed, E^T [64 channels x halo pixels] = W1 chunk . halo^T: the stage's W1 chunk (64
+  // K-major rows) is the A operand and the halo rows are B, so the halo pixels are the MMA's wide dimension.  The
+  // pixels, rounded up to whole 8-row atoms, split between the warpgroups as evenly as whole atoms allow: 152 + 144 at
+  // stride 2, 56 + 48 at stride 1.  Halo rows past HPX are stale and give accumulator columns that are never stored.
+  constexpr int kEN0 = ((HPX + 7) / 8 + 1) / 2 * 8;  // pixels of warpgroup 0
+  constexpr int kEN1 = (HPX + 7) / 8 * 8 - kEN0;     // pixels of warpgroup 1, from kEN0 on
+  // the projection: each warpgroup one half of the output columns, [wg half, (wg + 1) half)
+  const int half = a.cout_p / 2;
 
   // the first MMA of every expansion and of every tile's projection overwrites (scale_d = 0)
-  float acc1[kEM][kEN / 2];  // expansion: m block m0 + m, columns n0 .. n0 + kEN - 1 of the chunk
-  float acc2[2][32];         // projection column blocks nb = wg and wg + 2
+  float acc1[kEN0 / 2];  // expansion: channels 16 warp + lane / 4 (+ 8) of pixels p0 + 8 j + 2 quad (+ 1)
+  float acc2[kMaxCout / 4];  // projection: output columns wg half + 8 j + 2 quad (+ 1), j < half / 8
 #pragma unroll
-  for (int m = 0; m < kEM; ++m)
+  for (int i = 0; i < kEN0 / 2; ++i) acc1[i] = 0.f;
 #pragma unroll
-    for (int i = 0; i < kEN / 2; ++i) acc1[m][i] = 0.f;
-#pragma unroll
-  for (int j = 0; j < 2; ++j)
-#pragma unroll
-    for (int i = 0; i < 32; ++i) acc2[j][i] = 0.f;
+  for (int i = 0; i < kMaxCout / 4; ++i) acc2[i] = 0.f;
 
-  // acc1 = this warpgroup's halo rows . W1 chunk columns [n0, n0 + kEN)^T, issued and committed, not waited for
+  // acc1 = W1 chunk . this warpgroup's halo rows^T, issued and committed, not waited for
+  // (the width is chosen outside the K loop, so that each warpgroup's MMAs form one straight run ptxas can batch)
   auto expand_issue = [&](const uint8_t* stage) {
-    const uint32_t w1 = smem_u32(stage) + (uint32_t)(n0 * 128);
-    wgmma_fence();
-#pragma unroll
-    for (int m = 0; m < kEM; ++m)
+    const uint32_t w1 = smem_u32(stage), px = smem_u32(xs) + (uint32_t)(wg * kEN0 * 128);
+    auto issue = [&](auto width) {
       for (int kb = 0; kb < kbx; ++kb) {
-        const uint64_t da = make_smem_desc(smem_u32(xs + (kb * HR + (m0 + m) * 64) * 128));
-        const uint64_t db = make_smem_desc(w1 + (uint32_t)(kb * kChunk * 128));
+        const uint64_t da = make_smem_desc(w1 + (uint32_t)(kb * kChunk * 128));
+        const uint64_t db = make_smem_desc(px + (uint32_t)(kb * HR * 128));
         const int ksteps = min(4, (a.cin_p - kb * 64) / 16);
         for (int ks = 0; ks < ksteps; ++ks)
-          Wgmma<kEN>::mma(acc1[m], da + (uint64_t)(ks * 2), db + (uint64_t)(ks * 2), (kb | ks) ? 1u : 0u);
+          wgmma_into<decltype(width)::value>(acc1, da + (uint64_t)(ks * 2), db + (uint64_t)(ks * 2),
+                                             (kb | ks) ? 1u : 0u);
       }
+    };
+    wgmma_fence();
+    if (wg == 0) issue(std::integral_constant<int, kEN0>{});
+    else issue(std::integral_constant<int, kEN1>{});
     wgmma_commit();
   };
-  // E columns of this warpgroup = relu6(acc1 + b1), zero outside the image and past the chunk's channels.  The bias
-  // columns are read into registers before the first store into E (the compiler cannot move shared-memory loads above
-  // stores that may alias them), and the zero cases are selects, so each bf16 pair is a short branch-free chain.
-  auto expand_epilogue = [&](const uint8_t* stage, int nch, int gy0, int gx0) {
+  // Bit 2 j + k of this thread's mask: halo pixel p0 + 8 j + 2 quad + k of its warpgroup lies inside the image.  It
+  // depends on the tile only, so it is computed once per tile rather than in every chunk's epilogue.  The pixels'
+  // halo coordinates do not depend on the tile; the empty asm keeps the compiler from hoisting all 2 x kEN0 / 4 of
+  // them out of the tile loop, where they would not fit in the registers the chunk loop leaves.
+  auto inside_mask = [&](int gy0, int gx0) {
+    int p0 = wg * kEN0 + 2 * quad;
+    asm volatile("" : "+r"(p0));
+    uint64_t m = 0;
 #pragma unroll
-    for (int m = 0; m < kEM; ++m) reg_fence(acc1[m]);
-    const float* b1 = reinterpret_cast<const float*>(stage + a.l.dw) + 10 * kChunk;
-    float2 bias[kEN / 8];  // columns n0 + 8 j + 2 quad and the one after
+    for (int j = 0; j < kEN0 / 8; ++j)
 #pragma unroll
-    for (int j = 0; j < kEN / 8; ++j) bias[j] = *reinterpret_cast<const float2*>(b1 + n0 + 8 * j + 2 * quad);
-#pragma unroll
-    for (int m = 0; m < kEM; ++m)
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int p = (m0 + m) * 64 + warp * 16 + (lane >> 2) + 8 * h;
-        if (p >= HPX) continue;
+      for (int k = 0; k < 2; ++k) {
+        const int p = p0 + 8 * j + k;
         const int gy = gy0 + p / HALO, gx = gx0 + p % HALO;
-        const bool inside = gy >= 0 && gy < a.H && gx >= 0 && gx < a.W;
-#pragma unroll
-        for (int j = 0; j < kEN / 8; ++j) {
-          const bool keep = inside && n0 + 8 * j + 2 * quad < nch;
-          const float f0 = keep ? relu6f(acc1[m][4 * j + 2 * h] + bias[j].x) : 0.f;
-          const float f1 = keep ? relu6f(acc1[m][4 * j + 2 * h + 1] + bias[j].y) : 0.f;
-          *reinterpret_cast<__nv_bfloat162*>(e_own + e_off(p, n0 / 8 + j) + 2 * quad) = __floats2bfloat162_rn(f0, f1);
-        }
+        if (gy >= 0 && gy < a.H && gx >= 0 && gx < a.W) m |= 1ull << (2 * j + k);
       }
+    return m;
+  };
+  // E pixels of this warpgroup = relu6(acc1 + b1), zero outside the image and past the chunk's channels.  A thread's
+  // bf16 pair (channel r + 8 h, pixels 8 j + 2 quad, + 1) is one register of the 8 x 8 fragment (pixel group j,
+  // channel group 2 warp + h); stmatrix .trans writes the fragments back pixel-major, each pixel's 8 channels one
+  // 16-byte group at e_off, so E keeps the layout the depthwise reads.  The pixel groups past HPX's last whole atom
+  // (warpgroup 1's last one) store element by element, stopping at HPX.
+  auto expand_epilogue = [&](const uint8_t* stage, int nch, uint64_t inside) {
+    reg_fence(acc1);
+    const float* b1 = reinterpret_cast<const float*>(stage + a.l.dw) + 10 * kChunk;
+    const int r = 16 * warp + (lane >> 2);
+    const float bias[2] = {b1[r], b1[r + 8]};
+    // a channel past the chunk's stores zeros: its bits of the mask below are cleared
+    const uint32_t keep[2] = {r < nch ? ~0u : 0u, r + 8 < nch ? ~0u : 0u};
+    // The zero cases clear the bf16 halves of the packed pair (pixel 2 quad in the low half, the next in the high
+    // one): relu6f maps every input, NaN included, to a finite value, so masking after the conversion gives the same
+    // bits as selecting 0 before it.
+    auto pack = [&](int j, int h) {  // the fragment register of pixel group j, channel group 2 warp + h
+      const uint32_t bits = (uint32_t)(inside >> (2 * j));
+      const uint32_t mask = ((bits & 1u) * 0xffffu | (bits & 2u) * 0x7fff8000u) & keep[h];
+      const __nv_bfloat162 v = __floats2bfloat162_rn(relu6f(acc1[4 * j + 2 * h] + bias[h]),
+                                                     relu6f(acc1[4 * j + 2 * h + 1] + bias[h]));
+      return *reinterpret_cast<const uint32_t*>(&v) & mask;
+    };
+    auto store = [&](auto wgc) {
+      constexpr int P0 = decltype(wgc)::value * kEN0;
+      constexpr int NG = (decltype(wgc)::value ? kEN1 : kEN0) / 8;  // pixel groups of this warpgroup
+      constexpr int NFULL = (HPX - P0) / 8 < NG ? (HPX - P0) / 8 : NG;  // those entirely below HPX
+      // lane 8 i + k addresses row k of matrix i: pixel group j + i / 2, channel group 2 warp + i % 2
+      const int mi = lane >> 3;
+      const uint32_t e_base = smem_u32(e_own);
+#pragma unroll
+      for (int j = 0; j + 1 < NFULL; j += 2) {
+        const int p = P0 + 8 * (j + (mi >> 1)) + (lane & 7);
+        stmatrix_x4_trans(e_base + 2 * e_off(p, 2 * warp + (mi & 1)), pack(j, 0), pack(j, 1), pack(j + 1, 0),
+                          pack(j + 1, 1));
+      }
+      if (NFULL % 2) {
+        const int p = P0 + 8 * (NFULL - 1) + (lane & 7);
+        stmatrix_x2_trans(e_base + 2 * e_off(p, 2 * warp + (mi & 1)), pack(NFULL - 1, 0), pack(NFULL - 1, 1));
+      }
+#pragma unroll
+      for (int j = NFULL; j < NG; ++j)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const uint32_t v = pack(j, h);
+#pragma unroll
+          for (int k = 0; k < 2; ++k) {
+            const int p = P0 + 8 * j + 2 * quad + k;
+            if (p < HPX)
+              reinterpret_cast<uint16_t*>(e_own)[e_off(p, 2 * warp + h) + (lane >> 2)] = (uint16_t)(v >> (16 * k));
+          }
+        }
+    };
+    if (wg == 0) store(std::integral_constant<int, 0>{});
+    else store(std::integral_constant<int, 1>{});
   };
 
   PhaseClock clk;
@@ -277,6 +329,7 @@ fused_block_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_const
     const int b = tile / per_img, ty = (tile % per_img) / a.tiles_x, tx = tile % a.tiles_x;
     const int oy0 = ty * kTile, ox0 = tx * kTile;
     const int gy0 = oy0 * S - 1, gx0 = ox0 * S - 1;
+    const uint64_t inside = kExpand ? inside_mask(gy0, gx0) : 0;
     if (kExpand) {
       mbar_wait(xs_full, xs_phase);
       xs_phase ^= 1;
@@ -286,7 +339,7 @@ fused_block_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_const
       expand_issue(s0);
       wgmma_wait<0>();
       clk.lap(kExpandMma);
-      expand_epilogue(s0, min(kChunk, a.cmid_p), gy0, gx0);
+      expand_epilogue(s0, min(kChunk, a.cmid_p), inside);
       if (nchunks == 1) mbar_arrive(xs_empty);  // this thread's reads of the halo are complete
       clk.lap(kExpandEpi);
     }
@@ -364,16 +417,33 @@ fused_block_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_const
       named_bar_sync(kConsumerBar, pipe::kConsumerThreads);
       clk.lap(kBarrier);
 
-      // projection: acc2 += A2 [64 x nch] . W2_chunk [Cout x nch]^T
+      // projection: acc2 += A2 [64 x nch] . W2_chunk rows [wg half, (wg + 1) half)^T, one MMA of width half per k step
       wgmma_fence();
-      const uint64_t da = make_smem_desc(smem_u32(a2));
-#pragma unroll
-      for (int j = 0; j < 2; ++j) {
-        const int nb = wg + 2 * j;
-        if (nb < n2_blocks) {
-          const uint64_t db = make_smem_desc(smem_u32(sp) + a.l.w2 + (uint32_t)(nb * 64 * 128));
+      {
+        const uint64_t da = make_smem_desc(smem_u32(a2));
+        const uint64_t db = make_smem_desc(smem_u32(sp) + a.l.w2 + (uint32_t)(wg * half * 128));
+        auto project = [&](auto width) {
           for (int ks = 0; ks < nch / 16; ++ks)
-            Wgmma<64>::mma(acc2[j], da + (uint64_t)(ks * 2), db + (uint64_t)(ks * 2), (c0 | ks) ? 1u : 0u);
+            wgmma_into<decltype(width)::value>(acc2, da + (uint64_t)(ks * 2), db + (uint64_t)(ks * 2),
+                                               (c0 | ks) ? 1u : 0u);
+        };
+        switch (half) {  // cout_p is a multiple of 16 and at most kMaxCout (plan())
+          case 8: project(std::integral_constant<int, 8>{}); break;
+          case 16: project(std::integral_constant<int, 16>{}); break;
+          case 24: project(std::integral_constant<int, 24>{}); break;
+          case 32: project(std::integral_constant<int, 32>{}); break;
+          case 40: project(std::integral_constant<int, 40>{}); break;
+          case 48: project(std::integral_constant<int, 48>{}); break;
+          case 56: project(std::integral_constant<int, 56>{}); break;
+          case 64: project(std::integral_constant<int, 64>{}); break;
+          case 72: project(std::integral_constant<int, 72>{}); break;
+          case 80: project(std::integral_constant<int, 80>{}); break;
+          case 88: project(std::integral_constant<int, 88>{}); break;
+          case 96: project(std::integral_constant<int, 96>{}); break;
+          case 104: project(std::integral_constant<int, 104>{}); break;
+          case 112: project(std::integral_constant<int, 112>{}); break;
+          case 120: project(std::integral_constant<int, 120>{}); break;
+          case 128: project(std::integral_constant<int, 128>{}); break;
         }
       }
       wgmma_commit();
@@ -389,12 +459,11 @@ fused_block_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_const
       // Retires chunk c + 1's expansion too.  Waiting for it alone (wait_group 1) and running its epilogue under the
       // projection makes ptxas serialise the wgmmas (C7514), so the two retire together.
       wgmma_wait<0>();
-#pragma unroll
-      for (int j = 0; j < 2; ++j) reg_fence(acc2[j]);
+      reg_fence(acc2);
       if (!next || ahead) ring.release();
       clk.lap(kProjectMma);
       if (next) {
-        expand_epilogue(sn, min(kChunk, a.cmid_p - c0 - kChunk), gy0, gx0);
+        expand_epilogue(sn, min(kChunk, a.cmid_p - c0 - kChunk), inside);
         if (c + 2 == nchunks) mbar_arrive(xs_empty);  // this thread's reads of the halo are complete
         clk.lap(kExpandEpi);
       }
@@ -408,22 +477,17 @@ fused_block_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_const
       if (oy >= a.Ho || ox >= a.Wo) continue;
       const int64_t pix = ((int64_t)b * a.Ho + oy) * a.Wo + ox;
 #pragma unroll
-      for (int jb = 0; jb < 2; ++jb) {
-        const int nb = wg + 2 * jb;
-        if (nb >= n2_blocks) continue;
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const int n = nb * 64 + 8 * j + 2 * quad;
-          if (n >= a.cout_p) continue;
-          float f0 = acc2[jb][4 * j + 2 * h] + __ldg(&a.b2[n]);
-          float f1 = acc2[jb][4 * j + 2 * h + 1] + __ldg(&a.b2[n + 1]);
-          if (a.residual) {  // stride 1, cin_p == cout_p: the block input at the same pixel
-            const float2 r = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(a.X + pix * a.cin_p + n));
-            f0 += r.x;
-            f1 += r.y;
-          }
-          *reinterpret_cast<__nv_bfloat162*>(a.Y + pix * a.cout_p + n) = __floats2bfloat162_rn(f0, f1);
+      for (int j = 0; j < kMaxCout / 16; ++j) {
+        if (8 * j >= half) break;
+        const int n = wg * half + 8 * j + 2 * quad;
+        float f0 = acc2[4 * j + 2 * h] + __ldg(&a.b2[n]);
+        float f1 = acc2[4 * j + 2 * h + 1] + __ldg(&a.b2[n + 1]);
+        if (a.residual) {  // stride 1, cin_p == cout_p: the block input at the same pixel
+          const float2 r = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(a.X + pix * a.cin_p + n));
+          f0 += r.x;
+          f1 += r.y;
         }
+        *reinterpret_cast<__nv_bfloat162*>(a.Y + pix * a.cout_p + n) = __floats2bfloat162_rn(f0, f1);
       }
     }
     clk.lap(kEpilogue);

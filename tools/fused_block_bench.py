@@ -24,15 +24,16 @@ BLOCKS = [(501, 64, 144, None, 80, 1), (501, 64, 80, 432, 80, 2), (251, 32, 80, 
 
 
 def per_window(H, W, cin_p, cmid_p, cout_p, S):
-    """(issued MMA FLOP, compulsory HBM bytes) of one window: 8 x 8 output tiles, the halo rows padded to 64, the
-    expansion's K steps of 16 past cin_p skipped, the projection in 64-column blocks."""
+    """(issued MMA FLOP, compulsory HBM bytes) of one window: 8 x 8 output tiles, the expansion over the halo pixels
+    rounded up to 8-pixel atoms (its N) with the K steps of 16 past cin_p skipped, the projection over cout_p columns
+    (two halves of cout_p / 2)."""
     Ho, Wo = (H - 1) // S + 1, (W - 1) // S + 1
     tiles = math.ceil(Ho / 8) * math.ceil(Wo / 8)
-    hr = math.ceil(((7 * S + 3) ** 2) / 64) * 64
+    hp = math.ceil(((7 * S + 3) ** 2) / 8) * 8
     cm = cmid_p or cin_p
     chunks = math.ceil(cm / 64)
-    expand = 0 if cmid_p is None else 2 * hr * 64 * chunks * cin_p
-    project = 2 * 64 * math.ceil(cout_p / 64) * 64 * cm
+    expand = 0 if cmid_p is None else 2 * hp * 64 * chunks * cin_p
+    project = 2 * 64 * cout_p * cm
     return tiles * (expand + project), 2 * (H * W * cin_p + Ho * Wo * cout_p)
 
 
