@@ -92,6 +92,7 @@ SIGNATURES = {
     "am_knn_query_ex": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp]),
     "am_knn_filter_by_distance": (_i, [_vp, _vp, _i, _i, C.c_float, _i, _i, _vp]),
     "am_knn_pairwise": (_i, [_vp, _vp, _i, _vp]),
+    "am_knn_radius_walk": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _vp, _P(C.c_int32)]),
     "am_knn_get_vectors": (_i, [_vp, _vp, _i, _vp]),
     "am_knn_query_dev": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _vp]),
     "am_kmeans_fit": (_i, [_vp, _i64, _i, _i, _i, _i, _f, _u64, _vp, _vp, _vp, _P(_f), _P(_i)]),

@@ -862,6 +862,233 @@ filter_by_distance_kernel(const float* __restrict__ X, int64_t N, int d, int met
 }
 
 
+// ---------------------------------------------------------------- radius walk on device
+// voyager_manager.py:941-1367 (_execute_radius_walk) over the candidates _radius_walk_get_candidates (:842-938) leaves,
+// in one CTA.  The reference's steps and the state that restates each:
+//   * anchor distances (:927, get_direct_distance) in float64, one warp per candidate; the stable sort by that distance
+//     (:968) is a bitonic sort of (distance bits, input position) keys -- distances are >= 0 or +inf, so their bit
+//     patterns order like the values, and the position breaks ties the way a stable sort keeps them;
+//   * buckets of 50 in that order (:956, :970-974), walked one after the other until the playlist holds n songs (what
+//     the window-doubling loop at :1261-1281 amounts to);
+//   * the first song is sorted[0] (:1008-1013); its artist counts (:1041-1047) but not per bucket;
+//   * each bucket starts at its first unused candidate (:1091-1103; in bucket 0 that skips sorted[0]), accepted if it
+//     passes the artist rules and otherwise only dropped from the bucket (:1140-1163);
+//   * then greedily: score = 0.7 d(prev, cand) + 0.3 float32(d(anchor, cand)) (:1222), the first strict minimum in
+//     bucket order wins (:1223), prev is the last song APPENDED (:1174), and the bucket ends when no candidate passes;
+//   * the artist rules (:1120-1136, :1188-1211) apply when eliminate_duplicates and the cap is > 0: one song per artist
+//     per bucket, and an artist already in 2 buckets or at the cap is refused;
+//   * once the playlist holds n songs nothing later changes it (:1146, :1237, :1262), so the walk stops there;
+//   * _avoid_triple_adjacent (:1287-1318) on the final order.
+// Per-candidate state lives in global scratch (sort keys, per-artist counters, the playlist); only the distances from
+// the current song to the <= 50 candidates of the bucket are in shared memory.  Warp 0 keeps the books, every warp
+// computes distances.
+constexpr int kWalkThreads = 1024;
+constexpr int kWalkBucket = 50;    // BUCKET_SIZE, voyager_manager.py:956
+constexpr unsigned long long kWalkMissing = ~0ull;  // sort key of a candidate that is not in the index: after +inf
+
+__device__ __forceinline__ double walk_key_dist(unsigned long long k) { return __longlong_as_double((long long)k); }
+
+// artists[c] of input position c (-1: no artist); count / buckets / mark: per artist, the songs taken, the buckets it
+// has a song in, and the last bucket it took a song in
+__device__ __forceinline__ bool walk_artist_ok(int a, int bucket, int cap, const int* count, const int* buckets,
+                                               const int* mark) {
+  return a < 0 || !(mark[a] == bucket || buckets[a] >= 2 || count[a] >= cap);
+}
+
+__global__ void __launch_bounds__(kWalkThreads)
+radius_walk_kernel(const float* __restrict__ X, int64_t N, int d, int metric, const float* __restrict__ anchor,
+                   const int64_t* __restrict__ rows, const int32_t* __restrict__ artists, int n_cand, int n,
+                   int artist_rules, int cap, int64_t npad, unsigned long long* key, int* ord, int* count,
+                   int* buckets, int* mark, int* playlist, int32_t* __restrict__ out_pos,
+                   double* __restrict__ out_dist, int32_t* __restrict__ out_count) {
+  __shared__ double s_dprev[kWalkBucket];
+  __shared__ unsigned long long s_elig;  // candidates of the bucket that may be taken next
+  __shared__ int s_valid, s_len, s_prev_pos;  // valid candidates, playlist length, input position of the last song
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, warps = kWalkThreads / 32;
+  if (threadIdx.x == 0) s_valid = 0;
+  __syncthreads();
+
+  // ---- anchor distances and sort keys (padding sorts after every candidate)
+  for (int64_t i = warp; i < npad; i += warps) {
+    unsigned long long k = kWalkMissing;
+    const int64_t row = i < n_cand ? rows[i] : -1;
+    if (row >= 0 && row < N) {
+      k = (unsigned long long)__double_as_longlong(direct_distance(X + row * d, anchor, d, metric, lane));
+      if (lane == 0) atomicAdd(&s_valid, 1);
+    }
+    if (lane == 0) {
+      key[i] = k;
+      ord[i] = (int)i;
+    }
+  }
+  __syncthreads();
+  // ---- bitonic sort of (key, position) ascending
+  for (int64_t kk = 2; kk <= npad; kk <<= 1) {
+    for (int64_t j = kk >> 1; j > 0; j >>= 1) {
+      for (int64_t i = threadIdx.x; i < npad; i += kWalkThreads) {
+        const int64_t l = i ^ j;
+        if (l > i) {
+          const unsigned long long ki = key[i], kl = key[l];
+          const int oi = ord[i], ol = ord[l];
+          const bool i_after = ki > kl || (ki == kl && oi > ol);
+          if (i_after == ((i & kk) == 0)) {
+            key[i] = kl;
+            key[l] = ki;
+            ord[i] = ol;
+            ord[l] = oi;
+          }
+        }
+      }
+      __syncthreads();
+    }
+  }
+
+  // ---- the walk; sorted index s -> input position ord[s], anchor distance key[s]
+  const int m = s_valid;
+  if (threadIdx.x == 0) {
+    s_len = 0;
+    if (m > 0 && n > 0) {  // the first song (:1008-1013, :1041-1047)
+      playlist[0] = 0;
+      s_len = 1;
+      s_prev_pos = ord[0];
+      const int a = artists[ord[0]];
+      if (a >= 0) count[a] += 1;
+    }
+  }
+  __syncthreads();
+  for (int b = 0;; ++b) {
+    const bool go = (int64_t)b * kWalkBucket < m && s_len < n;  // read by every thread before warp 0 writes again
+    __syncthreads();
+    if (!go) break;
+    const int base = b * kWalkBucket, nb = min(kWalkBucket, m - base);
+    // warp 0's books for this bucket: candidates still available, playlist length, the artist of each lane's two
+    // candidates (j = lane, lane + 32)
+    unsigned long long avail = ((1ull << nb) - 1) & ~(b == 0 ? 1ull : 0ull);  // bucket 0 holds the first song
+    int len = 0, art[2] = {-1, -1};
+    // the candidates that may be taken next (a warp-wide ballot)
+    auto eligible = [&]() {
+      unsigned long long e = 0;
+      for (int h = 0; h < 2; ++h) {
+        const int j = lane + 32 * h;
+        const bool ok = j < nb && ((avail >> j) & 1) &&
+                        (!artist_rules || walk_artist_ok(art[h], b, cap, count, buckets, mark));
+        e |= (unsigned long long)__ballot_sync(0xffffffffu, ok) << (32 * h);
+      }
+      return e;
+    };
+    // take sorted index base + j (the bookkeeping of :1141-1161 / :1232-1253); lane 0 writes, the warp reads back
+    auto accept = [&](int j) {
+      avail &= ~(1ull << j);
+      if (lane == 0) {
+        if (len < n) {
+          playlist[len] = base + j;
+          s_prev_pos = ord[base + j];
+        }
+        const int a = artists[ord[base + j]];
+        if (a >= 0) {
+          count[a] += 1;
+          if (mark[a] != b) {
+            mark[a] = b;
+            buckets[a] += 1;
+          }
+        }
+      }
+      if (len < n) ++len;
+      __syncwarp();
+    };
+    if (warp == 0) {
+      len = s_len;
+      for (int h = 0; h < 2; ++h) {
+        const int j = lane + 32 * h;
+        if (j < nb) art[h] = artists[ord[base + j]];
+      }
+      if (avail) {  // the start (:1105-1163): the first available candidate, taken if the artist rules allow it
+        const int start = __ffsll((long long)avail) - 1;
+        if ((eligible() >> start) & 1) accept(start);
+        else avail &= ~(1ull << start);
+      }
+      const unsigned long long e = len < n ? eligible() : 0ull;
+      if (lane == 0) {
+        s_len = len;
+        s_elig = e;
+      }
+    }
+    // greedy steps (:1166-1253): every warp computes d(prev, cand) for the eligible candidates, warp 0 picks
+    for (;;) {
+      __syncthreads();  // s_elig / s_prev_pos published
+      const unsigned long long e = s_elig;
+      if (e == 0) break;
+      const float* prev = X + rows[s_prev_pos] * d;
+      for (int j = warp; j < nb; j += warps)
+        if ((e >> j) & 1) {
+          const double dist = direct_distance(X + rows[ord[base + j]] * d, prev, d, metric, lane);
+          if (lane == 0) s_dprev[j] = dist;
+        }
+      __syncthreads();  // distances ready
+      if (warp == 0) {
+        double best = INFINITY;  // a score must be strictly below +inf and below every earlier one (:1179, :1223)
+        int best_j = INT_MAX;
+        for (int h = 0; h < 2; ++h) {
+          const int j = lane + 32 * h;
+          if (j < nb && ((e >> j) & 1)) {
+            const double a32 = (double)(float)walk_key_dist(key[base + j]);  // the bucket's float32 array (:983)
+            const double score = __dadd_rn(__dmul_rn(0.7, s_dprev[j]), __dmul_rn(0.3, a32));
+            if (score < best) {
+              best = score;
+              best_j = j;
+            }
+          }
+        }
+        for (int o = 16; o > 0; o >>= 1) {  // the first minimum in bucket order
+          const double ob = __shfl_xor_sync(0xffffffffu, best, o);
+          const int oj = __shfl_xor_sync(0xffffffffu, best_j, o);
+          if (ob < best || (ob == best && oj < best_j)) {
+            best = ob;
+            best_j = oj;
+          }
+        }
+        unsigned long long next = 0;
+        if (best_j != INT_MAX) {
+          accept(best_j);
+          if (len < n) next = eligible();
+        }
+        if (lane == 0) {
+          s_len = len;
+          s_elig = next;
+        }
+      }
+    }
+  }
+
+  // ---- _avoid_triple_adjacent (:1287-1318) on the playlist, then the outputs
+  const int L = s_len;
+  if (threadIdx.x == 0) {
+    auto author = [&](int t) { return artists[ord[playlist[t]]]; };
+    int i = 0;
+    while (i <= L - 3) {
+      const int a1 = author(i);
+      if (a1 >= 0 && a1 == author(i + 1) && a1 == author(i + 2)) {
+        int j = i + 3;
+        while (j < L && author(j) == a1) ++j;
+        if (j < L) {  // swap the third with the first later song by another artist, then look at i again
+          const int t = playlist[i + 2];
+          playlist[i + 2] = playlist[j];
+          playlist[j] = t;
+          continue;
+        }
+      }
+      ++i;
+    }
+    *out_count = L;
+  }
+  __syncthreads();
+  for (int t = threadIdx.x; t < L; t += kWalkThreads) {
+    out_pos[t] = ord[playlist[t]];
+    out_dist[t] = walk_key_dist(key[playlist[t]]);
+  }
+}
+
+
 // ---------------------------------------------------------------- candidate post-processing helpers
 // Direct distances (get_direct_distance, voyager_manager.py:99-140) between all pairs of `n` stored rows: what the
 // radius walk (voyager_manager.py:1166-1258: score = 0.7 d(prev, cand) + 0.3 d(anchor, cand)) and the path logic
@@ -1347,5 +1574,73 @@ extern "C" int am_knn_get_vectors(const am_index* idx, const int64_t* ids, int n
   AM_LAUNCH(gather_rows_kernel, grid, 256, 0, st, idx->X.p, idx->N, idx->d, d_ids.p, n, d_out.p);
   AM_CUDA(cudaMemcpyAsync(out, d_out.p, (size_t)n * idx->d * 4, cudaMemcpyDeviceToHost, st));
   AM_CUDA(cudaStreamSynchronize(st));
+  return AM_OK;
+}
+
+extern "C" int am_knn_radius_walk(const am_index* idx, const float* anchor, const int64_t* rows, const int32_t* artists,
+                                  int n_cand, int n, int eliminate_duplicates, int max_songs_per_artist, int metric,
+                                  int32_t* out_pos, double* out_dist, int32_t* out_count) {
+  AM_CHECK(idx && anchor && out_count && (n_cand == 0 || (rows && artists)) && (n == 0 || (out_pos && out_dist)),
+           "am_knn_radius_walk: NULL argument");
+  AM_CHECK(n_cand >= 0 && n >= 0, "am_knn_radius_walk: negative size (n_cand = %d, n = %d)", n_cand, n);
+  AM_CHECK(metric == kMetricCos || metric == kMetricL2, "am_knn_radius_walk: metric %d is not 0 (angular) or 1 (euclidean)",
+           metric);
+  *out_count = 0;
+  if (n_cand == 0 || n == 0) return AM_OK;
+  int n_art = 0;
+  for (int i = 0; i < n_cand; ++i) {
+    AM_CHECK(artists[i] >= -1, "am_knn_radius_walk: artist id %d at %d is below -1", artists[i], i);
+    n_art = std::max(n_art, artists[i] + 1);
+  }
+  int64_t npad = 1;
+  while (npad < n_cand) npad <<= 1;
+  const int n_out = std::min(n, n_cand);
+  AM_TRY(ensure_init());
+  static thread_local Stream tst;  // re-entrant like am_knn_query
+  AM_TRY(tst.create());
+  cudaStream_t st = tst.s;
+  // inputs [anchor | rows | artists] go up in one copy, outputs [count | pos | dist] come back in one
+  const size_t b_anchor = Arena::pad((size_t)idx->d * 4), b_rows = Arena::pad((size_t)n_cand * 8),
+               b_art = Arena::pad((size_t)n_cand * 4);
+  const size_t b_cnt = Arena::pad(4), b_pos = Arena::pad((size_t)n_out * 4), b_dist = Arena::pad((size_t)n_out * 8);
+  const size_t b_in = b_anchor + b_rows + b_art, b_out = b_cnt + b_pos + b_dist;
+  const size_t b_scratch = Arena::pad((size_t)npad * 8) + Arena::pad((size_t)npad * 4) + 3 * Arena::pad((size_t)n_art * 4) +
+                           Arena::pad((size_t)n_out * 4);
+  static thread_local HostStage pin;
+  AM_TRY(pin.ensure(std::max(b_in, b_out)));
+  char* h = static_cast<char*>(pin.p);
+  std::memcpy(h, anchor, (size_t)idx->d * 4);
+  std::memcpy(h + b_anchor, rows, (size_t)n_cand * 8);
+  std::memcpy(h + b_anchor + b_rows, artists, (size_t)n_cand * 4);
+  Arena blk;
+  AM_TRY(blk.reserve(b_in + b_out + b_scratch, st));
+  float* d_anchor = blk.take<float>(idx->d);
+  int64_t* d_rows = blk.take<int64_t>(n_cand);
+  int32_t* d_art = blk.take<int32_t>(n_cand);
+  int32_t* d_cnt = blk.take<int32_t>(1);
+  int32_t* d_pos = blk.take<int32_t>(n_out);
+  double* d_dist = blk.take<double>(n_out);
+  unsigned long long* d_key = blk.take<unsigned long long>(npad);
+  int* d_ord = blk.take<int>(npad);
+  int* d_count = blk.take<int>(n_art);
+  int* d_buckets = blk.take<int>(n_art);
+  int* d_mark = blk.take<int>(n_art);
+  int* d_playlist = blk.take<int>(n_out);
+  AM_CUDA(cudaMemcpyAsync(d_anchor, h, b_in, cudaMemcpyHostToDevice, st));
+  if (n_art > 0) {
+    AM_CUDA(cudaMemsetAsync(d_count, 0, 2 * Arena::pad((size_t)n_art * 4), st));    // count, buckets
+    AM_CUDA(cudaMemsetAsync(d_mark, 0xff, (size_t)n_art * 4, st));                  // mark = -1: no bucket yet
+  }
+  const int rules = eliminate_duplicates && max_songs_per_artist > 0;
+  AM_LAUNCH(radius_walk_kernel, 1, kWalkThreads, 0, st, idx->X.p, idx->N, idx->d, metric, d_anchor, d_rows, d_art,
+            n_cand, n_out, rules, max_songs_per_artist, npad, d_key, d_ord, d_count, d_buckets, d_mark, d_playlist, d_pos,
+            d_dist, d_cnt);
+  AM_CUDA(cudaMemcpyAsync(h, d_cnt, b_out, cudaMemcpyDeviceToHost, st));
+  AM_CUDA(cudaStreamSynchronize(st));
+  int32_t cnt = 0;
+  std::memcpy(&cnt, h, 4);
+  std::memcpy(out_pos, h + b_cnt, (size_t)cnt * 4);
+  std::memcpy(out_dist, h + b_cnt + b_pos, (size_t)cnt * 8);
+  *out_count = cnt;
   return AM_OK;
 }

@@ -12,8 +12,11 @@ get_clustering_model).  tests/test_reference_shims.py applies exactly this to th
 """
 from __future__ import annotations
 
+import logging
 import os
 import sys
+
+logger = logging.getLogger(__name__)
 
 CLAP_NAMES = ("compute_mel_spectrogram", "analyze_audio_file", "initialize_clap_audio_model", "get_clap_audio_model",
               "unload_clap_audio_only", "unload_clap_model", "is_clap_model_loaded", "is_clap_audio_loaded")
@@ -47,12 +50,79 @@ def make_filter_by_distance(vm):
     return _filter_by_distance_b200
 
 
+RADIUS_WALK_NAMES = ("_radius_walk_get_candidates", "_execute_radius_walk")
+
+
+def make_radius_walk(vm):
+    """Replacements for voyager_manager._radius_walk_get_candidates (tasks/voyager_manager.py:842-938) and
+    _execute_radius_walk (:941-1367), patched as a pair: find_nearest_neighbors_by_id (:1469-1487) is their only
+    caller.  The candidate step keeps the reference's three filters and their fallbacks but no longer fetches one vector
+    per candidate (each get_vector is a device-to-host copy over the shim) or computes anchor distances on the host: it
+    hands on the candidates' index ids, and the walk runs anchor distances, sort, bucketed greedy walk, artist rules
+    and the triple-adjacency pass in one device call (am_knn_radius_walk).  Everything is looked up on `vm` at call
+    time, as the reference's own module globals are."""
+
+    def _radius_walk_get_candidates_b200(target_item_id, anchor_vector, initial_results, db_conn,
+                                         original_song_details, eliminate_duplicates, mood_similarity=None):
+        from app_helper import get_score_data_by_ids
+
+        if not initial_results:
+            return []
+        try:
+            temp = vm._filter_by_distance([{"item_id": target_item_id, "distance": 0.0}] + initial_results, db_conn)
+            results = [s for s in temp if s["item_id"] != target_item_id]
+        except Exception:
+            logger.exception("Radius walk: distance-based pre-filter failed, continuing with original candidate set.")
+            results = initial_results
+        try:
+            unique = vm._deduplicate_and_filter_neighbors(results, db_conn, original_song_details)
+        except Exception:
+            logger.exception("Radius walk: name-based dedupe failed, continuing without it.")
+            unique = results
+        try:
+            if vm.MOOD_SIMILARITY_ENABLE if mood_similarity is None else mood_similarity:
+                unique = vm._filter_by_mood_similarity(unique, target_item_id, db_conn)
+        except Exception:
+            logger.exception("Radius walk: mood-based pre-filter failed, continuing without it.")
+        if not unique:
+            return []
+        try:
+            details = {d["item_id"]: d for d in get_score_data_by_ids([r["item_id"] for r in unique])}
+        except Exception:
+            details = {}
+        out = []
+        for song in unique:
+            row = vm.reverse_id_map.get(song["item_id"])
+            if row is None:   # _get_cached_vector returns None: the reference drops the candidate
+                continue
+            info = details.get(song["item_id"], {})
+            out.append({"item_id": song["item_id"], "row": row, "title": info.get("title"),
+                        "author": info.get("author")})
+        return out
+
+    def _execute_radius_walk_b200(target_item_id, n, candidate_data, original_song_details=None,
+                                  eliminate_duplicates=False):
+        if not candidate_data:
+            return []
+        anchor = vm._get_cached_vector(target_item_id)
+        if anchor is None:
+            raise KeyError(f"radius walk: anchor item {target_item_id!r} is not in the loaded index")
+        artist_ids = {}
+        artists = [artist_ids.setdefault(c["author"], len(artist_ids)) if c.get("author") else -1
+                   for c in candidate_data]
+        pos, dist = vm.voyager_index.radius_walk(anchor, [c["row"] for c in candidate_data], artists, n,
+                                                 eliminate_duplicates, vm.MAX_SONGS_PER_ARTIST, vm.VOYAGER_METRIC)
+        return [{"item_id": candidate_data[p]["item_id"], "distance": float(d)} for p, d in zip(pos, dist)]
+
+    return _radius_walk_get_candidates_b200, _execute_radius_walk_b200
+
+
 METRIC_NAMES = ("silhouette_score", "davies_bouldin_score", "calinski_harabasz_score")
 
 
 def apply(clap=None, voyager_manager=None, clustering=None, allow_sklearn_fallback: bool = True,
           clustering_helper=None, song_alchemy=None, app_map=None, artist_gmm_manager=None,
-          gaussian_mixture=None) -> None:
+          gaussian_mixture=None, radius_walk=None) -> None:
     """clap / voyager_manager / clustering / clustering_helper: the reference's already imported tasks.* modules (pass
     only the ones to patch).  allow_sklearn_fallback keeps the reference's contract that a failing GPU k-means silently
     falls back to scikit-learn (tasks/clustering_gpu.py:130-148); this repository's own tests run with it off so a
@@ -66,7 +136,9 @@ def apply(clap=None, voyager_manager=None, clustering=None, allow_sklearn_fallba
     when it is imported, so install_voyager_shim() must come before `import tasks.artist_gmm_manager` and before
     `import tasks.analysis`, which imports it.  gaussian_mixture (the reference's tasks.clustering_gpu again) gets the
     GPU GPUGaussianMixture; get_clustering_model looks the class up at call time (:385).  clustering= alone leaves
-    that class to the reference."""
+    that class to the reference.  radius_walk (the reference's tasks.voyager_manager again) gets the device radius
+    walk: _radius_walk_get_candidates and _execute_radius_walk are replaced together (make_radius_walk);
+    voyager_manager= alone leaves the walk to the reference."""
     if clap is not None:
         from . import clap_analyzer as b200_clap
 
@@ -74,6 +146,9 @@ def apply(clap=None, voyager_manager=None, clustering=None, allow_sklearn_fallba
             setattr(clap, name, getattr(b200_clap, name))
     if voyager_manager is not None:
         voyager_manager._filter_by_distance = make_filter_by_distance(voyager_manager)
+    if radius_walk is not None:
+        for name, fn in zip(RADIUS_WALK_NAMES, make_radius_walk(radius_walk)):
+            setattr(radius_walk, name, fn)
     if clustering is not None:
         from . import clustering_gpu as b200_cg
 

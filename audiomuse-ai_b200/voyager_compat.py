@@ -277,6 +277,35 @@ class Index:
         keep = keep.astype(bool)
         return keep[0] if single else keep
 
+    # ------------------------------------------------------------------ radius walk (voyager_manager.py:941-1367)
+    def radius_walk(self, anchor, ids, artists, n: int, eliminate_duplicates: bool, max_songs_per_artist,
+                    metric: str):
+        """The reference's _execute_radius_walk over the stored vectors of `ids` (the candidates in the order the
+        candidate filters leave them; ids not in the index are dropped, as a missing vector is), in one device call.
+        artists: one int per candidate, a dense id per distinct truthy author and -1 for a falsy one.
+        max_songs_per_artist: config.MAX_SONGS_PER_ARTIST (None or <= 0 disables the artist rules); metric:
+        config.VOYAGER_METRIC ('angular' -> 1 - cos, anything else -> euclidean, as get_direct_distance reads it).
+        Returns (positions in `ids` in walk order, their float64 anchor distances)."""
+        a = np.ascontiguousarray(anchor, dtype=np.float32).reshape(-1)
+        if a.shape[0] != self.num_dimensions:
+            raise ValueError(f"anchor must have dimension {self.num_dimensions}, got {a.shape}")
+        rows = np.array([self._lookup(int(i)) for i in ids], dtype=np.int64)
+        art = np.ascontiguousarray(artists, dtype=np.int32)
+        if art.shape != rows.shape:
+            raise ValueError("ids and artists differ in length")
+        n = max(0, int(n))
+        cap = 0 if max_songs_per_artist is None else int(max_songs_per_artist)
+        pos = np.empty(max(n, 1), dtype=np.int32)
+        dist = np.empty(max(n, 1), dtype=np.float64)
+        count = C.c_int32(0)
+        if len(rows) and n:
+            h = self._ensure_built()
+            _lib.check(_lib.load().am_knn_radius_walk(h, _lib.ptr(a), _lib.ptr(rows), _lib.ptr(art), len(rows), n,
+                                                      int(bool(eliminate_duplicates)), cap,
+                                                      0 if metric == "angular" else 1, _lib.ptr(pos), _lib.ptr(dist),
+                                                      C.byref(count)))
+        return pos[:count.value].copy(), dist[:count.value].copy()
+
     # ------------------------------------------------------------------ persistence
     def as_bytes(self) -> bytes:
         with self._mu:

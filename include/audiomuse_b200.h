@@ -220,6 +220,19 @@ AM_API int am_knn_filter_by_distance(const am_index* idx, const int64_t* ids, in
  * the n stored rows `ids`: out f32[n, n], symmetric; +inf where a row id is outside [0, N).  Serves the radius
  * walk / path scoring (voyager_manager.py:1166-1258) without per-candidate get_vector round trips.  n <= 8192. */
 AM_API int am_knn_pairwise(const am_index* idx, const int64_t* ids, int n, float* out);
+/* The similar-tracks radius walk, voyager_manager.py:941-1367 (_execute_radius_walk), in one call: anchor f32[d];
+ * rows i64[n_cand] the candidates' stored rows in the order _radius_walk_get_candidates (:842-938) leaves them (-1 or
+ * any row outside [0, N): not in the index, dropped like a missing vector at :920-921); artists i32[n_cand] a dense id
+ * per distinct truthy author, -1 for a falsy one.  Sorts by the anchor distance (stable, :968), walks buckets of 50
+ * greedily on 0.7 d(prev) + 0.3 d(anchor) (:1166-1253) under the artist rules (one per artist per bucket, at most two
+ * buckets below the cap, the cap itself; only when eliminate_duplicates and max_songs_per_artist > 0, :1120-1136),
+ * stops at n songs and applies _avoid_triple_adjacent (:1287-1318).  metric: config.VOYAGER_METRIC as
+ * get_direct_distance reads it (:138-142), 0 angular (1 - cos) or 1 euclidean (||a - b||), from the stored rows in
+ * float64 whatever the index space.  out_pos i32[n] receives positions in `rows` in walk order, out_dist f64[n] their
+ * anchor distances, *out_count how many were written (<= n).  Re-entrant. */
+AM_API int am_knn_radius_walk(const am_index* idx, const float* anchor, const int64_t* rows, const int32_t* artists,
+                              int n_cand, int n, int eliminate_duplicates, int max_songs_per_artist, int metric,
+                              int32_t* out_pos, double* out_dist, int32_t* out_count);
 /* n stored rows in one device gather + one copy: out f32[n, d] */
 AM_API int am_knn_get_vectors(const am_index* idx, const int64_t* ids, int n, float* out);
 AM_API int am_knn_query_dev(const am_index* idx, const float* Q_dev, int nq, int k, int mode,
