@@ -52,20 +52,19 @@ def check_gpu_available() -> bool:
 
 
 def kmeans_fit(X, k, n_init=10, max_iter=300, tol=1e-4, seed=0, init_centers=None):
-    """-> (centers f32[k,d], labels i32[N], inertia, n_iter) via am_kmeans_fit."""
-    lib = _lib.load()
-    X = np.ascontiguousarray(X, dtype=np.float32)
-    if X.ndim != 2:
-        raise ValueError("X must be [N, d]")
+    """-> (centers f32[k,d], labels i32[N], inertia, n_iter) via am_kmeans_fit.  X and init_centers are validated as
+    scikit-learn does (ValueError for another rank, NaN or inf) before any device work."""
+    X = _finite_f32(X)
     N, d = X.shape
+    init = None
+    if init_centers is not None:
+        init = _finite_f32(init_centers)
+        if init.shape != (k, d):
+            raise ValueError(f"init_centers must be ({k}, {d})")
+    lib = _lib.load()
     centers = np.empty((k, d), dtype=np.float32)
     labels = np.empty((N,), dtype=np.int32)
     inertia, n_iter = C.c_float(0), C.c_int(0)
-    init = None
-    if init_centers is not None:
-        init = np.ascontiguousarray(init_centers, dtype=np.float32)
-        if init.shape != (k, d):
-            raise ValueError(f"init_centers must be ({k}, {d})")
     _lib.check(lib.am_kmeans_fit(_lib.ptr(X), N, d, int(k), int(n_init), int(max_iter), float(tol),
                                  int(seed) & 0xFFFFFFFFFFFFFFFF, None if init is None else _lib.ptr(init),
                                  _lib.ptr(centers), _lib.ptr(labels), C.byref(inertia), C.byref(n_iter)))

@@ -88,15 +88,17 @@ accumulate_kernel(const float* __restrict__ X, int64_t N, int d, const int32_t* 
   }
 }
 
-// C_new = sums / counts (empty clusters keep their centre); shift2 += ||C_new - C||^2
+// C_new = sums / counts; shift2 += ||C_new - C||^2.  A cluster that is still empty takes the new centre of cluster
+// `big` (sklearn's _average_centers: the first largest cluster), or keeps its centre when big < 0.
 __global__ void update_centers_kernel(const float* __restrict__ sums, const float* __restrict__ counts, int k,
-                                      int d, float* __restrict__ C, double* __restrict__ shift2) {
+                                      int d, int big, float* __restrict__ C, double* __restrict__ shift2) {
   const int j = blockIdx.x;
-  const float cnt = counts[j];
+  const int src = counts[j] > 0.f || big < 0 ? j : big;
+  const float cnt = counts[src];
   double local = 0.0;
   for (int i = threadIdx.x; i < d; i += blockDim.x) {
     const float old = C[(int64_t)j * d + i];
-    const float nw = cnt > 0.f ? sums[(int64_t)j * d + i] / cnt : old;
+    const float nw = cnt > 0.f ? sums[(int64_t)src * d + i] / cnt : old;
     C[(int64_t)j * d + i] = nw;
     const double df = (double)nw - (double)old;
     local += df * df;
@@ -129,7 +131,14 @@ __global__ void relocate_empty_kernel(const float* __restrict__ X, int d, const 
   }
 }
 
-// per-feature variance of X, summed (for sklearn's tol scaling): out[0] += sum_j var_j
+// X[i, :] -= mu (sign < 0) or += mu (sign > 0) for the N rows of X [N, d]
+__global__ void shift_rows_kernel(float* __restrict__ X, int64_t N, int d, const float* __restrict__ mu, int sign) {
+  const int64_t n = N * d;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
+    X[i] = sign < 0 ? X[i] - mu[i % d] : X[i] + mu[i % d];
+}
+
+// per-feature sums of X and X^2 in float64 (column means and sklearn's tol scaling)
 __global__ void column_moments_kernel(const float* __restrict__ X, int64_t N, int d, double* __restrict__ s1,
                                       double* __restrict__ s2) {
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
@@ -346,8 +355,9 @@ extern "C" int am_kmeans_plan_step(am_kmeans_plan* p, const float* centers_dev, 
   return AM_OK;  // stream-ordered: no synchronisation
 }
 
-// sklearn: tol_ = mean(var(X, axis=0)) * tol
-static int scaled_tolerance(const float* X, int64_t N, int d, float tol, cudaStream_t st, double* tol_abs) {
+// sklearn: tol_ = mean(var(X, axis=0)) * tol; mean[d] = the column means of X (rounded to float32)
+static int scaled_tolerance(const float* X, int64_t N, int d, float tol, cudaStream_t st, double* tol_abs,
+                            std::vector<float>& mean) {
   DevBuf<double> mom;
   AM_TRY(mom.alloc((size_t)2 * d));
   AM_CUDA(cudaMemsetAsync(mom.p, 0, (size_t)2 * d * 8, st));
@@ -357,9 +367,11 @@ static int scaled_tolerance(const float* X, int64_t N, int d, float tol, cudaStr
   AM_CUDA(cudaMemcpyAsync(hm.data(), mom.p, hm.size() * 8, cudaMemcpyDeviceToHost, st));
   AM_CUDA(cudaStreamSynchronize(st));
   double var_mean = 0.0;
+  mean.resize((size_t)d);
   for (int c = 0; c < d; ++c) {
     const double mu = hm[c] / N;
     var_mean += hm[d + c] / N - mu * mu;
+    mean[(size_t)c] = (float)mu;
   }
   *tol_abs = var_mean / d * tol;
   return AM_OK;
@@ -441,10 +453,17 @@ static int lloyd(am_kmeans_plan& step, int max_iter, double tol_abs, float* C, i
     std::vector<int32_t> empty;
     for (int j = 0; j < k; ++j)
       if (hcounts[j] == 0.f) empty.push_back(j);
-    if (!empty.empty() && (int64_t)empty.size() < N) {
+    int big = -1;
+    if (!empty.empty()) {
       hdist.resize((size_t)N);
       AM_CUDA(cudaMemcpyAsync(hdist.data(), dist, (size_t)N * 4, cudaMemcpyDeviceToHost, st));
       AM_CUDA(cudaStreamSynchronize(st));
+    }
+    // as sklearn: with every row on its centre (more clusters than distinct rows) relocation is pointless, and the
+    // empty clusters move to the first largest cluster's centre instead
+    if (!empty.empty() && *std::max_element(hdist.begin(), hdist.end()) == 0.f)
+      big = (int)(std::max_element(hcounts.begin(), hcounts.end()) - hcounts.begin());
+    else if (!empty.empty()) {
       std::vector<int64_t> order((size_t)N);
       for (int64_t i = 0; i < N; ++i) order[(size_t)i] = i;
       std::partial_sort(order.begin(), order.begin() + (int64_t)empty.size(), order.end(), [&](int64_t a, int64_t b) {
@@ -459,7 +478,7 @@ static int lloyd(am_kmeans_plan& step, int max_iter, double tol_abs, float* C, i
       AM_CUDA(cudaStreamSynchronize(st));  // far_dev / empty_dev are reused next time
     }
     AM_CUDA(cudaMemsetAsync(shift2_dev, 0, 8, st));
-    AM_LAUNCH(update_centers_kernel, k, 128, 0, st, sums, counts, k, d, C, shift2_dev);
+    AM_LAUNCH(update_centers_kernel, k, 128, 0, st, sums, counts, k, d, big, C, shift2_dev);
     double shift2 = 0.0;
     AM_CUDA(cudaMemcpyAsync(&shift2, shift2_dev, 8, cudaMemcpyDeviceToHost, st));
     AM_CUDA(cudaStreamSynchronize(st));
@@ -491,10 +510,18 @@ extern "C" int am_kmeans_fit(const float* X, int64_t N, int d, int k, int n_init
   AM_TRY(dBestL.alloc(N));
   AM_TRY(scal.alloc(2));  // [0] inertia, [1] shift2
   AM_CUDA(cudaMemcpyAsync(dX.p, X, (size_t)N * d * 4, cudaMemcpyHostToDevice, st.s));
+  double tol_abs = 0.0;
+  std::vector<float> hmean;
+  AM_TRY(scaled_tolerance(dX.p, N, d, tol, st.s, &tol_abs, hmean));
+  // as sklearn's KMeans.fit: Lloyd runs on the rows minus their column means, whose fp32 distances then do not lose
+  // ||mean||^2 to cancellation (seeding, tolerance and inertia do not change under the shift)
+  DevBuf<float> dmean;
+  AM_TRY(dmean.alloc((size_t)d));
+  AM_CUDA(cudaMemcpyAsync(dmean.p, hmean.data(), (size_t)d * 4, cudaMemcpyHostToDevice, st.s));
+  const auto shift_grid = [](int64_t n) { return (int)std::max<int64_t>(1, std::min<int64_t>((n + 255) / 256, (int64_t)sm_count() * 8)); };
+  AM_LAUNCH(shift_rows_kernel, shift_grid((int64_t)N * d), 256, 0, st.s, dX.p, N, d, dmean.p, -1);
   am_kmeans_plan step{dX.p, N, d, k};
   AM_TRY(step.create(kmeans_use_tensor_cores(N, d, k, KMeansUse::kFit), st.s));
-  double tol_abs = 0.0;
-  AM_TRY(scaled_tolerance(dX.p, N, d, tol, st.s, &tol_abs));
 
   SplitMix rng{seed ^ 0x5851f42d4c957f2dull};
   const int64_t nblk = (N + 1023) / 1024;
@@ -507,8 +534,10 @@ extern "C" int am_kmeans_fit(const float* X, int64_t N, int d, int k, int n_init
   double best_inertia = INFINITY;
   int best_iters = 0;
   for (int run = 0; run < (init_centers ? 1 : n_init); ++run) {
-    if (init_centers) AM_CUDA(cudaMemcpyAsync(dC.p, init_centers, (size_t)k * d * 4, cudaMemcpyHostToDevice, st.s));
-    else AM_TRY(kmeanspp_seed(dX.p, N, d, k, rng, dC.p, mind2.p, bsum.p, cand.p, bpot.p, st.s));
+    if (init_centers) {
+      AM_CUDA(cudaMemcpyAsync(dC.p, init_centers, (size_t)k * d * 4, cudaMemcpyHostToDevice, st.s));
+      AM_LAUNCH(shift_rows_kernel, shift_grid((int64_t)k * d), 256, 0, st.s, dC.p, (int64_t)k, d, dmean.p, -1);
+    } else AM_TRY(kmeanspp_seed(dX.p, N, d, k, rng, dC.p, mind2.p, bsum.p, cand.p, bpot.p, st.s));
     int it = 0;
     AM_TRY(lloyd(step, max_iter, tol_abs, dC.p, dL.p, sums.p, counts.p, dist.p, scal.p + 1, st.s, &it));
     // final E-step: labels and inertia consistent with the returned centres
@@ -523,6 +552,7 @@ extern "C" int am_kmeans_fit(const float* X, int64_t N, int d, int k, int n_init
       AM_CUDA(cudaMemcpyAsync(dBestL.p, dL.p, (size_t)N * 4, cudaMemcpyDeviceToDevice, st.s));
     }
   }
+  AM_LAUNCH(shift_rows_kernel, shift_grid((int64_t)k * d), 256, 0, st.s, dBestC.p, (int64_t)k, d, dmean.p, 1);
   AM_CUDA(cudaMemcpyAsync(centers, dBestC.p, (size_t)k * d * 4, cudaMemcpyDeviceToHost, st.s));
   AM_CUDA(cudaMemcpyAsync(labels, dBestL.p, (size_t)N * 4, cudaMemcpyDeviceToHost, st.s));
   AM_CUDA(cudaStreamSynchronize(st.s));

@@ -179,7 +179,9 @@ def _relocate_empty_clusters(x_local, labels, centers, sums, counts):
 
 class KMeansPlan:
     """am_kmeans_plan over this rank's rows (torch.cuda f32[n_local, d]): the split-bf16 copy is built once, every
-    step is one tensor-core assignment pass + one partial-sum pass, stream-ordered on torch's current stream."""
+    step is one tensor-core assignment pass + one partial-sum pass, stream-ordered on torch's current stream.
+    The rows are expected centred (column means near 0): both steps decide on fp32 ||c||^2 - 2 x.c, whose
+    cancellation grows with ||x||^2.  am_kmeans_fit centres its copy of the rows itself."""
 
     def __init__(self, x_local, k: int):
         import ctypes as C
@@ -235,7 +237,7 @@ def kmeans_lloyd_sharded(x_local, centers, max_iter=300, tol=1e-4, timing=None):
     the [k, d] sums and [k] counts (the only collective; + one scalar for the inertia at the end).
     tol=None runs exactly max_iter iterations without the convergence read-back (timing runs).
     `timing`, when a dict, receives {"assign_ms", "allreduce_ms"} device times summed over the iterations.
-    Returns (centers, labels_local, inertia, n_iter)."""
+    The rows are expected centred, as for KMeansPlan.  Returns (centers, labels_local, inertia, n_iter)."""
     import torch
 
     n_local, d = x_local.shape

@@ -79,12 +79,13 @@ def test_assign_dev_partial_sums_match_numpy():
     _lib.check(lib.am_kmeans_assign_dev(xd.data_ptr(), 5000, 96, cd.data_ptr(), 8, lab.data_ptr(), sums.data_ptr(),
                                         cnt.data_ptr(), inert.data_ptr(), C.c_void_p(torch.cuda.current_stream().cuda_stream)))
     torch.cuda.synchronize()
-    want_lab, want_inertia = okm.assign(x, centers)
-    np.testing.assert_array_equal(lab.cpu().numpy(), want_lab)
-    for j in range(8):
-        np.testing.assert_allclose(sums[j].cpu().numpy(), x[want_lab == j].sum(0), rtol=1e-4, atol=1e-3)
-        assert int(cnt[j].item()) == int((want_lab == j).sum())
-    assert abs(float(inert.item()) - want_inertia) <= 1e-3 * want_inertia
+    got = lab.cpu().numpy()
+    assert okm.accept(x, centers, got).all()
+    S, n = okm.sums_exact(x, got, 8)
+    np.testing.assert_array_equal(cnt.cpu().numpy(), n.astype(np.float32))
+    assert (np.abs(sums.cpu().numpy() - S) <= okm.sums_bound(x, got, 8)).all()
+    tot, bound = okm.inertia_bound(x, centers, got, tensor_cores=False)
+    assert abs(float(inert.item()) - tot) <= bound
 
 
 def test_sharded_lloyd_single_rank_matches_fit():
@@ -123,8 +124,7 @@ def test_config4_scale_properties():
     c5, l5, i5, it = cg.kmeans_fit(x, 128, init_centers=init, max_iter=5)
     assert i5 <= i1 * (1 + 1e-6) and it <= 5
     sub = rng.choice(len(x), 4000, replace=False)
-    want_lab, _ = okm.assign(x[sub], c5)
-    assert (l5[sub] == want_lab).mean() > 0.999
+    assert okm.accept(x[sub], c5, l5[sub]).all()
     _, inertia_chk = okm.assign(x[sub], c5)
     d2 = ((x[sub].astype(np.float64) - c5[l5[sub]].astype(np.float64)) ** 2).sum()
     assert abs(d2 - inertia_chk) <= 1e-3 * inertia_chk
@@ -180,8 +180,7 @@ def test_tensor_core_step_equals_debug_exact_step(n, d, k, kind):
     np.testing.assert_allclose(out["tc"][1], out["simt"][1], rtol=2e-5, atol=2e-3)
     assert abs(out["tc"][3] - out["simt"][3]) <= 1e-5 * out["simt"][3]
     np.testing.assert_allclose(out["tc"][4], out["simt"][4], rtol=0, atol=2e-3 * max(1.0, float(out["simt"][4].max())))
-    want_lab, want_inertia = okm.assign(x[:4000], centers)
-    assert (out["tc"][0][:4000] == want_lab).mean() > 0.999       # float64 oracle (ties aside)
+    assert okm.accept(x, centers, out["tc"][0]).all()              # float64 oracle, every row
 
 
 def test_plan_path_follows_the_shape():
