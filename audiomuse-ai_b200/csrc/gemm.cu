@@ -5,8 +5,10 @@
 //                 and the B tile [BN x 64] (bf16, 128-byte swizzle) into a shared-memory ring of up to 4 stages;
 //   warpgroups 1, 2   consumers, rows [0, 64) and [64, 128) of the tile: wgmma.mma_async m64nBNk16 straight from
 //                 the swizzled tiles into fp32 register accumulators, then the epilogue from registers:
-//                 alpha / bias / ReLU6 / residual -> bf16 or fp32 (+ the k-NN chunk maxima); a bf16 tile goes through
-//                 shared memory so that global stores are whole 16-byte chunks of consecutive columns.
+//                 alpha / bias / ReLU6 / residual -> bf16 or fp32 (+ the k-NN chunk maxima).  A bf16 tile is staged
+//                 in shared memory and leaves through TMA stores (cp.async.bulk.tensor ... bulk_group) that one
+//                 thread of the warpgroup issues; the warpgroup goes straight on to the next tile's MMAs and waits
+//                 for the stores to have read the staging tile only before it writes that tile again.
 // The ring and its barriers are tma_pipeline.cuh's.  While the consumers run an epilogue the producer is already
 // filling the ring with the next tile's first K blocks.
 #include "gemm_wgmma.cuh"
@@ -38,23 +40,40 @@ struct KernelArgs {
   void* D;
   int64_t ldd;
   int d_is_f32;
-  int d_vec;      // D rows allow 2-element vector stores (even ldd, aligned base)
+  int d_vec;      // fp32 D rows allow 2-element vector stores (even ldd, aligned base)
   float alpha;
   const float* bias;
   const float* col_sub;
   int act;
-  const __nv_bfloat16* residual;
+  const __nv_bfloat16* residual;  // bf16 D only; ld_res even and a 4-byte aligned base (2-element loads)
   int64_t ld_res;
-  int res_vec;    // residual rows allow 2-element vector loads
   float* chunk_max;  // k-NN: per-32-column maxima beside D (see Epilogue::chunk_max)
   int64_t ld_cm;
   int stages;     // smem ring depth
-  int staged;     // bf16 D leaves through a shared-memory tile as whole 16-byte row chunks (coalesced)
 };
 
-// per consumer warpgroup: 64 rows of the tile, rows padded by 16 bytes so the fragment writes spread over the banks
+// The bf16 staging tile of one consumer warpgroup: its 64 rows x BN columns as the boxes of the TMA stores, BN / 64
+// boxes of 64 columns (128-byte rows, SWIZZLE_128B), then, when BN % 64 != 0, one narrower box of the last BN % 64
+// columns through a second tensor map: 32- and 64-byte rows with the matching SWIZZLE_32B / _64B, 96-byte rows
+// unswizzled.  Every box starts 1024-byte aligned.  The swizzles spread a warp's fragment stores (8 rows x 4 column
+// pairs) over all 32 banks; only the 96-byte box has two-way conflicts.
 template <int BN>
-constexpr int stage_pitch() { return BN * 2 + 16; }
+constexpr int stage_bytes() { return 64 * BN * 2; }
+constexpr int tail_swizzle_bytes(int tail_cols) { return tail_cols == 16 ? 32 : tail_cols == 32 ? 64 : 0; }
+
+// byte offset in the staging tile of the bf16 pair at (row r, even column c)
+template <int BN>
+__device__ __forceinline__ uint32_t stage_offset(int r, int c) {
+  constexpr int kTail = BN % 64;
+  if (c < BN - kTail) {  // a 64-column box: 16-byte chunk index ^= row % 8
+    const uint32_t o = (uint32_t)(r * 128 + (c % 64) * 2);
+    return (uint32_t)(c / 64) * 8192u + (o ^ (((o >> 7) & 7u) << 4));
+  }
+  const uint32_t o = (uint32_t)(r * kTail * 2 + (c - (BN - kTail)) * 2);
+  constexpr int kSw = tail_swizzle_bytes(kTail);
+  const uint32_t sw = kSw == 32 ? ((o >> 7) & 1u) << 4 : kSw == 64 ? ((o >> 7) & 3u) << 4 : 0u;
+  return (uint32_t)(BN / 64) * 8192u + (o ^ sw);
+}
 
 __device__ __forceinline__ void tile_coords(const KernelArgs& a, int tile, int& m_blk, int& n_blk) {
   if (a.m_fastest) {
@@ -73,21 +92,46 @@ __device__ __forceinline__ float epi_act(float v, int act) {
   return v;
 }
 
+// bias[n] - col_sub[n] of this thread's column pair n, n + 1 (0 outside the matrix), loaded once per tile
+__device__ __forceinline__ void epi_cols(const KernelArgs& a, bool has_cols, int64_t n, float& cb0, float& cb1) {
+  cb0 = 0.f;
+  cb1 = 0.f;
+  if (!has_cols) return;
+  if (n < a.N) {
+    if (a.bias) cb0 += __ldg(&a.bias[n]);
+    if (a.col_sub) cb0 -= __ldg(&a.col_sub[n]);
+  }
+  if (n + 1 < a.N) {
+    if (a.bias) cb1 += __ldg(&a.bias[n + 1]);
+    if (a.col_sub) cb1 -= __ldg(&a.col_sub[n + 1]);
+  }
+}
+
+// act(alpha * v + cb): the epilogue before the residual
+__device__ __forceinline__ float epi_value(const KernelArgs& a, float v, float cb) {
+  if (a.alpha != 1.0f) v *= a.alpha;
+  return epi_act(v + cb, a.act);
+}
+
 template <int BN>
 __global__ void __launch_bounds__(kThreads, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
+                  const __grid_constant__ CUtensorMap map_d, const __grid_constant__ CUtensorMap map_d_tail,
                   const KernelArgs args) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  // after the ring: [2][64][stage_pitch] bf16 output tiles when args.staged
-  Ring ring(smem_raw, kATileBytes + BN * kChunkK * 2, args.stages, args.staged ? 2 * 64 * stage_pitch<BN>() : 0);
+  // after the ring, for a bf16 D: the two consumer warpgroups' staging tiles
+  Ring ring(smem_raw, kATileBytes + BN * kChunkK * 2, args.stages, args.d_is_f32 ? 0 : 2 * stage_bytes<BN>());
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int num_tiles = args.tiles_m * args.tiles_n;
-  const int num_kb = (args.K + kChunkK - 1) / kChunkK;
 
   if (threadIdx.x == 0) {
     prefetch_tensormap(&map_a);
     prefetch_tensormap(&map_b);
+    if (!args.d_is_f32) {
+      if (BN >= 64) prefetch_tensormap(&map_d);
+      if (BN % 64 != 0) prefetch_tensormap(&map_d_tail);
+    }
     ring.init();
   }
   __syncthreads();
@@ -96,6 +140,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
     regs_producer();
     // ===================== TMA producer =====================
     if (warp == 0 && elect_one_sync()) {
+      const int num_kb = (args.K + kChunkK - 1) / kChunkK;
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
         int m_blk, n_blk;
         tile_coords(args, tile, m_blk, n_blk);
@@ -120,137 +165,89 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
   for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
     int m_blk, n_blk;
     tile_coords(args, tile, m_blk, n_blk);
-    for (int kb = 0; kb < num_kb; ++kb) {
-      const uint32_t s = ring.wait();
-      const int ksteps = min(kChunkK, args.K - kb * kChunkK + 15) / 16;  // skip all-zero K tails
-      pipe::mma_chunk<BN>(acc, s + (uint32_t)(wg * 64 * 128), s + kATileBytes, ksteps, kb);
-      ring.release();
-    }
-    // ---- epilogue straight from the accumulator registers
+    pipe::mma_k_loop<BN>(ring, acc, (uint32_t)(wg * 64 * 128), (uint32_t)kATileBytes, args.K);
+    // ---- epilogue straight from the accumulator registers, each read once (an accumulator written by any other
+    //      instruction would make ptxas serialise every wgmma of the kernel)
     const int64_t n_base = (int64_t)n_blk * BN;
     const int64_t row0 = (int64_t)m_blk * kBlockM + wg * 64 + (wt >> 5) * 16 + (lane >> 2);
-#pragma unroll
-    for (int j = 0; j < BN / 8; ++j) {
-      const int64_t n = n_base + 8 * j + 2 * quad;  // this thread's two columns: n, n + 1
-      float cb0 = 0.f, cb1 = 0.f;
-      if (has_cols) {
-        if (n < args.N) {
-          if (args.bias) cb0 += __ldg(&args.bias[n]);
-          if (args.col_sub) cb0 -= __ldg(&args.col_sub[n]);
-        }
-        if (n + 1 < args.N) {
-          if (args.bias) cb1 += __ldg(&args.bias[n + 1]);
-          if (args.col_sub) cb1 -= __ldg(&args.col_sub[n + 1]);
-        }
-      }
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        float& f0 = acc[4 * j + 2 * h];
-        float& f1 = acc[4 * j + 2 * h + 1];
-        if (args.alpha != 1.0f) {
-          f0 *= args.alpha;
-          f1 *= args.alpha;
-        }
-        f0 = epi_act(f0 + cb0, args.act);
-        f1 = epi_act(f1 + cb1, args.act);
-      }
-    }
-    if (args.staged) {  // bf16: fragment -> shared tile -> 16-byte row chunks
-      uint8_t* stg = ring.extra() + wg * 64 * stage_pitch<BN>();
+    if (!args.d_is_f32) {  // bf16: fragment -> swizzled staging tile -> TMA stores (rows >= M, columns >= N clipped)
+      uint8_t* stg = ring.extra() + wg * stage_bytes<BN>();
       const int r_lo = (wt >> 5) * 16 + (lane >> 2);
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int64_t row = row0 + 8 * h;
-#pragma unroll
-        for (int j = 0; j < BN / 8; ++j) {
-          const int64_t n = n_base + 8 * j + 2 * quad;
-          float f0 = acc[4 * j + 2 * h], f1 = acc[4 * j + 2 * h + 1];
-          if (args.residual && row < args.M && n < args.N) {  // N % 8 == 0 here: both columns exist
-            const float2 rv = __bfloat1622float2(
-                *reinterpret_cast<const __nv_bfloat162*>(args.residual + row * args.ld_res + n));
-            f0 += rv.x;
-            f1 += rv.y;
-          }
-          *reinterpret_cast<__nv_bfloat162*>(stg + (r_lo + 8 * h) * stage_pitch<BN>() + (8 * j + 2 * quad) * 2) =
-              __floats2bfloat162_rn(f0, f1);
-        }
-      }
-      asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
-      const int64_t tile_row0 = (int64_t)m_blk * kBlockM + wg * 64;
-      for (int idx = wt; idx < 64 * (BN / 8); idx += 128) {
-        const int r = idx / (BN / 8), c8 = idx - r * (BN / 8);
-        const int64_t row = tile_row0 + r, n = n_base + 8 * c8;
-        if (row < args.M && n < args.N)
-          *reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(args.D) + row * args.ldd + n) =
-              *reinterpret_cast<const uint4*>(stg + r * stage_pitch<BN>() + c8 * 16);
-      }
-      asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");  // the tile is read before the next one is staged
-      continue;
-    }
-    if (args.chunk_max) {  // k-NN: the maximum of every 32-column chunk (columns >= N excluded); BN % 32 == 0 here
-#pragma unroll
-      for (int c = 0; c < BN / 32; ++c) {
-        float mx[2] = {-INFINITY, -INFINITY};
-#pragma unroll
-        for (int j = 4 * c; j < 4 * c + 4; ++j) {
-          const int64_t n = n_base + 8 * j + 2 * quad;
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            if (n < args.N) mx[h] = fmaxf(mx[h], acc[4 * j + 2 * h]);
-            if (n + 1 < args.N) mx[h] = fmaxf(mx[h], acc[4 * j + 2 * h + 1]);
-          }
-        }
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 1));
-          mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 2));
-          const int64_t row = row0 + 8 * h;
-          const int64_t n0 = n_base + 32 * c;
-          if (quad == 0 && row < args.M && n0 < args.N) args.chunk_max[row * args.ld_cm + (n0 >> 5)] = mx[h];
-        }
-      }
-    }
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int64_t row = row0 + 8 * h;
-      if (row >= args.M) continue;
+      if (wt == 0) bulk_wait_group_read<0>();  // the previous tile's stores have read the staging tile ...
+      named_bar_sync(1 + wg, 128);             // ... before any thread of the warpgroup writes it again
 #pragma unroll
       for (int j = 0; j < BN / 8; ++j) {
-        const int64_t n = n_base + 8 * j + 2 * quad;
-        if (n >= args.N) continue;
-        const bool pair = n + 1 < args.N;
-        float f0 = acc[4 * j + 2 * h], f1 = acc[4 * j + 2 * h + 1];
-        if (args.d_is_f32) {
-          float* d = reinterpret_cast<float*>(args.D) + row * args.ldd + n;
-          if (pair && args.d_vec) {
-            *reinterpret_cast<float2*>(d) = make_float2(f0, f1);
-          } else {
-            d[0] = f0;
-            if (pair) d[1] = f1;
-          }
-        } else {
-          if (args.residual) {
+        const int64_t n = n_base + 8 * j + 2 * quad;  // this thread's two columns: n, n + 1
+        float cb0, cb1;
+        epi_cols(args, has_cols, n, cb0, cb1);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int64_t row = row0 + 8 * h;
+          float f0 = epi_value(args, acc[4 * j + 2 * h], cb0), f1 = epi_value(args, acc[4 * j + 2 * h + 1], cb1);
+          if (args.residual && row < args.M && n < args.N) {
             const __nv_bfloat16* r = args.residual + row * args.ld_res + n;
-            if (pair && args.res_vec) {
+            if (n + 1 < args.N) {
               const float2 rv = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(r));
               f0 += rv.x;
               f1 += rv.y;
             } else {
               f0 += __bfloat162float(r[0]);
-              if (pair) f1 += __bfloat162float(r[1]);
             }
           }
-          __nv_bfloat16* d = reinterpret_cast<__nv_bfloat16*>(args.D) + row * args.ldd + n;
-          if (pair && args.d_vec) {
-            *reinterpret_cast<__nv_bfloat162*>(d) = __floats2bfloat162_rn(f0, f1);
-          } else {
-            d[0] = __float2bfloat16_rn(f0);
-            if (pair) d[1] = __float2bfloat16_rn(f1);
-          }
+          *reinterpret_cast<__nv_bfloat162*>(stg + stage_offset<BN>(r_lo + 8 * h, 8 * j + 2 * quad)) =
+              __floats2bfloat162_rn(f0, f1);
+        }
+      }
+      fence_proxy_async();  // the staging writes are visible to the TMA unit's reads
+      named_bar_sync(1 + wg, 128);
+      if (wt == 0) {
+        const int row_tile = m_blk * kBlockM + wg * 64;
+#pragma unroll
+        for (int b = 0; b < BN / 64; ++b) tma_store_2d(&map_d, stg + b * 8192, (int)n_base + 64 * b, row_tile);
+        if (BN % 64 != 0) tma_store_2d(&map_d_tail, stg + (BN / 64) * 8192, (int)n_base + BN - BN % 64, row_tile);
+        bulk_commit_group();
+      }
+      continue;
+    }
+    // fp32 D, stored from registers; k-NN: the maximum of every 32-column chunk (columns >= N excluded); BN % 32 == 0 when chunk_max is set
+    float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+      const int64_t n = n_base + 8 * j + 2 * quad;
+      const bool pair = n + 1 < args.N;
+      float cb0, cb1;
+      epi_cols(args, has_cols, n, cb0, cb1);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int64_t row = row0 + 8 * h;
+        float f0 = epi_value(args, acc[4 * j + 2 * h], cb0), f1 = epi_value(args, acc[4 * j + 2 * h + 1], cb1);
+        if (args.chunk_max) {
+          if (n < args.N) mx[h] = fmaxf(mx[h], f0);
+          if (pair) mx[h] = fmaxf(mx[h], f1);
+        }
+        if (row >= args.M || n >= args.N) continue;
+        float* d = reinterpret_cast<float*>(args.D) + row * args.ldd + n;
+        if (pair && args.d_vec) {
+          *reinterpret_cast<float2*>(d) = make_float2(f0, f1);
+        } else {
+          d[0] = f0;
+          if (pair) d[1] = f1;
+        }
+      }
+      if (args.chunk_max && j % 4 == 3) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 1));
+          mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 2));
+          const int64_t row = row0 + 8 * h;
+          const int64_t n0 = n_base + 8 * (j - 3);
+          if (quad == 0 && row < args.M && n0 < args.N) args.chunk_max[row * args.ld_cm + (n0 >> 5)] = mx[h];
+          mx[h] = -INFINITY;
         }
       }
     }
   }
+  if (!args.d_is_f32 && wt == 0) bulk_wait_group<0>();  // the last tile's stores are done before the CTA exits
 }
 
 // ---------------------------------------------------------------- SIMT reference (self test only)
@@ -334,10 +331,33 @@ int encode_map_nhwc_bf16(void* map_out, const void* base, int64_t n, int64_t h, 
   return AM_OK;
 }
 
+// The TMA map a bf16 D leaves through: [rows, cols] with rows `pitch_elems` apart (a multiple of 8), stored in boxes
+// of box_cols x 64 rows swizzled as stage_offset lays them out.
+static int encode_map_d(CUtensorMap* map_out, void* D, int64_t cols, int64_t rows, int64_t pitch_elems, int box_cols) {
+  const cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
+  const cuuint64_t strides[1] = {(cuuint64_t)pitch_elems * 2};
+  const cuuint32_t box[2] = {(cuuint32_t)box_cols, 64};
+  const cuuint32_t estr[2] = {1, 1};
+  const int sw = box_cols == 64 ? 128 : tail_swizzle_bytes(box_cols);
+  const CUtensorMapSwizzle swizzle = sw == 128  ? CU_TENSOR_MAP_SWIZZLE_128B
+                                     : sw == 64 ? CU_TENSOR_MAP_SWIZZLE_64B
+                                     : sw == 32 ? CU_TENSOR_MAP_SWIZZLE_32B
+                                                : CU_TENSOR_MAP_SWIZZLE_NONE;
+  CUresult r = get_encode()(map_out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, D, dims, strides, box, estr,
+                            CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle, CU_TENSOR_MAP_L2_PROMOTION_NONE,
+                            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    set_error("cuTensorMapEncodeTiled failed (%d) for D: cols=%lld rows=%lld pitch=%lld box_cols=%d", (int)r,
+              (long long)cols, (long long)rows, (long long)pitch_elems, box_cols);
+    return AM_ERR_CUDA;
+  }
+  return AM_OK;
+}
+
 // tile widths gemm_wgmma_kernel is instantiated for (the switch in gemm_bf16)
 static bool gemm_has_n(int n) {
-  return n == 16 || n == 32 || n == 48 || n == 64 || n == 80 || n == 96 || n == 112 || n == 128 || n == 160 ||
-         n == 192 || n == 224 || n == 256;
+  return n == 16 || n == 32 || n == 48 || n == 64 || n == 80 || n == 96 || n == 112 || n == 128 || n == 144 ||
+         n == 160 || n == 192 || n == 224 || n == 256;
 }
 
 // the smallest instantiated tile width >= n (n <= kMaxBlockN)
@@ -347,11 +367,21 @@ static int tile_n_for(int n) {
   return kMaxBlockN;
 }
 
+// N <= 256: one tile of the smallest width that holds N.  Wider: the width of at least 128 that pads N the least
+// (ties to the wider tile, fewer re-reads of A), e.g. 288 = 2 x 144, 1360 -> 11 x 128, 2592 = 18 x 144.  The k-NN
+// scores (chunk maxima) keep near-equal tiles of at most 256 columns, rounded to the 32-column chunks.
 static int pick_block_n(int64_t N, bool chunk_max) {
   const int64_t n16 = (int64_t)round_up((size_t)N, 16);
   int bn;
   if (n16 <= kMaxBlockN) {
     bn = (int)n16;
+  } else if (!chunk_max) {
+    int best = kMaxBlockN;
+    for (int c = kMaxBlockN; c >= 128; c -= 16) {
+      if (!gemm_has_n(c)) continue;
+      if ((N + c - 1) / c * c < (N + best - 1) / best * best) best = c;
+    }
+    return best;
   } else {
     const int64_t tiles = (n16 + kMaxBlockN - 1) / kMaxBlockN;
     bn = (int)round_up((size_t)((n16 + tiles - 1) / tiles), 16);
@@ -382,22 +412,24 @@ static KernelArgs make_args(int64_t M, int64_t N, int K, void* D, int64_t ldd, b
   a.ld_cm = ep.ld_cm;
   a.residual = ep.residual;
   a.ld_res = ep.ld_res;
-  a.res_vec = (ep.ld_res % 2 == 0 && (reinterpret_cast<uintptr_t>(ep.residual) & 3) == 0) ? 1 : 0;
-  a.staged = (!d_is_f32 && !ep.chunk_max && N % 8 == 0 && ldd % 8 == 0 && (reinterpret_cast<uintptr_t>(D) & 15) == 0 &&
-              (!ep.residual || (ep.ld_res % 2 == 0 && (reinterpret_cast<uintptr_t>(ep.residual) & 3) == 0))) ? 1 : 0;
   return a;
 }
 
 template <int BN>
 static int launch_bn(const CUtensorMap& map_a, const CUtensorMap& map_b, KernelArgs& args, cudaStream_t st) {
   AM_TRY(allow_dynamic_smem<gemm_wgmma_kernel<BN>>(kSmemMax));
+  CUtensorMap map_d = map_a, map_d_tail = map_a;  // unused for an fp32 D, and for the box kind BN lacks
+  if (!args.d_is_f32) {
+    if (BN >= 64) AM_TRY(encode_map_d(&map_d, args.D, args.N, args.M, args.ldd, 64));
+    if (BN % 64 != 0) AM_TRY(encode_map_d(&map_d_tail, args.D, args.N, args.M, args.ldd, BN % 64));
+  }
   const size_t stage_bytes = (size_t)kATileBytes + (size_t)BN * kChunkK * 2;
-  const size_t extra = args.staged ? 2 * 64 * stage_pitch<BN>() : 0;
+  const size_t extra = args.d_is_f32 ? 0 : 2 * (size_t)gemm::stage_bytes<BN>();
   args.stages = (int)std::min<size_t>(kStages, (kSmemMax - Ring::smem_bytes(0, 0, extra)) / stage_bytes);
   const size_t smem = Ring::smem_bytes(stage_bytes, args.stages, extra);
   const int tiles = args.tiles_m * args.tiles_n;
   const int grid = std::max(1, std::min(tiles, sm_count()));
-  AM_LAUNCH(gemm_wgmma_kernel<BN>, grid, kThreads, smem, st, map_a, map_b, args);
+  AM_LAUNCH(gemm_wgmma_kernel<BN>, grid, kThreads, smem, st, map_a, map_b, map_d, map_d_tail, args);
   return AM_OK;
 }
 
@@ -408,6 +440,11 @@ int gemm_bf16(const __nv_bfloat16* A, int64_t M, int64_t lda, const __nv_bfloat1
   AM_CHECK(lda % 8 == 0 && ldb % 8 == 0, "gemm: lda/ldb must be multiples of 8 elements (TMA 16-byte pitch)");
   AM_CHECK((reinterpret_cast<uintptr_t>(A) & 15) == 0 && (reinterpret_cast<uintptr_t>(B) & 15) == 0,
            "gemm: operands must be 16-byte aligned");
+  AM_CHECK(d_is_f32 || (ldd % 8 == 0 && (reinterpret_cast<uintptr_t>(D) & 15) == 0),
+           "gemm: a bf16 D needs ldd a multiple of 8 elements and a 16-byte aligned base (TMA stores)");
+  AM_CHECK(d_is_f32 || !ep.chunk_max, "gemm: chunk maxima need an fp32 D");
+  AM_CHECK(!ep.residual || (ep.ld_res % 2 == 0 && (reinterpret_cast<uintptr_t>(ep.residual) & 3) == 0),
+           "gemm: the residual needs an even ld_res and a 4-byte aligned base");
   AM_CHECK(available(), "gemm: wgmma path unavailable (needs sm_90 and cuTensorMapEncodeTiled)");
   KernelArgs args = make_args(M, N, K, D, ldd, d_is_f32, ep, m_fastest);
   CUtensorMap map_a, map_b;
@@ -422,6 +459,7 @@ int gemm_bf16(const __nv_bfloat16* A, int64_t M, int64_t lda, const __nv_bfloat1
     case 96: return launch_bn<96>(map_a, map_b, args, st);
     case 112: return launch_bn<112>(map_a, map_b, args, st);
     case 128: return launch_bn<128>(map_a, map_b, args, st);
+    case 144: return launch_bn<144>(map_a, map_b, args, st);
     case 160: return launch_bn<160>(map_a, map_b, args, st);
     case 192: return launch_bn<192>(map_a, map_b, args, st);
     case 224: return launch_bn<224>(map_a, map_b, args, st);

@@ -31,7 +31,9 @@ struct Epilogue {
 // cuTensorMapEncodeTiled
 bool available();
 
-// lda/ldb in elements, multiples of 8 (16-byte TMA row pitch).  ldd in elements of D.
+// lda/ldb in elements, multiples of 8 (16-byte TMA row pitch).  ldd in elements of D; a bf16 D leaves through TMA
+// stores, so its ldd is a multiple of 8 and its base 16-byte aligned.  A residual needs an even ld_res and a 4-byte
+// aligned base; chunk maxima need an fp32 D.
 // m_fastest: enumerate tiles with the M index fastest (B tile shared by consecutive CTAs;
 // right when A is small, e.g. k-NN queries); otherwise N fastest (A tile shared).
 int gemm_bf16(const __nv_bfloat16* A, int64_t M, int64_t lda, const __nv_bfloat16* B, int64_t N,

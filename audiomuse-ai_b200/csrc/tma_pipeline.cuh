@@ -100,18 +100,40 @@ struct Ring {
   }
 };
 
-// D[64 x N] (+)= A[64 x 64] . B[N x 64]^T for one K chunk of K-major SWIZZLE_128B tiles at shared addresses a, b:
-// `ksteps` 16-wide steps (fewer than 4 skips an all-zero K tail); chunk kb == 0 overwrites D.  Returns with the MMAs
-// complete.
-template <int N>
-__device__ __forceinline__ void mma_chunk(float (&acc)[N / 2], uint32_t a, uint32_t b, int ksteps, int kb) {
-  const uint64_t da = ptx::make_smem_desc(a), db = ptx::make_smem_desc(b);
+// The GEMM's whole K loop with one wgmma group in flight: the MMAs of chunk kb are issued and committed, then the
+// group of chunk kb - 1 is retired (wgmma.wait_group 1) and its stage released, so the tensor pipe never drains between
+// K chunks.  D[64 x N] = sum over the ceil(K / 64) chunks of A[64 x 64] . B[N x 64]^T (K-major SWIZZLE_128B tiles, the
+// A tile at byte offset a_off and the B tile at b_off of each stage), 16-wide K steps in order, all-zero K tails
+// skipped.  Returns with every MMA complete and every stage released; the accumulators are touched by no other
+// instruction until then.
+template <int N, int kMaxStages>
+__device__ __forceinline__ void mma_k_loop(Ring<kMaxStages>& ring, float (&acc)[N / 2], uint32_t a_off, uint32_t b_off,
+                                           int K) {
+  const int num_kb = (K + kChunkK - 1) / kChunkK;
+  int rd = ring.stage;  // the stage read next: one ahead of ring.stage (the one released next) inside the loop
+  uint32_t rd_phase = ring.phase;
   ptx::wgmma_fence();
 #pragma unroll 1
-  for (int ks = 0; ks < ksteps; ++ks)
-    ptx::Wgmma<N>::mma(acc, da + (uint64_t)(ks * 2), db + (uint64_t)(ks * 2), (kb | ks) ? 1u : 0u);
-  ptx::wgmma_commit();
-  ptx::wgmma_wait_all();
+  for (int kb = 0; kb < num_kb; ++kb) {
+    ptx::mbar_wait(&ring.full[rd], rd_phase);
+    const uint32_t s = ptx::smem_u32(ring.base + rd * ring.stage_bytes);
+    if (++rd == ring.stages) {
+      rd = 0;
+      rd_phase ^= 1;
+    }
+    const uint64_t da = ptx::make_smem_desc(s + a_off), db = ptx::make_smem_desc(s + b_off);
+    const int ksteps = min(kChunkK, K - kb * kChunkK + 15) / 16;  // skip all-zero K tails
+#pragma unroll 1
+    for (int ks = 0; ks < ksteps; ++ks)
+      ptx::Wgmma<N>::mma(acc, da + (uint64_t)(ks * 2), db + (uint64_t)(ks * 2), (kb | ks) ? 1u : 0u);
+    ptx::wgmma_commit();
+    if (kb > 0) {
+      ptx::wgmma_wait<1>();
+      ring.release();
+    }
+  }
+  ptx::wgmma_wait<0>();
+  ring.release();
   ptx::reg_fence(acc);
 }
 
