@@ -33,6 +33,13 @@ class MelCfg(C.Structure):
                 ("fmin", C.c_float), ("fmax", C.c_float), ("transpose", C.c_int)]
 
 
+class SongPathCfg(C.Structure):
+    """am_song_path_cfg"""
+    _fields_ = [("voyager_metric", C.c_int), ("path_metric", C.c_int), ("filter_lookback", C.c_int),
+                ("filter_batch", C.c_int), ("path_lookback", C.c_int), ("voyager_cap", C.c_int), ("path_cap", C.c_int),
+                ("stop_on_failure", C.c_int), ("filter_threshold", C.c_double), ("path_threshold", C.c_double)]
+
+
 _vp, _i, _i64, _f, _u64, _sz = C.c_void_p, C.c_int, C.c_int64, C.c_float, C.c_uint64, C.c_size_t
 _P = C.POINTER
 
@@ -93,6 +100,8 @@ SIGNATURES = {
     "am_knn_filter_by_distance": (_i, [_vp, _vp, _i, _i, C.c_float, _i, _i, _vp]),
     "am_knn_pairwise": (_i, [_vp, _vp, _i, _vp]),
     "am_knn_radius_walk": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _vp, _P(C.c_int32)]),
+    "am_knn_song_path": (_i, [_vp, _P(SongPathCfg), _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp, _P(C.c_int32), _vp,
+                              _vp, _vp, _P(C.c_int32), _i64, _vp, _vp, _P(C.c_int32), _vp]),
     "am_knn_get_vectors": (_i, [_vp, _vp, _i, _vp]),
     "am_knn_query_dev": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _vp]),
     "am_kmeans_fit": (_i, [_vp, _i64, _i, _i, _i, _i, _f, _u64, _vp, _vp, _vp, _P(_f), _P(_i)]),

@@ -14,6 +14,8 @@
 //   bitonic sort answers instead.
 #include "common.cuh"
 
+#include <math_constants.h>
+
 #include <algorithm>
 #include <cmath>
 #include <memory>
@@ -826,6 +828,12 @@ __device__ __forceinline__ double direct_distance(const float* a, const float* b
   return den == 0.0 ? INFINITY : 1.0 - fmin(1.0, fmax(-1.0, dot / den));
 }
 
+// The first kept item that item i of a list is compared with: the last `lookback` kept ones, or in a list longer
+// than the batch, the last `lookback` kept before i's batch (kept_at_batch) and every one kept since.
+__device__ __forceinline__ int filter_window_start(int kept, int kept_at_batch, bool batched, int lookback) {
+  return max(0, (batched ? kept_at_batch : kept) - lookback);
+}
+
 __global__ void __launch_bounds__(kFilterThreads)
 filter_by_distance_kernel(const float* __restrict__ X, int64_t N, int d, int metric, const int64_t* __restrict__ ids,
                           int n, double threshold, int lookback, int batch, unsigned char* __restrict__ keep) {
@@ -843,7 +851,7 @@ filter_by_distance_kernel(const float* __restrict__ X, int64_t N, int d, int met
     __syncthreads();
     bool valid = row >= 0 && row < N;  // the reference skips items whose vector is missing
     if (valid) {
-      const int start = max(0, (batched ? base : kept) - lookback);
+      const int start = filter_window_start(kept, base, batched, lookback);
       const float* a = X + row * d;
       for (int j = start + warp; j < kept; j += warps) {
         const double dist = direct_distance(a, X + (int64_t)s_kept[j] * d, d, metric, lane);
@@ -1085,6 +1093,210 @@ radius_walk_kernel(const float* __restrict__ X, int64_t N, int d, int metric, co
   for (int t = threadIdx.x; t < L; t += kWalkThreads) {
     out_pos[t] = ord[playlist[t]];
     out_dist[t] = walk_key_dist(key[playlist[t]]);
+  }
+}
+
+
+// ---------------------------------------------------------------- song path walk on device
+// path_manager.py:180-317 (_find_best_songs_for_job) over the chain find_nearest_neighbors_by_vector
+// (voyager_manager.py:1547-1657) runs on each job's k-NN prefix, for a sequence of jobs, in one CTA.  One pass over a
+// job's candidates in k-NN order does every stage, because each stage only looks at what came before it:
+//   * _filter_by_distance (:526-617): the item is compared with the kept window (filter_window_start) in the
+//     VOYAGER_METRIC distance; with no lookback the list is unchanged;
+//   * same-song dedupe (:1625-1636): an item without details, or whose signature this job already let through, is out;
+//   * the raw-author cap (:1638-1653, only when eliminate_duplicates and the cap is > 0; falsy authors are out);
+//   * [:n]: the pass ends after the n-th item that got this far;
+//   * acceptance (path_manager.py:211-291): used rows and signatures, the normalised-author cap, then the lookbacks
+//     against the path's last songs and this job's found songs, in PATH_DISTANCE_METRIC; the job ends once it has
+//     its songs.  A job that falls short gives back what it took (:294-312).
+// Per candidate, every warp computes the distances the decision may need (filter window, path window, found window)
+// and the threads look for the row among the used rows; then thread 0 decides and keeps the books.
+constexpr int kPathThreads = 512;
+
+// get_distance (path_manager.py:27-52): euclidean ||a - b||, angular arccos(clip(cos)) / pi (+inf when either row is
+// zero).  cos = 1 - (1 - cos) is exact for cos >= 0.5, which covers every distance below the thresholds.
+__device__ __forceinline__ double path_distance(const float* a, const float* b, int d, int metric, int lane) {
+  const double dd = direct_distance(a, b, d, metric, lane);
+  if (metric == kMetricL2 || dd == INFINITY) return dd;
+  return acos(1.0 - dd) / CUDART_PI;
+}
+
+struct SongPathArgs {
+  const float* X;
+  int64_t N;
+  int d;
+  int n_jobs;
+  const int32_t* job_off;     // [n_jobs + 1] candidate ranges
+  const int32_t* job_n;       // [n_jobs] the by-vector n (k_search)
+  const int32_t* job_need;    // [n_jobs] num_to_find
+  const int64_t* cand_row;    // [n_cand] stored row, -1: no vector
+  const int32_t* cand_sig;    // (title, author) signature key, -1: no details
+  const int32_t* cand_author; // normalised author key
+  const int32_t* cand_raw;    // raw author key, -1: falsy author
+  int64_t* used_row;          // [n_used + sum(need)] in / out
+  int32_t* n_used;
+  unsigned char* used_sig;    // [n_sig] in / out
+  int32_t* author_count;      // [n_author] in / out
+  int64_t* path_row;          // [n_path + sum(need)] in / out: the start song first
+  int32_t* n_path;
+  int64_t end_row;
+  am_song_path_cfg cfg;
+  int32_t* seen;              // [n_sig] scratch: the job that last let the signature through, -1 initially
+  int32_t* raw_mark;          // [n_raw] scratch: the job that last counted the raw author, -1 initially
+  int32_t* raw_count;         // [n_raw] scratch
+  int32_t* kept;              // [2 x max candidates per job] scratch: the filter's kept positions, then the job's found
+  int32_t* out_found;         // [n_jobs]
+  int32_t* out_pos;           // [sum(need)] accepted candidates, in path order
+  int32_t* out_failed;        // first failed job when stopping on failure, else -1
+  double* out_dist;           // [n_path + sum(need)] distances between consecutive songs of the path and the end song
+};
+
+__global__ void __launch_bounds__(kPathThreads) song_path_kernel(const SongPathArgs a) {
+  __shared__ int s_close;      // bit 0: filter window, bit 1: path window, bit 2: found window
+  __shared__ int s_used, s_stop;
+  __shared__ int s_kept, s_batch_kept, s_found, s_prod, s_n_used, s_n_path, s_n_out;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, warps = kPathThreads / 32;
+  const am_song_path_cfg& c = a.cfg;
+  const int lb_f = c.filter_lookback, lb_p = c.path_lookback;
+  for (int j = tid; j < a.n_jobs; j += kPathThreads) a.out_found[j] = 0;  // jobs after a stop are not run
+  if (tid == 0) {
+    s_n_used = *a.n_used;
+    s_n_path = *a.n_path;
+    s_n_out = 0;
+    *a.out_failed = -1;
+  }
+  __syncthreads();
+  for (int j = 0; j < a.n_jobs; ++j) {
+    const int base = a.job_off[j], m = a.job_off[j + 1] - base, n = a.job_n[j], need = a.job_need[j];
+    const bool batched = m > c.filter_batch;
+    if (tid == 0) {
+      s_kept = s_batch_kept = s_found = s_prod = s_stop = 0;
+    }
+    const int used0 = s_n_used;  // the rows this job adds are given back by truncation
+    __syncthreads();
+    int found_all = 0;  // thread 0: songs found so far
+    for (int i = 0; i < m; ++i) {
+      const int64_t row = a.cand_row[base + i];
+      const bool valid = row >= 0 && row < a.N;
+      if (tid == 0) {
+        s_close = 0;
+        s_used = 0;
+        if (batched && i % c.filter_batch == 0) s_batch_kept = s_kept;
+      }
+      __syncthreads();
+      if (valid) {
+        const int kept = s_kept, found = s_found, np = s_n_path;
+        const int f0 = lb_f > 0 ? filter_window_start(kept, s_batch_kept, batched, lb_f) : kept;
+        const int nf = kept - f0, npw = min(lb_p, np), nq = min(lb_p, found);
+        const float* x = a.X + row * a.d;
+        for (int t = warp; t < nf + npw + nq; t += warps) {
+          int64_t other;
+          int metric, bit;
+          double thr;
+          if (t < nf) {
+            other = a.cand_row[base + a.kept[f0 + t]];
+            metric = c.voyager_metric;
+            thr = c.filter_threshold;
+            bit = 1;
+          } else if (t < nf + npw) {
+            other = a.path_row[np - npw + (t - nf)];
+            metric = c.path_metric;
+            thr = c.path_threshold;
+            bit = 2;
+          } else {
+            other = a.cand_row[base + a.kept[m + found - nq + (t - nf - npw)]];
+            metric = c.path_metric;
+            thr = c.path_threshold;
+            bit = 4;
+          }
+          const float* y = a.X + other * a.d;
+          const double dist = bit == 1 ? direct_distance(x, y, a.d, metric, lane) : path_distance(x, y, a.d, metric, lane);
+          if (lane == 0 && dist < thr) atomicOr(&s_close, bit);
+        }
+      }
+      for (int t = tid; t < s_n_used; t += kPathThreads)
+        if (a.used_row[t] == row) s_used = 1;
+      __syncthreads();
+      if (tid == 0) {
+        const int close = s_close;
+        bool pass = true;
+        if (lb_f > 0) {  // _filter_by_distance: items without a vector are dropped, the kept ones form the window
+          pass = valid && !(close & 1);
+          if (pass) a.kept[s_kept++] = i;
+        }
+        const int sig = a.cand_sig[base + i];
+        if (pass && sig < 0) pass = false;
+        if (pass) {
+          if (a.seen[sig] == j) pass = false;
+          else a.seen[sig] = j;
+        }
+        if (pass && c.voyager_cap > 0) {
+          const int r = a.cand_raw[base + i];
+          if (r < 0) {
+            pass = false;
+          } else {
+            if (a.raw_mark[r] != j) {
+              a.raw_mark[r] = j;
+              a.raw_count[r] = 0;
+            }
+            if (a.raw_count[r] >= c.voyager_cap) pass = false;
+            else a.raw_count[r] += 1;
+          }
+        }
+        if (pass) {
+          s_prod += 1;
+          const int au = a.cand_author[base + i];
+          const bool ok = !s_used && !a.used_sig[sig] && !(c.path_cap > 0 && a.author_count[au] >= c.path_cap) && valid &&
+                          !(close & 2) && !(close & 4);
+          if (ok) {
+            ++found_all;
+            s_found = found_all;
+            a.used_row[s_n_used++] = row;
+            a.used_sig[sig] = 1;
+            a.author_count[au] += 1;
+            a.out_pos[s_n_out + found_all - 1] = base + i;
+            a.kept[m + found_all - 1] = i;  // the job's found list, behind the filter's (<= m entries each)
+          }
+          if (found_all >= need || s_prod >= n) s_stop = 1;
+        }
+      }
+      __syncthreads();
+      if (s_stop) break;
+    }
+    if (tid == 0) {
+      const int found = s_found;
+      if (found < need) {  // roll back (:294-312)
+        for (int t = 0; t < found; ++t) {
+          const int p = base + a.kept[m + t];
+          a.used_sig[a.cand_sig[p]] = 0;
+          int& cnt = a.author_count[a.cand_author[p]];
+          cnt = max(0, cnt - 1);
+        }
+        s_n_used = used0;
+        a.out_found[j] = 0;
+        if (c.stop_on_failure) {
+          *a.out_failed = j;
+          s_stop = 2;
+        }
+      } else {
+        for (int t = 0; t < found; ++t) a.path_row[s_n_path++] = a.cand_row[base + a.kept[m + t]];
+        s_n_out += found;
+        a.out_found[j] = found;
+      }
+    }
+    __syncthreads();
+    if (s_stop == 2) break;
+  }
+  // distances between consecutive songs of the path, the end song last
+  const int np = s_n_path;
+  for (int t = warp; t < np; t += warps) {
+    const int64_t r0 = a.path_row[t], r1 = t + 1 < np ? a.path_row[t + 1] : a.end_row;
+    const double dist = path_distance(a.X + r0 * a.d, a.X + r1 * a.d, a.d, c.path_metric, lane);
+    if (lane == 0) a.out_dist[t] = dist;
+  }
+  if (tid == 0) {
+    *a.n_used = s_n_used;
+    *a.n_path = np;
   }
 }
 
@@ -1642,5 +1854,127 @@ extern "C" int am_knn_radius_walk(const am_index* idx, const float* anchor, cons
   std::memcpy(out_pos, h + b_cnt, (size_t)cnt * 4);
   std::memcpy(out_dist, h + b_cnt + b_pos, (size_t)cnt * 8);
   *out_count = cnt;
+  return AM_OK;
+}
+
+extern "C" int am_knn_song_path(const am_index* idx, const am_song_path_cfg* cfg, int n_jobs, const int32_t* job_off,
+                                const int32_t* job_n, const int32_t* job_need, const int64_t* cand_rows,
+                                const int32_t* cand_sig, const int32_t* cand_author, const int32_t* cand_author_raw,
+                                int n_sig, int n_author, int64_t* used_rows, int32_t* n_used, unsigned char* used_sig,
+                                int32_t* author_count, int64_t* path_rows, int32_t* n_path, int64_t end_row,
+                                int32_t* out_found, int32_t* out_pos, int32_t* out_failed, double* out_dist) {
+  AM_CHECK(idx && cfg && n_used && n_path && out_failed && (n_jobs == 0 || (job_off && job_n && job_need && out_found)),
+           "am_knn_song_path: NULL argument");
+  AM_CHECK(n_jobs >= 0 && n_sig >= 0 && n_author >= 0 && *n_used >= 0 && *n_path >= 1,
+           "am_knn_song_path: negative size, or no start song in the path");
+  AM_CHECK(cfg->voyager_metric == kMetricCos || cfg->voyager_metric == kMetricL2, "am_knn_song_path: voyager_metric %d",
+           cfg->voyager_metric);
+  AM_CHECK(cfg->path_metric == kMetricCos || cfg->path_metric == kMetricL2, "am_knn_song_path: path_metric %d",
+           cfg->path_metric);
+  AM_CHECK(cfg->filter_batch > 0, "am_knn_song_path: filter_batch must be positive");
+  AM_CHECK(end_row >= 0 && end_row < idx->N, "am_knn_song_path: end row %lld out of range", (long long)end_row);
+  AM_CHECK(n_jobs == 0 || job_off[0] == 0, "am_knn_song_path: job_off[0] must be 0");
+  int64_t total_need = 0;
+  int max_m = 0;
+  for (int j = 0; j < n_jobs; ++j) {
+    AM_CHECK(job_off[j + 1] >= job_off[j] && job_n[j] >= 1 && job_need[j] >= 1,
+             "am_knn_song_path: job %d: bad range, n or num_to_find", j);
+    total_need += job_need[j];
+    max_m = std::max(max_m, job_off[j + 1] - job_off[j]);
+  }
+  const int n_cand = n_jobs ? job_off[n_jobs] : 0;
+  AM_CHECK(n_cand == 0 || (cand_rows && cand_sig && cand_author && cand_author_raw), "am_knn_song_path: NULL candidates");
+  AM_CHECK(total_need == 0 || out_pos, "am_knn_song_path: NULL out_pos");
+  int n_raw = 0;
+  for (int i = 0; i < n_cand; ++i) {
+    AM_CHECK(cand_sig[i] >= -1 && cand_sig[i] < n_sig && cand_author[i] >= 0 && cand_author[i] < n_author &&
+                 cand_author_raw[i] >= -1,
+             "am_knn_song_path: candidate %d has a key out of range", i);
+    n_raw = std::max(n_raw, cand_author_raw[i] + 1);
+  }
+  const int nu = *n_used, np = *n_path;
+  for (int t = 0; t < np; ++t)
+    AM_CHECK(path_rows[t] >= 0 && path_rows[t] < idx->N, "am_knn_song_path: path row %d out of range", t);
+  const int64_t cap_used = nu + total_need, cap_path = np + total_need;
+  AM_TRY(ensure_init());
+  static thread_local Stream tst;  // re-entrant like am_knn_query
+  AM_TRY(tst.create());
+  cudaStream_t st = tst.s;
+  using A = Arena;
+  // [inputs | state | outputs | scratch]: inputs and state go up in one copy, state and outputs come back in one
+  const size_t b_in = A::pad((n_jobs + 1) * 4) + 2 * A::pad(n_jobs * 4) + A::pad((size_t)n_cand * 8) + 3 * A::pad((size_t)n_cand * 4);
+  const size_t b_state = A::pad(16) + A::pad(cap_used * 8) + A::pad(cap_path * 8) + A::pad((size_t)n_author * 4) + A::pad(n_sig);
+  const size_t b_out = A::pad(n_jobs * 4) + A::pad(total_need * 4) + A::pad(cap_path * 8);
+  const size_t b_scratch = A::pad((size_t)n_sig * 4) + 2 * A::pad((size_t)n_raw * 4) + A::pad((size_t)2 * max_m * 4);
+  static thread_local HostStage pin;
+  AM_TRY(pin.ensure(b_in + b_state + b_out));
+  Arena blk;
+  AM_TRY(blk.reserve(b_in + b_state + b_out + b_scratch, st));
+  char* const d0 = blk.buf.p;
+  int32_t* d_off = blk.take<int32_t>(n_jobs + 1);
+  int32_t* d_n = blk.take<int32_t>(n_jobs);
+  int32_t* d_need = blk.take<int32_t>(n_jobs);
+  int64_t* d_row = blk.take<int64_t>(n_cand);
+  int32_t* d_sig = blk.take<int32_t>(n_cand);
+  int32_t* d_au = blk.take<int32_t>(n_cand);
+  int32_t* d_raw = blk.take<int32_t>(n_cand);
+  int32_t* d_hdr = blk.take<int32_t>(4);  // n_used, n_path, failed
+  int64_t* d_used = blk.take<int64_t>(cap_used);
+  int64_t* d_path = blk.take<int64_t>(cap_path);
+  int32_t* d_count = blk.take<int32_t>(n_author);
+  unsigned char* d_usig = blk.take<unsigned char>(n_sig);
+  int32_t* d_found = blk.take<int32_t>(n_jobs);
+  int32_t* d_pos = blk.take<int32_t>(total_need);
+  double* d_dist = blk.take<double>(cap_path);
+  int32_t* d_seen = blk.take<int32_t>(n_sig);
+  int32_t* d_mark = blk.take<int32_t>(n_raw);
+  int32_t* d_rcount = blk.take<int32_t>(n_raw);
+  int32_t* d_kept = blk.take<int32_t>((size_t)2 * max_m);
+  char* h = static_cast<char*>(pin.p);
+  auto put = [&](const void* src, const void* dev, size_t bytes) {
+    if (bytes) std::memcpy(h + (static_cast<const char*>(dev) - d0), src, bytes);
+  };
+  put(job_off, d_off, (n_jobs ? n_jobs + 1 : 0) * 4);
+  put(job_n, d_n, n_jobs * 4);
+  put(job_need, d_need, n_jobs * 4);
+  put(cand_rows, d_row, (size_t)n_cand * 8);
+  put(cand_sig, d_sig, (size_t)n_cand * 4);
+  put(cand_author, d_au, (size_t)n_cand * 4);
+  put(cand_author_raw, d_raw, (size_t)n_cand * 4);
+  const int32_t hdr[4] = {nu, np, -1, 0};
+  put(hdr, d_hdr, 16);
+  put(used_rows, d_used, (size_t)nu * 8);
+  put(path_rows, d_path, (size_t)np * 8);
+  put(author_count, d_count, (size_t)n_author * 4);
+  put(used_sig, d_usig, (size_t)n_sig);
+  AM_CUDA(cudaMemcpyAsync(d0, h, b_in + b_state, cudaMemcpyHostToDevice, st));
+  AM_CUDA(cudaMemsetAsync(d_seen, 0xff, A::pad((size_t)n_sig * 4) + A::pad((size_t)n_raw * 4), st));  // seen, raw_mark: -1
+  SongPathArgs a{idx->X.p, idx->N, idx->d, n_jobs, d_off, d_n, d_need, d_row, d_sig, d_au, d_raw, d_used, d_hdr, d_usig,
+                 d_count, d_path, d_hdr + 1, end_row, *cfg, d_seen, d_mark, d_rcount, d_kept, d_found, d_pos, d_hdr + 2,
+                 d_dist};
+  AM_LAUNCH(song_path_kernel, 1, kPathThreads, 0, st, a);
+  char* const s0 = reinterpret_cast<char*>(d_hdr);
+  AM_CUDA(cudaMemcpyAsync(h + (s0 - d0), s0, b_state + b_out, cudaMemcpyDeviceToHost, st));
+  AM_CUDA(cudaStreamSynchronize(st));
+  auto get = [&](void* dst, const void* dev, size_t bytes) {
+    if (bytes) std::memcpy(dst, h + (static_cast<const char*>(dev) - d0), bytes);
+  };
+  int32_t out_hdr[4];
+  get(out_hdr, d_hdr, 16);
+  int64_t taken = 0;
+  get(out_found, d_found, n_jobs * 4);
+  for (int j = 0; j < n_jobs; ++j) taken += out_found[j];
+  AM_CHECK(out_hdr[0] >= nu && out_hdr[0] <= cap_used && out_hdr[1] >= np && out_hdr[1] <= cap_path && taken <= total_need,
+           "am_knn_song_path: inconsistent result (used %d of %lld, path %d of %lld, taken %lld of %lld)", out_hdr[0],
+           (long long)cap_used, out_hdr[1], (long long)cap_path, (long long)taken, (long long)total_need);
+  *n_used = out_hdr[0];
+  *n_path = out_hdr[1];
+  *out_failed = out_hdr[2];
+  get(out_pos, d_pos, taken * 4);
+  get(used_rows, d_used, (size_t)out_hdr[0] * 8);
+  get(path_rows, d_path, (size_t)out_hdr[1] * 8);
+  get(author_count, d_count, (size_t)n_author * 4);
+  get(used_sig, d_usig, (size_t)n_sig);
+  get(out_dist, d_dist, (size_t)out_hdr[1] * 8);
   return AM_OK;
 }

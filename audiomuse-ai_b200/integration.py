@@ -122,7 +122,7 @@ METRIC_NAMES = ("silhouette_score", "davies_bouldin_score", "calinski_harabasz_s
 
 def apply(clap=None, voyager_manager=None, clustering=None, allow_sklearn_fallback: bool = True,
           clustering_helper=None, song_alchemy=None, app_map=None, artist_gmm_manager=None,
-          gaussian_mixture=None, radius_walk=None) -> None:
+          gaussian_mixture=None, radius_walk=None, path_manager=None, app_path=None) -> None:
     """clap / voyager_manager / clustering / clustering_helper: the reference's already imported tasks.* modules (pass
     only the ones to patch).  allow_sklearn_fallback keeps the reference's contract that a failing GPU k-means silently
     falls back to scikit-learn (tasks/clustering_gpu.py:130-148); this repository's own tests run with it off so a
@@ -138,7 +138,10 @@ def apply(clap=None, voyager_manager=None, clustering=None, allow_sklearn_fallba
     GPU GPUGaussianMixture; get_clustering_model looks the class up at call time (:385).  clustering= alone leaves
     that class to the reference.  radius_walk (the reference's tasks.voyager_manager again) gets the device radius
     walk: _radius_walk_get_candidates and _execute_radius_walk are replaced together (make_radius_walk);
-    voyager_manager= alone leaves the walk to the reference."""
+    voyager_manager= alone leaves the walk to the reference.  path_manager (the reference's tasks.path_manager) gets the
+    device song path as find_path_between_songs (song_path.make_song_path, over the voyager_manager module whose
+    functions path_manager imported); app_path binds that name when it is imported (app_path.py:5), so pass it too for
+    the Song Path endpoint to use it."""
     if clap is not None:
         from . import clap_analyzer as b200_clap
 
@@ -149,6 +152,15 @@ def apply(clap=None, voyager_manager=None, clustering=None, allow_sklearn_fallba
     if radius_walk is not None:
         for name, fn in zip(RADIUS_WALK_NAMES, make_radius_walk(radius_walk)):
             setattr(radius_walk, name, fn)
+    if app_path is not None and path_manager is None:
+        raise ValueError("app_path= takes the device song path from path_manager=: pass both")
+    if path_manager is not None:
+        from . import song_path
+
+        fn = song_path.make_song_path(sys.modules[path_manager.get_vector_by_id.__module__], path_manager)
+        path_manager.find_path_between_songs = fn
+        if app_path is not None:
+            app_path.find_path_between_songs = fn
     if clustering is not None:
         from . import clustering_gpu as b200_cg
 

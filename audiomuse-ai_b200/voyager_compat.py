@@ -306,6 +306,47 @@ class Index:
                                                       C.byref(count)))
         return pos[:count.value].copy(), dist[:count.value].copy()
 
+    # ------------------------------------------------------------------ song path (path_manager.py:180-317)
+    def song_path(self, cfg, job_off, job_n, job_need, cand_ids, cand_sig, cand_author, cand_author_raw, used_ids,
+                  used_sig, author_count, path_ids, end_id):
+        """The song path's centroid jobs over their k-NN prefixes in one device call (am_knn_song_path).
+        cfg: an _lib.SongPathCfg.  job_off i32[n_jobs + 1] delimits each job's candidates in cand_ids (index ids in
+        k-NN order; ids not in the index have no vector); cand_sig / cand_author / cand_author_raw are the dense keys
+        the header describes.  used_sig (u8) and author_count (i32) are updated in place.  Returns (found i32[n_jobs],
+        accepted candidate positions in path order, the failed job or None, used ids, path ids, f64 distances between
+        consecutive path songs and the end song)."""
+        n_jobs = len(job_n)
+        off = np.ascontiguousarray(job_off, dtype=np.int32)
+        jn = np.ascontiguousarray(job_n, dtype=np.int32)
+        need = np.ascontiguousarray(job_need, dtype=np.int32)
+        if off.shape != (n_jobs + 1,) or need.shape != (n_jobs,):
+            raise ValueError("job_off / job_need do not match job_n")
+        rows = np.array([self._lookup(int(i)) for i in cand_ids], dtype=np.int64)
+        keys = [np.ascontiguousarray(k, dtype=np.int32) for k in (cand_sig, cand_author, cand_author_raw)]
+        if any(k.shape != rows.shape for k in keys) or (n_jobs and off[-1] != len(rows)):
+            raise ValueError("candidate arrays differ in length")
+        if used_sig.dtype != np.uint8 or author_count.dtype != np.int32:
+            raise ValueError("used_sig must be uint8 and author_count int32")
+        total = int(need.sum())
+        used = np.empty(len(used_ids) + total, dtype=np.int64)
+        used[:len(used_ids)] = [self._row_of(i) for i in used_ids]
+        path = np.empty(len(path_ids) + total, dtype=np.int64)
+        path[:len(path_ids)] = [self._row_of(i) for i in path_ids]
+        n_used, n_path, failed = C.c_int32(len(used_ids)), C.c_int32(len(path_ids)), C.c_int32(-1)
+        found = np.zeros(max(n_jobs, 1), dtype=np.int32)
+        pos = np.empty(max(total, 1), dtype=np.int32)
+        dist = np.empty(len(path), dtype=np.float64)
+        h = self._ensure_built()
+        _lib.check(_lib.load().am_knn_song_path(
+            h, C.byref(cfg), n_jobs, _lib.ptr(off), _lib.ptr(jn), _lib.ptr(need), _lib.ptr(rows), _lib.ptr(keys[0]),
+            _lib.ptr(keys[1]), _lib.ptr(keys[2]), len(used_sig), len(author_count), _lib.ptr(used), C.byref(n_used),
+            _lib.ptr(used_sig), _lib.ptr(author_count), _lib.ptr(path), C.byref(n_path), self._row_of(end_id),
+            _lib.ptr(found), _lib.ptr(pos), C.byref(failed), _lib.ptr(dist)))
+        found = found[:n_jobs].copy()
+        return (found, pos[:int(found.sum())].copy(), None if failed.value < 0 else failed.value,
+                self._ids[used[:n_used.value]].tolist(), self._ids[path[:n_path.value]].tolist(),
+                dist[:n_path.value].copy())
+
     # ------------------------------------------------------------------ persistence
     def as_bytes(self) -> bytes:
         with self._mu:

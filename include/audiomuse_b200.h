@@ -233,6 +233,41 @@ AM_API int am_knn_pairwise(const am_index* idx, const int64_t* ids, int n, float
 AM_API int am_knn_radius_walk(const am_index* idx, const float* anchor, const int64_t* rows, const int32_t* artists,
                               int n_cand, int n, int eliminate_duplicates, int max_songs_per_artist, int metric,
                               int32_t* out_pos, double* out_dist, int32_t* out_count);
+/* The configuration path_manager.py and voyager_manager.py read at call time, for am_knn_song_path.  Metrics are
+ * 0 angular or 1 euclidean: voyager_metric is config.VOYAGER_METRIC as get_direct_distance reads it (1 - cos),
+ * path_metric config.PATH_DISTANCE_METRIC as get_distance reads it (arccos(cos) / pi). */
+typedef struct am_song_path_cfg {
+  int voyager_metric;
+  int path_metric;
+  int filter_lookback;     /* voyager_manager.DUPLICATE_DISTANCE_CHECK_LOOKBACK (<= 0: no distance filter) */
+  int filter_batch;        /* voyager_manager.BATCH_SIZE_VECTOR_OPS */
+  int path_lookback;       /* path_manager.DUPLICATE_DISTANCE_CHECK_LOOKBACK (<= 0: no path lookback) */
+  int voyager_cap;         /* the by-vector raw-author cap: MAX_SONGS_PER_ARTIST when eliminate_duplicates, else 0 */
+  int path_cap;            /* path_manager.MAX_SONGS_PER_ARTIST (<= 0: off) */
+  int stop_on_failure;     /* path_fix_size: stop at the first failed job instead of skipping it */
+  double filter_threshold; /* DUPLICATE_DISTANCE_THRESHOLD_* for voyager_metric */
+  double path_threshold;   /* DUPLICATE_DISTANCE_THRESHOLD_* for path_metric */
+} am_song_path_cfg;
+
+/* The song path's centroid jobs, path_manager.py:180-317 (_find_best_songs_for_job) over the by-vector chain
+ * (voyager_manager.py:1589-1657), in one call.  Job j's candidates are entries job_off[j] .. job_off[j+1] of the
+ * candidate arrays, its k-NN prefix in order; job_n[j] is its k_search, job_need[j] its num_to_find (both >= 1).
+ * Per candidate: cand_rows its stored row (-1: no vector), cand_sig a dense key of its (title, author) signature after
+ * strip().lower() (-1: no details), cand_author a dense key of its normalised author, cand_author_raw a dense key of
+ * its raw author (-1: falsy).  The carried state, read and updated: used_rows[*n_used] the rows taken (start and end
+ * song included), used_sig[n_sig] a flag per signature, author_count[n_author] songs per normalised author,
+ * path_rows[*n_path] the path so far, start song first.  used_rows and path_rows have room for sum(job_need) more.
+ * Jobs run in order; a failed job gives back what it took and stops the call when cfg->stop_on_failure, else the
+ * next job runs.  out_found[j] receives the songs job j took (0: failed or not run), out_pos the accepted candidates
+ * (entries of the candidate arrays) in path order, *out_failed the job that stopped the call or -1, and out_dist
+ * f64[*n_path] the path_metric distances between consecutive rows of path_rows followed by end_row, in float64 from
+ * the stored rows.  Re-entrant. */
+AM_API int am_knn_song_path(const am_index* idx, const am_song_path_cfg* cfg, int n_jobs, const int32_t* job_off,
+                            const int32_t* job_n, const int32_t* job_need, const int64_t* cand_rows,
+                            const int32_t* cand_sig, const int32_t* cand_author, const int32_t* cand_author_raw,
+                            int n_sig, int n_author, int64_t* used_rows, int32_t* n_used, unsigned char* used_sig,
+                            int32_t* author_count, int64_t* path_rows, int32_t* n_path, int64_t end_row,
+                            int32_t* out_found, int32_t* out_pos, int32_t* out_failed, double* out_dist);
 /* n stored rows in one device gather + one copy: out f32[n, d] */
 AM_API int am_knn_get_vectors(const am_index* idx, const int64_t* ids, int n, float* out);
 AM_API int am_knn_query_dev(const am_index* idx, const float* Q_dev, int nq, int k, int mode,

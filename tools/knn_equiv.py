@@ -9,7 +9,7 @@ selection (chunk maxima, row streaming, full sort) runs: cosine / euclidean / in
 staging limit); k of 1, 50, 500, 600 and len(index); modes 0, 1 and 2.  Per call: ids, distances, and the kernels
 launched with their counts (am_profile_report, template arguments stripped).  Also am_knn_query_dev on a 20 000 x 200
 euclidean self-query as the spectral and UMAP graphs issue it, and the duplicate filter, pairwise distances,
-get_vectors and get_vector.  A query with k > 4032 is answered by the full sort alone: its kernel list may differ
+get_vectors and get_vector, and the radius walk under both metrics and artist rules.  A query with k > 4032 is answered by the full sort alone: its kernel list may differ
 from the other build's by the scoring kernels only; get_vector's launches are not compared (it used to copy from a
 host mirror of the rows, and gathers its row on the device now).  Needs an H100."""
 import ctypes as C
@@ -75,6 +75,13 @@ def _collect():
             ids = [int(i) for i in lists[0][:40]]
             out[f"{sname}/N{N}/d{d}/pairwise"] = idx.pairwise_distances(ids + [N + 7])
             out[f"{sname}/N{N}/d{d}/get_vectors"] = idx.get_vectors(ids)
+            pool = [int(i) for i in out[f"{sname}/N{N}/d{d}/nq16/k500/mode0/ids"][0]] if N >= 500 else ids
+            artists = [i % 7 - 1 for i in range(len(pool))]
+            for metric in ("angular", "euclidean"):
+                for ed, cap in ((True, 1), (True, 3), (False, 3)):
+                    pos, dist = idx.radius_walk(q[0], pool, artists, 200, ed, cap, metric)
+                    out[f"{sname}/N{N}/d{d}/radius_walk/{metric}/ed{int(ed)}/cap{cap}/pos"] = pos
+                    out[f"{sname}/N{N}/d{d}/radius_walk/{metric}/ed{int(ed)}/cap{cap}/dist"] = dist
             out[f"{sname}/N{N}/d{d}/other_kernels"] = _kernels()
             one = np.empty((5, d), np.float32)
             for j, i in enumerate(ids[:5]):
