@@ -98,7 +98,6 @@ SIGNATURES = {
     "am_knn_query": (_i, [_vp, _vp, _i, _i, _vp, _vp]),
     "am_knn_query_ex": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp]),
     "am_knn_filter_by_distance": (_i, [_vp, _vp, _i, _i, C.c_float, _i, _i, _vp]),
-    "am_knn_pairwise": (_i, [_vp, _vp, _i, _vp]),
     "am_knn_radius_walk": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _vp, _P(C.c_int32)]),
     "am_knn_song_path": (_i, [_vp, _P(SongPathCfg), _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp, _P(C.c_int32), _vp,
                               _vp, _vp, _P(C.c_int32), _i64, _vp, _vp, _P(C.c_int32), _vp]),

@@ -1,0 +1,680 @@
+// Candidate post-processing on the stored rows of the k-NN index (knn.cu): the duplicate filter, the radius walk and
+// the song path's jobs, each one kernel behind one host call.
+#include "knn.cuh"
+
+#include <math_constants.h>
+
+#include <algorithm>
+
+namespace am {
+
+// ---------------------------------------------------------------- duplicate filter on device
+// voyager_manager.py:526-617 (_filter_by_distance) + :487-524 (_compute_distance_batch): walk a result list in
+// order and drop an item whose DIRECT distance (get_direct_distance, :99-140: cosine = 1 - cos with both norms
+// recomputed, euclidean = ||a - b||, not squared) to a recently kept item is below the threshold.  "Recently
+// kept": lists of <= `batch` items compare with the last `lookback` kept items; longer lists are cut into
+// batches of `batch`, and an item is compared with the last `lookback` items kept BEFORE its batch plus
+// everything kept so far inside the batch.  One CTA per list; the walk is sequential, the comparisons of one
+// item are spread over the warps; float64 accumulation.
+constexpr int kFilterThreads = 256;
+constexpr int kFilterCap = 4096;  // items per list
+
+// get_direct_distance (voyager_manager.py:99-140) between stored rows a and b, one warp, float64 accumulation:
+// euclidean ||a - b||, otherwise 1 - cos (+inf when either row is zero)
+__device__ __forceinline__ double direct_distance(const float* a, const float* b, int d, int metric, int lane) {
+  double dot = 0.0, na = 0.0, nb = 0.0, d2 = 0.0;
+  for (int t = lane; t < d; t += 32) {
+    const double av = (double)__ldg(&a[t]), bv = (double)__ldg(&b[t]);
+    dot = fma(av, bv, dot);
+    na = fma(av, av, na);
+    nb = fma(bv, bv, nb);
+    const double df = av - bv;
+    d2 = fma(df, df, d2);
+  }
+  dot = warp_sum(dot);
+  na = warp_sum(na);
+  nb = warp_sum(nb);
+  d2 = warp_sum(d2);
+  if (metric == kMetricL2) return sqrt(d2);
+  const double den = sqrt(na) * sqrt(nb);
+  return den == 0.0 ? INFINITY : 1.0 - fmin(1.0, fmax(-1.0, dot / den));
+}
+
+// The first kept item that item i of a list is compared with: the last `lookback` kept ones, or in a list longer
+// than the batch, the last `lookback` kept before i's batch (kept_at_batch) and every one kept since.
+__device__ __forceinline__ int filter_window_start(int kept, int kept_at_batch, bool batched, int lookback) {
+  return max(0, (batched ? kept_at_batch : kept) - lookback);
+}
+
+__global__ void __launch_bounds__(kFilterThreads)
+filter_by_distance_kernel(const float* __restrict__ X, int64_t N, int d, int metric, const int64_t* __restrict__ ids,
+                          int n, double threshold, int lookback, int batch, unsigned char* __restrict__ keep) {
+  __shared__ int s_kept[kFilterCap];
+  __shared__ int s_close;
+  const int64_t* my_ids = ids + (int64_t)blockIdx.x * n;
+  unsigned char* my_keep = keep + (int64_t)blockIdx.x * n;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, warps = kFilterThreads / 32;
+  int kept = 0, base = 0;  // base: number kept when the current batch started
+  const bool batched = n > batch;
+  for (int i = 0; i < n; ++i) {
+    if (batched && i % batch == 0) base = kept;
+    const int64_t row = my_ids[i];
+    if (threadIdx.x == 0) s_close = 0;
+    __syncthreads();
+    bool valid = row >= 0 && row < N;  // the reference skips items whose vector is missing
+    if (valid) {
+      const int start = filter_window_start(kept, base, batched, lookback);
+      const float* a = X + row * d;
+      for (int j = start + warp; j < kept; j += warps) {
+        const double dist = direct_distance(a, X + (int64_t)s_kept[j] * d, d, metric, lane);
+        if (lane == 0 && dist < threshold) s_close = 1;
+      }
+    }
+    __syncthreads();
+    const bool keep_it = valid && !s_close;
+    if (threadIdx.x == 0) {
+      my_keep[i] = keep_it ? 1 : 0;
+      if (keep_it) s_kept[kept] = (int)row;
+    }
+    if (keep_it) ++kept;
+    __syncthreads();
+  }
+}
+
+
+// ---------------------------------------------------------------- radius walk on device
+// voyager_manager.py:941-1367 (_execute_radius_walk) over the candidates _radius_walk_get_candidates (:842-938) leaves,
+// in one CTA.  The reference's steps and the state that restates each:
+//   * anchor distances (:927, get_direct_distance) in float64, one warp per candidate; the stable sort by that distance
+//     (:968) is a bitonic sort of (distance bits, input position) keys -- distances are >= 0 or +inf, so their bit
+//     patterns order like the values, and the position breaks ties the way a stable sort keeps them;
+//   * buckets of 50 in that order (:956, :970-974), walked one after the other until the playlist holds n songs (what
+//     the window-doubling loop at :1261-1281 amounts to);
+//   * the first song is sorted[0] (:1008-1013); its artist counts (:1041-1047) but not per bucket;
+//   * each bucket starts at its first unused candidate (:1091-1103; in bucket 0 that skips sorted[0]), accepted if it
+//     passes the artist rules and otherwise only dropped from the bucket (:1140-1163);
+//   * then greedily: score = 0.7 d(prev, cand) + 0.3 float32(d(anchor, cand)) (:1222), the first strict minimum in
+//     bucket order wins (:1223), prev is the last song APPENDED (:1174), and the bucket ends when no candidate passes;
+//   * the artist rules (:1120-1136, :1188-1211) apply when eliminate_duplicates and the cap is > 0: one song per artist
+//     per bucket, and an artist already in 2 buckets or at the cap is refused;
+//   * once the playlist holds n songs nothing later changes it (:1146, :1237, :1262), so the walk stops there;
+//   * _avoid_triple_adjacent (:1287-1318) on the final order.
+// Per-candidate state lives in global scratch (sort keys, per-artist counters, the playlist); only the distances from
+// the current song to the <= 50 candidates of the bucket are in shared memory.  Warp 0 keeps the books, every warp
+// computes distances.
+constexpr int kWalkThreads = 1024;
+constexpr int kWalkBucket = 50;    // BUCKET_SIZE, voyager_manager.py:956
+constexpr unsigned long long kWalkMissing = ~0ull;  // sort key of a candidate that is not in the index: after +inf
+
+__device__ __forceinline__ double walk_key_dist(unsigned long long k) { return __longlong_as_double((long long)k); }
+
+// artists[c] of input position c (-1: no artist); count / buckets / mark: per artist, the songs taken, the buckets it
+// has a song in, and the last bucket it took a song in
+__device__ __forceinline__ bool walk_artist_ok(int a, int bucket, int cap, const int* count, const int* buckets,
+                                               const int* mark) {
+  return a < 0 || !(mark[a] == bucket || buckets[a] >= 2 || count[a] >= cap);
+}
+
+__global__ void __launch_bounds__(kWalkThreads)
+radius_walk_kernel(const float* __restrict__ X, int64_t N, int d, int metric, const float* __restrict__ anchor,
+                   const int64_t* __restrict__ rows, const int32_t* __restrict__ artists, int n_cand, int n,
+                   int artist_rules, int cap, int64_t npad, unsigned long long* key, int* ord, int* count,
+                   int* buckets, int* mark, int* playlist, int32_t* __restrict__ out_pos,
+                   double* __restrict__ out_dist, int32_t* __restrict__ out_count) {
+  __shared__ double s_dprev[kWalkBucket];
+  __shared__ unsigned long long s_elig;  // candidates of the bucket that may be taken next
+  __shared__ int s_valid, s_len, s_prev_pos;  // valid candidates, playlist length, input position of the last song
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, warps = kWalkThreads / 32;
+  if (threadIdx.x == 0) s_valid = 0;
+  __syncthreads();
+
+  // ---- anchor distances and sort keys (padding sorts after every candidate)
+  for (int64_t i = warp; i < npad; i += warps) {
+    unsigned long long k = kWalkMissing;
+    const int64_t row = i < n_cand ? rows[i] : -1;
+    if (row >= 0 && row < N) {
+      k = (unsigned long long)__double_as_longlong(direct_distance(X + row * d, anchor, d, metric, lane));
+      if (lane == 0) atomicAdd(&s_valid, 1);
+    }
+    if (lane == 0) {
+      key[i] = k;
+      ord[i] = (int)i;
+    }
+  }
+  __syncthreads();
+  // ---- bitonic sort of (key, position) ascending
+  for (int64_t kk = 2; kk <= npad; kk <<= 1) {
+    for (int64_t j = kk >> 1; j > 0; j >>= 1) {
+      for (int64_t i = threadIdx.x; i < npad; i += kWalkThreads) {
+        const int64_t l = i ^ j;
+        if (l > i) {
+          const unsigned long long ki = key[i], kl = key[l];
+          const int oi = ord[i], ol = ord[l];
+          const bool i_after = ki > kl || (ki == kl && oi > ol);
+          if (i_after == ((i & kk) == 0)) {
+            key[i] = kl;
+            key[l] = ki;
+            ord[i] = ol;
+            ord[l] = oi;
+          }
+        }
+      }
+      __syncthreads();
+    }
+  }
+
+  // ---- the walk; sorted index s -> input position ord[s], anchor distance key[s]
+  const int m = s_valid;
+  if (threadIdx.x == 0) {
+    s_len = 0;
+    if (m > 0 && n > 0) {  // the first song (:1008-1013, :1041-1047)
+      playlist[0] = 0;
+      s_len = 1;
+      s_prev_pos = ord[0];
+      const int a = artists[ord[0]];
+      if (a >= 0) count[a] += 1;
+    }
+  }
+  __syncthreads();
+  for (int b = 0;; ++b) {
+    const bool go = (int64_t)b * kWalkBucket < m && s_len < n;  // read by every thread before warp 0 writes again
+    __syncthreads();
+    if (!go) break;
+    const int base = b * kWalkBucket, nb = min(kWalkBucket, m - base);
+    // warp 0's books for this bucket: candidates still available, playlist length, the artist of each lane's two
+    // candidates (j = lane, lane + 32)
+    unsigned long long avail = ((1ull << nb) - 1) & ~(b == 0 ? 1ull : 0ull);  // bucket 0 holds the first song
+    int len = 0, art[2] = {-1, -1};
+    // the candidates that may be taken next (a warp-wide ballot)
+    auto eligible = [&]() {
+      unsigned long long e = 0;
+      for (int h = 0; h < 2; ++h) {
+        const int j = lane + 32 * h;
+        const bool ok = j < nb && ((avail >> j) & 1) &&
+                        (!artist_rules || walk_artist_ok(art[h], b, cap, count, buckets, mark));
+        e |= (unsigned long long)__ballot_sync(0xffffffffu, ok) << (32 * h);
+      }
+      return e;
+    };
+    // take sorted index base + j (the bookkeeping of :1141-1161 / :1232-1253); lane 0 writes, the warp reads back
+    auto accept = [&](int j) {
+      avail &= ~(1ull << j);
+      if (lane == 0) {
+        if (len < n) {
+          playlist[len] = base + j;
+          s_prev_pos = ord[base + j];
+        }
+        const int a = artists[ord[base + j]];
+        if (a >= 0) {
+          count[a] += 1;
+          if (mark[a] != b) {
+            mark[a] = b;
+            buckets[a] += 1;
+          }
+        }
+      }
+      if (len < n) ++len;
+      __syncwarp();
+    };
+    if (warp == 0) {
+      len = s_len;
+      for (int h = 0; h < 2; ++h) {
+        const int j = lane + 32 * h;
+        if (j < nb) art[h] = artists[ord[base + j]];
+      }
+      if (avail) {  // the start (:1105-1163): the first available candidate, taken if the artist rules allow it
+        const int start = __ffsll((long long)avail) - 1;
+        if ((eligible() >> start) & 1) accept(start);
+        else avail &= ~(1ull << start);
+      }
+      const unsigned long long e = len < n ? eligible() : 0ull;
+      if (lane == 0) {
+        s_len = len;
+        s_elig = e;
+      }
+    }
+    // greedy steps (:1166-1253): every warp computes d(prev, cand) for the eligible candidates, warp 0 picks
+    for (;;) {
+      __syncthreads();  // s_elig / s_prev_pos published
+      const unsigned long long e = s_elig;
+      if (e == 0) break;
+      const float* prev = X + rows[s_prev_pos] * d;
+      for (int j = warp; j < nb; j += warps)
+        if ((e >> j) & 1) {
+          const double dist = direct_distance(X + rows[ord[base + j]] * d, prev, d, metric, lane);
+          if (lane == 0) s_dprev[j] = dist;
+        }
+      __syncthreads();  // distances ready
+      if (warp == 0) {
+        double best = INFINITY;  // a score must be strictly below +inf and below every earlier one (:1179, :1223)
+        int best_j = INT_MAX;
+        for (int h = 0; h < 2; ++h) {
+          const int j = lane + 32 * h;
+          if (j < nb && ((e >> j) & 1)) {
+            const double a32 = (double)(float)walk_key_dist(key[base + j]);  // the bucket's float32 array (:983)
+            const double score = __dadd_rn(__dmul_rn(0.7, s_dprev[j]), __dmul_rn(0.3, a32));
+            if (score < best) {
+              best = score;
+              best_j = j;
+            }
+          }
+        }
+        for (int o = 16; o > 0; o >>= 1) {  // the first minimum in bucket order
+          const double ob = __shfl_xor_sync(0xffffffffu, best, o);
+          const int oj = __shfl_xor_sync(0xffffffffu, best_j, o);
+          if (ob < best || (ob == best && oj < best_j)) {
+            best = ob;
+            best_j = oj;
+          }
+        }
+        unsigned long long next = 0;
+        if (best_j != INT_MAX) {
+          accept(best_j);
+          if (len < n) next = eligible();
+        }
+        if (lane == 0) {
+          s_len = len;
+          s_elig = next;
+        }
+      }
+    }
+  }
+
+  // ---- _avoid_triple_adjacent (:1287-1318) on the playlist, then the outputs
+  const int L = s_len;
+  if (threadIdx.x == 0) {
+    auto author = [&](int t) { return artists[ord[playlist[t]]]; };
+    int i = 0;
+    while (i <= L - 3) {
+      const int a1 = author(i);
+      if (a1 >= 0 && a1 == author(i + 1) && a1 == author(i + 2)) {
+        int j = i + 3;
+        while (j < L && author(j) == a1) ++j;
+        if (j < L) {  // swap the third with the first later song by another artist, then look at i again
+          const int t = playlist[i + 2];
+          playlist[i + 2] = playlist[j];
+          playlist[j] = t;
+          continue;
+        }
+      }
+      ++i;
+    }
+    *out_count = L;
+  }
+  __syncthreads();
+  for (int t = threadIdx.x; t < L; t += kWalkThreads) {
+    out_pos[t] = ord[playlist[t]];
+    out_dist[t] = walk_key_dist(key[playlist[t]]);
+  }
+}
+
+
+// ---------------------------------------------------------------- song path walk on device
+// path_manager.py:180-317 (_find_best_songs_for_job) over the chain find_nearest_neighbors_by_vector
+// (voyager_manager.py:1547-1657) runs on each job's k-NN prefix, for a sequence of jobs, in one CTA.  One pass over a
+// job's candidates in k-NN order does every stage, because each stage only looks at what came before it:
+//   * _filter_by_distance (:526-617): the item is compared with the kept window (filter_window_start) in the
+//     VOYAGER_METRIC distance; with no lookback the list is unchanged;
+//   * same-song dedupe (:1625-1636): an item without details, or whose signature this job already let through, is out;
+//   * the raw-author cap (:1638-1653, only when eliminate_duplicates and the cap is > 0; falsy authors are out);
+//   * [:n]: the pass ends after the n-th item that got this far;
+//   * acceptance (path_manager.py:211-291): used rows and signatures, the normalised-author cap, then the lookbacks
+//     against the path's last songs and this job's found songs, in PATH_DISTANCE_METRIC; the job ends once it has
+//     its songs.  A job that falls short gives back what it took (:294-312).
+// Per candidate, every warp computes the distances the decision may need (filter window, path window, found window)
+// and the threads look for the row among the used rows; then thread 0 decides and keeps the books.
+constexpr int kPathThreads = 512;
+
+// get_distance (path_manager.py:27-52): euclidean ||a - b||, angular arccos(clip(cos)) / pi (+inf when either row is
+// zero).  cos = 1 - (1 - cos) is exact for cos >= 0.5, which covers every distance below the thresholds.
+__device__ __forceinline__ double path_distance(const float* a, const float* b, int d, int metric, int lane) {
+  const double dd = direct_distance(a, b, d, metric, lane);
+  if (metric == kMetricL2 || dd == INFINITY) return dd;
+  return acos(1.0 - dd) / CUDART_PI;
+}
+
+struct SongPathArgs {
+  const float* X;
+  int64_t N;
+  int d;
+  int n_jobs;
+  const int32_t* job_off;     // [n_jobs + 1] candidate ranges
+  const int32_t* job_n;       // [n_jobs] the by-vector n (k_search)
+  const int32_t* job_need;    // [n_jobs] num_to_find
+  const int64_t* cand_row;    // [n_cand] stored row, -1: no vector
+  const int32_t* cand_sig;    // (title, author) signature key, -1: no details
+  const int32_t* cand_author; // normalised author key
+  const int32_t* cand_raw;    // raw author key, -1: falsy author
+  int64_t* used_row;          // [n_used + sum(need)] in / out
+  int32_t* n_used;
+  unsigned char* used_sig;    // [n_sig] in / out
+  int32_t* author_count;      // [n_author] in / out
+  int64_t* path_row;          // [n_path + sum(need)] in / out: the start song first
+  int32_t* n_path;
+  int64_t end_row;
+  am_song_path_cfg cfg;
+  int32_t* seen;              // [n_sig] scratch: the job that last let the signature through, -1 initially
+  int32_t* raw_mark;          // [n_raw] scratch: the job that last counted the raw author, -1 initially
+  int32_t* raw_count;         // [n_raw] scratch
+  int32_t* kept;              // [2 x max candidates per job] scratch: the filter's kept positions, then the job's found
+  int32_t* out_found;         // [n_jobs]
+  int32_t* out_pos;           // [sum(need)] accepted candidates, in path order
+  int32_t* out_failed;        // first failed job when stopping on failure, else -1
+  double* out_dist;           // [n_path + sum(need)] distances between consecutive songs of the path and the end song
+};
+
+__global__ void __launch_bounds__(kPathThreads) song_path_kernel(const SongPathArgs a) {
+  __shared__ int s_close;      // bit 0: filter window, bit 1: path window, bit 2: found window
+  __shared__ int s_used, s_stop;
+  __shared__ int s_kept, s_batch_kept, s_found, s_prod, s_n_used, s_n_path, s_n_out;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, warps = kPathThreads / 32;
+  const am_song_path_cfg& c = a.cfg;
+  const int lb_f = c.filter_lookback, lb_p = c.path_lookback;
+  for (int j = tid; j < a.n_jobs; j += kPathThreads) a.out_found[j] = 0;  // jobs after a stop are not run
+  if (tid == 0) {
+    s_n_used = *a.n_used;
+    s_n_path = *a.n_path;
+    s_n_out = 0;
+    *a.out_failed = -1;
+  }
+  __syncthreads();
+  for (int j = 0; j < a.n_jobs; ++j) {
+    const int base = a.job_off[j], m = a.job_off[j + 1] - base, n = a.job_n[j], need = a.job_need[j];
+    const bool batched = m > c.filter_batch;
+    if (tid == 0) {
+      s_kept = s_batch_kept = s_found = s_prod = s_stop = 0;
+    }
+    const int used0 = s_n_used;  // the rows this job adds are given back by truncation
+    __syncthreads();
+    int found_all = 0;  // thread 0: songs found so far
+    for (int i = 0; i < m; ++i) {
+      const int64_t row = a.cand_row[base + i];
+      const bool valid = row >= 0 && row < a.N;
+      if (tid == 0) {
+        s_close = 0;
+        s_used = 0;
+        if (batched && i % c.filter_batch == 0) s_batch_kept = s_kept;
+      }
+      __syncthreads();
+      if (valid) {
+        const int kept = s_kept, found = s_found, np = s_n_path;
+        const int f0 = lb_f > 0 ? filter_window_start(kept, s_batch_kept, batched, lb_f) : kept;
+        const int nf = kept - f0, npw = min(lb_p, np), nq = min(lb_p, found);
+        const float* x = a.X + row * a.d;
+        for (int t = warp; t < nf + npw + nq; t += warps) {
+          int64_t other;
+          int metric, bit;
+          double thr;
+          if (t < nf) {
+            other = a.cand_row[base + a.kept[f0 + t]];
+            metric = c.voyager_metric;
+            thr = c.filter_threshold;
+            bit = 1;
+          } else if (t < nf + npw) {
+            other = a.path_row[np - npw + (t - nf)];
+            metric = c.path_metric;
+            thr = c.path_threshold;
+            bit = 2;
+          } else {
+            other = a.cand_row[base + a.kept[m + found - nq + (t - nf - npw)]];
+            metric = c.path_metric;
+            thr = c.path_threshold;
+            bit = 4;
+          }
+          const float* y = a.X + other * a.d;
+          const double dist = bit == 1 ? direct_distance(x, y, a.d, metric, lane) : path_distance(x, y, a.d, metric, lane);
+          if (lane == 0 && dist < thr) atomicOr(&s_close, bit);
+        }
+      }
+      for (int t = tid; t < s_n_used; t += kPathThreads)
+        if (a.used_row[t] == row) s_used = 1;
+      __syncthreads();
+      if (tid == 0) {
+        const int close = s_close;
+        bool pass = true;
+        if (lb_f > 0) {  // _filter_by_distance: items without a vector are dropped, the kept ones form the window
+          pass = valid && !(close & 1);
+          if (pass) a.kept[s_kept++] = i;
+        }
+        const int sig = a.cand_sig[base + i];
+        if (pass && sig < 0) pass = false;
+        if (pass) {
+          if (a.seen[sig] == j) pass = false;
+          else a.seen[sig] = j;
+        }
+        if (pass && c.voyager_cap > 0) {
+          const int r = a.cand_raw[base + i];
+          if (r < 0) {
+            pass = false;
+          } else {
+            if (a.raw_mark[r] != j) {
+              a.raw_mark[r] = j;
+              a.raw_count[r] = 0;
+            }
+            if (a.raw_count[r] >= c.voyager_cap) pass = false;
+            else a.raw_count[r] += 1;
+          }
+        }
+        if (pass) {
+          s_prod += 1;
+          const int au = a.cand_author[base + i];
+          const bool ok = !s_used && !a.used_sig[sig] && !(c.path_cap > 0 && a.author_count[au] >= c.path_cap) && valid &&
+                          !(close & 2) && !(close & 4);
+          if (ok) {
+            ++found_all;
+            s_found = found_all;
+            a.used_row[s_n_used++] = row;
+            a.used_sig[sig] = 1;
+            a.author_count[au] += 1;
+            a.out_pos[s_n_out + found_all - 1] = base + i;
+            a.kept[m + found_all - 1] = i;  // the job's found list, behind the filter's (<= m entries each)
+          }
+          if (found_all >= need || s_prod >= n) s_stop = 1;
+        }
+      }
+      __syncthreads();
+      if (s_stop) break;
+    }
+    if (tid == 0) {
+      const int found = s_found;
+      if (found < need) {  // roll back (:294-312)
+        for (int t = 0; t < found; ++t) {
+          const int p = base + a.kept[m + t];
+          a.used_sig[a.cand_sig[p]] = 0;
+          int& cnt = a.author_count[a.cand_author[p]];
+          cnt = max(0, cnt - 1);
+        }
+        s_n_used = used0;
+        a.out_found[j] = 0;
+        if (c.stop_on_failure) {
+          *a.out_failed = j;
+          s_stop = 2;
+        }
+      } else {
+        for (int t = 0; t < found; ++t) a.path_row[s_n_path++] = a.cand_row[base + a.kept[m + t]];
+        s_n_out += found;
+        a.out_found[j] = found;
+      }
+    }
+    __syncthreads();
+    if (s_stop == 2) break;
+  }
+  // distances between consecutive songs of the path, the end song last
+  const int np = s_n_path;
+  for (int t = warp; t < np; t += warps) {
+    const int64_t r0 = a.path_row[t], r1 = t + 1 < np ? a.path_row[t + 1] : a.end_row;
+    const double dist = path_distance(a.X + r0 * a.d, a.X + r1 * a.d, a.d, c.path_metric, lane);
+    if (lane == 0) a.out_dist[t] = dist;
+  }
+  if (tid == 0) {
+    *a.n_used = s_n_used;
+    *a.n_path = np;
+  }
+}
+
+}  // namespace am
+
+using namespace am;
+
+extern "C" int am_knn_filter_by_distance(const am_index* idx, const int64_t* ids, int n_lists, int n, float threshold,
+                                         int lookback, int batch, unsigned char* keep) {
+  AM_CHECK(idx && (ids || n_lists * n == 0) && (keep || n_lists * n == 0), "am_knn_filter_by_distance: NULL argument");
+  AM_CHECK(n_lists >= 0 && n >= 0 && n <= kFilterCap, "am_knn_filter_by_distance: list length %d exceeds %d", n, kFilterCap);
+  AM_CHECK(batch > 0, "am_knn_filter_by_distance: batch must be positive");
+  if (n_lists == 0 || n == 0) return AM_OK;
+  if (lookback <= 0) {  // the reference returns the list unchanged
+    std::memset(keep, 1, (size_t)n_lists * n);
+    return AM_OK;
+  }
+  cudaStream_t st;
+  AM_TRY(HostCall::thread_stream(&st));
+  HostCall call(st, kStageLimit);
+  int64_t* d_ids;
+  unsigned char* d_keep;
+  call.up(&d_ids, ids, (size_t)n_lists * n);
+  call.down(&d_keep, (size_t)n_lists * n, keep);
+  AM_TRY(call.start());
+  AM_LAUNCH(filter_by_distance_kernel, n_lists, kFilterThreads, 0, st, idx->X.p, idx->N, idx->d, idx->metric, d_ids, n,
+            (double)threshold, lookback, batch, d_keep);
+  return call.finish();
+}
+
+extern "C" int am_knn_radius_walk(const am_index* idx, const float* anchor, const int64_t* rows, const int32_t* artists,
+                                  int n_cand, int n, int eliminate_duplicates, int max_songs_per_artist, int metric,
+                                  int32_t* out_pos, double* out_dist, int32_t* out_count) {
+  AM_CHECK(idx && anchor && out_count && (n_cand == 0 || (rows && artists)) && (n == 0 || (out_pos && out_dist)),
+           "am_knn_radius_walk: NULL argument");
+  AM_CHECK(n_cand >= 0 && n >= 0, "am_knn_radius_walk: negative size (n_cand = %d, n = %d)", n_cand, n);
+  AM_CHECK(metric == kMetricCos || metric == kMetricL2, "am_knn_radius_walk: metric %d is not 0 (angular) or 1 (euclidean)",
+           metric);
+  *out_count = 0;
+  if (n_cand == 0 || n == 0) return AM_OK;
+  int n_art = 0;
+  for (int i = 0; i < n_cand; ++i) {
+    AM_CHECK(artists[i] >= -1, "am_knn_radius_walk: artist id %d at %d is below -1", artists[i], i);
+    n_art = std::max(n_art, artists[i] + 1);
+  }
+  int64_t npad = 1;
+  while (npad < n_cand) npad <<= 1;
+  const int n_out = std::min(n, n_cand);
+  cudaStream_t st;
+  AM_TRY(HostCall::thread_stream(&st));
+  HostCall call(st, HostCall::kAlways);
+  float* d_anchor;
+  int64_t* d_rows;
+  int32_t *d_art, *d_cnt, *d_pos;
+  double* d_dist;
+  unsigned long long* d_key;
+  int *d_ord, *d_count, *d_buckets, *d_mark, *d_playlist;
+  call.up(&d_anchor, anchor, (size_t)idx->d);
+  call.up(&d_rows, rows, (size_t)n_cand);
+  call.up(&d_art, artists, (size_t)n_cand);
+  call.down(&d_cnt, 1);
+  call.down(&d_pos, (size_t)n_out);
+  call.down(&d_dist, (size_t)n_out);
+  call.device(&d_key, (size_t)npad);
+  call.device(&d_ord, (size_t)npad);
+  call.device(&d_count, (size_t)n_art, 0);
+  call.device(&d_buckets, (size_t)n_art, 0);
+  call.device(&d_mark, (size_t)n_art, 0xff);  // -1: no bucket yet
+  call.device(&d_playlist, (size_t)n_out);
+  AM_TRY(call.start());
+  const int rules = eliminate_duplicates && max_songs_per_artist > 0;
+  AM_LAUNCH(radius_walk_kernel, 1, kWalkThreads, 0, st, idx->X.p, idx->N, idx->d, metric, d_anchor, d_rows, d_art,
+            n_cand, n_out, rules, max_songs_per_artist, npad, d_key, d_ord, d_count, d_buckets, d_mark, d_playlist, d_pos,
+            d_dist, d_cnt);
+  AM_TRY(call.finish());
+  const int32_t cnt = *call.mirror(d_cnt);
+  call.get(out_pos, d_pos, (size_t)cnt);
+  call.get(out_dist, d_dist, (size_t)cnt);
+  *out_count = cnt;
+  return AM_OK;
+}
+
+extern "C" int am_knn_song_path(const am_index* idx, const am_song_path_cfg* cfg, int n_jobs, const int32_t* job_off,
+                                const int32_t* job_n, const int32_t* job_need, const int64_t* cand_rows,
+                                const int32_t* cand_sig, const int32_t* cand_author, const int32_t* cand_author_raw,
+                                int n_sig, int n_author, int64_t* used_rows, int32_t* n_used, unsigned char* used_sig,
+                                int32_t* author_count, int64_t* path_rows, int32_t* n_path, int64_t end_row,
+                                int32_t* out_found, int32_t* out_pos, int32_t* out_failed, double* out_dist) {
+  AM_CHECK(idx && cfg && n_used && n_path && out_failed && (n_jobs == 0 || (job_off && job_n && job_need && out_found)),
+           "am_knn_song_path: NULL argument");
+  AM_CHECK(n_jobs >= 0 && n_sig >= 0 && n_author >= 0 && *n_used >= 0 && *n_path >= 1,
+           "am_knn_song_path: negative size, or no start song in the path");
+  AM_CHECK(cfg->voyager_metric == kMetricCos || cfg->voyager_metric == kMetricL2, "am_knn_song_path: voyager_metric %d",
+           cfg->voyager_metric);
+  AM_CHECK(cfg->path_metric == kMetricCos || cfg->path_metric == kMetricL2, "am_knn_song_path: path_metric %d",
+           cfg->path_metric);
+  AM_CHECK(cfg->filter_batch > 0, "am_knn_song_path: filter_batch must be positive");
+  AM_CHECK(end_row >= 0 && end_row < idx->N, "am_knn_song_path: end row %lld out of range", (long long)end_row);
+  AM_CHECK(n_jobs == 0 || job_off[0] == 0, "am_knn_song_path: job_off[0] must be 0");
+  int64_t total_need = 0;
+  int max_m = 0;
+  for (int j = 0; j < n_jobs; ++j) {
+    AM_CHECK(job_off[j + 1] >= job_off[j] && job_n[j] >= 1 && job_need[j] >= 1,
+             "am_knn_song_path: job %d: bad range, n or num_to_find", j);
+    total_need += job_need[j];
+    max_m = std::max(max_m, job_off[j + 1] - job_off[j]);
+  }
+  const int n_cand = n_jobs ? job_off[n_jobs] : 0;
+  AM_CHECK(n_cand == 0 || (cand_rows && cand_sig && cand_author && cand_author_raw), "am_knn_song_path: NULL candidates");
+  AM_CHECK(total_need == 0 || out_pos, "am_knn_song_path: NULL out_pos");
+  int n_raw = 0;
+  for (int i = 0; i < n_cand; ++i) {
+    AM_CHECK(cand_sig[i] >= -1 && cand_sig[i] < n_sig && cand_author[i] >= 0 && cand_author[i] < n_author &&
+                 cand_author_raw[i] >= -1,
+             "am_knn_song_path: candidate %d has a key out of range", i);
+    n_raw = std::max(n_raw, cand_author_raw[i] + 1);
+  }
+  const int nu = *n_used, np = *n_path;
+  for (int t = 0; t < np; ++t)
+    AM_CHECK(path_rows[t] >= 0 && path_rows[t] < idx->N, "am_knn_song_path: path row %d out of range", t);
+  const int64_t cap_used = nu + total_need, cap_path = np + total_need;
+  cudaStream_t st;
+  AM_TRY(HostCall::thread_stream(&st));
+  HostCall call(st, HostCall::kAlways);
+  SongPathArgs a{idx->X.p, idx->N, idx->d, n_jobs};
+  a.end_row = end_row;
+  a.cfg = *cfg;
+  int32_t* d_hdr;  // n_used, n_path, failed
+  const int32_t hdr[4] = {nu, np, -1, 0};
+  call.up(&a.job_off, job_off, n_jobs ? (size_t)n_jobs + 1 : 0);
+  call.up(&a.job_n, job_n, (size_t)n_jobs);
+  call.up(&a.job_need, job_need, (size_t)n_jobs);
+  call.up(&a.cand_row, cand_rows, (size_t)n_cand);
+  call.up(&a.cand_sig, cand_sig, (size_t)n_cand);
+  call.up(&a.cand_author, cand_author, (size_t)n_cand);
+  call.up(&a.cand_raw, cand_author_raw, (size_t)n_cand);
+  call.both(&d_hdr, hdr, 4, 4);
+  call.both(&a.used_row, used_rows, (size_t)nu, (size_t)cap_used);
+  call.both(&a.path_row, path_rows, (size_t)np, (size_t)cap_path);
+  call.both(&a.author_count, author_count, (size_t)n_author, (size_t)n_author, author_count);
+  call.both(&a.used_sig, used_sig, (size_t)n_sig, (size_t)n_sig, used_sig);
+  call.down(&a.out_found, (size_t)n_jobs, out_found);
+  call.down(&a.out_pos, (size_t)total_need);
+  call.down(&a.out_dist, (size_t)cap_path);
+  call.device(&a.seen, (size_t)n_sig, 0xff);  // -1: no job let the signature through yet
+  call.device(&a.raw_mark, (size_t)n_raw, 0xff);
+  call.device(&a.raw_count, (size_t)n_raw);
+  call.device(&a.kept, (size_t)2 * max_m);
+  AM_TRY(call.start());
+  a.n_used = d_hdr;
+  a.n_path = d_hdr + 1;
+  a.out_failed = d_hdr + 2;
+  AM_LAUNCH(song_path_kernel, 1, kPathThreads, 0, st, a);
+  AM_TRY(call.finish());
+  const int32_t* out_hdr = call.mirror(d_hdr);
+  int64_t taken = 0;
+  for (int j = 0; j < n_jobs; ++j) taken += out_found[j];
+  AM_CHECK(out_hdr[0] >= nu && out_hdr[0] <= cap_used && out_hdr[1] >= np && out_hdr[1] <= cap_path && taken <= total_need,
+           "am_knn_song_path: inconsistent result (used %d of %lld, path %d of %lld, taken %lld of %lld)", out_hdr[0],
+           (long long)cap_used, out_hdr[1], (long long)cap_path, (long long)taken, (long long)total_need);
+  *n_used = out_hdr[0];
+  *n_path = out_hdr[1];
+  *out_failed = out_hdr[2];
+  call.get(out_pos, a.out_pos, (size_t)taken);
+  call.get(used_rows, a.used_row, (size_t)out_hdr[0]);
+  call.get(path_rows, a.path_row, (size_t)out_hdr[1]);
+  call.get(out_dist, a.out_dist, (size_t)out_hdr[1]);
+  return AM_OK;
+}

@@ -89,8 +89,7 @@ class Index:
                 raise ValueError("ids and vectors differ in length")
             fresh = np.ones(len(v), dtype=bool)
             if start and ids is not None:
-                for a, i in enumerate(new_ids):
-                    row = self._lookup(int(i))
+                for a, row in enumerate(self._rows_of(new_ids, strict=False)):
                     if row >= 0:
                         self._rows[row] = v[a]
                         fresh[a] = False
@@ -182,20 +181,24 @@ class Index:
     def ids(self):
         return [int(i) for i in self._ids]
 
-    def _lookup(self, id: int) -> int:
-        """row of `id`, or -1: O(1) (identity ids, else a dict kept beside the id array)"""
-        if self._identity_ids:
-            return id if 0 <= id < len(self._ids) else -1
-        return self._id_to_row.get(id, -1)
-
     def __contains__(self, id):
-        return self._lookup(int(id)) >= 0
+        return self._rows_of([id], strict=False)[0] >= 0
+
+    def _rows_of(self, ids, strict: bool) -> np.ndarray:
+        """i64 rows of `ids` (any shape): a range test for identity ids, else one pass over the id dict.  An id that is
+        not in the index raises KeyError when `strict`, and becomes -1 otherwise."""
+        a = np.asarray(ids, dtype=np.int64)
+        if self._identity_ids:
+            rows = np.where((a >= 0) & (a < len(self._ids)), a, -1)
+        else:
+            get = self._id_to_row.get
+            rows = np.fromiter((get(int(i), -1) for i in a.ravel()), dtype=np.int64, count=a.size).reshape(a.shape)
+        if strict and (rows < 0).any():
+            raise KeyError(f"id {int(a.ravel()[np.argmax(rows.ravel() < 0)])} not in index")
+        return rows
 
     def _row_of(self, id) -> int:
-        row = self._lookup(int(id))
-        if row < 0:
-            raise KeyError(f"id {int(id)} not in index")
-        return row
+        return int(self._rows_of([id], strict=True)[0])
 
     def get_vector(self, id) -> np.ndarray:
         """The STORED vector: unit-normalised for Space.Cosine, like voyager.  One row gathered on the device and
@@ -204,26 +207,11 @@ class Index:
 
     def get_vectors(self, ids) -> np.ndarray:
         """Stored vectors of several ids: one device gather + one copy (no host mirror of the library)."""
-        rows = np.array([self._row_of(i) for i in ids], dtype=np.int64)
+        rows = self._rows_of(ids, strict=True)
         out = np.empty((len(rows), self.num_dimensions), dtype=np.float32)
         if len(rows):
             h = self._ensure_built()
             _lib.check(_lib.load().am_knn_get_vectors(h, _lib.ptr(rows), len(rows), _lib.ptr(out)))
-        return out
-
-    def pairwise_distances(self, ids) -> np.ndarray:
-        """f32[n, n] direct distances (voyager_manager.get_direct_distance for this index's metric: cosine / inner
-        product 1 - cos, euclidean ||a - b||) between the stored vectors of `ids`; +inf for unknown ids."""
-        rows = np.empty((len(ids),), dtype=np.int64)
-        for a, i in enumerate(ids):
-            try:
-                rows[a] = self._row_of(i)
-            except Exception:
-                rows[a] = -1
-        out = np.empty((len(rows), len(rows)), dtype=np.float32)
-        if len(rows):
-            h = self._ensure_built()
-            _lib.check(_lib.load().am_knn_pairwise(h, _lib.ptr(rows), len(rows), _lib.ptr(out)))
         return out
 
     # ------------------------------------------------------------------ query
@@ -262,13 +250,7 @@ class Index:
         arr = np.asarray(ids)
         single = arr.ndim == 1
         lists = arr[np.newaxis, :] if single else arr
-        rows = np.full(lists.shape, -1, dtype=np.int64)
-        for a in range(lists.shape[0]):
-            for b in range(lists.shape[1]):
-                try:
-                    rows[a, b] = self._row_of(int(lists[a, b]))
-                except Exception:
-                    rows[a, b] = -1
+        rows = self._rows_of(lists, strict=False)
         keep = np.zeros(lists.shape, dtype=np.uint8)
         if lists.size:
             h = self._ensure_built()
@@ -289,7 +271,7 @@ class Index:
         a = np.ascontiguousarray(anchor, dtype=np.float32).reshape(-1)
         if a.shape[0] != self.num_dimensions:
             raise ValueError(f"anchor must have dimension {self.num_dimensions}, got {a.shape}")
-        rows = np.array([self._lookup(int(i)) for i in ids], dtype=np.int64)
+        rows = self._rows_of(ids, strict=False)
         art = np.ascontiguousarray(artists, dtype=np.int32)
         if art.shape != rows.shape:
             raise ValueError("ids and artists differ in length")
@@ -321,7 +303,7 @@ class Index:
         need = np.ascontiguousarray(job_need, dtype=np.int32)
         if off.shape != (n_jobs + 1,) or need.shape != (n_jobs,):
             raise ValueError("job_off / job_need do not match job_n")
-        rows = np.array([self._lookup(int(i)) for i in cand_ids], dtype=np.int64)
+        rows = self._rows_of(cand_ids, strict=False)
         keys = [np.ascontiguousarray(k, dtype=np.int32) for k in (cand_sig, cand_author, cand_author_raw)]
         if any(k.shape != rows.shape for k in keys) or (n_jobs and off[-1] != len(rows)):
             raise ValueError("candidate arrays differ in length")
@@ -329,9 +311,9 @@ class Index:
             raise ValueError("used_sig must be uint8 and author_count int32")
         total = int(need.sum())
         used = np.empty(len(used_ids) + total, dtype=np.int64)
-        used[:len(used_ids)] = [self._row_of(i) for i in used_ids]
+        used[:len(used_ids)] = self._rows_of(used_ids, strict=True)
         path = np.empty(len(path_ids) + total, dtype=np.int64)
-        path[:len(path_ids)] = [self._row_of(i) for i in path_ids]
+        path[:len(path_ids)] = self._rows_of(path_ids, strict=True)
         n_used, n_path, failed = C.c_int32(len(used_ids)), C.c_int32(len(path_ids)), C.c_int32(-1)
         found = np.zeros(max(n_jobs, 1), dtype=np.int32)
         pos = np.empty(max(total, 1), dtype=np.int32)

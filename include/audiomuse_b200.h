@@ -216,10 +216,6 @@ AM_API int am_knn_query_ex(const am_index* idx, const float* Q, int nq, int k, i
  * for the index metric (cosine / inner product: 1 - cos; euclidean: ||a - b||), in float64.  n <= 4096. */
 AM_API int am_knn_filter_by_distance(const am_index* idx, const int64_t* ids, int n_lists, int n, float threshold,
                                      int lookback, int batch, unsigned char* keep);
-/* Direct distances (voyager_manager.py:99-140, get_direct_distance for the index metric) between all pairs of
- * the n stored rows `ids`: out f32[n, n], symmetric; +inf where a row id is outside [0, N).  Serves the radius
- * walk / path scoring (voyager_manager.py:1166-1258) without per-candidate get_vector round trips.  n <= 8192. */
-AM_API int am_knn_pairwise(const am_index* idx, const int64_t* ids, int n, float* out);
 /* The similar-tracks radius walk, voyager_manager.py:941-1367 (_execute_radius_walk), in one call: anchor f32[d];
  * rows i64[n_cand] the candidates' stored rows in the order _radius_walk_get_candidates (:842-938) leaves them (-1 or
  * any row outside [0, N): not in the index, dropped like a missing vector at :920-921); artists i32[n_cand] a dense id

@@ -165,9 +165,8 @@ def test_filter_by_distance_euclidean_large_list():
 
 
 @pytest.mark.parametrize("space_name", ["Cosine", "Euclidean"])
-def test_pairwise_and_get_vectors(space_name, golden_dir):
-    """am_knn_pairwise = the reference's get_direct_distance on every pair (oracle restatement pinned by
-    knn_distance_golden.json); am_knn_get_vectors = the stored rows."""
+def test_get_vectors(space_name):
+    """am_knn_get_vectors and am_knn_get_vector = the stored rows."""
     from audiomuse_ai_b200 import voyager_compat as vc
     rng = np.random.default_rng(9)
     x = rng.standard_normal((500, 200)).astype(np.float32)
@@ -181,14 +180,6 @@ def test_pairwise_and_get_vectors(space_name, golden_dir):
     for j, i in enumerate(ids):   # the one-row C entry point
         _lib.check(_lib.load().am_knn_get_vector(idx._ensure_built(), ctypes.c_int64(idx._row_of(i)), _lib.ptr(one)))
         np.testing.assert_array_equal(one, stored[j])
-    dm = idx.pairwise_distances(ids + [10_000])
-    assert dm.shape == (38, 38) and np.isinf(dm[-1, :-1]).all() and np.isinf(dm[:-1, -1]).all()
-    fn = oknn.direct_euclidean_distance if space_name == "Euclidean" else oknn.direct_cosine_distance
-    for a in range(37):
-        for b in range(37):
-            want = fn(stored[a], stored[b])
-            assert abs(dm[a, b] - want) <= 2e-6 + 1e-6 * abs(want), (a, b, dm[a, b], want)
-    np.testing.assert_array_equal(dm, dm.T)
 
 
 def test_queries_are_reentrant_across_threads():

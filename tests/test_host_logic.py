@@ -75,6 +75,15 @@ def test_voyager_compat_host_side_contract(tmp_path):
     assert sorted(idx.ids) == sorted(list(range(100, 140)) + [300, 301, 302])
     with pytest.raises(KeyError):
         idx._row_of(9999)
+    # the vectorised lookup: -1 for a missing id, or KeyError naming the first missing id; any shape
+    ids = np.array([[300, 7, 100], [9999, 139, 302]], dtype=np.uint64)
+    np.testing.assert_array_equal(idx._rows_of(ids, strict=False), [[40, -1, 0], [-1, 39, 42]])
+    with pytest.raises(KeyError, match="id 7 not in index"):
+        idx._rows_of(ids, strict=True)
+    ident = vc.Index(vc.Space.Cosine, num_dimensions=16)
+    ident.add_items(x[:5])
+    np.testing.assert_array_equal(ident._rows_of([4, 5, -1, 0], strict=False), [4, -1, -1, 0])
+    assert ident._rows_of([], strict=True).shape == (0,)
     with pytest.raises(vc.RecallError):
         idx.query(x[0], k=44)
     p = tmp_path / "i.amix"

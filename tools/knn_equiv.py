@@ -8,8 +8,9 @@ selection (chunk maxima, row streaming, full sort) runs: cosine / euclidean / in
 64, 96, 200, 512 and 1000 (bf16 row pitch 64 to 1024); 1 to 4096 queries (the host API on both sides of its 2 MiB
 staging limit); k of 1, 50, 500, 600 and len(index); modes 0, 1 and 2.  Per call: ids, distances, and the kernels
 launched with their counts (am_profile_report, template arguments stripped).  Also am_knn_query_dev on a 20 000 x 200
-euclidean self-query as the spectral and UMAP graphs issue it, and the duplicate filter, pairwise distances,
-get_vectors and get_vector, and the radius walk under both metrics and artist rules.  A query with k > 4032 is answered by the full sort alone: its kernel list may differ
+euclidean self-query as the spectral and UMAP graphs issue it, and the duplicate filter, get_vectors and get_vector,
+the radius walk under both metrics and artist rules, and the song path on seeded jobs (_song_paths).  A query with
+k > 4032 is answered by the full sort alone: its kernel list may differ
 from the other build's by the scoring kernels only; get_vector's launches are not compared (it used to copy from a
 host mirror of the rows, and gathers its row on the device now).  Needs an H100."""
 import ctypes as C
@@ -49,6 +50,49 @@ def _data(N, d, seed):
     return x, q[rng.permutation(len(q))].astype(np.float32)
 
 
+def _song_paths(idx, x, lists, key):
+    """Index.song_path over seeded jobs on the k-NN lists `lists` (rows = ids): lists shorter and longer than the
+    filter batch, filter lookback 0 and 3, both caps off and on, stop_on_failure 0 and 1, both metrics.  The last job
+    asks for more songs than its list can give, so it fails and gives back what it took.  Every output is recorded,
+    with the in / out state arrays after the call."""
+    out = {}
+    rng = np.random.default_rng(len(x))
+    sizes = (30, 300, 12, 200, 45, 250)  # filter_batch 50: lists on both sides of it
+    cand = np.concatenate([lists[j % len(lists)][:m] for j, m in enumerate(sizes)]).astype(np.int64)
+    cand[rng.integers(0, len(cand), 5)] = len(x) + 3  # ids without a vector
+    off = np.concatenate([[0], np.cumsum(sizes)]).astype(np.int32)
+    job_n = np.array([m - m // 5 for m in sizes], np.int32)
+    need = np.array([3, 8, 2, 6, 4, 10_000], np.int32)
+    sig = np.where(cand % 53 == 0, -1, cand % 97).astype(np.int32)
+    author = (cand % 11).astype(np.int32)
+    raw = (cand % 13 - 1).astype(np.int32)
+    a, b = x[lists[0][:-1]].astype(np.float64), x[lists[0][1:]].astype(np.float64)
+    cos = (a * b).sum(1) / np.linalg.norm(a, axis=1) / np.linalg.norm(b, axis=1)
+    thr = {0: (np.quantile(1 - cos, 0.3), np.quantile(np.arccos(np.clip(cos, -1, 1)) / np.pi, 0.3)),
+           1: (np.quantile(np.linalg.norm(a - b, axis=1), 0.3),) * 2}
+    for metric in (0, 1):
+        for lookback in (0, 3):
+            for cap in (0, 2):
+                for stop in (0, 1):
+                    cfg = _lib.SongPathCfg(voyager_metric=metric, path_metric=metric, filter_lookback=lookback,
+                                           filter_batch=50, path_lookback=2, voyager_cap=cap, path_cap=cap,
+                                           stop_on_failure=stop, filter_threshold=float(thr[metric][0]),
+                                           path_threshold=float(thr[metric][1]))
+                    used_sig = np.zeros(97, np.uint8)
+                    used_sig[[5, 17]] = 1
+                    author_count = np.zeros(11, np.int32)
+                    author_count[3] = 2
+                    found, pos, failed, used, path, dist = idx.song_path(
+                        cfg, off, job_n, need, cand, sig, author, raw, [int(lists[1][0]), int(lists[2][1])], used_sig,
+                        author_count, [int(lists[0][0])], int(lists[3][-1]))
+                    k = f"{key}/song_path/m{metric}/lb{lookback}/cap{cap}/stop{stop}"
+                    out.update({k + "/found": found, k + "/pos": pos, k + "/failed": np.array([-1 if failed is None
+                                                                                                else failed]),
+                                k + "/used": np.array(used), k + "/path": np.array(path), k + "/dist": dist,
+                                k + "/used_sig": used_sig, k + "/author_count": author_count})
+    return out
+
+
 def _collect():
     out = {}
     _lib.profile_enable(True)
@@ -73,7 +117,6 @@ def _collect():
             for batch in (20, 50):
                 out[f"{sname}/N{N}/d{d}/filter/batch{batch}"] = idx.filter_by_distance(lists, thr, lookback=3, batch=batch)
             ids = [int(i) for i in lists[0][:40]]
-            out[f"{sname}/N{N}/d{d}/pairwise"] = idx.pairwise_distances(ids + [N + 7])
             out[f"{sname}/N{N}/d{d}/get_vectors"] = idx.get_vectors(ids)
             pool = [int(i) for i in out[f"{sname}/N{N}/d{d}/nq16/k500/mode0/ids"][0]] if N >= 500 else ids
             artists = [i % 7 - 1 for i in range(len(pool))]
@@ -82,6 +125,9 @@ def _collect():
                     pos, dist = idx.radius_walk(q[0], pool, artists, 200, ed, cap, metric)
                     out[f"{sname}/N{N}/d{d}/radius_walk/{metric}/ed{int(ed)}/cap{cap}/pos"] = pos
                     out[f"{sname}/N{N}/d{d}/radius_walk/{metric}/ed{int(ed)}/cap{cap}/dist"] = dist
+            if (N, d) == (2000, 200):
+                out.update(_song_paths(idx, x, out[f"{sname}/N{N}/d{d}/nq16/k500/mode0/ids"].astype(np.int64),
+                                       f"{sname}/N{N}/d{d}"))
             out[f"{sname}/N{N}/d{d}/other_kernels"] = _kernels()
             one = np.empty((5, d), np.float32)
             for j, i in enumerate(ids[:5]):
