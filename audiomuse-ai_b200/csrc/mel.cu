@@ -19,36 +19,7 @@
 
 #include <cmath>
 
-namespace am {
-
-constexpr int kNfft = 2048;
-constexpr int kNc = 1024;       // complex FFT length
-constexpr int kFramesPerCta = 16;
-constexpr int kWarps = 8;
-constexpr int kThreads = kWarps * 32;
-constexpr int kTrStride = 33;   // padded row stride of the per-warp transpose buffer
-
-struct MelTables {
-  float* window;      // [2048]
-  float2* fft_tw;     // [32*32]  fft_tw[k1*32 + n2] = W_1024^(n2*k1)
-  float2* post_tw;    // [1024]   W_2048^k
-  int* band_start;    // [n_mels] first FFT bin with non-zero weight
-  int* band_len;      // [n_mels]
-  int* band_off;      // [n_mels] offset into weights
-  float* weights;     // [nnz]
-};
-
-}  // namespace am
-
-struct am_mel_plan {
-  am_mel_cfg cfg;
-  int center = 1;    // 1: librosa center=True (reflect pad n_fft/2); 0: frame t starts at t * hop
-  int log_mode = 0;  // 0: 10 log10(max(1e-10, .)) (power_to_db); 1: log10(1 + 10000 .) (tasks/analysis.py:374)
-  am::MelTables t;
-  int max_bin;   // highest FFT bin with non-zero mel weight
-  int nnz;
-  am::DevBuf<char> storage;
-};
+#include "mel.cuh"
 
 namespace am {
 
@@ -93,85 +64,6 @@ int build_filterbank(const am_mel_cfg& c, std::vector<float>& w /* [n_mels * bin
     }
   }
   return AM_OK;
-}
-
-// ---------------------------------------------------------------- device: 32-point FFT
-// Only ever called with compile-time indices (fft32_stage's template arguments and unrolled loop counters), so every
-// call folds to a constant.
-__host__ __device__ constexpr float cos32(int i) {  // cos(2*pi*i/32), i in [0,16)
-  switch (i) {
-    case 0: return 1.0f;
-    case 1: return 0.98078528040323044913f;
-    case 2: return 0.92387953251128675613f;
-    case 3: return 0.83146961230254523708f;
-    case 4: return 0.70710678118654752440f;
-    case 5: return 0.55557023301960222474f;
-    case 6: return 0.38268343236508977173f;
-    case 7: return 0.19509032201612826785f;
-    case 8: return 0.0f;
-    case 9: return -0.19509032201612826785f;
-    case 10: return -0.38268343236508977173f;
-    case 11: return -0.55557023301960222474f;
-    case 12: return -0.70710678118654752440f;
-    case 13: return -0.83146961230254523708f;
-    case 14: return -0.92387953251128675613f;
-    default: return -0.98078528040323044913f;
-  }
-}
-// sin(2*pi*i/32) for i in [0,16): sin(x) = cos(x - pi/2) -> index i-8; cos is even.
-__host__ __device__ constexpr float sin32i(int i) { return cos32(i >= 8 ? i - 8 : 8 - i); }
-
-__host__ __device__ constexpr int rev5(int i) {
-  return ((i & 1) << 4) | ((i & 2) << 2) | (i & 4) | ((i & 8) >> 2) | ((i & 16) >> 4);
-}
-
-// One radix-2 decimation-in-frequency stage of butterfly span kHalf.  The stage is a template argument so that
-// every index and twiddle is a compile-time constant: with a runtime `half` loop nvcc kept the stage loop rolled,
-// put re/im in local memory and looked the twiddles up through an indirect branch.  Products that feed a later
-// addition are rounded on their own (__fmul_rn): straight-line code would otherwise let nvcc contract them into
-// FMAs and change the result in the last bits.
-template <int kHalf>
-__device__ __forceinline__ void fft32_stage(float (&re)[32], float (&im)[32]) {
-#pragma unroll
-  for (int base = 0; base < 32; base += 2 * kHalf) {
-#pragma unroll
-    for (int j = 0; j < kHalf; ++j) {
-      const int a = base + j, b = a + kHalf;
-      const float ar = re[a], ai = im[a], br = re[b], bi = im[b];
-      re[a] = ar + br;
-      im[a] = ai + bi;
-      const float dr = ar - br, di = ai - bi;
-      const int idx = j * (16 / kHalf);  // twiddle W_32^idx = cos - i sin
-      if (idx == 0) {
-        re[b] = dr;
-        im[b] = di;
-      } else if (idx == 8) {  // * (-i)
-        re[b] = di;
-        im[b] = -dr;
-      } else if (idx == 4) {  // * (1 - i)/sqrt2
-        re[b] = __fmul_rn(dr + di, 0.70710678118654752440f);
-        im[b] = __fmul_rn(di - dr, 0.70710678118654752440f);
-      } else if (idx == 12) {  // * (-1 - i)/sqrt2
-        re[b] = __fmul_rn(di - dr, 0.70710678118654752440f);
-        im[b] = __fmul_rn(-(dr + di), 0.70710678118654752440f);
-      } else {
-        const float c = cos32(idx), s = sin32i(idx);
-        re[b] = fmaf(dr, c, di * s);
-        im[b] = fmaf(di, c, -dr * s);
-      }
-    }
-  }
-}
-
-// In-place radix-2 decimation-in-frequency, forward (e^{-i...}).  Input natural order,
-// output bit-reversed: X[k] is left in element rev5(k).  Straight-line code; trivial
-// twiddles cost no multiplies.
-__device__ __forceinline__ void fft32(float (&re)[32], float (&im)[32]) {
-  fft32_stage<16>(re, im);
-  fft32_stage<8>(re, im);
-  fft32_stage<4>(re, im);
-  fft32_stage<2>(re, im);
-  fft32_stage<1>(re, im);
 }
 
 // ---------------------------------------------------------------- device: kernel
@@ -224,7 +116,7 @@ mel_kernel(const void* __restrict__ pcm, int n_samples, int hop, int T, int n_me
   const int nf = min(kFramesPerCta, T - t0);
   const long long seg_base = (long long)b * n_samples;
 
-  // ---- stage samples (reflect padding of n_fft/2 resolved here) and tables
+  // ---- stage samples (reflect or zero padding of n_fft/2 resolved here) and tables
   const int count = (nf - 1) * hop + frame_len;
   const int p0 = t0 * hop - (center ? frame_len / 2 : 0);  // index into the unpadded window of the first sample
   bool staged = false;
@@ -262,11 +154,18 @@ mel_kernel(const void* __restrict__ pcm, int n_samples, int hop, int T, int n_me
     }
   }
   if (!staged) {
-    for (int i = tid; i < count; i += kThreads) {
-      int src = p0 + i;
-      if (src < 0) src = -src;
-      if (src >= n_samples) src = 2 * (n_samples - 1) - src;
-      s_x[i] = load_sample<kI16>(pcm, seg_base + src);
+    if (center == 2) {
+      for (int i = tid; i < count; i += kThreads) {
+        const int src = p0 + i;
+        s_x[i] = (src >= 0 && src < n_samples) ? load_sample<kI16>(pcm, seg_base + src) : 0.f;
+      }
+    } else {
+      for (int i = tid; i < count; i += kThreads) {
+        int src = p0 + i;
+        if (src < 0) src = -src;
+        if (src >= n_samples) src = 2 * (n_samples - 1) - src;
+        s_x[i] = load_sample<kI16>(pcm, seg_base + src);
+      }
     }
   }
   for (int i = tid; i < kNfft - frame_len; i += kThreads) s_x[count + i] = 0.f;  // finite tail under the zero window
@@ -294,66 +193,7 @@ mel_kernel(const void* __restrict__ pcm, int n_samples, int hop, int T, int n_me
   const int n_band_iter = (n_mels + 31) >> 5;
 
   for (int f = warp; f < nf; f += kWarps) {
-    float re[32], im[32];
-    // ---- z[n] = x[2n]w[2n] + i x[2n+1]w[2n+1];  lane = n2, element n1 holds z[32*n1 + n2]
-    const float2* xf = reinterpret_cast<const float2*>(s_x + f * hop);
-    const float2* wf = reinterpret_cast<const float2*>(s_win);
-#pragma unroll
-    for (int n1 = 0; n1 < 32; ++n1) {
-      const float2 x = xf[32 * n1 + lane];
-      const float2 w = wf[32 * n1 + lane];
-      re[n1] = __fmul_rn(x.x, w.x);  // not contracted into the first butterflies
-      im[n1] = __fmul_rn(x.y, w.y);
-    }
-    fft32(re, im);  // element i = Y[k1 = rev5(i)] for this n2
-    // ---- twiddle W_1024^(n2*k1) and transpose to lane = k1, element = n2
-#pragma unroll
-    for (int i = 0; i < 32; ++i) {
-      const int k1 = rev5(i);
-      const float2 w = s_tw[k1 * 32 + lane];
-      const float r = re[i], q = im[i];
-      re[i] = fmaf(r, w.x, -q * w.y);
-      im[i] = fmaf(r, w.y, q * w.x);
-    }
-#pragma unroll
-    for (int i = 0; i < 32; ++i) tr[rev5(i) * kTrStride + lane] = re[i];
-    __syncwarp();
-#pragma unroll
-    for (int n2 = 0; n2 < 32; ++n2) re[n2] = tr[lane * kTrStride + n2];
-    __syncwarp();
-#pragma unroll
-    for (int i = 0; i < 32; ++i) tr[rev5(i) * kTrStride + lane] = im[i];
-    __syncwarp();
-#pragma unroll
-    for (int n2 = 0; n2 < 32; ++n2) im[n2] = tr[lane * kTrStride + n2];
-    __syncwarp();
-    fft32(re, im);  // element i = Z[k1 + 32*k2], k1 = lane, k2 = rev5(i)
-
-    // ---- real-FFT split + power:  X[k] = (Z[k]+Z*[N-k])/2 - (i/2) W_2048^k (Z[k]-Z*[N-k])
-    const int partner = (32 - lane) & 31;
-#pragma unroll
-    for (int i = 0; i < 32; ++i) {
-      const int k2 = rev5(i);
-      if (k2 < kK2) {  // compile time
-        float pr = __shfl_sync(0xffffffffu, re[31 - i], partner);
-        float pi = __shfl_sync(0xffffffffu, im[31 - i], partner);
-        if (lane == 0) {  // N-k = 32*(32-k2): same lane, element rev5((32-k2)&31)
-          pr = re[rev5((32 - k2) & 31)];
-          pi = im[rev5((32 - k2) & 31)];
-        }
-        const int k = lane + 32 * k2;
-        const float2 w = __ldg(&tb.post_tw[k]);  // (cos, -sin)
-        const float er = re[i] + pr, ei = im[i] - pi;
-        const float orr = re[i] - pr, oi = im[i] + pi;
-        const float xr = 0.5f * (er + fmaf(w.x, oi, w.y * orr));
-        const float xi = 0.5f * (ei - fmaf(w.x, orr, -w.y * oi));
-        tr[k] = fmaf(xr, xr, xi * xi);
-      }
-    }
-    if (max_bin >= kNc && lane == 0) {  // Nyquist bin: X[1024] = Re Z[0] - Im Z[0]
-      const float ny = re[0] - im[0];
-      tr[kNc] = ny * ny;
-    }
+    warp_power_spectrum<kK2>(s_x + f * hop, s_win, s_tw, tb.post_tw, tr, lane, max_bin >= kNc);
     __syncwarp();
 
     // ---- triangular mel filters (CSR), ascending-bin summation, then dB
@@ -513,9 +353,9 @@ extern "C" int am_mel_plan_create(const am_mel_cfg* cfg, am_mel_plan** out) {
 extern "C" void am_mel_plan_free(am_mel_plan* plan) { delete plan; }
 
 // same tables, other framing / compression: center = 0 (librosa center=False), log_mode = 1 (log10(1 + 10000 x)) is
-// the MusiCNN front end of tasks/analysis.py:371-375
+// the MusiCNN front end of tasks/analysis.py:371-375; center = 2 (zero padding) is onset_strength's melspectrogram
 extern "C" int am_mel_plan_create_ex(const am_mel_cfg* cfg, int center, int log_mode, am_mel_plan** out) {
-  AM_CHECK((center == 0 || center == 1) && (log_mode == 0 || log_mode == 1), "am_mel_plan_create_ex: bad mode");
+  AM_CHECK((center >= 0 && center <= 2) && (log_mode == 0 || log_mode == 1), "am_mel_plan_create_ex: bad mode");
   AM_TRY(am_mel_plan_create(cfg, out));
   (*out)->center = center;
   (*out)->log_mode = log_mode;
@@ -531,7 +371,8 @@ extern "C" int am_mel_batch_dev(const am_mel_plan* plan, const void* pcm_dev, in
                                 int n_samples, float* out_dev, void* stream) {
   AM_CHECK(plan && pcm_dev && out_dev, "am_mel_batch_dev: NULL argument");
   AM_CHECK(B >= 0, "am_mel_batch_dev: negative batch");
-  AM_CHECK(plan->center ? n_samples > plan->cfg.n_fft / 2 : n_samples >= plan->cfg.n_fft,
+  AM_CHECK(plan->center == 2 ? n_samples >= 1
+                             : (plan->center ? n_samples > plan->cfg.n_fft / 2 : n_samples >= plan->cfg.n_fft),
            "mel: window of %d samples is shorter than %s", n_samples, plan->center ? "the reflect pad" : "one frame");
   if (B == 0) return AM_OK;
   const am_mel_cfg& c = plan->cfg;
@@ -571,7 +412,8 @@ static int mel_batch_host(const void* pcm, int is_i16, int B, int n_samples, con
                           float* out, int center = 1, int log_mode = 0) {
   AM_CHECK(pcm && out, "am_mel_batch: NULL buffer");
   AM_TRY(validate_cfg(cfg));
-  AM_CHECK(B >= 0 && cfg && (center ? n_samples > cfg->n_fft / 2 : n_samples >= cfg->n_fft),
+  AM_CHECK(B >= 0 && cfg &&
+               (center == 2 ? n_samples >= 1 : (center ? n_samples > cfg->n_fft / 2 : n_samples >= cfg->n_fft)),
            "am_mel_batch: bad shape B=%d n_samples=%d", B, n_samples);
   if (B == 0) return AM_OK;
   am_mel_plan* plan = nullptr;
@@ -608,7 +450,7 @@ extern "C" int am_mel_batch_i16(const int16_t* pcm, int B, int n_samples, const 
 }
 extern "C" int am_mel_batch_ex(const float* pcm, int B, int n_samples, const am_mel_cfg* cfg, int center, int log_mode,
                                float* out) {
-  AM_CHECK((center == 0 || center == 1) && (log_mode == 0 || log_mode == 1), "am_mel_batch_ex: bad mode");
+  AM_CHECK((center >= 0 && center <= 2) && (log_mode == 0 || log_mode == 1), "am_mel_batch_ex: bad mode");
   return mel_batch_host(pcm, 0, B, n_samples, cfg, out, center, log_mode);
 }
 

@@ -122,7 +122,7 @@ METRIC_NAMES = ("silhouette_score", "davies_bouldin_score", "calinski_harabasz_s
 
 def apply(clap=None, voyager_manager=None, clustering=None, allow_sklearn_fallback: bool = True,
           clustering_helper=None, song_alchemy=None, app_map=None, artist_gmm_manager=None,
-          gaussian_mixture=None, radius_walk=None, path_manager=None, app_path=None) -> None:
+          gaussian_mixture=None, radius_walk=None, path_manager=None, app_path=None, analysis=None) -> None:
     """clap / voyager_manager / clustering / clustering_helper: the reference's already imported tasks.* modules (pass
     only the ones to patch).  allow_sklearn_fallback keeps the reference's contract that a failing GPU k-means silently
     falls back to scikit-learn (tasks/clustering_gpu.py:130-148); this repository's own tests run with it off so a
@@ -141,7 +141,14 @@ def apply(clap=None, voyager_manager=None, clustering=None, allow_sklearn_fallba
     voyager_manager= alone leaves the walk to the reference.  path_manager (the reference's tasks.path_manager) gets the
     device song path as find_path_between_songs (song_path.make_song_path, over the voyager_manager module whose
     functions path_manager imported); app_path binds that name when it is imported (app_path.py:5), so pass it too for
-    the Song Path endpoint to use it."""
+    the Song Path endpoint to use it.  analysis (the reference's tasks.analysis) gets track_features.LibrosaFacade as
+    its `librosa`: analyze_track's beat_track, rms and chroma_stft (:344-348) run on the device, every other librosa use
+    of the module goes to the librosa it imported; sys.modules["librosa"] is left alone."""
+    if analysis is not None:
+        from . import track_features
+
+        if not isinstance(analysis.librosa, track_features.LibrosaFacade):
+            analysis.librosa = track_features.LibrosaFacade(analysis.librosa)
     if clap is not None:
         from . import clap_analyzer as b200_clap
 

@@ -91,7 +91,8 @@ AM_API int am_mel_batch_dev(const am_mel_plan* plan, const void* pcm_dev, int pc
 /* Sibling front end on the same kernel (SURVEY 8(f) row 4): tasks/analysis.py:371-375 feeds MusiCNN with
  * librosa.feature.melspectrogram(sr=16000, n_fft=512, hop_length=256, n_mels=96, center=False, norm='slaney') and
  * log10(1 + 10000 x).  center: 1 = reflect pad n_fft/2 (T = 1 + n/hop), 0 = frame t starts at t*hop
- * (T = 1 + (n - n_fft)/hop); log_mode: 0 = 10 log10(max(1e-10, x)), 1 = log10(1 + 10000 x). */
+ * (T = 1 + (n - n_fft)/hop), 2 = zero pad n_fft/2 (librosa's pad_mode='constant', T = 1 + n/hop, any n >= 1);
+ * log_mode: 0 = 10 log10(max(1e-10, x)), 1 = log10(1 + 10000 x). */
 AM_API int am_mel_plan_create_ex(const am_mel_cfg* cfg, int center, int log_mode, am_mel_plan** out);
 AM_API int am_mel_num_frames_ex(const am_mel_cfg* cfg, int center, int n_samples);
 AM_API int am_mel_batch_ex(const float* pcm, int B, int n_samples, const am_mel_cfg* cfg, int center, int log_mode,
@@ -434,6 +435,36 @@ AM_API int am_gmm_full_fit(const double* X, int64_t N, int d, int K, int n_init,
                            double* covariances, double* precisions_cholesky, double* lower_bounds, int32_t* n_iter,
                            int32_t* converged, int32_t* best_init, int64_t* labels, int32_t* ill_defined, int32_t* kpp,
                            double* init_lower_bounds, int32_t* init_n_iter, int32_t* init_converged, float* phase_ms);
+
+/* ------------------------------------------------------------------ track features: tempo, energy, chroma
+ * The three librosa 0.11.0 calls of tasks/analysis.py:344-348 (analyze_track) for a batch of tracks:
+ * beat.beat_track(y, sr)'s tempo (beat positions are not computed), feature.rms(y) and feature.chroma_stft(y, sr), all
+ * with n_fft 2048, hop 512, periodic Hann, center=True and zero padding, so a track of n samples has T = 1 + n / 512
+ * frames.  oracle/track_features.py states every step in float64.  A plan per sample rate; the call is synchronous.
+ *   samples      f32, the tracks one after the other; offsets i64[n_tracks + 1] (offsets[0] = 0, every track >= 1
+ *                sample, every sample finite: AM_ERR_INVALID before any device work otherwise)
+ *   what         AM_TF_TEMPO | AM_TF_RMS | AM_TF_CHROMA: which outputs to compute (the others are not touched)
+ *   tempo        f64[n_tracks]: the tempo estimate in bpm, 0 when the onset envelope is all zero
+ *   rms          f32[sum T]: per-frame RMS, track i at frame offset F_i = sum_{j<i} T_j
+ *   chroma       f32[12 sum T]: track i's (12, T_i) row-major chromagram at 12 F_i
+ *   optional     (NULL: not returned) tuning f64[n_tracks] (the estimate_tuning result the filterbank used; with
+ *                AM_TF_CHROMA), onset_env f32[sum T] and tempogram f64[n_tracks, win] (the tempogram's mean over frames;
+ *                with AM_TF_TEMPO), histogram i32[n_tracks, 100] (pitch_tuning's residual counts) and threshold
+ *                f32[n_tracks] (the median peak magnitude; both with AM_TF_CHROMA)
+ * Bit-identical between calls, and a track's results do not depend on the other tracks of the batch.
+ * am_track_features_plan_info: win = floor(8 sr / 512) tempogram lags, piptrack's bins [kmin, kmax). */
+#define AM_TF_TEMPO 1
+#define AM_TF_RMS 2
+#define AM_TF_CHROMA 4
+#define AM_TRACK_FEATURES_MIN_SR 8000
+#define AM_TRACK_FEATURES_MAX_SR 48000
+typedef struct am_track_features_plan am_track_features_plan;
+AM_API int am_track_features_plan_create(int sr, am_track_features_plan** out);
+AM_API void am_track_features_plan_free(am_track_features_plan* plan);
+AM_API int am_track_features_plan_info(const am_track_features_plan* plan, int* win, int* kmin, int* kmax);
+AM_API int am_track_features(const am_track_features_plan* plan, const float* samples, const int64_t* offsets,
+                             int n_tracks, int what, double* tempo, float* rms, float* chroma, double* tuning,
+                             float* onset_env, double* tempogram, int32_t* histogram, float* threshold);
 
 #ifdef __cplusplus
 }
