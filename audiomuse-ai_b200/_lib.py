@@ -40,6 +40,16 @@ class SongPathCfg(C.Structure):
                 ("stop_on_failure", C.c_int), ("filter_threshold", C.c_double), ("path_threshold", C.c_double)]
 
 
+class AlchemyCfg(C.Structure):
+    """am_alchemy_cfg"""
+    _fields_ = [("voyager_metric", C.c_int), ("path_metric", C.c_int), ("filter_lookback", C.c_int),
+                ("filter_batch", C.c_int), ("voyager_cap", C.c_int), ("n", C.c_int), ("skip_chain", C.c_int),
+                ("filter_threshold", C.c_double), ("subtract_threshold", C.c_double)]
+
+
+ALCHEMY_MAX_N, ALCHEMY_MAX_CANDIDATES = 600, 3000   # AM_ALCHEMY_MAX_N, AM_ALCHEMY_MAX_CANDIDATES
+
+
 _vp, _i, _i64, _f, _u64, _sz = C.c_void_p, C.c_int, C.c_int64, C.c_float, C.c_uint64, C.c_size_t
 _P = C.POINTER
 
@@ -101,6 +111,8 @@ SIGNATURES = {
     "am_knn_radius_walk": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _vp, _P(C.c_int32)]),
     "am_knn_song_path": (_i, [_vp, _P(SongPathCfg), _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp, _P(C.c_int32), _vp,
                               _vp, _vp, _P(C.c_int32), _i64, _vp, _vp, _P(C.c_int32), _vp]),
+    "am_knn_alchemy": (_i, [_vp, _P(AlchemyCfg), _vp, _vp, _i, _vp, _vp, _vp, _i, _i, _vp, _P(C.c_int32), _vp, _vp, _vp,
+                            _vp, _vp]),
     "am_knn_get_vectors": (_i, [_vp, _vp, _i, _vp]),
     "am_knn_query_dev": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _vp]),
     "am_kmeans_fit": (_i, [_vp, _i64, _i, _i, _i, _i, _f, _u64, _vp, _vp, _vp, _P(_f), _P(_i)]),

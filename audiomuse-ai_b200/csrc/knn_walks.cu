@@ -309,14 +309,61 @@ radius_walk_kernel(const float* __restrict__ X, int64_t N, int d, int metric, co
 }
 
 
+// ---------------------------------------------------------------- the by-vector chain
+// find_nearest_neighbors_by_vector (voyager_manager.py:1589-1657) after its k-NN query, for the song path's jobs and for
+// Song Alchemy: one item at a time in k-NN order, each stage looking only at what came before it.
+//   * _filter_by_distance (:526-617): the item is compared with the kept window (window_start) in the VOYAGER_METRIC
+//     distance; items without a vector are dropped; with no lookback the list is unchanged;
+//   * same-song dedupe (:1625-1636): an item without details, or whose signature this list already let through, is out;
+//   * the raw-author cap (:1638-1653, only when eliminate_duplicates and the cap is > 0; falsy authors are out).
+// The caller computes the window's distances with all its warps; step() is thread 0's decision and books.
+struct ByVectorChain {
+  int32_t* kept;       // the filter's kept positions
+  int32_t* seen;       // [n_sig] the list that last let the signature through, -1 initially
+  int32_t* raw_mark;   // [n_raw] the list that last counted the raw author, -1 initially
+  int32_t* raw_count;  // [n_raw]
+
+  // the first kept position the next item is compared with (n_kept: none)
+  __device__ __forceinline__ int window_start(int n_kept, int batch_kept, bool batched, int lookback) const {
+    return lookback > 0 ? filter_window_start(n_kept, batch_kept, batched, lookback) : n_kept;
+  }
+
+  // item i of list `list`: valid = it has a vector, close = it came within the threshold of the window, sig / raw its
+  // signature and raw-author keys (-1: no details / falsy author).  True when it passes all three stages.
+  __device__ __forceinline__ bool step(int list, int i, bool valid, bool close, int sig, int raw, int lookback, int cap,
+                                       int& n_kept) const {
+    bool pass = true;
+    if (lookback > 0) {  // the kept ones form the window
+      pass = valid && !close;
+      if (pass) kept[n_kept++] = i;
+    }
+    if (pass && sig < 0) pass = false;
+    if (pass) {
+      if (seen[sig] == list) pass = false;
+      else seen[sig] = list;
+    }
+    if (pass && cap > 0) {
+      if (raw < 0) {
+        pass = false;
+      } else {
+        if (raw_mark[raw] != list) {
+          raw_mark[raw] = list;
+          raw_count[raw] = 0;
+        }
+        if (raw_count[raw] >= cap) pass = false;
+        else raw_count[raw] += 1;
+      }
+    }
+    return pass;
+  }
+};
+
+
 // ---------------------------------------------------------------- song path walk on device
 // path_manager.py:180-317 (_find_best_songs_for_job) over the chain find_nearest_neighbors_by_vector
 // (voyager_manager.py:1547-1657) runs on each job's k-NN prefix, for a sequence of jobs, in one CTA.  One pass over a
 // job's candidates in k-NN order does every stage, because each stage only looks at what came before it:
-//   * _filter_by_distance (:526-617): the item is compared with the kept window (filter_window_start) in the
-//     VOYAGER_METRIC distance; with no lookback the list is unchanged;
-//   * same-song dedupe (:1625-1636): an item without details, or whose signature this job already let through, is out;
-//   * the raw-author cap (:1638-1653, only when eliminate_duplicates and the cap is > 0; falsy authors are out);
+//   * the by-vector chain (ByVectorChain, each job a list of its own);
 //   * [:n]: the pass ends after the n-th item that got this far;
 //   * acceptance (path_manager.py:211-291): used rows and signatures, the normalised-author cap, then the lookbacks
 //     against the path's last songs and this job's found songs, in PATH_DISTANCE_METRIC; the job ends once it has
@@ -370,6 +417,7 @@ __global__ void __launch_bounds__(kPathThreads) song_path_kernel(const SongPathA
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, warps = kPathThreads / 32;
   const am_song_path_cfg& c = a.cfg;
   const int lb_f = c.filter_lookback, lb_p = c.path_lookback;
+  const ByVectorChain chain{a.kept, a.seen, a.raw_mark, a.raw_count};
   for (int j = tid; j < a.n_jobs; j += kPathThreads) a.out_found[j] = 0;  // jobs after a stop are not run
   if (tid == 0) {
     s_n_used = *a.n_used;
@@ -398,7 +446,7 @@ __global__ void __launch_bounds__(kPathThreads) song_path_kernel(const SongPathA
       __syncthreads();
       if (valid) {
         const int kept = s_kept, found = s_found, np = s_n_path;
-        const int f0 = lb_f > 0 ? filter_window_start(kept, s_batch_kept, batched, lb_f) : kept;
+        const int f0 = chain.window_start(kept, s_batch_kept, batched, lb_f);
         const int nf = kept - f0, npw = min(lb_p, np), nq = min(lb_p, found);
         const float* x = a.X + row * a.d;
         for (int t = warp; t < nf + npw + nq; t += warps) {
@@ -431,30 +479,8 @@ __global__ void __launch_bounds__(kPathThreads) song_path_kernel(const SongPathA
       __syncthreads();
       if (tid == 0) {
         const int close = s_close;
-        bool pass = true;
-        if (lb_f > 0) {  // _filter_by_distance: items without a vector are dropped, the kept ones form the window
-          pass = valid && !(close & 1);
-          if (pass) a.kept[s_kept++] = i;
-        }
         const int sig = a.cand_sig[base + i];
-        if (pass && sig < 0) pass = false;
-        if (pass) {
-          if (a.seen[sig] == j) pass = false;
-          else a.seen[sig] = j;
-        }
-        if (pass && c.voyager_cap > 0) {
-          const int r = a.cand_raw[base + i];
-          if (r < 0) {
-            pass = false;
-          } else {
-            if (a.raw_mark[r] != j) {
-              a.raw_mark[r] = j;
-              a.raw_count[r] = 0;
-            }
-            if (a.raw_count[r] >= c.voyager_cap) pass = false;
-            else a.raw_count[r] += 1;
-          }
-        }
+        const bool pass = chain.step(j, i, valid, close & 1, sig, a.cand_raw[base + i], lb_f, c.voyager_cap, s_kept);
         if (pass) {
           s_prod += 1;
           const int au = a.cand_author[base + i];
@@ -512,7 +538,133 @@ __global__ void __launch_bounds__(kPathThreads) song_path_kernel(const SongPathA
   }
 }
 
+// ---------------------------------------------------------------- Song Alchemy on device
+// song_alchemy (tasks/song_alchemy.py:371-1115) between its centroids and its projection, in one CTA:
+//   * the by-vector chain (ByVectorChain) over the add centroid's k-NN list, cut at [:n] (n = 3 n_results,
+//     voyager_manager.py:1657); skipped for the single-song temperature-0 branch (:423-427), whose list is the
+//     reference's find_nearest_neighbors_by_id;
+//   * the add and subtract song rows are taken out (:441-446);
+//   * the subtract filter (:448-486): d(sub, v) >= threshold keeps the candidate, otherwise it is filtered out;
+//   * the distance to the add centroid (:916-930).
+// The centroids are float64, as the reference's means of float64 copies are.  Both distances are song_alchemy's own
+// (not get_distance's): angular arccos(clip(c / (|c| or 1) . v / (|v| or 1))) / pi, so a zero vector is at 0.5, and
+// euclidean ||c - v||, in float64 from the stored rows.  The chain walks its items one at a time like the song path; the
+// rest is one warp per chain survivor.
+constexpr int kAlchemyThreads = 512;
+
+struct AlchemyArgs {
+  const float* X;
+  int64_t N;
+  int d;
+  int m;                    // candidates
+  const double* add_c;      // [d]
+  const double* sub_c;      // [d] or null: no subtract filter
+  const int64_t* cand_row;  // [m] stored row, -1: no vector
+  const int32_t* cand_sig;  // [m] signature key, -1: no details
+  const int32_t* cand_raw;  // [m] raw author key, -1: falsy author
+  const int64_t* excl_row;  // [n_excl]
+  int n_excl;
+  am_alchemy_cfg cfg;
+  int32_t* seen;            // [n_sig] scratch, -1 initially
+  int32_t* raw_mark;        // [n_raw] scratch, -1 initially
+  int32_t* raw_count;       // [n_raw] scratch
+  int32_t* kept;            // [m] scratch: the filter's kept positions
+  int32_t* out_count;       // the chain's survivors
+  int32_t* out_pos;         // [min(m, n)] their positions in the candidate arrays, in order
+  unsigned char* out_status;  // [min(m, n)] 0 taken out, 1 kept, 2 filtered out
+  double* out_dsub;         // [min(m, n)]
+  double* out_dadd;         // [min(m, n)]
+  float* out_rows;          // [min(m, n), d] or null
+};
+
+// song_alchemy's distance from centroid c (float64) to stored row v, one warp
+__device__ __forceinline__ double alchemy_distance(const double* c, const float* v, int d, int metric, int lane) {
+  double dot = 0.0, nc = 0.0, nv = 0.0, d2 = 0.0;
+  for (int t = lane; t < d; t += 32) {
+    const double cv = c[t], vv = (double)__ldg(&v[t]);
+    dot = fma(cv, vv, dot);
+    nc = fma(cv, cv, nc);
+    nv = fma(vv, vv, nv);
+    const double df = cv - vv;
+    d2 = fma(df, df, d2);
+  }
+  dot = warp_sum(dot);
+  nc = warp_sum(nc);
+  nv = warp_sum(nv);
+  d2 = warp_sum(d2);
+  if (metric == kMetricL2) return sqrt(d2);
+  nc = sqrt(nc);
+  nv = sqrt(nv);
+  const double cs = dot / ((nc == 0.0 ? 1.0 : nc) * (nv == 0.0 ? 1.0 : nv));
+  return acos(fmin(1.0, fmax(-1.0, cs))) / CUDART_PI;
+}
+
+__global__ void __launch_bounds__(kAlchemyThreads) alchemy_kernel(const AlchemyArgs a) {
+  __shared__ int s_close, s_kept, s_batch_kept, s_n;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, warps = kAlchemyThreads / 32;
+  const am_alchemy_cfg& c = a.cfg;
+  const int lb = c.filter_lookback;
+  const ByVectorChain chain{a.kept, a.seen, a.raw_mark, a.raw_count};
+  if (tid == 0) s_kept = s_batch_kept = s_n = 0;
+  __syncthreads();
+  if (c.skip_chain) {
+    for (int i = tid; i < a.m; i += kAlchemyThreads) a.out_pos[i] = i;
+    if (tid == 0) s_n = a.m;
+  } else {
+    const bool batched = a.m > c.filter_batch;
+    for (int i = 0; i < a.m; ++i) {
+      const int64_t row = a.cand_row[i];
+      const bool valid = row >= 0 && row < a.N;
+      if (tid == 0) {
+        s_close = 0;
+        if (batched && i % c.filter_batch == 0) s_batch_kept = s_kept;
+      }
+      __syncthreads();
+      if (valid) {
+        const int kept = s_kept, f0 = chain.window_start(kept, s_batch_kept, batched, lb);
+        const float* x = a.X + row * a.d;
+        for (int t = f0 + warp; t < kept; t += warps) {
+          const double dist = direct_distance(x, a.X + a.cand_row[a.kept[t]] * a.d, a.d, c.voyager_metric, lane);
+          if (lane == 0 && dist < c.filter_threshold) s_close = 1;
+        }
+      }
+      __syncthreads();
+      if (tid == 0 && chain.step(0, i, valid, s_close, a.cand_sig[i], a.cand_raw[i], lb, c.voyager_cap, s_kept))
+        a.out_pos[s_n++] = i;
+      __syncthreads();
+      if (s_n >= c.n) break;
+    }
+  }
+  __syncthreads();
+  const int n = s_n;
+  for (int t = warp; t < n; t += warps) {
+    const int64_t row = a.cand_row[a.out_pos[t]];
+    bool out = row < 0 || row >= a.N;  // no vector: the subtract filter skips it (:465), the distances do (:921)
+    for (int e = 0; e < a.n_excl && !out; ++e) out = a.excl_row[e] == row;
+    unsigned char status = 0;
+    double dsub = 0.0, dadd = 0.0;
+    if (!out) {
+      const float* v = a.X + row * a.d;
+      dadd = alchemy_distance(a.add_c, v, a.d, c.path_metric, lane);
+      status = 1;
+      if (a.sub_c) {
+        dsub = alchemy_distance(a.sub_c, v, a.d, c.path_metric, lane);
+        if (!(dsub >= c.subtract_threshold)) status = 2;
+      }
+      if (a.out_rows)
+        for (int k = lane; k < a.d; k += 32) a.out_rows[(int64_t)t * a.d + k] = v[k];
+    }
+    if (lane == 0) {
+      a.out_status[t] = status;
+      a.out_dsub[t] = dsub;
+      a.out_dadd[t] = dadd;
+    }
+  }
+  if (tid == 0) *a.out_count = n;
+}
+
 }  // namespace am
+
 
 using namespace am;
 
@@ -676,5 +828,71 @@ extern "C" int am_knn_song_path(const am_index* idx, const am_song_path_cfg* cfg
   call.get(used_rows, a.used_row, (size_t)out_hdr[0]);
   call.get(path_rows, a.path_row, (size_t)out_hdr[1]);
   call.get(out_dist, a.out_dist, (size_t)out_hdr[1]);
+  return AM_OK;
+}
+
+extern "C" int am_knn_alchemy(const am_index* idx, const am_alchemy_cfg* cfg, const double* add_centroid,
+                              const double* sub_centroid, int n_cand, const int64_t* cand_rows, const int32_t* cand_sig,
+                              const int32_t* cand_author_raw, int n_sig, int n_excl, const int64_t* excl_rows,
+                              int32_t* out_count, int32_t* out_pos, unsigned char* out_status, double* out_dsub,
+                              double* out_dadd, float* out_rows) {
+  AM_CHECK(idx && cfg && add_centroid && out_count && (n_excl == 0 || excl_rows), "am_knn_alchemy: NULL argument");
+  AM_CHECK(cfg->voyager_metric == kMetricCos || cfg->voyager_metric == kMetricL2, "am_knn_alchemy: voyager_metric %d",
+           cfg->voyager_metric);
+  AM_CHECK(cfg->path_metric == kMetricCos || cfg->path_metric == kMetricL2, "am_knn_alchemy: path_metric %d",
+           cfg->path_metric);
+  AM_CHECK(cfg->filter_batch > 0, "am_knn_alchemy: filter_batch must be positive");
+  AM_CHECK(cfg->n >= 1 && cfg->n <= AM_ALCHEMY_MAX_N, "am_knn_alchemy: n = %d is outside [1, %d]", cfg->n,
+           AM_ALCHEMY_MAX_N);
+  AM_CHECK(n_cand >= 0 && n_cand <= AM_ALCHEMY_MAX_CANDIDATES && (!cfg->skip_chain || n_cand <= cfg->n),
+           "am_knn_alchemy: %d candidates (at most %d, and at most n without the chain)", n_cand,
+           AM_ALCHEMY_MAX_CANDIDATES);
+  AM_CHECK(n_sig >= 0 && n_excl >= 0, "am_knn_alchemy: negative size");
+  const int n_out = std::min(n_cand, cfg->n);
+  AM_CHECK(n_cand == 0 || (cand_rows && cand_sig && cand_author_raw), "am_knn_alchemy: NULL candidates");
+  AM_CHECK(n_out == 0 || (out_pos && out_status && out_dsub && out_dadd), "am_knn_alchemy: NULL output");
+  int n_raw = 0;
+  for (int i = 0; i < n_cand; ++i) {
+    AM_CHECK(cand_sig[i] >= -1 && cand_sig[i] < n_sig && cand_author_raw[i] >= -1,
+             "am_knn_alchemy: candidate %d has a key out of range", i);
+    n_raw = std::max(n_raw, cand_author_raw[i] + 1);
+  }
+  *out_count = 0;
+  if (n_cand == 0) return AM_OK;
+  cudaStream_t st;
+  AM_TRY(HostCall::thread_stream(&st));
+  HostCall call(st, HostCall::kAlways);
+  AlchemyArgs a{idx->X.p, idx->N, idx->d, n_cand};
+  a.n_excl = n_excl;
+  a.cfg = *cfg;
+  call.up(&a.add_c, add_centroid, (size_t)idx->d);
+  call.up(&a.sub_c, sub_centroid, sub_centroid ? (size_t)idx->d : 0);
+  call.up(&a.cand_row, cand_rows, (size_t)n_cand);
+  call.up(&a.cand_sig, cand_sig, (size_t)n_cand);
+  call.up(&a.cand_raw, cand_author_raw, (size_t)n_cand);
+  call.up(&a.excl_row, excl_rows, (size_t)n_excl);
+  call.down(&a.out_count, 1);
+  call.down(&a.out_pos, (size_t)n_out);
+  call.down(&a.out_status, (size_t)n_out);
+  call.down(&a.out_dsub, (size_t)n_out);
+  call.down(&a.out_dadd, (size_t)n_out);
+  call.down(&a.out_rows, out_rows ? (size_t)n_out * idx->d : 0);
+  call.device(&a.seen, (size_t)n_sig, 0xff);  // -1: no signature let through yet
+  call.device(&a.raw_mark, (size_t)n_raw, 0xff);
+  call.device(&a.raw_count, (size_t)n_raw);
+  call.device(&a.kept, (size_t)n_cand);
+  AM_TRY(call.start());
+  if (!sub_centroid) a.sub_c = nullptr;
+  if (!out_rows) a.out_rows = nullptr;
+  AM_LAUNCH(alchemy_kernel, 1, kAlchemyThreads, 0, st, a);
+  AM_TRY(call.finish());
+  const int32_t cnt = *call.mirror(a.out_count);
+  AM_CHECK(cnt >= 0 && cnt <= n_out, "am_knn_alchemy: inconsistent result (%d of at most %d)", cnt, n_out);
+  call.get(out_pos, a.out_pos, (size_t)cnt);
+  call.get(out_status, a.out_status, (size_t)cnt);
+  call.get(out_dsub, a.out_dsub, (size_t)cnt);
+  call.get(out_dadd, a.out_dadd, (size_t)cnt);
+  if (out_rows) call.get(out_rows, a.out_rows, (size_t)cnt * idx->d);
+  *out_count = cnt;
   return AM_OK;
 }

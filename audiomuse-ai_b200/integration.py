@@ -122,7 +122,8 @@ METRIC_NAMES = ("silhouette_score", "davies_bouldin_score", "calinski_harabasz_s
 
 def apply(clap=None, voyager_manager=None, clustering=None, allow_sklearn_fallback: bool = True,
           clustering_helper=None, song_alchemy=None, app_map=None, artist_gmm_manager=None,
-          gaussian_mixture=None, radius_walk=None, path_manager=None, app_path=None, analysis=None) -> None:
+          gaussian_mixture=None, radius_walk=None, path_manager=None, app_path=None, analysis=None, alchemy=None,
+          app_alchemy=None) -> None:
     """clap / voyager_manager / clustering / clustering_helper: the reference's already imported tasks.* modules (pass
     only the ones to patch).  allow_sklearn_fallback keeps the reference's contract that a failing GPU k-means silently
     falls back to scikit-learn (tasks/clustering_gpu.py:130-148); this repository's own tests run with it off so a
@@ -141,7 +142,10 @@ def apply(clap=None, voyager_manager=None, clustering=None, allow_sklearn_fallba
     voyager_manager= alone leaves the walk to the reference.  path_manager (the reference's tasks.path_manager) gets the
     device song path as find_path_between_songs (song_path.make_song_path, over the voyager_manager module whose
     functions path_manager imported); app_path binds that name when it is imported (app_path.py:5), so pass it too for
-    the Song Path endpoint to use it.  analysis (the reference's tasks.analysis) gets track_features.LibrosaFacade as
+    the Song Path endpoint to use it.  alchemy (the reference's tasks.song_alchemy) gets the device Song Alchemy as
+    song_alchemy (alchemy.make_song_alchemy, over the voyager_manager module whose functions song_alchemy imported);
+    app_alchemy binds that name when it is imported (app_alchemy.py:4), so pass it too for the Alchemy endpoint to use
+    it.  song_alchemy= alone still only replaces _project_with_umap.  analysis (the reference's tasks.analysis) gets track_features.LibrosaFacade as
     its `librosa`: analyze_track's beat_track, rms and chroma_stft (:344-348) run on the device, every other librosa use
     of the module goes to the librosa it imported; sys.modules["librosa"] is left alone."""
     if analysis is not None:
@@ -168,6 +172,15 @@ def apply(clap=None, voyager_manager=None, clustering=None, allow_sklearn_fallba
         path_manager.find_path_between_songs = fn
         if app_path is not None:
             app_path.find_path_between_songs = fn
+    if app_alchemy is not None and alchemy is None:
+        raise ValueError("app_alchemy= takes the device Song Alchemy from alchemy=: pass both")
+    if alchemy is not None:
+        from . import alchemy as b200_alchemy
+
+        fn = b200_alchemy.make_song_alchemy(alchemy, sys.modules[alchemy.find_nearest_neighbors_by_id.__module__])
+        alchemy.song_alchemy = fn
+        if app_alchemy is not None:
+            app_alchemy.song_alchemy = fn
     if clustering is not None:
         from . import clustering_gpu as b200_cg
 

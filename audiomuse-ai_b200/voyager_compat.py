@@ -329,6 +329,45 @@ class Index:
                 self._ids[used[:n_used.value]].tolist(), self._ids[path[:n_path.value]].tolist(),
                 dist[:n_path.value].copy())
 
+    # ------------------------------------------------------------------ Song Alchemy (tasks/song_alchemy.py:420-930)
+    def alchemy(self, cfg, add_centroid, sub_centroid, cand_ids, cand_sig, cand_author_raw, n_sig, excl_ids,
+                rows: bool = False):
+        """Song Alchemy's candidate list in one device call (am_knn_alchemy).  cfg: an _lib.AlchemyCfg.  cand_ids are
+        index ids in k-NN order (ids not in the index have no vector), cand_sig / cand_author_raw the dense keys the
+        header describes, n_sig the number of signature keys; excl_ids the add and subtract songs' ids in the index.
+        The centroids stay float64.  Returns (positions in cand_ids of the chain's survivors, their status: 1 kept,
+        2 filtered out, 0 taken out; f64 distances to the subtract and add centroids, and their f32 stored rows when
+        `rows`, else None)."""
+        add = np.ascontiguousarray(add_centroid, dtype=np.float64).reshape(-1)
+        sub = None if sub_centroid is None else np.ascontiguousarray(sub_centroid, dtype=np.float64).reshape(-1)
+        if add.shape[0] != self.num_dimensions or (sub is not None and sub.shape[0] != self.num_dimensions):
+            raise ValueError(f"centroids must have dimension {self.num_dimensions}")
+        cand = self._rows_of(cand_ids, strict=False)
+        sig = np.ascontiguousarray(cand_sig, dtype=np.int32)
+        raw = np.ascontiguousarray(cand_author_raw, dtype=np.int32)
+        if sig.shape != cand.shape or raw.shape != cand.shape:
+            raise ValueError("candidate arrays differ in length")
+        if not 1 <= cfg.n <= _lib.ALCHEMY_MAX_N or len(cand) > _lib.ALCHEMY_MAX_CANDIDATES or (
+                cfg.skip_chain and len(cand) > cfg.n):
+            raise ValueError(f"{len(cand)} candidates for n = {cfg.n}: n must be in [1, {_lib.ALCHEMY_MAX_N}], the "
+                             f"candidates at most {_lib.ALCHEMY_MAX_CANDIDATES}, and at most n without the chain")
+        excl = self._rows_of(excl_ids, strict=True)
+        n_out = max(1, min(len(cand), int(cfg.n)))
+        count = C.c_int32(0)
+        pos = np.empty(n_out, dtype=np.int32)
+        status = np.empty(n_out, dtype=np.uint8)
+        dsub = np.empty(n_out, dtype=np.float64)
+        dadd = np.empty(n_out, dtype=np.float64)
+        out_rows = np.empty((n_out, self.num_dimensions), dtype=np.float32) if rows else None
+        h = self._ensure_built()
+        _lib.check(_lib.load().am_knn_alchemy(
+            h, C.byref(cfg), _lib.ptr(add), None if sub is None else _lib.ptr(sub), len(cand), _lib.ptr(cand),
+            _lib.ptr(sig), _lib.ptr(raw), int(n_sig), len(excl), _lib.ptr(excl), C.byref(count), _lib.ptr(pos),
+            _lib.ptr(status), _lib.ptr(dsub), _lib.ptr(dadd), None if out_rows is None else _lib.ptr(out_rows)))
+        k = count.value
+        return (pos[:k].copy(), status[:k].copy(), dsub[:k].copy(), dadd[:k].copy(),
+                None if out_rows is None else out_rows[:k].copy())
+
     # ------------------------------------------------------------------ persistence
     def as_bytes(self) -> bytes:
         with self._mu:

@@ -265,6 +265,38 @@ AM_API int am_knn_song_path(const am_index* idx, const am_song_path_cfg* cfg, in
                             int n_sig, int n_author, int64_t* used_rows, int32_t* n_used, unsigned char* used_sig,
                             int32_t* author_count, int64_t* path_rows, int32_t* n_path, int64_t end_row,
                             int32_t* out_found, int32_t* out_pos, int32_t* out_failed, double* out_dist);
+/* The configuration song_alchemy and voyager_manager.py read at call time, for am_knn_alchemy.  Metrics as in
+ * am_song_path_cfg; path_metric is config.PATH_DISTANCE_METRIC as song_alchemy reads it (:456, :923). */
+#define AM_ALCHEMY_MAX_N 600            /* 3 x config.ALCHEMY_MAX_N_RESULTS (200) */
+#define AM_ALCHEMY_MAX_CANDIDATES 3000  /* the by-vector query for n = 600 with eliminate_duplicates: 600 + 4 x 600 */
+typedef struct am_alchemy_cfg {
+  int voyager_metric;
+  int path_metric;
+  int filter_lookback;        /* voyager_manager.DUPLICATE_DISTANCE_CHECK_LOOKBACK (<= 0: no distance filter) */
+  int filter_batch;           /* voyager_manager.BATCH_SIZE_VECTOR_OPS */
+  int voyager_cap;            /* the by-vector raw-author cap: MAX_SONGS_PER_ARTIST when eliminate_duplicates, else 0 */
+  int n;                      /* the by-vector n, 3 x n_results: the chain stops at n survivors */
+  int skip_chain;             /* the candidates are the final neighbour list (the single-song temperature-0 branch) */
+  double filter_threshold;    /* DUPLICATE_DISTANCE_THRESHOLD_* for voyager_metric */
+  double subtract_threshold;  /* the subtract filter keeps a candidate at distance >= this from the subtract centroid */
+} am_alchemy_cfg;
+
+/* Song Alchemy's candidate list, tasks/song_alchemy.py:420-486 and :916-930, in one call.  The candidates are the add
+ * centroid's k-NN list in order (the by-vector chain of voyager_manager.py:1589-1657 runs on them and stops at cfg->n
+ * survivors), or with cfg->skip_chain the neighbour list itself (n_cand <= cfg->n).  Per candidate: cand_rows its stored
+ * row (-1: no vector), cand_sig the dense key of its (title, author) signature after strip().lower() (-1: no details),
+ * cand_author_raw a dense key of its raw author (-1: falsy).  excl_rows[n_excl] are the add and subtract songs' rows:
+ * they are taken out of the survivors.  add_centroid f64[d]; sub_centroid f64[d] or NULL (no subtract filter).
+ * *out_count receives the chain's survivors (<= min(n_cand, cfg->n)); for each, in order: out_pos its entry in the
+ * candidate arrays, out_status 1 kept, 2 filtered out (d(sub) < subtract_threshold) or 0 taken out (excluded or without
+ * a vector), out_dsub and out_dadd its song_alchemy distances to the centroids in float64 (0 where not computed), and
+ * out_rows f32[d] its stored row (out_rows may be NULL: nothing gathered; rows of entries taken out are not written).
+ * Re-entrant. */
+AM_API int am_knn_alchemy(const am_index* idx, const am_alchemy_cfg* cfg, const double* add_centroid,
+                          const double* sub_centroid, int n_cand, const int64_t* cand_rows, const int32_t* cand_sig,
+                          const int32_t* cand_author_raw, int n_sig, int n_excl, const int64_t* excl_rows,
+                          int32_t* out_count, int32_t* out_pos, unsigned char* out_status, double* out_dsub,
+                          double* out_dadd, float* out_rows);
 /* n stored rows in one device gather + one copy: out f32[n, d] */
 AM_API int am_knn_get_vectors(const am_index* idx, const int64_t* ids, int n, float* out);
 AM_API int am_knn_query_dev(const am_index* idx, const float* Q_dev, int nq, int k, int mode,
