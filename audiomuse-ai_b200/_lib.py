@@ -47,6 +47,12 @@ class AlchemyCfg(C.Structure):
                 ("filter_threshold", C.c_double), ("subtract_threshold", C.c_double)]
 
 
+class SimilarCfg(C.Structure):
+    """am_similar_cfg"""
+    _fields_ = [("metric", C.c_int), ("filter_lookback", C.c_int), ("filter_batch", C.c_int), ("cap", C.c_int),
+                ("mood_sum", C.c_int), ("filter_threshold", C.c_double), ("mood_threshold", C.c_double)]
+
+
 ALCHEMY_MAX_N, ALCHEMY_MAX_CANDIDATES = 600, 3000   # AM_ALCHEMY_MAX_N, AM_ALCHEMY_MAX_CANDIDATES
 
 
@@ -113,6 +119,9 @@ SIGNATURES = {
                               _vp, _vp, _P(C.c_int32), _i64, _vp, _vp, _P(C.c_int32), _vp]),
     "am_knn_alchemy": (_i, [_vp, _P(AlchemyCfg), _vp, _vp, _i, _vp, _vp, _vp, _i, _i, _vp, _P(C.c_int32), _vp, _vp, _vp,
                             _vp, _vp]),
+    "am_knn_similar": (_i, [_vp, _P(SimilarCfg), _i64, _i, _i, _vp, _vp, _vp, _i, _vp, _vp, _vp, _i, _P(C.c_int32), _vp,
+                            _vp]),
+    "am_knn_farthest": (_i, [_vp, _vp, _i64, _P(_i64), _P(_f)]),
     "am_knn_get_vectors": (_i, [_vp, _vp, _i, _vp]),
     "am_knn_query_dev": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _vp]),
     "am_kmeans_fit": (_i, [_vp, _i64, _i, _i, _i, _i, _f, _u64, _vp, _vp, _vp, _P(_f), _P(_i)]),

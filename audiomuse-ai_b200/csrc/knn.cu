@@ -762,6 +762,78 @@ static int full_sort_query(const SelectParams& p, int q, cudaStream_t st) {
   return AM_OK;
 }
 
+// ---------------------------------------------------------------- farthest stored row
+// get_max_distance_for_id (voyager_manager.py:1660-1702) walks query(k = N) -- (float64 distance asc, row asc), each
+// distance returned as float32 -- and keeps the first strict maximum of the float32 distances, skipping the target.
+// Among the rows at the float32 maximum that is the smallest float64 distance, then the smallest row.  One pass computes
+// every distance with exact_distance on the query the query path prepares, so each is the value query() returns; each
+// warp keeps its best row, each block reduces its warps', and one block reduces the blocks'.  A NaN distance never wins
+// (dist > max is false), as in the reference's loop.
+constexpr int kFarThreads = 256;
+
+struct FarBest {
+  float f;    // the float32 distance query() returns
+  double dd;  // the float64 distance it orders by
+  int64_t row;  // -1: none
+};
+
+__device__ __forceinline__ bool far_better(const FarBest& a, const FarBest& b) {
+  if (a.row < 0) return false;
+  if (b.row < 0) return true;
+  return a.f > b.f || (a.f == b.f && (a.dd < b.dd || (a.dd == b.dd && a.row < b.row)));
+}
+
+// the block's best of `cand` (one per thread), written by thread 0 to *out
+__device__ __forceinline__ void far_block_reduce(FarBest cand, FarBest* out) {
+  __shared__ FarBest s_best[kFarThreads / 32];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  for (int o = 16; o > 0; o >>= 1) {
+    FarBest other;
+    other.f = __shfl_down_sync(0xffffffffu, cand.f, o);
+    other.dd = __shfl_down_sync(0xffffffffu, cand.dd, o);
+    other.row = __shfl_down_sync(0xffffffffu, cand.row, o);
+    if (lane + o < 32 && far_better(other, cand)) cand = other;
+  }
+  if (lane == 0) s_best[warp] = cand;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    FarBest best = s_best[0];
+    for (int w = 1; w < kFarThreads / 32; ++w)
+      if (far_better(s_best[w], best)) best = s_best[w];
+    *out = best;
+  }
+}
+
+// pass 1: one warp per row, grid-stride; block b's best to part[b]
+__global__ void __launch_bounds__(kFarThreads) farthest_kernel(SelectParams p, int64_t exclude_row,
+                                                               FarBest* __restrict__ part) {
+  const int lane = threadIdx.x & 31;
+  const int64_t warps = (int64_t)gridDim.x * (kFarThreads / 32);
+  FarBest best{0.f, 0.0, -1};
+  for (int64_t row = (int64_t)blockIdx.x * (kFarThreads / 32) + (threadIdx.x >> 5); row < p.N; row += warps) {
+    const double dd = exact_distance(p, 0, row, lane);
+    const FarBest c{(float)dd, dd, row};
+    if (row != exclude_row && !isnan(c.f) && far_better(c, best)) best = c;
+  }
+  if (lane != 0) best.row = -1;  // every lane holds the warp's best; lane 0 speaks for it
+  far_block_reduce(best, &part[blockIdx.x]);
+}
+
+// pass 2: one block over the blocks' bests
+__global__ void __launch_bounds__(kFarThreads) farthest_reduce_kernel(const FarBest* __restrict__ part, int n_part,
+                                                                      int64_t* __restrict__ out_row,
+                                                                      float* __restrict__ out_dist) {
+  __shared__ FarBest s_out;
+  FarBest best{0.f, 0.0, -1};
+  for (int b = threadIdx.x; b < n_part; b += kFarThreads)
+    if (far_better(part[b], best)) best = part[b];
+  far_block_reduce(best, &s_out);
+  if (threadIdx.x == 0) {
+    *out_row = s_out.row;
+    *out_dist = s_out.row >= 0 ? s_out.f : 0.0f;
+  }
+}
+
 static float reduce_max_host(const float* dev, int64_t n, cudaStream_t st, int* status) {
   std::vector<float> h(n);
   cudaError_t e = cudaMemcpyAsync(h.data(), dev, n * 4, cudaMemcpyDeviceToHost, st);
@@ -1193,5 +1265,44 @@ extern "C" int am_knn_get_vectors(const am_index* idx, const int64_t* ids, int n
   AM_TRY(call.start());
   const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(((int64_t)n * idx->d + 255) / 256, (int64_t)sm_count() * 8));
   AM_LAUNCH(gather_rows_kernel, grid, 256, 0, st, idx->X.p, idx->N, idx->d, d_ids, n, d_out);
+  return call.finish();
+}
+
+extern "C" int am_knn_farthest(const am_index* idx, const float* query, int64_t exclude_row, int64_t* out_row,
+                               float* out_dist) {
+  AM_CHECK(idx && query && out_row && out_dist, "am_knn_farthest: NULL argument");
+  AM_CHECK(exclude_row >= -1 && exclude_row < idx->N, "am_knn_farthest: excluded row %lld out of range",
+           (long long)exclude_row);
+  *out_row = -1;
+  *out_dist = 0.0f;
+  if (idx->N == 0) return AM_OK;
+  cudaStream_t st;
+  AM_TRY(HostCall::thread_stream(&st));
+  const int d = idx->d;
+  const int n_part = (int)std::max<int64_t>(1, std::min<int64_t>((idx->N + 7) / 8, (int64_t)sm_count() * 8));
+  HostCall call(st, HostCall::kAlways);
+  float *dQ, *dQs, *dD;
+  double* qnorm;
+  int64_t* dR;
+  FarBest* part;
+  call.up(&dQ, query, (size_t)d);
+  call.down(&dR, 1, out_row);
+  call.down(&dD, 1, out_dist);
+  call.device(&dQs, (size_t)d);
+  call.device(&qnorm, 1);
+  call.device(&part, (size_t)n_part);
+  AM_TRY(call.start());
+  // the query as knn_query_impl prepares it for a single query of k = N (query_prepare_kernel, then exact_distance)
+  AM_LAUNCH(query_prepare_kernel, 1, 256, 0, st, dQ, 1, d, idx->dpad, idx->metric, dQs, qnorm, nullptr, nullptr);
+  SelectParams p{};
+  p.N = idx->N;
+  p.d = d;
+  p.metric = idx->metric;
+  p.X = idx->X.p;
+  p.xnorm2 = idx->xnorm2.p;
+  p.Q = dQ;
+  p.qnorm = qnorm;
+  AM_LAUNCH(farthest_kernel, n_part, kFarThreads, 0, st, p, exclude_row, part);
+  AM_LAUNCH(farthest_reduce_kernel, 1, kFarThreads, 0, st, part, n_part, dR, dD);
   return call.finish();
 }

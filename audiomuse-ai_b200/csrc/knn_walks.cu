@@ -315,6 +315,9 @@ radius_walk_kernel(const float* __restrict__ X, int64_t N, int d, int metric, co
 //   * _filter_by_distance (:526-617): the item is compared with the kept window (window_start) in the VOYAGER_METRIC
 //     distance; items without a vector are dropped; with no lookback the list is unchanged;
 //   * same-song dedupe (:1625-1636): an item without details, or whose signature this list already let through, is out;
+//   * the mood stage of find_nearest_neighbors_by_id (:1512, _filter_by_mood_similarity): the caller's verdict, taken
+//     after the signature is marked (the reference's dedupe marks a song the mood filter then drops); the by-vector
+//     callers pass true;
 //   * the raw-author cap (:1638-1653, only when eliminate_duplicates and the cap is > 0; falsy authors are out).
 // The caller computes the window's distances with all its warps; step() is thread 0's decision and books.
 struct ByVectorChain {
@@ -329,9 +332,10 @@ struct ByVectorChain {
   }
 
   // item i of list `list`: valid = it has a vector, close = it came within the threshold of the window, sig / raw its
-  // signature and raw-author keys (-1: no details / falsy author).  True when it passes all three stages.
-  __device__ __forceinline__ bool step(int list, int i, bool valid, bool close, int sig, int raw, int lookback, int cap,
-                                       int& n_kept) const {
+  // signature and raw-author keys (-1: no details / falsy author), mood whether it passes the mood stage.  True when it
+  // passes every stage.
+  __device__ __forceinline__ bool step(int list, int i, bool valid, bool close, int sig, int raw, bool mood, int lookback,
+                                       int cap, int& n_kept) const {
     bool pass = true;
     if (lookback > 0) {  // the kept ones form the window
       pass = valid && !close;
@@ -342,6 +346,7 @@ struct ByVectorChain {
       if (seen[sig] == list) pass = false;
       else seen[sig] = list;
     }
+    if (pass && !mood) pass = false;
     if (pass && cap > 0) {
       if (raw < 0) {
         pass = false;
@@ -480,7 +485,8 @@ __global__ void __launch_bounds__(kPathThreads) song_path_kernel(const SongPathA
       if (tid == 0) {
         const int close = s_close;
         const int sig = a.cand_sig[base + i];
-        const bool pass = chain.step(j, i, valid, close & 1, sig, a.cand_raw[base + i], lb_f, c.voyager_cap, s_kept);
+        const bool pass = chain.step(j, i, valid, close & 1, sig, a.cand_raw[base + i], true, lb_f, c.voyager_cap,
+                                     s_kept);
         if (pass) {
           s_prod += 1;
           const int au = a.cand_author[base + i];
@@ -629,7 +635,7 @@ __global__ void __launch_bounds__(kAlchemyThreads) alchemy_kernel(const AlchemyA
         }
       }
       __syncthreads();
-      if (tid == 0 && chain.step(0, i, valid, s_close, a.cand_sig[i], a.cand_raw[i], lb, c.voyager_cap, s_kept))
+      if (tid == 0 && chain.step(0, i, valid, s_close, a.cand_sig[i], a.cand_raw[i], true, lb, c.voyager_cap, s_kept))
         a.out_pos[s_n++] = i;
       __syncthreads();
       if (s_n >= c.n) break;
@@ -661,6 +667,122 @@ __global__ void __launch_bounds__(kAlchemyThreads) alchemy_kernel(const AlchemyA
     }
   }
   if (tid == 0) *a.out_count = n;
+}
+
+
+// ---------------------------------------------------------------- plain similar-tracks requests on device
+// find_nearest_neighbors_by_id without the radius walk (voyager_manager.py:1493-1545) and
+// find_nearest_neighbors_by_vector (:1589-1657) after their k-NN query, in one CTA: the by-vector chain (ByVectorChain)
+// over the request's list in k-NN order, stopping once n items have passed ([:n]).  A by-id request differs in three
+// places:
+//   * its target goes first into _filter_by_distance at distance 0 (:1497-1502): it is the first kept item of the
+//     window (the list it heads is one longer, which moves the batch boundaries) and is never output (:1505);
+//   * the dedupe starts with the target's signature already seen (:662-665);
+//   * the mood stage (:1508-1514, _filter_by_mood_similarity :714-822) runs between the dedupe and the cap when the
+//     caller passes a mood table: a candidate without parsed features is dropped, otherwise its mood distance
+//     sum(|target[f] - cand[f]|) / 6 over the six features, summed in float64 as Python's sum() does (mood_distance),
+//     must be <= the threshold.
+// Every warp computes the filter window's distances; thread 0 decides and keeps the books.
+constexpr int kSimilarThreads = 512;
+constexpr int kMoodFeatures = 6;  // danceable, aggressive, happy, party, relaxed, sad (:775)
+
+struct SimilarArgs {
+  const float* X;
+  int64_t N;
+  int d;
+  int m;                          // candidates
+  int n;                          // the request's n
+  int64_t target_row;             // -1: a by-vector request
+  int target_sig;                 // the signature seen before the first candidate, -1: none
+  const int64_t* cand_row;        // [m] stored row, -1: no vector
+  const int32_t* cand_sig;        // [m] signature key, -1: no details
+  const int32_t* cand_raw;        // [m] raw author key, -1: falsy author
+  const double* mood;             // [m, 6] the candidates' features, or null: no mood stage
+  const unsigned char* mood_ok;   // [m] 1: the candidate's features parsed
+  const double* target_mood;      // [6]
+  am_similar_cfg cfg;
+  int32_t* seen;                  // [n_sig] scratch, -1 initially
+  int32_t* raw_mark;              // [n_raw] scratch, -1 initially
+  int32_t* raw_count;             // [n_raw] scratch
+  int32_t* kept;                  // [m + 1] scratch: the filter's kept items (the target is item 0 of a by-id list)
+  int32_t* out_count;
+  int32_t* out_pos;               // [min(m, n)] the survivors' positions in the candidate arrays, in order
+  double* out_mood;               // [min(m, n)] their mood distances (mood stage only)
+};
+
+// the normalised mood distance of :789-795, sum(|t - c|) / 6, with Python's sum() of floats and no contraction:
+// CPython >= 3.12 (compensated = 1) starts from the first term and adds the others with Neumaier's compensation, added
+// back at the end when it is non-zero and finite; older versions add left to right.
+__device__ __forceinline__ double mood_distance(const double* t, const double* c, int compensated) {
+  double s = fabs(__dsub_rn(t[0], c[0])), comp = 0.0;
+#pragma unroll
+  for (int f = 1; f < kMoodFeatures; ++f) {
+    const double x = fabs(__dsub_rn(t[f], c[f])), u = __dadd_rn(s, x);
+    if (compensated)
+      comp = __dadd_rn(comp, fabs(s) >= fabs(x) ? __dadd_rn(__dsub_rn(s, u), x) : __dadd_rn(__dsub_rn(x, u), s));
+    s = u;
+  }
+  if (comp != 0.0 && isfinite(comp)) s = __dadd_rn(s, comp);
+  return __ddiv_rn(s, (double)kMoodFeatures);
+}
+
+__global__ void __launch_bounds__(kSimilarThreads) similar_kernel(const SimilarArgs a) {
+  __shared__ int s_close, s_kept, s_batch_kept, s_n;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, warps = kSimilarThreads / 32;
+  const am_similar_cfg& c = a.cfg;
+  const int lb = c.filter_lookback;
+  const ByVectorChain chain{a.kept, a.seen, a.raw_mark, a.raw_count};
+  const int by_id = a.target_row >= 0 ? 1 : 0;
+  const int L = a.m + by_id;  // the list _filter_by_distance sees
+  const bool batched = L > c.filter_batch;
+  auto row_of = [&](int i) { return by_id && i == 0 ? a.target_row : a.cand_row[i - by_id]; };
+  if (tid == 0) {
+    s_kept = s_batch_kept = s_n = 0;
+    if (a.target_sig >= 0) a.seen[a.target_sig] = 0;
+  }
+  __syncthreads();
+  for (int i = 0; i < L; ++i) {
+    const int64_t row = row_of(i);
+    const bool valid = row >= 0 && row < a.N;
+    if (tid == 0) {
+      s_close = 0;
+      if (batched && i % c.filter_batch == 0) s_batch_kept = s_kept;
+    }
+    __syncthreads();
+    if (valid) {
+      const int kept = s_kept, f0 = chain.window_start(kept, s_batch_kept, batched, lb);
+      const float* x = a.X + row * a.d;
+      for (int t = f0 + warp; t < kept; t += warps) {
+        const double dist = direct_distance(x, a.X + row_of(a.kept[t]) * a.d, a.d, c.metric, lane);
+        if (lane == 0 && dist < c.filter_threshold) s_close = 1;
+      }
+    }
+    __syncthreads();
+    if (tid == 0) {
+      if (by_id && i == 0) {
+        if (lb > 0 && valid && !s_close) a.kept[s_kept++] = 0;  // the target: only a member of the window
+      } else {
+        const int p = i - by_id;
+        bool mood = true;
+        double md = 0.0;
+        if (a.mood) {
+          mood = a.mood_ok[p] != 0;
+          if (mood) {
+            md = mood_distance(a.target_mood, a.mood + (int64_t)p * kMoodFeatures, c.mood_sum);
+            mood = md <= c.mood_threshold;
+          }
+        }
+        if (chain.step(0, i, valid, s_close, a.cand_sig[p], a.cand_raw[p], mood, lb, c.cap, s_kept)) {
+          a.out_pos[s_n] = p;
+          if (a.out_mood) a.out_mood[s_n] = md;
+          ++s_n;
+        }
+      }
+    }
+    __syncthreads();
+    if (s_n >= a.n) break;
+  }
+  if (tid == 0) *a.out_count = s_n;
 }
 
 }  // namespace am
@@ -893,6 +1015,65 @@ extern "C" int am_knn_alchemy(const am_index* idx, const am_alchemy_cfg* cfg, co
   call.get(out_dsub, a.out_dsub, (size_t)cnt);
   call.get(out_dadd, a.out_dadd, (size_t)cnt);
   if (out_rows) call.get(out_rows, a.out_rows, (size_t)cnt * idx->d);
+  *out_count = cnt;
+  return AM_OK;
+}
+
+extern "C" int am_knn_similar(const am_index* idx, const am_similar_cfg* cfg, int64_t target_row, int target_sig,
+                              int n_cand, const int64_t* cand_rows, const int32_t* cand_sig,
+                              const int32_t* cand_author_raw, int n_sig, const double* mood, const unsigned char* mood_ok,
+                              const double* target_mood, int n, int32_t* out_count, int32_t* out_pos,
+                              double* out_mood) {
+  AM_CHECK(idx && cfg && out_count, "am_knn_similar: NULL argument");
+  AM_CHECK(cfg->metric == kMetricCos || cfg->metric == kMetricL2, "am_knn_similar: metric %d is not 0 (angular) or 1 "
+           "(euclidean)", cfg->metric);
+  AM_CHECK(cfg->filter_batch > 0, "am_knn_similar: filter_batch must be positive");
+  AM_CHECK(n_cand >= 0 && n_sig >= 0, "am_knn_similar: negative size");
+  AM_CHECK(target_row >= -1 && target_row < idx->N, "am_knn_similar: target row %lld out of range",
+           (long long)target_row);
+  AM_CHECK(target_sig >= -1 && target_sig < n_sig, "am_knn_similar: target signature %d out of range", target_sig);
+  AM_CHECK(!mood || (mood_ok && target_mood), "am_knn_similar: a mood table needs its flags and the target's features");
+  const int n_out = std::max(0, std::min(n_cand, n));
+  AM_CHECK(n_cand == 0 || (cand_rows && cand_sig && cand_author_raw), "am_knn_similar: NULL candidates");
+  AM_CHECK(n_out == 0 || (out_pos && (!mood || out_mood)), "am_knn_similar: NULL output");
+  int n_raw = 0;
+  for (int i = 0; i < n_cand; ++i) {
+    AM_CHECK(cand_sig[i] >= -1 && cand_sig[i] < n_sig && cand_author_raw[i] >= -1,
+             "am_knn_similar: candidate %d has a key out of range", i);
+    n_raw = std::max(n_raw, cand_author_raw[i] + 1);
+  }
+  *out_count = 0;
+  if (n_out == 0) return AM_OK;
+  cudaStream_t st;
+  AM_TRY(HostCall::thread_stream(&st));
+  HostCall call(st, HostCall::kAlways);
+  SimilarArgs a{idx->X.p, idx->N, idx->d, n_cand, n, target_row, target_sig};
+  a.cfg = *cfg;
+  call.up(&a.cand_row, cand_rows, (size_t)n_cand);
+  call.up(&a.cand_sig, cand_sig, (size_t)n_cand);
+  call.up(&a.cand_raw, cand_author_raw, (size_t)n_cand);
+  call.up(&a.mood, mood, mood ? (size_t)n_cand * kMoodFeatures : 0);
+  call.up(&a.mood_ok, mood_ok, mood ? (size_t)n_cand : 0);
+  call.up(&a.target_mood, target_mood, mood ? (size_t)kMoodFeatures : 0);
+  call.down(&a.out_count, 1);
+  call.down(&a.out_pos, (size_t)n_out);
+  call.down(&a.out_mood, mood ? (size_t)n_out : 0);
+  call.device(&a.seen, (size_t)n_sig, 0xff);  // -1: no signature let through yet
+  call.device(&a.raw_mark, (size_t)n_raw, 0xff);
+  call.device(&a.raw_count, (size_t)n_raw);
+  call.device(&a.kept, (size_t)n_cand + 1);
+  AM_TRY(call.start());
+  if (!mood) {
+    a.mood = a.target_mood = nullptr;
+    a.mood_ok = nullptr;
+    a.out_mood = nullptr;
+  }
+  AM_LAUNCH(similar_kernel, 1, kSimilarThreads, 0, st, a);
+  AM_TRY(call.finish());
+  const int32_t cnt = *call.mirror(a.out_count);
+  AM_CHECK(cnt >= 0 && cnt <= n_out, "am_knn_similar: inconsistent result (%d of at most %d)", cnt, n_out);
+  call.get(out_pos, a.out_pos, (size_t)cnt);
+  if (mood) call.get(out_mood, a.out_mood, (size_t)cnt);
   *out_count = cnt;
   return AM_OK;
 }

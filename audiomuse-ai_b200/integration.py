@@ -117,13 +117,15 @@ def make_radius_walk(vm):
     return _radius_walk_get_candidates_b200, _execute_radius_walk_b200
 
 
+SIMILAR_NAMES = ("find_nearest_neighbors_by_id", "find_nearest_neighbors_by_vector", "get_max_distance_for_id")
+
 METRIC_NAMES = ("silhouette_score", "davies_bouldin_score", "calinski_harabasz_score")
 
 
 def apply(clap=None, voyager_manager=None, clustering=None, allow_sklearn_fallback: bool = True,
           clustering_helper=None, song_alchemy=None, app_map=None, artist_gmm_manager=None,
           gaussian_mixture=None, radius_walk=None, path_manager=None, app_path=None, analysis=None, alchemy=None,
-          app_alchemy=None) -> None:
+          app_alchemy=None, similar=None, app_voyager=None, sonic_fingerprint=None) -> None:
     """clap / voyager_manager / clustering / clustering_helper: the reference's already imported tasks.* modules (pass
     only the ones to patch).  allow_sklearn_fallback keeps the reference's contract that a failing GPU k-means silently
     falls back to scikit-learn (tasks/clustering_gpu.py:130-148); this repository's own tests run with it off so a
@@ -145,7 +147,12 @@ def apply(clap=None, voyager_manager=None, clustering=None, allow_sklearn_fallba
     the Song Path endpoint to use it.  alchemy (the reference's tasks.song_alchemy) gets the device Song Alchemy as
     song_alchemy (alchemy.make_song_alchemy, over the voyager_manager module whose functions song_alchemy imported);
     app_alchemy binds that name when it is imported (app_alchemy.py:4), so pass it too for the Alchemy endpoint to use
-    it.  song_alchemy= alone still only replaces _project_with_umap.  analysis (the reference's tasks.analysis) gets track_features.LibrosaFacade as
+    it.  song_alchemy= alone still only replaces _project_with_umap.  similar (the reference's tasks.voyager_manager
+    again) gets the device plain similar-tracks requests as find_nearest_neighbors_by_id,
+    find_nearest_neighbors_by_vector and get_max_distance_for_id (similar_tracks.make_*); app_voyager
+    (app_voyager.py:10-12) and sonic_fingerprint (tasks.sonic_fingerprint_manager, :7) bind those names when they are
+    imported, so pass them too for their endpoints to use them, and app_path (app_path.py:6) gets
+    find_nearest_neighbors_by_vector when similar= is passed with it.  analysis (the reference's tasks.analysis) gets track_features.LibrosaFacade as
     its `librosa`: analyze_track's beat_track, rms and chroma_stft (:344-348) run on the device, every other librosa use
     of the module goes to the librosa it imported; sys.modules["librosa"] is left alone."""
     if analysis is not None:
@@ -163,8 +170,23 @@ def apply(clap=None, voyager_manager=None, clustering=None, allow_sklearn_fallba
     if radius_walk is not None:
         for name, fn in zip(RADIUS_WALK_NAMES, make_radius_walk(radius_walk)):
             setattr(radius_walk, name, fn)
-    if app_path is not None and path_manager is None:
+    if app_path is not None and path_manager is None and similar is None:
         raise ValueError("app_path= takes the device song path from path_manager=: pass both")
+    if (app_voyager is not None or sonic_fingerprint is not None) and similar is None:
+        raise ValueError("app_voyager= / sonic_fingerprint= take the device similar-tracks requests from similar=: "
+                         "pass it too")
+    if similar is not None:
+        from . import similar_tracks
+
+        fns = {name: getattr(similar_tracks, "make_" + name)(similar) for name in SIMILAR_NAMES}
+        for name, fn in fns.items():
+            setattr(similar, name, fn)
+            if app_voyager is not None:
+                setattr(app_voyager, name, fn)
+        if sonic_fingerprint is not None:
+            sonic_fingerprint.find_nearest_neighbors_by_vector = fns["find_nearest_neighbors_by_vector"]
+        if app_path is not None:
+            app_path.find_nearest_neighbors_by_vector = fns["find_nearest_neighbors_by_vector"]
     if path_manager is not None:
         from . import song_path
 

@@ -368,6 +368,51 @@ class Index:
         return (pos[:k].copy(), status[:k].copy(), dsub[:k].copy(), dadd[:k].copy(),
                 None if out_rows is None else out_rows[:k].copy())
 
+    # ------------------------------------------------------------------ similar tracks (voyager_manager.py:1493-1702)
+    def similar(self, cfg, target_id, target_sig, cand_ids, cand_sig, cand_author_raw, n_sig, n: int, mood=None,
+                mood_ok=None, target_mood=None):
+        """A plain similar-tracks request after its k-NN query in one device call (am_knn_similar).  cfg: an
+        _lib.SimilarCfg.  target_id: the by-id request's target (index id), or None for a by-vector request;
+        target_sig its signature key (-1: none).  cand_ids are index ids in k-NN order (ids not in the index have no
+        vector), cand_sig / cand_author_raw the dense keys the header describes, n_sig the number of signature keys.
+        mood f64[n_cand, 6] / mood_ok / target_mood f64[6] run the mood stage, mood=None skips it.  Returns (positions in
+        cand_ids of the survivors, in order; their f64 mood distances, or None without the mood stage)."""
+        cand = self._rows_of(cand_ids, strict=False)
+        sig = np.ascontiguousarray(cand_sig, dtype=np.int32)
+        raw = np.ascontiguousarray(cand_author_raw, dtype=np.int32)
+        if sig.shape != cand.shape or raw.shape != cand.shape or cand.ndim != 1:
+            raise ValueError("candidate arrays differ in length")
+        target = -1 if target_id is None else self._row_of(target_id)
+        if mood is not None:
+            mood = np.ascontiguousarray(mood, dtype=np.float64).reshape(len(cand), 6)
+            mood_ok = np.ascontiguousarray(mood_ok, dtype=np.uint8)
+            target_mood = np.ascontiguousarray(target_mood, dtype=np.float64).reshape(6)
+            if mood_ok.shape != cand.shape:
+                raise ValueError("mood_ok and the candidates differ in length")
+        n_out = max(1, min(len(cand), int(n)))
+        count = C.c_int32(0)
+        pos = np.empty(n_out, dtype=np.int32)
+        md = np.empty(n_out, dtype=np.float64)
+        h = self._ensure_built()
+        _lib.check(_lib.load().am_knn_similar(
+            h, C.byref(cfg), target, int(target_sig), len(cand), _lib.ptr(cand), _lib.ptr(sig), _lib.ptr(raw), int(n_sig),
+            None if mood is None else _lib.ptr(mood), None if mood is None else _lib.ptr(mood_ok),
+            None if mood is None else _lib.ptr(target_mood), int(n), C.byref(count), _lib.ptr(pos), _lib.ptr(md)))
+        k = count.value
+        return pos[:k].copy(), (None if mood is None else md[:k].copy())
+
+    def farthest(self, id):
+        """get_max_distance_for_id's answer for the stored vector of `id` in one pass (am_knn_farthest): (the largest
+        float32 distance query(k=len) would return to another id, that id), or (0.0, None) when there is none."""
+        row = self._row_of(id)
+        q = self.get_vector(id)
+        out_row, out_dist = C.c_int64(-1), C.c_float(0.0)
+        h = self._ensure_built()
+        _lib.check(_lib.load().am_knn_farthest(h, _lib.ptr(q), row, C.byref(out_row), C.byref(out_dist)))
+        if out_row.value < 0:
+            return 0.0, None
+        return float(out_dist.value), int(self._ids[out_row.value])
+
     # ------------------------------------------------------------------ persistence
     def as_bytes(self) -> bytes:
         with self._mu:

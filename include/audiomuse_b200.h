@@ -297,6 +297,41 @@ AM_API int am_knn_alchemy(const am_index* idx, const am_alchemy_cfg* cfg, const 
                           const int32_t* cand_author_raw, int n_sig, int n_excl, const int64_t* excl_rows,
                           int32_t* out_count, int32_t* out_pos, unsigned char* out_status, double* out_dsub,
                           double* out_dadd, float* out_rows);
+/* The configuration voyager_manager.py reads at call time, for am_knn_similar.  metric: config.VOYAGER_METRIC as
+ * get_direct_distance reads it, 0 angular (1 - cos) or 1 euclidean (||a - b||). */
+typedef struct am_similar_cfg {
+  int metric;
+  int filter_lookback;      /* DUPLICATE_DISTANCE_CHECK_LOOKBACK (<= 0: no distance filter) */
+  int filter_batch;         /* BATCH_SIZE_VECTOR_OPS */
+  int cap;                  /* the raw-author cap: MAX_SONGS_PER_ARTIST when eliminate_duplicates, else 0 (off) */
+  int mood_sum;             /* how the mood distance sums, as Python's sum() of floats: 1 compensated (CPython >= 3.12,
+                               Neumaier), 0 left to right (older versions) */
+  double filter_threshold;  /* DUPLICATE_DISTANCE_THRESHOLD_* for metric */
+  double mood_threshold;    /* MOOD_SIMILARITY_THRESHOLD */
+} am_similar_cfg;
+
+/* A plain similar-tracks request after its k-NN query, in one call: find_nearest_neighbors_by_id without the radius
+ * walk (voyager_manager.py:1493-1545) when target_row >= 0, find_nearest_neighbors_by_vector (:1589-1657) when it is -1.
+ * The candidates are the query's list in order: cand_rows their stored rows (-1: no vector), cand_sig the dense key of
+ * their (title, author) signature after strip().lower() (-1: no details), cand_author_raw a dense key of their raw
+ * author (-1: falsy).  Runs the distance filter (a by-id request's target heads the list, as the first kept item of the
+ * window, and is never output), the same-song dedupe (starting with signature target_sig already seen, -1: none), the
+ * mood stage when mood is not NULL, the raw-author cap, and stops after n survivors.  Mood stage: mood f64[n_cand, 6]
+ * holds each candidate's danceable, aggressive, happy, party, relaxed and sad (0 where missing), mood_ok u8[n_cand] 1
+ * where its features parsed (0: the candidate is dropped), target_mood f64[6] the target's; a candidate is kept when
+ * sum(|target - candidate|) / 6, summed in that order in float64 as cfg->mood_sum says, is <= cfg->mood_threshold.  *out_count receives the
+ * survivors (<= min(n_cand, n)); out_pos their entries in the candidate arrays in order, out_mood (mood stage only)
+ * their mood distances.  Re-entrant. */
+AM_API int am_knn_similar(const am_index* idx, const am_similar_cfg* cfg, int64_t target_row, int target_sig,
+                          int n_cand, const int64_t* cand_rows, const int32_t* cand_sig, const int32_t* cand_author_raw,
+                          int n_sig, const double* mood, const unsigned char* mood_ok, const double* target_mood, int n,
+                          int32_t* out_count, int32_t* out_pos, double* out_mood);
+/* get_max_distance_for_id (voyager_manager.py:1660-1702) in one pass over the stored rows: of the distances
+ * am_knn_query would return for `query` f32[d] with k = N, the largest float32 one, skipping exclude_row (-1: none);
+ * among rows at that float32 value the one query() lists first (smaller float64 distance, then smaller row).
+ * *out_row receives its row and *out_dist that float32 distance; with no other row, -1 and 0.  Deterministic. */
+AM_API int am_knn_farthest(const am_index* idx, const float* query, int64_t exclude_row, int64_t* out_row,
+                           float* out_dist);
 /* n stored rows in one device gather + one copy: out f32[n, d] */
 AM_API int am_knn_get_vectors(const am_index* idx, const int64_t* ids, int n, float* out);
 AM_API int am_knn_query_dev(const am_index* idx, const float* Q_dev, int nq, int k, int mode,
