@@ -151,6 +151,7 @@ SIGNATURES = {
     "am_artist_gmm_fit": (_i, [_vp, _i64, _i, _vp, _i, _vp, _vp, _i, _i, C.c_double, C.c_double, _vp, _i64]
                           + [_vp] * 12),
     "am_gmm_full_fit": (_i, [_vp, _i64, _i, _i, _i, _i, C.c_double, C.c_double, _vp, _i64] + [_vp] * 15),
+    "am_gmm_fit": (_i, [_vp, _i64, _i, _i, _i, _i, _i, C.c_double, C.c_double, _vp, _i64] + [_vp] * 15),
     "am_track_features_plan_create": (_i, [_i, _P(_vp)]),
     "am_track_features_plan_free": (None, [_vp]),
     "am_track_features_plan_info": (_i, [_vp, _P(_i), _P(_i), _P(_i)]),

@@ -24,6 +24,8 @@ so a missing CUDA library can never masquerade as the GPU path).
         (am_gmm_full_fit, csrc/gmm.cu): scikit-learn's k-means++ initialisation on the generator's own draws and float64
         EM on the tensor cores.  Sets means_, weights_, covariances_, precisions_cholesky_, lower_bound_,
         lower_bounds_, n_iter_, converged_, labels_, using_gpu.  Only covariance_type='full' runs on the device.
+    GPUGaussianMixtureAnyCovariance(...): the same for all four covariance types ('diag', 'tied' and 'spherical'
+        through am_gmm_fit); integration.apply(gaussian_mixture=..., gmm_all_covariance_types=True) installs it.
 """
 from __future__ import annotations
 
@@ -508,6 +510,8 @@ GMM_MAX_D = 256             # AM_GMM_MAX_D
 GMM_MAX_K = 512             # AM_GMM_MAX_K
 GMM_MAX_COMPONENTS = 65535  # AM_GMM_MAX_COMPONENTS: n_init n_components
 GMM_COVARIANCE_TYPE = "full"
+GMM_COVARIANCE_TYPES = {"diag": 1, "tied": 2, "spherical": 3}   # AM_GMM_DIAG, AM_GMM_TIED, AM_GMM_SPHERICAL; 'full' is
+                                                                 # am_gmm_full_fit
 _ILL_DEFINED = ("Fitting the mixture model failed because some components have ill-defined empirical covariance (for "
                 "instance caused by singleton or collapsed samples). Try to decrease the number of components, increase "
                 "reg_covar, or scale the input data.")
@@ -516,6 +520,8 @@ _ILL_DEFINED = ("Fitting the mixture model failed because some components have i
 @dataclass
 class GmmFit:
     """One GaussianMixture fit: the best init's parameters (float64), its bounds and the labels of one more E-step.
+    covariances and precisions_cholesky have scikit-learn's shapes for the fit's covariance type: full [K, d, d], tied
+    [d, d], diag [K, d], spherical [K].
     With intermediates=True also kpp i32[n_init, K] (the k-means++ rows) and, per init, lower_bounds
     f64[n_init, max_iter] (NaN after its n_iter), n_iter and converged."""
     weights: np.ndarray
@@ -572,12 +578,14 @@ def _check_gmm_params(n_components, n_init, max_iter, tol, reg_covar):
 
 
 def gmm_fit(X, n_components, n_init=10, max_iter=100, tol=1e-3, reg_covar=1e-4, random_state=None,
-            intermediates=False) -> GmmFit:
-    """GaussianMixture(n_components, covariance_type='full', init_params='k-means++', n_init, max_iter, tol,
-    reg_covar, random_state).fit_predict(X) on the device, in float64 whatever X's dtype.  The k-means++ draws come
-    from check_random_state(random_state) on the host, so the generator ends where scikit-learn's fit leaves it.
-    ValueError for invalid input (before any device work) and for an ill-defined covariance; B200Error when the
-    device fails."""
+            intermediates=False, covariance_type="full") -> GmmFit:
+    """GaussianMixture(n_components, covariance_type, init_params='k-means++', n_init, max_iter, tol, reg_covar,
+    random_state).fit_predict(X) on the device, in float64 whatever X's dtype: am_gmm_full_fit for 'full', am_gmm_fit
+    for 'diag', 'tied' and 'spherical'.  The k-means++ draws come from check_random_state(random_state) on the host,
+    so the generator ends where scikit-learn's fit leaves it.  ValueError for invalid input (before any device work)
+    and for an ill-defined covariance; B200Error when the device fails."""
+    if covariance_type != "full" and covariance_type not in GMM_COVARIANCE_TYPES:
+        raise ValueError(f"covariance_type must be one of 'full', 'tied', 'diag', 'spherical', got {covariance_type!r}")
     _check_gmm_params(n_components, n_init, max_iter, tol, reg_covar)
     X = _check_gmm_input(X, int(n_components))
     N, d = X.shape
@@ -586,8 +594,9 @@ def gmm_fit(X, n_components, n_init=10, max_iter=100, tol=1e-3, reg_covar=1e-4, 
     draws = np.ascontiguousarray(kpp_draws(random_state, K, n_init))
     w = np.empty(K)
     m = np.empty((K, d))
-    cv = np.empty((K, d, d))
-    pc = np.empty((K, d, d))
+    shape = {"full": (K, d, d), "tied": (d, d), "diag": (K, d), "spherical": (K,)}[covariance_type]
+    cv = np.empty(shape)
+    pc = np.empty(shape)
     lbs = np.empty(max_iter)
     it, conv, best, bad = C.c_int32(0), C.c_int32(0), C.c_int32(0), C.c_int32(0)
     labels = np.empty(N, np.int64)
@@ -597,10 +606,14 @@ def gmm_fit(X, n_components, n_init=10, max_iter=100, tol=1e-3, reg_covar=1e-4, 
     iit = np.empty(n_init, np.int32) if intermediates else None
     iconv = np.empty(n_init, np.int32) if intermediates else None
     opt = lambda a: None if a is None else _lib.ptr(a)   # noqa: E731
-    _lib.check(lib.am_gmm_full_fit(
-        _lib.ptr(X), N, d, K, n_init, max_iter, float(tol), float(reg_covar), _lib.ptr(draws), len(draws),
-        _lib.ptr(w), _lib.ptr(m), _lib.ptr(cv), _lib.ptr(pc), _lib.ptr(lbs), C.byref(it), C.byref(conv), C.byref(best),
-        _lib.ptr(labels), C.byref(bad), opt(kpp), opt(ilb), opt(iit), opt(iconv), _lib.ptr(ms)))
+    outputs = (_lib.ptr(w), _lib.ptr(m), _lib.ptr(cv), _lib.ptr(pc), _lib.ptr(lbs), C.byref(it), C.byref(conv),
+               C.byref(best), _lib.ptr(labels), C.byref(bad), opt(kpp), opt(ilb), opt(iit), opt(iconv), _lib.ptr(ms))
+    if covariance_type == "full":
+        _lib.check(lib.am_gmm_full_fit(_lib.ptr(X), N, d, K, n_init, max_iter, float(tol), float(reg_covar),
+                                       _lib.ptr(draws), len(draws), *outputs))
+    else:
+        _lib.check(lib.am_gmm_fit(_lib.ptr(X), N, d, K, GMM_COVARIANCE_TYPES[covariance_type], n_init, max_iter,
+                                  float(tol), float(reg_covar), _lib.ptr(draws), len(draws), *outputs))
     if bad.value:
         raise ValueError(_ILL_DEFINED)
     n = int(it.value)
@@ -613,8 +626,11 @@ def gmm_fit(X, n_components, n_init=10, max_iter=100, tol=1e-3, reg_covar=1e-4, 
 
 class GPUGaussianMixture:
     """tasks/clustering_gpu.py:284-309 (sklearn.mixture.GaussianMixture there) on the device through gmm_fit, for
-    covariance_type='full' and init_params='k-means++'; other values are refused with ValueError.  max_iter and tol
-    are scikit-learn's defaults.  The clustering task reads means_ for the centres (clustering_helper.py:324-325)."""
+    the covariance types in DEVICE_COVARIANCE_TYPES and init_params='k-means++'; other values are refused with
+    ValueError.  max_iter and tol are scikit-learn's defaults.  The clustering task reads means_ for the centres
+    (clustering_helper.py:324-325)."""
+
+    DEVICE_COVARIANCE_TYPES = ("full",)
 
     def __init__(self, n_components, covariance_type="full", init_params="k-means++", n_init=10, random_state=None,
                  reg_covar=1e-4, max_iter=100, tol=1e-3):
@@ -639,8 +655,9 @@ class GPUGaussianMixture:
         self.using_gpu = False
 
     def _validate(self, X):
-        if self.covariance_type != "full":
-            raise ValueError(f"covariance_type={self.covariance_type!r} is not supported on the GPU (only 'full')")
+        if self.covariance_type not in self.DEVICE_COVARIANCE_TYPES:
+            raise ValueError(f"covariance_type={self.covariance_type!r} is not supported on the GPU (only "
+                             f"{', '.join(map(repr, self.DEVICE_COVARIANCE_TYPES))})")
         if self.init_params != "k-means++":
             raise ValueError(f"init_params={self.init_params!r} is not supported on the GPU (only 'k-means++')")
         _check_gmm_params(self.n_components, self.n_init, self.max_iter, self.tol, self.reg_covar)
@@ -654,7 +671,8 @@ class GPUGaussianMixture:
         state = rs.get_state() if isinstance(rs, np.random.RandomState) else None
         try:
             f = gmm_fit(X64, int(self.n_components), n_init=int(self.n_init), max_iter=int(self.max_iter),
-                        tol=self.tol, reg_covar=self.reg_covar, random_state=rs)
+                        tol=self.tol, reg_covar=self.reg_covar, random_state=rs,
+                        covariance_type=self.covariance_type)
             dt = X.dtype if isinstance(X, np.ndarray) and X.dtype in (np.float32, np.float64) else np.float64
             self.weights_, self.means_ = f.weights.astype(dt), f.means.astype(dt)
             self.covariances_, self.precisions_cholesky_ = f.covariances.astype(dt), f.precisions_cholesky.astype(dt)
@@ -687,6 +705,15 @@ class GPUGaussianMixture:
     def fit(self, X):
         self.fit_predict(X)
         return self
+
+
+class GPUGaussianMixtureAnyCovariance(GPUGaussianMixture):
+    """GPUGaussianMixture for every covariance type the clustering task's GMM_COVARIANCE_TYPE may name: 'full',
+    'tied', 'diag' and 'spherical' all fit on the device, and covariances_ / precisions_cholesky_ have scikit-learn's
+    shapes for the type, in the input's dtype.  The generator handling, the B200_ALLOW_SKLEARN_FALLBACK path (which
+    fits scikit-learn with the same type) and the ConvergenceWarning are GPUGaussianMixture's."""
+
+    DEVICE_COVARIANCE_TYPES = ("full", "tied", "diag", "spherical")
 
 
 def get_clustering_model(method, params, use_gpu=False):

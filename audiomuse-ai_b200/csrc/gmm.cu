@@ -17,6 +17,21 @@
 //             one CTA per (component, 32-column panel) by forward substitution (trinv_kernel); a pivot <= 0 or not
 //             finite sets the ill-defined flag instead of failing the launch
 //
+// am_gmm_fit runs the same seeding, initialisation, normaliser, convergence loop, best-init choice and labelling for
+// covariance_type 'diag', 'tied' and 'spherical'; only the covariance M-step, the precision factor and the E-step differ,
+// each in scikit-learn 1.9's operation order:
+//
+//   diag      resp^T (X o X) on DMMA (gram_kernel<false> on a device copy of X o X), cov = (that / nk - mu^2) + reg,
+//             prec_chol = 1 / sqrt(cov) (diag_cov_kernel); the E-step runs the DMMA products X (mu o prec)^T and
+//             (X o X) prec^T in one kernel and adds them as (sum mu^2 prec - 2 X (mu o prec)^T) + (X o X) prec^T
+//             (lin_estep_kernel)
+//   spherical the diag covariance averaged over the features; the E-step product is X mu^T, scaled by the precision
+//             after the dot product, plus |x|^2 prec
+//   tied      X^T X once per fit (gram_kernel<true> with unit weights and zero means), then per init
+//             cov = (X^T X - sum_k nk mu mu^T) / sum nk + reg (tied_cov_kernel), the same Cholesky and inverse as 'full'
+//             over n_init matrices, and an E-step that forms X P once per (row tile, init) and loops over the init's K
+//             components in the epilogue (estep_kernel<true>)
+//
 // Every reduction runs in a fixed order and no floating-point atomics are used, so two calls give bit-identical
 // results.
 #include "common.cuh"
@@ -190,6 +205,12 @@ __global__ void fill_kernel(double* __restrict__ p, int64_t n, double v) {
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) p[i] = v;
 }
 
+// xx = x o x elementwise
+__global__ void square_kernel(const double* __restrict__ x, int64_t n, double* __restrict__ xx) {
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
+    xx[i] = x[i] * x[i];
+}
+
 __global__ void onehot_kernel(const int* __restrict__ idx, int C, int64_t Np, double* __restrict__ resp) {
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c < C) resp[c * Np + idx[c]] = 1.0;
@@ -352,6 +373,85 @@ __global__ void weights_kernel(const double* __restrict__ nk, int n_init, int K,
   for (int k = 0; k < K; ++k) w[init * K + k] = nk[init * K + k] / s;
 }
 
+// diag / spherical (sph), one CTA per component, thread j = feature (d <= kThreads): the diag covariance
+// cov_j = ((sum over chunks in order of resp^T (X o X)) / nk - mu_j^2) + reg_covar.
+// diag: cov[c][j], prec[c][j] = 1 / sqrt(cov_j) (any cov_j <= 0 sets *fail), logdet = sum_j log prec_j, and the E-step
+// columns W[c] = [mu o prec_chol^2 | prec_chol^2] (stride 2 dp), cst[c] = sum_j mu_j^2 prec_chol_j^2.
+// spherical: cov[c] = mean_j cov_j, prec[c] = 1 / sqrt(cov[c]) (cov[c] <= 0 sets *fail), logdet = d log prec,
+// scale[c] = prec^2 and cst[c] = sum_j mu_j^2 (the E-step columns are the means themselves).
+__global__ void __launch_bounds__(kThreads)
+diag_cov_kernel(bool sph, const double* __restrict__ part, int S, int Cp, int d64, int d, int dp, int K,
+                const int* __restrict__ active, const double* __restrict__ nk, const double* __restrict__ means,
+                const double* __restrict__ w, double reg_covar, double* __restrict__ cov, double* __restrict__ prec,
+                double* __restrict__ W, double* __restrict__ cst, double* __restrict__ scale,
+                double* __restrict__ logdet, double* __restrict__ logw, int* __restrict__ fail) {
+  __shared__ double red[kWarps];
+  const int c = blockIdx.x, j = threadIdx.x;
+  if (!active[c / K]) return;
+  double v = 0.0, mu = 0.0;
+  if (j < d) {
+    double s = 0.0;
+    for (int q = 0; q < S; ++q) s += part[((int64_t)q * Cp + c) * d64 + j];
+    mu = means[(int64_t)c * dp + j];
+    v = (s / nk[c] - __dmul_rn(mu, mu)) + reg_covar;   // mu^2 rounded before the subtraction, as scikit-learn
+  }
+  if (!sph) {
+    double ld = 0.0, m2 = 0.0;
+    if (j < d) {
+      if (v <= 0.0) *fail = 1;
+      const double pc = 1.0 / sqrt(v), p = pc * pc;
+      cov[(int64_t)c * dp + j] = v;
+      prec[(int64_t)c * dp + j] = pc;
+      W[(int64_t)c * 2 * dp + j] = mu * p;
+      W[(int64_t)c * 2 * dp + dp + j] = p;
+      ld = log(pc);
+      m2 = mu * mu * p;
+    }
+    const double tl = block_sum(ld, red);
+    const double tm = block_sum(m2, red);
+    if (j == 0) {
+      logdet[c] = tl;
+      cst[c] = tm;
+      logw[c] = log(w[c]);
+    }
+  } else {
+    const double tv = block_sum(v, red);
+    const double tm = block_sum(mu * mu, red);
+    if (j == 0) {
+      const double cv = tv / d;
+      if (cv <= 0.0) *fail = 1;
+      const double pc = 1.0 / sqrt(cv);
+      cov[c] = cv;
+      prec[c] = pc;
+      scale[c] = pc * pc;
+      cst[c] = tm;
+      logdet[c] = d * log(pc);
+      logw[c] = log(w[c]);
+    }
+  }
+}
+
+// tied, blockIdx.x = init, blockIdx.y = row i: cov[init][i][j] = (XtX[i][j] - sum_k (nk_k mu_ki) mu_kj) / sum_k nk_k,
+// + reg_covar on the diagonal
+__global__ void __launch_bounds__(kThreads)
+tied_cov_kernel(const double* __restrict__ xtx, int d, int dp, int K, const int* __restrict__ active,
+                const double* __restrict__ nk, const double* __restrict__ means, double reg_covar,
+                double* __restrict__ cov) {
+  const int init = blockIdx.x, i = blockIdx.y;
+  if (!active[init]) return;
+  const double* n = nk + (int64_t)init * K;
+  const double* mu = means + (int64_t)init * K * dp;
+  double tot = 0.0;
+  for (int k = 0; k < K; ++k) tot += n[k];
+  for (int j = threadIdx.x; j < d; j += kThreads) {
+    double m2 = 0.0;
+    for (int k = 0; k < K; ++k) m2 = fma(mu[(int64_t)k * dp + i] * n[k], mu[(int64_t)k * dp + j], m2);
+    double s = (xtx[(int64_t)i * dp + j] - m2) / tot;
+    if (i == j) s += reg_covar;
+    cov[((int64_t)init * dp + i) * dp + j] = s;
+  }
+}
+
 // ---------------------------------------------------------------- Cholesky, inverse, E-step constants
 // One CTA per component: cov = L L^T into Lw (lower, row-major, stride dp), 32-column panels left to right.  A panel's
 // rows are updated with the finished columns (the panel's own rows of L staged in shared memory), then factored in
@@ -440,7 +540,8 @@ trinv_kernel(const double* __restrict__ Lw, int d, int dp, int K, const int* __r
   }
 }
 
-// mP[c] = mu_c P_c, logdet[c] = sum log diag P_c, logw[c] = log w_c
+// mP[c] = mu_c P_c, logdet[c] = sum log diag P_c, logw[c] = log w_c; kTied: P_c is the init's one matrix
+template <bool kTied>
 __global__ void __launch_bounds__(kThreads)
 prep_kernel(const double* __restrict__ means, const double* __restrict__ prec, const double* __restrict__ w, int d,
             int dp, int K, const int* __restrict__ active, double* __restrict__ mP, double* __restrict__ logdet,
@@ -448,7 +549,7 @@ prep_kernel(const double* __restrict__ means, const double* __restrict__ prec, c
   __shared__ double red[kWarps];
   const int c = blockIdx.x;
   if (!active[c / K]) return;
-  const double* P = prec + (int64_t)c * dp * dp;
+  const double* P = prec + (int64_t)(kTied ? c / K : c) * dp * dp;
   const double* mu = means + (int64_t)c * dp;
   double ld = 0.0;
   for (int j = threadIdx.x; j < d; j += kThreads) {
@@ -472,6 +573,9 @@ constexpr int kXLd = 16 + 4;
 // blockIdx.x = 64-row tile, blockIdx.y = component: lp[c][n] = -0.5 (d log 2 pi + |x_n P_c - mu_c P_c|^2) + log det
 // P_c + log w_c.  Warp w owns rows 16 (w & 3) .. + 16 and the n-tiles 2 j + (w >> 2), j < 16, so the skipped
 // below-diagonal slabs cost both column halves alike.
+// kTied: blockIdx.y = init, P is the init's one matrix; X P is formed once and the epilogue runs for each of the
+// init's K components in turn.
+template <bool kTied>
 __global__ void __launch_bounds__(kThreads)
 estep_kernel(const double* __restrict__ X, int64_t Np, int d, int dp, int K, const int* __restrict__ active,
              const double* __restrict__ prec, const double* __restrict__ mP, const double* __restrict__ logdet,
@@ -481,7 +585,7 @@ estep_kernel(const double* __restrict__ X, int64_t Np, int d, int dp, int K, con
   double* Ps = sm + kEM * kXLd;          // [16][dp + 4]
   __shared__ double red[2][kEM];
   const int c = blockIdx.y;
-  if (!active[c / K]) return;
+  if (!active[kTied ? c : c / K]) return;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g = lane >> 2, t = lane & 3;
   const int mt = warp & 3, h = warp >> 2, pld = dp + 4;
   const int64_t r0 = (int64_t)blockIdx.x * kEM;
@@ -514,33 +618,114 @@ estep_kernel(const double* __restrict__ X, int64_t Np, int d, int dp, int K, con
     }
     __syncthreads();
   }
-  const double* m = mP + (int64_t)c * dp;
-  double sa = 0.0, sb = 0.0;
+  // full: one pass for component c; tied: one pass per component of init c, on the same X P
+  for (int k = 0; k < (kTied ? K : 1); ++k) {
+    const int ck = kTied ? c * K + k : c;
+    const double* m = mP + (int64_t)ck * dp;
+    double sa = 0.0, sb = 0.0;
 #pragma unroll
-  for (int j = 0; j < 16; ++j) {
-    const int n0 = (2 * j + h) * 8;
-    if (n0 < dp) {
-      const double m0 = m[n0 + 2 * t], m1 = m[n0 + 2 * t + 1];
-      const double y0 = acc[j][0] - m0, y1 = acc[j][1] - m1, y2 = acc[j][2] - m0, y3 = acc[j][3] - m1;
-      sa = fma(y0, y0, sa);
-      sa = fma(y1, y1, sa);
-      sb = fma(y2, y2, sb);
-      sb = fma(y3, y3, sb);
+    for (int j = 0; j < 16; ++j) {
+      const int n0 = (2 * j + h) * 8;
+      if (n0 < dp) {
+        const double m0 = m[n0 + 2 * t], m1 = m[n0 + 2 * t + 1];
+        const double y0 = acc[j][0] - m0, y1 = acc[j][1] - m1, y2 = acc[j][2] - m0, y3 = acc[j][3] - m1;
+        sa = fma(y0, y0, sa);
+        sa = fma(y1, y1, sa);
+        sb = fma(y2, y2, sb);
+        sb = fma(y3, y3, sb);
+      }
     }
+    sa += __shfl_xor_sync(0xffffffffu, sa, 1);
+    sa += __shfl_xor_sync(0xffffffffu, sa, 2);
+    sb += __shfl_xor_sync(0xffffffffu, sb, 1);
+    sb += __shfl_xor_sync(0xffffffffu, sb, 2);
+    if (t == 0) {
+      red[h][mt * 16 + g] = sa;
+      red[h][mt * 16 + g + 8] = sb;
+    }
+    __syncthreads();
+    if (tid < kEM) {
+      const double sq = red[0][tid] + red[1][tid];
+      lp[(int64_t)ck * Np + r0 + tid] = (-0.5 * (d * kLog2Pi + sq) + logdet[ck]) + logw[ck];
+    }
+    if (kTied) __syncthreads();   // red is reused by the next component
   }
-  sa += __shfl_xor_sync(0xffffffffu, sa, 1);
-  sa += __shfl_xor_sync(0xffffffffu, sa, 2);
-  sb += __shfl_xor_sync(0xffffffffu, sb, 1);
-  sb += __shfl_xor_sync(0xffffffffu, sb, 2);
-  if (t == 0) {
-    red[h][mt * 16 + g] = sa;
-    red[h][mt * 16 + g + 8] = sb;
-  }
-  __syncthreads();
-  if (tid < kEM) {
-    const double sq = red[0][tid] + red[1][tid];
-    lp[(int64_t)c * Np + r0 + tid] = (-0.5 * (d * kLog2Pi + sq) + logdet[c]) + logw[c];
-  }
+}
+
+// diag / spherical (sph) E-step: blockIdx.x = 64-row tile, blockIdx.y = 64-component tile, the products
+// t2[n][c] = sum_k X[n][k] W[c][k] and (diag) t3[n][c] = sum_k X2[n][k] W[c][dp + k] on DMMA (the fragment layout of
+// gram_kernel), X2 the device copy of X o X, W row-major [C][ka] (diag: [mu o prec | prec], ka = 2 dp; spherical: the
+// means, ka = dp).  Then, in scikit-learn's order,
+//   diag:      log_prob = (cst[c] - 2 t2) + t3                               (sum mu^2 prec - 2 X (mu prec)^T + X^2 prec^T)
+//   spherical: log_prob = (cst[c] s - 2 (t2 s)) + xsq[n] s,  s = scale[c]    (sum mu^2 prec - 2 (X mu^T) prec + |x|^2 prec)
+// and lp[c][n] = -0.5 (d log 2 pi + log_prob) + log det + log w, for the components of active inits only.  Every
+// product is rounded before it is added (__dmul_rn keeps nvcc from fusing it into an FMA), as numpy rounds it.
+__global__ void __launch_bounds__(kThreads)
+lin_estep_kernel(bool sph, const double* __restrict__ X, const double* __restrict__ X2, int64_t Np, int d, int dp,
+                 int C, int K, const int* __restrict__ active, const double* __restrict__ W, int ka,
+                 const double* __restrict__ cst, const double* __restrict__ scale, const double* __restrict__ xsq,
+                 const double* __restrict__ logdet, const double* __restrict__ logw, double* __restrict__ lp) {
+  __shared__ __align__(16) double Us[kBK][kLd];
+  __shared__ __align__(16) double Vs[kBK][kLd];
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g = lane >> 2, t = lane & 3;
+  const int64_t r0 = (int64_t)blockIdx.x * kTile;
+  const int c0 = blockIdx.y * kTile;
+  bool any = false;            // a tile of converged inits is left alone
+  for (int q = c0; q < min(C, c0 + kTile); q += K) any |= active[q / K] != 0;
+  if (!any && (min(C, c0 + kTile) - 1) / K != c0 / K) any = active[(min(C, c0 + kTile) - 1) / K] != 0;
+  if (!any) return;
+  const int mt = warp & 3, nh = warp >> 2;
+  // acc += A[rows] W[components][woff ...]^T over the dp columns of A
+  auto product = [&](const double* __restrict__ A, int woff, double (&acc)[4][4]) {
+#pragma unroll
+    for (int a = 0; a < 4; ++a)
+#pragma unroll
+      for (int b = 0; b < 4; ++b) acc[a][b] = 0.0;
+    for (int k0 = 0; k0 < dp; k0 += kBK) {
+#pragma unroll
+      for (int q = 0; q < kBK * kTile / kThreads; ++q) {
+        const int e = tid + q * kThreads;
+        const int r = e & 31, m = e >> 5;    // consecutive threads walk one row's (one component's) k range
+        const int k = k0 + r;
+        Us[r][m] = k < dp ? A[(r0 + m) * dp + k] : 0.0;
+        Vs[r][m] = (c0 + m < C && k < dp) ? W[(int64_t)(c0 + m) * ka + woff + k] : 0.0;
+      }
+      __syncthreads();
+#pragma unroll
+      for (int kk = 0; kk < kBK; kk += 16) {
+        double a[8];
+#pragma unroll
+        for (int i = 0; i < 8; ++i) a[i] = Us[kk + t + 4 * (i >> 1)][mt * 16 + g + 8 * (i & 1)];
+#pragma unroll
+        for (int nt = 0; nt < 4; ++nt) {
+          double b[4];
+#pragma unroll
+          for (int i = 0; i < 4; ++i) b[i] = Vs[kk + t + 4 * i][nh * 32 + nt * 8 + g];
+          dmma(acc[nt], a, b);
+        }
+      }
+      __syncthreads();
+    }
+  };
+  double t2[4][4], t3[4][4];
+  product(X, 0, t2);
+  if (!sph) product(X2, dp, t3);
+#pragma unroll
+  for (int nt = 0; nt < 4; ++nt)
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      const int64_t n = r0 + mt * 16 + g + 8 * (q >> 1);
+      const int c = c0 + nh * 32 + nt * 8 + 2 * t + (q & 1);
+      if (c >= C || !active[c / K]) continue;
+      double lpv;
+      if (sph) {
+        const double s = scale[c];
+        lpv = (__dmul_rn(cst[c], s) - 2.0 * __dmul_rn(t2[nt][q], s)) + __dmul_rn(xsq[n], s);
+      } else {
+        lpv = (cst[c] - 2.0 * t2[nt][q]) + t3[nt][q];
+      }
+      lp[(int64_t)c * Np + n] = (-0.5 * (__dmul_rn(d, kLog2Pi) + lpv) + logdet[c]) + logw[c];
+    }
 }
 
 // thread per (row, init): scipy's logsumexp over the init's K log-probabilities (the maxima split off, the rest
@@ -613,34 +798,43 @@ __global__ void pack_kernel(const double* __restrict__ src, int c0, int K, int r
 
 using namespace am;
 
-extern "C" int am_gmm_full_fit(const double* X, int64_t N, int d, int K, int n_init, int max_iter, double tol,
-                               double reg_covar, const double* draws, int64_t n_draws, double* weights,
-                               double* means, double* covariances, double* precisions_cholesky,
-                               double* lower_bounds, int32_t* n_iter, int32_t* converged, int32_t* best_init,
-                               int64_t* labels, int32_t* ill_defined, int32_t* kpp, double* init_lower_bounds,
-                               int32_t* init_n_iter, int32_t* init_converged, float* phase_ms) {
+namespace {
+
+constexpr int kFull = 0;   // the other types are AM_GMM_DIAG, AM_GMM_TIED and AM_GMM_SPHERICAL
+
+// One fit of any covariance type; fn names the C entry point in error messages.  'full' keeps am_gmm_full_fit's
+// launch sequence; the other types replace the covariance M-step, the precision factor and the E-step only.
+int gmm_fit(const char* fn, int type, const double* X, int64_t N, int d, int K, int n_init, int max_iter, double tol,
+            double reg_covar, const double* draws, int64_t n_draws, double* weights, double* means,
+            double* covariances, double* precisions_cholesky, double* lower_bounds, int32_t* n_iter,
+            int32_t* converged, int32_t* best_init, int64_t* labels, int32_t* ill_defined, int32_t* kpp,
+            double* init_lower_bounds, int32_t* init_n_iter, int32_t* init_converged, float* phase_ms) {
   using namespace gm;
   AM_CHECK(X && draws && weights && means && covariances && precisions_cholesky && lower_bounds && n_iter &&
                converged && best_init && labels && ill_defined,
-           "am_gmm_full_fit: a required pointer is null");
+           "%s: a required pointer is null", fn);
   AM_CHECK(d >= 1 && d <= AM_GMM_MAX_D && K >= 1 && K <= AM_GMM_MAX_K,
-           "am_gmm_full_fit: need 1 <= d <= %d and 1 <= K <= %d (got d = %d, K = %d)", AM_GMM_MAX_D, AM_GMM_MAX_K, d, K);
-  AM_CHECK(N >= K && N <= ((int64_t)1 << 31) - 64, "am_gmm_full_fit: need K <= N < 2^31 - 64 (got N = %lld, K = %d)",
+           "%s: need 1 <= d <= %d and 1 <= K <= %d (got d = %d, K = %d)", fn, AM_GMM_MAX_D, AM_GMM_MAX_K, d, K);
+  AM_CHECK(N >= K && N <= ((int64_t)1 << 31) - 64, "%s: need K <= N < 2^31 - 64 (got N = %lld, K = %d)", fn,
            (long long)N, K);
   AM_CHECK(n_init >= 1 && max_iter >= 1 && tol >= 0.0 && reg_covar >= 0.0,
-           "am_gmm_full_fit: need n_init >= 1, max_iter >= 1, tol >= 0, reg_covar >= 0");
-  AM_CHECK((int64_t)n_init * K <= AM_GMM_MAX_COMPONENTS,
-           "am_gmm_full_fit: n_init K = %lld components exceeds %d", (long long)n_init * K, AM_GMM_MAX_COMPONENTS);
+           "%s: need n_init >= 1, max_iter >= 1, tol >= 0, reg_covar >= 0", fn);
+  AM_CHECK((int64_t)n_init * K <= AM_GMM_MAX_COMPONENTS, "%s: n_init K = %lld components exceeds %d", fn,
+           (long long)n_init * K, AM_GMM_MAX_COMPONENTS);
   const int L = n_local_trials(K);
   const int64_t per_init = 1 + (int64_t)(K - 1) * L;
-  AM_CHECK(n_draws >= n_init * per_init, "am_gmm_full_fit: %lld draws, K = %d with n_init = %d needs %lld",
+  AM_CHECK(n_draws >= n_init * per_init, "%s: %lld draws, K = %d with n_init = %d needs %lld", fn,
            (long long)n_draws, K, n_init, (long long)(n_init * per_init));
   AM_TRY(ensure_init());
+  const bool full = type == kFull, tied = type == AM_GMM_TIED, sph = type == AM_GMM_SPHERICAL;
+  const bool lin = type == AM_GMM_DIAG || sph;       // the E-step is one product of the rows with per-component columns
 
   const int dp = (d + 15) / 16 * 16, d64 = (dp + kTile - 1) / kTile * kTile;
   const int64_t Np = (N + kEM - 1) / kEM * kEM;
   const int C = n_init * K;
   const int Cp = (C + kTile - 1) / kTile * kTile;
+  const int ka = sph ? dp : 2 * dp;                 // diag / spherical: row stride of the E-step columns W
+  const int Cm = tied ? n_init : C;                 // covariance and precision matrices (tied: one per init)
 
   // the first centre of each init: choice(N, p=uniform) = searchsorted(cumsum(1/N) / last, u, 'right')
   std::vector<int> cand0((size_t)n_init * kMaxTrials, 0);
@@ -668,7 +862,7 @@ extern "C" int am_gmm_full_fit(const double* X, int64_t N, int d, int K, int n_i
   const int cov_tiles = (d64 / kTile) * (d64 / kTile + 1) / 2;
   int64_t mchunk = 0, cchunk = 0;
   const int Sm = split((int64_t)(Cp / kTile) * (d64 / kTile), mchunk);
-  const int Sc = split((int64_t)C * cov_tiles, cchunk);
+  const int Sc = split((int64_t)(tied ? 1 : C) * cov_tiles, cchunk);   // tied: the one X^T X
 
   Stream st;
   AM_TRY(st.create());
@@ -685,9 +879,13 @@ extern "C" int am_gmm_full_fit(const double* X, int64_t N, int d, int K, int n_i
   for (auto& e : ev) AM_CUDA(cudaEventCreate(&e));
 
   const int nb_kpp = (int)((N + kKppRows - 1) / kKppRows);
+  const size_t cov_n = full ? (size_t)C * dp * dp : tied ? (size_t)n_init * dp * dp : sph ? (size_t)C : (size_t)C * dp;
+  const size_t out_n = full ? (size_t)K * d * d : tied ? (size_t)d * d : sph ? (size_t)K : (size_t)K * d;
+  const size_t pack_n = std::max(out_n, (size_t)K * d);   // dOut also stages the means
   DevBuf<double> dX, dXsq, dResp, dClose, dCums, dDist, dPart, dNk, dW, dLogw, dLogdet, dMeans, dMP, dCov, dLw, dPrec,
       dLpn, dLb, dPm, dPc, dOut;
-  DevBuf<int> dCand, dIdx, dActive, dFail;
+  DevBuf<double> dX2, dPm2, dWcol, dCst, dScale, dXtX, dUnit, dZero;   // diag / spherical / tied only
+  DevBuf<int> dCand, dIdx, dActive, dFail, dOn;
   DevBuf<int64_t> dLab;
   AM_TRY(dX.alloc((size_t)Np * dp));
   AM_TRY(dXsq.alloc((size_t)Np));
@@ -701,28 +899,44 @@ extern "C" int am_gmm_full_fit(const double* X, int64_t N, int d, int K, int n_i
   AM_TRY(dLogw.alloc(C));
   AM_TRY(dLogdet.alloc(C));
   AM_TRY(dMeans.alloc((size_t)C * dp));
-  AM_TRY(dMP.alloc((size_t)C * dp));
-  AM_TRY(dCov.alloc((size_t)C * dp * dp));
-  AM_TRY(dLw.alloc((size_t)C * dp * dp));
-  AM_TRY(dPrec.alloc((size_t)C * dp * dp));
+  AM_TRY(dCov.alloc(cov_n));
+  AM_TRY(dPrec.alloc(cov_n));
   AM_TRY(dLpn.alloc((size_t)n_init * Np));
   AM_TRY(dLb.alloc(n_init));
   AM_TRY(dPm.alloc((size_t)Sm * Cp * d64));
-  AM_TRY(dPc.alloc((size_t)Sc * C * d64 * d64));
-  AM_TRY(dOut.alloc((size_t)K * d * d));
+  AM_TRY(dOut.alloc(pack_n));
   AM_TRY(dCand.alloc((size_t)n_init * kMaxTrials));
   AM_TRY(dIdx.alloc(C));
   AM_TRY(dActive.alloc(n_init));
   AM_TRY(dFail.alloc(1));
   AM_TRY(dLab.alloc((size_t)N));
+  if (full || tied) {
+    AM_TRY(dMP.alloc((size_t)C * dp));
+    AM_TRY(dLw.alloc(cov_n));
+    AM_TRY(dPc.alloc((size_t)Sc * (tied ? 1 : C) * d64 * d64));
+  }
+  if (lin) {
+    AM_TRY(dX2.alloc((size_t)Np * dp));
+    AM_TRY(dPm2.alloc((size_t)Sm * Cp * d64));
+    AM_TRY(dCst.alloc(C));
+    if (sph) AM_TRY(dScale.alloc(C));
+    else AM_TRY(dWcol.alloc((size_t)C * ka));
+  }
+  if (tied) {
+    AM_TRY(dXtX.alloc((size_t)dp * dp));
+    AM_TRY(dUnit.alloc((size_t)Np));
+    AM_TRY(dZero.alloc((size_t)dp));
+    AM_TRY(dOn.alloc(1));
+  }
 
   AM_CUDA(cudaMemsetAsync(dX.p, 0, dX.n * 8, s));
   AM_CUDA(cudaMemcpy2DAsync(dX.p, (size_t)dp * 8, X, (size_t)d * 8, (size_t)d * 8, (size_t)N, cudaMemcpyHostToDevice, s));
   AM_CUDA(cudaMemsetAsync(dXsq.p, 0, dXsq.n * 8, s));
   AM_CUDA(cudaMemsetAsync(dMeans.p, 0, dMeans.n * 8, s));
-  AM_CUDA(cudaMemsetAsync(dMP.p, 0, dMP.n * 8, s));
+  if (dMP.p) AM_CUDA(cudaMemsetAsync(dMP.p, 0, dMP.n * 8, s));
   AM_CUDA(cudaMemsetAsync(dPrec.p, 0, dPrec.n * 8, s));
-  AM_CUDA(cudaMemsetAsync(dPc.p, 0, dPc.n * 8, s));
+  if (dPc.p) AM_CUDA(cudaMemsetAsync(dPc.p, 0, dPc.n * 8, s));
+  if (dWcol.p) AM_CUDA(cudaMemsetAsync(dWcol.p, 0, dWcol.n * 8, s));
   AM_CUDA(cudaMemsetAsync(dFail.p, 0, 4, s));
   AM_CUDA(cudaMemcpyAsync(dCand.p, cand0.data(), cand0.size() * 4, cudaMemcpyHostToDevice, s));
   DevBuf<double> dDraws;
@@ -737,7 +951,8 @@ extern "C" int am_gmm_full_fit(const double* X, int64_t N, int d, int K, int n_i
   AM_TRY(allow_dynamic_smem<kpp_dist_kernel>((size_t)kMaxTrials * AM_GMM_MAX_D * 8));
   AM_TRY(allow_dynamic_smem<chol_kernel>(((size_t)kPanel * AM_GMM_MAX_D + (size_t)AM_GMM_MAX_D * (kPanel + 1)) * 8));
   AM_TRY(allow_dynamic_smem<trinv_kernel>((size_t)AM_GMM_MAX_D * kPanel * 8));
-  AM_TRY(allow_dynamic_smem<estep_kernel>(((size_t)kEM * kXLd + 16 * (size_t)(AM_GMM_MAX_D + 4)) * 8));
+  AM_TRY(allow_dynamic_smem<estep_kernel<false>>(((size_t)kEM * kXLd + 16 * (size_t)(AM_GMM_MAX_D + 4)) * 8));
+  AM_TRY(allow_dynamic_smem<estep_kernel<true>>(((size_t)kEM * kXLd + 16 * (size_t)(AM_GMM_MAX_D + 4)) * 8));
 
   // ---- k-means++
   AM_CUDA(cudaEventRecord(ev[0], s));
@@ -752,31 +967,67 @@ extern "C" int am_gmm_full_fit(const double* X, int64_t N, int d, int K, int n_i
   }
   AM_CUDA(cudaMemsetAsync(dResp.p, 0, dResp.n * 8, s));
   AM_LAUNCH(onehot_kernel, ceil_div(C, 256), 256, 0, s, dIdx.p, C, Np, dResp.p);
+  if (lin) AM_LAUNCH(square_kernel, grid_for(dX.n), 256, 0, s, dX.p, (int64_t)dX.n, dX2.p);
+  if (tied) {   // X^T X over all rows, unweighted: gram_kernel<true> with one component, unit weights, zero mean
+    AM_LAUNCH(fill_kernel, grid_for(Np), 256, 0, s, dUnit.p, Np, 1.0);
+    AM_CUDA(cudaMemsetAsync(dZero.p, 0, dZero.n * 8, s));
+    const int one = 1;
+    AM_CUDA(cudaMemcpyAsync(dOn.p, &one, 4, cudaMemcpyHostToDevice, s));
+    AM_LAUNCH(gram_kernel<true>, dim3(1, cov_tiles, Sc), kThreads, 0, s, dX.p, dUnit.p, dZero.p, Np, dp, 1, 1, dOn.p,
+              cchunk, dPc.p);
+    AM_LAUNCH(cov_reduce_kernel, dim3(1, d), 256, 0, s, dPc.p, Sc, 1, d64, d, dp, 1, dOn.p, dUnit.p, 0.0, dXtX.p);
+  }
   AM_CUDA(cudaEventRecord(ev[1], s));
 
-  // ---- M-step (init = true: the initialisation's weights nk / N) and the precision Cholesky factors
+  // ---- M-step (init = true: the initialisation's weights nk / N) and the precision factors
   auto mstep = [&](bool init, cudaEvent_t e_mid) -> int {
     AM_LAUNCH(nk_kernel, C, kThreads, 0, s, dResp.p, Np, K, dActive.p, dNk.p);
     AM_LAUNCH(gram_kernel<false>, dim3(Cp / kTile, d64 / kTile, Sm), kThreads, 0, s, dX.p, dResp.p, dMeans.p, Np, dp,
               C, K, dActive.p, mchunk, dPm.p);
     AM_LAUNCH(means_reduce_kernel, C, d64, 0, s, dPm.p, Sm, Cp, d64, dp, K, dActive.p, dNk.p, dMeans.p);
-    AM_LAUNCH(gram_kernel<true>, dim3(C, cov_tiles, Sc), kThreads, 0, s, dX.p, dResp.p, dMeans.p, Np, dp, C, K,
-              dActive.p, cchunk, dPc.p);
-    AM_LAUNCH(cov_reduce_kernel, dim3(C, d), 256, 0, s, dPc.p, Sc, C, d64, d, dp, K, dActive.p, dNk.p, reg_covar,
-              dCov.p);
+    if (full) {
+      AM_LAUNCH(gram_kernel<true>, dim3(C, cov_tiles, Sc), kThreads, 0, s, dX.p, dResp.p, dMeans.p, Np, dp, C, K,
+                dActive.p, cchunk, dPc.p);
+      AM_LAUNCH(cov_reduce_kernel, dim3(C, d), 256, 0, s, dPc.p, Sc, C, d64, d, dp, K, dActive.p, dNk.p, reg_covar,
+                dCov.p);
+    } else if (tied) {
+      AM_LAUNCH(tied_cov_kernel, dim3(n_init, d), kThreads, 0, s, dXtX.p, d, dp, K, dActive.p, dNk.p, dMeans.p,
+                reg_covar, dCov.p);
+    } else {
+      AM_LAUNCH(gram_kernel<false>, dim3(Cp / kTile, d64 / kTile, Sm), kThreads, 0, s, dX2.p, dResp.p, dMeans.p, Np,
+                dp, C, K, dActive.p, mchunk, dPm2.p);
+    }
     AM_LAUNCH(weights_kernel, ceil_div(n_init, 64), 64, 0, s, dNk.p, n_init, K, dActive.p, init ? (double)N : 0.0,
               dW.p);
     AM_CUDA(cudaEventRecord(e_mid, s));
-    AM_LAUNCH(chol_kernel, C, kThreads, chol_smem, s, dCov.p, d, dp, K, dActive.p, dLw.p, dFail.p);
-    AM_LAUNCH(trinv_kernel, dim3(C, ceil_div(d, kPanel)), kThreads, trinv_smem, s, dLw.p, d, dp, K, dActive.p,
+    if (lin) {
+      AM_LAUNCH(diag_cov_kernel, C, kThreads, 0, s, sph, dPm2.p, Sm, Cp, d64, d, dp, K, dActive.p, dNk.p, dMeans.p, dW.p, reg_covar,
+                dCov.p, dPrec.p, dWcol.p, dCst.p, dScale.p, dLogdet.p, dLogw.p, dFail.p);
+      return AM_OK;
+    }
+    const int kc = full ? K : 1;                     // components per covariance matrix's active flag
+    AM_LAUNCH(chol_kernel, Cm, kThreads, chol_smem, s, dCov.p, d, dp, kc, dActive.p, dLw.p, dFail.p);
+    AM_LAUNCH(trinv_kernel, dim3(Cm, ceil_div(d, kPanel)), kThreads, trinv_smem, s, dLw.p, d, dp, kc, dActive.p,
               dFail.p, dPrec.p);
-    AM_LAUNCH(prep_kernel, C, kThreads, 0, s, dMeans.p, dPrec.p, dW.p, d, dp, K, dActive.p, dMP.p, dLogdet.p,
-              dLogw.p);
+    if (tied)
+      AM_LAUNCH(prep_kernel<true>, C, kThreads, 0, s, dMeans.p, dPrec.p, dW.p, d, dp, K, dActive.p, dMP.p, dLogdet.p,
+                dLogw.p);
+    else
+      AM_LAUNCH(prep_kernel<false>, C, kThreads, 0, s, dMeans.p, dPrec.p, dW.p, d, dp, K, dActive.p, dMP.p, dLogdet.p,
+                dLogw.p);
     return AM_OK;
   };
   auto estep = [&]() -> int {
-    AM_LAUNCH(estep_kernel, dim3((unsigned)(Np / kEM), C), kThreads, estep_smem, s, dX.p, Np, d, dp, K, dActive.p,
-              dPrec.p, dMP.p, dLogdet.p, dLogw.p, dResp.p);
+    if (lin) {
+      AM_LAUNCH(lin_estep_kernel, dim3((unsigned)(Np / kTile), Cp / kTile), kThreads, 0, s, sph, dX.p, sph ? nullptr : dX2.p, Np, d, dp,
+                C, K, dActive.p, sph ? dMeans.p : dWcol.p, ka, dCst.p, dScale.p, dXsq.p, dLogdet.p, dLogw.p, dResp.p);
+    } else if (tied) {
+      AM_LAUNCH(estep_kernel<true>, dim3((unsigned)(Np / kEM), n_init), kThreads, estep_smem, s, dX.p, Np, d, dp, K,
+                dActive.p, dPrec.p, dMP.p, dLogdet.p, dLogw.p, dResp.p);
+    } else {
+      AM_LAUNCH(estep_kernel<false>, dim3((unsigned)(Np / kEM), C), kThreads, estep_smem, s, dX.p, Np, d, dp, K,
+                dActive.p, dPrec.p, dMP.p, dLogdet.p, dLogw.p, dResp.p);
+    }
     return AM_OK;
   };
   auto normalise = [&](int64_t* lab) -> int {
@@ -786,7 +1037,7 @@ extern "C" int am_gmm_full_fit(const double* X, int64_t N, int d, int K, int n_i
     return AM_OK;
   };
 
-  float ms[5] = {0.f, 0.f, 0.f, 0.f, 0.f};   // seeding, E-step, normaliser, M-step, Cholesky
+  float ms[5] = {0.f, 0.f, 0.f, 0.f, 0.f};   // seeding, E-step, normaliser, M-step, precision factors
   auto add = [&](int slot, cudaEvent_t a, cudaEvent_t b) -> int {
     float t = 0.f;
     AM_CUDA(cudaEventElapsedTime(&t, a, b));
@@ -867,13 +1118,44 @@ extern "C" int am_gmm_full_fit(const double* X, int64_t N, int d, int K, int n_i
   AM_LAUNCH(pack_kernel, grid_for((int64_t)K * d), 256, 0, s, dMeans.p, c0, K, 1, d, dp, (int64_t)dp, dOut.p);
   AM_CUDA(cudaMemcpyAsync(means, dOut.p, (size_t)K * d * 8, cudaMemcpyDeviceToHost, s));
   AM_CUDA(cudaStreamSynchronize(s));
-  AM_LAUNCH(pack_kernel, grid_for((int64_t)K * d * d), 256, 0, s, dCov.p, c0, K, d, d, dp, (int64_t)dp * dp, dOut.p);
-  AM_CUDA(cudaMemcpyAsync(covariances, dOut.p, (size_t)K * d * d * 8, cudaMemcpyDeviceToHost, s));
-  AM_CUDA(cudaStreamSynchronize(s));
-  AM_LAUNCH(pack_kernel, grid_for((int64_t)K * d * d), 256, 0, s, dPrec.p, c0, K, d, d, dp, (int64_t)dp * dp, dOut.p);
-  AM_CUDA(cudaMemcpyAsync(precisions_cholesky, dOut.p, (size_t)K * d * d * 8, cudaMemcpyDeviceToHost, s));
-  AM_CUDA(cudaStreamSynchronize(s));
+  // covariances and precisions_cholesky in scikit-learn's shapes: full [K, d, d], tied [d, d], diag [K, d],
+  // spherical [K]
+  const int pc0 = tied ? best : c0, pK = tied ? 1 : K, rows = full || tied ? d : 1, cols = sph ? 1 : d;
+  const int64_t sc = full || tied ? (int64_t)dp * dp : sph ? 1 : dp;
+  for (int q = 0; q < 2; ++q) {
+    AM_LAUNCH(pack_kernel, grid_for((int64_t)out_n), 256, 0, s, q ? dPrec.p : dCov.p, pc0, pK, rows, cols, dp, sc,
+              dOut.p);
+    AM_CUDA(cudaMemcpyAsync(q ? precisions_cholesky : covariances, dOut.p, out_n * 8, cudaMemcpyDeviceToHost, s));
+    AM_CUDA(cudaStreamSynchronize(s));
+  }
   if (phase_ms)
     for (int q = 0; q < 5; ++q) phase_ms[q] = ms[q];
   return AM_OK;
+}
+
+}  // namespace
+
+extern "C" int am_gmm_full_fit(const double* X, int64_t N, int d, int K, int n_init, int max_iter, double tol,
+                               double reg_covar, const double* draws, int64_t n_draws, double* weights,
+                               double* means, double* covariances, double* precisions_cholesky,
+                               double* lower_bounds, int32_t* n_iter, int32_t* converged, int32_t* best_init,
+                               int64_t* labels, int32_t* ill_defined, int32_t* kpp, double* init_lower_bounds,
+                               int32_t* init_n_iter, int32_t* init_converged, float* phase_ms) {
+  return gmm_fit("am_gmm_full_fit", kFull, X, N, d, K, n_init, max_iter, tol, reg_covar, draws, n_draws, weights,
+                 means, covariances, precisions_cholesky, lower_bounds, n_iter, converged, best_init, labels,
+                 ill_defined, kpp, init_lower_bounds, init_n_iter, init_converged, phase_ms);
+}
+
+extern "C" int am_gmm_fit(const double* X, int64_t N, int d, int K, int covariance_type, int n_init, int max_iter,
+                          double tol, double reg_covar, const double* draws, int64_t n_draws, double* weights,
+                          double* means, double* covariances, double* precisions_cholesky, double* lower_bounds,
+                          int32_t* n_iter, int32_t* converged, int32_t* best_init, int64_t* labels,
+                          int32_t* ill_defined, int32_t* kpp, double* init_lower_bounds, int32_t* init_n_iter,
+                          int32_t* init_converged, float* phase_ms) {
+  AM_CHECK(covariance_type == AM_GMM_DIAG || covariance_type == AM_GMM_TIED || covariance_type == AM_GMM_SPHERICAL,
+           "am_gmm_fit: covariance_type %d is not AM_GMM_DIAG, AM_GMM_TIED or AM_GMM_SPHERICAL (full: am_gmm_full_fit)",
+           covariance_type);
+  return gmm_fit("am_gmm_fit", covariance_type, X, N, d, K, n_init, max_iter, tol, reg_covar, draws, n_draws, weights,
+                 means, covariances, precisions_cholesky, lower_bounds, n_iter, converged, best_init, labels,
+                 ill_defined, kpp, init_lower_bounds, init_n_iter, init_converged, phase_ms);
 }

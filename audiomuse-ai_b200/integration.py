@@ -125,7 +125,8 @@ METRIC_NAMES = ("silhouette_score", "davies_bouldin_score", "calinski_harabasz_s
 def apply(clap=None, voyager_manager=None, clustering=None, allow_sklearn_fallback: bool = True,
           clustering_helper=None, song_alchemy=None, app_map=None, artist_gmm_manager=None,
           gaussian_mixture=None, radius_walk=None, path_manager=None, app_path=None, analysis=None, alchemy=None,
-          app_alchemy=None, similar=None, app_voyager=None, sonic_fingerprint=None) -> None:
+          app_alchemy=None, similar=None, app_voyager=None, sonic_fingerprint=None,
+          gmm_all_covariance_types: bool = False) -> None:
     """clap / voyager_manager / clustering / clustering_helper: the reference's already imported tasks.* modules (pass
     only the ones to patch).  allow_sklearn_fallback keeps the reference's contract that a failing GPU k-means silently
     falls back to scikit-learn (tasks/clustering_gpu.py:130-148); this repository's own tests run with it off so a
@@ -139,8 +140,10 @@ def apply(clap=None, voyager_manager=None, clustering=None, allow_sklearn_fallba
     when it is imported, so install_voyager_shim() must come before `import tasks.artist_gmm_manager` and before
     `import tasks.analysis`, which imports it.  gaussian_mixture (the reference's tasks.clustering_gpu again) gets the
     GPU GPUGaussianMixture; get_clustering_model looks the class up at call time (:385).  clustering= alone leaves
-    that class to the reference.  radius_walk (the reference's tasks.voyager_manager again) gets the device radius
-    walk: _radius_walk_get_candidates and _execute_radius_walk are replaced together (make_radius_walk);
+    that class to the reference.  With gmm_all_covariance_types=True it gets GPUGaussianMixtureAnyCovariance instead,
+    which also fits config.GMM_COVARIANCE_TYPE = 'diag', 'tied' and 'spherical' on the device (GPUGaussianMixture
+    refuses them, and the reference's _apply_clustering_model then fits scikit-learn on the CPU).  radius_walk (the
+    reference's tasks.voyager_manager again) gets the device radius walk: _radius_walk_get_candidates and _execute_radius_walk are replaced together (make_radius_walk);
     voyager_manager= alone leaves the walk to the reference.  path_manager (the reference's tasks.path_manager) gets the
     device song path as find_path_between_songs (song_path.make_song_path, over the voyager_manager module whose
     functions path_manager imported); app_path binds that name when it is imported (app_path.py:5), so pass it too for
@@ -155,6 +158,8 @@ def apply(clap=None, voyager_manager=None, clustering=None, allow_sklearn_fallba
     find_nearest_neighbors_by_vector when similar= is passed with it.  analysis (the reference's tasks.analysis) gets track_features.LibrosaFacade as
     its `librosa`: analyze_track's beat_track, rms and chroma_stft (:344-348) run on the device, every other librosa use
     of the module goes to the librosa it imported; sys.modules["librosa"] is left alone."""
+    if gmm_all_covariance_types and gaussian_mixture is None:
+        raise ValueError("gmm_all_covariance_types= selects the class installed by gaussian_mixture=: pass both")
     if analysis is not None:
         from . import track_features
 
@@ -214,7 +219,8 @@ def apply(clap=None, voyager_manager=None, clustering=None, allow_sklearn_fallba
     if gaussian_mixture is not None:
         from . import clustering_gpu as b200_cg
 
-        gaussian_mixture.GPUGaussianMixture = b200_cg.GPUGaussianMixture
+        gaussian_mixture.GPUGaussianMixture = (b200_cg.GPUGaussianMixtureAnyCovariance if gmm_all_covariance_types
+                                               else b200_cg.GPUGaussianMixture)
     if clustering_helper is not None:
         from . import cluster_metrics as b200_cm
 

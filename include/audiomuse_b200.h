@@ -503,6 +503,27 @@ AM_API int am_gmm_full_fit(const double* X, int64_t N, int d, int K, int n_init,
                            int32_t* converged, int32_t* best_init, int64_t* labels, int32_t* ill_defined, int32_t* kpp,
                            double* init_lower_bounds, int32_t* init_n_iter, int32_t* init_converged, float* phase_ms);
 
+/* ------------------------------------------------------------------ clustering-task Gaussian mixture, other covariances
+ * The same fit for covariance_type 'diag', 'tied' or 'spherical' (config.GMM_COVARIANCE_TYPE, which
+ * tasks/clustering_gpu.py:284-309, 385-392 and tasks/clustering_helper.py:295-302 hand to scikit-learn's
+ * GaussianMixture), with am_gmm_full_fit's arguments, limits, seeding, convergence rule, best-init choice and outputs
+ * except for the shapes of the two type-dependent arrays:
+ *   covariance_type      covariances              precisions_cholesky
+ *   AM_GMM_DIAG          f64[K, d]                f64[K, d]             1 / sqrt(cov), elementwise
+ *   AM_GMM_TIED          f64[d, d]                f64[d, d]             upper triangular, as 'full'
+ *   AM_GMM_SPHERICAL     f64[K]                   f64[K]
+ * ill_defined is 1 when a diag or spherical variance was <= 0 or a tied Cholesky pivot was <= 0 or not finite.
+ * Any other covariance_type is AM_ERR_INVALID ('full' runs through am_gmm_full_fit). */
+#define AM_GMM_DIAG 1
+#define AM_GMM_TIED 2
+#define AM_GMM_SPHERICAL 3
+AM_API int am_gmm_fit(const double* X, int64_t N, int d, int K, int covariance_type, int n_init, int max_iter,
+                      double tol, double reg_covar, const double* draws, int64_t n_draws, double* weights,
+                      double* means, double* covariances, double* precisions_cholesky, double* lower_bounds,
+                      int32_t* n_iter, int32_t* converged, int32_t* best_init, int64_t* labels, int32_t* ill_defined,
+                      int32_t* kpp, double* init_lower_bounds, int32_t* init_n_iter, int32_t* init_converged,
+                      float* phase_ms);
+
 /* ------------------------------------------------------------------ track features: tempo, energy, chroma
  * The three librosa 0.11.0 calls of tasks/analysis.py:344-348 (analyze_track) for a batch of tracks:
  * beat.beat_track(y, sr)'s tempo (beat positions are not computed), feature.rms(y) and feature.chroma_stft(y, sr), all
