@@ -166,6 +166,8 @@ DEBUG_SIGNATURES = {
     "am_probe_pipe": (_i, [_i, _i, _i, _P(C.c_double)]),
     "am_debug_block": (_i, [_i] * 10 + [_vp] * 10 + [_P(_i)]),
     "am_debug_kmeans_step": (_i, [_i, _vp, _i64, _i, _i] + [_vp] * 7),
+    "am_debug_encoder_plan": (_i, [_vp, _i] + [_vp] * 5),
+    "am_debug_encoder_trace": (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp]),
 }
 
 _lib = None

@@ -17,6 +17,7 @@
 #include <algorithm>
 #include <cmath>
 #include <cstdio>
+#include <functional>
 #include <memory>
 
 #include "depthwise.cuh"
@@ -768,11 +769,11 @@ static int forward_late(am_model* m, const ForwardPlan& p, int n, cudaStream_t s
   return AM_OK;
 }
 
-// head row program for `n` windows at once; the last op writes out_dev
-static int head_forward(am_model* m, int n, float* out_dev, cudaStream_t st) {
+// head row program for `n` windows at once, ops [lo, hi) (default: all after the pooling); the last op writes out_dev
+static int head_forward(am_model* m, int n, float* out_dev, cudaStream_t st, size_t lo = 1, size_t hi = SIZE_MAX) {
   if (n <= 0) return AM_OK;
   const int64_t rows = n;
-  for (size_t q = 1; q < m->head.size(); ++q) {
+  for (size_t q = lo; q < std::min(hi, m->head.size()); ++q) {
     const HeadOp& h = *m->head[q];
     const bool last = q + 1 == m->head.size();
     float* dst = last ? out_dev : m->regs[(size_t)h.dst]->p;
@@ -844,6 +845,84 @@ static int ensure_workspace(am_model* m, const ForwardPlan& p, int nb, int n_tot
     kmax = std::max(kmax, round_up((size_t)m->reg_dim[r], 8));
   }
   AM_TRY(m->a3.ensure(nt * 3 * kmax));
+  return AM_OK;
+}
+
+// ---------------------------------------------------------------- debug trace (csrc/debug/encoder_debug.cu)
+// Hidden like every symbol without AM_API: libaudiomuse_b200.so does not export these, the debug library calls them.
+
+// the plan for windows of T frames as flat records (include/audiomuse_b200_debug.h, am_debug_encoder_plan)
+int debug_encoder_plan(am_model* m, int T, std::vector<int>* steps, std::vector<int>* layers, std::vector<int>* head,
+                       std::vector<float>* head_eps, int* late_step) {
+  const ForwardPlan* p;
+  AM_TRY(plan_for(m, T, &p));
+  for (const Step& t : p->steps)
+    steps->insert(steps->end(), {t.kind, (int)t.first, (int)t.last, t.in.H, t.in.W, t.out.H, t.out.W, t.cout_p,
+                                 t.starts_block ? 1 : 0});
+  for (const auto& l : m->layers)
+    layers->insert(layers->end(), {l->type, l->cin, l->cout, l->kh, l->kw, l->stride, l->pad_t, l->pad_b, l->pad_l,
+                                   l->pad_r, l->act, l->gate_act, l->cmid, l->h_is_time, l->residual, l->block_start,
+                                   l->cin_p, l->cout_p});
+  for (const auto& h : m->head) {
+    head->insert(head->end(), {h->kind, h->a, h->b, h->dst, h->K, h->N, h->act, h->stride});
+    head_eps->insert(head_eps->end(), {h->eps, h->eps2});
+  }
+  *late_step = (int)p->late_step;
+  return AM_OK;
+}
+
+// One forward pass of B windows (mel_dev) through run_steps / forward_late / head_forward, as am_clap_embed_dev runs
+// it, with every intermediate handed to the callbacks (after a stream synchronise):
+//   on_step(q, out, elems): step q's output for all B windows, bf16 NHWC.  The steps run unchanged: each one is
+//     observed by re-running the prefix of its phase ([0, q], or [late_step, q] on the early phase's late_in) with
+//     step q writing to a separate buffer, in the phase's own window chunks.
+//   on_head(q, out, elems): head op q's result f32 [B, dim] (op 0: the pooling); the ops run one head_forward each.
+// The last op writes the embedding to out_dev.
+int debug_encoder_trace(am_model* m, const float* mel_dev, int B, int T, float* out_dev,
+                        const std::function<int(size_t, const __nv_bfloat16*, size_t)>& on_step,
+                        const std::function<int(size_t, const float*, size_t)>& on_head) {
+  cudaStream_t st = m->stream.s;
+  const ForwardPlan* p;
+  AM_TRY(plan_for(m, T, &p));
+  const int sub = early_sub(*p, B);
+  AM_TRY(ensure_workspace(m, *p, sub, B));
+  size_t most = 0;
+  for (const Step& t : p->steps) most = std::max(most, (size_t)t.out.H * t.out.W * t.cout_p);
+  DevBuf<__nv_bfloat16> obs;
+  AM_TRY(obs.alloc(most * B));
+  const __nv_bfloat16* o;
+  auto observe = [&](size_t q) -> int {
+    AM_CUDA(cudaStreamSynchronize(st));
+    const Step& t = p->steps[q];
+    return on_step(q, obs.p, (size_t)B * t.out.H * t.out.W * t.cout_p);
+  };
+  for (size_t q = 0; q < p->late_step; ++q) {
+    const size_t per = (size_t)p->steps[q].out.H * p->steps[q].out.W * p->steps[q].cout_p;
+    for (int b0 = 0; b0 < B; b0 += sub)
+      AM_TRY(run_steps(m, *p, mel_dev + (size_t)b0 * m->n_mels * T, nullptr, 0, q + 1, std::min(sub, B - b0),
+                       obs.p + (size_t)b0 * per, &o, st));
+    AM_TRY(observe(q));
+  }
+  for (int b0 = 0; b0 < B; b0 += sub)
+    AM_TRY(forward_early(m, *p, mel_dev + (size_t)b0 * m->n_mels * T, std::min(sub, B - b0), b0, st));
+  const size_t per_win = (size_t)p->split.H * p->split.W * p->split_c;
+  for (size_t q = p->late_step; q < p->steps.size(); ++q) {
+    const size_t per = (size_t)p->steps[q].out.H * p->steps[q].out.W * p->steps[q].cout_p;
+    for (int b0 = 0; b0 < B; b0 += m->late_sub)
+      AM_TRY(run_steps(m, *p, nullptr, m->late_in.p + (size_t)b0 * per_win, p->late_step, q + 1,
+                       std::min(m->late_sub, B - b0), obs.p + (size_t)b0 * per, &o, st));
+    AM_TRY(observe(q));
+  }
+  AM_TRY(forward_late(m, *p, B, st));
+  AM_CUDA(cudaStreamSynchronize(st));
+  AM_TRY(on_head(0, m->regs[(size_t)m->head[0]->dst]->p, (size_t)B * m->head_cin));
+  for (size_t q = 1; q < m->head.size(); ++q) {
+    AM_TRY(head_forward(m, B, out_dev, st, q, q + 1));
+    AM_CUDA(cudaStreamSynchronize(st));
+    const HeadOp& h = *m->head[q];
+    const float* r = q + 1 == m->head.size() ? out_dev : m->regs[(size_t)h.dst]->p;
+    AM_TRY(on_head(q, r, (size_t)B * m->reg_dim[(size_t)h.dst]));
+  }
   return AM_OK;
 }
 

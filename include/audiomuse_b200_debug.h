@@ -41,6 +41,24 @@ AM_API int am_debug_kmeans_step(int path, const float* X_dev, int64_t N, int d, 
                                 int32_t* labels_dev, float* sums_dev, float* counts_dev, float* inertia_dev,
                                 float* dist_dev, void* stream);
 
+/* debug: the encoder's execution plan for windows of T frames.  counts[4] = steps, late_step (the first step of the
+ * late phase), layers, head ops.  The arrays may be NULL; else, sized from counts:
+ *   steps  [n_steps, 9]:  kind (kStepStem .. kStepSqueezeExcite), first, last layer, in H, in W, out H, out W, cout_p,
+ *                         starts_block
+ *   layers [n_layers, 18]: type, cin, cout, kh, kw, stride, pad_t, pad_b, pad_l, pad_r, act, gate_act, cmid,
+ *                         h_is_time, residual, block_start, cin_p, cout_p
+ *   head   [n_head, 8]:   kind, a, b, dst, K, N (the width it writes), act, stride;  head_eps [n_head, 2]: eps, eps2 */
+#define AM_TRACE_STEP_INTS 9
+#define AM_TRACE_LAYER_INTS 18
+#define AM_TRACE_HEAD_INTS 8
+AM_API int am_debug_encoder_plan(am_model* m, int T, int* counts, int* steps, int* layers, int* head, float* head_eps);
+/* debug: one forward pass of B windows of the host log-mel [B, n_mels, T] through the encoder's own dispatch, traced.
+ * steps_out: every step's output in plan order, each raw bf16 NHWC [B, out H, out W, cout_p] (padded channels
+ * included); head_out: every head op's result in program order, each f32 [B, N] (op 0: the pooling); emb [B, emb]:
+ * the embedding, as am_clap_embed computes it.  Synchronises before it returns. */
+AM_API int am_debug_encoder_trace(am_model* m, const float* mel, int B, int T, uint16_t* steps_out, float* head_out,
+                                  float* emb);
+
 #ifdef __cplusplus
 }
 #endif

@@ -35,14 +35,15 @@ def test_library_exports_every_declared_symbol(lib):
     assert set(_lib.SIGNATURES) == set(names), set(_lib.SIGNATURES) ^ set(names)
 
 
-def test_product_library_ships_no_debug_entry_points(lib):
-    """The probes, self tests and debug entry points (include/audiomuse_b200_debug.h, am_debug_kmeans_step among
-    them) live in libaudiomuse_b200_debug.so only."""
+def test_debug_and_trace_entry_points_live_in_the_debug_library_only(lib):
+    """The probes, self tests, debug entry points and the encoder trace (include/audiomuse_b200_debug.h,
+    am_debug_kmeans_step and am_debug_encoder_trace among them) live in libaudiomuse_b200_debug.so only."""
     from audiomuse_ai_b200 import _lib
     txt = open(os.path.join(ROOT, "include", "audiomuse_b200_debug.h")).read()
     dbg_names = sorted(set(re.findall(r"AM_API\s+[\w\s\*]+?\b(am_\w+)\s*\(", txt)))
     assert set(dbg_names) == set(_lib.DEBUG_SIGNATURES) == {"am_selftest_gemm", "am_bench_gemm", "am_probe_pipe",
-                                                            "am_debug_block", "am_debug_kmeans_step"}
+                                                            "am_debug_block", "am_debug_kmeans_step",
+                                                            "am_debug_encoder_plan", "am_debug_encoder_trace"}
     dbg = _lib.load_debug()
     for n in dbg_names:
         assert hasattr(dbg, n)
