@@ -24,7 +24,7 @@ from collections import namedtuple
 import numpy as np
 
 from . import _lib
-from .song_path import Keys, query_size, signature
+from .by_vector import Keys, candidate_keys, chain_config, query_size
 
 logger = logging.getLogger(__name__)
 
@@ -36,19 +36,13 @@ _SIDES = (_Side("__add_id__", "__add_anchor__", "__add_mood__", "__add_artist_co
 
 def config(sa, vm, n, subtract_distance, skip_chain):
     """am_alchemy_cfg and the subtract threshold from the two modules' configuration as they hold it now."""
-    ed = bool(vm.SIMILARITY_ELIMINATE_DUPLICATES_DEFAULT)
-    cap = vm.MAX_SONGS_PER_ARTIST
-    v_ang, p_ang = vm.VOYAGER_METRIC == "angular", sa.config.PATH_DISTANCE_METRIC == "angular"
+    p_ang = sa.config.PATH_DISTANCE_METRIC == "angular"
     if subtract_distance is None:
         subtract_distance = (sa.config.ALCHEMY_SUBTRACT_DISTANCE_ANGULAR if p_ang
                              else sa.config.ALCHEMY_SUBTRACT_DISTANCE_EUCLIDEAN)
     return _lib.AlchemyCfg(
-        voyager_metric=0 if v_ang else 1, path_metric=0 if p_ang else 1,
-        filter_lookback=int(vm.DUPLICATE_DISTANCE_CHECK_LOOKBACK), filter_batch=int(vm.BATCH_SIZE_VECTOR_OPS),
-        voyager_cap=int(cap) if ed and cap is not None and cap > 0 else 0, n=int(n), skip_chain=int(skip_chain),
-        filter_threshold=float(vm.DUPLICATE_DISTANCE_THRESHOLD_COSINE if v_ang
-                               else vm.DUPLICATE_DISTANCE_THRESHOLD_EUCLIDEAN),
-        subtract_threshold=float(subtract_distance))
+        **chain_config(vm, bool(vm.SIMILARITY_ELIMINATE_DUPLICATES_DEFAULT)), path_metric=0 if p_ang else 1, n=int(n),
+        skip_chain=int(skip_chain), subtract_threshold=float(subtract_distance))
 
 
 def sample(ids, distances, temperature, n):
@@ -308,8 +302,7 @@ def make_song_alchemy(sa, vm):
             items, skip_chain = listed, True
         details = {d["item_id"]: d for d in sa.get_score_data_by_ids(items)} if items else {}
         sig, raw = Keys(), Keys()
-        cand_sig = [sig(signature(details[i])) if i in details else -1 for i in items]
-        cand_raw = [raw(details[i]["author"]) if i in details and details[i].get("author") else -1 for i in items]
+        cand_sig, cand_raw = candidate_keys(items, details, sig, raw)
         own = [it["id"] for it in add_items + (subtract_items or []) if it.get("type") == "song" and it.get("id")]
         excl = list(dict.fromkeys(vm.reverse_id_map[i] for i in own if i in vm.reverse_id_map))
         to_coord, comp = _map_coords(sa)

@@ -1,5 +1,7 @@
-// Candidate post-processing on the stored rows of the k-NN index (knn.cu): the duplicate filter, the radius walk and
-// the song path's jobs, each one kernel behind one host call.
+// Candidate post-processing on the stored rows of the k-NN index (knn.cu), each one kernel behind one host call: the
+// duplicate filter, the radius walk, and the by-vector chain's requests -- the song path's jobs, Song Alchemy and the
+// plain similar-tracks queries.  The duplicate filter and the chain's requests walk their lists through one filter window
+// (FilterWindow) and one per-item walk (walk_list).
 #include "knn.cuh"
 
 #include <math_constants.h>
@@ -8,20 +10,15 @@
 
 namespace am {
 
-// ---------------------------------------------------------------- duplicate filter on device
-// voyager_manager.py:526-617 (_filter_by_distance) + :487-524 (_compute_distance_batch): walk a result list in
-// order and drop an item whose DIRECT distance (get_direct_distance, :99-140: cosine = 1 - cos with both norms
-// recomputed, euclidean = ||a - b||, not squared) to a recently kept item is below the threshold.  "Recently
-// kept": lists of <= `batch` items compare with the last `lookback` kept items; longer lists are cut into
-// batches of `batch`, and an item is compared with the last `lookback` items kept BEFORE its batch plus
-// everything kept so far inside the batch.  One CTA per list; the walk is sequential, the comparisons of one
-// item are spread over the warps; float64 accumulation.
-constexpr int kFilterThreads = 256;
-constexpr int kFilterCap = 4096;  // items per list
+// ---------------------------------------------------------------- distances
+// a . b, |a|^2, |b|^2 and |a - b|^2 between a (stored row or float64 centroid) and stored row b, one warp, float64
+// accumulation
+struct Moments {
+  double dot, na, nb, d2;
+};
 
-// get_direct_distance (voyager_manager.py:99-140) between stored rows a and b, one warp, float64 accumulation:
-// euclidean ||a - b||, otherwise 1 - cos (+inf when either row is zero)
-__device__ __forceinline__ double direct_distance(const float* a, const float* b, int d, int metric, int lane) {
+template <class T>
+__device__ __forceinline__ Moments warp_moments(const T* a, const float* b, int d, int lane) {
   double dot = 0.0, na = 0.0, nb = 0.0, d2 = 0.0;
   for (int t = lane; t < d; t += 32) {
     const double av = (double)__ldg(&a[t]), bv = (double)__ldg(&b[t]);
@@ -31,54 +28,113 @@ __device__ __forceinline__ double direct_distance(const float* a, const float* b
     const double df = av - bv;
     d2 = fma(df, df, d2);
   }
-  dot = warp_sum(dot);
-  na = warp_sum(na);
-  nb = warp_sum(nb);
-  d2 = warp_sum(d2);
-  if (metric == kMetricL2) return sqrt(d2);
-  const double den = sqrt(na) * sqrt(nb);
-  return den == 0.0 ? INFINITY : 1.0 - fmin(1.0, fmax(-1.0, dot / den));
+  return {warp_sum(dot), warp_sum(na), warp_sum(nb), warp_sum(d2)};
 }
 
-// The first kept item that item i of a list is compared with: the last `lookback` kept ones, or in a list longer
-// than the batch, the last `lookback` kept before i's batch (kept_at_batch) and every one kept since.
-__device__ __forceinline__ int filter_window_start(int kept, int kept_at_batch, bool batched, int lookback) {
-  return max(0, (batched ? kept_at_batch : kept) - lookback);
+// get_direct_distance (voyager_manager.py:99-140) between stored rows a and b: euclidean ||a - b||, otherwise 1 - cos
+// (+inf when either row is zero)
+__device__ __forceinline__ double direct_distance(const float* a, const float* b, int d, int metric, int lane) {
+  const Moments m = warp_moments(a, b, d, lane);
+  if (metric == kMetricL2) return sqrt(m.d2);
+  const double den = sqrt(m.na) * sqrt(m.nb);
+  return den == 0.0 ? INFINITY : 1.0 - fmin(1.0, fmax(-1.0, m.dot / den));
 }
+
+
+// ---------------------------------------------------------------- the filter window and the per-item walk
+// _filter_by_distance (voyager_manager.py:526-617) + :487-524 (_compute_distance_batch) over one list in order: an item
+// whose DIRECT distance to a recently kept item is below the threshold is dropped, and so is an item without a vector.
+// "Recently kept": lists of <= `batch` items compare with the last `lookback` kept items; longer lists are cut into
+// batches of `batch`, and an item is compared with the last `lookback` items kept BEFORE its batch plus everything kept
+// so far inside the batch.  With no lookback the reference returns the list unchanged: nothing is compared and every
+// item passes.  Every thread holds the same counts and admits every item; thread 0 writes the kept list.
+struct FilterWindow {
+  const float* X;
+  int64_t N;
+  int d, metric;
+  double threshold;
+  int lookback, batch;
+  bool batched;      // the list is longer than one batch
+  int* kept;         // the kept items' positions in the list
+  int n = 0;         // kept so far
+  int at_batch = 0;  // kept when the current batch started
+
+  __device__ FilterWindow(const float* X, int64_t N, int d, int metric, double threshold, int lookback, int batch,
+                          int L, int* kept)
+      : X(X), N(N), d(d), metric(metric), threshold(threshold), lookback(lookback), batch(batch), batched(L > batch),
+        kept(kept) {}
+
+  // the first kept position item i is compared with (n: none)
+  __device__ __forceinline__ int start(int i) {
+    if (batched && i % batch == 0) at_batch = n;
+    return lookback > 0 ? max(0, (batched ? at_batch : n) - lookback) : n;
+  }
+
+  // whether item i passes the filter; valid: it has a vector, close: it came within the threshold of the window
+  __device__ __forceinline__ bool admit(int i, bool valid, bool close) {
+    if (lookback <= 0) return true;
+    if (!valid || close) return false;
+    if (threadIdx.x == 0) kept[n] = i;
+    ++n;
+    return true;
+  }
+};
+
+constexpr int kClose = 1;  // walk flag: the item came within the threshold of the filter window
+
+// The walk over a list of L items, one item at a time, three barriers an item.  row_of(i) is item i's stored row (-1 or
+// >= N: no vector).  Between the first two barriers every warp computes the item's distances to the window and then
+// extra(row, valid, slot) runs on every thread: the caller's own per-item work, whose distance slots continue the
+// window's (slot is the first this warp takes, when valid), so that all the item's distances are spread over the warps
+// as one range; it returns the flag bits above kClose that the thread found.  After the second barrier every thread
+// admits the item to the window and thread 0 runs decide(i, row, valid, passed the filter, flags), which keeps the
+// books and returns true to end the walk.
+struct NoExtra {
+  __device__ int operator()(int64_t, bool, int) const { return 0; }
+};
+
+template <class RowOf, class Extra, class Decide>
+__device__ __forceinline__ void walk_list(FilterWindow& w, int L, RowOf row_of, Extra extra, Decide decide) {
+  __shared__ int s_flags;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, warps = blockDim.x >> 5;
+  for (int i = 0; i < L; ++i) {
+    const int64_t row = row_of(i);
+    const bool valid = row >= 0 && row < w.N;  // the reference skips items whose vector is missing
+    const int f0 = w.start(i);
+    if (threadIdx.x == 0) s_flags = 0;
+    __syncthreads();
+    int flags = 0, t = f0 + warp;  // slot t - f0
+    if (valid)
+      for (; t < w.n; t += warps) {
+        const double dist = direct_distance(w.X + row * w.d, w.X + row_of(w.kept[t]) * w.d, w.d, w.metric, lane);
+        if (lane == 0 && dist < w.threshold) flags = kClose;
+      }
+    flags |= extra(row, valid, t - w.n);
+    if (flags) atomicOr(&s_flags, flags);
+    __syncthreads();
+    const int f = s_flags;
+    const bool pass = w.admit(i, valid, f & kClose);
+    bool stop = false;
+    if (threadIdx.x == 0) stop = decide(i, row, valid, pass, f);
+    if (__syncthreads_or(stop)) break;
+  }
+}
+
+// One CTA per list, the comparisons of one item spread over the warps.
+constexpr int kFilterThreads = 256;
+constexpr int kFilterCap = 4096;  // items per list
 
 __global__ void __launch_bounds__(kFilterThreads)
 filter_by_distance_kernel(const float* __restrict__ X, int64_t N, int d, int metric, const int64_t* __restrict__ ids,
                           int n, double threshold, int lookback, int batch, unsigned char* __restrict__ keep) {
   __shared__ int s_kept[kFilterCap];
-  __shared__ int s_close;
   const int64_t* my_ids = ids + (int64_t)blockIdx.x * n;
   unsigned char* my_keep = keep + (int64_t)blockIdx.x * n;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, warps = kFilterThreads / 32;
-  int kept = 0, base = 0;  // base: number kept when the current batch started
-  const bool batched = n > batch;
-  for (int i = 0; i < n; ++i) {
-    if (batched && i % batch == 0) base = kept;
-    const int64_t row = my_ids[i];
-    if (threadIdx.x == 0) s_close = 0;
-    __syncthreads();
-    bool valid = row >= 0 && row < N;  // the reference skips items whose vector is missing
-    if (valid) {
-      const int start = filter_window_start(kept, base, batched, lookback);
-      const float* a = X + row * d;
-      for (int j = start + warp; j < kept; j += warps) {
-        const double dist = direct_distance(a, X + (int64_t)s_kept[j] * d, d, metric, lane);
-        if (lane == 0 && dist < threshold) s_close = 1;
-      }
-    }
-    __syncthreads();
-    const bool keep_it = valid && !s_close;
-    if (threadIdx.x == 0) {
-      my_keep[i] = keep_it ? 1 : 0;
-      if (keep_it) s_kept[kept] = (int)row;
-    }
-    if (keep_it) ++kept;
-    __syncthreads();
-  }
+  FilterWindow w(X, N, d, metric, threshold, lookback, batch, n, s_kept);
+  walk_list(w, n, [&](int i) { return my_ids[i]; }, NoExtra{}, [&](int i, int64_t, bool, bool pass, int) {
+    my_keep[i] = pass ? 1 : 0;
+    return false;
+  });
 }
 
 
@@ -310,56 +366,42 @@ radius_walk_kernel(const float* __restrict__ X, int64_t N, int d, int metric, co
 
 
 // ---------------------------------------------------------------- the by-vector chain
-// find_nearest_neighbors_by_vector (voyager_manager.py:1589-1657) after its k-NN query, for the song path's jobs and for
-// Song Alchemy: one item at a time in k-NN order, each stage looking only at what came before it.
-//   * _filter_by_distance (:526-617): the item is compared with the kept window (window_start) in the VOYAGER_METRIC
-//     distance; items without a vector are dropped; with no lookback the list is unchanged;
+// find_nearest_neighbors_by_vector (voyager_manager.py:1589-1657) after its k-NN query, for the song path's jobs, Song
+// Alchemy and the plain similar-tracks requests: one item at a time in k-NN order (walk_list), each stage looking only at
+// what came before it.
+//   * _filter_by_distance (:526-617) in the VOYAGER_METRIC distance: the filter window;
 //   * same-song dedupe (:1625-1636): an item without details, or whose signature this list already let through, is out;
 //   * the mood stage of find_nearest_neighbors_by_id (:1512, _filter_by_mood_similarity): the caller's verdict, taken
 //     after the signature is marked (the reference's dedupe marks a song the mood filter then drops); the by-vector
 //     callers pass true;
 //   * the raw-author cap (:1638-1653, only when eliminate_duplicates and the cap is > 0; falsy authors are out).
-// The caller computes the window's distances with all its warps; step() is thread 0's decision and books.
+// step() is thread 0's decision and books for the stages after the filter.
 struct ByVectorChain {
-  int32_t* kept;       // the filter's kept positions
-  int32_t* seen;       // [n_sig] the list that last let the signature through, -1 initially
-  int32_t* raw_mark;   // [n_raw] the list that last counted the raw author, -1 initially
-  int32_t* raw_count;  // [n_raw]
+  const int64_t* row;  // [n_cand] stored row, -1: no vector
+  const int32_t* sig;  // [n_cand] (title, author) signature key, -1: no details
+  const int32_t* raw;  // [n_cand] raw author key, -1: falsy author
+  int32_t* kept;       // [longest list] scratch: the filter window's kept positions
+  int32_t* seen;       // [n_sig] scratch: the list that last let the signature through, -1 initially
+  int32_t* raw_mark;   // [n_raw] scratch: the list that last counted the raw author, -1 initially
+  int32_t* raw_count;  // [n_raw] scratch
 
-  // the first kept position the next item is compared with (n_kept: none)
-  __device__ __forceinline__ int window_start(int n_kept, int batch_kept, bool batched, int lookback) const {
-    return lookback > 0 ? filter_window_start(n_kept, batch_kept, batched, lookback) : n_kept;
-  }
-
-  // item i of list `list`: valid = it has a vector, close = it came within the threshold of the window, sig / raw its
-  // signature and raw-author keys (-1: no details / falsy author), mood whether it passes the mood stage.  True when it
-  // passes every stage.
-  __device__ __forceinline__ bool step(int list, int i, bool valid, bool close, int sig, int raw, bool mood, int lookback,
-                                       int cap, int& n_kept) const {
-    bool pass = true;
-    if (lookback > 0) {  // the kept ones form the window
-      pass = valid && !close;
-      if (pass) kept[n_kept++] = i;
-    }
-    if (pass && sig < 0) pass = false;
-    if (pass) {
-      if (seen[sig] == list) pass = false;
-      else seen[sig] = list;
-    }
-    if (pass && !mood) pass = false;
-    if (pass && cap > 0) {
-      if (raw < 0) {
-        pass = false;
-      } else {
-        if (raw_mark[raw] != list) {
-          raw_mark[raw] = list;
-          raw_count[raw] = 0;
-        }
-        if (raw_count[raw] >= cap) pass = false;
-        else raw_count[raw] += 1;
+  // candidate p of list `list`: pass = it passed the filter, mood = it passes the mood stage.  True when it passes every
+  // stage.
+  __device__ __forceinline__ bool step(int list, int p, bool pass, bool mood, int cap) const {
+    const int s = sig[p], r = raw[p];  // both loads in flight before the books' dependent ones
+    if (!pass || s < 0 || seen[s] == list) return false;
+    seen[s] = list;
+    if (!mood) return false;
+    if (cap > 0) {
+      if (r < 0) return false;
+      if (raw_mark[r] != list) {
+        raw_mark[r] = list;
+        raw_count[r] = 0;
       }
+      if (raw_count[r] >= cap) return false;
+      raw_count[r] += 1;
     }
-    return pass;
+    return true;
   }
 };
 
@@ -373,9 +415,10 @@ struct ByVectorChain {
 //   * acceptance (path_manager.py:211-291): used rows and signatures, the normalised-author cap, then the lookbacks
 //     against the path's last songs and this job's found songs, in PATH_DISTANCE_METRIC; the job ends once it has
 //     its songs.  A job that falls short gives back what it took (:294-312).
-// Per candidate, every warp computes the distances the decision may need (filter window, path window, found window)
-// and the threads look for the row among the used rows; then thread 0 decides and keeps the books.
+// Per candidate the walk's extra work is the path window's and the found window's distances, and the threads' look
+// for the row among the used rows.
 constexpr int kPathThreads = 512;
+constexpr int kPathClose = 2, kFoundClose = 4, kUsed = 8;  // walk flags
 
 // get_distance (path_manager.py:27-52): euclidean ||a - b||, angular arccos(clip(cos)) / pi (+inf when either row is
 // zero).  cos = 1 - (1 - cos) is exact for cos >= 0.5, which covers every distance below the thresholds.
@@ -393,10 +436,8 @@ struct SongPathArgs {
   const int32_t* job_off;     // [n_jobs + 1] candidate ranges
   const int32_t* job_n;       // [n_jobs] the by-vector n (k_search)
   const int32_t* job_need;    // [n_jobs] num_to_find
-  const int64_t* cand_row;    // [n_cand] stored row, -1: no vector
-  const int32_t* cand_sig;    // (title, author) signature key, -1: no details
+  ByVectorChain chain;        // the candidates, kept: [max candidates per job]
   const int32_t* cand_author; // normalised author key
-  const int32_t* cand_raw;    // raw author key, -1: falsy author
   int64_t* used_row;          // [n_used + sum(need)] in / out
   int32_t* n_used;
   unsigned char* used_sig;    // [n_sig] in / out
@@ -405,10 +446,7 @@ struct SongPathArgs {
   int32_t* n_path;
   int64_t end_row;
   am_song_path_cfg cfg;
-  int32_t* seen;              // [n_sig] scratch: the job that last let the signature through, -1 initially
-  int32_t* raw_mark;          // [n_raw] scratch: the job that last counted the raw author, -1 initially
-  int32_t* raw_count;         // [n_raw] scratch
-  int32_t* kept;              // [2 x max candidates per job] scratch: the filter's kept positions, then the job's found
+  int32_t* found;             // [max candidates per job] scratch: the job's found songs, by position in its list
   int32_t* out_found;         // [n_jobs]
   int32_t* out_pos;           // [sum(need)] accepted candidates, in path order
   int32_t* out_failed;        // first failed job when stopping on failure, else -1
@@ -416,103 +454,65 @@ struct SongPathArgs {
 };
 
 __global__ void __launch_bounds__(kPathThreads) song_path_kernel(const SongPathArgs a) {
-  __shared__ int s_close;      // bit 0: filter window, bit 1: path window, bit 2: found window
-  __shared__ int s_used, s_stop;
-  __shared__ int s_kept, s_batch_kept, s_found, s_prod, s_n_used, s_n_path, s_n_out;
+  __shared__ int s_found, s_n_used, s_n_path;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, warps = kPathThreads / 32;
   const am_song_path_cfg& c = a.cfg;
-  const int lb_f = c.filter_lookback, lb_p = c.path_lookback;
-  const ByVectorChain chain{a.kept, a.seen, a.raw_mark, a.raw_count};
+  const ByVectorChain& chain = a.chain;
   for (int j = tid; j < a.n_jobs; j += kPathThreads) a.out_found[j] = 0;  // jobs after a stop are not run
+  int n_out = 0;  // thread 0: songs taken so far
   if (tid == 0) {
     s_n_used = *a.n_used;
     s_n_path = *a.n_path;
-    s_n_out = 0;
     *a.out_failed = -1;
   }
   __syncthreads();
   for (int j = 0; j < a.n_jobs; ++j) {
     const int base = a.job_off[j], m = a.job_off[j + 1] - base, n = a.job_n[j], need = a.job_need[j];
-    const bool batched = m > c.filter_batch;
-    if (tid == 0) {
-      s_kept = s_batch_kept = s_found = s_prod = s_stop = 0;
-    }
-    const int used0 = s_n_used;  // the rows this job adds are given back by truncation
-    __syncthreads();
-    int found_all = 0;  // thread 0: songs found so far
-    for (int i = 0; i < m; ++i) {
-      const int64_t row = a.cand_row[base + i];
-      const bool valid = row >= 0 && row < a.N;
-      if (tid == 0) {
-        s_close = 0;
-        s_used = 0;
-        if (batched && i % c.filter_batch == 0) s_batch_kept = s_kept;
-      }
-      __syncthreads();
-      if (valid) {
-        const int kept = s_kept, found = s_found, np = s_n_path;
-        const int f0 = chain.window_start(kept, s_batch_kept, batched, lb_f);
-        const int nf = kept - f0, npw = min(lb_p, np), nq = min(lb_p, found);
-        const float* x = a.X + row * a.d;
-        for (int t = warp; t < nf + npw + nq; t += warps) {
-          int64_t other;
-          int metric, bit;
-          double thr;
-          if (t < nf) {
-            other = a.cand_row[base + a.kept[f0 + t]];
-            metric = c.voyager_metric;
-            thr = c.filter_threshold;
-            bit = 1;
-          } else if (t < nf + npw) {
-            other = a.path_row[np - npw + (t - nf)];
-            metric = c.path_metric;
-            thr = c.path_threshold;
-            bit = 2;
-          } else {
-            other = a.cand_row[base + a.kept[m + found - nq + (t - nf - npw)]];
-            metric = c.path_metric;
-            thr = c.path_threshold;
-            bit = 4;
+    const int64_t* rows = chain.row + base;
+    int found = 0, prod = 0;  // thread 0: songs found, items through the chain
+    if (tid == 0) s_found = 0;
+    const int used0 = s_n_used;  // thread 0: the rows this job adds are given back by truncation
+    FilterWindow w(a.X, a.N, a.d, c.voyager_metric, c.filter_threshold, c.filter_lookback, c.filter_batch, m,
+                   chain.kept);
+    walk_list(
+        w, m, [&](int i) { return rows[i]; },
+        [&](int64_t row, bool valid, int slot) {
+          int flags = 0;
+          if (valid) {
+            const int np = s_n_path, nfound = s_found, npw = min(c.path_lookback, np), nq = min(c.path_lookback, nfound);
+            for (int u = slot; u < npw + nq; u += warps) {
+              const int64_t other = u < npw ? a.path_row[np - npw + u] : rows[a.found[nfound - nq + (u - npw)]];
+              const double dist = path_distance(a.X + row * a.d, a.X + other * a.d, a.d, c.path_metric, lane);
+              if (lane == 0 && dist < c.path_threshold) flags |= u < npw ? kPathClose : kFoundClose;
+            }
           }
-          const float* y = a.X + other * a.d;
-          const double dist = bit == 1 ? direct_distance(x, y, a.d, metric, lane) : path_distance(x, y, a.d, metric, lane);
-          if (lane == 0 && dist < thr) atomicOr(&s_close, bit);
-        }
-      }
-      for (int t = tid; t < s_n_used; t += kPathThreads)
-        if (a.used_row[t] == row) s_used = 1;
-      __syncthreads();
-      if (tid == 0) {
-        const int close = s_close;
-        const int sig = a.cand_sig[base + i];
-        const bool pass = chain.step(j, i, valid, close & 1, sig, a.cand_raw[base + i], true, lb_f, c.voyager_cap,
-                                     s_kept);
-        if (pass) {
-          s_prod += 1;
-          const int au = a.cand_author[base + i];
-          const bool ok = !s_used && !a.used_sig[sig] && !(c.path_cap > 0 && a.author_count[au] >= c.path_cap) && valid &&
-                          !(close & 2) && !(close & 4);
+          for (int t = tid; t < s_n_used; t += kPathThreads)
+            if (a.used_row[t] == row) flags |= kUsed;
+          return flags;
+        },
+        [&](int i, int64_t row, bool valid, bool pass, int flags) {
+          const int p = base + i;
+          if (!chain.step(j, p, pass, true, c.voyager_cap)) return false;
+          ++prod;
+          const int sig = chain.sig[p], au = a.cand_author[p];
+          const bool ok = !(flags & kUsed) && !a.used_sig[sig] && !(c.path_cap > 0 && a.author_count[au] >= c.path_cap) &&
+                          valid && !(flags & (kPathClose | kFoundClose));
           if (ok) {
-            ++found_all;
-            s_found = found_all;
             a.used_row[s_n_used++] = row;
             a.used_sig[sig] = 1;
             a.author_count[au] += 1;
-            a.out_pos[s_n_out + found_all - 1] = base + i;
-            a.kept[m + found_all - 1] = i;  // the job's found list, behind the filter's (<= m entries each)
+            a.out_pos[n_out + found] = p;
+            a.found[found++] = i;
+            s_found = found;
           }
-          if (found_all >= need || s_prod >= n) s_stop = 1;
-        }
-      }
-      __syncthreads();
-      if (s_stop) break;
-    }
+          return found >= need || prod >= n;
+        });
+    bool failed = false;
     if (tid == 0) {
-      const int found = s_found;
       if (found < need) {  // roll back (:294-312)
         for (int t = 0; t < found; ++t) {
-          const int p = base + a.kept[m + t];
-          a.used_sig[a.cand_sig[p]] = 0;
+          const int p = base + a.found[t];
+          a.used_sig[chain.sig[p]] = 0;
           int& cnt = a.author_count[a.cand_author[p]];
           cnt = max(0, cnt - 1);
         }
@@ -520,16 +520,15 @@ __global__ void __launch_bounds__(kPathThreads) song_path_kernel(const SongPathA
         a.out_found[j] = 0;
         if (c.stop_on_failure) {
           *a.out_failed = j;
-          s_stop = 2;
+          failed = true;
         }
       } else {
-        for (int t = 0; t < found; ++t) a.path_row[s_n_path++] = a.cand_row[base + a.kept[m + t]];
-        s_n_out += found;
+        for (int t = 0; t < found; ++t) a.path_row[s_n_path++] = rows[a.found[t]];
+        n_out += found;
         a.out_found[j] = found;
       }
     }
-    __syncthreads();
-    if (s_stop == 2) break;
+    if (__syncthreads_or(failed)) break;
   }
   // distances between consecutive songs of the path, the end song last
   const int np = s_n_path;
@@ -554,8 +553,7 @@ __global__ void __launch_bounds__(kPathThreads) song_path_kernel(const SongPathA
 //   * the distance to the add centroid (:916-930).
 // The centroids are float64, as the reference's means of float64 copies are.  Both distances are song_alchemy's own
 // (not get_distance's): angular arccos(clip(c / (|c| or 1) . v / (|v| or 1))) / pi, so a zero vector is at 0.5, and
-// euclidean ||c - v||, in float64 from the stored rows.  The chain walks its items one at a time like the song path; the
-// rest is one warp per chain survivor.
+// euclidean ||c - v||, in float64 from the stored rows.  The chain is the walk; the rest is one warp per chain survivor.
 constexpr int kAlchemyThreads = 512;
 
 struct AlchemyArgs {
@@ -565,16 +563,10 @@ struct AlchemyArgs {
   int m;                    // candidates
   const double* add_c;      // [d]
   const double* sub_c;      // [d] or null: no subtract filter
-  const int64_t* cand_row;  // [m] stored row, -1: no vector
-  const int32_t* cand_sig;  // [m] signature key, -1: no details
-  const int32_t* cand_raw;  // [m] raw author key, -1: falsy author
+  ByVectorChain chain;      // kept: [m]
   const int64_t* excl_row;  // [n_excl]
   int n_excl;
   am_alchemy_cfg cfg;
-  int32_t* seen;            // [n_sig] scratch, -1 initially
-  int32_t* raw_mark;        // [n_raw] scratch, -1 initially
-  int32_t* raw_count;       // [n_raw] scratch
-  int32_t* kept;            // [m] scratch: the filter's kept positions
   int32_t* out_count;       // the chain's survivors
   int32_t* out_pos;         // [min(m, n)] their positions in the candidate arrays, in order
   unsigned char* out_status;  // [min(m, n)] 0 taken out, 1 kept, 2 filtered out
@@ -585,66 +577,34 @@ struct AlchemyArgs {
 
 // song_alchemy's distance from centroid c (float64) to stored row v, one warp
 __device__ __forceinline__ double alchemy_distance(const double* c, const float* v, int d, int metric, int lane) {
-  double dot = 0.0, nc = 0.0, nv = 0.0, d2 = 0.0;
-  for (int t = lane; t < d; t += 32) {
-    const double cv = c[t], vv = (double)__ldg(&v[t]);
-    dot = fma(cv, vv, dot);
-    nc = fma(cv, cv, nc);
-    nv = fma(vv, vv, nv);
-    const double df = cv - vv;
-    d2 = fma(df, df, d2);
-  }
-  dot = warp_sum(dot);
-  nc = warp_sum(nc);
-  nv = warp_sum(nv);
-  d2 = warp_sum(d2);
-  if (metric == kMetricL2) return sqrt(d2);
-  nc = sqrt(nc);
-  nv = sqrt(nv);
-  const double cs = dot / ((nc == 0.0 ? 1.0 : nc) * (nv == 0.0 ? 1.0 : nv));
+  const Moments m = warp_moments(c, v, d, lane);
+  if (metric == kMetricL2) return sqrt(m.d2);
+  const double nc = sqrt(m.na), nv = sqrt(m.nb);
+  const double cs = m.dot / ((nc == 0.0 ? 1.0 : nc) * (nv == 0.0 ? 1.0 : nv));
   return acos(fmin(1.0, fmax(-1.0, cs))) / CUDART_PI;
 }
 
 __global__ void __launch_bounds__(kAlchemyThreads) alchemy_kernel(const AlchemyArgs a) {
-  __shared__ int s_close, s_kept, s_batch_kept, s_n;
+  __shared__ int s_n;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, warps = kAlchemyThreads / 32;
   const am_alchemy_cfg& c = a.cfg;
-  const int lb = c.filter_lookback;
-  const ByVectorChain chain{a.kept, a.seen, a.raw_mark, a.raw_count};
-  if (tid == 0) s_kept = s_batch_kept = s_n = 0;
-  __syncthreads();
   if (c.skip_chain) {
     for (int i = tid; i < a.m; i += kAlchemyThreads) a.out_pos[i] = i;
     if (tid == 0) s_n = a.m;
   } else {
-    const bool batched = a.m > c.filter_batch;
-    for (int i = 0; i < a.m; ++i) {
-      const int64_t row = a.cand_row[i];
-      const bool valid = row >= 0 && row < a.N;
-      if (tid == 0) {
-        s_close = 0;
-        if (batched && i % c.filter_batch == 0) s_batch_kept = s_kept;
-      }
-      __syncthreads();
-      if (valid) {
-        const int kept = s_kept, f0 = chain.window_start(kept, s_batch_kept, batched, lb);
-        const float* x = a.X + row * a.d;
-        for (int t = f0 + warp; t < kept; t += warps) {
-          const double dist = direct_distance(x, a.X + a.cand_row[a.kept[t]] * a.d, a.d, c.voyager_metric, lane);
-          if (lane == 0 && dist < c.filter_threshold) s_close = 1;
-        }
-      }
-      __syncthreads();
-      if (tid == 0 && chain.step(0, i, valid, s_close, a.cand_sig[i], a.cand_raw[i], true, lb, c.voyager_cap, s_kept))
-        a.out_pos[s_n++] = i;
-      __syncthreads();
-      if (s_n >= c.n) break;
-    }
+    int n = 0;  // thread 0: survivors
+    FilterWindow w(a.X, a.N, a.d, c.voyager_metric, c.filter_threshold, c.filter_lookback, c.filter_batch, a.m,
+                   a.chain.kept);
+    walk_list(w, a.m, [&](int i) { return a.chain.row[i]; }, NoExtra{}, [&](int i, int64_t, bool, bool pass, int) {
+      if (a.chain.step(0, i, pass, true, c.voyager_cap)) a.out_pos[n++] = i;
+      return n >= c.n;
+    });
+    if (tid == 0) s_n = n;
   }
   __syncthreads();
   const int n = s_n;
   for (int t = warp; t < n; t += warps) {
-    const int64_t row = a.cand_row[a.out_pos[t]];
+    const int64_t row = a.chain.row[a.out_pos[t]];
     bool out = row < 0 || row >= a.N;  // no vector: the subtract filter skips it (:465), the distances do (:921)
     for (int e = 0; e < a.n_excl && !out; ++e) out = a.excl_row[e] == row;
     unsigned char status = 0;
@@ -675,14 +635,13 @@ __global__ void __launch_bounds__(kAlchemyThreads) alchemy_kernel(const AlchemyA
 // find_nearest_neighbors_by_vector (:1589-1657) after their k-NN query, in one CTA: the by-vector chain (ByVectorChain)
 // over the request's list in k-NN order, stopping once n items have passed ([:n]).  A by-id request differs in three
 // places:
-//   * its target goes first into _filter_by_distance at distance 0 (:1497-1502): it is the first kept item of the
-//     window (the list it heads is one longer, which moves the batch boundaries) and is never output (:1505);
+//   * its target goes first into _filter_by_distance at distance 0 (:1497-1502): it is item 0 of the walk, a member of
+//     the window only (the list it heads is one longer, which moves the batch boundaries) and never output (:1505);
 //   * the dedupe starts with the target's signature already seen (:662-665);
 //   * the mood stage (:1508-1514, _filter_by_mood_similarity :714-822) runs between the dedupe and the cap when the
 //     caller passes a mood table: a candidate without parsed features is dropped, otherwise its mood distance
 //     sum(|target[f] - cand[f]|) / 6 over the six features, summed in float64 as Python's sum() does (mood_distance),
 //     must be <= the threshold.
-// Every warp computes the filter window's distances; thread 0 decides and keeps the books.
 constexpr int kSimilarThreads = 512;
 constexpr int kMoodFeatures = 6;  // danceable, aggressive, happy, party, relaxed, sad (:775)
 
@@ -694,17 +653,11 @@ struct SimilarArgs {
   int n;                          // the request's n
   int64_t target_row;             // -1: a by-vector request
   int target_sig;                 // the signature seen before the first candidate, -1: none
-  const int64_t* cand_row;        // [m] stored row, -1: no vector
-  const int32_t* cand_sig;        // [m] signature key, -1: no details
-  const int32_t* cand_raw;        // [m] raw author key, -1: falsy author
+  ByVectorChain chain;            // kept: [m + 1]
   const double* mood;             // [m, 6] the candidates' features, or null: no mood stage
   const unsigned char* mood_ok;   // [m] 1: the candidate's features parsed
   const double* target_mood;      // [6]
   am_similar_cfg cfg;
-  int32_t* seen;                  // [n_sig] scratch, -1 initially
-  int32_t* raw_mark;              // [n_raw] scratch, -1 initially
-  int32_t* raw_count;             // [n_raw] scratch
-  int32_t* kept;                  // [m + 1] scratch: the filter's kept items (the target is item 0 of a by-id list)
   int32_t* out_count;
   int32_t* out_pos;               // [min(m, n)] the survivors' positions in the candidate arrays, in order
   double* out_mood;               // [min(m, n)] their mood distances (mood stage only)
@@ -727,42 +680,17 @@ __device__ __forceinline__ double mood_distance(const double* t, const double* c
 }
 
 __global__ void __launch_bounds__(kSimilarThreads) similar_kernel(const SimilarArgs a) {
-  __shared__ int s_close, s_kept, s_batch_kept, s_n;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, warps = kSimilarThreads / 32;
   const am_similar_cfg& c = a.cfg;
-  const int lb = c.filter_lookback;
-  const ByVectorChain chain{a.kept, a.seen, a.raw_mark, a.raw_count};
   const int by_id = a.target_row >= 0 ? 1 : 0;
   const int L = a.m + by_id;  // the list _filter_by_distance sees
-  const bool batched = L > c.filter_batch;
-  auto row_of = [&](int i) { return by_id && i == 0 ? a.target_row : a.cand_row[i - by_id]; };
-  if (tid == 0) {
-    s_kept = s_batch_kept = s_n = 0;
-    if (a.target_sig >= 0) a.seen[a.target_sig] = 0;
-  }
-  __syncthreads();
-  for (int i = 0; i < L; ++i) {
-    const int64_t row = row_of(i);
-    const bool valid = row >= 0 && row < a.N;
-    if (tid == 0) {
-      s_close = 0;
-      if (batched && i % c.filter_batch == 0) s_batch_kept = s_kept;
-    }
-    __syncthreads();
-    if (valid) {
-      const int kept = s_kept, f0 = chain.window_start(kept, s_batch_kept, batched, lb);
-      const float* x = a.X + row * a.d;
-      for (int t = f0 + warp; t < kept; t += warps) {
-        const double dist = direct_distance(x, a.X + row_of(a.kept[t]) * a.d, a.d, c.metric, lane);
-        if (lane == 0 && dist < c.filter_threshold) s_close = 1;
-      }
-    }
-    __syncthreads();
-    if (tid == 0) {
-      if (by_id && i == 0) {
-        if (lb > 0 && valid && !s_close) a.kept[s_kept++] = 0;  // the target: only a member of the window
-      } else {
+  int n = 0;                  // thread 0: survivors
+  if (threadIdx.x == 0 && a.target_sig >= 0) a.chain.seen[a.target_sig] = 0;
+  FilterWindow w(a.X, a.N, a.d, c.metric, c.filter_threshold, c.filter_lookback, c.filter_batch, L, a.chain.kept);
+  walk_list(
+      w, L, [&](int i) { return by_id && i == 0 ? a.target_row : a.chain.row[i - by_id]; }, NoExtra{},
+      [&](int i, int64_t, bool, bool pass, int) {
         const int p = i - by_id;
+        if (p < 0) return false;  // the target
         bool mood = true;
         double md = 0.0;
         if (a.mood) {
@@ -772,17 +700,14 @@ __global__ void __launch_bounds__(kSimilarThreads) similar_kernel(const SimilarA
             mood = md <= c.mood_threshold;
           }
         }
-        if (chain.step(0, i, valid, s_close, a.cand_sig[p], a.cand_raw[p], mood, lb, c.cap, s_kept)) {
-          a.out_pos[s_n] = p;
-          if (a.out_mood) a.out_mood[s_n] = md;
-          ++s_n;
+        if (a.chain.step(0, p, pass, mood, c.cap)) {
+          a.out_pos[n] = p;
+          if (a.out_mood) a.out_mood[n] = md;
+          ++n;
         }
-      }
-    }
-    __syncthreads();
-    if (s_n >= a.n) break;
-  }
-  if (tid == 0) *a.out_count = s_n;
+        return n >= a.n;
+      });
+  if (threadIdx.x == 0) *a.out_count = n;
 }
 
 }  // namespace am
@@ -865,6 +790,42 @@ extern "C" int am_knn_radius_walk(const am_index* idx, const float* anchor, cons
   return AM_OK;
 }
 
+// The by-vector chain's candidates of one host call: check() validates them with the chain's metric and filter batch,
+// declare() puts their uploads and the chain's scratch on the call.
+struct ChainHost {
+  const char* fn;  // the entry point, for messages
+  int n_cand;
+  const int64_t* rows;
+  const int32_t* sig;  // -1: no details, else < n_sig
+  const int32_t* raw;  // -1: falsy author
+  int n_sig;
+  int n_raw = 0;  // raw-author keys, found by check()
+
+  int check(int metric, int filter_batch) {
+    AM_CHECK(metric == kMetricCos || metric == kMetricL2, "%s: metric %d is not 0 (angular) or 1 (euclidean)", fn,
+             metric);
+    AM_CHECK(filter_batch > 0, "%s: filter_batch must be positive", fn);
+    AM_CHECK(n_cand >= 0 && n_sig >= 0, "%s: negative size", fn);
+    AM_CHECK(n_cand == 0 || (rows && sig && raw), "%s: NULL candidates", fn);
+    for (int i = 0; i < n_cand; ++i) {
+      AM_CHECK(sig[i] >= -1 && sig[i] < n_sig && raw[i] >= -1, "%s: candidate %d has a key out of range", fn, i);
+      n_raw = std::max(n_raw, raw[i] + 1);
+    }
+    return AM_OK;
+  }
+
+  // n_kept: the longest list the filter window walks
+  void declare(HostCall& call, ByVectorChain* c, size_t n_kept) const {
+    call.up(&c->row, rows, (size_t)n_cand);
+    call.up(&c->sig, sig, (size_t)n_cand);
+    call.up(&c->raw, raw, (size_t)n_cand);
+    call.device(&c->kept, n_kept);
+    call.device(&c->seen, (size_t)n_sig, 0xff);  // -1: no list let the signature through yet
+    call.device(&c->raw_mark, (size_t)n_raw, 0xff);
+    call.device(&c->raw_count, (size_t)n_raw);
+  }
+};
+
 extern "C" int am_knn_song_path(const am_index* idx, const am_song_path_cfg* cfg, int n_jobs, const int32_t* job_off,
                                 const int32_t* job_n, const int32_t* job_need, const int64_t* cand_rows,
                                 const int32_t* cand_sig, const int32_t* cand_author, const int32_t* cand_author_raw,
@@ -875,11 +836,8 @@ extern "C" int am_knn_song_path(const am_index* idx, const am_song_path_cfg* cfg
            "am_knn_song_path: NULL argument");
   AM_CHECK(n_jobs >= 0 && n_sig >= 0 && n_author >= 0 && *n_used >= 0 && *n_path >= 1,
            "am_knn_song_path: negative size, or no start song in the path");
-  AM_CHECK(cfg->voyager_metric == kMetricCos || cfg->voyager_metric == kMetricL2, "am_knn_song_path: voyager_metric %d",
-           cfg->voyager_metric);
   AM_CHECK(cfg->path_metric == kMetricCos || cfg->path_metric == kMetricL2, "am_knn_song_path: path_metric %d",
            cfg->path_metric);
-  AM_CHECK(cfg->filter_batch > 0, "am_knn_song_path: filter_batch must be positive");
   AM_CHECK(end_row >= 0 && end_row < idx->N, "am_knn_song_path: end row %lld out of range", (long long)end_row);
   AM_CHECK(n_jobs == 0 || job_off[0] == 0, "am_knn_song_path: job_off[0] must be 0");
   int64_t total_need = 0;
@@ -891,15 +849,12 @@ extern "C" int am_knn_song_path(const am_index* idx, const am_song_path_cfg* cfg
     max_m = std::max(max_m, job_off[j + 1] - job_off[j]);
   }
   const int n_cand = n_jobs ? job_off[n_jobs] : 0;
-  AM_CHECK(n_cand == 0 || (cand_rows && cand_sig && cand_author && cand_author_raw), "am_knn_song_path: NULL candidates");
+  ChainHost chain{"am_knn_song_path", n_cand, cand_rows, cand_sig, cand_author_raw, n_sig};
+  AM_TRY(chain.check(cfg->voyager_metric, cfg->filter_batch));
+  AM_CHECK(n_cand == 0 || cand_author, "am_knn_song_path: NULL candidates");
   AM_CHECK(total_need == 0 || out_pos, "am_knn_song_path: NULL out_pos");
-  int n_raw = 0;
-  for (int i = 0; i < n_cand; ++i) {
-    AM_CHECK(cand_sig[i] >= -1 && cand_sig[i] < n_sig && cand_author[i] >= 0 && cand_author[i] < n_author &&
-                 cand_author_raw[i] >= -1,
-             "am_knn_song_path: candidate %d has a key out of range", i);
-    n_raw = std::max(n_raw, cand_author_raw[i] + 1);
-  }
+  for (int i = 0; i < n_cand; ++i)
+    AM_CHECK(cand_author[i] >= 0 && cand_author[i] < n_author, "am_knn_song_path: candidate %d has a key out of range", i);
   const int nu = *n_used, np = *n_path;
   for (int t = 0; t < np; ++t)
     AM_CHECK(path_rows[t] >= 0 && path_rows[t] < idx->N, "am_knn_song_path: path row %d out of range", t);
@@ -915,10 +870,8 @@ extern "C" int am_knn_song_path(const am_index* idx, const am_song_path_cfg* cfg
   call.up(&a.job_off, job_off, n_jobs ? (size_t)n_jobs + 1 : 0);
   call.up(&a.job_n, job_n, (size_t)n_jobs);
   call.up(&a.job_need, job_need, (size_t)n_jobs);
-  call.up(&a.cand_row, cand_rows, (size_t)n_cand);
-  call.up(&a.cand_sig, cand_sig, (size_t)n_cand);
   call.up(&a.cand_author, cand_author, (size_t)n_cand);
-  call.up(&a.cand_raw, cand_author_raw, (size_t)n_cand);
+  chain.declare(call, &a.chain, (size_t)max_m);
   call.both(&d_hdr, hdr, 4, 4);
   call.both(&a.used_row, used_rows, (size_t)nu, (size_t)cap_used);
   call.both(&a.path_row, path_rows, (size_t)np, (size_t)cap_path);
@@ -927,10 +880,7 @@ extern "C" int am_knn_song_path(const am_index* idx, const am_song_path_cfg* cfg
   call.down(&a.out_found, (size_t)n_jobs, out_found);
   call.down(&a.out_pos, (size_t)total_need);
   call.down(&a.out_dist, (size_t)cap_path);
-  call.device(&a.seen, (size_t)n_sig, 0xff);  // -1: no job let the signature through yet
-  call.device(&a.raw_mark, (size_t)n_raw, 0xff);
-  call.device(&a.raw_count, (size_t)n_raw);
-  call.device(&a.kept, (size_t)2 * max_m);
+  call.device(&a.found, (size_t)max_m);
   AM_TRY(call.start());
   a.n_used = d_hdr;
   a.n_path = d_hdr + 1;
@@ -959,26 +909,18 @@ extern "C" int am_knn_alchemy(const am_index* idx, const am_alchemy_cfg* cfg, co
                               int32_t* out_count, int32_t* out_pos, unsigned char* out_status, double* out_dsub,
                               double* out_dadd, float* out_rows) {
   AM_CHECK(idx && cfg && add_centroid && out_count && (n_excl == 0 || excl_rows), "am_knn_alchemy: NULL argument");
-  AM_CHECK(cfg->voyager_metric == kMetricCos || cfg->voyager_metric == kMetricL2, "am_knn_alchemy: voyager_metric %d",
-           cfg->voyager_metric);
   AM_CHECK(cfg->path_metric == kMetricCos || cfg->path_metric == kMetricL2, "am_knn_alchemy: path_metric %d",
            cfg->path_metric);
-  AM_CHECK(cfg->filter_batch > 0, "am_knn_alchemy: filter_batch must be positive");
   AM_CHECK(cfg->n >= 1 && cfg->n <= AM_ALCHEMY_MAX_N, "am_knn_alchemy: n = %d is outside [1, %d]", cfg->n,
            AM_ALCHEMY_MAX_N);
   AM_CHECK(n_cand >= 0 && n_cand <= AM_ALCHEMY_MAX_CANDIDATES && (!cfg->skip_chain || n_cand <= cfg->n),
            "am_knn_alchemy: %d candidates (at most %d, and at most n without the chain)", n_cand,
            AM_ALCHEMY_MAX_CANDIDATES);
-  AM_CHECK(n_sig >= 0 && n_excl >= 0, "am_knn_alchemy: negative size");
+  AM_CHECK(n_excl >= 0, "am_knn_alchemy: negative size");
+  ChainHost chain{"am_knn_alchemy", n_cand, cand_rows, cand_sig, cand_author_raw, n_sig};
+  AM_TRY(chain.check(cfg->voyager_metric, cfg->filter_batch));
   const int n_out = std::min(n_cand, cfg->n);
-  AM_CHECK(n_cand == 0 || (cand_rows && cand_sig && cand_author_raw), "am_knn_alchemy: NULL candidates");
   AM_CHECK(n_out == 0 || (out_pos && out_status && out_dsub && out_dadd), "am_knn_alchemy: NULL output");
-  int n_raw = 0;
-  for (int i = 0; i < n_cand; ++i) {
-    AM_CHECK(cand_sig[i] >= -1 && cand_sig[i] < n_sig && cand_author_raw[i] >= -1,
-             "am_knn_alchemy: candidate %d has a key out of range", i);
-    n_raw = std::max(n_raw, cand_author_raw[i] + 1);
-  }
   *out_count = 0;
   if (n_cand == 0) return AM_OK;
   cudaStream_t st;
@@ -989,9 +931,7 @@ extern "C" int am_knn_alchemy(const am_index* idx, const am_alchemy_cfg* cfg, co
   a.cfg = *cfg;
   call.up(&a.add_c, add_centroid, (size_t)idx->d);
   call.up(&a.sub_c, sub_centroid, sub_centroid ? (size_t)idx->d : 0);
-  call.up(&a.cand_row, cand_rows, (size_t)n_cand);
-  call.up(&a.cand_sig, cand_sig, (size_t)n_cand);
-  call.up(&a.cand_raw, cand_author_raw, (size_t)n_cand);
+  chain.declare(call, &a.chain, (size_t)n_cand);
   call.up(&a.excl_row, excl_rows, (size_t)n_excl);
   call.down(&a.out_count, 1);
   call.down(&a.out_pos, (size_t)n_out);
@@ -999,10 +939,6 @@ extern "C" int am_knn_alchemy(const am_index* idx, const am_alchemy_cfg* cfg, co
   call.down(&a.out_dsub, (size_t)n_out);
   call.down(&a.out_dadd, (size_t)n_out);
   call.down(&a.out_rows, out_rows ? (size_t)n_out * idx->d : 0);
-  call.device(&a.seen, (size_t)n_sig, 0xff);  // -1: no signature let through yet
-  call.device(&a.raw_mark, (size_t)n_raw, 0xff);
-  call.device(&a.raw_count, (size_t)n_raw);
-  call.device(&a.kept, (size_t)n_cand);
   AM_TRY(call.start());
   if (!sub_centroid) a.sub_c = nullptr;
   if (!out_rows) a.out_rows = nullptr;
@@ -1025,23 +961,14 @@ extern "C" int am_knn_similar(const am_index* idx, const am_similar_cfg* cfg, in
                               const double* target_mood, int n, int32_t* out_count, int32_t* out_pos,
                               double* out_mood) {
   AM_CHECK(idx && cfg && out_count, "am_knn_similar: NULL argument");
-  AM_CHECK(cfg->metric == kMetricCos || cfg->metric == kMetricL2, "am_knn_similar: metric %d is not 0 (angular) or 1 "
-           "(euclidean)", cfg->metric);
-  AM_CHECK(cfg->filter_batch > 0, "am_knn_similar: filter_batch must be positive");
-  AM_CHECK(n_cand >= 0 && n_sig >= 0, "am_knn_similar: negative size");
+  ChainHost chain{"am_knn_similar", n_cand, cand_rows, cand_sig, cand_author_raw, n_sig};
+  AM_TRY(chain.check(cfg->metric, cfg->filter_batch));
   AM_CHECK(target_row >= -1 && target_row < idx->N, "am_knn_similar: target row %lld out of range",
            (long long)target_row);
   AM_CHECK(target_sig >= -1 && target_sig < n_sig, "am_knn_similar: target signature %d out of range", target_sig);
   AM_CHECK(!mood || (mood_ok && target_mood), "am_knn_similar: a mood table needs its flags and the target's features");
   const int n_out = std::max(0, std::min(n_cand, n));
-  AM_CHECK(n_cand == 0 || (cand_rows && cand_sig && cand_author_raw), "am_knn_similar: NULL candidates");
   AM_CHECK(n_out == 0 || (out_pos && (!mood || out_mood)), "am_knn_similar: NULL output");
-  int n_raw = 0;
-  for (int i = 0; i < n_cand; ++i) {
-    AM_CHECK(cand_sig[i] >= -1 && cand_sig[i] < n_sig && cand_author_raw[i] >= -1,
-             "am_knn_similar: candidate %d has a key out of range", i);
-    n_raw = std::max(n_raw, cand_author_raw[i] + 1);
-  }
   *out_count = 0;
   if (n_out == 0) return AM_OK;
   cudaStream_t st;
@@ -1049,19 +976,13 @@ extern "C" int am_knn_similar(const am_index* idx, const am_similar_cfg* cfg, in
   HostCall call(st, HostCall::kAlways);
   SimilarArgs a{idx->X.p, idx->N, idx->d, n_cand, n, target_row, target_sig};
   a.cfg = *cfg;
-  call.up(&a.cand_row, cand_rows, (size_t)n_cand);
-  call.up(&a.cand_sig, cand_sig, (size_t)n_cand);
-  call.up(&a.cand_raw, cand_author_raw, (size_t)n_cand);
+  chain.declare(call, &a.chain, (size_t)n_cand + 1);
   call.up(&a.mood, mood, mood ? (size_t)n_cand * kMoodFeatures : 0);
   call.up(&a.mood_ok, mood_ok, mood ? (size_t)n_cand : 0);
   call.up(&a.target_mood, target_mood, mood ? (size_t)kMoodFeatures : 0);
   call.down(&a.out_count, 1);
   call.down(&a.out_pos, (size_t)n_out);
   call.down(&a.out_mood, mood ? (size_t)n_out : 0);
-  call.device(&a.seen, (size_t)n_sig, 0xff);  // -1: no signature let through yet
-  call.device(&a.raw_mark, (size_t)n_raw, 0xff);
-  call.device(&a.raw_count, (size_t)n_raw);
-  call.device(&a.kept, (size_t)n_cand + 1);
   AM_TRY(call.start());
   if (!mood) {
     a.mood = a.target_mood = nullptr;

@@ -22,7 +22,7 @@ import sys
 import numpy as np
 
 from . import _lib
-from .song_path import Keys, signature
+from .by_vector import Keys, candidate_keys, chain_config, query_size, signature
 
 logger = logging.getLogger(__name__)
 
@@ -50,15 +50,10 @@ def mood_row(features):
 
 def config(vm, eliminate_duplicates):
     """am_similar_cfg from voyager_manager's configuration as it holds it now."""
-    ang = vm.VOYAGER_METRIC == "angular"
-    cap = vm.MAX_SONGS_PER_ARTIST
+    ch = chain_config(vm, eliminate_duplicates)
     return _lib.SimilarCfg(
-        metric=0 if ang else 1, filter_lookback=int(vm.DUPLICATE_DISTANCE_CHECK_LOOKBACK),
-        filter_batch=int(vm.BATCH_SIZE_VECTOR_OPS),
-        cap=int(cap) if eliminate_duplicates and cap is not None and cap > 0 else 0,
+        metric=ch.pop("voyager_metric"), cap=ch.pop("voyager_cap"), **ch,
         mood_sum=1 if sys.version_info >= (3, 12) else 0,   # sum() of floats is compensated from CPython 3.12 on
-        filter_threshold=float(vm.DUPLICATE_DISTANCE_THRESHOLD_COSINE if ang
-                               else vm.DUPLICATE_DISTANCE_THRESHOLD_EUCLIDEAN),
         mood_threshold=float(vm.MOOD_SIMILARITY_THRESHOLD))
 
 
@@ -71,12 +66,6 @@ def by_id_query_size(n, eliminate_duplicates, radius_similarity, mood_similarity
         q = n + max(3, int(n * 0.20)) + 1
     if mood_similarity:
         q = n + max(20, int(n * (8 if eliminate_duplicates else 4))) + 1
-    return min(q, size)
-
-
-def by_vector_query_size(n, eliminate_duplicates, size):
-    """voyager_manager.py:1561-1573 (without the floor at 0: the caller skips the query at <= 0)."""
-    q = n + int(n * 4) if eliminate_duplicates else n + int(n * 0.2)
     return min(q, size)
 
 
@@ -101,8 +90,7 @@ def _run(vm, items, distances, n, eliminate_duplicates, target=None, target_deta
     details = {d["item_id"]: d for d in get_score_data_by_ids(items)}
     sig, raw = Keys(), Keys()
     target_sig = sig(signature(target_details)) if target_details is not None else -1
-    cand_sig = [sig(signature(details[i])) if i in details else -1 for i in items]
-    cand_raw = [raw(details[i]["author"]) if i in details and details[i].get("author") else -1 for i in items]
+    cand_sig, cand_raw = candidate_keys(items, details, sig, raw)
     table = ok = target_mood = None
     if mood:
         t = target_details.get("other_features")
@@ -197,7 +185,7 @@ def make_find_nearest_neighbors_by_vector(vm):
             raise RuntimeError("Voyager index is not loaded in memory.")
         if eliminate_duplicates is None:
             eliminate_duplicates = vm.SIMILARITY_ELIMINATE_DUPLICATES_DEFAULT
-        k = by_vector_query_size(n, eliminate_duplicates, len(vm.voyager_index))
+        k = query_size(n, eliminate_duplicates, len(vm.voyager_index))
         if k <= 0:
             ids, dists = [], []
         else:

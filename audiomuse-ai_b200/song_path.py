@@ -14,10 +14,12 @@ path_manager (pm) modules at call time, as the reference reads its own module gl
 from __future__ import annotations
 
 import logging
+from itertools import accumulate
 
 import numpy as np
 
 from . import _lib
+from .by_vector import Keys, candidate_keys, chain_config, normalize, query_size, signature
 
 logger = logging.getLogger(__name__)
 
@@ -87,47 +89,14 @@ def merge_jobs(jobs, i, intermediate, metric):
     a["indices"] = a["indices"] + b["indices"]
 
 
-def query_size(n, eliminate_duplicates, size):
-    """voyager_manager.py:1561-1573: the neighbours find_nearest_neighbors_by_vector asks the index for."""
-    q = n + int(n * 4) if eliminate_duplicates else n + int(n * 0.2)
-    return max(0, min(q, size))
-
-
-def normalize(text):
-    """_normalize_string / _normalize_signature's field normalisation."""
-    return (text or "").strip().lower()
-
-
-def signature(details):
-    return normalize(details.get("author")), normalize(details.get("title"))
-
-
-class Keys:
-    """Dense int keys, assigned in order of first appearance."""
-
-    def __init__(self):
-        self.ids = {}
-
-    def __call__(self, value):
-        return self.ids.setdefault(value, len(self.ids))
-
-    def __len__(self):
-        return len(self.ids)
-
-
 def config(vm, pm, stop_on_failure):
     """am_song_path_cfg from the two modules' configuration as they hold it now."""
-    ed = bool(vm.SIMILARITY_ELIMINATE_DUPLICATES_DEFAULT)
-    vcap = vm.MAX_SONGS_PER_ARTIST
     pcap = pm.MAX_SONGS_PER_ARTIST
-    v_ang, p_ang = vm.VOYAGER_METRIC == "angular", pm.PATH_DISTANCE_METRIC == "angular"
+    p_ang = pm.PATH_DISTANCE_METRIC == "angular"
     return _lib.SongPathCfg(
-        voyager_metric=0 if v_ang else 1, path_metric=0 if p_ang else 1,
-        filter_lookback=int(vm.DUPLICATE_DISTANCE_CHECK_LOOKBACK), filter_batch=int(vm.BATCH_SIZE_VECTOR_OPS),
+        **chain_config(vm, bool(vm.SIMILARITY_ELIMINATE_DUPLICATES_DEFAULT)), path_metric=0 if p_ang else 1,
         path_lookback=int(pm.DUPLICATE_DISTANCE_CHECK_LOOKBACK),
-        voyager_cap=int(vcap) if ed and vcap is not None and vcap > 0 else 0,
         path_cap=int(pcap) if pcap is not None and pcap > 0 else 0, stop_on_failure=int(bool(stop_on_failure)),
-        filter_threshold=float(vm.DUPLICATE_DISTANCE_THRESHOLD_COSINE if v_ang else vm.DUPLICATE_DISTANCE_THRESHOLD_EUCLIDEAN),
         path_threshold=float(pm.DUPLICATE_DISTANCE_THRESHOLD_COSINE if p_ang else pm.DUPLICATE_DISTANCE_THRESHOLD_EUCLIDEAN))
 
 
@@ -183,22 +152,16 @@ class _Request:
         """One am_knn_song_path call over `jobs`; returns (songs found per job, item ids taken, failed job or None,
         distances along the path to the end song)."""
         vm = self.vm
-        off, cand, sig, author, raw = [0], [], [], [], []
-        for j in jobs:
-            for item in j["items"]:
-                d = self.details.get(item)
-                cand.append(vm.reverse_id_map.get(item, -1))
-                sig.append(-1 if d is None else self.sig(signature(d)))
-                author.append(self.author(normalize(d.get("author")) if d is not None else ""))
-                raw.append(self.raw(d["author"]) if d is not None and d.get("author") else -1)
-            off.append(len(cand))
+        items = [it for j in jobs for it in j["items"]]
+        off = list(accumulate((len(j["items"]) for j in jobs), initial=0))
+        sig, raw = candidate_keys(items, self.details, self.sig, self.raw)
+        author = [self.author(normalize(self.details[i].get("author")) if i in self.details else "") for i in items]
         self.used_sig = np.concatenate([self.used_sig, np.zeros(len(self.sig) - len(self.used_sig), np.uint8)])
         self.author_count = np.concatenate([self.author_count,
                                             np.zeros(len(self.author) - len(self.author_count), np.int32)])
         found, pos, failed, self.used_ids, self.path_ids, dist = vm.voyager_index.song_path(
-            cfg, off, [j["k"] for j in jobs], [j["need"] for j in jobs], cand, sig, author, raw, self.used_ids,
-            self.used_sig, self.author_count, self.path_ids, self.end_row)
-        items = [it for j in jobs for it in j["items"]]
+            cfg, off, [j["k"] for j in jobs], [j["need"] for j in jobs], [vm.reverse_id_map.get(i, -1) for i in items],
+            sig, author, raw, self.used_ids, self.used_sig, self.author_count, self.path_ids, self.end_row)
         return found, [items[p] for p in pos], failed, dist
 
 

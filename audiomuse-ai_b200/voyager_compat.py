@@ -200,6 +200,15 @@ class Index:
     def _row_of(self, id) -> int:
         return int(self._rows_of([id], strict=True)[0])
 
+    def _candidates(self, cand_ids, *keys):
+        """(i64 rows of the candidate ids, -1 for an id not in the index, then each key array as i32), all 1-D and of one
+        length."""
+        rows = self._rows_of(cand_ids, strict=False)
+        keys = [np.ascontiguousarray(k, dtype=np.int32) for k in keys]
+        if rows.ndim != 1 or any(k.shape != rows.shape for k in keys):
+            raise ValueError("candidate arrays differ in length")
+        return (rows, *keys)
+
     def get_vector(self, id) -> np.ndarray:
         """The STORED vector: unit-normalised for Space.Cosine, like voyager.  One row gathered on the device and
         copied back (no host mirror of the library)."""
@@ -303,9 +312,8 @@ class Index:
         need = np.ascontiguousarray(job_need, dtype=np.int32)
         if off.shape != (n_jobs + 1,) or need.shape != (n_jobs,):
             raise ValueError("job_off / job_need do not match job_n")
-        rows = self._rows_of(cand_ids, strict=False)
-        keys = [np.ascontiguousarray(k, dtype=np.int32) for k in (cand_sig, cand_author, cand_author_raw)]
-        if any(k.shape != rows.shape for k in keys) or (n_jobs and off[-1] != len(rows)):
+        rows, sig, author, raw = self._candidates(cand_ids, cand_sig, cand_author, cand_author_raw)
+        if n_jobs and off[-1] != len(rows):
             raise ValueError("candidate arrays differ in length")
         if used_sig.dtype != np.uint8 or author_count.dtype != np.int32:
             raise ValueError("used_sig must be uint8 and author_count int32")
@@ -320,8 +328,8 @@ class Index:
         dist = np.empty(len(path), dtype=np.float64)
         h = self._ensure_built()
         _lib.check(_lib.load().am_knn_song_path(
-            h, C.byref(cfg), n_jobs, _lib.ptr(off), _lib.ptr(jn), _lib.ptr(need), _lib.ptr(rows), _lib.ptr(keys[0]),
-            _lib.ptr(keys[1]), _lib.ptr(keys[2]), len(used_sig), len(author_count), _lib.ptr(used), C.byref(n_used),
+            h, C.byref(cfg), n_jobs, _lib.ptr(off), _lib.ptr(jn), _lib.ptr(need), _lib.ptr(rows), _lib.ptr(sig),
+            _lib.ptr(author), _lib.ptr(raw), len(used_sig), len(author_count), _lib.ptr(used), C.byref(n_used),
             _lib.ptr(used_sig), _lib.ptr(author_count), _lib.ptr(path), C.byref(n_path), self._row_of(end_id),
             _lib.ptr(found), _lib.ptr(pos), C.byref(failed), _lib.ptr(dist)))
         found = found[:n_jobs].copy()
@@ -342,11 +350,7 @@ class Index:
         sub = None if sub_centroid is None else np.ascontiguousarray(sub_centroid, dtype=np.float64).reshape(-1)
         if add.shape[0] != self.num_dimensions or (sub is not None and sub.shape[0] != self.num_dimensions):
             raise ValueError(f"centroids must have dimension {self.num_dimensions}")
-        cand = self._rows_of(cand_ids, strict=False)
-        sig = np.ascontiguousarray(cand_sig, dtype=np.int32)
-        raw = np.ascontiguousarray(cand_author_raw, dtype=np.int32)
-        if sig.shape != cand.shape or raw.shape != cand.shape:
-            raise ValueError("candidate arrays differ in length")
+        cand, sig, raw = self._candidates(cand_ids, cand_sig, cand_author_raw)
         if not 1 <= cfg.n <= _lib.ALCHEMY_MAX_N or len(cand) > _lib.ALCHEMY_MAX_CANDIDATES or (
                 cfg.skip_chain and len(cand) > cfg.n):
             raise ValueError(f"{len(cand)} candidates for n = {cfg.n}: n must be in [1, {_lib.ALCHEMY_MAX_N}], the "
@@ -377,11 +381,7 @@ class Index:
         vector), cand_sig / cand_author_raw the dense keys the header describes, n_sig the number of signature keys.
         mood f64[n_cand, 6] / mood_ok / target_mood f64[6] run the mood stage, mood=None skips it.  Returns (positions in
         cand_ids of the survivors, in order; their f64 mood distances, or None without the mood stage)."""
-        cand = self._rows_of(cand_ids, strict=False)
-        sig = np.ascontiguousarray(cand_sig, dtype=np.int32)
-        raw = np.ascontiguousarray(cand_author_raw, dtype=np.int32)
-        if sig.shape != cand.shape or raw.shape != cand.shape or cand.ndim != 1:
-            raise ValueError("candidate arrays differ in length")
+        cand, sig, raw = self._candidates(cand_ids, cand_sig, cand_author_raw)
         target = -1 if target_id is None else self._row_of(target_id)
         if mood is not None:
             mood = np.ascontiguousarray(mood, dtype=np.float64).reshape(len(cand), 6)

@@ -8,7 +8,7 @@ import types
 import numpy as np
 import pytest
 
-from audiomuse_ai_b200 import integration, similar_tracks as st, voyager_compat as vc
+from audiomuse_ai_b200 import by_vector, integration, similar_tracks as st, voyager_compat as vc
 from oracle import knn as oknn
 from oracle import similar_tracks as osim
 from tests.golden import make_similar_tracks_golden as gen
@@ -194,14 +194,14 @@ def test_index_similar_checks_its_arrays_before_the_library():
         idx.farthest(17)
 
 
-def test_query_sizes_follow_the_reference():
+def test_by_id_and_by_vector_query_sizes_follow_the_reference():
     assert st.by_id_query_size(10, True, False, None, 10**6) == 10 + 30 + 1
     assert st.by_id_query_size(10, False, False, None, 10**6) == 10 + 3 + 1
     assert st.by_id_query_size(100, False, True, None, 10**6) == 100 + 300 + 1
     assert st.by_id_query_size(500, True, False, True, 10**6) == 4501
     assert st.by_id_query_size(500, False, False, True, 10**6) == 2501
     assert st.by_id_query_size(500, True, False, True, 3000) == 3000
-    assert st.by_vector_query_size(100, True, 10**6) == 500 and st.by_vector_query_size(100, False, 10**6) == 120
+    assert by_vector.query_size(100, True, 10**6) == 500 and by_vector.query_size(100, False, 10**6) == 120
 
 
 # ------------------------------------------------------------------------------------------------ the early returns

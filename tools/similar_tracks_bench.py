@@ -103,7 +103,7 @@ class Reference:
 
     def by_vector(self, vec, n, ed):
         vm = self.vm
-        ids, dists = vm.voyager_index.query(vec, k=st.by_vector_query_size(n, ed, len(vm.voyager_index)))
+        ids, dists = vm.voyager_index.query(vec, k=st.query_size(n, ed, len(vm.voyager_index)))
         kept = self.filter([{"item_id": vm.id_map[int(i)], "distance": float(d)} for i, d in zip(ids, dists)])
         det = self.details([s["item_id"] for s in kept])
         unique, added = [], []
