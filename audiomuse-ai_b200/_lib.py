@@ -105,6 +105,13 @@ SIGNATURES = {
     "am_clap_embed_tracks_submit": (_i, [_vp, _P(MelCfg), _vp, _i, _vp, _i, _vp]),
     "am_clap_embed_tracks_collect": (_i, [_vp]),
     "am_clap_embed_tracks_dev": (_i, [_vp, _vp, _vp, _i, _vp, _i, _i, _vp, _vp]),
+    "am_text_load": (_i, [C.c_char_p, _P(_vp)]),
+    "am_text_load_mem": (_i, [_vp, _sz, _P(_vp)]),
+    "am_text_describe_file": (_i, [C.c_char_p, C.c_char_p, _i]),
+    "am_text_embedding_dim": (_i, [_vp]),
+    "am_text_release_workspace": (_i, [_vp]),
+    "am_text_free": (None, [_vp]),
+    "am_text_embed": (_i, [_vp, _vp, _vp, _i, _i, _vp]),
     "am_knn_build": (_i, [_vp, _i64, _i, _i, _P(_vp)]),
     "am_knn_build_dev": (_i, [_vp, _i64, _i, _i, _vp, _P(_vp)]),
     "am_knn_free": (None, [_vp]),

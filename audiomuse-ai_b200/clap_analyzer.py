@@ -267,6 +267,76 @@ class B200Session:
             pass
 
 
+class B200TextSession:
+    """Duck type of the onnxruntime.InferenceSession the reference keeps in ``_text_session``
+    (tasks/clap_analyzer.py:168-240): ``run(None, {'input_ids': i64[B, T], 'attention_mask': i64[B, T]}) ->
+    [f32[B, dim]]``, plus ``get_inputs`` and ``get_providers``.  `path` is the deployed clap_text_model.onnx (tensor
+    data inline or in `<name>.onnx.data`), `blob` the same bytes with inline data; both are lowered by am_text_load.
+    Calls from several threads are serialised on the session's lock."""
+
+    def __init__(self, blob: Optional[bytes] = None, path: Optional[str] = None):
+        lib = _lib.load()
+        self._lib = lib
+        self._h = None
+        h = C.c_void_p()
+        if path is not None:
+            _lib.check(lib.am_text_load(os.fsencode(path), C.byref(h)))
+        elif blob is not None:
+            buf = (C.c_char * len(blob)).from_buffer_copy(blob)
+            _lib.check(lib.am_text_load_mem(C.cast(buf, C.c_void_p), len(blob), C.byref(h)))
+        else:
+            raise ValueError("B200TextSession needs a model path or a model blob")
+        self._h = h
+        self.embedding_dim = int(lib.am_text_embedding_dim(h))
+        self._mu = threading.Lock()
+
+    @staticmethod
+    def describe(path: str) -> str:
+        """The program am_text_load would run for `path` (needs no GPU)."""
+        lib = _lib.load()
+        buf = C.create_string_buffer(1 << 16)
+        _lib.check(min(0, lib.am_text_describe_file(os.fsencode(path), buf, len(buf))))
+        return buf.value.decode()
+
+    def get_providers(self):
+        return ["B200ExecutionProvider"]
+
+    def get_inputs(self):
+        return [SimpleNamespace(name="input_ids", shape=["batch_size", "sequence_length"], type="tensor(int64)"),
+                SimpleNamespace(name="attention_mask", shape=["batch_size", "sequence_length"], type="tensor(int64)")]
+
+    def run(self, output_names, input_feed):
+        ids = np.ascontiguousarray(input_feed["input_ids"], dtype=np.int64)
+        mask = np.ascontiguousarray(input_feed["attention_mask"], dtype=np.int64)
+        if ids.ndim != 2 or mask.shape != ids.shape:
+            raise ValueError(f"input_ids and attention_mask must both be [B, T], got {ids.shape} and {mask.shape}")
+        B, T = ids.shape
+        out = np.empty((B, self.embedding_dim), dtype=np.float32)
+        if B == 0:
+            return [out]
+        with self._mu:
+            if self._h is None:
+                raise RuntimeError("B200TextSession.run: the session is closed")
+            _lib.check(self._lib.am_text_embed(self._h, _lib.ptr(ids), _lib.ptr(mask), B, T, _lib.ptr(out)))
+        return [out]
+
+    def release_workspace(self) -> None:
+        with self._mu:
+            _lib.check(self._lib.am_text_release_workspace(self._h))
+
+    def close(self):
+        with self._mu:
+            if getattr(self, "_h", None):
+                self._lib.am_text_free(self._h)
+                self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
 def _weights_path() -> str:
     """The reference's own model file, config.CLAP_AUDIO_MODEL_PATH (config.py:375; an ONNX ModelProto, read and
     lowered by am_clap_load); CLAP_B200_WEIGHTS_PATH, when set, overrides it (an AMW1 blob or another ONNX file)."""

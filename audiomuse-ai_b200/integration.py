@@ -22,6 +22,40 @@ CLAP_NAMES = ("compute_mel_spectrogram", "analyze_audio_file", "initialize_clap_
               "unload_clap_audio_only", "unload_clap_model", "is_clap_model_loaded", "is_clap_audio_loaded")
 
 
+def _apply_clap_text(text_module, clap_module) -> None:
+    from . import clap_analyzer as b200_clap
+
+    def _load_text_model():
+        path = text_module.config.CLAP_TEXT_MODEL_PATH
+        logger.info("Loading CLAP text model from %s on the GPU", path)
+        return b200_clap.B200TextSession(path=path)
+
+    text_module._load_text_model = _load_text_model
+    if clap_module is None:
+        return
+    unload_audio, audio_loaded = clap_module.unload_clap_model, clap_module.is_clap_model_loaded
+
+    def unload_clap_model() -> bool:
+        freed = unload_audio()
+        session = text_module._text_session
+        if session is not None:
+            try:
+                close = getattr(session, "close", None)
+                if close is not None:
+                    close()
+            finally:
+                text_module._text_session = None
+                text_module._tokenizer = None
+            freed = True
+        return freed
+
+    def is_clap_model_loaded() -> bool:
+        return audio_loaded() or text_module._text_session is not None
+
+    clap_module.unload_clap_model = unload_clap_model
+    clap_module.is_clap_model_loaded = is_clap_model_loaded
+
+
 def install_voyager_shim() -> None:
     """`import voyager` in tasks/voyager_manager.py:12 and tasks/clap_text_search.py resolves to the flat exact index:
     Index(space, num_dimensions, M, ef_construction), add_items, query, get_vector, len, .ef, save / load,
@@ -126,7 +160,7 @@ def apply(clap=None, voyager_manager=None, clustering=None, allow_sklearn_fallba
           clustering_helper=None, song_alchemy=None, app_map=None, artist_gmm_manager=None,
           gaussian_mixture=None, radius_walk=None, path_manager=None, app_path=None, analysis=None, alchemy=None,
           app_alchemy=None, similar=None, app_voyager=None, sonic_fingerprint=None,
-          gmm_all_covariance_types: bool = False) -> None:
+          gmm_all_covariance_types: bool = False, clap_text=None) -> None:
     """clap / voyager_manager / clustering / clustering_helper: the reference's already imported tasks.* modules (pass
     only the ones to patch).  allow_sklearn_fallback keeps the reference's contract that a failing GPU k-means silently
     falls back to scikit-learn (tasks/clustering_gpu.py:130-148); this repository's own tests run with it off so a
@@ -157,7 +191,13 @@ def apply(clap=None, voyager_manager=None, clustering=None, allow_sklearn_fallba
     imported, so pass them too for their endpoints to use them, and app_path (app_path.py:6) gets
     find_nearest_neighbors_by_vector when similar= is passed with it.  analysis (the reference's tasks.analysis) gets track_features.LibrosaFacade as
     its `librosa`: analyze_track's beat_track, rms and chroma_stft (:344-348) run on the device, every other librosa use
-    of the module goes to the librosa it imported; sys.modules["librosa"] is left alone."""
+    of the module goes to the librosa it imported; sys.modules["librosa"] is left alone.  clap_text (the reference's
+    tasks.clap_analyzer) gets a _load_text_model that returns a B200TextSession over config.CLAP_TEXT_MODEL_PATH, read
+    when it is called; initialize_clap_text_model looks that name up at call time (:300), so text search's query
+    embeddings and get_text_embeddings_batch run on the device while the tokenizer, get_text_embedding and
+    search_by_text stay the reference's.  With clap= as well, the installed unload_clap_model and is_clap_model_loaded
+    also close and clear the module's _text_session (and its tokenizer, as the reference's unload does), so the idle
+    unload timer frees the text model too."""
     if gmm_all_covariance_types and gaussian_mixture is None:
         raise ValueError("gmm_all_covariance_types= selects the class installed by gaussian_mixture=: pass both")
     if analysis is not None:
@@ -170,6 +210,8 @@ def apply(clap=None, voyager_manager=None, clustering=None, allow_sklearn_fallba
 
         for name in CLAP_NAMES:
             setattr(clap, name, getattr(b200_clap, name))
+    if clap_text is not None:
+        _apply_clap_text(clap_text, clap)
     if voyager_manager is not None:
         voyager_manager._filter_by_distance = make_filter_by_distance(voyager_manager)
     if radius_walk is not None:

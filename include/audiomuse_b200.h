@@ -191,6 +191,32 @@ AM_API int am_clap_embed_tracks_dev(am_model* m, const am_mel_plan* plan, const 
                              int n_samples, const int32_t* seg_offsets_dev, int n_tracks,
                              int n_segments, float* out_dev, void* stream);
 
+/* ------------------------------------------------------------------ CLAP text encoder
+ * Replaces the onnxruntime session over CLAP_TEXT_MODEL_PATH (tasks/clap_analyzer.py:168-240) that
+ * get_text_embedding (:577-628) and get_text_embeddings_batch (:631-687) run on
+ * {'input_ids', 'attention_mask'} int64 [B, T] -> 'text_embedding' f32[B, dim].
+ *
+ * am_text_load takes the deployed clap_text_model.onnx (TextCLAPWrapper of query/pythorch.sh:95-127: RoBERTa, its
+ * pooler, Linear -> ReLU -> Linear and F.normalize; torch.onnx.export opset 17 with constant folding), with tensor
+ * data inline or in `<name>.onnx.data` next to it.  The graph is lowered to the text program (csrc/text_model.cu
+ * lists the accepted patterns, eager and SDPA attention among them); any other node fails the load with its name and
+ * operator in am_last_error().  No CUDA work happens before the first load. */
+typedef struct am_text_model am_text_model;
+AM_API int am_text_load(const char* model_path, am_text_model** out);
+/* same from memory (ONNX bytes with inline tensor data) */
+AM_API int am_text_load_mem(const void* blob, size_t nbytes, am_text_model** out);
+/* host-only, needs no GPU: parses + lowers `model_path` and writes the program (dimensions, attention form, one line
+ * per layer, pooler and projection) into buf (NUL terminated, truncated to cap); returns the size needed, or a
+ * negative am_status */
+AM_API int am_text_describe_file(const char* model_path, char* buf, int cap);
+AM_API int am_text_embedding_dim(const am_text_model* m);
+/* frees the per-(B, T) workspace; weights stay */
+AM_API int am_text_release_workspace(am_text_model* m);
+AM_API void am_text_free(am_text_model* m);
+/* host: ids, mask int64 [B, T] -> out f32[B, dim], each row L2-normalised as the graph's F.normalize does.
+ * T + pad id must stay below the model's position count (RoBERTa: T <= 512).  Same (B, T) input, same bits. */
+AM_API int am_text_embed(am_text_model* m, const int64_t* ids, const int64_t* mask, int B, int T, float* out);
+
 /* ------------------------------------------------------------------ K4: exact k-NN index
  * Replaces the voyager.Index object (voyager==2.1.0) used at tasks/voyager_manager.py:183,
  * 341-346,1397,1447,1580,1681 and tasks/clap_text_search.py:173,242,263,493.
