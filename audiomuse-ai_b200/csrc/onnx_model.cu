@@ -26,7 +26,6 @@
 #include <cmath>
 #include <cstdlib>
 #include <map>
-#include <memory>
 #include <set>
 
 namespace am {
@@ -50,74 +49,14 @@ struct Val {
   int reg = -1, dim = 0;
 };
 
-#define LOWER_FAIL(node, ...)                                                                     \
-  do {                                                                                            \
-    char _b[512];                                                                                 \
-    std::snprintf(_b, sizeof _b, __VA_ARGS__);                                                    \
-    set_error("onnx: cannot lower node '%s' (%s): %s", (node).name.empty() ? (node).out[0].c_str() : (node).name.c_str(), \
-              (node).op.c_str(), _b);                                                             \
-    return AM_ERR_INVALID;                                                                        \
-  } while (0)
-
-struct Lowerer {
-  OGraph& g;
+struct Lowerer : GraphIndex {
   ModelSpec& spec;
   std::map<std::string, Val> vals;
-  std::map<std::string, std::vector<int>> consumers;
-  std::map<std::string, const OTensor*> consts;
-  std::vector<std::unique_ptr<OTensor>> owned;
   std::vector<std::string> layer_input;  // value name each emitted layer reads
   std::string cur;                        // value name of the trunk's latest activation
-  std::set<std::string> graph_outputs;
 
-  Lowerer(OGraph& g_, ModelSpec& s_) : g(g_), spec(s_) {}
+  Lowerer(OGraph& g_, ModelSpec& s_) : GraphIndex(g_), spec(s_) {}
 
-  const OTensor* cst(const std::string& name) const {
-    auto it = consts.find(name);
-    return it == consts.end() ? nullptr : it->second;
-  }
-  const OTensor* cin(const ONode& n, size_t idx) const { return idx < n.in.size() && !n.in[idx].empty() ? cst(n.in[idx]) : nullptr; }
-  // the single consumer of a value (or -1 when it has several / is a graph output)
-  int sole_consumer(const std::string& name) const {
-    auto it = consumers.find(name);
-    if (it == consumers.end() || it->second.size() != 1 || graph_outputs.count(name)) return -1;
-    return it->second[0];
-  }
-  static int64_t attr_i(const ONode& n, const char* k, int64_t dflt) {
-    auto it = n.attrs.find(k);
-    return it != n.attrs.end() && it->second.has_i ? it->second.i : dflt;
-  }
-  static float attr_f(const ONode& n, const char* k, float dflt) {
-    auto it = n.attrs.find(k);
-    return it != n.attrs.end() && it->second.has_f ? it->second.f : dflt;
-  }
-  static std::vector<int64_t> attr_ints(const ONode& n, const char* k) {
-    auto it = n.attrs.find(k);
-    return it != n.attrs.end() ? it->second.ints : std::vector<int64_t>();
-  }
-  // integer list given as attribute `k` (older opsets / torch's serializer) or as constant input `idx`
-  bool ints_of(const ONode& n, const char* k, size_t idx, std::vector<int64_t>* out) const {
-    if (const OTensor* t = cin(n, idx)) {
-      out->clear();
-      for (size_t q = 0; q < t->count(); ++q) out->push_back((int64_t)t->at(q));
-      return true;
-    }
-    auto it = n.attrs.find(k);
-    if (it == n.attrs.end()) return false;
-    *out = it->second.ints;
-    return true;
-  }
-  bool scalar_of(const ONode& n, const char* k, size_t idx, float* out) const {
-    if (const OTensor* t = cin(n, idx)) {
-      if (t->count() != 1) return false;
-      *out = (float)t->at(0);
-      return true;
-    }
-    auto it = n.attrs.find(k);
-    if (it == n.attrs.end() || !it->second.has_f) return false;
-    *out = it->second.f;
-    return true;
-  }
   int new_reg(int dim) {
     spec.reg_dim.push_back(dim);
     return spec.n_regs++;
@@ -142,8 +81,8 @@ struct Lowerer {
       return (std::fabs(a - 1.0f / 6.0f) < 1e-6f && std::fabs(b - 0.5f) < 1e-6f) ? kActHardSigmoid : -1;
     }
     if (n.op == "Clip") {
-      float lo = -INFINITY, hi = INFINITY;
-      const bool has_lo = scalar_of(n, "min", 1, &lo), has_hi = scalar_of(n, "max", 2, &hi);
+      double lo = -INFINITY, hi = INFINITY;
+      const bool has_lo = scalar_of(n, 1, &lo, "min"), has_hi = scalar_of(n, 2, &hi, "max");
       if (has_lo && lo == 0.f && has_hi && hi == 6.f) return kActRelu6;
       if (has_lo && lo == 0.f && (!has_hi || std::isinf(hi))) return kActRelu;
       return -1;
@@ -152,10 +91,12 @@ struct Lowerer {
   }
 
   int run();
+  int lower_match(const Match& m);
   int lower_view_op(ONode& n, const Val& v);
   int lower_conv(ONode& n);
   int lower_trunk_pool(ONode& n, int ni);
-  int lower_vec(ONode& n, int ni);
+  Val emit(VecOp op, int dim);
+  int lower_vec(ONode& n);
   int finish();
 };
 
@@ -237,8 +178,8 @@ int Lowerer::lower_view_op(ONode& n, const Val& v) {
   } else if (n.op == "Pad") {
     std::vector<int64_t> pads;
     if (!ints_of(n, "pads", 1, &pads) || pads.size() != 8) LOWER_FAIL(n, "needs 8 constant pads on a rank-4 view");
-    float val = 0.f;
-    scalar_of(n, "value", 2, &val);
+    double val = 0.0;
+    scalar_of(n, 2, &val, "value");
     auto it = n.attrs.find("mode");
     if ((it != n.attrs.end() && it->second.s != "constant") || val != 0.f) LOWER_FAIL(n, "only constant zero padding");
     if (pads[0] || pads[1] || pads[4] || pads[5]) LOWER_FAIL(n, "pads batch / channel axes");
@@ -468,23 +409,50 @@ int Lowerer::lower_trunk_pool(ONode& n, int ni) {
   return AM_OK;
 }
 
-static bool close_to(double a, double b, double tol = 1e-5) { return std::fabs(a - b) <= tol * std::max(1.0, std::fabs(b)); }
+Val Lowerer::emit(VecOp op, int dim) {
+  op.dst = new_reg(dim);
+  if (!op.N) op.N = dim;
+  spec.head.push_back(op);
+  Val o;
+  o.kind = kVec;
+  o.reg = op.dst;
+  o.dim = dim;
+  return o;
+}
 
-int Lowerer::lower_vec(ONode& n, int ni) {
+// a LayerNorm, exact GELU or L2 normalise of a feature row: one head op
+int Lowerer::lower_match(const Match& m) {
+  const ONode& n = g.nodes[(size_t)m.nodes[0]];
+  auto it = vals.find(m.in);
+  if (it == vals.end() || it->second.kind != kVec) LOWER_FAIL(n, "reads '%s', which is not a pooled feature row", m.in.c_str());
+  const Val x = it->second;
+  VecOp op;
+  op.a = x.reg;
+  if (m.kind == Match::kGelu) {
+    op.kind = kVecUnary;
+    op.act = kActGelu;
+  } else if (m.axis != -1 && m.axis != 1) {
+    LOWER_FAIL(n, "normalises axis %lld of a feature row", (long long)m.axis);
+  } else if (m.kind == Match::kL2Norm) {
+    op.kind = kVecL2Norm;
+    op.eps2 = m.eps;
+  } else {
+    if ((m.gamma && (int)m.gamma->count() != x.dim) || (m.beta && (int)m.beta->count() != x.dim))
+      LOWER_FAIL(n, "LayerNorm affine of a width other than the row's %d", x.dim);
+    op.kind = kVecLayerNorm;
+    op.eps = m.eps;
+    op.w = m.gamma ? m.gamma->f : std::vector<float>((size_t)x.dim, 1.f);
+    op.bias = m.beta ? m.beta->f : std::vector<float>((size_t)x.dim, 0.f);
+  }
+  vals[m.out] = emit(op, x.dim);
+  return AM_OK;
+}
+
+int Lowerer::lower_vec(ONode& n) {
   auto vec_in = [&](size_t idx) -> const Val* {
     if (idx >= n.in.size()) return nullptr;
     auto it = vals.find(n.in[idx]);
     return it != vals.end() && it->second.kind == kVec ? &it->second : nullptr;
-  };
-  auto emit = [&](VecOp op, int dim) {
-    op.dst = new_reg(dim);
-    if (!op.N) op.N = dim;
-    spec.head.push_back(op);
-    Val o;
-    o.kind = kVec;
-    o.reg = op.dst;
-    o.dim = dim;
-    return o;
   };
   const Val* x0 = vec_in(0);
   const Val* x1 = vec_in(1);
@@ -495,40 +463,19 @@ int Lowerer::lower_vec(ONode& n, int ni) {
     return AM_OK;
   }
   if (op == "MatMul" || op == "Gemm") {
-    const OTensor* w = cin(n, 1);
-    if (!x0 || !w || w->dims.size() != 2) LOWER_FAIL(n, "needs (feature rows) x (constant matrix)");
-    const bool tb = op == "Gemm" && attr_i(n, "transB", 0) != 0;
-    if (op == "Gemm" && (attr_i(n, "transA", 0) != 0 || attr_f(n, "alpha", 1.f) != 1.f || attr_f(n, "beta", 1.f) != 1.f))
-      LOWER_FAIL(n, "Gemm with transA / alpha / beta");
-    const int K = (int)(tb ? w->dims[1] : w->dims[0]), N = (int)(tb ? w->dims[0] : w->dims[1]);
-    if (K != x0->dim) LOWER_FAIL(n, "matrix expects %d inputs, the row has %d", K, x0->dim);
+    if (!x0) LOWER_FAIL(n, "needs (feature rows) x (constant matrix)");
     VecOp l;
     l.kind = kVecLinear;
     l.a = x0->reg;
-    l.K = K;
-    l.N = N;
-    l.w.resize((size_t)N * K);
-    for (int o = 0; o < N; ++o)
-      for (int k = 0; k < K; ++k) l.w[(size_t)o * K + k] = tb ? w->f[(size_t)o * K + k] : w->f[(size_t)k * N + o];
+    AM_TRY(linear_weight(n, &l.K, &l.N, &l.w));
+    if (l.K != x0->dim) LOWER_FAIL(n, "matrix expects %d inputs, the row has %d", l.K, x0->dim);
     if (op == "Gemm") {
       if (const OTensor* b = cin(n, 2)) {
-        if ((int)b->count() != N) LOWER_FAIL(n, "bias of %zu for %d outputs", b->count(), N);
+        if ((int)b->count() != l.N) LOWER_FAIL(n, "bias of %zu for %d outputs", b->count(), l.N);
         l.bias = b->f;
       }
     }
-    vals[n.out[0]] = emit(l, N);
-    return AM_OK;
-  }
-  if (op == "LayerNormalization") {
-    const OTensor *ga = cin(n, 1), *be = cin(n, 2);
-    if (!x0 || !ga || (int)ga->count() != x0->dim) LOWER_FAIL(n, "needs a feature row and a constant scale of its width");
-    VecOp l;
-    l.kind = kVecLayerNorm;
-    l.a = x0->reg;
-    l.eps = attr_f(n, "epsilon", 1e-5f);
-    l.w = ga->f;
-    l.bias = be ? be->f : std::vector<float>((size_t)x0->dim, 0.f);
-    vals[n.out[0]] = emit(l, x0->dim);
+    vals[n.out[0]] = emit(l, l.N);
     return AM_OK;
   }
   int act = act_of(n);
@@ -548,123 +495,6 @@ int Lowerer::lower_vec(ONode& n, int ni) {
     u.act = act;
     vals[act_out] = emit(u, x0->dim);
     return AM_OK;
-  }
-  // ---- GELU, exact form: x * 0.5 * (1 + erf(x / sqrt(2)))  exported as Div, Erf, Add, Mul, Mul
-  if (op == "Div" && x0 && cin(n, 1) && cin(n, 1)->count() == 1 && close_to(cin(n, 1)->at(0), std::sqrt(2.0), 1e-4)) {
-    do {
-      int er = -1;
-      for (int c : consumers[n.out[0]])
-        if (g.nodes[c].op == "Erf") er = c;
-      if (er < 0 || consumers[n.out[0]].size() != 1) break;
-      const int ad = sole_consumer(g.nodes[er].out[0]);
-      if (ad < 0 || g.nodes[ad].op != "Add") break;
-      const OTensor* one = cin(g.nodes[ad], 1) ? cin(g.nodes[ad], 1) : cin(g.nodes[ad], 0);
-      if (!one || one->count() != 1 || !close_to(one->at(0), 1.0)) break;
-      const int m1 = sole_consumer(g.nodes[ad].out[0]);
-      if (m1 < 0 || g.nodes[m1].op != "Mul") break;
-      const std::string& xin = g.nodes[m1].in[0] == g.nodes[ad].out[0] ? g.nodes[m1].in[1] : g.nodes[m1].in[0];
-      if (xin != n.in[0]) break;
-      const int m2 = sole_consumer(g.nodes[m1].out[0]);
-      if (m2 < 0 || g.nodes[m2].op != "Mul") break;
-      const OTensor* half = cin(g.nodes[m2], 1) ? cin(g.nodes[m2], 1) : cin(g.nodes[m2], 0);
-      if (!half || half->count() != 1 || !close_to(half->at(0), 0.5)) break;
-      VecOp u;
-      u.kind = kVecUnary;
-      u.a = x0->reg;
-      u.act = kActGelu;
-      vals[g.nodes[m2].out[0]] = emit(u, x0->dim);
-      for (int q : {ni, er, ad, m1, m2}) g.nodes[q].done = true;
-      return AM_OK;
-    } while (false);
-    LOWER_FAIL(n, "division by sqrt(2) that is not part of an exact-GELU pattern");
-  }
-  // ---- LayerNorm, decomposed: ReduceMean, Sub, Pow 2, ReduceMean, Add eps, Sqrt, Div, Mul g, Add b
-  if (op == "ReduceMean" && x0) {
-    do {
-      std::vector<int64_t> axes;
-      if (!ints_of(n, "axes", 1, &axes) || axes.size() != 1 || (axes[0] != -1 && axes[0] != 1)) break;
-      int sb = -1;
-      for (int c : consumers[n.out[0]])
-        if (g.nodes[c].op == "Sub" && g.nodes[c].in[0] == n.in[0]) sb = c;
-      if (sb < 0 || consumers[n.out[0]].size() != 1) break;
-      const std::string& cen = g.nodes[sb].out[0];
-      int pw = -1, dv = -1;
-      for (int c : consumers[cen]) {
-        if (g.nodes[c].op == "Pow") pw = c;
-        if (g.nodes[c].op == "Div" && g.nodes[c].in[0] == cen) dv = c;
-      }
-      if (pw < 0 || dv < 0 || consumers[cen].size() != 2) break;
-      const OTensor* two = cin(g.nodes[pw], 1);
-      if (!two || two->count() != 1 || !close_to(two->at(0), 2.0)) break;
-      const int rm = sole_consumer(g.nodes[pw].out[0]);
-      if (rm < 0 || g.nodes[rm].op != "ReduceMean") break;
-      const int ae = sole_consumer(g.nodes[rm].out[0]);
-      if (ae < 0 || g.nodes[ae].op != "Add") break;
-      const OTensor* eps = cin(g.nodes[ae], 1) ? cin(g.nodes[ae], 1) : cin(g.nodes[ae], 0);
-      if (!eps || eps->count() != 1) break;
-      const int sq = sole_consumer(g.nodes[ae].out[0]);
-      if (sq < 0 || g.nodes[sq].op != "Sqrt") break;
-      if (sole_consumer(g.nodes[sq].out[0]) != dv) break;
-      VecOp l;
-      l.kind = kVecLayerNorm;
-      l.a = x0->reg;
-      l.eps = (float)eps->at(0);
-      l.w.assign((size_t)x0->dim, 1.f);
-      l.bias.assign((size_t)x0->dim, 0.f);
-      std::vector<int> used = {ni, sb, pw, rm, ae, sq, dv};
-      std::string out = g.nodes[dv].out[0];
-      const int mg = sole_consumer(out);
-      if (mg >= 0 && g.nodes[mg].op == "Mul") {
-        const OTensor* ga = cin(g.nodes[mg], 1) ? cin(g.nodes[mg], 1) : cin(g.nodes[mg], 0);
-        if (ga && (int)ga->count() == x0->dim) {
-          l.w = ga->f;
-          used.push_back(mg);
-          out = g.nodes[mg].out[0];
-          const int ab = sole_consumer(out);
-          if (ab >= 0 && g.nodes[ab].op == "Add") {
-            const OTensor* be = cin(g.nodes[ab], 1) ? cin(g.nodes[ab], 1) : cin(g.nodes[ab], 0);
-            if (be && (int)be->count() == x0->dim) {
-              l.bias = be->f;
-              used.push_back(ab);
-              out = g.nodes[ab].out[0];
-            }
-          }
-        }
-      }
-      vals[out] = emit(l, x0->dim);
-      for (int q : used) g.nodes[q].done = true;
-      return AM_OK;
-    } while (false);
-    LOWER_FAIL(n, "row mean that is not part of a LayerNorm pattern");
-  }
-  // ---- F.normalize: ReduceL2(keepdims) -> Clip(min eps) -> [Expand(., Shape(x))] -> Div(x, .)
-  if (op == "ReduceL2" && x0) {
-    do {
-      std::vector<int64_t> axes;
-      if (!ints_of(n, "axes", 1, &axes) || axes.size() != 1 || (axes[0] != -1 && axes[0] != 1)) break;
-      int at = sole_consumer(n.out[0]);
-      float eps = 0.f;
-      std::vector<int> used = {ni};
-      if (at >= 0 && g.nodes[at].op == "Clip") {
-        if (!scalar_of(g.nodes[at], "min", 1, &eps)) break;
-        used.push_back(at);
-        at = sole_consumer(g.nodes[at].out[0]);
-      }
-      if (at >= 0 && g.nodes[at].op == "Expand") {
-        used.push_back(at);
-        at = sole_consumer(g.nodes[at].out[0]);
-      }
-      if (at < 0 || g.nodes[at].op != "Div" || g.nodes[at].in[0] != n.in[0]) break;
-      used.push_back(at);
-      VecOp l;
-      l.kind = kVecL2Norm;
-      l.a = x0->reg;
-      l.eps2 = eps;
-      vals[g.nodes[at].out[0]] = emit(l, x0->dim);
-      for (int q : used) g.nodes[q].done = true;
-      return AM_OK;
-    } while (false);
-    LOWER_FAIL(n, "row norm that is not part of an L2-normalise pattern");
   }
   if (op == "Add" && x0 && x1) {
     if (x0->dim != x1->dim) LOWER_FAIL(n, "adds rows of %d and %d", x0->dim, x1->dim);
@@ -715,41 +545,23 @@ int Lowerer::run() {
     set_error("onnx: the graph has no output");
     return AM_ERR_INVALID;
   }
-  for (const auto& o : g.outputs) graph_outputs.insert(o);
-  for (auto& kv : g.init) consts[kv.first] = &kv.second;
-  for (size_t i = 0; i < g.nodes.size(); ++i)
-    for (const auto& in : g.nodes[i].in)
-      if (!in.empty()) consumers[in].push_back((int)i);
+  AM_TRY(build());
   {
     Val in;
     in.kind = kView;
     in.perm = {0, 1, 2, 3};
     vals[g.inputs[0]] = in;
   }
-  // constants first: the pattern matchers look ahead of the node being lowered
-  for (ONode& n : g.nodes) {
-    if (n.op != "Constant" || n.out.empty()) continue;
-    auto it = n.attrs.find("value");
-    if (it != n.attrs.end() && it->second.has_t) {
-      consts[n.out[0]] = &it->second.t;
-      continue;
-    }
-    auto fi = n.attrs.find("value_float");
-    auto ii = n.attrs.find("value_int");
-    auto t = std::make_unique<OTensor>();
-    if (fi != n.attrs.end() && fi->second.has_f) t->f.push_back(fi->second.f);
-    else if (ii != n.attrs.end() && ii->second.has_i) {
-      t->is_int = true;
-      t->i.push_back(ii->second.i);
-    } else LOWER_FAIL(n, "Constant without a tensor value");
-    consts[n.out[0]] = t.get();
-    owned.push_back(std::move(t));
-  }
   for (size_t ni = 0; ni < g.nodes.size(); ++ni) {
     ONode& n = g.nodes[ni];
     if (n.done) continue;
     if (n.out.empty()) continue;
-    if (n.op == "Constant") continue;  // registered by the pre-pass above
+    if (n.op == "Constant") continue;  // registered by the index
+    if (const Match* m = match_starting(ni)) {
+      AM_TRY(lower_match(*m));
+      for (int q : m->nodes) g.nodes[(size_t)q].done = true;
+      continue;
+    }
     if (n.in.empty() || n.in[0].empty()) LOWER_FAIL(n, "node without a data input");
     // which kind of value does it read?
     auto it0 = vals.find(n.in[0]);
@@ -762,7 +574,7 @@ int Lowerer::run() {
       LOWER_FAIL(n, "shape arithmetic is only supported inside F.normalize");
     }
     if (v.kind == kVec || (in1 && it1->second.kind == kVec)) {
-      AM_TRY(lower_vec(n, (int)ni));
+      AM_TRY(lower_vec(n));
       continue;
     }
     if (n.op == "Conv") {
@@ -787,8 +599,8 @@ int Lowerer::run() {
       std::vector<int64_t> pads;
       if (!ints_of(n, "pads", 1, &pads) || pads.size() != 8 || pads[0] || pads[1] || pads[4] || pads[5])
         LOWER_FAIL(n, "needs 8 constant pads on the spatial axes");
-      float val = 0.f;
-      scalar_of(n, "value", 2, &val);
+      double val = 0.0;
+      scalar_of(n, 2, &val, "value");
       if (val != 0.f) LOWER_FAIL(n, "non-zero pad value");
       Val o = v;
       o.pad_t += (int)pads[2];

@@ -96,10 +96,9 @@ enum TKind {
   tHid,                                              // a LayerNorm output: the hidden state
   tLin,                                              // MatMul (+ bias) of a hidden-like value by a constant
   tRes,                                              // tLin + residual hidden: waiting for its LayerNorm
-  tLnMean, tLnD, tLnSq, tLnVar, tLnVarE, tLnStd, tLnNorm, tLnScaled,  // decomposed LayerNorm
   tHeads, tScores, tProbs, tCtx, tCtxT, tCtxFlat,    // attention
-  tGHalf, tGDiv, tGErf, tGOne, tGProd, tGelu,        // Erf-GELU
-  tTok0, tPooled, tP1, tOutPre, tL2, tL2Clip, tOut   // pooler, projection, normalise
+  tGelu,                                             // GELU of the FFN's up projection
+  tTok0, tPooled, tP1, tOut                          // pooler, projection, normalise
 };
 
 struct TV {
@@ -116,83 +115,22 @@ struct TV {
   bool scaled_inputs = false;  // tScores: Q / K^T were scaled (SDPA form)
   bool masked = false;
   int q = -1, k = -1, v = -1;  // tScores / tProbs / tCtx*: linears
-  float eps = 0.f;             // tLnVarE..: LayerNorm eps
-  int ln_in = -1;              // tLn*: index into the lowerer's pending LayerNorm inputs
-  std::vector<float> gamma;    // tLnScaled
 };
 
-#define TFAIL(node, ...)                                                                                    \
-  do {                                                                                                      \
-    char _b[512];                                                                                           \
-    std::snprintf(_b, sizeof _b, __VA_ARGS__);                                                              \
-    set_error("onnx: cannot lower node '%s' (%s): %s", (node).name.empty() ? ((node).out.empty() ? "" : (node).out[0].c_str()) \
-                                                                           : (node).name.c_str(),           \
-              (node).op.c_str(), _b);                                                                       \
-    return AM_ERR_INVALID;                                                                                  \
-  } while (0)
-
-struct TextLowerer {
-  OGraph& g;
+struct TextLowerer : GraphIndex {
   Program& p;
   std::map<std::string, TV> vals;
-  std::map<std::string, OTensor> consts;  // Constant nodes
   std::vector<Linear> lins;
-  std::vector<TV> ln_inputs;  // the pre-LayerNorm value of each LayerNorm under way
   // the layer being assembled
   text::Layer cur;
   int stage = 0;  // 0: embeddings, 1: after the embedding LN or a layer's last LN, 2: after attention's LN
   int mask_kind = 0;  // 1 arithmetic (Cast/Sub/Mul), 2 masked_fill (Where)
 
-  TextLowerer(OGraph& g_, Program& p_) : g(g_), p(p_) {}
+  TextLowerer(OGraph& g_, Program& p_) : GraphIndex(g_), p(p_) {}
 
-  const OTensor* cst(const std::string& n) const {  // an initializer or the value of a Constant node
-    auto i = g.init.find(n);
-    if (i != g.init.end()) return &i->second;
-    auto it = consts.find(n);
-    return it == consts.end() ? nullptr : &it->second;
-  }
-  const OTensor* cin(const ONode& n, size_t i) const { return i < n.in.size() && !n.in[i].empty() ? cst(n.in[i]) : nullptr; }
   const TV* val(const std::string& n) const {
     auto it = vals.find(n);
     return it == vals.end() ? nullptr : &it->second;
-  }
-  static bool scalar(const OTensor* t, double* v) {
-    if (!t || t->count() != 1) return false;
-    *v = t->at(0);
-    return true;
-  }
-  static int64_t attr_i(const ONode& n, const char* k, int64_t d) {
-    auto it = n.attrs.find(k);
-    return it != n.attrs.end() && it->second.has_i ? it->second.i : d;
-  }
-  static std::vector<int64_t> attr_ints(const ONode& n, const char* k) {
-    auto it = n.attrs.find(k);
-    return it != n.attrs.end() ? it->second.ints : std::vector<int64_t>();
-  }
-  bool axes_last(const ONode& n, int rank_hint) const {  // ReduceMean / ReduceL2 / Softmax over the last axis
-    std::vector<int64_t> ax = attr_ints(n, "axes");
-    if (ax.empty())
-      if (const OTensor* t = cin(n, 1))
-        for (size_t i = 0; i < t->count(); ++i) ax.push_back((int64_t)t->at(i));
-    return ax.size() == 1 && (ax[0] == -1 || ax[0] == rank_hint - 1);
-  }
-  // a constant weight of a MatMul (x @ W: W is [K, N]) or Gemm (transB: [N, K]) as an [N, K] linear
-  int new_linear(const ONode& n, const OTensor* w, bool w_is_nk, int K_expect) {
-    if (!w || w->dims.size() != 2 || w->is_int) return -1;
-    Linear L;
-    const int r = (int)w->dims[0], c = (int)w->dims[1];
-    L.K = w_is_nk ? c : r;
-    L.N = w_is_nk ? r : c;
-    if (K_expect && L.K != K_expect) return -1;
-    L.w.resize((size_t)L.N * L.K);
-    for (int i = 0; i < r; ++i)
-      for (int j = 0; j < c; ++j) {
-        const float x = w->f[(size_t)i * c + j];
-        if (w_is_nk) L.w[(size_t)i * c + j] = x;
-        else L.w[(size_t)j * r + i] = x;
-      }
-    lins.push_back(std::move(L));
-    return (int)lins.size() - 1;
   }
   bool bias_of(const OTensor* t, int lin) {
     if (!t || t->is_int || (int)t->count() != lins[lin].N) return false;
@@ -206,67 +144,79 @@ struct TextLowerer {
   }
 
   int node(ONode& n);
-  int finish_ln(ONode& n, const TV& norm_src, const std::vector<float>& gamma, const std::vector<float>& beta, float eps);
+  int lower_match(const Match& m);
+  int finish_ln(const ONode& n, const TV& x, const Match& m);
   int run();
 };
 
 static bool is_int64min(int64_t v) { return v == INT64_MIN; }
 
-int TextLowerer::finish_ln(ONode& n, const TV& x, const std::vector<float>& gamma, const std::vector<float>& beta, float eps) {
-  LN ln{gamma, beta, eps};
-  if (gamma.size() != beta.size() || (x.kind != tEmb && (int)gamma.size() != p.H))
-    TFAIL(n, "LayerNorm affine of %zu / %zu for hidden %d", gamma.size(), beta.size(), p.H);
+int TextLowerer::finish_ln(const ONode& n, const TV& x, const Match& m) {
+  if (m.axis != -1 && m.axis != 2) LOWER_FAIL(n, "normalises an axis other than the last");
+  const size_t w = m.gamma ? m.gamma->count() : (size_t)p.H;
+  LN ln{m.gamma ? m.gamma->f : std::vector<float>(w, 1.f), m.beta ? m.beta->f : std::vector<float>(w, 0.f), m.eps};
+  if (ln.g.size() != ln.b.size() || (x.kind != tEmb && (int)ln.g.size() != p.H))
+    LOWER_FAIL(n, "LayerNorm affine of %zu / %zu for hidden %d", ln.g.size(), ln.b.size(), p.H);
   TV h;
   h.kind = tHid;
   if (x.kind == tEmb) {
-    if (stage != 0 || !x.word || !x.posr) TFAIL(n, "embedding LayerNorm without word and position rows");
-    if (p.H == 0) p.H = (int)gamma.size();
-    if ((int)gamma.size() != p.H) TFAIL(n, "LayerNorm of %zu on hidden %d", gamma.size(), p.H);
+    if (stage != 0 || !x.word || !x.posr) LOWER_FAIL(n, "embedding LayerNorm without word and position rows");
+    if (p.H == 0) p.H = (int)ln.g.size();
+    if ((int)ln.g.size() != p.H) LOWER_FAIL(n, "LayerNorm of %zu on hidden %d", ln.g.size(), p.H);
     if (p.type_row.empty()) p.type_row.assign((size_t)p.H, 0.f);
     p.emb_ln = ln;
     stage = 1;
   } else if (x.kind == tRes) {
     const TV& l = x;  // tRes carries the linear and what it read
     if (l.src == tCtxFlat) {
-      if (stage != 1 || cur.qkv.N == 0) TFAIL(n, "attention output LayerNorm out of order");
+      if (stage != 1 || cur.qkv.N == 0) LOWER_FAIL(n, "attention output LayerNorm out of order");
       cur.o = lins[l.lin];
       cur.ln1 = ln;
       stage = 2;
     } else if (l.src == tGelu) {
-      if (stage != 2 || cur.f1.N == 0) TFAIL(n, "FFN LayerNorm out of order");
+      if (stage != 2 || cur.f1.N == 0) LOWER_FAIL(n, "FFN LayerNorm out of order");
       cur.f2 = lins[l.lin];
       cur.ln2 = ln;
       p.layers.push_back(std::move(cur));
       cur = text::Layer();
       stage = 1;
     } else {
-      TFAIL(n, "residual LayerNorm after an unexpected linear");
+      LOWER_FAIL(n, "residual LayerNorm after an unexpected linear");
     }
   } else {
-    TFAIL(n, "LayerNorm of a value that is neither the embedding sum nor a residual sum");
+    LOWER_FAIL(n, "LayerNorm of a value that is neither the embedding sum nor a residual sum");
   }
-  vals[n.out[0]] = h;
+  vals[m.out] = h;
+  return AM_OK;
+}
+
+// a LayerNorm, GELU or F.normalize: lowered where the model has one, rejected anywhere else
+int TextLowerer::lower_match(const Match& m) {
+  const ONode& n = g.nodes[(size_t)m.nodes[0]];
+  const TV* x = val(m.in);
+  if (!x) LOWER_FAIL(n, "input '%s' is not produced by a supported node", m.in.c_str());
+  if (m.kind == Match::kLayerNorm) return finish_ln(n, *x, m);
+  if (m.kind == Match::kGelu) {
+    if (x->kind != tLin || x->src != tHid || stage != 2) LOWER_FAIL(n, "GELU of a value other than the FFN's up projection");
+    TV v = *x;
+    v.kind = tGelu;
+    vals[m.out] = v;
+    return AM_OK;
+  }
+  if (x->kind != tLin || x->src != tP1) LOWER_FAIL(n, "L2 normalise of a value other than the projection");
+  if (m.axis != -1 && m.axis != 1) LOWER_FAIL(n, "norm over an axis other than the last");
+  if (!m.clamp || m.eps <= 0 || m.eps > 1e-6) LOWER_FAIL(n, "norm clamp other than F.normalize's");
+  p.p2 = lins[x->lin];
+  p.normalize = true;
+  TV v;
+  v.kind = tOut;
+  vals[m.out] = v;
   return AM_OK;
 }
 
 int TextLowerer::node(ONode& n) {
   const std::string& op = n.op;
-  if (n.out.empty()) TFAIL(n, "no output");
-  if (op == "Constant") {
-    auto it = n.attrs.find("value");
-    if (it == n.attrs.end() || !it->second.has_t) {
-      auto f = n.attrs.find("value_float");
-      auto i = n.attrs.find("value_int");
-      OTensor t;
-      if (f != n.attrs.end()) t.f = {f->second.f};
-      else if (i != n.attrs.end()) { t.is_int = true; t.i = {i->second.i}; }
-      else TFAIL(n, "Constant without a tensor value");
-      consts[n.out[0]] = t;
-      return AM_OK;
-    }
-    consts[n.out[0]] = it->second.t;
-    return AM_OK;
-  }
+  if (n.out.empty()) LOWER_FAIL(n, "no output");
   // inputs: constants, or values with a kind
   std::vector<const TV*> in(n.in.size(), nullptr);
   bool all_const = true, shape_or_const = true, mask_like = true;
@@ -274,7 +224,7 @@ int TextLowerer::node(ONode& n) {
     if (n.in[i].empty() || cst(n.in[i])) continue;
     all_const = false;
     in[i] = val(n.in[i]);
-    if (!in[i]) TFAIL(n, "input '%s' is not produced by a supported node", n.in[i].c_str());
+    if (!in[i]) LOWER_FAIL(n, "input '%s' is not produced by a supported node", n.in[i].c_str());
     if (in[i]->kind != tShape) shape_or_const = false;
     if (in[i]->kind != tShape && in[i]->kind != tMask) mask_like = false;
   }
@@ -284,14 +234,14 @@ int TextLowerer::node(ONode& n) {
                                                   "ConstantOfShape", "Mul", "Add", "Sub", "Div", "Equal", "Where",
                                                   "Cast", "Slice", "Range", "Expand", "Not", "Identity"};
 
-  if (all_const && op != "Shape") TFAIL(n, "operator on constants only (not folded at export)");
+  if (all_const && op != "Shape") LOWER_FAIL(n, "operator on constants only (not folded at export)");
   if (op == "Shape") {
     TV v;
     v.kind = tShape;
     return out(v);
   }
   if (shape_or_const) {
-    if (!kShapeOps.count(op)) TFAIL(n, "operator not supported in shape arithmetic");
+    if (!kShapeOps.count(op)) LOWER_FAIL(n, "operator not supported in shape arithmetic");
     TV v;
     v.kind = tShape;
     if (op == "Concat") {
@@ -310,7 +260,7 @@ int TextLowerer::node(ONode& n) {
   if (mask_like && (kind(0) == tMask || kind(1) == tMask || kind(2) == tMask)) {
     static const std::set<std::string> kMaskOps = {"Unsqueeze", "Cast", "Sub", "Mul", "Where", "Expand", "Equal", "Not",
                                                    "Reshape", "Identity", "Slice", "Squeeze"};
-    if (!kMaskOps.count(op)) TFAIL(n, "operator not supported in the attention-mask construction");
+    if (!kMaskOps.count(op)) LOWER_FAIL(n, "operator not supported in the attention-mask construction");
     if (op == "Where") mask_kind = 2;
     if (op == "Mul" && mask_kind == 0) mask_kind = 1;
     TV v;
@@ -326,19 +276,19 @@ int TextLowerer::node(ONode& n) {
     }
   }
   if (op == "Identity" || op == "Dropout") {
-    if (!in[0]) TFAIL(n, "identity of a constant");
+    if (!in[0]) LOWER_FAIL(n, "identity of a constant");
     return out(*in[0]);
   }
   if (op == "Cast") {
     const int k = kind(0);
     if (k == tPosNe || k == tPosMul || k == tPos || k == tPosCum) return out(*in[0]);
-    TFAIL(n, "Cast of an unsupported value");
+    LOWER_FAIL(n, "Cast of an unsupported value");
   }
 
   // ---------------------------------------------------------------- position ids
   if (op == "Equal" && kind(0) == tIds) {
     double c;
-    if (!scalar(cin(n, 1), &c)) TFAIL(n, "input_ids compared with a non-constant");
+    if (!scalar_of(n, 1, &c)) LOWER_FAIL(n, "input_ids compared with a non-constant");
     TV v;
     v.kind = tPosEq;
     v.pad = (int64_t)c;
@@ -351,7 +301,7 @@ int TextLowerer::node(ONode& n) {
   }
   if (op == "CumSum" && kind(0) == tPosNe) {
     double ax;
-    if (!scalar(cin(n, 1), &ax) || (ax != 1 && ax != -1)) TFAIL(n, "cumulative sum over an axis other than the sequence");
+    if (!scalar_of(n, 1, &ax) || (ax != 1 && ax != -1)) LOWER_FAIL(n, "cumulative sum over an axis other than the sequence");
     TV v = *in[0];
     v.kind = tPosCum;
     return out(v);
@@ -364,8 +314,8 @@ int TextLowerer::node(ONode& n) {
   if (op == "Add" && (kind(0) == tPosMul || kind(1) == tPosMul)) {
     double c;
     const TV& a = *(kind(0) == tPosMul ? in[0] : in[1]);
-    if (!scalar(cin(n, kind(0) == tPosMul ? 1 : 0), &c) || (int64_t)c != a.pad)
-      TFAIL(n, "position ids offset by something other than the padding id %lld", (long long)a.pad);
+    if (!scalar_of(n, kind(0) == tPosMul ? 1 : 0, &c) || (int64_t)c != a.pad)
+      LOWER_FAIL(n, "position ids offset by something other than the padding id %lld", (long long)a.pad);
     TV v = a;
     v.kind = tPos;
     return out(v);
@@ -379,14 +329,14 @@ int TextLowerer::node(ONode& n) {
       TV v;
       v.kind = tEmb;
       if (kind(1) == tIds) {
-        if (!p.word.empty()) TFAIL(n, "a second word-embedding gather");
+        if (!p.word.empty()) LOWER_FAIL(n, "a second word-embedding gather");
         p.vocab = (int)tab->dims[0];
         p.H = (int)tab->dims[1];
         p.word = tab->f;
         v.word = true;
       } else if (kind(1) == tPos) {
-        if (!p.pos.empty()) TFAIL(n, "a second position-embedding gather");
-        if (p.H && tab->dims[1] != p.H) TFAIL(n, "position table width %lld, hidden %d", (long long)tab->dims[1], p.H);
+        if (!p.pos.empty()) LOWER_FAIL(n, "a second position-embedding gather");
+        if (p.H && tab->dims[1] != p.H) LOWER_FAIL(n, "position table width %lld, hidden %d", (long long)tab->dims[1], p.H);
         p.max_pos = (int)tab->dims[0];
         p.pad_id = (int)in[1]->pad;
         p.pos = tab->f;
@@ -395,18 +345,18 @@ int TextLowerer::node(ONode& n) {
         p.type_row = tab->f;
         v.type = true;
       } else {
-        TFAIL(n, "gather from a table by an index that is neither input_ids nor the position ids");
+        LOWER_FAIL(n, "gather from a table by an index that is neither input_ids nor the position ids");
       }
       return out(v);
     }
     if (kind(0) == tHid && axis == 1) {
       double c;
-      if (!scalar(cin(n, 1), &c) || c != 0) TFAIL(n, "pooler reads a token other than the first");
+      if (!scalar_of(n, 1, &c) || c != 0) LOWER_FAIL(n, "pooler reads a token other than the first");
       TV v;
       v.kind = tTok0;
       return out(v);
     }
-    TFAIL(n, "unsupported gather");
+    LOWER_FAIL(n, "unsupported gather");
   }
   if (op == "Add" && (kind(0) == tEmb || kind(1) == tEmb)) {
     TV v;
@@ -417,119 +367,44 @@ int TextLowerer::node(ONode& n) {
         v.posr |= in[i]->posr;
         v.type |= in[i]->type;
       } else if (const OTensor* t = cin(n, i)) {  // the constant-folded token-type row
-        if (p.H == 0 || (int)t->count() != p.H || v.type) TFAIL(n, "embedding sum plus a constant of %zu values", t->count());
+        if (p.H == 0 || (int)t->count() != p.H || v.type) LOWER_FAIL(n, "embedding sum plus a constant of %zu values", t->count());
         p.type_row = t->f;
         v.type = true;
       } else {
-        TFAIL(n, "embedding sum plus an unsupported value");
+        LOWER_FAIL(n, "embedding sum plus an unsupported value");
       }
     }
     return out(v);
-  }
-
-  // ---------------------------------------------------------------- LayerNorm (op, or decomposed)
-  if (op == "LayerNormalization" && (kind(0) == tEmb || kind(0) == tRes)) {
-    const OTensor *ga = cin(n, 1), *be = cin(n, 2);
-    if (!ga || !be) TFAIL(n, "non-constant affine");
-    if (attr_i(n, "axis", -1) != -1 && attr_i(n, "axis", -1) != 2) TFAIL(n, "normalises an axis other than the last");
-    auto it = n.attrs.find("epsilon");
-    return finish_ln(n, *in[0], ga->f, be->f, it != n.attrs.end() && it->second.has_f ? it->second.f : 1e-5f);
-  }
-  if (op == "ReduceMean" && (kind(0) == tEmb || kind(0) == tRes)) {
-    if (!axes_last(n, 3) || attr_i(n, "keepdims", 1) != 1) TFAIL(n, "mean over an axis other than the last");
-    ln_inputs.push_back(*in[0]);
-    TV v;
-    v.kind = tLnMean;
-    v.ln_in = (int)ln_inputs.size() - 1;
-    vals[n.in[0]].ln_in = v.ln_in;  // the Sub that follows pairs the input with its mean
-    return out(v);
-  }
-  if (op == "Sub" && kind(1) == tLnMean && in[0] && in[0]->ln_in == in[1]->ln_in) {
-    TV v;
-    v.kind = tLnD;
-    v.ln_in = in[1]->ln_in;
-    return out(v);
-  }
-  if ((op == "Mul" && kind(0) == tLnD && n.in[0] == n.in[1]) || (op == "Pow" && kind(0) == tLnD)) {
-    double e = 2;
-    if (op == "Pow" && (!scalar(cin(n, 1), &e) || e != 2)) TFAIL(n, "power other than 2 in a LayerNorm");
-    TV v = *in[0];
-    v.kind = tLnSq;
-    return out(v);
-  }
-  if (op == "ReduceMean" && kind(0) == tLnSq) {
-    if (!axes_last(n, 3)) TFAIL(n, "variance over an axis other than the last");
-    TV v = *in[0];
-    v.kind = tLnVar;
-    return out(v);
-  }
-  if (op == "Add" && (kind(0) == tLnVar || kind(1) == tLnVar)) {
-    double e;
-    if (!scalar(cin(n, kind(0) == tLnVar ? 1 : 0), &e)) TFAIL(n, "non-constant LayerNorm eps");
-    TV v = *in[kind(0) == tLnVar ? 0 : 1];
-    v.kind = tLnVarE;
-    v.eps = (float)e;
-    return out(v);
-  }
-  if (op == "Sqrt" && kind(0) == tLnVarE) {
-    TV v = *in[0];
-    v.kind = tLnStd;
-    return out(v);
-  }
-  if (op == "Div" && kind(0) == tLnD && kind(1) == tLnStd && in[0]->ln_in == in[1]->ln_in) {
-    TV v = *in[1];
-    v.kind = tLnNorm;
-    return out(v);
-  }
-  if (op == "Mul" && (kind(0) == tLnNorm || kind(1) == tLnNorm)) {
-    const OTensor* ga = cin(n, kind(0) == tLnNorm ? 1 : 0);
-    if (!ga || ga->is_int) TFAIL(n, "non-constant LayerNorm scale");
-    TV v = *in[kind(0) == tLnNorm ? 0 : 1];
-    v.kind = tLnScaled;
-    v.gamma = ga->f;
-    return out(v);
-  }
-  if (op == "Add" && (kind(0) == tLnScaled || kind(1) == tLnScaled)) {
-    const OTensor* be = cin(n, kind(0) == tLnScaled ? 1 : 0);
-    if (!be || be->is_int) TFAIL(n, "non-constant LayerNorm shift");
-    const TV& s = *in[kind(0) == tLnScaled ? 0 : 1];
-    return finish_ln(n, ln_inputs[(size_t)s.ln_in], s.gamma, be->f, s.eps);
   }
 
   // ---------------------------------------------------------------- linears
   if (op == "MatMul" || op == "Gemm") {
     const int k0 = kind(0);
     if (k0 == tHid || k0 == tCtxFlat || k0 == tGelu || k0 == tTok0 || k0 == tPooled || k0 == tP1) {
-      bool nk = false;
-      if (op == "Gemm") {
-        if (attr_i(n, "transA", 0)) TFAIL(n, "transposed activation");
-        float alpha = 1.f, beta = 1.f;
-        if (n.attrs.count("alpha")) alpha = n.attrs["alpha"].f;
-        if (n.attrs.count("beta")) beta = n.attrs["beta"].f;
-        if (alpha != 1.f || beta != 1.f) TFAIL(n, "alpha %g beta %g", alpha, beta);
-        nk = attr_i(n, "transB", 0) != 0;
-      }
       if (k0 == tGelu) {  // the FFN's down projection: the linear that fed GELU was its up projection
-        if (stage != 2 || cur.f1.N) TFAIL(n, "FFN out of order");
+        if (stage != 2 || cur.f1.N) LOWER_FAIL(n, "FFN out of order");
         cur.f1 = lins[in[0]->lin];
         p.ffn = cur.f1.N;
       }
       const int K = k0 == tGelu ? p.ffn : (k0 == tP1 ? 0 : p.H);
-      const int li = new_linear(n, cin(n, 1), nk, K);
-      if (li < 0) TFAIL(n, "weight must be a constant [%d, N] matrix", K);
+      Linear L;
+      AM_TRY(linear_weight(n, &L.K, &L.N, &L.w));
+      if (K && L.K != K) LOWER_FAIL(n, "weight must be a constant [%d, N] matrix", K);
+      lins.push_back(std::move(L));
+      const int li = (int)lins.size() - 1;
       TV v;
       v.kind = tLin;
       v.lin = li;
       v.src = k0;
       if (op == "Gemm" && n.in.size() > 2 && !n.in[2].empty()) {
-        if (!bias_of(cin(n, 2), li)) TFAIL(n, "non-constant or mis-sized bias");
+        if (!bias_of(cin(n, 2), li)) LOWER_FAIL(n, "non-constant or mis-sized bias");
         v.has_bias = true;
       }
       return out(v);
     }
     if (op == "MatMul" && kind(0) == tHeads && kind(1) == tHeads) {
       const TV &q = *in[0], &k = *in[1];
-      if (q.state != 1 || k.state != 2) TFAIL(n, "scores need Q as [B, heads, T, dh] and K as [B, heads, dh, T]");
+      if (q.state != 1 || k.state != 2) LOWER_FAIL(n, "scores need Q as [B, heads, T, dh] and K as [B, heads, dh, T]");
       TV v;
       v.kind = tScores;
       v.q = q.lin;
@@ -541,24 +416,24 @@ int TextLowerer::node(ONode& n) {
       return out(v);
     }
     if (op == "MatMul" && kind(0) == tProbs && kind(1) == tHeads) {
-      if (in[1]->state != 1) TFAIL(n, "V must be [B, heads, T, dh]");
+      if (in[1]->state != 1) LOWER_FAIL(n, "V must be [B, heads, T, dh]");
       TV v = *in[0];
       v.kind = tCtx;
       v.v = in[1]->lin;
       return out(v);
     }
-    TFAIL(n, "matrix product of unsupported operands");
+    LOWER_FAIL(n, "matrix product of unsupported operands");
   }
   if (op == "Add" && (kind(0) == tLin || kind(1) == tLin) && (cin(n, 0) || cin(n, 1))) {
     TV v = *in[kind(0) == tLin ? 0 : 1];
-    if (v.has_bias) TFAIL(n, "second bias on a linear");
-    if (!bias_of(cin(n, kind(0) == tLin ? 1 : 0), v.lin)) TFAIL(n, "bias does not match the linear's %d outputs", lins[v.lin].N);
+    if (v.has_bias) LOWER_FAIL(n, "second bias on a linear");
+    if (!bias_of(cin(n, kind(0) == tLin ? 1 : 0), v.lin)) LOWER_FAIL(n, "bias does not match the linear's %d outputs", lins[v.lin].N);
     v.has_bias = true;
     return out(v);
   }
   if (op == "Add" && ((kind(0) == tLin && kind(1) == tHid) || (kind(0) == tHid && kind(1) == tLin))) {
     TV v = *in[kind(0) == tLin ? 0 : 1];
-    if (v.src != tCtxFlat && v.src != tGelu) TFAIL(n, "residual added to an unexpected linear");
+    if (v.src != tCtxFlat && v.src != tGelu) LOWER_FAIL(n, "residual added to an unexpected linear");
     v.kind = tRes;
     return out(v);
   }
@@ -572,12 +447,12 @@ int TextLowerer::node(ONode& n) {
     } else if (s && s->kind == tShape) {
       shp = s->known;
     }
-    if (shp.size() != 4 || is_int64min(shp[2]) || is_int64min(shp[3])) TFAIL(n, "split into heads needs a constant [.., heads, dh] tail");
+    if (shp.size() != 4 || is_int64min(shp[2]) || is_int64min(shp[3])) LOWER_FAIL(n, "split into heads needs a constant [.., heads, dh] tail");
     int64_t nh = shp[2], dh = shp[3];
     const int N = lins[in[0]->lin].N;
     if (nh == -1 && dh > 0) nh = N / dh;
     if (dh == -1 && nh > 0) dh = N / nh;
-    if (nh <= 0 || dh <= 0 || nh * dh != N) TFAIL(n, "%lld heads of %lld for %d features", (long long)nh, (long long)dh, N);
+    if (nh <= 0 || dh <= 0 || nh * dh != N) LOWER_FAIL(n, "%lld heads of %lld for %d features", (long long)nh, (long long)dh, N);
     TV v = *in[0];
     v.kind = tHeads;
     v.state = 0;
@@ -589,34 +464,34 @@ int TextLowerer::node(ONode& n) {
     const std::vector<int64_t> perm = attr_ints(n, "perm");
     TV v = *in[0];
     if (v.kind == tCtx) {
-      if (perm != std::vector<int64_t>{0, 2, 1, 3}) TFAIL(n, "context transposed other than back to [B, T, heads, dh]");
+      if (perm != std::vector<int64_t>{0, 2, 1, 3}) LOWER_FAIL(n, "context transposed other than back to [B, T, heads, dh]");
       v.kind = tCtxT;
       return out(v);
     }
     if (v.state == 0 && perm == std::vector<int64_t>{0, 2, 1, 3}) v.state = 1;
     else if (v.state == 0 && perm == std::vector<int64_t>{0, 2, 3, 1}) v.state = 2;
     else if (v.state == 1 && perm == std::vector<int64_t>{0, 1, 3, 2}) v.state = 2;
-    else TFAIL(n, "unsupported head transpose");
+    else LOWER_FAIL(n, "unsupported head transpose");
     return out(v);
   }
   if ((op == "Mul" || op == "Div") && (kind(0) == tHeads || kind(0) == tScores)) {
     double c;
-    if (!scalar(cin(n, 1), &c) || c == 0) TFAIL(n, "scaled by a non-constant");
+    if (!scalar_of(n, 1, &c) || c == 0) LOWER_FAIL(n, "scaled by a non-constant");
     TV v = *in[0];
-    if (v.kind == tScores && v.masked) TFAIL(n, "scale after the mask");
+    if (v.kind == tScores && v.masked) LOWER_FAIL(n, "scale after the mask");
     v.scale *= op == "Mul" ? c : 1.0 / c;
     return out(v);
   }
   if (op == "Add" && ((kind(0) == tScores && kind(1) == tMask) || (kind(0) == tMask && kind(1) == tScores))) {
     TV v = *in[kind(0) == tScores ? 0 : 1];
-    if (v.masked) TFAIL(n, "second mask");
+    if (v.masked) LOWER_FAIL(n, "second mask");
     v.masked = true;
     return out(v);
   }
   if (op == "Softmax" && kind(0) == tScores) {
     const int64_t ax = attr_i(n, "axis", -1);
-    if (ax != -1 && ax != 3) TFAIL(n, "softmax over axis %lld", (long long)ax);
-    if (!in[0]->masked) TFAIL(n, "scores without the attention mask");
+    if (ax != -1 && ax != 3) LOWER_FAIL(n, "softmax over axis %lld", (long long)ax);
+    if (!in[0]->masked) LOWER_FAIL(n, "scores without the attention mask");
     TV v = *in[0];
     v.kind = tProbs;
     return out(v);
@@ -627,12 +502,12 @@ int TextLowerer::node(ONode& n) {
     std::vector<int64_t> shp;
     if (const OTensor* t = cin(n, 1)) for (size_t q = 0; q < t->count(); ++q) shp.push_back((int64_t)t->at(q));
     else if (in[1] && in[1]->kind == tShape) shp = in[1]->known;
-    if (shp.size() != 3 || (shp[2] != Hh && shp[2] != -1)) TFAIL(n, "context not merged back to [B, T, %d]", Hh);
+    if (shp.size() != 3 || (shp[2] != Hh && shp[2] != -1)) LOWER_FAIL(n, "context not merged back to [B, T, %d]", Hh);
     // the layer's Q, K, V: one fused linear [3H, H]
-    if (stage != 1 || cur.qkv.N) TFAIL(n, "attention out of order");
+    if (stage != 1 || cur.qkv.N) LOWER_FAIL(n, "attention out of order");
     const Linear &q = lins[v.q], &k = lins[v.k], &vv = lins[v.v];
-    if (q.N != p.H || k.N != p.H || vv.N != p.H) TFAIL(n, "Q / K / V widths %d / %d / %d for hidden %d", q.N, k.N, vv.N, p.H);
-    if (p.heads && (p.heads != v.nh || p.dh != v.dh)) TFAIL(n, "%d heads of %d after %d of %d", v.nh, v.dh, p.heads, p.dh);
+    if (q.N != p.H || k.N != p.H || vv.N != p.H) LOWER_FAIL(n, "Q / K / V widths %d / %d / %d for hidden %d", q.N, k.N, vv.N, p.H);
+    if (p.heads && (p.heads != v.nh || p.dh != v.dh)) LOWER_FAIL(n, "%d heads of %d after %d of %d", v.nh, v.dh, p.heads, p.dh);
     p.heads = v.nh;
     p.dh = v.dh;
     Linear f;
@@ -651,48 +526,9 @@ int TextLowerer::node(ONode& n) {
     return out(v);
   }
 
-  // ---------------------------------------------------------------- Erf-GELU of the FFN's up projection
-  auto gelu_part = [&](int i) { return kind(i) == tLin || (kind(i) >= tGHalf && kind(i) <= tGelu); };
-  if (gelu_part(0) || gelu_part(1)) {
-    const int li = gelu_part(0) ? 0 : 1;
-    const TV& a = *in[li];
-    double c = 0;
-    const bool has_c = scalar(cin(n, 1 - li), &c);
-    auto g = [&](int k) {
-      TV v = a;
-      v.kind = k;
-      return out(v);
-    };
-    if (a.kind == tLin && a.src == tHid && stage == 2) {
-      if (op == "Mul" && has_c && c == 0.5) return g(tGHalf);
-      if (op == "Div" && li == 0 && has_c && std::fabs(c - std::sqrt(2.0)) < 1e-6) return g(tGDiv);
-      if (op == "Mul" && has_c && std::fabs(c - std::sqrt(0.5)) < 1e-6) return g(tGDiv);
-    }
-    if (op == "Erf" && a.kind == tGDiv) return g(tGErf);
-    if (op == "Add" && a.kind == tGErf && has_c && c == 1.0) return g(tGOne);
-    if (op == "Mul" && !has_c && in[0] && in[1]) {
-      const TV *x = in[0], *y = in[1];
-      if (x->kind == tGOne) std::swap(x, y);
-      if (y->kind == tGOne && x->lin == y->lin) {
-        if (x->kind == tGHalf) return g(tGelu);
-        if (x->kind == tLin) return g(tGProd);
-      }
-    }
-    if (op == "Mul" && a.kind == tGProd && has_c && c == 0.5) return g(tGelu);
-    if (a.kind == tGelu || a.kind == tGProd || a.kind == tGOne || a.kind == tGErf || a.kind == tGDiv || a.kind == tGHalf)
-      TFAIL(n, "not part of an Erf-GELU");
-  }
-  if (op == "Gelu" && kind(0) == tLin && in[0]->src == tHid && stage == 2) {
-    auto it = n.attrs.find("approximate");
-    if (it != n.attrs.end() && it->second.s != "none") TFAIL(n, "tanh-approximated GELU");
-    TV v = *in[0];
-    v.kind = tGelu;
-    return out(v);
-  }
-
   // ---------------------------------------------------------------- pooler, projection, normalise
   if (op == "Tanh" && kind(0) == tLin && in[0]->src == tTok0) {
-    if (!in[0]->has_bias) TFAIL(n, "pooler without a bias");
+    if (!in[0]->has_bias) LOWER_FAIL(n, "pooler without a bias");
     p.pool = lins[in[0]->lin];
     TV v;
     v.kind = tPooled;
@@ -704,34 +540,7 @@ int TextLowerer::node(ONode& n) {
     v.kind = tP1;
     return out(v);
   }
-  if (op == "ReduceL2" && kind(0) == tLin && in[0]->src == tP1) {
-    if (!axes_last(n, 2) || attr_i(n, "keepdims", 1) != 1) TFAIL(n, "norm over an axis other than the last");
-    p.p2 = lins[in[0]->lin];
-    TV v;
-    v.kind = tL2;
-    vals[n.in[0]].kind = tOutPre;
-    return out(v);
-  }
-  if (op == "Clip" && kind(0) == tL2) {
-    double lo;
-    if (!scalar(cin(n, 1), &lo) || lo <= 0 || lo > 1e-6) TFAIL(n, "norm clamp other than F.normalize's");
-    TV v;
-    v.kind = tL2Clip;
-    return out(v);
-  }
-  if (op == "Max" && kind(0) == tL2) {
-    TV v;
-    v.kind = tL2Clip;
-    return out(v);
-  }
-  if (op == "Expand" && kind(0) == tL2Clip) return out(*in[0]);
-  if (op == "Div" && kind(0) == tOutPre && kind(1) == tL2Clip) {
-    p.normalize = true;
-    TV v;
-    v.kind = tOut;
-    return out(v);
-  }
-  TFAIL(n, "operator not supported here");
+  LOWER_FAIL(n, "operator not supported here");
 }
 
 int TextLowerer::run() {
@@ -749,7 +558,17 @@ int TextLowerer::run() {
     }
     vals[s] = v;
   }
-  for (ONode& n : g.nodes) AM_TRY(node(n));
+  AM_TRY(build());
+  for (size_t i = 0; i < g.nodes.size(); ++i) {
+    ONode& n = g.nodes[i];
+    if (n.done || n.op == "Constant") continue;  // Constant nodes are registered by the index
+    if (const Match* m = match_starting(i)) {
+      AM_TRY(lower_match(*m));
+      for (int q : m->nodes) g.nodes[(size_t)q].done = true;
+    } else {
+      AM_TRY(node(n));
+    }
+  }
   if (g.outputs.size() != 1 || !val(g.outputs[0]) || val(g.outputs[0])->kind != tOut) {
     set_error("onnx: the graph's output is not an L2-normalised projection of the pooled hidden state");
     return AM_ERR_INVALID;

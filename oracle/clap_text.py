@@ -16,6 +16,7 @@ utilities do not trace, so this module restates the model with plain tensor oper
   ``"where"`` is transformers' ``masked_fill`` form (``Expand/Cast/Sub/Where``);
 * ``layernorm_op=True`` and ``gelu="F"`` use ``nn.LayerNorm`` and ``F.gelu``, as ``RobertaModel`` does (the exporter
   writes one ``LayerNormalization`` op, and ``Div/Erf/Add/Mul/Mul``); the defaults write both out by hand;
+* ``ln_affine=False`` drops every LayerNorm's scale and shift, so the decomposed form ends at its ``Div``;
 * the position ids are RoBERTa's ``cumsum(ids != pad) * (ids != pad) + pad``; the token-type embedding is row 0 of
   its table, added as a constant (what constant folding leaves of it).
 
@@ -56,17 +57,19 @@ def small_config(**kw) -> TextConfig:
 
 
 class _LN(nn.Module):
-    def __init__(self, n, eps):
+    def __init__(self, n, eps, affine=True):
         super().__init__()
-        self.weight = nn.Parameter(torch.ones(n))
-        self.bias = nn.Parameter(torch.zeros(n))
-        self.eps = eps
+        if affine:
+            self.weight = nn.Parameter(torch.ones(n))
+            self.bias = nn.Parameter(torch.zeros(n))
+        self.eps, self.affine = eps, affine
 
     def forward(self, x):  # decomposed, as the exporter writes LayerNorm at opset 17 when it is not fused
         mu = x.mean(-1, keepdim=True)
         d = x - mu
         var = (d * d).mean(-1, keepdim=True)
-        return d / torch.sqrt(var + self.eps) * self.weight + self.bias
+        y = d / torch.sqrt(var + self.eps)
+        return y * self.weight + self.bias if self.affine else y
 
 
 class _Lin(nn.Module):
@@ -88,13 +91,14 @@ def _ns(**kw):
 
 class TextCLAP(nn.Module):
     def __init__(self, cfg: TextConfig, attention: str = "eager", mask: str = "arith", layernorm_op: bool = False,
-                 gelu: str = "erf"):
+                 gelu: str = "erf", ln_affine: bool = True):
         super().__init__()
         assert attention in ("eager", "sdpa") and mask in ("arith", "where") and gelu in ("erf", "F")
+        assert ln_affine or not layernorm_op
         self.cfg, self.attention, self.mask_form, self.layernorm_op = cfg, attention, mask, layernorm_op
-        self.gelu = gelu
+        self.gelu, self.ln_affine = gelu, ln_affine
         H = cfg.hidden
-        ln = (lambda: nn.LayerNorm(H, eps=cfg.eps)) if layernorm_op else (lambda: _LN(H, cfg.eps))
+        ln = (lambda: nn.LayerNorm(H, eps=cfg.eps)) if layernorm_op else (lambda: _LN(H, cfg.eps, ln_affine))
         emb = _ns(word_embeddings=nn.Embedding(cfg.vocab, H, padding_idx=cfg.pad_id),
                   position_embeddings=nn.Embedding(cfg.max_pos, H, padding_idx=cfg.pad_id),
                   token_type_embeddings=nn.Embedding(cfg.type_vocab, H), LayerNorm=ln())
@@ -182,7 +186,7 @@ def export_onnx_bytes(model: TextCLAP, B: int = 1, T: int = 77) -> bytes:
     with tempfile.TemporaryDirectory() as d:
         src, dst = os.path.join(d, "model.pt"), os.path.join(d, "model.onnx")
         torch.save({"cfg": dict(model.cfg.__dict__), "attention": model.attention, "mask": model.mask_form,
-                    "layernorm_op": model.layernorm_op, "gelu": model.gelu,
+                    "layernorm_op": model.layernorm_op, "gelu": model.gelu, "ln_affine": model.ln_affine,
                     "state": {k: v.float() for k, v in model.state_dict().items()}}, src)
         subprocess.run([sys.executable, "-m", "oracle.clap_text", src, dst, str(B), str(T)], cwd=root, check=True)
         with open(dst, "rb") as f:
@@ -230,7 +234,8 @@ if __name__ == "__main__":  # python -m oracle.clap_text <saved model> <out.onnx
     import sys
 
     blob = torch.load(sys.argv[1])
-    m = TextCLAP(TextConfig(**blob["cfg"]), blob["attention"], blob["mask"], blob["layernorm_op"], blob["gelu"]).float()
+    m = TextCLAP(TextConfig(**blob["cfg"]), blob["attention"], blob["mask"], blob["layernorm_op"], blob["gelu"],
+                 blob["ln_affine"]).float()
     m.load_state_dict(blob["state"])
     with open(sys.argv[2], "wb") as f:
         f.write(_export_in_process(m, int(sys.argv[3]), int(sys.argv[4])))

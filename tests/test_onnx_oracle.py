@@ -2,6 +2,7 @@
 that produced the files -- the reference's own export check (student_onnx_model.py:640-650, max diff < 1e-5) --
 and the library's host-side loader / lowering (am_clap_describe_file needs no GPU)."""
 import ctypes as C
+import math
 import os
 
 import numpy as np
@@ -64,11 +65,33 @@ def test_interpreter_matches_torch_mobilenet_and_rewrites(small_mn, tmp_path):
     assert {"GlobalAveragePool", "HardSigmoid", "Gemm", "Relu"} <= ops  # a structurally different graph
 
 
+class _FunctionalHeadStudent(phinet.StudentCLAPAudio):
+    """The student with its projection head written out by hand, in the forms the exporter then writes: GELU as
+    (x * 0.5) * (1 + erf(x * sqrt(1/2))), LayerNorm with Mul(d, d) for the square, and F.normalize's clamp as Max."""
+
+    def forward(self, mel_spec):
+        feats = self.phinet(mel_spec.squeeze(1).transpose(1, 2))
+        h = self.projection_head
+        e1 = h.linear1(feats)
+        x = e1 + h.linear2(e1 * 0.5 * (1.0 + torch.erf(e1 * math.sqrt(0.5))))
+        d = x - x.mean(-1, keepdim=True)
+        ln = h.layer_norm
+        x = d / torch.sqrt((d * d).mean(-1, keepdim=True) + ln.eps) * ln.weight + ln.bias
+        return x / torch.maximum(x.norm(p=2, dim=1, keepdim=True), torch.tensor(1e-12))
+
+
 def test_loader_lowers_student_onnx_like_the_blob(small_student, tmp_path):
     """The graph-driven lowering of the exported student must arrive at the same layer program as the
-    hand-written state_dict exporter (weights.export_blob)."""
+    hand-written state_dict exporter (weights.export_blob), whether the head's GELU, LayerNorm and L2 normalise
+    come from modules or are written out by hand (_FunctionalHeadStudent)."""
     cfg, model = small_student
+    functional = _FunctionalHeadStudent(cfg)
+    functional.load_state_dict(model.state_dict())
     p_onnx = onnx_export.export_onnx(model, str(tmp_path / "s.onnx"))
+    p_fn = onnx_export.export_onnx(functional, str(tmp_path / "fn.onnx"))
+    with open(p_fn, "rb") as f:
+        data = f.read()
+    assert b"\x22\x03Max" in data and b"\x22\x03Pow" not in data and b"LayerNormalization" not in data
     wcfg = weights.StudentConfig(alpha=cfg.alpha, num_layers=cfg.num_layers, trunk_dim=cfg.trunk_dim)
     p_amw = tmp_path / "s.amw"
     p_amw.write_bytes(weights.export_blob(model.state_dict(), wcfg))
@@ -80,6 +103,7 @@ def test_loader_lowers_student_onnx_like_the_blob(small_student, tmp_path):
         import re
         return [re.sub(r"r-?\d+", "r", l) for l in strip(lines)]
 
+    assert norm(describe(p_fn).splitlines()) == norm(d_amw)
     assert norm(d_onnx) == norm(d_amw)
     assert "stem" in d_onnx[1] and "H=time" in d_onnx[1]
     assert sum("+residual" in l for l in d_onnx) == 3

@@ -120,12 +120,17 @@ def test_describe_lowers_every_attention_and_mask_form(small_files, attention, m
     _expect_program(describe(files[(attention, mask)]), cfg, attention, mask)
 
 
-@pytest.mark.parametrize("attention,mask", [("eager", "arith"), ("sdpa", "where")])
-def test_describe_layernorm_op_and_functional_gelu(tmp_path, attention, mask):
-    """nn.LayerNorm and F.gelu, as RobertaModel writes them: one LayerNormalization op and Div/Erf/Add/Mul/Mul."""
+@pytest.mark.parametrize("attention,mask,ln_op", [
+    pytest.param("eager", "arith", True, id="eager-arith"),
+    pytest.param("sdpa", "where", True, id="sdpa-where"),
+    pytest.param("eager", "where", False, id="eager-where-ln_without_affine")])
+def test_describe_layernorm_op_and_functional_gelu(tmp_path, attention, mask, ln_op):
+    """nn.LayerNorm and F.gelu, as RobertaModel writes them: one LayerNormalization op and Div/Erf/Add/Mul/Mul.  Without
+    ln_op, decomposed LayerNorms without scale and shift (their Div is the hidden state) and F.gelu."""
     cfg = ct.small_config()
-    data = ct.export_onnx_bytes(ct.TextCLAP(cfg, attention, mask, layernorm_op=True, gelu="F").init_random(4))
-    assert data.count(b"LayerNormalization") >= 2 * cfg.layers + 1
+    model = ct.TextCLAP(cfg, attention, mask, layernorm_op=ln_op, gelu="F", ln_affine=ln_op).init_random(4)
+    data = ct.export_onnx_bytes(model)
+    assert (data.count(b"LayerNormalization") >= 2 * cfg.layers + 1) == ln_op
     p = str(tmp_path / "ln_op.onnx")
     with open(p, "wb") as f:
         f.write(data)
