@@ -29,8 +29,10 @@ class B200OutOfMemory(B200Error, MemoryError):
 
 
 class MelCfg(C.Structure):
+    """am_mel_cfg; framing and log_mode default to 0, CLAP's mel"""
     _fields_ = [("sr", C.c_int), ("n_fft", C.c_int), ("hop", C.c_int), ("n_mels", C.c_int),
-                ("fmin", C.c_float), ("fmax", C.c_float), ("transpose", C.c_int)]
+                ("fmin", C.c_float), ("fmax", C.c_float), ("transpose", C.c_int), ("framing", C.c_int),
+                ("log_mode", C.c_int)]
 
 
 class SongPathCfg(C.Structure):
@@ -72,21 +74,12 @@ SIGNATURES = {
     "am_mel_plan_free": (None, [_vp]),
     "am_mel_filterbank": (_i, [_P(MelCfg), _vp]),
     "am_mel_num_frames": (_i, [_P(MelCfg), _i]),
-    "am_mel_batch": (_i, [_vp, _i, _i, _P(MelCfg), _vp]),
-    "am_mel_batch_i16": (_i, [_vp, _i, _i, _P(MelCfg), _vp]),
+    "am_mel_batch": (_i, [_vp, _i, _i, _i, _P(MelCfg), _vp]),
     "am_mel_batch_dev": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp]),
-    "am_mel_plan_create_ex": (_i, [_P(MelCfg), _i, _i, _P(_vp)]),
-    "am_mel_num_frames_ex": (_i, [_P(MelCfg), _i, _i]),
-    "am_mel_batch_ex": (_i, [_vp, _i, _i, _P(MelCfg), _i, _i, _vp]),
     "am_pcm_to_segments": (_i, [_vp, _i64, _vp, _i, _P(_i)]),
     "am_wav_info": (_i, [C.c_char_p, _P(_i), _P(_i), _P(_i64), _P(_i)]),
     "am_wav_decode_mono": (_i, [C.c_char_p, _i64, _vp, _i64, _P(_i64), _P(_i)]),
     "am_wav_to_segments": (_i, [C.c_char_p, C.c_double, _vp, _i, _P(_i), _P(C.c_double)]),
-    "am_resample_plan_create": (_i, [_i, _i, _P(_vp)]),
-    "am_resample_plan_free": (None, [_vp]),
-    "am_resample_out_len": (_i64, [_vp, _i64]),
-    "am_resample_dev": (_i, [_vp, _vp, _i64, _vp, _vp]),
-    "am_resample_filter": (_i, [_i, _i, _vp, _i, _P(_i), _P(_i), _P(_i), _P(_i64)]),
     "am_resample": (_i, [_vp, _i64, _i, _i, _vp, _i64, _P(_i64)]),
     "am_num_segments": (_i, [_i64]),
     "am_audio_to_segments_dev": (_i, [_vp, _i64, _vp, _i, _P(_i), _vp]),
@@ -115,11 +108,7 @@ SIGNATURES = {
     "am_knn_build": (_i, [_vp, _i64, _i, _i, _P(_vp)]),
     "am_knn_build_dev": (_i, [_vp, _i64, _i, _i, _vp, _P(_vp)]),
     "am_knn_free": (None, [_vp]),
-    "am_knn_size": (_i64, [_vp]),
-    "am_knn_dim": (_i, [_vp]),
-    "am_knn_get_vector": (_i, [_vp, _i64, _vp]),
-    "am_knn_query": (_i, [_vp, _vp, _i, _i, _vp, _vp]),
-    "am_knn_query_ex": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp]),
+    "am_knn_query": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp]),
     "am_knn_filter_by_distance": (_i, [_vp, _vp, _i, _i, C.c_float, _i, _i, _vp]),
     "am_knn_radius_walk": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _vp, _P(C.c_int32)]),
     "am_knn_song_path": (_i, [_vp, _P(SongPathCfg), _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp, _P(C.c_int32), _vp,
@@ -157,7 +146,6 @@ SIGNATURES = {
     "am_umap_plan_free": (None, [_vp]),
     "am_artist_gmm_fit": (_i, [_vp, _i64, _i, _vp, _i, _vp, _vp, _i, _i, C.c_double, C.c_double, _vp, _i64]
                           + [_vp] * 12),
-    "am_gmm_full_fit": (_i, [_vp, _i64, _i, _i, _i, _i, C.c_double, C.c_double, _vp, _i64] + [_vp] * 15),
     "am_gmm_fit": (_i, [_vp, _i64, _i, _i, _i, _i, _i, C.c_double, C.c_double, _vp, _i64] + [_vp] * 15),
     "am_track_features_plan_create": (_i, [_i, _P(_vp)]),
     "am_track_features_plan_free": (None, [_vp]),

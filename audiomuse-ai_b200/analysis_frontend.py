@@ -6,7 +6,8 @@ row 4: a sibling tower sharing K1's machinery).
 The reference computes ``librosa.feature.melspectrogram(y, sr=16000, n_fft=512, hop_length=256, n_mels=96,
 window='hann', center=False, power=2.0, norm='slaney', htk=False)``, compresses with ``log10(1 + 10000 x)`` and cuts
 non-overlapping patches of 187 frames, transposed to (frames, mels).  Here the mel + compression is one launch of
-``mel_kernel`` in its center=False / log1p-style mode (``am_mel_batch_ex``); the patch cut is a reshape.
+``mel_kernel`` in its center=False / log1p-style mode (``am_mel_batch`` with framing 1, log_mode 1); the patch cut is
+a reshape.
 """
 from __future__ import annotations
 
@@ -24,12 +25,12 @@ def musicnn_log_mel(audio: np.ndarray, sr: int = 16000) -> np.ndarray:
     """float32 (96, T): log10(1 + 10000 * mel_power), T = 1 + (len - 512) // 256."""
     lib = _lib.load()
     x = np.ascontiguousarray(audio, dtype=np.float32).reshape(1, -1)
-    cfg = _lib.MelCfg(int(sr), N_FFT, HOP, N_MELS, 0.0, float(sr) / 2.0, 0)
-    T = int(lib.am_mel_num_frames_ex(C.byref(cfg), 0, x.shape[1]))
-    if T <= 0:
+    cfg = _lib.MelCfg(int(sr), N_FFT, HOP, N_MELS, 0.0, float(sr) / 2.0, 0, framing=1, log_mode=1)
+    T = int(lib.am_mel_num_frames(C.byref(cfg), x.shape[1]))
+    if T <= 0:  # shorter than one frame
         return np.zeros((N_MELS, 0), dtype=np.float32)
     out = np.empty((1, N_MELS, T), dtype=np.float32)
-    _lib.check(lib.am_mel_batch_ex(_lib.ptr(x), 1, x.shape[1], C.byref(cfg), 0, 1, _lib.ptr(out)))
+    _lib.check(lib.am_mel_batch(_lib.ptr(x), 0, 1, x.shape[1], C.byref(cfg), _lib.ptr(out)))
     return out[0]
 
 

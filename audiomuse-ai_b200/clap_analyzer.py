@@ -87,11 +87,10 @@ def compute_mel_spectrogram_batch(audio: np.ndarray, sr: int = 48000) -> np.ndar
     T = 1 + n // cfg.hop
     shape = (B, 1, T, cfg.n_mels) if cfg.transpose else (B, 1, cfg.n_mels, T)
     out = np.empty(shape, dtype=np.float32)
-    if audio.dtype == np.int16:
-        _lib.check(lib.am_mel_batch_i16(_lib.ptr(audio), B, n, C.byref(cfg), _lib.ptr(out)))
-    else:
+    is_i16 = audio.dtype == np.int16
+    if not is_i16:
         audio = np.ascontiguousarray(audio, dtype=np.float32)
-        _lib.check(lib.am_mel_batch(_lib.ptr(audio), B, n, C.byref(cfg), _lib.ptr(out)))
+    _lib.check(lib.am_mel_batch(_lib.ptr(audio), int(is_i16), B, n, C.byref(cfg), _lib.ptr(out)))
     return out
 
 

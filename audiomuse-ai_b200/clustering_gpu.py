@@ -21,11 +21,11 @@ so a missing CUDA library can never masquerade as the GPU path).
 
     GPUGaussianMixture(n_components, covariance_type='full', init_params='k-means++', n_init, random_state,
         reg_covar).fit_predict(X)   :284-309 -> the reference wraps sklearn.mixture.GaussianMixture; here gmm_fit
-        (am_gmm_full_fit, csrc/gmm.cu): scikit-learn's k-means++ initialisation on the generator's own draws and float64
+        (am_gmm_fit, csrc/gmm.cu): scikit-learn's k-means++ initialisation on the generator's own draws and float64
         EM on the tensor cores.  Sets means_, weights_, covariances_, precisions_cholesky_, lower_bound_,
         lower_bounds_, n_iter_, converged_, labels_, using_gpu.  Only covariance_type='full' runs on the device.
-    GPUGaussianMixtureAnyCovariance(...): the same for all four covariance types ('diag', 'tied' and 'spherical'
-        through am_gmm_fit); integration.apply(gaussian_mixture=..., gmm_all_covariance_types=True) installs it.
+    GPUGaussianMixtureAnyCovariance(...): the same for all four covariance types;
+        integration.apply(gaussian_mixture=..., gmm_all_covariance_types=True) installs it.
 """
 from __future__ import annotations
 
@@ -510,8 +510,7 @@ GMM_MAX_D = 256             # AM_GMM_MAX_D
 GMM_MAX_K = 512             # AM_GMM_MAX_K
 GMM_MAX_COMPONENTS = 65535  # AM_GMM_MAX_COMPONENTS: n_init n_components
 GMM_COVARIANCE_TYPE = "full"
-GMM_COVARIANCE_TYPES = {"diag": 1, "tied": 2, "spherical": 3}   # AM_GMM_DIAG, AM_GMM_TIED, AM_GMM_SPHERICAL; 'full' is
-                                                                 # am_gmm_full_fit
+GMM_COVARIANCE_TYPES = {"full": 0, "diag": 1, "tied": 2, "spherical": 3}   # AM_GMM_FULL, _DIAG, _TIED, _SPHERICAL
 _ILL_DEFINED = ("Fitting the mixture model failed because some components have ill-defined empirical covariance (for "
                 "instance caused by singleton or collapsed samples). Try to decrease the number of components, increase "
                 "reg_covar, or scale the input data.")
@@ -580,11 +579,11 @@ def _check_gmm_params(n_components, n_init, max_iter, tol, reg_covar):
 def gmm_fit(X, n_components, n_init=10, max_iter=100, tol=1e-3, reg_covar=1e-4, random_state=None,
             intermediates=False, covariance_type="full") -> GmmFit:
     """GaussianMixture(n_components, covariance_type, init_params='k-means++', n_init, max_iter, tol, reg_covar,
-    random_state).fit_predict(X) on the device, in float64 whatever X's dtype: am_gmm_full_fit for 'full', am_gmm_fit
-    for 'diag', 'tied' and 'spherical'.  The k-means++ draws come from check_random_state(random_state) on the host,
-    so the generator ends where scikit-learn's fit leaves it.  ValueError for invalid input (before any device work)
-    and for an ill-defined covariance; B200Error when the device fails."""
-    if covariance_type != "full" and covariance_type not in GMM_COVARIANCE_TYPES:
+    random_state).fit_predict(X) on the device (am_gmm_fit), in float64 whatever X's dtype.  The k-means++ draws come
+    from check_random_state(random_state) on the host, so the generator ends where scikit-learn's fit leaves it.
+    ValueError for invalid input (before any device work) and for an ill-defined covariance; B200Error when the device
+    fails."""
+    if covariance_type not in GMM_COVARIANCE_TYPES:
         raise ValueError(f"covariance_type must be one of 'full', 'tied', 'diag', 'spherical', got {covariance_type!r}")
     _check_gmm_params(n_components, n_init, max_iter, tol, reg_covar)
     X = _check_gmm_input(X, int(n_components))
@@ -608,12 +607,8 @@ def gmm_fit(X, n_components, n_init=10, max_iter=100, tol=1e-3, reg_covar=1e-4, 
     opt = lambda a: None if a is None else _lib.ptr(a)   # noqa: E731
     outputs = (_lib.ptr(w), _lib.ptr(m), _lib.ptr(cv), _lib.ptr(pc), _lib.ptr(lbs), C.byref(it), C.byref(conv),
                C.byref(best), _lib.ptr(labels), C.byref(bad), opt(kpp), opt(ilb), opt(iit), opt(iconv), _lib.ptr(ms))
-    if covariance_type == "full":
-        _lib.check(lib.am_gmm_full_fit(_lib.ptr(X), N, d, K, n_init, max_iter, float(tol), float(reg_covar),
-                                       _lib.ptr(draws), len(draws), *outputs))
-    else:
-        _lib.check(lib.am_gmm_fit(_lib.ptr(X), N, d, K, GMM_COVARIANCE_TYPES[covariance_type], n_init, max_iter,
-                                  float(tol), float(reg_covar), _lib.ptr(draws), len(draws), *outputs))
+    _lib.check(lib.am_gmm_fit(_lib.ptr(X), N, d, K, GMM_COVARIANCE_TYPES[covariance_type], n_init, max_iter,
+                              float(tol), float(reg_covar), _lib.ptr(draws), len(draws), *outputs))
     if bad.value:
         raise ValueError(_ILL_DEFINED)
     n = int(it.value)

@@ -59,7 +59,7 @@ void prof_mark(const char* name, cudaStream_t st, int end);
   } while (0)
 
 int ensure_init();          // lazy context creation; AM_OK or error
-int mel_plan_hop(const am_mel_plan* plan);  // mel.cu
+int mel_plan_frames(const am_mel_plan* plan, int n_samples);  // mel.cu: frames T, or AM_ERR_INVALID (too short)
 int sm_count();             // SMs of the active device
 int device_cc();            // major*10+minor
 

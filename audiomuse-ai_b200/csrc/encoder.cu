@@ -1176,8 +1176,8 @@ extern "C" int am_clap_embed_tracks_dev(am_model* m, const am_mel_plan* plan, co
   AM_CHECK(n_tracks >= 0 && n_segments >= 0 && (pcm_dev || n_segments == 0), "am_clap_embed_tracks_dev: bad sizes");
   if (n_tracks == 0) return AM_OK;
   cudaStream_t st = (cudaStream_t)stream;
-  const int hop = mel_plan_hop(plan);
-  const int T = 1 + n_samples / hop;
+  const int T = mel_plan_frames(plan, n_samples);
+  if (T < 0) return T;
   const ForwardPlan* p;
   AM_TRY(plan_for(m, T, &p));
   const int sub = early_sub(*p, n_segments);
@@ -1211,7 +1211,9 @@ extern "C" int am_clap_embed_tracks_submit(am_model* m, const am_mel_cfg* cfg, c
                                            const int32_t* seg_offsets, int n_tracks, float* out) {
   AM_CHECK(m && cfg && seg_offsets && out, "am_clap_embed_tracks: NULL argument");
   AM_CHECK(n_tracks >= 0, "am_clap_embed_tracks: negative track count");
-  AM_CHECK(cfg->n_mels == m->n_mels && cfg->transpose == 0, "am_clap_embed_tracks: mel cfg does not match the model");
+  // the encoder is defined on CLAP's mel only: reflect padding and power_to_db
+  AM_CHECK(cfg->n_mels == m->n_mels && cfg->transpose == 0 && cfg->framing == 0 && cfg->log_mode == 0,
+           "am_clap_embed_tracks: mel cfg does not match the model");
   AM_CHECK(m->n_submitted - m->n_collected < 2, "am_clap_embed_tracks_submit: two calls are already in flight; collect one");
   const bool warm = m->n_submitted > m->n_collected;  // an earlier batch is still running
   am_model::Ticket& tk = m->tickets[m->n_submitted & 1];
@@ -1241,7 +1243,8 @@ extern "C" int am_clap_embed_tracks_submit(am_model* m, const am_mel_cfg* cfg, c
     if (!m->ev_copied[i]) AM_CUDA(cudaEventCreateWithFlags(&m->ev_copied[i], cudaEventDisableTiming));
     if (!m->ev_done[i]) AM_CUDA(cudaEventCreateWithFlags(&m->ev_done[i], cudaEventDisableTiming));
   }
-  const int T = 1 + n_samples / cfg->hop;
+  const int T = mel_plan_frames(plan, n_samples);
+  if (T < 0) return T;
   const ForwardPlan* p;
   AM_TRY(plan_for(m, T, &p));
   const int sub = early_sub(*p, n_segments);

@@ -5,7 +5,7 @@
 //                                      behind WAVE_FORMAT_EXTENSIBLE), any channel count, down-mixed to mono float32
 //                                      by the channel mean (librosa.to_mono).  Integer scaling follows libsndfile's
 //                                      float read (x / 2^(bits-1)), which is what librosa.load returns.
-//   am_resample_*                      device: rational polyphase resampler, the algorithm of
+//   am_resample                        device: rational polyphase resampler, the algorithm of
 //                                      scipy.signal.resample_poly (zero-phase Kaiser(5.0)-windowed sinc of half length
 //                                      10 max(up, down), gain up, cut-off 1 / max(up, down)); the common real-library
 //                                      case 44.1 kHz -> 48 kHz is up / down = 160 / 147, 21 taps per output sample.
@@ -184,7 +184,7 @@ audio_to_segments_kernel(const float* __restrict__ audio, int64_t L, int seg, in
 
 using namespace am;
 
-struct am_resample_plan {
+struct ResamplePlan {
   ResamplePlanHost host;
   DevBuf<float> poly_dev;
 };
@@ -315,80 +315,56 @@ extern "C" int am_wav_to_segments(const char* path, double max_seconds, int16_t*
   return am_pcm_to_segments(audio.data(), got, seg, max_seg, n_seg);
 }
 
-extern "C" int am_resample_plan_create(int sr_in, int sr_out, am_resample_plan** out) {
-  AM_CHECK(out != nullptr, "am_resample_plan_create: out is NULL");
-  *out = nullptr;
-  AM_CHECK(sr_in > 0 && sr_out > 0, "am_resample_plan_create: bad rates %d -> %d", sr_in, sr_out);
+static int resample_plan_create(int sr_in, int sr_out, ResamplePlan** out) {
+  AM_CHECK(sr_in > 0 && sr_out > 0, "am_resample: bad rates %d -> %d", sr_in, sr_out);
   const int g = std::gcd(sr_in, sr_out);
   const int up = sr_out / g, down = sr_in / g;
-  AM_CHECK(up <= 1024 && down <= 4096, "am_resample_plan_create: %d -> %d needs up / down = %d / %d (unsupported ratio)", sr_in,
+  AM_CHECK(up <= 1024 && down <= 4096, "am_resample: %d -> %d needs up / down = %d / %d (unsupported ratio)", sr_in,
            sr_out, up, down);
   AM_TRY(ensure_init());
-  auto p = std::make_unique<am_resample_plan>();
+  auto p = std::make_unique<ResamplePlan>();
   build_filter(up, down, &p->host);
-  AM_CHECK((size_t)up * p->host.taps * 4 <= 200 * 1024, "am_resample_plan_create: polyphase table too large");
+  AM_CHECK((size_t)up * p->host.taps * 4 <= 200 * 1024, "am_resample: polyphase table too large");
   AM_TRY(p->poly_dev.alloc(p->host.poly.size()));
   AM_CUDA(cudaMemcpy(p->poly_dev.p, p->host.poly.data(), p->host.poly.size() * 4, cudaMemcpyHostToDevice));
   *out = p.release();
   return AM_OK;
 }
 
-extern "C" void am_resample_plan_free(am_resample_plan* p) { delete p; }
-
-// host-only (no GPU): the polyphase table the plan uploads, poly f32[up, taps] with poly[p, i] = h[p + i * up - pre_pad]
-extern "C" int am_resample_filter(int sr_in, int sr_out, float* poly, int cap, int* up, int* down, int* taps,
-                                  int64_t* pre_remove) {
-  AM_CHECK(sr_in > 0 && sr_out > 0 && up && down && taps && pre_remove, "am_resample_filter: bad argument");
-  const int g = std::gcd(sr_in, sr_out);
-  ResamplePlanHost h;
-  build_filter(sr_out / g, sr_in / g, &h);
-  *up = h.up;
-  *down = h.down;
-  *taps = h.taps;
-  *pre_remove = h.n_pre_remove;
-  if (poly) {
-    AM_CHECK(cap >= (int)h.poly.size(), "am_resample_filter: table needs %zu floats", h.poly.size());
-    std::memcpy(poly, h.poly.data(), h.poly.size() * 4);
-  }
-  return AM_OK;
-}
-
-extern "C" int64_t am_resample_out_len(const am_resample_plan* p, int64_t n_in) {
-  if (!p || n_in <= 0) return 0;
+static int64_t resample_out_len(const ResamplePlan* p, int64_t n_in) {
   return (n_in * p->host.up + p->host.down - 1) / p->host.down;  // ceil(n * up / down), as resample_poly
 }
 
-extern "C" int am_resample_dev(const am_resample_plan* p, const float* x_dev, int64_t n_in, float* y_dev, void* stream) {
-  AM_CHECK(p && x_dev && y_dev && n_in > 0, "am_resample_dev: bad argument");
-  const int64_t n_out = am_resample_out_len(p, n_in);
-  const size_t smem = p->host.poly.size() * 4;  // <= 200 KiB (am_resample_plan_create)
+static int resample_dev(const ResamplePlan* p, const float* x_dev, int64_t n_in, float* y_dev, cudaStream_t stream) {
+  const int64_t n_out = resample_out_len(p, n_in);
+  const size_t smem = p->host.poly.size() * 4;  // <= 200 KiB (resample_plan_create)
   AM_TRY(allow_dynamic_smem<resample_kernel>(200 * 1024));
   const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((n_out + 255) / 256, (int64_t)sm_count() * 8));
-  AM_LAUNCH(resample_kernel, grid, 256, smem, (cudaStream_t)stream, x_dev, n_in, p->poly_dev.p, p->host.up, p->host.down,
+  AM_LAUNCH(resample_kernel, grid, 256, smem, stream, x_dev, n_in, p->poly_dev.p, p->host.up, p->host.down,
             p->host.taps, p->host.n_pre_remove, y_dev, n_out);
   return AM_OK;
 }
 
-// host convenience: x f32[n_in] at sr_in -> y f32[am_resample_out_len] at sr_out.  Re-entrant and stream-ordered (called
+// x f32[n_in] at sr_in -> y f32[ceil(n_in * up / down)] at sr_out.  Re-entrant and stream-ordered (called
 // from decoder threads while the encoder runs): the plan of a rate pair is built once and cached, scratch comes from
 // the stream-ordered pool of the calling thread's own stream -- no cudaMalloc / cudaFree, which would wait for every
 // kernel in flight on the device.
 extern "C" int am_resample(const float* x, int64_t n_in, int sr_in, int sr_out, float* y, int64_t cap, int64_t* n_out) {
   AM_CHECK(x && y && n_out && n_in > 0, "am_resample: bad argument");
   static std::mutex mu;
-  static std::map<std::pair<int, int>, am_resample_plan*> plans;  // process lifetime
-  am_resample_plan* p = nullptr;
+  static std::map<std::pair<int, int>, ResamplePlan*> plans;  // process lifetime
+  ResamplePlan* p = nullptr;
   {
     std::lock_guard<std::mutex> lk(mu);
     auto it = plans.find({sr_in, sr_out});
     if (it == plans.end()) {
-      AM_TRY(am_resample_plan_create(sr_in, sr_out, &p));
+      AM_TRY(resample_plan_create(sr_in, sr_out, &p));
       plans[{sr_in, sr_out}] = p;
     } else {
       p = it->second;
     }
   }
-  *n_out = am_resample_out_len(p, n_in);
+  *n_out = resample_out_len(p, n_in);
   AM_CHECK(cap >= *n_out, "am_resample: output buffer of %lld samples, need %lld", (long long)cap, (long long)*n_out);
   static thread_local Stream st;
   AM_TRY(st.create());
@@ -396,7 +372,7 @@ extern "C" int am_resample(const float* x, int64_t n_in, int sr_in, int sr_out, 
   AM_TRY(dx.alloc((size_t)n_in, st.s));
   AM_TRY(dy.alloc((size_t)*n_out, st.s));
   AM_CUDA(cudaMemcpyAsync(dx.p, x, (size_t)n_in * 4, cudaMemcpyHostToDevice, st.s));
-  AM_TRY(am_resample_dev(p, dx.p, n_in, dy.p, st.s));
+  AM_TRY(resample_dev(p, dx.p, n_in, dy.p, st.s));
   AM_CUDA(cudaMemcpyAsync(y, dy.p, (size_t)*n_out * 4, cudaMemcpyDeviceToHost, st.s));
   AM_CUDA(cudaStreamSynchronize(st.s));
   return AM_OK;

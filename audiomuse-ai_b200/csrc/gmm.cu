@@ -18,8 +18,8 @@
 //             finite sets the ill-defined flag instead of failing the launch
 //
 // am_gmm_fit runs the same seeding, initialisation, normaliser, convergence loop, best-init choice and labelling for
-// covariance_type 'diag', 'tied' and 'spherical'; only the covariance M-step, the precision factor and the E-step differ,
-// each in scikit-learn 1.9's operation order:
+// every covariance_type.  For 'diag', 'tied' and 'spherical' only the covariance M-step, the precision factor and the
+// E-step differ from 'full', each in scikit-learn 1.9's operation order:
 //
 //   diag      resp^T (X o X) on DMMA (gram_kernel<false> on a device copy of X o X), cov = (that / nk - mu^2) + reg,
 //             prec_chol = 1 / sqrt(cov) (diag_cov_kernel); the E-step runs the DMMA products X (mu o prec)^T and
@@ -798,35 +798,31 @@ __global__ void pack_kernel(const double* __restrict__ src, int c0, int K, int r
 
 using namespace am;
 
-namespace {
-
-constexpr int kFull = 0;   // the other types are AM_GMM_DIAG, AM_GMM_TIED and AM_GMM_SPHERICAL
-
-// One fit of any covariance type; fn names the C entry point in error messages.  'full' keeps am_gmm_full_fit's
-// launch sequence; the other types replace the covariance M-step, the precision factor and the E-step only.
-int gmm_fit(const char* fn, int type, const double* X, int64_t N, int d, int K, int n_init, int max_iter, double tol,
-            double reg_covar, const double* draws, int64_t n_draws, double* weights, double* means,
-            double* covariances, double* precisions_cholesky, double* lower_bounds, int32_t* n_iter,
-            int32_t* converged, int32_t* best_init, int64_t* labels, int32_t* ill_defined, int32_t* kpp,
-            double* init_lower_bounds, int32_t* init_n_iter, int32_t* init_converged, float* phase_ms) {
+extern "C" int am_gmm_fit(const double* X, int64_t N, int d, int K, int type, int n_init, int max_iter, double tol,
+                          double reg_covar, const double* draws, int64_t n_draws, double* weights, double* means,
+                          double* covariances, double* precisions_cholesky, double* lower_bounds, int32_t* n_iter,
+                          int32_t* converged, int32_t* best_init, int64_t* labels, int32_t* ill_defined, int32_t* kpp,
+                          double* init_lower_bounds, int32_t* init_n_iter, int32_t* init_converged, float* phase_ms) {
   using namespace gm;
+  AM_CHECK(type == AM_GMM_FULL || type == AM_GMM_DIAG || type == AM_GMM_TIED || type == AM_GMM_SPHERICAL,
+           "am_gmm_fit: covariance_type %d is not AM_GMM_FULL, AM_GMM_DIAG, AM_GMM_TIED or AM_GMM_SPHERICAL", type);
   AM_CHECK(X && draws && weights && means && covariances && precisions_cholesky && lower_bounds && n_iter &&
                converged && best_init && labels && ill_defined,
-           "%s: a required pointer is null", fn);
+           "am_gmm_fit: a required pointer is null");
   AM_CHECK(d >= 1 && d <= AM_GMM_MAX_D && K >= 1 && K <= AM_GMM_MAX_K,
-           "%s: need 1 <= d <= %d and 1 <= K <= %d (got d = %d, K = %d)", fn, AM_GMM_MAX_D, AM_GMM_MAX_K, d, K);
-  AM_CHECK(N >= K && N <= ((int64_t)1 << 31) - 64, "%s: need K <= N < 2^31 - 64 (got N = %lld, K = %d)", fn,
+           "am_gmm_fit: need 1 <= d <= %d and 1 <= K <= %d (got d = %d, K = %d)", AM_GMM_MAX_D, AM_GMM_MAX_K, d, K);
+  AM_CHECK(N >= K && N <= ((int64_t)1 << 31) - 64, "am_gmm_fit: need K <= N < 2^31 - 64 (got N = %lld, K = %d)",
            (long long)N, K);
   AM_CHECK(n_init >= 1 && max_iter >= 1 && tol >= 0.0 && reg_covar >= 0.0,
-           "%s: need n_init >= 1, max_iter >= 1, tol >= 0, reg_covar >= 0", fn);
-  AM_CHECK((int64_t)n_init * K <= AM_GMM_MAX_COMPONENTS, "%s: n_init K = %lld components exceeds %d", fn,
+           "am_gmm_fit: need n_init >= 1, max_iter >= 1, tol >= 0, reg_covar >= 0");
+  AM_CHECK((int64_t)n_init * K <= AM_GMM_MAX_COMPONENTS, "am_gmm_fit: n_init K = %lld components exceeds %d",
            (long long)n_init * K, AM_GMM_MAX_COMPONENTS);
   const int L = n_local_trials(K);
   const int64_t per_init = 1 + (int64_t)(K - 1) * L;
-  AM_CHECK(n_draws >= n_init * per_init, "%s: %lld draws, K = %d with n_init = %d needs %lld", fn,
+  AM_CHECK(n_draws >= n_init * per_init, "am_gmm_fit: %lld draws, K = %d with n_init = %d needs %lld",
            (long long)n_draws, K, n_init, (long long)(n_init * per_init));
   AM_TRY(ensure_init());
-  const bool full = type == kFull, tied = type == AM_GMM_TIED, sph = type == AM_GMM_SPHERICAL;
+  const bool full = type == AM_GMM_FULL, tied = type == AM_GMM_TIED, sph = type == AM_GMM_SPHERICAL;
   const bool lin = type == AM_GMM_DIAG || sph;       // the E-step is one product of the rows with per-component columns
 
   const int dp = (d + 15) / 16 * 16, d64 = (dp + kTile - 1) / kTile * kTile;
@@ -1131,31 +1127,4 @@ int gmm_fit(const char* fn, int type, const double* X, int64_t N, int d, int K, 
   if (phase_ms)
     for (int q = 0; q < 5; ++q) phase_ms[q] = ms[q];
   return AM_OK;
-}
-
-}  // namespace
-
-extern "C" int am_gmm_full_fit(const double* X, int64_t N, int d, int K, int n_init, int max_iter, double tol,
-                               double reg_covar, const double* draws, int64_t n_draws, double* weights,
-                               double* means, double* covariances, double* precisions_cholesky,
-                               double* lower_bounds, int32_t* n_iter, int32_t* converged, int32_t* best_init,
-                               int64_t* labels, int32_t* ill_defined, int32_t* kpp, double* init_lower_bounds,
-                               int32_t* init_n_iter, int32_t* init_converged, float* phase_ms) {
-  return gmm_fit("am_gmm_full_fit", kFull, X, N, d, K, n_init, max_iter, tol, reg_covar, draws, n_draws, weights,
-                 means, covariances, precisions_cholesky, lower_bounds, n_iter, converged, best_init, labels,
-                 ill_defined, kpp, init_lower_bounds, init_n_iter, init_converged, phase_ms);
-}
-
-extern "C" int am_gmm_fit(const double* X, int64_t N, int d, int K, int covariance_type, int n_init, int max_iter,
-                          double tol, double reg_covar, const double* draws, int64_t n_draws, double* weights,
-                          double* means, double* covariances, double* precisions_cholesky, double* lower_bounds,
-                          int32_t* n_iter, int32_t* converged, int32_t* best_init, int64_t* labels,
-                          int32_t* ill_defined, int32_t* kpp, double* init_lower_bounds, int32_t* init_n_iter,
-                          int32_t* init_converged, float* phase_ms) {
-  AM_CHECK(covariance_type == AM_GMM_DIAG || covariance_type == AM_GMM_TIED || covariance_type == AM_GMM_SPHERICAL,
-           "am_gmm_fit: covariance_type %d is not AM_GMM_DIAG, AM_GMM_TIED or AM_GMM_SPHERICAL (full: am_gmm_full_fit)",
-           covariance_type);
-  return gmm_fit("am_gmm_fit", covariance_type, X, N, d, K, n_init, max_iter, tol, reg_covar, draws, n_draws, weights,
-                 means, covariances, precisions_cholesky, lower_bounds, n_iter, converged, best_init, labels,
-                 ill_defined, kpp, init_lower_bounds, init_n_iter, init_converged, phase_ms);
 }

@@ -914,12 +914,6 @@ extern "C" int am_knn_build_dev(const float* X_dev, int64_t N, int d, int metric
 }
 
 extern "C" void am_knn_free(am_index* idx) { delete idx; }
-extern "C" int64_t am_knn_size(const am_index* idx) { return idx ? idx->N : 0; }
-extern "C" int am_knn_dim(const am_index* idx) { return idx ? idx->d : 0; }
-
-extern "C" int am_knn_get_vector(const am_index* idx, int64_t id, float* out) {
-  return am_knn_get_vectors(idx, &id, 1, out);
-}
 
 // ---------------------------------------------------------------- the memory of a host call
 int HostCall::thread_stream(cudaStream_t* st) {
@@ -1211,8 +1205,7 @@ extern "C" int am_knn_query_dev(const am_index* idx, const float* Q_dev, int nq,
                         [&](int, int, bool results_only) { return results_only ? AM_OK : call.finish(); });
 }
 
-extern "C" int am_knn_query_ex(const am_index* idx, const float* Q, int nq, int k, int mode, int64_t* ids,
-                               float* dist) {
+extern "C" int am_knn_query(const am_index* idx, const float* Q, int nq, int k, int mode, int64_t* ids, float* dist) {
   AM_CHECK(idx && (Q || nq == 0) && (ids || nq * (int64_t)k == 0) && (dist || nq * (int64_t)k == 0),
            "am_knn_query: NULL argument");
   AM_TRY(check_query(idx, nq, k));
@@ -1241,10 +1234,6 @@ extern "C" int am_knn_query_ex(const am_index* idx, const float* Q, int nq, int 
     AM_CUDA(cudaStreamSynchronize(st));
     return AM_OK;
   });
-}
-
-extern "C" int am_knn_query(const am_index* idx, const float* Q, int nq, int k, int64_t* ids, float* dist) {
-  return am_knn_query_ex(idx, Q, nq, k, 0, ids, dist);
 }
 
 extern "C" int am_knn_get_vectors(const am_index* idx, const int64_t* ids, int n, float* out) {

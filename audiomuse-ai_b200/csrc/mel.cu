@@ -14,6 +14,10 @@
 //     (each lane owns bands lane, lane+32, ...) -> dB.
 //   The 16 x n_mels tile is staged in smem and written with 64-byte row segments.
 //
+// The same tables run two other framings and a second compression (am_mel_cfg.framing / log_mode): no padding with
+// log10(1 + 10000 x) is the MusiCNN front end of tasks/analysis.py:371-375; zero padding is onset_strength's
+// melspectrogram (track_features.cu).
+//
 // Algorithmic traffic per 10 s window: 480000*2 B (PCM16) or *4 B (f32) in, 128*1001*4 B out.
 #include "common.cuh"
 
@@ -237,8 +241,6 @@ static size_t mel_smem_bytes(int hop, int n_mels, int nnz) {
   return floats * sizeof(float);
 }
 
-int mel_plan_hop(const am_mel_plan* plan) { return plan->cfg.hop; }
-
 static int validate_cfg(const am_mel_cfg* c) {
   AM_CHECK(c != nullptr, "mel cfg is NULL");
   AM_CHECK(c->n_fft == 2048 || c->n_fft == 1024 || c->n_fft == 512, "mel: n_fft must be 2048, 1024 or 512 (got %d)",
@@ -246,16 +248,30 @@ static int validate_cfg(const am_mel_cfg* c) {
   AM_CHECK(c->hop > 0 && (c->hop % 2) == 0 && c->hop <= kNfft, "mel: hop must be even, in (0, 2048]");
   AM_CHECK(c->n_mels > 0 && c->n_mels <= 256, "mel: n_mels must be in [1, 256]");
   AM_CHECK(c->sr > 0, "mel: sr must be positive");
+  AM_CHECK(c->framing >= 0 && c->framing <= 2, "mel: framing must be 0 (reflect pad), 1 (none) or 2 (zero pad), got %d",
+           c->framing);
+  AM_CHECK(c->log_mode == 0 || c->log_mode == 1, "mel: log_mode must be 0 or 1, got %d", c->log_mode);
   return AM_OK;
 }
+
+// The frames T of a window of n_samples under c's framing, or AM_ERR_INVALID for a window shorter than the framing
+// accepts: reflect padding needs more than n_fft / 2 samples, no padding one whole frame, zero padding one sample.
+static int frame_count(const am_mel_cfg& c, int n_samples) {
+  const int shortest = c.framing == 0 ? c.n_fft / 2 + 1 : (c.framing == 1 ? c.n_fft : 1);
+  AM_CHECK(n_samples >= shortest, "mel: framing %d needs a window of at least %d samples, got %d", c.framing, shortest,
+           n_samples);
+  return c.framing == 1 ? 1 + (n_samples - c.n_fft) / c.hop : 1 + n_samples / c.hop;
+}
+
+int mel_plan_frames(const am_mel_plan* plan, int n_samples) { return frame_count(plan->cfg, n_samples); }
 
 }  // namespace am
 
 using namespace am;
 
 extern "C" int am_mel_num_frames(const am_mel_cfg* cfg, int n_samples) {
-  if (!cfg || cfg->hop <= 0 || n_samples < 0) return AM_ERR_INVALID;
-  return 1 + n_samples / cfg->hop;
+  AM_TRY(validate_cfg(cfg));
+  return frame_count(*cfg, n_samples);
 }
 
 // host-only helper (no GPU): the filterbank the plan uploads, dense f32[n_mels, n_fft/2+1]
@@ -313,6 +329,7 @@ extern "C" int am_mel_plan_create(const am_mel_cfg* cfg, am_mel_plan** out) {
   }
   auto* plan = new am_mel_plan();
   plan->cfg = *cfg;
+  plan->center = cfg->framing == 0 ? 1 : (cfg->framing == 1 ? 0 : 2);
   plan->max_bin = max_bin;
   plan->nnz = (int)wts.size();
   // one allocation, 256-byte aligned slices
@@ -352,31 +369,14 @@ extern "C" int am_mel_plan_create(const am_mel_cfg* cfg, am_mel_plan** out) {
 
 extern "C" void am_mel_plan_free(am_mel_plan* plan) { delete plan; }
 
-// same tables, other framing / compression: center = 0 (librosa center=False), log_mode = 1 (log10(1 + 10000 x)) is
-// the MusiCNN front end of tasks/analysis.py:371-375; center = 2 (zero padding) is onset_strength's melspectrogram
-extern "C" int am_mel_plan_create_ex(const am_mel_cfg* cfg, int center, int log_mode, am_mel_plan** out) {
-  AM_CHECK((center >= 0 && center <= 2) && (log_mode == 0 || log_mode == 1), "am_mel_plan_create_ex: bad mode");
-  AM_TRY(am_mel_plan_create(cfg, out));
-  (*out)->center = center;
-  (*out)->log_mode = log_mode;
-  return AM_OK;
-}
-
-extern "C" int am_mel_num_frames_ex(const am_mel_cfg* cfg, int center, int n_samples) {
-  if (!cfg || cfg->hop <= 0) return 0;
-  return center ? 1 + n_samples / cfg->hop : (n_samples >= cfg->n_fft ? 1 + (n_samples - cfg->n_fft) / cfg->hop : 0);
-}
-
 extern "C" int am_mel_batch_dev(const am_mel_plan* plan, const void* pcm_dev, int pcm_is_i16, int B,
                                 int n_samples, float* out_dev, void* stream) {
   AM_CHECK(plan && pcm_dev && out_dev, "am_mel_batch_dev: NULL argument");
   AM_CHECK(B >= 0, "am_mel_batch_dev: negative batch");
-  AM_CHECK(plan->center == 2 ? n_samples >= 1
-                             : (plan->center ? n_samples > plan->cfg.n_fft / 2 : n_samples >= plan->cfg.n_fft),
-           "mel: window of %d samples is shorter than %s", n_samples, plan->center ? "the reflect pad" : "one frame");
+  const int T = frame_count(plan->cfg, n_samples);
+  if (T < 0) return T;
   if (B == 0) return AM_OK;
   const am_mel_cfg& c = plan->cfg;
-  const int T = plan->center ? 1 + n_samples / c.hop : 1 + (n_samples - c.n_fft) / c.hop;
   const size_t smem = mel_smem_bytes(c.hop, c.n_mels, plan->nnz);
   cudaStream_t st = (cudaStream_t)stream;
   for (int b0 = 0; b0 < B; b0 += 65535) {  // gridDim.y limit
@@ -390,36 +390,33 @@ extern "C" int am_mel_batch_dev(const am_mel_plan* plan, const void* pcm_dev, in
     if (pcm_is_i16) {
       if (narrow) {
         AM_LAUNCH((mel_kernel<true, 19>), grid, kThreads, smem, st, in, n_samples, c.hop, T, c.n_mels, max_bin,
-                  c.transpose, c.n_fft, shift, plan->nnz, plan->center, plan->log_mode, plan->t, o);
+                  c.transpose, c.n_fft, shift, plan->nnz, plan->center, c.log_mode, plan->t, o);
       } else {
         AM_LAUNCH((mel_kernel<true, 32>), grid, kThreads, smem, st, in, n_samples, c.hop, T, c.n_mels, max_bin,
-                  c.transpose, c.n_fft, shift, plan->nnz, plan->center, plan->log_mode, plan->t, o);
+                  c.transpose, c.n_fft, shift, plan->nnz, plan->center, c.log_mode, plan->t, o);
       }
     } else {
       if (narrow) {
         AM_LAUNCH((mel_kernel<false, 19>), grid, kThreads, smem, st, in, n_samples, c.hop, T, c.n_mels, max_bin,
-                  c.transpose, c.n_fft, shift, plan->nnz, plan->center, plan->log_mode, plan->t, o);
+                  c.transpose, c.n_fft, shift, plan->nnz, plan->center, c.log_mode, plan->t, o);
       } else {
         AM_LAUNCH((mel_kernel<false, 32>), grid, kThreads, smem, st, in, n_samples, c.hop, T, c.n_mels, max_bin,
-                  c.transpose, c.n_fft, shift, plan->nnz, plan->center, plan->log_mode, plan->t, o);
+                  c.transpose, c.n_fft, shift, plan->nnz, plan->center, c.log_mode, plan->t, o);
       }
     }
   }
   return AM_OK;
 }
 
-static int mel_batch_host(const void* pcm, int is_i16, int B, int n_samples, const am_mel_cfg* cfg,
-                          float* out, int center = 1, int log_mode = 0) {
+extern "C" int am_mel_batch(const void* pcm, int pcm_is_i16, int B, int n_samples, const am_mel_cfg* cfg, float* out) {
   AM_CHECK(pcm && out, "am_mel_batch: NULL buffer");
-  AM_TRY(validate_cfg(cfg));
-  AM_CHECK(B >= 0 && cfg &&
-               (center == 2 ? n_samples >= 1 : (center ? n_samples > cfg->n_fft / 2 : n_samples >= cfg->n_fft)),
-           "am_mel_batch: bad shape B=%d n_samples=%d", B, n_samples);
+  AM_CHECK(B >= 0, "am_mel_batch: negative batch");
+  const int T = am_mel_num_frames(cfg, n_samples);
+  if (T < 0) return T;
   if (B == 0) return AM_OK;
   am_mel_plan* plan = nullptr;
-  AM_TRY(am_mel_plan_create_ex(cfg, center, log_mode, &plan));
-  const int T = am_mel_num_frames_ex(cfg, center, n_samples);
-  const size_t in_bytes = (size_t)B * n_samples * (is_i16 ? 2 : 4);
+  AM_TRY(am_mel_plan_create(cfg, &plan));
+  const size_t in_bytes = (size_t)B * n_samples * (pcm_is_i16 ? 2 : 4);
   const size_t out_elems = (size_t)B * cfg->n_mels * T;
   DevBuf<char> d_in;
   DevBuf<float> d_out;
@@ -431,7 +428,7 @@ static int mel_batch_host(const void* pcm, int is_i16, int B, int n_samples, con
     cudaError_t e = cudaMemcpyAsync(d_in.p, pcm, in_bytes, cudaMemcpyHostToDevice, st.s);
     if (e != cudaSuccess) s = cuda_fail(e, "H2D pcm", __FILE__, __LINE__);
   }
-  if (s == AM_OK) s = am_mel_batch_dev(plan, d_in.p, is_i16, B, n_samples, d_out.p, st.s);
+  if (s == AM_OK) s = am_mel_batch_dev(plan, d_in.p, pcm_is_i16, B, n_samples, d_out.p, st.s);
   if (s == AM_OK) {
     cudaError_t e = cudaMemcpyAsync(out, d_out.p, out_elems * 4, cudaMemcpyDeviceToHost, st.s);
     if (e == cudaSuccess) e = cudaStreamSynchronize(st.s);
@@ -439,19 +436,6 @@ static int mel_batch_host(const void* pcm, int is_i16, int B, int n_samples, con
   }
   am_mel_plan_free(plan);
   return s;
-}
-
-extern "C" int am_mel_batch(const float* pcm, int B, int n_samples, const am_mel_cfg* cfg, float* out) {
-  return mel_batch_host(pcm, 0, B, n_samples, cfg, out);
-}
-extern "C" int am_mel_batch_i16(const int16_t* pcm, int B, int n_samples, const am_mel_cfg* cfg,
-                                float* out) {
-  return mel_batch_host(pcm, 1, B, n_samples, cfg, out);
-}
-extern "C" int am_mel_batch_ex(const float* pcm, int B, int n_samples, const am_mel_cfg* cfg, int center, int log_mode,
-                               float* out) {
-  AM_CHECK((center >= 0 && center <= 2) && (log_mode == 0 || log_mode == 1), "am_mel_batch_ex: bad mode");
-  return mel_batch_host(pcm, 0, B, n_samples, cfg, out, center, log_mode);
 }
 
 // tasks/clap_analyzer.py:502-523 (host side: decode stays on the host, SURVEY 8(a))

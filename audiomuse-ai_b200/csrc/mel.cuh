@@ -27,9 +27,7 @@ struct MelTables {
 
 struct am_mel_plan {
   am_mel_cfg cfg;
-  int center = 1;    // 1: librosa center=True (reflect pad n_fft/2); 0: frame t starts at t * hop;
-                     // 2: center=True with pad_mode='constant' (zero pad n_fft/2)
-  int log_mode = 0;  // 0: 10 log10(max(1e-10, .)) (power_to_db); 1: log10(1 + 10000 .) (tasks/analysis.py:374)
+  int center;    // cfg.framing as mel_kernel takes it: 1 reflect pad n_fft/2, 0 no padding, 2 zero pad n_fft/2
   am::MelTables t;
   int max_bin;   // highest FFT bin with non-zero mel weight
   int nnz;

@@ -517,8 +517,8 @@ extern "C" int am_track_features_plan_create(int sr, am_track_features_plan** ou
   p->kmin = lo;
   p->kmax = hi + 1;
   p->cap = (int)round_up((size_t)((p->kmax - p->kmin + 2) / 2), 32);
-  am_mel_cfg cfg{sr, kNfft, kTfHop, kTfMels, 0.0f, (float)sr / 2.0f, 0};
-  int s = am_mel_plan_create_ex(&cfg, 2, 0, &p->mel);
+  am_mel_cfg cfg{sr, kNfft, kTfHop, kTfMels, 0.0f, (float)sr / 2.0f, 0, /* framing: zero pad */ 2, 0};
+  int s = am_mel_plan_create(&cfg, &p->mel);
   if (s == AM_OK) s = allow_dynamic_smem<tf_spectrum_kernel<false>>(tf_spectrum_smem());
   if (s == AM_OK) s = allow_dynamic_smem<tf_spectrum_kernel<true>>(tf_spectrum_smem());
   if (s != AM_OK) {

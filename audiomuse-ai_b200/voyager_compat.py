@@ -240,7 +240,7 @@ class Index:
         dist = np.empty((nq, k), dtype=np.float32)
         if k > 0 and nq > 0:
             h = self._ensure_built()
-            st = _lib.load().am_knn_query_ex(h, _lib.ptr(q), nq, k, int(mode), _lib.ptr(ids), _lib.ptr(dist))
+            st = _lib.load().am_knn_query(h, _lib.ptr(q), nq, k, int(mode), _lib.ptr(ids), _lib.ptr(dist))
             if st == _lib.AM_ERR_RECALL:
                 raise RecallError(_lib.last_error())
             _lib.check(st)

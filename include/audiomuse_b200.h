@@ -62,41 +62,38 @@ AM_API int am_profile_report(char* buf, int cap);
  * config.CLAP_AUDIO_* (config.py:386-392). */
 typedef struct am_mel_cfg {
   int sr;         /* 48000 */
-  int n_fft;      /* 2048 (student), 1024 (teacher, config.py:384) or 512; win_length == n_fft, periodic Hann,
-                   * center=True, reflect pad */
+  int n_fft;      /* 2048 (student), 1024 (teacher, config.py:384) or 512; win_length == n_fft, periodic Hann */
   int hop;        /* 480 */
   int n_mels;     /* 128 */
   float fmin;     /* 0 */
   float fmax;     /* 14000 */
   int transpose;  /* 0: [B, n_mels, T] (student)   1: [B, T, n_mels] (teacher layout) */
+  /* Zero is CLAP's mel in both trailing fields.  The MusiCNN front end of tasks/analysis.py:371-375
+   * (librosa.feature.melspectrogram(sr=16000, n_fft=512, hop_length=256, n_mels=96, center=False, norm='slaney'),
+   * then log10(1 + 10000 x)) is framing 1, log_mode 1; onset_strength's melspectrogram is framing 2. */
+  int framing;    /* 0: reflect pad n_fft/2 (librosa center=True), T = 1 + n/hop, n > n_fft/2;
+                   * 1: no padding (center=False), frame t starts at t*hop, T = 1 + (n - n_fft)/hop, n >= n_fft;
+                   * 2: zero pad n_fft/2 (pad_mode='constant'), T = 1 + n/hop, n >= 1 */
+  int log_mode;   /* 0: 10 log10(max(1e-10, x)) (power_to_db)   1: log10(1 + 10000 x) */
 } am_mel_cfg;
 
 typedef struct am_mel_plan am_mel_plan;
+/* AM_ERR_INVALID for a framing or log_mode outside the values above */
 AM_API int am_mel_plan_create(const am_mel_cfg* cfg, am_mel_plan** out);
 AM_API void am_mel_plan_free(am_mel_plan* plan);
 /* host-only (no GPU): the dense filterbank f32[n_mels, n_fft/2+1] the plan uploads
  * (librosa.filters.mel(htk=False, norm='slaney') semantics) */
 AM_API int am_mel_filterbank(const am_mel_cfg* cfg, float* out);
-/* frames for a segment of n_samples: 1 + n_samples / hop */
+/* host-only: frames T of a window of n_samples under cfg's framing; AM_ERR_INVALID for a window shorter than the
+ * framing accepts */
 AM_API int am_mel_num_frames(const am_mel_cfg* cfg, int n_samples);
 
-/* host: pcm f32[B, n_samples] -> out f32[B, n_mels, T] (or [B, T, n_mels]) */
-AM_API int am_mel_batch(const float* pcm, int B, int n_samples, const am_mel_cfg* cfg, float* out);
-/* host: PCM16 windows as produced by am_pcm_to_segments (value q means q / 32767.0f) */
-AM_API int am_mel_batch_i16(const int16_t* pcm, int B, int n_samples, const am_mel_cfg* cfg, float* out);
-/* device: pcm_is_i16 selects int16 (q/32767) or float32 samples */
+/* pcm_is_i16 selects int16 (q / 32767.0f: PCM16 windows as produced by am_pcm_to_segments) or float32 samples.
+ * host: pcm[B, n_samples] -> out f32[B, n_mels, T] (or [B, T, n_mels]) */
+AM_API int am_mel_batch(const void* pcm, int pcm_is_i16, int B, int n_samples, const am_mel_cfg* cfg, float* out);
+/* device: the same on a plan, stream-ordered */
 AM_API int am_mel_batch_dev(const am_mel_plan* plan, const void* pcm_dev, int pcm_is_i16, int B,
                      int n_samples, float* out_dev, void* stream);
-
-/* Sibling front end on the same kernel (SURVEY 8(f) row 4): tasks/analysis.py:371-375 feeds MusiCNN with
- * librosa.feature.melspectrogram(sr=16000, n_fft=512, hop_length=256, n_mels=96, center=False, norm='slaney') and
- * log10(1 + 10000 x).  center: 1 = reflect pad n_fft/2 (T = 1 + n/hop), 0 = frame t starts at t*hop
- * (T = 1 + (n - n_fft)/hop), 2 = zero pad n_fft/2 (librosa's pad_mode='constant', T = 1 + n/hop, any n >= 1);
- * log_mode: 0 = 10 log10(max(1e-10, x)), 1 = log10(1 + 10000 x). */
-AM_API int am_mel_plan_create_ex(const am_mel_cfg* cfg, int center, int log_mode, am_mel_plan** out);
-AM_API int am_mel_num_frames_ex(const am_mel_cfg* cfg, int center, int n_samples);
-AM_API int am_mel_batch_ex(const float* pcm, int B, int n_samples, const am_mel_cfg* cfg, int center, int log_mode,
-                           float* out);
 
 /* tasks/clap_analyzer.py:502-523: clip to [-1,1], *32767 -> int16 (truncation), then the
  * 10 s / 5 s-hop windowing incl. the right-aligned tail window.  Host-side.
@@ -121,16 +118,8 @@ AM_API int am_wav_to_segments(const char* path, double max_seconds, int16_t* seg
 /* Device polyphase resampler: the algorithm of scipy.signal.resample_poly(x, up, down) with up / down = sr_out / sr_in
  * reduced (44.1 kHz -> 48 kHz: 160 / 147), Kaiser(5.0)-windowed sinc of half length 10 max(up, down), float64
  * accumulation.  librosa resamples with soxr_hq, which cannot be installed here: parity is pinned against scipy, NOT
- * against librosa, for files that are not already at 48 kHz. */
-typedef struct am_resample_plan am_resample_plan;
-AM_API int am_resample_plan_create(int sr_in, int sr_out, am_resample_plan** out);
-AM_API void am_resample_plan_free(am_resample_plan* plan);
-AM_API int64_t am_resample_out_len(const am_resample_plan* plan, int64_t n_in); /* ceil(n_in * up / down) */
-/* host-only: the plan's polyphase table poly f32[up, taps] (poly == NULL: sizes only) and its output offset; output
- * sample k is sum_i poly[t % up, i] * x[t / up - i] with t = (k + pre_remove) * down */
-AM_API int am_resample_filter(int sr_in, int sr_out, float* poly, int cap, int* up, int* down, int* taps,
-                              int64_t* pre_remove);
-AM_API int am_resample_dev(const am_resample_plan* plan, const float* x_dev, int64_t n_in, float* y_dev, void* stream);
+ * against librosa, for files that are not already at 48 kHz.
+ * x f32[n_in] at sr_in -> y f32[*n_out] at sr_out, *n_out = ceil(n_in * up / down) <= cap. */
 AM_API int am_resample(const float* x, int64_t n_in, int sr_in, int sr_out, float* y, int64_t cap, int64_t* n_out);
 /* windows a waveform of L samples at 48 kHz produces (tasks/clap_analyzer.py:510-521) */
 AM_API int am_num_segments(int64_t L);
@@ -226,15 +215,10 @@ typedef struct am_index am_index;
 AM_API int am_knn_build(const float* X, int64_t N, int d, int metric, am_index** out);
 AM_API int am_knn_build_dev(const float* X_dev, int64_t N, int d, int metric, void* stream, am_index** out);
 AM_API void am_knn_free(am_index* idx);
-AM_API int64_t am_knn_size(const am_index* idx);
-AM_API int am_knn_dim(const am_index* idx);
-AM_API int am_knn_get_vector(const am_index* idx, int64_t id, float* out /* [d] */);
 /* Q f32[nq,d] -> ids i64[nq,k], dist f32[nq,k]; ascending distance, ties by lower id.
- * Exact: candidates are re-ranked with float64 accumulation.  Re-entrant. */
-AM_API int am_knn_query(const am_index* idx, const float* Q, int nq, int k, int64_t* ids, float* dist);
-/* mode: 0 auto, 1 force fp32 scoring pass, 2 force bf16 tensor-core filter pass */
-AM_API int am_knn_query_ex(const am_index* idx, const float* Q, int nq, int k, int mode, int64_t* ids,
-                    float* dist);
+ * Exact: candidates are re-ranked with float64 accumulation.  Re-entrant.
+ * mode: 0 auto, 1 force fp32 scoring pass, 2 force bf16 tensor-core filter pass */
+AM_API int am_knn_query(const am_index* idx, const float* Q, int nq, int k, int mode, int64_t* ids, float* dist);
 /* Device version of voyager_manager.py:526-617 (_filter_by_distance, with :487-524 for lists longer than `batch`):
  * ids i64[n_lists, n] are row ids in result order (rows outside [0, N) are dropped like missing vectors);
  * keep u8[n_lists, n] receives 1 for the items the reference's greedy walk keeps.  threshold / lookback are
@@ -504,42 +488,34 @@ AM_API int am_artist_gmm_fit(const float* rows, int64_t n_rows, int d, const int
                              float* weights, float* means, float* covariances, int32_t* kpp, int32_t* labels,
                              float* phase_ms);
 
-/* ------------------------------------------------------------------ clustering-task Gaussian mixture, full covariance
- * GaussianMixture(K, covariance_type='full', init_params='k-means++', n_init, max_iter, tol, reg_covar).fit_predict
- * (tasks/clustering_helper._apply_clustering_model, method 'gmm') in float64.  Synchronous.
+/* ------------------------------------------------------------------ clustering-task Gaussian mixture
+ * GaussianMixture(K, covariance_type, init_params='k-means++', n_init, max_iter, tol, reg_covar).fit_predict
+ * (tasks/clustering_helper._apply_clustering_model, method 'gmm'; config.GMM_COVARIANCE_TYPE, which
+ * tasks/clustering_gpu.py:284-309, 385-392 and tasks/clustering_helper.py:295-302 hand to scikit-learn) in float64.
+ * Synchronous.
  *   X            f64[N, d], K <= N, 1 <= d <= AM_GMM_MAX_D, 1 <= K <= AM_GMM_MAX_K,
  *                n_init K <= AM_GMM_MAX_COMPONENTS (the components of all inits are one launch dimension)
+ *   covariance_type  AM_GMM_FULL, AM_GMM_DIAG, AM_GMM_TIED or AM_GMM_SPHERICAL; any other value is AM_ERR_INVALID
  *   draws        f64[n_draws]: the generator's random_sample() in order; init i uses the 1 + (K - 1)(2 + floor(ln K))
  *                doubles from i times that count (at least n_init times it)
  *   outputs      the best init's (first strictly greatest final lower bound) weights f64[K], means f64[K, d],
- *                covariances and precisions_cholesky f64[K, d, d], lower_bounds f64[max_iter] (NaN after n_iter),
+ *                covariances and precisions_cholesky (shapes below), lower_bounds f64[max_iter] (NaN after n_iter),
  *                n_iter, converged, best_init, labels i64[N] (argmax of one more E-step)
- *   ill_defined  1 when a Cholesky pivot of any init was <= 0 or not finite (scikit-learn's ValueError); the other
- *                outputs are then not written
+ *   ill_defined  1 when a full or tied Cholesky pivot of any init was <= 0 or not finite, or a diag or spherical
+ *                variance was <= 0 (scikit-learn's ValueError); the other outputs are then not written
  *   optional     kpp i32[n_init, K] (k-means++ rows), init_lower_bounds f64[n_init, max_iter], init_n_iter and
  *                init_converged i32[n_init], phase_ms f32[5] (device ms of seeding, E-step, normaliser, M-step,
  *                Cholesky and inverse, from CUDA events)
- * The workspace (about n_init K (N + 3 d^2) doubles) is allocated per call on the call's own stream. */
+ * The workspace (about n_init K (N + 3 d^2) doubles for 'full') is allocated per call on the call's own stream.
+ *   covariance_type      covariances              precisions_cholesky
+ *   AM_GMM_FULL          f64[K, d, d]             f64[K, d, d]          upper triangular
+ *   AM_GMM_DIAG          f64[K, d]                f64[K, d]             1 / sqrt(cov), elementwise
+ *   AM_GMM_TIED          f64[d, d]                f64[d, d]             upper triangular, as 'full'
+ *   AM_GMM_SPHERICAL     f64[K]                   f64[K] */
 #define AM_GMM_MAX_D 256
 #define AM_GMM_MAX_K 512
 #define AM_GMM_MAX_COMPONENTS 65535
-AM_API int am_gmm_full_fit(const double* X, int64_t N, int d, int K, int n_init, int max_iter, double tol,
-                           double reg_covar, const double* draws, int64_t n_draws, double* weights, double* means,
-                           double* covariances, double* precisions_cholesky, double* lower_bounds, int32_t* n_iter,
-                           int32_t* converged, int32_t* best_init, int64_t* labels, int32_t* ill_defined, int32_t* kpp,
-                           double* init_lower_bounds, int32_t* init_n_iter, int32_t* init_converged, float* phase_ms);
-
-/* ------------------------------------------------------------------ clustering-task Gaussian mixture, other covariances
- * The same fit for covariance_type 'diag', 'tied' or 'spherical' (config.GMM_COVARIANCE_TYPE, which
- * tasks/clustering_gpu.py:284-309, 385-392 and tasks/clustering_helper.py:295-302 hand to scikit-learn's
- * GaussianMixture), with am_gmm_full_fit's arguments, limits, seeding, convergence rule, best-init choice and outputs
- * except for the shapes of the two type-dependent arrays:
- *   covariance_type      covariances              precisions_cholesky
- *   AM_GMM_DIAG          f64[K, d]                f64[K, d]             1 / sqrt(cov), elementwise
- *   AM_GMM_TIED          f64[d, d]                f64[d, d]             upper triangular, as 'full'
- *   AM_GMM_SPHERICAL     f64[K]                   f64[K]
- * ill_defined is 1 when a diag or spherical variance was <= 0 or a tied Cholesky pivot was <= 0 or not finite.
- * Any other covariance_type is AM_ERR_INVALID ('full' runs through am_gmm_full_fit). */
+#define AM_GMM_FULL 0
 #define AM_GMM_DIAG 1
 #define AM_GMM_TIED 2
 #define AM_GMM_SPHERICAL 3

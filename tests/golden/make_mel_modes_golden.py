@@ -4,10 +4,10 @@
     python tests/golden/make_mel_modes_golden.py [--out PATH]     # needs a GPU; default tests/golden/mel_modes_golden.json
 
 Runs the library of the tree this file sits in over seeded 1 s inputs: the CLAP student configuration (48 kHz, n_fft
-2048, hop 480, 128 mels to 14 kHz) on float32 and int16 input with reflect padding (center 1), the teacher's
-transposed n_fft 1024 layout, and the MusiCNN front end (16 kHz, n_fft 512, hop 256, 96 mels) with frames starting
-at t * hop (center 0), in both compressions, and records each output's shape and the SHA-256 of its bytes.
-mel_modes_golden.json was written by the library as it was before the zero-pad mode (center 2) was added to the
+2048, hop 480, 128 mels to 14 kHz) on float32 and int16 input with reflect padding (am_mel_cfg.framing 0), the
+teacher's transposed n_fft 1024 layout, and the MusiCNN front end (16 kHz, n_fft 512, hop 256, 96 mels) with frames
+starting at t * hop (framing 1), in both compressions, and records each output's shape and the SHA-256 of its bytes.
+mel_modes_golden.json was written by the library as it was before the zero-pad mode (framing 2) was added to the
 kernel."""
 import argparse
 import ctypes as C
@@ -26,32 +26,29 @@ if ROOT not in sys.path:
 CLAP = (48000, 2048, 480, 128, 0.0, 14000.0, 0)
 TEACHER = (48000, 1024, 480, 64, 50.0, 14000.0, 1)
 MUSICNN = (16000, 512, 256, 96, 0.0, 8000.0, 0)
-# name -> (cfg, int16 input, center, log_mode, seed)
+# name -> (cfg, int16 input, framing, log_mode, seed)
 CASES = {
-    "clap_f32": (CLAP, False, 1, 0, 1),
-    "clap_i16": (CLAP, True, 1, 0, 2),
-    "teacher_f32": (TEACHER, False, 1, 0, 3),
-    "musicnn_log1p": (MUSICNN, False, 0, 1, 4),
-    "musicnn_db": (MUSICNN, False, 0, 0, 5),
-    "clap_center0": (CLAP, False, 0, 0, 6),
+    "clap_f32": (CLAP, False, 0, 0, 1),
+    "clap_i16": (CLAP, True, 0, 0, 2),
+    "teacher_f32": (TEACHER, False, 0, 0, 3),
+    "musicnn_log1p": (MUSICNN, False, 1, 1, 4),
+    "musicnn_db": (MUSICNN, False, 1, 0, 5),
+    "clap_center0": (CLAP, False, 1, 0, 6),
 }
 
 
 def mel_case(name):
     from audiomuse_ai_b200 import _lib
-    cfg_t, i16, center, log_mode, seed = CASES[name]
-    cfg = _lib.MelCfg(*cfg_t)
+    cfg_t, i16, framing, log_mode, seed = CASES[name]
+    cfg = _lib.MelCfg(*cfg_t, framing, log_mode)
     lib = _lib.load()
     rng = np.random.default_rng(seed)
     n = cfg_t[0]
     x = (0.3 * rng.standard_normal((2, n))).clip(-1, 1).astype(np.float32)
-    T = lib.am_mel_num_frames_ex(C.byref(cfg), center, n)
+    T = lib.am_mel_num_frames(C.byref(cfg), n)
     out = np.zeros((2, T, cfg_t[3]) if cfg_t[6] else (2, cfg_t[3], T), np.float32)
-    if i16:
-        q = (x * 32767.0).astype(np.int16)
-        _lib.check(lib.am_mel_batch_i16(_lib.ptr(q), 2, n, C.byref(cfg), _lib.ptr(out)))
-    else:
-        _lib.check(lib.am_mel_batch_ex(_lib.ptr(x), 2, n, C.byref(cfg), center, log_mode, _lib.ptr(out)))
+    pcm = (x * 32767.0).astype(np.int16) if i16 else x
+    _lib.check(lib.am_mel_batch(_lib.ptr(pcm), int(i16), 2, n, C.byref(cfg), _lib.ptr(out)))
     return out
 
 

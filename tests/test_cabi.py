@@ -73,6 +73,26 @@ def test_filterbank_bit_identical_to_oracle(lib):
     assert lib.am_mel_num_frames(C.byref(cfg), 480000) == 1001
 
 
+def test_mel_framings_and_out_of_range_modes(lib):
+    """am_mel_num_frames counts frames under each framing and refuses a window shorter than the framing accepts; a
+    framing, log_mode or covariance type outside its values is AM_ERR_INVALID before any device work."""
+    from audiomuse_ai_b200 import _lib
+
+    def cfg(framing=0, log_mode=0):
+        return _lib.MelCfg(16000, 512, 256, 96, 0.0, 8000.0, 0, framing, log_mode)
+    for framing, n, T in ((0, 48000, 188), (0, 257, 2), (1, 48000, 186), (1, 512, 1), (2, 48000, 188), (2, 1, 1)):
+        assert lib.am_mel_num_frames(C.byref(cfg(framing)), n) == T, (framing, n)
+    for framing, n in ((0, 256), (1, 511), (2, 0)):
+        assert lib.am_mel_num_frames(C.byref(cfg(framing)), n) == _lib.AM_ERR_INVALID, (framing, n)
+    plan = C.c_void_p()
+    for framing, log_mode, word in ((3, 0, "framing"), (-1, 0, "framing"), (0, 2, "log_mode")):
+        assert lib.am_mel_plan_create(C.byref(cfg(framing, log_mode)), C.byref(plan)) == _lib.AM_ERR_INVALID
+        assert word in _lib.last_error() and not plan.value
+        assert lib.am_mel_num_frames(C.byref(cfg(framing, log_mode)), 48000) == _lib.AM_ERR_INVALID
+    assert lib.am_gmm_fit(None, 100, 2, 2, 4, 1, 10, 1e-3, 1e-6, None, 0, *[None] * 15) == _lib.AM_ERR_INVALID
+    assert "am_gmm_fit: covariance_type 4" in _lib.last_error()
+
+
 def test_pcm_to_segments_matches_reference_goldens(lib, golden_dir):
     """C-ABI windowing + int16 truncation == the reference's analyze_audio_file (golden)."""
     from make_golden import SEGMENT_CASE_LENGTHS, golden_waveform

@@ -186,3 +186,23 @@ def test_embed_tracks_stream_matches_blocking_calls():
     it.close()                                  # in-flight batches are drained
     np.testing.assert_array_equal(sess.embed_tracks(*batches[1]), want[1])
     assert list(sess.embed_tracks_stream(iter([]))) == []
+
+
+def test_embed_tracks_refuses_mel_modes_other_than_clap():
+    """The encoder is defined on CLAP's mel only: am_clap_embed_tracks_submit refuses another framing or compression
+    before it opens a ticket, and the session keeps working."""
+    import ctypes as C
+    from audiomuse_ai_b200 import _lib, clap_analyzer as ca, corpus, weights
+    sess = ca.B200Session.from_state_dict(weights.random_state_dict(0))
+    pcm = corpus.synth_pcm_batch(2, start=30)
+    offs = np.arange(3, dtype=np.int32)
+    want = sess.embed_tracks(pcm, offs)
+    out = np.empty_like(want)
+    for framing, log_mode in ((1, 0), (2, 0), (0, 1)):
+        cfg = ca._mel_cfg(transpose=False)
+        cfg.framing, cfg.log_mode = framing, log_mode
+        st = sess._lib.am_clap_embed_tracks_submit(sess._h, C.byref(cfg), _lib.ptr(pcm), pcm.shape[1],
+                                                   _lib.ptr(offs), 2, _lib.ptr(out))
+        assert st == _lib.AM_ERR_INVALID and "does not match the model" in _lib.last_error()
+    np.testing.assert_array_equal(sess.embed_tracks(pcm, offs), want)
+    np.testing.assert_array_equal(next(sess.embed_tracks_stream(iter([(pcm, offs)]))), want)

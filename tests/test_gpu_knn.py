@@ -1,5 +1,4 @@
 """K4 parity: exact GPU index vs the float64 oracle -- identical ids (bit-exact index work)."""
-import ctypes
 import functools
 import os
 
@@ -165,8 +164,8 @@ def test_filter_by_distance_euclidean_large_list():
 
 
 @pytest.mark.parametrize("space_name", ["Cosine", "Euclidean"])
-def test_get_vectors(space_name):
-    """am_knn_get_vectors and am_knn_get_vector = the stored rows."""
+def test_get_vectors_of_many_rows_and_of_one(space_name):
+    """am_knn_get_vectors, of many rows and of one, = the stored rows."""
     from audiomuse_ai_b200 import voyager_compat as vc
     rng = np.random.default_rng(9)
     x = rng.standard_normal((500, 200)).astype(np.float32)
@@ -177,8 +176,9 @@ def test_get_vectors(space_name):
     np.testing.assert_array_equal(stored, np.stack([idx.get_vector(i) for i in ids]))
     from audiomuse_ai_b200 import _lib
     one = np.empty(200, np.float32)
-    for j, i in enumerate(ids):   # the one-row C entry point
-        _lib.check(_lib.load().am_knn_get_vector(idx._ensure_built(), ctypes.c_int64(idx._row_of(i)), _lib.ptr(one)))
+    for j, i in enumerate(ids):   # one row per call
+        row = np.array([idx._row_of(i)], np.int64)
+        _lib.check(_lib.load().am_knn_get_vectors(idx._ensure_built(), _lib.ptr(row), 1, _lib.ptr(one)))
         np.testing.assert_array_equal(one, stored[j])
 
 

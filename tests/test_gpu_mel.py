@@ -144,7 +144,7 @@ def test_other_fft_sizes_teacher_config(n_fft, n_mels, fmin, transpose):
 @pytest.mark.parametrize("seconds", [3.5, 30.0])
 def test_musicnn_front_end_matches_oracle(seconds):
     """tasks/analysis.py:368-391: mel 96 / n_fft 512 / hop 256 at 16 kHz, center=False, log10(1 + 10000 x), patches of
-    187 frames -- on the same kernel in its second framing / compression mode (am_mel_batch_ex)."""
+    187 frames -- on the same kernel in its second framing / compression mode (am_mel_batch, framing 1, log_mode 1)."""
     from audiomuse_ai_b200 import analysis_frontend as af
     rng = np.random.default_rng(int(seconds * 10))
     n = int(seconds * 16000)

@@ -168,8 +168,8 @@ def test_invalid_input_is_rejected_before_device_work():
     assert lib.am_track_features_plan_create(96000, C.byref(h)) == _lib.AM_ERR_INVALID
 
 
-def test_existing_mel_modes_unchanged():
-    """The reflect (center 1) and frame-start (center 0) modes of the mel kernel, in both compressions and both input
+def test_existing_mel_modes_replay_their_golden():
+    """The reflect (framing 0) and frame-start (framing 1) modes of the mel kernel, in both compressions and both input
     types, give the bits they gave before the zero-pad mode was added (tests/golden/mel_modes_golden.json, written by
     the library before that change)."""
     import json
@@ -182,14 +182,14 @@ def test_existing_mel_modes_unchanged():
         assert digest(mel_case(name)) == g[name], name
 
 
-def test_zero_pad_mel_mode_against_oracle():
+def test_zero_pad_framing_against_oracle():
     from audiomuse_ai_b200 import _lib
     import ctypes as C
     y = otf.synth_track("chord", 3.0, 16000, 12)
-    cfg = _lib.MelCfg(16000, 2048, 512, 128, 0.0, 8000.0, 0)
+    cfg = _lib.MelCfg(16000, 2048, 512, 128, 0.0, 8000.0, 0, framing=2)
     T = 1 + len(y) // 512
     out = np.zeros((1, 128, T), np.float32)
-    _lib.check(_lib.load().am_mel_batch_ex(_lib.ptr(y), 1, len(y), C.byref(cfg), 2, 0, _lib.ptr(out)))
+    _lib.check(_lib.load().am_mel_batch(_lib.ptr(y), 0, 1, len(y), C.byref(cfg), _lib.ptr(out)))
     ref = otf.mel_db(otf.stft_power(y), 16000)
     assert np.max(np.abs(out[0] - np.maximum(ref, -100.0))) <= 2e-3
 

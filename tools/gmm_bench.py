@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Time the clustering task's GaussianMixture on the GPU (am_gmm_full_fit / am_gmm_fit, csrc/gmm.cu).
+"""Time the clustering task's GaussianMixture on the GPU (am_gmm_fit, csrc/gmm.cu).
 
     python tools/gmm_bench.py [--shapes 20000x60,20000x100,100000x60,100000x100] [--no-check]
                               [--covariance-type full|diag|tied|spherical]

@@ -3,7 +3,7 @@
     python tools/gmm_equiv.py dump FILE.npz       # on the build to compare against
     python tools/gmm_equiv.py compare FILE.npz    # on the build under test: every array np.array_equal
 
-Records every output of gmm_fit(X, K, ...) with the default covariance_type ('full', am_gmm_full_fit) and
+Records every output of gmm_fit(X, K, ...) with the default covariance_type ('full', AM_GMM_FULL) and
 intermediates=True, except the phase times: the weights, means, covariances, precision factors, bounds, n_iter,
 converged, best init, labels, k-means++ rows and every init's bounds, iterations and convergence.  The inputs are
 tests/test_gpu_gmm.py's full-fit sets (ragged N, d up to 256, K in {1, 2, 40, 100}, N = K, overlap, duplicated rows)

@@ -131,7 +131,8 @@ def _collect():
             out[f"{sname}/N{N}/d{d}/other_kernels"] = _kernels()
             one = np.empty((5, d), np.float32)
             for j, i in enumerate(ids[:5]):
-                _lib.check(_lib.load().am_knn_get_vector(idx._ensure_built(), C.c_int64(i), _lib.ptr(one[j])))
+                row = np.array([i], np.int64)
+                _lib.check(_lib.load().am_knn_get_vectors(idx._ensure_built(), _lib.ptr(row), 1, _lib.ptr(one[j])))
             out[f"{sname}/N{N}/d{d}/get_vector"] = one
             _kernels()
     # the spectral / UMAP graph: euclidean self-query of device rows, mode 0, on the caller's stream
