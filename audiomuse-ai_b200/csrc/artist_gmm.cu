@@ -23,6 +23,7 @@
 // touch the arithmetic.  The per-problem products are [n x d] x [d x K <= 16]: too narrow for wgmma, and float64 is
 // what keeps the decisions equal to scikit-learn's, so this is CUDA-core code by design.
 #include "common.cuh"
+#include "host_call.cuh"
 
 #include <algorithm>
 #include <cmath>
@@ -698,7 +699,6 @@ extern "C" int am_artist_gmm_fit(const float* rows, int64_t n_rows, int d, const
            n_init * draws_per_init(kmax));
   for (int64_t e = 0; e < n_rows * d; ++e)
     AM_CHECK(std::isfinite(rows[e]), "am_artist_gmm_fit: row %lld has a NaN or infinity", (long long)(e / d));
-  AM_TRY(ensure_init());
 
   // every problem (artist, K, init) with K <= n; the first k-means++ centre is choice(n, p=uniform) on the host
   const int A = n_artists;
@@ -734,9 +734,8 @@ extern "C" int am_artist_gmm_fit(const float* rows, int64_t n_rows, int d, const
       }
   }
 
-  Stream st;
-  AM_TRY(st.create());
-  cudaStream_t s = st.s;
+  cudaStream_t s;
+  AM_TRY(HostCall::thread_stream(&s));
   cudaEvent_t ev[4] = {};
   for (auto& e : ev) AM_CUDA(cudaEventCreate(&e));
   struct EvGuard {
@@ -747,55 +746,39 @@ extern "C" int am_artist_gmm_fit(const float* rows, int64_t n_rows, int d, const
     }
   } evg{ev};
   const int P_all = (int)all.size();
-  DevBuf<float> dX, dW, dM, dC;
-  DevBuf<int64_t> dOff;
-  DevBuf<int> dLo, dHi, dFirst, dCounter;
-  DevBuf<double> dDraws, dBic, dLb;
-  DevBuf<int32_t> dChosen, dIt, dKpp, dLab;
-  DevBuf<uint8_t> dFailed, dConv;
-  DevBuf<Result> dRes;
-  DevBuf<Problem> dProbs;
-  AM_TRY(dX.alloc((size_t)n_rows * d));
-  AM_TRY(dOff.alloc(A + 1));
-  AM_TRY(dLo.alloc(A));
-  AM_TRY(dHi.alloc(A));
-  AM_TRY(dFirst.alloc(A));
-  AM_TRY(dCounter.alloc(1));
-  AM_TRY(dDraws.alloc(std::max<int64_t>(1, n_draws)));
-  AM_TRY(dBic.alloc((size_t)A * kMaxK));
-  AM_TRY(dFailed.alloc((size_t)A * kMaxK));
-  AM_TRY(dLb.alloc((size_t)A * kMaxK * n_init));
-  AM_TRY(dIt.alloc((size_t)A * kMaxK * n_init));
-  AM_TRY(dConv.alloc((size_t)A * kMaxK * n_init));
-  AM_TRY(dRes.alloc((size_t)A * kMaxK * n_init));
-  AM_TRY(dChosen.alloc(A));
-  AM_TRY(dW.alloc((size_t)A * kMaxK));
-  AM_TRY(dM.alloc((size_t)A * kMaxK * d));
-  AM_TRY(dC.alloc((size_t)A * kMaxK * d));
-  AM_TRY(dProbs.alloc(std::max(1, P_all)));
-  if (kpp) AM_TRY(dKpp.alloc((size_t)A * kMaxK * n_init * kMaxK));
-  if (labels) AM_TRY(dLab.alloc((size_t)kMaxK * n_init * n_rows));
-  AM_CUDA(cudaMemcpyAsync(dX.p, rows, (size_t)n_rows * d * 4, cudaMemcpyHostToDevice, s));
-  AM_CUDA(cudaMemcpyAsync(dOff.p, offsets, (A + 1) * 8, cudaMemcpyHostToDevice, s));
-  AM_CUDA(cudaMemcpyAsync(dLo.p, k_lo, A * 4, cudaMemcpyHostToDevice, s));
-  AM_CUDA(cudaMemcpyAsync(dHi.p, k_hi, A * 4, cudaMemcpyHostToDevice, s));
-  AM_CUDA(cudaMemcpyAsync(dFirst.p, art_first.data(), A * 4, cudaMemcpyHostToDevice, s));
-  AM_CUDA(cudaMemcpyAsync(dDraws.p, draws, n_draws * 8, cudaMemcpyHostToDevice, s));
-  AM_CUDA(cudaMemsetAsync(dW.p, 0, dW.n * 4, s));
-  AM_CUDA(cudaMemsetAsync(dM.p, 0, dM.n * 4, s));
-  AM_CUDA(cudaMemsetAsync(dC.p, 0, dC.n * 4, s));
-  AM_CUDA(cudaMemsetAsync(dLb.p, 0xff, dLb.n * 8, s));       // NaN: an init that never ran
-  AM_CUDA(cudaMemsetAsync(dIt.p, 0, dIt.n * 4, s));
-  AM_CUDA(cudaMemsetAsync(dConv.p, 0, dConv.n, s));
-  if (kpp) AM_CUDA(cudaMemsetAsync(dKpp.p, 0xff, dKpp.n * 4, s));
-  if (labels) AM_CUDA(cudaMemsetAsync(dLab.p, 0xff, dLab.n * 4, s));
-  {
-    // problems with K > n never run: they report failed
-    std::vector<Result> init_res((size_t)A * kMaxK * n_init, Result{NAN, NAN, 0, 0, 1, 0});
-    AM_CUDA(cudaMemcpyAsync(dRes.p, init_res.data(), init_res.size() * sizeof(Result), cudaMemcpyHostToDevice, s));
-    AM_CUDA(cudaStreamSynchronize(s));
-  }
-  AM_CUDA(cudaMemcpyAsync(dProbs.p, all.data(), P_all * sizeof(Problem), cudaMemcpyHostToDevice, s));
+  const size_t n_ak = (size_t)A * kMaxK, n_aki = n_ak * n_init;
+  // problems with K > n never run: they report failed
+  const std::vector<Result> init_res(n_aki, Result{NAN, NAN, 0, 0, 1, 0});
+  HostCall call(s, 0, HostCall::Memory::Owned);
+  float *dX, *dW, *dM, *dC;
+  int64_t* dOff;
+  int *dLo, *dHi, *dFirst, *dCounter;
+  double *dDraws, *dBic, *dLb;
+  int32_t *dChosen, *dIt, *dKpp, *dLab;
+  uint8_t *dFailed, *dConv;
+  Result* dRes;
+  Problem* dProbs;
+  call.up(&dX, rows, (size_t)n_rows * d);
+  call.up(&dOff, offsets, (size_t)A + 1);
+  call.up(&dLo, k_lo, (size_t)A);
+  call.up(&dHi, k_hi, (size_t)A);
+  call.up(&dFirst, art_first.data(), (size_t)A);
+  call.up(&dRes, init_res.data(), n_aki);
+  call.both(&dDraws, draws, (size_t)n_draws, (size_t)std::max<int64_t>(1, n_draws));
+  call.both(&dProbs, all.data(), (size_t)P_all, (size_t)std::max(1, P_all));
+  call.down(&dChosen, (size_t)A, chosen_k);
+  call.down(&dBic, n_ak, bic);
+  call.down(&dFailed, n_ak, failed);
+  call.down(&dLb, n_aki, lower_bound, 0xff);  // NaN: an init that never ran
+  call.down(&dIt, n_aki, n_iter, 0);
+  call.down(&dConv, n_aki, converged, 0);
+  call.down(&dW, n_ak, weights, 0);
+  call.down(&dM, n_ak * d, means, 0);
+  call.down(&dC, n_ak * d, covariances, 0);
+  call.down(&dKpp, kpp ? n_aki * kMaxK : 0, kpp, 0xff);
+  call.down(&dLab, labels ? (size_t)kMaxK * n_init * n_rows : 0, labels, 0xff);
+  call.device(&dCounter, 1);
+  AM_TRY(call.start());
   AM_TRY(allow_dynamic_smem<fit_kernel>(kSmemBytes));
 
   // chunks of whole artists whose scratch fits the budget
@@ -828,7 +811,7 @@ extern "C" int am_artist_gmm_fit(const float* rows, int64_t n_rows, int d, const
     // the gather in phase 2 reads each problem's scratch offsets
     const int pb = art_first[a0], pe = a1 < A ? art_first[a1] : P_all;
     if (pe > pb)
-      AM_CUDA(cudaMemcpyAsync(dProbs.p + pb, all.data() + pb, (pe - pb) * sizeof(Problem), cudaMemcpyHostToDevice, s));
+      AM_CUDA(cudaMemcpyAsync(dProbs + pb, all.data() + pb, (pe - pb) * sizeof(Problem), cudaMemcpyHostToDevice, s));
     std::stable_sort(runs.begin(), runs.end(), [](const Problem& x, const Problem& y) {
       return (int64_t)x.n * x.K > (int64_t)y.n * y.K;
     });
@@ -838,17 +821,17 @@ extern "C" int am_artist_gmm_fit(const float* rows, int64_t n_rows, int d, const
       AM_CUDA(cudaMemcpyAsync(dRuns.p, runs.data(), runs.size() * sizeof(Problem), cudaMemcpyHostToDevice, s));
     AM_TRY(dscr.ensure((size_t)std::max<int64_t>(1, dsz)));
     AM_TRY(iscr.ensure((size_t)std::max<int64_t>(1, isz)));
-    AM_CUDA(cudaMemsetAsync(dCounter.p, 0, 4, s));
+    AM_CUDA(cudaMemsetAsync(dCounter, 0, 4, s));
     AM_CUDA(cudaEventRecord(ev[0], s));
     if (!runs.empty()) {
       const int grid = std::min<int>((int)runs.size(), 2 * sm_count());
-      AM_LAUNCH(fit_kernel, grid, kThreads, kSmemBytes, s, dX.p, d, dRuns.p, (int)runs.size(), dCounter.p, dDraws.p,
-                n_init, max_iter, tol, reg_covar, dscr.p, iscr.p, dRes.p, kpp ? dKpp.p : nullptr,
-                labels ? dLab.p : nullptr, n_rows);
+      AM_LAUNCH(fit_kernel, grid, kThreads, kSmemBytes, s, dX, d, dRuns.p, (int)runs.size(), dCounter, dDraws,
+                n_init, max_iter, tol, reg_covar, dscr.p, iscr.p, dRes, kpp ? dKpp : nullptr,
+                labels ? dLab : nullptr, n_rows);
     }
     AM_CUDA(cudaEventRecord(ev[1], s));
-    AM_LAUNCH(select_kernel, a1 - a0, kThreads, 0, s, dProbs.p, dFirst.p, a0, dOff.p, dLo.p, dHi.p, d, n_init, dRes.p,
-              dscr.p, dChosen.p, dBic.p, dFailed.p, dLb.p, dIt.p, dConv.p, dW.p, dM.p, dC.p);
+    AM_LAUNCH(select_kernel, a1 - a0, kThreads, 0, s, dProbs, dFirst, a0, dOff, dLo, dHi, d, n_init, dRes,
+              dscr.p, dChosen, dBic, dFailed, dLb, dIt, dConv, dW, dM, dC);
     AM_CUDA(cudaEventRecord(ev[2], s));
     AM_CUDA(cudaStreamSynchronize(s));
     float ms = 0.f;
@@ -858,18 +841,7 @@ extern "C" int am_artist_gmm_fit(const float* rows, int64_t n_rows, int d, const
     sel_ms += ms;
     a0 = a1;
   }
-  AM_CUDA(cudaMemcpyAsync(chosen_k, dChosen.p, A * 4, cudaMemcpyDeviceToHost, s));
-  AM_CUDA(cudaMemcpyAsync(bic, dBic.p, dBic.n * 8, cudaMemcpyDeviceToHost, s));
-  AM_CUDA(cudaMemcpyAsync(failed, dFailed.p, dFailed.n, cudaMemcpyDeviceToHost, s));
-  AM_CUDA(cudaMemcpyAsync(lower_bound, dLb.p, dLb.n * 8, cudaMemcpyDeviceToHost, s));
-  AM_CUDA(cudaMemcpyAsync(n_iter, dIt.p, dIt.n * 4, cudaMemcpyDeviceToHost, s));
-  AM_CUDA(cudaMemcpyAsync(converged, dConv.p, dConv.n, cudaMemcpyDeviceToHost, s));
-  AM_CUDA(cudaMemcpyAsync(weights, dW.p, dW.n * 4, cudaMemcpyDeviceToHost, s));
-  AM_CUDA(cudaMemcpyAsync(means, dM.p, dM.n * 4, cudaMemcpyDeviceToHost, s));
-  AM_CUDA(cudaMemcpyAsync(covariances, dC.p, dC.n * 4, cudaMemcpyDeviceToHost, s));
-  if (kpp) AM_CUDA(cudaMemcpyAsync(kpp, dKpp.p, dKpp.n * 4, cudaMemcpyDeviceToHost, s));
-  if (labels) AM_CUDA(cudaMemcpyAsync(labels, dLab.p, dLab.n * 4, cudaMemcpyDeviceToHost, s));
-  AM_CUDA(cudaStreamSynchronize(s));
+  AM_TRY(call.finish());
   if (phase_ms) {
     phase_ms[0] = fit_ms;
     phase_ms[1] = sel_ms;

@@ -16,6 +16,7 @@
 //       SMALLEST root among its core neighbours -- which is what scikit-learn's index-ordered depth-first expansion
 //       produces, clusters being numbered by their lowest core index.
 #include "common.cuh"
+#include "host_call.cuh"
 
 #include <algorithm>
 #include <vector>
@@ -282,30 +283,27 @@ using namespace am;
 
 extern "C" int am_pca_moments(const float* X, int64_t N, int d, double* mean, double* cov) {
   AM_CHECK(X && mean && cov && N >= 2 && d >= 1 && d <= 8192, "am_pca_moments: bad argument (need N >= 2, 1 <= d <= 8192)");
-  AM_TRY(ensure_init());
-  Stream st;
-  AM_TRY(st.create());
-  DevBuf<float> dX;
-  DevBuf<double> dM, dC;
-  AM_TRY(dX.alloc((size_t)N * d));
-  AM_TRY(dM.alloc((size_t)d));
-  AM_TRY(dC.alloc((size_t)d * d));
-  AM_CUDA(cudaMemcpyAsync(dX.p, X, (size_t)N * d * 4, cudaMemcpyHostToDevice, st.s));
-  AM_CUDA(cudaMemsetAsync(dM.p, 0, (size_t)d * 8, st.s));
-  AM_CUDA(cudaMemsetAsync(dC.p, 0, (size_t)d * d * 8, st.s));
+  cudaStream_t st;
+  AM_TRY(HostCall::thread_stream(&st));
+  HostCall call(st, 0, HostCall::Memory::Owned);
+  float* dX;
+  double *dM, *dC;
+  call.up(&dX, X, (size_t)N * d);
+  call.device(&dM, (size_t)d, 0);
+  call.down(&dC, (size_t)d * d, cov, 0);
+  AM_TRY(call.start());
   const int slabs = (int)std::max<int64_t>(1, std::min<int64_t>(64, N / 256));
-  AM_LAUNCH(col_sum_kernel, dim3((unsigned)ceil_div(d, 128), (unsigned)slabs), 128, 0, st.s, dX.p, N, d, dM.p);
+  AM_LAUNCH(col_sum_kernel, dim3((unsigned)ceil_div(d, 128), (unsigned)slabs), 128, 0, st, dX, N, d, dM);
   std::vector<double> hm((size_t)d);
-  AM_CUDA(cudaMemcpyAsync(hm.data(), dM.p, (size_t)d * 8, cudaMemcpyDeviceToHost, st.s));
-  AM_CUDA(cudaStreamSynchronize(st.s));
+  AM_CUDA(cudaMemcpyAsync(hm.data(), dM, (size_t)d * 8, cudaMemcpyDeviceToHost, st));
+  AM_CUDA(cudaStreamSynchronize(st));
   for (int c = 0; c < d; ++c) hm[(size_t)c] /= (double)N;
-  AM_CUDA(cudaMemcpyAsync(dM.p, hm.data(), (size_t)d * 8, cudaMemcpyHostToDevice, st.s));
+  AM_CUDA(cudaMemcpyAsync(dM, hm.data(), (size_t)d * 8, cudaMemcpyHostToDevice, st));
   const int tiles = ceil_div(d, kCovTile);
   const int zs = (int)std::max<int64_t>(1, std::min<int64_t>(N / 512, (int64_t)4 * sm_count() / std::max(1, tiles * (tiles + 1) / 2)));
-  AM_LAUNCH(cov_kernel, dim3((unsigned)tiles, (unsigned)tiles, (unsigned)std::max(1, zs)), 256, 0, st.s, dX.p, N, d, dM.p, dC.p);
-  AM_LAUNCH(cov_finish_kernel, (unsigned)(((int64_t)d * d + 255) / 256), 256, 0, st.s, dC.p, d, 1.0 / (double)(N - 1));
-  AM_CUDA(cudaMemcpyAsync(cov, dC.p, (size_t)d * d * 8, cudaMemcpyDeviceToHost, st.s));
-  AM_CUDA(cudaStreamSynchronize(st.s));
+  AM_LAUNCH(cov_kernel, dim3((unsigned)tiles, (unsigned)tiles, (unsigned)std::max(1, zs)), 256, 0, st, dX, N, d, dM, dC);
+  AM_LAUNCH(cov_finish_kernel, (unsigned)(((int64_t)d * d + 255) / 256), 256, 0, st, dC, d, 1.0 / (double)(N - 1));
+  AM_TRY(call.finish());
   std::copy(hm.begin(), hm.end(), mean);
   return AM_OK;
 }
@@ -313,58 +311,51 @@ extern "C" int am_pca_moments(const float* X, int64_t N, int d, double* mean, do
 extern "C" int am_pca_project(const float* X, int64_t N, int d, const double* mean, const float* components, int k,
                               float* Y) {
   AM_CHECK(X && mean && components && Y && N >= 1 && d >= 1 && k >= 1 && d <= 8192, "am_pca_project: bad argument");
-  AM_TRY(ensure_init());
-  Stream st;
-  AM_TRY(st.create());
-  DevBuf<float> dX, dW, dY;
-  DevBuf<double> dM;
-  AM_TRY(dX.alloc((size_t)N * d));
-  AM_TRY(dM.alloc((size_t)d));
-  AM_TRY(dW.alloc((size_t)k * d));
-  AM_TRY(dY.alloc((size_t)N * k));
-  AM_CUDA(cudaMemcpyAsync(dX.p, X, (size_t)N * d * 4, cudaMemcpyHostToDevice, st.s));
-  AM_CUDA(cudaMemcpyAsync(dM.p, mean, (size_t)d * 8, cudaMemcpyHostToDevice, st.s));
-  AM_CUDA(cudaMemcpyAsync(dW.p, components, (size_t)k * d * 4, cudaMemcpyHostToDevice, st.s));
+  cudaStream_t st;
+  AM_TRY(HostCall::thread_stream(&st));
+  HostCall call(st, 0, HostCall::Memory::Owned);
+  float *dX, *dW, *dY;
+  double* dM;
+  call.up(&dX, X, (size_t)N * d);
+  call.up(&dM, mean, (size_t)d);
+  call.up(&dW, components, (size_t)k * d);
+  call.down(&dY, (size_t)N * k, Y);
+  AM_TRY(call.start());
   const size_t smem = (size_t)8 * d * 4;
   AM_CHECK(smem <= 200 * 1024, "am_pca_project: %d features do not fit the row buffer", d);
   AM_TRY(allow_dynamic_smem<pca_project_kernel>(200 * 1024));
   const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((N + 7) / 8, (int64_t)sm_count() * 8));
-  AM_LAUNCH(pca_project_kernel, grid, 256, smem, st.s, dX.p, N, d, dM.p, dW.p, k, dY.p);
-  AM_CUDA(cudaMemcpyAsync(Y, dY.p, (size_t)N * k * 4, cudaMemcpyDeviceToHost, st.s));
-  AM_CUDA(cudaStreamSynchronize(st.s));
-  return AM_OK;
+  AM_LAUNCH(pca_project_kernel, grid, 256, smem, st, dX, N, d, dM, dW, k, dY);
+  return call.finish();
 }
 
 extern "C" int am_dbscan(const float* X, int64_t N64, int d, double eps, int min_samples, int32_t* labels, int* n_clusters) {
   AM_CHECK(X && labels && N64 >= 1 && N64 <= (1 << 20) && d >= 1 && eps > 0.0 && eps * eps <= 3.0e38 && min_samples >= 1,
            "am_dbscan: bad argument (1 <= N <= 2^20, 0 < eps, eps^2 finite in float, min_samples >= 1)");
-  AM_TRY(ensure_init());
   const int N = (int)N64, words = (N + 31) / 32;
-  Stream st;
-  AM_TRY(st.create());
-  DevBuf<float> dX;
-  DevBuf<uint32_t> adj;
-  DevBuf<int> count, label, out;
-  DevBuf<unsigned char> core;
-  AM_TRY(dX.alloc((size_t)N * d));
-  AM_TRY(adj.alloc((size_t)N * words));
-  AM_TRY(count.alloc((size_t)N));
-  AM_TRY(label.alloc((size_t)N));
-  AM_TRY(out.alloc((size_t)N));
-  AM_TRY(core.alloc((size_t)N));
-  AM_CUDA(cudaMemcpyAsync(dX.p, X, (size_t)N * d * 4, cudaMemcpyHostToDevice, st.s));
-  AM_CUDA(cudaMemsetAsync(count.p, 0, (size_t)N * 4, st.s));
-  AM_CUDA(cudaMemsetAsync(adj.p, 0, (size_t)N * words * 4, st.s));
+  cudaStream_t st;
+  AM_TRY(HostCall::thread_stream(&st));
+  HostCall call(st, 0, HostCall::Memory::Owned);
+  std::vector<int> h((size_t)N);
+  float* dX;
+  uint32_t* adj;
+  int *count, *label, *out;
+  unsigned char* core;
+  call.up(&dX, X, (size_t)N * d);
+  call.down(&out, (size_t)N, h.data());
+  call.device(&adj, (size_t)N * words, 0);
+  call.device(&count, (size_t)N, 0);
+  call.device(&label, (size_t)N);
+  call.device(&core, (size_t)N);
+  AM_TRY(call.start());
   const unsigned tiles = (unsigned)ceil_div(N, kDbTile);
   const double eps2 = eps * eps;
-  AM_LAUNCH(dbscan_adj_kernel, dim3(tiles, tiles), 256, 0, st.s, dX.p, N, d, (float)eps2, eps2, adj.p, words, count.p);
-  AM_LAUNCH(dbscan_init_kernel, (unsigned)ceil_div(N, 256), 256, 0, st.s, count.p, N, min_samples, label.p, core.p);
-  AM_LAUNCH(dbscan_hook_kernel, (unsigned)ceil_div(N, 8), 256, 0, st.s, adj.p, words, N, core.p, label.p);
-  AM_LAUNCH(dbscan_compress_kernel, (unsigned)ceil_div(N, 256), 256, 0, st.s, N, core.p, label.p);
-  AM_LAUNCH(dbscan_border_kernel, (unsigned)ceil_div(N, 8), 256, 0, st.s, adj.p, words, N, core.p, label.p, out.p);
-  std::vector<int> h((size_t)N);
-  AM_CUDA(cudaMemcpyAsync(h.data(), out.p, (size_t)N * 4, cudaMemcpyDeviceToHost, st.s));
-  AM_CUDA(cudaStreamSynchronize(st.s));
+  AM_LAUNCH(dbscan_adj_kernel, dim3(tiles, tiles), 256, 0, st, dX, N, d, (float)eps2, eps2, adj, words, count);
+  AM_LAUNCH(dbscan_init_kernel, (unsigned)ceil_div(N, 256), 256, 0, st, count, N, min_samples, label, core);
+  AM_LAUNCH(dbscan_hook_kernel, (unsigned)ceil_div(N, 8), 256, 0, st, adj, words, N, core, label);
+  AM_LAUNCH(dbscan_compress_kernel, (unsigned)ceil_div(N, 256), 256, 0, st, N, core, label);
+  AM_LAUNCH(dbscan_border_kernel, (unsigned)ceil_div(N, 8), 256, 0, st, adj, words, N, core, label, out);
+  AM_TRY(call.finish());
   // component labels are the lowest core index of each component: number them in that order (scikit-learn's numbering)
   std::vector<int> roots;
   for (int i = 0; i < N; ++i)

@@ -28,6 +28,7 @@
 //   seg_dist_kernel           per-label sums of ||x - c|| and ||x - c||^2
 //   host                      the L x L centroid step and scikit-learn's special cases.
 #include "gemm_wgmma.cuh"
+#include "host_call.cuh"
 #include "split_bf16.cuh"
 #include "tma_pipeline.cuh"
 
@@ -332,23 +333,20 @@ extern "C" int am_cluster_scores(const float* X, int64_t N, int d, const int32_t
     for (int c = 0; c < L; ++c)
       std::fill(seg.begin() + off[(size_t)c], seg.begin() + off[(size_t)c + 1], c);
   }
-  AM_TRY(ensure_init());
+  cudaStream_t st;
+  AM_TRY(HostCall::thread_stream(&st));
   AM_CHECK(!sil || gemm::available(), "am_cluster_scores: the silhouette kernel needs an sm_90 device with TMA");
-  Stream st;
-  AM_TRY(st.create());
-  DevBuf<float> dX, dXp;
-  DevBuf<int32_t> dPerm, dSeg, dOff;
-  AM_TRY(dX.alloc((size_t)N * d));
-  AM_TRY(dXp.alloc((size_t)N * d));
-  AM_TRY(dPerm.alloc((size_t)N));
-  AM_TRY(dSeg.alloc((size_t)N));
-  AM_TRY(dOff.alloc((size_t)L + 1));
-  AM_CUDA(cudaMemcpyAsync(dX.p, X, (size_t)N * d * 4, cudaMemcpyHostToDevice, st.s));
-  AM_CUDA(cudaMemcpyAsync(dPerm.p, perm.data(), (size_t)N * 4, cudaMemcpyHostToDevice, st.s));
-  AM_CUDA(cudaMemcpyAsync(dSeg.p, seg.data(), (size_t)N * 4, cudaMemcpyHostToDevice, st.s));
-  AM_CUDA(cudaMemcpyAsync(dOff.p, off.data(), ((size_t)L + 1) * 4, cudaMemcpyHostToDevice, st.s));
+  HostCall call(st, 0, HostCall::Memory::Owned);
+  float *dX, *dXp;
+  int32_t *dPerm, *dSeg, *dOff;
+  call.up(&dX, X, (size_t)N * d);
+  call.up(&dPerm, perm.data(), (size_t)N);
+  call.up(&dSeg, seg.data(), (size_t)N);
+  call.up(&dOff, off.data(), (size_t)L + 1);
+  call.device(&dXp, (size_t)N * d);
+  AM_TRY(call.start());
   const int row_grid = (int)std::max<int64_t>(1, std::min<int64_t>((N + 7) / 8, (int64_t)sm_count() * 16));
-  AM_LAUNCH(gather_rows_kernel, row_grid, 256, 0, st.s, dX.p, N, d, dPerm.p, dXp.p);
+  AM_LAUNCH(gather_rows_kernel, row_grid, 256, 0, st, dX, N, d, dPerm, dXp);
 
   if (sil) {
     const int dp = (int)round_up((size_t)d, 64);
@@ -360,9 +358,9 @@ extern "C" int am_cluster_scores(const float* X, int64_t N, int d, const int32_t
     AM_TRY(dSamples.alloc((size_t)N));
     AM_TRY(S.alloc((size_t)N * L));
     AM_TRY(total.alloc(1));
-    AM_CUDA(cudaMemsetAsync(S.p, 0, (size_t)N * L * 8, st.s));
-    AM_CUDA(cudaMemsetAsync(total.p, 0, 8, st.s));
-    AM_LAUNCH(split_rows_kernel, row_grid, 256, 0, st.s, dXp.p, N, d, dp, Xs.p, nullptr);
+    AM_CUDA(cudaMemsetAsync(S.p, 0, (size_t)N * L * 8, st));
+    AM_CUDA(cudaMemsetAsync(total.p, 0, 8, st));
+    AM_LAUNCH(split_rows_kernel, row_grid, 256, 0, st, dXp, N, d, dp, Xs.p, nullptr);
     CUtensorMap map;
     AM_TRY(gemm::encode_map_bf16(&map, Xs.p, 2 * dp, N, 2 * dp, kTile));
     SilArgs a{};
@@ -376,19 +374,19 @@ extern "C" int am_cluster_scores(const float* X, int64_t N, int d, const int32_t
     a.blocks_per_split = (a.col_blocks + splits - 1) / splits;
     splits = (a.col_blocks + a.blocks_per_split - 1) / a.blocks_per_split;  // every split non-empty
     a.xn = xn.p;
-    a.seg = dSeg.p;
-    a.off = dOff.p;
+    a.seg = dSeg;
+    a.off = dOff;
     a.S = S.p;
     AM_TRY(allow_dynamic_smem<silhouette_tc_kernel<true>>(kSmem));
     AM_TRY(allow_dynamic_smem<silhouette_tc_kernel<false>>(kSmem));
-    AM_LAUNCH(silhouette_tc_kernel<true>, dim3((unsigned)tiles, 1u), kThreads, kSmem, st.s, map, a);
-    AM_LAUNCH(silhouette_tc_kernel<false>, dim3((unsigned)tiles, (unsigned)splits), kThreads, kSmem, st.s, map, a);
-    AM_LAUNCH(silhouette_finish_kernel, row_grid, 256, 0, st.s, S.p, N, L, dSeg.p, dOff.p, dPerm.p, dSamples.p,
+    AM_LAUNCH(silhouette_tc_kernel<true>, dim3((unsigned)tiles, 1u), kThreads, kSmem, st, map, a);
+    AM_LAUNCH(silhouette_tc_kernel<false>, dim3((unsigned)tiles, (unsigned)splits), kThreads, kSmem, st, map, a);
+    AM_LAUNCH(silhouette_finish_kernel, row_grid, 256, 0, st, S.p, N, L, dSeg, dOff, dPerm, dSamples.p,
               total.p);
     double t = 0.0;
-    AM_CUDA(cudaMemcpyAsync(&t, total.p, 8, cudaMemcpyDeviceToHost, st.s));
-    if (samples) AM_CUDA(cudaMemcpyAsync(samples, dSamples.p, (size_t)N * 4, cudaMemcpyDeviceToHost, st.s));
-    AM_CUDA(cudaStreamSynchronize(st.s));
+    AM_CUDA(cudaMemcpyAsync(&t, total.p, 8, cudaMemcpyDeviceToHost, st));
+    if (samples) AM_CUDA(cudaMemcpyAsync(samples, dSamples.p, (size_t)N * 4, cudaMemcpyDeviceToHost, st));
+    AM_CUDA(cudaStreamSynchronize(st));
     scores[0] = t / (double)N;
   }
 
@@ -397,23 +395,23 @@ extern "C" int am_cluster_scores(const float* X, int64_t N, int d, const int32_t
     AM_TRY(cent.alloc((size_t)L * d));
     AM_TRY(dsum.alloc((size_t)L));
     AM_TRY(dsq.alloc((size_t)L));
-    AM_CUDA(cudaMemsetAsync(cent.p, 0, (size_t)L * d * 8, st.s));
-    AM_CUDA(cudaMemsetAsync(dsum.p, 0, (size_t)L * 8, st.s));
-    AM_CUDA(cudaMemsetAsync(dsq.p, 0, (size_t)L * 8, st.s));
+    AM_CUDA(cudaMemsetAsync(cent.p, 0, (size_t)L * d * 8, st));
+    AM_CUDA(cudaMemsetAsync(dsum.p, 0, (size_t)L * 8, st));
+    AM_CUDA(cudaMemsetAsync(dsq.p, 0, (size_t)L * 8, st));
     const int slabs = (int)std::max<int64_t>(1, std::min<int64_t>(1024, N / 64));
-    AM_LAUNCH(seg_col_sum_kernel, dim3((unsigned)ceil_div(d, 128), (unsigned)slabs), 128, 0, st.s, dXp.p, N, d,
-              dSeg.p, cent.p);
-    AM_LAUNCH(centroid_kernel, (unsigned)(((int64_t)L * d + 255) / 256), 256, 0, st.s, cent.p, L, d, dOff.p);
+    AM_LAUNCH(seg_col_sum_kernel, dim3((unsigned)ceil_div(d, 128), (unsigned)slabs), 128, 0, st, dXp, N, d,
+              dSeg, cent.p);
+    AM_LAUNCH(centroid_kernel, (unsigned)(((int64_t)L * d + 255) / 256), 256, 0, st, cent.p, L, d, dOff);
     const int64_t warps = (int64_t)sm_count() * 64;
     const int64_t chunk = std::max<int64_t>(1, (N + warps - 1) / warps);
     const int64_t used = (N + chunk - 1) / chunk;
-    AM_LAUNCH(seg_dist_kernel, (unsigned)((used + 7) / 8), 256, 0, st.s, dXp.p, N, d, dSeg.p, cent.p, chunk, dsum.p,
+    AM_LAUNCH(seg_dist_kernel, (unsigned)((used + 7) / 8), 256, 0, st, dXp, N, d, dSeg, cent.p, chunk, dsum.p,
               dsq.p);
     std::vector<double> hc((size_t)L * d), hs((size_t)L), hq((size_t)L);
-    AM_CUDA(cudaMemcpyAsync(hc.data(), cent.p, (size_t)L * d * 8, cudaMemcpyDeviceToHost, st.s));
-    AM_CUDA(cudaMemcpyAsync(hs.data(), dsum.p, (size_t)L * 8, cudaMemcpyDeviceToHost, st.s));
-    AM_CUDA(cudaMemcpyAsync(hq.data(), dsq.p, (size_t)L * 8, cudaMemcpyDeviceToHost, st.s));
-    AM_CUDA(cudaStreamSynchronize(st.s));
+    AM_CUDA(cudaMemcpyAsync(hc.data(), cent.p, (size_t)L * d * 8, cudaMemcpyDeviceToHost, st));
+    AM_CUDA(cudaMemcpyAsync(hs.data(), dsum.p, (size_t)L * 8, cudaMemcpyDeviceToHost, st));
+    AM_CUDA(cudaMemcpyAsync(hq.data(), dsq.p, (size_t)L * 8, cudaMemcpyDeviceToHost, st));
+    AM_CUDA(cudaStreamSynchronize(st));
     if (which & 4) {  // sklearn.metrics.calinski_harabasz_score
       std::vector<double> mean((size_t)d, 0.0);
       for (int k = 0; k < L; ++k) {

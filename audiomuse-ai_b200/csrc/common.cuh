@@ -125,32 +125,6 @@ struct PinnedBuf {
   }
 };
 
-// stream-ordered scratch (cudaMallocAsync pool): no device-wide sync on alloc/free, so hot entry
-// points stay re-entrant without paying cudaMalloc/cudaFree per call
-template <typename T>
-struct AsyncBuf {
-  T* p = nullptr;
-  cudaStream_t st = nullptr;
-  AsyncBuf() = default;
-  AsyncBuf(const AsyncBuf&) = delete;
-  AsyncBuf& operator=(const AsyncBuf&) = delete;
-  ~AsyncBuf() {
-    if (p) cudaFreeAsync(p, st);
-  }
-  int alloc(size_t count, cudaStream_t stream) {
-    if (p) cudaFreeAsync(p, st);
-    p = nullptr;
-    st = stream;
-    if (count == 0) return AM_OK;
-    cudaError_t e = cudaMallocAsync(&p, count * sizeof(T), stream);
-    if (e != cudaSuccess) {
-      p = nullptr;
-      return cuda_fail(e, "cudaMallocAsync", __FILE__, __LINE__);
-    }
-    return AM_OK;
-  }
-};
-
 struct Stream {
   cudaStream_t s = nullptr;
   ~Stream() {

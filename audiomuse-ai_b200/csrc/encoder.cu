@@ -13,6 +13,7 @@
 // (bn0 + pad + 3x3 stride-2 on the single input channel + 1x1 + BN + ReLU6) reads the fp32
 // log-mel directly and is computed in fp32.  The head (<= 2.5 MMAC per window) runs in fp32.
 #include "common.cuh"
+#include "host_call.cuh"
 
 #include <algorithm>
 #include <cmath>
@@ -1157,16 +1158,13 @@ extern "C" int am_clap_embed(am_model* m, const float* mel, int B, int T, float*
   AM_CHECK(m && mel && out, "am_clap_embed: NULL argument");
   AM_CHECK(B >= 0 && T > 0, "am_clap_embed: bad shape B=%d T=%d", B, T);
   if (B == 0) return AM_OK;
-  DevBuf<float> d_mel, d_out;
-  const size_t mel_elems = (size_t)B * m->n_mels * T;
-  AM_TRY(d_mel.alloc(mel_elems));
-  AM_TRY(d_out.alloc((size_t)B * m->emb));
-  cudaStream_t st = m->stream.s;
-  AM_CUDA(cudaMemcpyAsync(d_mel.p, mel, mel_elems * 4, cudaMemcpyHostToDevice, st));
-  AM_TRY(am_clap_embed_dev(m, d_mel.p, B, T, d_out.p, st));
-  AM_CUDA(cudaMemcpyAsync(out, d_out.p, (size_t)B * m->emb * 4, cudaMemcpyDeviceToHost, st));
-  AM_CUDA(cudaStreamSynchronize(st));
-  return AM_OK;
+  HostCall call(m->stream.s, 0, HostCall::Memory::Owned);
+  float *d_mel, *d_out;
+  call.up(&d_mel, mel, (size_t)B * m->n_mels * T);
+  call.down(&d_out, (size_t)B * m->emb, out);
+  AM_TRY(call.start());
+  AM_TRY(am_clap_embed_dev(m, d_mel, B, T, d_out, m->stream.s));
+  return call.finish();
 }
 
 extern "C" int am_clap_embed_tracks_dev(am_model* m, const am_mel_plan* plan, const int16_t* pcm_dev, int n_samples,

@@ -16,6 +16,7 @@
 //                                      so a resampled waveform never returns to the host.
 // Other containers (mp3 / flac / ogg ...) stay with the reference's own loader (pydub / ffmpeg): decode stays on host.
 #include "common.cuh"
+#include "host_call.cuh"
 
 #include <algorithm>
 #include <cmath>
@@ -366,16 +367,15 @@ extern "C" int am_resample(const float* x, int64_t n_in, int sr_in, int sr_out, 
   }
   *n_out = resample_out_len(p, n_in);
   AM_CHECK(cap >= *n_out, "am_resample: output buffer of %lld samples, need %lld", (long long)cap, (long long)*n_out);
-  static thread_local Stream st;
-  AM_TRY(st.create());
-  AsyncBuf<float> dx, dy;
-  AM_TRY(dx.alloc((size_t)n_in, st.s));
-  AM_TRY(dy.alloc((size_t)*n_out, st.s));
-  AM_CUDA(cudaMemcpyAsync(dx.p, x, (size_t)n_in * 4, cudaMemcpyHostToDevice, st.s));
-  AM_TRY(resample_dev(p, dx.p, n_in, dy.p, st.s));
-  AM_CUDA(cudaMemcpyAsync(y, dy.p, (size_t)*n_out * 4, cudaMemcpyDeviceToHost, st.s));
-  AM_CUDA(cudaStreamSynchronize(st.s));
-  return AM_OK;
+  cudaStream_t st;
+  AM_TRY(HostCall::thread_stream(&st));
+  HostCall call(st, 0, HostCall::Memory::Pool);
+  float *dx, *dy;
+  call.up(&dx, x, (size_t)n_in);
+  call.down(&dy, (size_t)*n_out, y);
+  AM_TRY(call.start());
+  AM_TRY(resample_dev(p, dx, n_in, dy, st));
+  return call.finish();
 }
 
 // windows a waveform of L samples produces (clap_analyzer.py:510-521): 1 when L <= 480000, else the regular windows

@@ -35,6 +35,7 @@
 // Every reduction runs in a fixed order and no floating-point atomics are used, so two calls give bit-identical
 // results.
 #include "common.cuh"
+#include "host_call.cuh"
 
 #include <algorithm>
 #include <cmath>
@@ -821,7 +822,6 @@ extern "C" int am_gmm_fit(const double* X, int64_t N, int d, int K, int type, in
   const int64_t per_init = 1 + (int64_t)(K - 1) * L;
   AM_CHECK(n_draws >= n_init * per_init, "am_gmm_fit: %lld draws, K = %d with n_init = %d needs %lld",
            (long long)n_draws, K, n_init, (long long)(n_init * per_init));
-  AM_TRY(ensure_init());
   const bool full = type == AM_GMM_FULL, tied = type == AM_GMM_TIED, sph = type == AM_GMM_SPHERICAL;
   const bool lin = type == AM_GMM_DIAG || sph;       // the E-step is one product of the rows with per-component columns
 
@@ -860,9 +860,8 @@ extern "C" int am_gmm_fit(const double* X, int64_t N, int d, int K, int type, in
   const int Sm = split((int64_t)(Cp / kTile) * (d64 / kTile), mchunk);
   const int Sc = split((int64_t)(tied ? 1 : C) * cov_tiles, cchunk);   // tied: the one X^T X
 
-  Stream st;
-  AM_TRY(st.create());
-  cudaStream_t s = st.s;
+  cudaStream_t s;
+  AM_TRY(HostCall::thread_stream(&s));
   constexpr int kEv = 12;
   cudaEvent_t ev[kEv] = {};
   struct EvGuard {
@@ -878,68 +877,53 @@ extern "C" int am_gmm_fit(const double* X, int64_t N, int d, int K, int type, in
   const size_t cov_n = full ? (size_t)C * dp * dp : tied ? (size_t)n_init * dp * dp : sph ? (size_t)C : (size_t)C * dp;
   const size_t out_n = full ? (size_t)K * d * d : tied ? (size_t)d * d : sph ? (size_t)K : (size_t)K * d;
   const size_t pack_n = std::max(out_n, (size_t)K * d);   // dOut also stages the means
-  DevBuf<double> dX, dXsq, dResp, dClose, dCums, dDist, dPart, dNk, dW, dLogw, dLogdet, dMeans, dMP, dCov, dLw, dPrec,
-      dLpn, dLb, dPm, dPc, dOut;
-  DevBuf<double> dX2, dPm2, dWcol, dCst, dScale, dXtX, dUnit, dZero;   // diag / spherical / tied only
-  DevBuf<int> dCand, dIdx, dActive, dFail, dOn;
-  DevBuf<int64_t> dLab;
-  AM_TRY(dX.alloc((size_t)Np * dp));
-  AM_TRY(dXsq.alloc((size_t)Np));
-  AM_TRY(dResp.alloc((size_t)C * Np));
-  AM_TRY(dClose.alloc((size_t)n_init * Np));
-  AM_TRY(dCums.alloc((size_t)n_init * Np));
-  AM_TRY(dDist.alloc((size_t)n_init * kMaxTrials * Np));
-  AM_TRY(dPart.alloc((size_t)n_init * kMaxTrials * nb_kpp));
-  AM_TRY(dNk.alloc(C));
-  AM_TRY(dW.alloc(C));
-  AM_TRY(dLogw.alloc(C));
-  AM_TRY(dLogdet.alloc(C));
-  AM_TRY(dMeans.alloc((size_t)C * dp));
-  AM_TRY(dCov.alloc(cov_n));
-  AM_TRY(dPrec.alloc(cov_n));
-  AM_TRY(dLpn.alloc((size_t)n_init * Np));
-  AM_TRY(dLb.alloc(n_init));
-  AM_TRY(dPm.alloc((size_t)Sm * Cp * d64));
-  AM_TRY(dOut.alloc(pack_n));
-  AM_TRY(dCand.alloc((size_t)n_init * kMaxTrials));
-  AM_TRY(dIdx.alloc(C));
-  AM_TRY(dActive.alloc(n_init));
-  AM_TRY(dFail.alloc(1));
-  AM_TRY(dLab.alloc((size_t)N));
-  if (full || tied) {
-    AM_TRY(dMP.alloc((size_t)C * dp));
-    AM_TRY(dLw.alloc(cov_n));
-    AM_TRY(dPc.alloc((size_t)Sc * (tied ? 1 : C) * d64 * d64));
-  }
-  if (lin) {
-    AM_TRY(dX2.alloc((size_t)Np * dp));
-    AM_TRY(dPm2.alloc((size_t)Sm * Cp * d64));
-    AM_TRY(dCst.alloc(C));
-    if (sph) AM_TRY(dScale.alloc(C));
-    else AM_TRY(dWcol.alloc((size_t)C * ka));
-  }
-  if (tied) {
-    AM_TRY(dXtX.alloc((size_t)dp * dp));
-    AM_TRY(dUnit.alloc((size_t)Np));
-    AM_TRY(dZero.alloc((size_t)dp));
-    AM_TRY(dOn.alloc(1));
-  }
-
-  AM_CUDA(cudaMemsetAsync(dX.p, 0, dX.n * 8, s));
-  AM_CUDA(cudaMemcpy2DAsync(dX.p, (size_t)dp * 8, X, (size_t)d * 8, (size_t)d * 8, (size_t)N, cudaMemcpyHostToDevice, s));
-  AM_CUDA(cudaMemsetAsync(dXsq.p, 0, dXsq.n * 8, s));
-  AM_CUDA(cudaMemsetAsync(dMeans.p, 0, dMeans.n * 8, s));
-  if (dMP.p) AM_CUDA(cudaMemsetAsync(dMP.p, 0, dMP.n * 8, s));
-  AM_CUDA(cudaMemsetAsync(dPrec.p, 0, dPrec.n * 8, s));
-  if (dPc.p) AM_CUDA(cudaMemsetAsync(dPc.p, 0, dPc.n * 8, s));
-  if (dWcol.p) AM_CUDA(cudaMemsetAsync(dWcol.p, 0, dWcol.n * 8, s));
-  AM_CUDA(cudaMemsetAsync(dFail.p, 0, 4, s));
-  AM_CUDA(cudaMemcpyAsync(dCand.p, cand0.data(), cand0.size() * 4, cudaMemcpyHostToDevice, s));
-  DevBuf<double> dDraws;
-  AM_TRY(dDraws.alloc((size_t)n_init * per_init));
-  AM_CUDA(cudaMemcpyAsync(dDraws.p, draws, (size_t)n_init * per_init * 8, cudaMemcpyHostToDevice, s));
+  const size_t x_n = (size_t)Np * dp, close_n = (size_t)n_init * Np;
   std::vector<int> act(n_init, 1);
-  AM_CUDA(cudaMemcpyAsync(dActive.p, act.data(), n_init * 4, cudaMemcpyHostToDevice, s));
+  const int one = 1;
+  HostCall call(s, 0, HostCall::Memory::Owned);
+  double *dX, *dXsq, *dResp, *dClose, *dCums, *dDist, *dPart, *dNk, *dW, *dLogw, *dLogdet, *dMeans, *dMP, *dCov, *dLw,
+      *dPrec, *dLpn, *dLb, *dPm, *dPc, *dOut, *dDraws;
+  double *dX2, *dPm2, *dWcol, *dCst, *dScale, *dXtX, *dUnit, *dZero;   // diag / spherical / tied only
+  int *dCand, *dIdx, *dActive, *dFail, *dOn;
+  int64_t* dLab;
+  call.up(&dCand, cand0.data(), cand0.size());
+  call.up(&dDraws, draws, (size_t)n_init * per_init);
+  call.up(&dActive, act.data(), (size_t)n_init);
+  call.up(&dOn, &one, tied ? 1 : 0);
+  call.down(&dLab, (size_t)N, labels);
+  call.device(&dX, x_n, 0);   // the rows are copied in after start(), pitched
+  call.device(&dXsq, (size_t)Np, 0);
+  call.device(&dMeans, (size_t)C * dp, 0);
+  call.device(&dMP, full || tied ? (size_t)C * dp : 0, 0);
+  call.device(&dPrec, cov_n, 0);
+  call.device(&dPc, full || tied ? (size_t)Sc * (tied ? 1 : C) * d64 * d64 : 0, 0);
+  call.device(&dWcol, lin && !sph ? (size_t)C * ka : 0, 0);
+  call.device(&dFail, 1, 0);
+  call.device(&dResp, (size_t)C * Np, 0);
+  call.device(&dZero, tied ? (size_t)dp : 0, 0);
+  call.device(&dClose, close_n);
+  call.device(&dCums, (size_t)n_init * Np);
+  call.device(&dDist, (size_t)n_init * kMaxTrials * Np);
+  call.device(&dPart, (size_t)n_init * kMaxTrials * nb_kpp);
+  call.device(&dNk, (size_t)C);
+  call.device(&dW, (size_t)C);
+  call.device(&dLogw, (size_t)C);
+  call.device(&dLogdet, (size_t)C);
+  call.device(&dCov, cov_n);
+  call.device(&dLpn, (size_t)n_init * Np);
+  call.device(&dLb, (size_t)n_init);
+  call.device(&dPm, (size_t)Sm * Cp * d64);
+  call.device(&dOut, pack_n);
+  call.device(&dIdx, (size_t)C);
+  call.device(&dLw, full || tied ? cov_n : 0);
+  call.device(&dX2, lin ? x_n : 0);
+  call.device(&dPm2, lin ? (size_t)Sm * Cp * d64 : 0);
+  call.device(&dCst, lin ? (size_t)C : 0);
+  call.device(&dScale, sph ? (size_t)C : 0);
+  call.device(&dXtX, tied ? (size_t)dp * dp : 0);
+  call.device(&dUnit, tied ? (size_t)Np : 0);
+  AM_TRY(call.start());
+  AM_CUDA(cudaMemcpy2DAsync(dX, (size_t)dp * 8, X, (size_t)d * 8, (size_t)d * 8, (size_t)N, cudaMemcpyHostToDevice, s));
 
   const size_t chol_smem = ((size_t)kPanel * dp + (size_t)dp * (kPanel + 1)) * 8;
   const size_t trinv_smem = (size_t)dp * kPanel * 8;
@@ -952,84 +936,80 @@ extern "C" int am_gmm_fit(const double* X, int64_t N, int d, int K, int type, in
 
   // ---- k-means++
   AM_CUDA(cudaEventRecord(ev[0], s));
-  AM_LAUNCH(rownorm_kernel, grid_for(N * 32), kThreads, 0, s, dX.p, N, dp, dXsq.p);
-  AM_LAUNCH(fill_kernel, grid_for(dClose.n), 256, 0, s, dClose.p, (int64_t)dClose.n, (double)INFINITY);
+  AM_LAUNCH(rownorm_kernel, grid_for(N * 32), kThreads, 0, s, dX, N, dp, dXsq);
+  AM_LAUNCH(fill_kernel, grid_for(close_n), 256, 0, s, dClose, (int64_t)close_n, (double)INFINITY);
   for (int cc = 0; cc < K; ++cc) {
     const int Lc = cc == 0 ? 1 : L;
-    AM_LAUNCH(kpp_dist_kernel, dim3(nb_kpp, n_init), kThreads, (size_t)Lc * dp * 8, s, dX.p, N, Np, dp, dXsq.p,
-              dCand.p, Lc, dClose.p, dDist.p, dPart.p);
-    AM_LAUNCH(kpp_pick_kernel, n_init, kPickThreads, 0, s, N, Np, K, cc, Lc, nb_kpp, dPart.p, dDist.p, dClose.p,
-              dCums.p, dCand.p, dIdx.p, dDraws.p, per_init, L);
+    AM_LAUNCH(kpp_dist_kernel, dim3(nb_kpp, n_init), kThreads, (size_t)Lc * dp * 8, s, dX, N, Np, dp, dXsq,
+              dCand, Lc, dClose, dDist, dPart);
+    AM_LAUNCH(kpp_pick_kernel, n_init, kPickThreads, 0, s, N, Np, K, cc, Lc, nb_kpp, dPart, dDist, dClose,
+              dCums, dCand, dIdx, dDraws, per_init, L);
   }
-  AM_CUDA(cudaMemsetAsync(dResp.p, 0, dResp.n * 8, s));
-  AM_LAUNCH(onehot_kernel, ceil_div(C, 256), 256, 0, s, dIdx.p, C, Np, dResp.p);
-  if (lin) AM_LAUNCH(square_kernel, grid_for(dX.n), 256, 0, s, dX.p, (int64_t)dX.n, dX2.p);
+  AM_LAUNCH(onehot_kernel, ceil_div(C, 256), 256, 0, s, dIdx, C, Np, dResp);
+  if (lin) AM_LAUNCH(square_kernel, grid_for(x_n), 256, 0, s, dX, (int64_t)x_n, dX2);
   if (tied) {   // X^T X over all rows, unweighted: gram_kernel<true> with one component, unit weights, zero mean
-    AM_LAUNCH(fill_kernel, grid_for(Np), 256, 0, s, dUnit.p, Np, 1.0);
-    AM_CUDA(cudaMemsetAsync(dZero.p, 0, dZero.n * 8, s));
-    const int one = 1;
-    AM_CUDA(cudaMemcpyAsync(dOn.p, &one, 4, cudaMemcpyHostToDevice, s));
-    AM_LAUNCH(gram_kernel<true>, dim3(1, cov_tiles, Sc), kThreads, 0, s, dX.p, dUnit.p, dZero.p, Np, dp, 1, 1, dOn.p,
-              cchunk, dPc.p);
-    AM_LAUNCH(cov_reduce_kernel, dim3(1, d), 256, 0, s, dPc.p, Sc, 1, d64, d, dp, 1, dOn.p, dUnit.p, 0.0, dXtX.p);
+    AM_LAUNCH(fill_kernel, grid_for(Np), 256, 0, s, dUnit, Np, 1.0);
+    AM_LAUNCH(gram_kernel<true>, dim3(1, cov_tiles, Sc), kThreads, 0, s, dX, dUnit, dZero, Np, dp, 1, 1, dOn,
+              cchunk, dPc);
+    AM_LAUNCH(cov_reduce_kernel, dim3(1, d), 256, 0, s, dPc, Sc, 1, d64, d, dp, 1, dOn, dUnit, 0.0, dXtX);
   }
   AM_CUDA(cudaEventRecord(ev[1], s));
 
   // ---- M-step (init = true: the initialisation's weights nk / N) and the precision factors
   auto mstep = [&](bool init, cudaEvent_t e_mid) -> int {
-    AM_LAUNCH(nk_kernel, C, kThreads, 0, s, dResp.p, Np, K, dActive.p, dNk.p);
-    AM_LAUNCH(gram_kernel<false>, dim3(Cp / kTile, d64 / kTile, Sm), kThreads, 0, s, dX.p, dResp.p, dMeans.p, Np, dp,
-              C, K, dActive.p, mchunk, dPm.p);
-    AM_LAUNCH(means_reduce_kernel, C, d64, 0, s, dPm.p, Sm, Cp, d64, dp, K, dActive.p, dNk.p, dMeans.p);
+    AM_LAUNCH(nk_kernel, C, kThreads, 0, s, dResp, Np, K, dActive, dNk);
+    AM_LAUNCH(gram_kernel<false>, dim3(Cp / kTile, d64 / kTile, Sm), kThreads, 0, s, dX, dResp, dMeans, Np, dp,
+              C, K, dActive, mchunk, dPm);
+    AM_LAUNCH(means_reduce_kernel, C, d64, 0, s, dPm, Sm, Cp, d64, dp, K, dActive, dNk, dMeans);
     if (full) {
-      AM_LAUNCH(gram_kernel<true>, dim3(C, cov_tiles, Sc), kThreads, 0, s, dX.p, dResp.p, dMeans.p, Np, dp, C, K,
-                dActive.p, cchunk, dPc.p);
-      AM_LAUNCH(cov_reduce_kernel, dim3(C, d), 256, 0, s, dPc.p, Sc, C, d64, d, dp, K, dActive.p, dNk.p, reg_covar,
-                dCov.p);
+      AM_LAUNCH(gram_kernel<true>, dim3(C, cov_tiles, Sc), kThreads, 0, s, dX, dResp, dMeans, Np, dp, C, K,
+                dActive, cchunk, dPc);
+      AM_LAUNCH(cov_reduce_kernel, dim3(C, d), 256, 0, s, dPc, Sc, C, d64, d, dp, K, dActive, dNk, reg_covar,
+                dCov);
     } else if (tied) {
-      AM_LAUNCH(tied_cov_kernel, dim3(n_init, d), kThreads, 0, s, dXtX.p, d, dp, K, dActive.p, dNk.p, dMeans.p,
-                reg_covar, dCov.p);
+      AM_LAUNCH(tied_cov_kernel, dim3(n_init, d), kThreads, 0, s, dXtX, d, dp, K, dActive, dNk, dMeans,
+                reg_covar, dCov);
     } else {
-      AM_LAUNCH(gram_kernel<false>, dim3(Cp / kTile, d64 / kTile, Sm), kThreads, 0, s, dX2.p, dResp.p, dMeans.p, Np,
-                dp, C, K, dActive.p, mchunk, dPm2.p);
+      AM_LAUNCH(gram_kernel<false>, dim3(Cp / kTile, d64 / kTile, Sm), kThreads, 0, s, dX2, dResp, dMeans, Np,
+                dp, C, K, dActive, mchunk, dPm2);
     }
-    AM_LAUNCH(weights_kernel, ceil_div(n_init, 64), 64, 0, s, dNk.p, n_init, K, dActive.p, init ? (double)N : 0.0,
-              dW.p);
+    AM_LAUNCH(weights_kernel, ceil_div(n_init, 64), 64, 0, s, dNk, n_init, K, dActive, init ? (double)N : 0.0,
+              dW);
     AM_CUDA(cudaEventRecord(e_mid, s));
     if (lin) {
-      AM_LAUNCH(diag_cov_kernel, C, kThreads, 0, s, sph, dPm2.p, Sm, Cp, d64, d, dp, K, dActive.p, dNk.p, dMeans.p, dW.p, reg_covar,
-                dCov.p, dPrec.p, dWcol.p, dCst.p, dScale.p, dLogdet.p, dLogw.p, dFail.p);
+      AM_LAUNCH(diag_cov_kernel, C, kThreads, 0, s, sph, dPm2, Sm, Cp, d64, d, dp, K, dActive, dNk, dMeans, dW, reg_covar,
+                dCov, dPrec, dWcol, dCst, dScale, dLogdet, dLogw, dFail);
       return AM_OK;
     }
     const int kc = full ? K : 1;                     // components per covariance matrix's active flag
-    AM_LAUNCH(chol_kernel, Cm, kThreads, chol_smem, s, dCov.p, d, dp, kc, dActive.p, dLw.p, dFail.p);
-    AM_LAUNCH(trinv_kernel, dim3(Cm, ceil_div(d, kPanel)), kThreads, trinv_smem, s, dLw.p, d, dp, kc, dActive.p,
-              dFail.p, dPrec.p);
+    AM_LAUNCH(chol_kernel, Cm, kThreads, chol_smem, s, dCov, d, dp, kc, dActive, dLw, dFail);
+    AM_LAUNCH(trinv_kernel, dim3(Cm, ceil_div(d, kPanel)), kThreads, trinv_smem, s, dLw, d, dp, kc, dActive,
+              dFail, dPrec);
     if (tied)
-      AM_LAUNCH(prep_kernel<true>, C, kThreads, 0, s, dMeans.p, dPrec.p, dW.p, d, dp, K, dActive.p, dMP.p, dLogdet.p,
-                dLogw.p);
+      AM_LAUNCH(prep_kernel<true>, C, kThreads, 0, s, dMeans, dPrec, dW, d, dp, K, dActive, dMP, dLogdet,
+                dLogw);
     else
-      AM_LAUNCH(prep_kernel<false>, C, kThreads, 0, s, dMeans.p, dPrec.p, dW.p, d, dp, K, dActive.p, dMP.p, dLogdet.p,
-                dLogw.p);
+      AM_LAUNCH(prep_kernel<false>, C, kThreads, 0, s, dMeans, dPrec, dW, d, dp, K, dActive, dMP, dLogdet,
+                dLogw);
     return AM_OK;
   };
   auto estep = [&]() -> int {
     if (lin) {
-      AM_LAUNCH(lin_estep_kernel, dim3((unsigned)(Np / kTile), Cp / kTile), kThreads, 0, s, sph, dX.p, sph ? nullptr : dX2.p, Np, d, dp,
-                C, K, dActive.p, sph ? dMeans.p : dWcol.p, ka, dCst.p, dScale.p, dXsq.p, dLogdet.p, dLogw.p, dResp.p);
+      AM_LAUNCH(lin_estep_kernel, dim3((unsigned)(Np / kTile), Cp / kTile), kThreads, 0, s, sph, dX, sph ? nullptr : dX2, Np, d, dp,
+                C, K, dActive, sph ? dMeans : dWcol, ka, dCst, dScale, dXsq, dLogdet, dLogw, dResp);
     } else if (tied) {
-      AM_LAUNCH(estep_kernel<true>, dim3((unsigned)(Np / kEM), n_init), kThreads, estep_smem, s, dX.p, Np, d, dp, K,
-                dActive.p, dPrec.p, dMP.p, dLogdet.p, dLogw.p, dResp.p);
+      AM_LAUNCH(estep_kernel<true>, dim3((unsigned)(Np / kEM), n_init), kThreads, estep_smem, s, dX, Np, d, dp, K,
+                dActive, dPrec, dMP, dLogdet, dLogw, dResp);
     } else {
-      AM_LAUNCH(estep_kernel<false>, dim3((unsigned)(Np / kEM), C), kThreads, estep_smem, s, dX.p, Np, d, dp, K,
-                dActive.p, dPrec.p, dMP.p, dLogdet.p, dLogw.p, dResp.p);
+      AM_LAUNCH(estep_kernel<false>, dim3((unsigned)(Np / kEM), C), kThreads, estep_smem, s, dX, Np, d, dp, K,
+                dActive, dPrec, dMP, dLogdet, dLogw, dResp);
     }
     return AM_OK;
   };
   auto normalise = [&](int64_t* lab) -> int {
-    AM_LAUNCH(norm_kernel, dim3((unsigned)ceil_div((int)Np, 256), n_init), 256, 0, s, dResp.p, N, Np, K, dActive.p,
-              dLpn.p, lab);
-    if (!lab) AM_LAUNCH(lb_kernel, n_init, kThreads, 0, s, dLpn.p, N, Np, dActive.p, dLb.p);
+    AM_LAUNCH(norm_kernel, dim3((unsigned)ceil_div((int)Np, 256), n_init), 256, 0, s, dResp, N, Np, K, dActive,
+              dLpn, lab);
+    if (!lab) AM_LAUNCH(lb_kernel, n_init, kThreads, 0, s, dLpn, N, Np, dActive, dLb);
     return AM_OK;
   };
 
@@ -1043,12 +1023,12 @@ extern "C" int am_gmm_fit(const double* X, int64_t N, int d, int K, int type, in
   AM_TRY(mstep(true, ev[2]));
   AM_CUDA(cudaEventRecord(ev[3], s));
   int fail = 0;
-  AM_CUDA(cudaMemcpyAsync(&fail, dFail.p, 4, cudaMemcpyDeviceToHost, s));
+  AM_CUDA(cudaMemcpyAsync(&fail, dFail, 4, cudaMemcpyDeviceToHost, s));
   AM_CUDA(cudaStreamSynchronize(s));
   AM_TRY(add(0, ev[0], ev[1]));
   AM_TRY(add(3, ev[1], ev[2]));
   AM_TRY(add(4, ev[2], ev[3]));
-  if (kpp) AM_CUDA(cudaMemcpy(kpp, dIdx.p, (size_t)C * 4, cudaMemcpyDeviceToHost));
+  if (kpp) AM_CUDA(cudaMemcpy(kpp, dIdx, (size_t)C * 4, cudaMemcpyDeviceToHost));
 
   std::vector<double> lb(n_init, -INFINITY), traj((size_t)n_init * max_iter, NAN);
   std::vector<int> it_of(n_init, 0), conv_of(n_init, 0);
@@ -1062,8 +1042,8 @@ extern "C" int am_gmm_fit(const double* X, int64_t N, int d, int K, int type, in
     AM_TRY(mstep(false, ev[7]));
     AM_CUDA(cudaEventRecord(ev[8], s));
     std::vector<double> got(n_init);
-    AM_CUDA(cudaMemcpyAsync(got.data(), dLb.p, n_init * 8, cudaMemcpyDeviceToHost, s));
-    AM_CUDA(cudaMemcpyAsync(&fail, dFail.p, 4, cudaMemcpyDeviceToHost, s));
+    AM_CUDA(cudaMemcpyAsync(got.data(), dLb, n_init * 8, cudaMemcpyDeviceToHost, s));
+    AM_CUDA(cudaMemcpyAsync(&fail, dFail, 4, cudaMemcpyDeviceToHost, s));
     AM_CUDA(cudaStreamSynchronize(s));
     AM_TRY(add(1, ev[4], ev[5]));
     AM_TRY(add(2, ev[5], ev[6]));
@@ -1081,7 +1061,7 @@ extern "C" int am_gmm_fit(const double* X, int64_t N, int d, int K, int type, in
         --running;
       }
     }
-    if (running > 0) AM_CUDA(cudaMemcpyAsync(dActive.p, act.data(), n_init * 4, cudaMemcpyHostToDevice, s));
+    if (running > 0) AM_CUDA(cudaMemcpyAsync(dActive, act.data(), n_init * 4, cudaMemcpyHostToDevice, s));
   }
   *ill_defined = fail ? 1 : 0;
   if (fail) return AM_OK;
@@ -1105,23 +1085,22 @@ extern "C" int am_gmm_fit(const double* X, int64_t N, int d, int K, int type, in
   // labels: one more E-step on the best init's parameters
   std::fill(act.begin(), act.end(), 0);
   act[best] = 1;
-  AM_CUDA(cudaMemcpyAsync(dActive.p, act.data(), n_init * 4, cudaMemcpyHostToDevice, s));
+  AM_CUDA(cudaMemcpyAsync(dActive, act.data(), n_init * 4, cudaMemcpyHostToDevice, s));
   AM_TRY(estep());
-  AM_TRY(normalise(dLab.p));
+  AM_TRY(normalise(dLab));
   const int c0 = best * K;
-  AM_CUDA(cudaMemcpyAsync(labels, dLab.p, (size_t)N * 8, cudaMemcpyDeviceToHost, s));
-  AM_CUDA(cudaMemcpyAsync(weights, dW.p + c0, (size_t)K * 8, cudaMemcpyDeviceToHost, s));
-  AM_LAUNCH(pack_kernel, grid_for((int64_t)K * d), 256, 0, s, dMeans.p, c0, K, 1, d, dp, (int64_t)dp, dOut.p);
-  AM_CUDA(cudaMemcpyAsync(means, dOut.p, (size_t)K * d * 8, cudaMemcpyDeviceToHost, s));
-  AM_CUDA(cudaStreamSynchronize(s));
+  AM_CUDA(cudaMemcpyAsync(weights, dW + c0, (size_t)K * 8, cudaMemcpyDeviceToHost, s));
+  AM_LAUNCH(pack_kernel, grid_for((int64_t)K * d), 256, 0, s, dMeans, c0, K, 1, d, dp, (int64_t)dp, dOut);
+  AM_CUDA(cudaMemcpyAsync(means, dOut, (size_t)K * d * 8, cudaMemcpyDeviceToHost, s));
+  AM_TRY(call.finish());  // the labels
   // covariances and precisions_cholesky in scikit-learn's shapes: full [K, d, d], tied [d, d], diag [K, d],
   // spherical [K]
   const int pc0 = tied ? best : c0, pK = tied ? 1 : K, rows = full || tied ? d : 1, cols = sph ? 1 : d;
   const int64_t sc = full || tied ? (int64_t)dp * dp : sph ? 1 : dp;
   for (int q = 0; q < 2; ++q) {
-    AM_LAUNCH(pack_kernel, grid_for((int64_t)out_n), 256, 0, s, q ? dPrec.p : dCov.p, pc0, pK, rows, cols, dp, sc,
-              dOut.p);
-    AM_CUDA(cudaMemcpyAsync(q ? precisions_cholesky : covariances, dOut.p, out_n * 8, cudaMemcpyDeviceToHost, s));
+    AM_LAUNCH(pack_kernel, grid_for((int64_t)out_n), 256, 0, s, q ? dPrec : dCov, pc0, pK, rows, cols, dp, sc,
+              dOut);
+    AM_CUDA(cudaMemcpyAsync(q ? precisions_cholesky : covariances, dOut, out_n * 8, cudaMemcpyDeviceToHost, s));
     AM_CUDA(cudaStreamSynchronize(s));
   }
   if (phase_ms)

@@ -14,6 +14,7 @@
 // sums / counts which the host all-reduces (NCCL) before dividing.
 #include "common.cuh"
 #include "gemm_wgmma.cuh"
+#include "host_call.cuh"
 #include "kmeans_tc.cuh"
 
 #include <algorithm>
@@ -494,68 +495,63 @@ extern "C" int am_kmeans_fit(const float* X, int64_t N, int d, int k, int n_init
   AM_CHECK(X && centers && labels, "am_kmeans_fit: NULL buffer");
   AM_CHECK(N > 0 && d > 0 && k > 0 && k <= N, "am_kmeans_fit: need 0 < k <= N (N=%lld k=%d)", (long long)N, k);
   AM_CHECK(max_iter > 0 && n_init > 0, "am_kmeans_fit: max_iter and n_init must be positive");
-  AM_TRY(ensure_init());
-  Stream st;
-  AM_TRY(st.create());
-  DevBuf<float> dX, dC, dBestC, sums, counts, dist, mind2, cand;
-  DevBuf<int32_t> dL, dBestL;
-  DevBuf<double> scal, bsum, bpot;
-  AM_TRY(dX.alloc((size_t)N * d));
-  AM_TRY(dC.alloc((size_t)k * d));
-  AM_TRY(dBestC.alloc((size_t)k * d));
-  AM_TRY(sums.alloc((size_t)k * d));
-  AM_TRY(counts.alloc(k));
-  AM_TRY(dist.alloc((size_t)N));
-  AM_TRY(dL.alloc(N));
-  AM_TRY(dBestL.alloc(N));
-  AM_TRY(scal.alloc(2));  // [0] inertia, [1] shift2
-  AM_CUDA(cudaMemcpyAsync(dX.p, X, (size_t)N * d * 4, cudaMemcpyHostToDevice, st.s));
+  cudaStream_t st;
+  AM_TRY(HostCall::thread_stream(&st));
+  const int64_t nblk = (N + 1023) / 1024;
+  HostCall call(st, 0, HostCall::Memory::Owned);
+  float *dX, *dC, *dBestC, *sums, *counts, *dist, *mind2, *cand, *dmean;
+  int32_t *dL, *dBestL;
+  double *scal, *bsum, *bpot;
+  call.up(&dX, X, (size_t)N * d);
+  call.down(&dBestC, (size_t)k * d, centers);
+  call.down(&dBestL, (size_t)N, labels);
+  call.device(&dC, (size_t)k * d);
+  call.device(&sums, (size_t)k * d);
+  call.device(&counts, (size_t)k);
+  call.device(&dist, (size_t)N);
+  call.device(&dL, (size_t)N);
+  call.device(&scal, 2);  // [0] inertia, [1] shift2
+  call.device(&dmean, (size_t)d);
+  call.device(&mind2, init_centers ? 0 : (size_t)N);  // k-means++ scratch
+  call.device(&bsum, init_centers ? 0 : (size_t)nblk);
+  call.device(&cand, init_centers ? 0 : (size_t)kMaxTrials * d);
+  call.device(&bpot, init_centers ? 0 : (size_t)nblk * kMaxTrials);
+  AM_TRY(call.start());
   double tol_abs = 0.0;
   std::vector<float> hmean;
-  AM_TRY(scaled_tolerance(dX.p, N, d, tol, st.s, &tol_abs, hmean));
+  AM_TRY(scaled_tolerance(dX, N, d, tol, st, &tol_abs, hmean));
   // as sklearn's KMeans.fit: Lloyd runs on the rows minus their column means, whose fp32 distances then do not lose
   // ||mean||^2 to cancellation (seeding, tolerance and inertia do not change under the shift)
-  DevBuf<float> dmean;
-  AM_TRY(dmean.alloc((size_t)d));
-  AM_CUDA(cudaMemcpyAsync(dmean.p, hmean.data(), (size_t)d * 4, cudaMemcpyHostToDevice, st.s));
+  AM_CUDA(cudaMemcpyAsync(dmean, hmean.data(), (size_t)d * 4, cudaMemcpyHostToDevice, st));
   const auto shift_grid = [](int64_t n) { return (int)std::max<int64_t>(1, std::min<int64_t>((n + 255) / 256, (int64_t)sm_count() * 8)); };
-  AM_LAUNCH(shift_rows_kernel, shift_grid((int64_t)N * d), 256, 0, st.s, dX.p, N, d, dmean.p, -1);
-  am_kmeans_plan step{dX.p, N, d, k};
-  AM_TRY(step.create(kmeans_use_tensor_cores(N, d, k, KMeansUse::kFit), st.s));
+  AM_LAUNCH(shift_rows_kernel, shift_grid((int64_t)N * d), 256, 0, st, dX, N, d, dmean, -1);
+  am_kmeans_plan step{dX, N, d, k};
+  AM_TRY(step.create(kmeans_use_tensor_cores(N, d, k, KMeansUse::kFit), st));
 
   SplitMix rng{seed ^ 0x5851f42d4c957f2dull};
-  const int64_t nblk = (N + 1023) / 1024;
-  if (!init_centers) {
-    AM_TRY(mind2.alloc(N));
-    AM_TRY(bsum.alloc(nblk));
-    AM_TRY(cand.alloc((size_t)kMaxTrials * d));
-    AM_TRY(bpot.alloc((size_t)nblk * kMaxTrials));
-  }
   double best_inertia = INFINITY;
   int best_iters = 0;
   for (int run = 0; run < (init_centers ? 1 : n_init); ++run) {
     if (init_centers) {
-      AM_CUDA(cudaMemcpyAsync(dC.p, init_centers, (size_t)k * d * 4, cudaMemcpyHostToDevice, st.s));
-      AM_LAUNCH(shift_rows_kernel, shift_grid((int64_t)k * d), 256, 0, st.s, dC.p, (int64_t)k, d, dmean.p, -1);
-    } else AM_TRY(kmeanspp_seed(dX.p, N, d, k, rng, dC.p, mind2.p, bsum.p, cand.p, bpot.p, st.s));
+      AM_CUDA(cudaMemcpyAsync(dC, init_centers, (size_t)k * d * 4, cudaMemcpyHostToDevice, st));
+      AM_LAUNCH(shift_rows_kernel, shift_grid((int64_t)k * d), 256, 0, st, dC, (int64_t)k, d, dmean, -1);
+    } else AM_TRY(kmeanspp_seed(dX, N, d, k, rng, dC, mind2, bsum, cand, bpot, st));
     int it = 0;
-    AM_TRY(lloyd(step, max_iter, tol_abs, dC.p, dL.p, sums.p, counts.p, dist.p, scal.p + 1, st.s, &it));
+    AM_TRY(lloyd(step, max_iter, tol_abs, dC, dL, sums, counts, dist, scal + 1, st, &it));
     // final E-step: labels and inertia consistent with the returned centres
-    AM_TRY(step.step(dC.p, dL.p, nullptr, nullptr, scal.p, nullptr, st.s));
+    AM_TRY(step.step(dC, dL, nullptr, nullptr, scal, nullptr, st));
     double inert = 0.0;
-    AM_CUDA(cudaMemcpyAsync(&inert, scal.p, 8, cudaMemcpyDeviceToHost, st.s));
-    AM_CUDA(cudaStreamSynchronize(st.s));
+    AM_CUDA(cudaMemcpyAsync(&inert, scal, 8, cudaMemcpyDeviceToHost, st));
+    AM_CUDA(cudaStreamSynchronize(st));
     if (inert < best_inertia) {  // keep the best restart
       best_inertia = inert;
       best_iters = it;
-      AM_CUDA(cudaMemcpyAsync(dBestC.p, dC.p, (size_t)k * d * 4, cudaMemcpyDeviceToDevice, st.s));
-      AM_CUDA(cudaMemcpyAsync(dBestL.p, dL.p, (size_t)N * 4, cudaMemcpyDeviceToDevice, st.s));
+      AM_CUDA(cudaMemcpyAsync(dBestC, dC, (size_t)k * d * 4, cudaMemcpyDeviceToDevice, st));
+      AM_CUDA(cudaMemcpyAsync(dBestL, dL, (size_t)N * 4, cudaMemcpyDeviceToDevice, st));
     }
   }
-  AM_LAUNCH(shift_rows_kernel, shift_grid((int64_t)k * d), 256, 0, st.s, dBestC.p, (int64_t)k, d, dmean.p, 1);
-  AM_CUDA(cudaMemcpyAsync(centers, dBestC.p, (size_t)k * d * 4, cudaMemcpyDeviceToHost, st.s));
-  AM_CUDA(cudaMemcpyAsync(labels, dBestL.p, (size_t)N * 4, cudaMemcpyDeviceToHost, st.s));
-  AM_CUDA(cudaStreamSynchronize(st.s));
+  AM_LAUNCH(shift_rows_kernel, shift_grid((int64_t)k * d), 256, 0, st, dBestC, (int64_t)k, d, dmean, 1);
+  AM_TRY(call.finish());
   if (inertia) *inertia = (float)best_inertia;
   if (n_iter) *n_iter = best_iters;
   return AM_OK;

@@ -12,6 +12,7 @@
 //   If the superset overflows the on-chip candidate buffer (k > ~4000, e.g. the reference's
 //   k = len(index) max-distance scan, voyager_manager.py:1681) a full float64 pass + global
 //   bitonic sort answers instead.
+#include "host_call.cuh"
 #include "knn.cuh"
 
 #include <algorithm>
@@ -915,64 +916,6 @@ extern "C" int am_knn_build_dev(const float* X_dev, int64_t N, int d, int metric
 
 extern "C" void am_knn_free(am_index* idx) { delete idx; }
 
-// ---------------------------------------------------------------- the memory of a host call
-int HostCall::thread_stream(cudaStream_t* st) {
-  AM_TRY(ensure_init());
-  static thread_local Stream s;  // one per calling thread (Flask gthread x4), so the entry points are re-entrant
-  AM_TRY(s.create());
-  *st = s.s;
-  return AM_OK;
-}
-
-int HostCall::start() {
-  auto rank = [](const Part& p) { return p.dir != Device ? (int)p.dir : Device + (p.fill < 0 ? 256 : p.fill); };
-  std::stable_sort(parts_.begin(), parts_.end(), [&](const Part& a, const Part& b) { return rank(a) < rank(b); });
-  size_t off = 0;
-  for (Part& p : parts_) {
-    p.off = off;
-    off += round_up(p.bytes, 256);
-    if (p.dir == Up) back_begin_ = off;
-    if (p.dir <= Both) up_end_ = off;
-    if (p.dir <= Down) back_end_ = off;
-  }
-  AM_TRY(dev_.alloc(off, st_));
-  for (const Part& p : parts_) {
-    char* ptr = dev_.p + p.off;
-    std::memcpy(p.slot, &ptr, sizeof ptr);
-  }
-  staged_ = back_end_ <= limit_;  // [up | both | down] starts at 0
-  if (staged_) {
-    static thread_local PinnedBuf<char> mirror;  // grows to the largest staged call of the thread
-    AM_TRY(mirror.ensure(back_end_));
-    host_ = mirror.p;
-    for (const Part& p : parts_)
-      if (p.up_bytes) std::memcpy(host_ + p.off, p.src, p.up_bytes);
-    if (up_end_) AM_CUDA(cudaMemcpyAsync(dev_.p, host_, up_end_, cudaMemcpyHostToDevice, st_));
-  } else {
-    for (const Part& p : parts_)
-      if (p.up_bytes) AM_CUDA(cudaMemcpyAsync(dev_.p + p.off, p.src, p.up_bytes, cudaMemcpyHostToDevice, st_));
-  }
-  for (size_t i = 0, j; i < parts_.size(); i = j) {  // one memset per run of device parts with the same fill byte
-    const Part& p = parts_[i];
-    for (j = i + 1; j < parts_.size() && p.dir == Device && p.fill >= 0 && parts_[j].fill == p.fill;) ++j;
-    const size_t end = parts_[j - 1].off + round_up(parts_[j - 1].bytes, 256);
-    if (p.dir == Device && p.fill >= 0 && end > p.off) AM_CUDA(cudaMemsetAsync(dev_.p + p.off, p.fill, end - p.off, st_));
-  }
-  return AM_OK;
-}
-
-int HostCall::finish() {
-  if (staged_ && back_end_ > back_begin_)
-    AM_CUDA(cudaMemcpyAsync(host_ + back_begin_, dev_.p + back_begin_, back_end_ - back_begin_, cudaMemcpyDeviceToHost,
-                            st_));
-  for (const Part& p : parts_)
-    if (!staged_ && p.dst && p.bytes) AM_CUDA(cudaMemcpyAsync(p.dst, dev_.p + p.off, p.bytes, cudaMemcpyDeviceToHost, st_));
-  AM_CUDA(cudaStreamSynchronize(st_));
-  for (const Part& p : parts_)
-    if (staged_ && p.dst && p.bytes) std::memcpy(p.dst, host_ + p.off, p.bytes);
-  return AM_OK;
-}
-
 // ---------------------------------------------------------------- query plan
 // Everything about a query call that follows from (index, nq, k, mode), decided before anything is launched.
 enum class Scorer {
@@ -1197,7 +1140,8 @@ extern "C" int am_knn_query_dev(const am_index* idx, const float* Q_dev, int nq,
   QueryPlan pl;
   AM_TRY(plan_query(idx, nq, k, mode, &pl));
   const cudaStream_t st = (cudaStream_t)stream;
-  HostCall call(st, 0);  // the caller's stream, nothing pinned: only the overflow flags come back
+  // the caller's stream, nothing pinned: only the overflow flags come back
+  HostCall call(st, 0, HostCall::Memory::Pool);
   QueryBufs b;
   query_parts(call, pl, nq, &b);
   AM_TRY(call.start());
@@ -1214,7 +1158,7 @@ extern "C" int am_knn_query(const am_index* idx, const float* Q, int nq, int k, 
   AM_TRY(HostCall::thread_stream(&st));
   QueryPlan pl;
   AM_TRY(plan_query(idx, nq, k, mode, &pl));
-  HostCall call(st, kStageLimit);
+  HostCall call(st, kStageLimit, HostCall::Memory::Pool);
   float *dQ, *dD;
   int64_t* dI;
   call.up(&dQ, Q, (size_t)nq * idx->d);
@@ -1246,7 +1190,7 @@ extern "C" int am_knn_get_vectors(const am_index* idx, const int64_t* ids, int n
   cudaStream_t st;
   AM_TRY(HostCall::thread_stream(&st));
   // a whole library (Index._materialise_rows) goes straight to the caller's array instead of pinning its size for good
-  HostCall call(st, kStageLimit);
+  HostCall call(st, kStageLimit, HostCall::Memory::Pool);
   int64_t* d_ids;
   float* d_out;
   call.up(&d_ids, ids, (size_t)n);
@@ -1269,7 +1213,7 @@ extern "C" int am_knn_farthest(const am_index* idx, const float* query, int64_t 
   AM_TRY(HostCall::thread_stream(&st));
   const int d = idx->d;
   const int n_part = (int)std::max<int64_t>(1, std::min<int64_t>((idx->N + 7) / 8, (int64_t)sm_count() * 8));
-  HostCall call(st, HostCall::kAlways);
+  HostCall call(st, HostCall::kAlways, HostCall::Memory::Pool);
   float *dQ, *dQs, *dD;
   double* qnorm;
   int64_t* dR;

@@ -2,6 +2,7 @@
 // duplicate filter, the radius walk, and the by-vector chain's requests -- the song path's jobs, Song Alchemy and the
 // plain similar-tracks queries.  The duplicate filter and the chain's requests walk their lists through one filter window
 // (FilterWindow) and one per-item walk (walk_list).
+#include "host_call.cuh"
 #include "knn.cuh"
 
 #include <math_constants.h>
@@ -727,7 +728,7 @@ extern "C" int am_knn_filter_by_distance(const am_index* idx, const int64_t* ids
   }
   cudaStream_t st;
   AM_TRY(HostCall::thread_stream(&st));
-  HostCall call(st, kStageLimit);
+  HostCall call(st, kStageLimit, HostCall::Memory::Pool);
   int64_t* d_ids;
   unsigned char* d_keep;
   call.up(&d_ids, ids, (size_t)n_lists * n);
@@ -758,7 +759,7 @@ extern "C" int am_knn_radius_walk(const am_index* idx, const float* anchor, cons
   const int n_out = std::min(n, n_cand);
   cudaStream_t st;
   AM_TRY(HostCall::thread_stream(&st));
-  HostCall call(st, HostCall::kAlways);
+  HostCall call(st, HostCall::kAlways, HostCall::Memory::Pool);
   float* d_anchor;
   int64_t* d_rows;
   int32_t *d_art, *d_cnt, *d_pos;
@@ -861,7 +862,7 @@ extern "C" int am_knn_song_path(const am_index* idx, const am_song_path_cfg* cfg
   const int64_t cap_used = nu + total_need, cap_path = np + total_need;
   cudaStream_t st;
   AM_TRY(HostCall::thread_stream(&st));
-  HostCall call(st, HostCall::kAlways);
+  HostCall call(st, HostCall::kAlways, HostCall::Memory::Pool);
   SongPathArgs a{idx->X.p, idx->N, idx->d, n_jobs};
   a.end_row = end_row;
   a.cfg = *cfg;
@@ -925,7 +926,7 @@ extern "C" int am_knn_alchemy(const am_index* idx, const am_alchemy_cfg* cfg, co
   if (n_cand == 0) return AM_OK;
   cudaStream_t st;
   AM_TRY(HostCall::thread_stream(&st));
-  HostCall call(st, HostCall::kAlways);
+  HostCall call(st, HostCall::kAlways, HostCall::Memory::Pool);
   AlchemyArgs a{idx->X.p, idx->N, idx->d, n_cand};
   a.n_excl = n_excl;
   a.cfg = *cfg;
@@ -973,7 +974,7 @@ extern "C" int am_knn_similar(const am_index* idx, const am_similar_cfg* cfg, in
   if (n_out == 0) return AM_OK;
   cudaStream_t st;
   AM_TRY(HostCall::thread_stream(&st));
-  HostCall call(st, HostCall::kAlways);
+  HostCall call(st, HostCall::kAlways, HostCall::Memory::Pool);
   SimilarArgs a{idx->X.p, idx->N, idx->d, n_cand, n, target_row, target_sig};
   a.cfg = *cfg;
   chain.declare(call, &a.chain, (size_t)n_cand + 1);

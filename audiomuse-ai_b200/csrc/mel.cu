@@ -20,8 +20,10 @@
 //
 // Algorithmic traffic per 10 s window: 480000*2 B (PCM16) or *4 B (f32) in, 128*1001*4 B out.
 #include "common.cuh"
+#include "host_call.cuh"
 
 #include <cmath>
+#include <memory>
 
 #include "mel.cuh"
 
@@ -416,26 +418,17 @@ extern "C" int am_mel_batch(const void* pcm, int pcm_is_i16, int B, int n_sample
   if (B == 0) return AM_OK;
   am_mel_plan* plan = nullptr;
   AM_TRY(am_mel_plan_create(cfg, &plan));
-  const size_t in_bytes = (size_t)B * n_samples * (pcm_is_i16 ? 2 : 4);
-  const size_t out_elems = (size_t)B * cfg->n_mels * T;
-  DevBuf<char> d_in;
-  DevBuf<float> d_out;
-  Stream st;
-  int s = d_in.alloc(in_bytes);
-  if (s == AM_OK) s = d_out.alloc(out_elems);
-  if (s == AM_OK) s = st.create();
-  if (s == AM_OK) {
-    cudaError_t e = cudaMemcpyAsync(d_in.p, pcm, in_bytes, cudaMemcpyHostToDevice, st.s);
-    if (e != cudaSuccess) s = cuda_fail(e, "H2D pcm", __FILE__, __LINE__);
-  }
-  if (s == AM_OK) s = am_mel_batch_dev(plan, d_in.p, pcm_is_i16, B, n_samples, d_out.p, st.s);
-  if (s == AM_OK) {
-    cudaError_t e = cudaMemcpyAsync(out, d_out.p, out_elems * 4, cudaMemcpyDeviceToHost, st.s);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(st.s);
-    if (e != cudaSuccess) s = cuda_fail(e, "D2H mel", __FILE__, __LINE__);
-  }
-  am_mel_plan_free(plan);
-  return s;
+  const std::unique_ptr<am_mel_plan> owner(plan);
+  cudaStream_t st;
+  AM_TRY(HostCall::thread_stream(&st));
+  HostCall call(st, 0, HostCall::Memory::Owned);
+  const char* d_in;
+  float* d_out;
+  call.up(&d_in, (const char*)pcm, (size_t)B * n_samples * (pcm_is_i16 ? 2 : 4));
+  call.down(&d_out, (size_t)B * cfg->n_mels * T, out);
+  AM_TRY(call.start());
+  AM_TRY(am_mel_batch_dev(plan, d_in, pcm_is_i16, B, n_samples, d_out, st));
+  return call.finish();
 }
 
 // tasks/clap_analyzer.py:502-523 (host side: decode stays on the host, SURVEY 8(a))

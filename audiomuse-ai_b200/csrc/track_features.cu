@@ -22,6 +22,7 @@
 // Tracks are zero-padded to the longest track of their group, which is exact: librosa pads with zeros too, and only
 // each track's own T frames are kept.  Every reduction has a fixed order and no floating-point atomics are used, so
 // two calls give identical bits and a track gives the same result alone as in any batch.
+#include "host_call.cuh"
 #include "mel.cuh"
 
 #include <algorithm>
@@ -667,10 +668,12 @@ extern "C" int am_track_features(const am_track_features_plan* plan, const float
     groups.push_back(g);
   }
 
-  Stream st;
-  AM_TRY(st.create());
-  DevBuf<char> ws;
-  AM_TRY(ws.alloc(ws_max));
+  cudaStream_t st;
+  AM_TRY(HostCall::thread_stream(&st));
+  HostCall call(st, 0, HostCall::Memory::Owned);
+  char* ws;
+  call.device(&ws, ws_max);
+  AM_TRY(call.start());
   for (const Group& g : groups) {
     const int nb = g.nb;
     const long long L = g.L;
@@ -679,7 +682,7 @@ extern "C" int am_track_features(const am_track_features_plan* plan, const float
     const long long nT = foff[g.b0 + nb] - foff[g.b0];
     const int n_blk = (Tmax + kTgFrames - 1) / kTgFrames;
     Workspace w;
-    carve(ws.p, w, nb, L, Tmax, n_in, nT, win, cap, want_tempo, want_rms, want_chroma);
+    carve(ws, w, nb, L, Tmax, n_in, nT, win, cap, want_tempo, want_rms, want_chroma);
     float* d_x = w.x;
     float* d_pad = w.pad;
     long long* d_off = w.off;
@@ -692,31 +695,31 @@ extern "C" int am_track_features(const am_track_features_plan* plan, const float
       h_foff[i] = foff[g.b0 + i] - foff[g.b0];
     }
     for (int i = 0; i < nb; ++i) h_n[i] = h_off[i + 1] - h_off[i];
-    AM_CUDA(cudaMemcpyAsync(d_x, samples + offsets[g.b0], n_in * 4, cudaMemcpyHostToDevice, st.s));
-    AM_CUDA(cudaMemcpyAsync(d_off, h_off.data(), (nb + 1) * 8, cudaMemcpyHostToDevice, st.s));
-    AM_CUDA(cudaMemcpyAsync(d_n, h_n.data(), nb * 8, cudaMemcpyHostToDevice, st.s));
-    AM_CUDA(cudaMemcpyAsync(d_foff, h_foff.data(), (nb + 1) * 8, cudaMemcpyHostToDevice, st.s));
-    AM_CUDA(cudaMemcpyAsync(d_T, T.data() + g.b0, nb * 4, cudaMemcpyHostToDevice, st.s));
-    AM_LAUNCH(tf_pad_kernel, dim3((unsigned)std::min<long long>(ceil_div((int)std::min<long long>(L, INT32_MAX), 256), 4096), nb), 256, 0, st.s,
+    AM_CUDA(cudaMemcpyAsync(d_x, samples + offsets[g.b0], n_in * 4, cudaMemcpyHostToDevice, st));
+    AM_CUDA(cudaMemcpyAsync(d_off, h_off.data(), (nb + 1) * 8, cudaMemcpyHostToDevice, st));
+    AM_CUDA(cudaMemcpyAsync(d_n, h_n.data(), nb * 8, cudaMemcpyHostToDevice, st));
+    AM_CUDA(cudaMemcpyAsync(d_foff, h_foff.data(), (nb + 1) * 8, cudaMemcpyHostToDevice, st));
+    AM_CUDA(cudaMemcpyAsync(d_T, T.data() + g.b0, nb * 4, cudaMemcpyHostToDevice, st));
+    AM_LAUNCH(tf_pad_kernel, dim3((unsigned)std::min<long long>(ceil_div((int)std::min<long long>(L, INT32_MAX), 256), 4096), nb), 256, 0, st,
               d_x, d_off, (int)L, d_pad);
 
     if (want_tempo) {
       float *d_db = w.db, *d_dbmax = w.db_max, *d_env = w.env;
       double *d_part = w.part, *d_tg = w.tg;
       int *d_anyp = w.any_part, *d_any = w.any;
-      AM_TRY(am_mel_batch_dev(plan->mel, d_pad, 0, nb, (int)L, d_db, st.s));
-      AM_LAUNCH(tf_db_max_kernel, nb, 1024, 0, st.s, d_db, d_T, Tmax, d_dbmax);
-      AM_LAUNCH(tf_onset_kernel, dim3(ceil_div(Tmax, 8), nb), 256, 0, st.s, d_db, d_dbmax, d_T, d_foff, Tmax, d_env);
-      AM_LAUNCH(tf_tempogram_kernel, dim3(n_blk, nb), kTgThreads, 0, st.s, d_env, d_T, d_foff, win, n_blk, d_part,
+      AM_TRY(am_mel_batch_dev(plan->mel, d_pad, 0, nb, (int)L, d_db, st));
+      AM_LAUNCH(tf_db_max_kernel, nb, 1024, 0, st, d_db, d_T, Tmax, d_dbmax);
+      AM_LAUNCH(tf_onset_kernel, dim3(ceil_div(Tmax, 8), nb), 256, 0, st, d_db, d_dbmax, d_T, d_foff, Tmax, d_env);
+      AM_LAUNCH(tf_tempogram_kernel, dim3(n_blk, nb), kTgThreads, 0, st, d_env, d_T, d_foff, win, n_blk, d_part,
                 d_anyp);
-      AM_LAUNCH(tf_tempogram_reduce, nb, 256, 0, st.s, d_part, d_anyp, d_T, win, n_blk, d_tg, d_any);
+      AM_LAUNCH(tf_tempogram_reduce, nb, 256, 0, st, d_part, d_anyp, d_T, win, n_blk, d_tg, d_any);
       std::vector<double> h_tg((size_t)nb * win);
       std::vector<int> h_any(nb);
-      AM_CUDA(cudaMemcpyAsync(h_tg.data(), d_tg, h_tg.size() * 8, cudaMemcpyDeviceToHost, st.s));
-      AM_CUDA(cudaMemcpyAsync(h_any.data(), d_any, nb * 4, cudaMemcpyDeviceToHost, st.s));
+      AM_CUDA(cudaMemcpyAsync(h_tg.data(), d_tg, h_tg.size() * 8, cudaMemcpyDeviceToHost, st));
+      AM_CUDA(cudaMemcpyAsync(h_any.data(), d_any, nb * 4, cudaMemcpyDeviceToHost, st));
       if (onset_env)
-        AM_CUDA(cudaMemcpyAsync(onset_env + foff[g.b0], d_env, nT * 4, cudaMemcpyDeviceToHost, st.s));
-      AM_CUDA(cudaStreamSynchronize(st.s));
+        AM_CUDA(cudaMemcpyAsync(onset_env + foff[g.b0], d_env, nT * 4, cudaMemcpyDeviceToHost, st));
+      AM_CUDA(cudaStreamSynchronize(st));
       for (int i = 0; i < nb; ++i)
         tempo[g.b0 + i] = h_any[i] ? tempo_from_tg(h_tg.data() + (size_t)i * win, win, plan->sr) : 0.0;
       if (tempogram) std::memcpy(tempogram + (size_t)g.b0 * win, h_tg.data(), h_tg.size() * 8);
@@ -744,21 +747,21 @@ extern "C" int am_track_features(const am_track_features_plan* plan, const float
       a.chroma_fb = w.fb;
       a.chroma = d_chroma;
       const dim3 grid(ceil_div(Tmax, kFramesPerCta), nb);
-      AM_LAUNCH(tf_spectrum_kernel<false>, grid, kThreads, tf_spectrum_smem(), st.s, a, plan->mel->t);
+      AM_LAUNCH(tf_spectrum_kernel<false>, grid, kThreads, tf_spectrum_smem(), st, a, plan->mel->t);
       if (want_chroma) {
-        AM_LAUNCH(tf_tuning_kernel, nb, kTuneThreads, 0, st.s, a.pk_mag, a.pk_bin, a.pk_count, d_T, d_foff, cap,
+        AM_LAUNCH(tf_tuning_kernel, nb, kTuneThreads, 0, st, a.pk_mag, a.pk_bin, a.pk_count, d_T, d_foff, cap,
                   d_thr, d_hist, d_tun);
-        AM_LAUNCH(tf_chroma_fb_kernel, nb, 256, 0, st.s, d_tun, plan->sr, w.fb);
-        AM_LAUNCH(tf_spectrum_kernel<true>, grid, kThreads, tf_spectrum_smem(), st.s, a, plan->mel->t);
-        AM_CUDA(cudaMemcpyAsync(chroma + 12 * foff[g.b0], d_chroma, nT * 12 * 4, cudaMemcpyDeviceToHost, st.s));
-        if (tuning) AM_CUDA(cudaMemcpyAsync(tuning + g.b0, d_tun, nb * 8, cudaMemcpyDeviceToHost, st.s));
-        if (threshold) AM_CUDA(cudaMemcpyAsync(threshold + g.b0, d_thr, nb * 4, cudaMemcpyDeviceToHost, st.s));
+        AM_LAUNCH(tf_chroma_fb_kernel, nb, 256, 0, st, d_tun, plan->sr, w.fb);
+        AM_LAUNCH(tf_spectrum_kernel<true>, grid, kThreads, tf_spectrum_smem(), st, a, plan->mel->t);
+        AM_CUDA(cudaMemcpyAsync(chroma + 12 * foff[g.b0], d_chroma, nT * 12 * 4, cudaMemcpyDeviceToHost, st));
+        if (tuning) AM_CUDA(cudaMemcpyAsync(tuning + g.b0, d_tun, nb * 8, cudaMemcpyDeviceToHost, st));
+        if (threshold) AM_CUDA(cudaMemcpyAsync(threshold + g.b0, d_thr, nb * 4, cudaMemcpyDeviceToHost, st));
         if (histogram)
           AM_CUDA(cudaMemcpyAsync(histogram + (size_t)g.b0 * kHistBins, d_hist, (size_t)nb * kHistBins * 4,
-                                  cudaMemcpyDeviceToHost, st.s));
+                                  cudaMemcpyDeviceToHost, st));
       }
-      if (want_rms) AM_CUDA(cudaMemcpyAsync(rms + foff[g.b0], d_rms, nT * 4, cudaMemcpyDeviceToHost, st.s));
-      AM_CUDA(cudaStreamSynchronize(st.s));
+      if (want_rms) AM_CUDA(cudaMemcpyAsync(rms + foff[g.b0], d_rms, nT * 4, cudaMemcpyDeviceToHost, st));
+      AM_CUDA(cudaStreamSynchronize(st));
     }
   }
   return AM_OK;
