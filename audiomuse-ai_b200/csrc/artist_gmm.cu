@@ -736,15 +736,8 @@ extern "C" int am_artist_gmm_fit(const float* rows, int64_t n_rows, int d, const
 
   cudaStream_t s;
   AM_TRY(HostCall::thread_stream(&s));
-  cudaEvent_t ev[4] = {};
-  for (auto& e : ev) AM_CUDA(cudaEventCreate(&e));
-  struct EvGuard {
-    cudaEvent_t* e;
-    ~EvGuard() {
-      for (int i = 0; i < 4; ++i)
-        if (e[i]) cudaEventDestroy(e[i]);
-    }
-  } evg{ev};
+  Event ev[3];
+  for (auto& e : ev) AM_TRY(e.create());
   const int P_all = (int)all.size();
   const size_t n_ak = (size_t)A * kMaxK, n_aki = n_ak * n_init;
   // problems with K > n never run: they report failed
@@ -822,23 +815,20 @@ extern "C" int am_artist_gmm_fit(const float* rows, int64_t n_rows, int d, const
     AM_TRY(dscr.ensure((size_t)std::max<int64_t>(1, dsz)));
     AM_TRY(iscr.ensure((size_t)std::max<int64_t>(1, isz)));
     AM_CUDA(cudaMemsetAsync(dCounter, 0, 4, s));
-    AM_CUDA(cudaEventRecord(ev[0], s));
+    AM_CUDA(cudaEventRecord(ev[0].e, s));
     if (!runs.empty()) {
       const int grid = std::min<int>((int)runs.size(), 2 * sm_count());
       AM_LAUNCH(fit_kernel, grid, kThreads, kSmemBytes, s, dX, d, dRuns.p, (int)runs.size(), dCounter, dDraws,
                 n_init, max_iter, tol, reg_covar, dscr.p, iscr.p, dRes, kpp ? dKpp : nullptr,
                 labels ? dLab : nullptr, n_rows);
     }
-    AM_CUDA(cudaEventRecord(ev[1], s));
+    AM_CUDA(cudaEventRecord(ev[1].e, s));
     AM_LAUNCH(select_kernel, a1 - a0, kThreads, 0, s, dProbs, dFirst, a0, dOff, dLo, dHi, d, n_init, dRes,
               dscr.p, dChosen, dBic, dFailed, dLb, dIt, dConv, dW, dM, dC);
-    AM_CUDA(cudaEventRecord(ev[2], s));
+    AM_CUDA(cudaEventRecord(ev[2].e, s));
     AM_CUDA(cudaStreamSynchronize(s));
-    float ms = 0.f;
-    AM_CUDA(cudaEventElapsedTime(&ms, ev[0], ev[1]));
-    fit_ms += ms;
-    AM_CUDA(cudaEventElapsedTime(&ms, ev[1], ev[2]));
-    sel_ms += ms;
+    AM_TRY(add_elapsed_ms(fit_ms, ev[0], ev[1]));
+    AM_TRY(add_elapsed_ms(sel_ms, ev[1], ev[2]));
     a0 = a1;
   }
   AM_TRY(call.finish());

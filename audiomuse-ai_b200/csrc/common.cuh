@@ -137,6 +137,32 @@ struct Stream {
   }
 };
 
+struct Event {
+  cudaEvent_t e = nullptr;
+  Event() = default;
+  Event(const Event&) = delete;
+  Event& operator=(const Event&) = delete;
+  ~Event() {
+    if (e) cudaEventDestroy(e);
+  }
+  int create(unsigned flags = cudaEventDefault) {
+    if (e) return AM_OK;
+    cudaError_t r = cudaEventCreateWithFlags(&e, flags);
+    if (r == cudaSuccess) return AM_OK;
+    e = nullptr;
+    return cuda_fail(r, "cudaEventCreate", __FILE__, __LINE__);
+  }
+};
+
+// ms += the time between two completed events recorded with timing
+inline int add_elapsed_ms(float& ms, const Event& from, const Event& to) {
+  float t = 0.f;
+  cudaError_t r = cudaEventElapsedTime(&t, from.e, to.e);
+  if (r != cudaSuccess) return cuda_fail(r, "cudaEventElapsedTime", __FILE__, __LINE__);
+  ms += t;
+  return AM_OK;
+}
+
 inline size_t round_up(size_t x, size_t m) { return (x + m - 1) / m * m; }
 inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 // blocks of 256 threads for a grid-stride kernel over `total_threads` items: at most 16 per SM
@@ -146,6 +172,11 @@ inline int grid_for(int64_t total_threads) {
 }
 
 // ---------------------------------------------------------------- symmetrised k-NN graphs (spectral.cu)
+// The k exact euclidean nearest rows of every row of host X f32[N, d] (knn.cu's index, ids ascending distance): X is
+// uploaded into dX, which stays with the caller, and ids i64[N, k] and dist f32[N, k] are filled; all three are
+// allocated here.  t0 and t1 are recorded on `st` around the index build and query.  Stream-ordered.
+int knn_self_query(const float* X, int64_t N, int d, int k, cudaStream_t st, const Event& t0, const Event& t1,
+                   DevBuf<float>& dX, DevBuf<int64_t>& ids, DevBuf<float>& dist);
 // CSR of k-NN lists ids i64[N, k] (device; a row's own id and ids outside [0, N) are skipped), columns ascending per
 // row.  memb == nullptr: the affinity 0.5 (C + C^T) into w32 (0.5 or 1) and dd = sqrt(row sums).  memb f64[N, k] (a
 // value per list entry): the fuzzy union A + A^T - A o A^T into w64.  Allocates the outputs; synchronises.

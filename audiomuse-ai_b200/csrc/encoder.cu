@@ -361,14 +361,14 @@ struct am_model {
   am::DevBuf<int16_t> pcm_stage[2];
   am::DevBuf<int32_t> off_stage;
   am::DevBuf<float> out_stage;
-  cudaEvent_t ev_copied[2] = {nullptr, nullptr}, ev_done[2] = {nullptr, nullptr};
+  am::Event ev_copied[2], ev_done[2];
   // submitted-but-not-collected host calls (am_clap_embed_tracks_submit / _collect): results land in pinned
   // staging first, so the D2H is truly asynchronous and the NEXT call's H2D + early blocks overlap this call's tail
   struct Ticket {
     am::PinnedBuf<float> stage;
     float* user_out = nullptr;
     size_t count = 0;
-    cudaEvent_t ready = nullptr;
+    am::Event ready;
     bool open = false;
   } tickets[2];
   unsigned n_submitted = 0, n_collected = 0;
@@ -377,13 +377,7 @@ struct am_model {
   am_mel_cfg host_plan_cfg{};        // tables + cudaMalloc + upload: ~1 ms, was paid on every call)
   int fused_blocks = 1;      // AM_FUSED_BLOCKS=0: every block layer by layer (fused_block.cu otherwise)
   ~am_model() {
-    for (int i = 0; i < 2; ++i) {
-      if (ev_copied[i]) cudaEventDestroy(ev_copied[i]);
-      if (ev_done[i]) cudaEventDestroy(ev_done[i]);
-    }
     if (host_plan) am_mel_plan_free(host_plan);
-    for (auto& t : tickets)
-      if (t.ready) cudaEventDestroy(t.ready);
   }
 };
 
@@ -1200,7 +1194,7 @@ extern "C" int am_clap_embed_tracks_collect(am_model* m) {
   ++m->n_collected;
   t.open = false;
   if (t.count == 0) return AM_OK;
-  AM_CUDA(cudaEventSynchronize(t.ready));
+  AM_CUDA(cudaEventSynchronize(t.ready.e));
   std::memcpy(t.user_out, t.stage.p, t.count * sizeof(float));
   return AM_OK;
 }
@@ -1238,8 +1232,8 @@ extern "C" int am_clap_embed_tracks_submit(am_model* m, const am_mel_cfg* cfg, c
   AM_TRY(m->copy_stream.create());
   cudaStream_t cs = m->copy_stream.s;
   for (int i = 0; i < 2; ++i) {
-    if (!m->ev_copied[i]) AM_CUDA(cudaEventCreateWithFlags(&m->ev_copied[i], cudaEventDisableTiming));
-    if (!m->ev_done[i]) AM_CUDA(cudaEventCreateWithFlags(&m->ev_done[i], cudaEventDisableTiming));
+    AM_TRY(m->ev_copied[i].create(cudaEventDisableTiming));
+    AM_TRY(m->ev_done[i].create(cudaEventDisableTiming));
   }
   const int T = mel_plan_frames(plan, n_samples);
   if (T < 0) return T;
@@ -1255,7 +1249,7 @@ extern "C" int am_clap_embed_tracks_submit(am_model* m, const am_mel_cfg* cfg, c
   AM_TRY(m->out_stage.ensure((size_t)n_tracks * m->emb));
   const size_t out_count = (size_t)n_tracks * m->emb;
   AM_TRY(tk.stage.ensure(out_count));
-  if (!tk.ready) AM_CUDA(cudaEventCreateWithFlags(&tk.ready, cudaEventDisableTiming));
+  AM_TRY(tk.ready.create(cudaEventDisableTiming));
   if (std::getenv("AM_TEST_FAIL_SUBMIT")) {  // test hook: a submit that fails after its allocations (tests/test_gpu_encoder.py)
     set_error("am_clap_embed_tracks_submit: out of memory (injected by AM_TEST_FAIL_SUBMIT)");
     return AM_ERR_OOM;
@@ -1273,14 +1267,14 @@ extern "C" int am_clap_embed_tracks_submit(am_model* m, const am_mel_cfg* cfg, c
       const int nb = std::min(std::min(want, sub), n_segments - b0);
       const int slot = c & 1;
       // slot free again (its last reader may belong to the previous, still running, submitted call)
-      if (m->slot_used[slot]) AM_CUDA(cudaStreamWaitEvent(cs, m->ev_done[slot], 0));
+      if (m->slot_used[slot]) AM_CUDA(cudaStreamWaitEvent(cs, m->ev_done[slot].e, 0));
       m->slot_used[slot] = true;
       AM_CUDA(cudaMemcpyAsync(m->pcm_stage[slot].p, pcm + (size_t)b0 * n_samples, (size_t)nb * n_samples * 2,
                               cudaMemcpyHostToDevice, cs));
-      AM_CUDA(cudaEventRecord(m->ev_copied[slot], cs));
-      AM_CUDA(cudaStreamWaitEvent(st, m->ev_copied[slot], 0));
+      AM_CUDA(cudaEventRecord(m->ev_copied[slot].e, cs));
+      AM_CUDA(cudaStreamWaitEvent(st, m->ev_copied[slot].e, 0));
       AM_TRY(am_mel_batch_dev(plan, m->pcm_stage[slot].p, 1, nb, n_samples, m->mel_ws.p, st));
-      AM_CUDA(cudaEventRecord(m->ev_done[slot], st));  // the mel kernel was the staging slot's only reader
+      AM_CUDA(cudaEventRecord(m->ev_done[slot].e, st));  // the mel kernel was the staging slot's only reader
       AM_TRY(forward_early(m, *p, m->mel_ws.p, nb, b0, st));
       b0 += nb;
     }
@@ -1288,7 +1282,7 @@ extern "C" int am_clap_embed_tracks_submit(am_model* m, const am_mel_cfg* cfg, c
     AM_TRY(head_forward(m, n_segments, m->seg_emb.p, st));
     AM_LAUNCH(track_pool_kernel, n_tracks, 256, 0, st, m->seg_emb.p, m->off_stage.p, m->emb, m->out_stage.p);
     AM_CUDA(cudaMemcpyAsync(tk.stage.p, m->out_stage.p, out_count * 4, cudaMemcpyDeviceToHost, st));
-    AM_CUDA(cudaEventRecord(tk.ready, st));
+    AM_CUDA(cudaEventRecord(tk.ready.e, st));
     return AM_OK;
   };
   const int s = enqueue();

@@ -862,16 +862,8 @@ extern "C" int am_gmm_fit(const double* X, int64_t N, int d, int K, int type, in
 
   cudaStream_t s;
   AM_TRY(HostCall::thread_stream(&s));
-  constexpr int kEv = 12;
-  cudaEvent_t ev[kEv] = {};
-  struct EvGuard {
-    cudaEvent_t* e;
-    ~EvGuard() {
-      for (int i = 0; i < kEv; ++i)
-        if (e[i]) cudaEventDestroy(e[i]);
-    }
-  } evg{ev};
-  for (auto& e : ev) AM_CUDA(cudaEventCreate(&e));
+  Event ev[9];
+  for (auto& e : ev) AM_TRY(e.create());
 
   const int nb_kpp = (int)((N + kKppRows - 1) / kKppRows);
   const size_t cov_n = full ? (size_t)C * dp * dp : tied ? (size_t)n_init * dp * dp : sph ? (size_t)C : (size_t)C * dp;
@@ -935,7 +927,7 @@ extern "C" int am_gmm_fit(const double* X, int64_t N, int d, int K, int type, in
   AM_TRY(allow_dynamic_smem<estep_kernel<true>>(((size_t)kEM * kXLd + 16 * (size_t)(AM_GMM_MAX_D + 4)) * 8));
 
   // ---- k-means++
-  AM_CUDA(cudaEventRecord(ev[0], s));
+  AM_CUDA(cudaEventRecord(ev[0].e, s));
   AM_LAUNCH(rownorm_kernel, grid_for(N * 32), kThreads, 0, s, dX, N, dp, dXsq);
   AM_LAUNCH(fill_kernel, grid_for(close_n), 256, 0, s, dClose, (int64_t)close_n, (double)INFINITY);
   for (int cc = 0; cc < K; ++cc) {
@@ -953,10 +945,10 @@ extern "C" int am_gmm_fit(const double* X, int64_t N, int d, int K, int type, in
               cchunk, dPc);
     AM_LAUNCH(cov_reduce_kernel, dim3(1, d), 256, 0, s, dPc, Sc, 1, d64, d, dp, 1, dOn, dUnit, 0.0, dXtX);
   }
-  AM_CUDA(cudaEventRecord(ev[1], s));
+  AM_CUDA(cudaEventRecord(ev[1].e, s));
 
   // ---- M-step (init = true: the initialisation's weights nk / N) and the precision factors
-  auto mstep = [&](bool init, cudaEvent_t e_mid) -> int {
+  auto mstep = [&](bool init, const Event& e_mid) -> int {
     AM_LAUNCH(nk_kernel, C, kThreads, 0, s, dResp, Np, K, dActive, dNk);
     AM_LAUNCH(gram_kernel<false>, dim3(Cp / kTile, d64 / kTile, Sm), kThreads, 0, s, dX, dResp, dMeans, Np, dp,
               C, K, dActive, mchunk, dPm);
@@ -975,7 +967,7 @@ extern "C" int am_gmm_fit(const double* X, int64_t N, int d, int K, int type, in
     }
     AM_LAUNCH(weights_kernel, ceil_div(n_init, 64), 64, 0, s, dNk, n_init, K, dActive, init ? (double)N : 0.0,
               dW);
-    AM_CUDA(cudaEventRecord(e_mid, s));
+    AM_CUDA(cudaEventRecord(e_mid.e, s));
     if (lin) {
       AM_LAUNCH(diag_cov_kernel, C, kThreads, 0, s, sph, dPm2, Sm, Cp, d64, d, dp, K, dActive, dNk, dMeans, dW, reg_covar,
                 dCov, dPrec, dWcol, dCst, dScale, dLogdet, dLogw, dFail);
@@ -1014,41 +1006,35 @@ extern "C" int am_gmm_fit(const double* X, int64_t N, int d, int K, int type, in
   };
 
   float ms[5] = {0.f, 0.f, 0.f, 0.f, 0.f};   // seeding, E-step, normaliser, M-step, precision factors
-  auto add = [&](int slot, cudaEvent_t a, cudaEvent_t b) -> int {
-    float t = 0.f;
-    AM_CUDA(cudaEventElapsedTime(&t, a, b));
-    ms[slot] += t;
-    return AM_OK;
-  };
   AM_TRY(mstep(true, ev[2]));
-  AM_CUDA(cudaEventRecord(ev[3], s));
+  AM_CUDA(cudaEventRecord(ev[3].e, s));
   int fail = 0;
   AM_CUDA(cudaMemcpyAsync(&fail, dFail, 4, cudaMemcpyDeviceToHost, s));
   AM_CUDA(cudaStreamSynchronize(s));
-  AM_TRY(add(0, ev[0], ev[1]));
-  AM_TRY(add(3, ev[1], ev[2]));
-  AM_TRY(add(4, ev[2], ev[3]));
+  AM_TRY(add_elapsed_ms(ms[0], ev[0], ev[1]));
+  AM_TRY(add_elapsed_ms(ms[3], ev[1], ev[2]));
+  AM_TRY(add_elapsed_ms(ms[4], ev[2], ev[3]));
   if (kpp) AM_CUDA(cudaMemcpy(kpp, dIdx, (size_t)C * 4, cudaMemcpyDeviceToHost));
 
   std::vector<double> lb(n_init, -INFINITY), traj((size_t)n_init * max_iter, NAN);
   std::vector<int> it_of(n_init, 0), conv_of(n_init, 0);
   int running = n_init;
   for (int it = 1; it <= max_iter && running > 0 && !fail; ++it) {
-    AM_CUDA(cudaEventRecord(ev[4], s));
+    AM_CUDA(cudaEventRecord(ev[4].e, s));
     AM_TRY(estep());
-    AM_CUDA(cudaEventRecord(ev[5], s));
+    AM_CUDA(cudaEventRecord(ev[5].e, s));
     AM_TRY(normalise(nullptr));
-    AM_CUDA(cudaEventRecord(ev[6], s));
+    AM_CUDA(cudaEventRecord(ev[6].e, s));
     AM_TRY(mstep(false, ev[7]));
-    AM_CUDA(cudaEventRecord(ev[8], s));
+    AM_CUDA(cudaEventRecord(ev[8].e, s));
     std::vector<double> got(n_init);
     AM_CUDA(cudaMemcpyAsync(got.data(), dLb, n_init * 8, cudaMemcpyDeviceToHost, s));
     AM_CUDA(cudaMemcpyAsync(&fail, dFail, 4, cudaMemcpyDeviceToHost, s));
     AM_CUDA(cudaStreamSynchronize(s));
-    AM_TRY(add(1, ev[4], ev[5]));
-    AM_TRY(add(2, ev[5], ev[6]));
-    AM_TRY(add(3, ev[6], ev[7]));
-    AM_TRY(add(4, ev[7], ev[8]));
+    AM_TRY(add_elapsed_ms(ms[1], ev[4], ev[5]));
+    AM_TRY(add_elapsed_ms(ms[2], ev[5], ev[6]));
+    AM_TRY(add_elapsed_ms(ms[3], ev[6], ev[7]));
+    AM_TRY(add_elapsed_ms(ms[4], ev[7], ev[8]));
     for (int i = 0; i < n_init; ++i) {
       if (!act[i]) continue;
       const double prev = lb[i];

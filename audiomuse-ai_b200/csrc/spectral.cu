@@ -27,6 +27,7 @@
 
 #include <algorithm>
 #include <cmath>
+#include <memory>
 
 struct am_spectral_plan {
   int64_t N = 0;
@@ -498,6 +499,22 @@ int knn_csr_build(const int64_t* ids, const double* memb, int64_t N, int k, cuda
   return AM_OK;
 }
 
+int knn_self_query(const float* X, int64_t N, int d, int k, cudaStream_t st, const Event& t0, const Event& t1,
+                   DevBuf<float>& dX, DevBuf<int64_t>& ids, DevBuf<float>& dist) {
+  AM_TRY(dX.alloc((size_t)N * d));
+  AM_CUDA(cudaMemcpyAsync(dX.p, X, (size_t)N * d * 4, cudaMemcpyHostToDevice, st));
+  AM_TRY(ids.alloc((size_t)N * k));
+  AM_TRY(dist.alloc((size_t)N * k));
+  AM_CUDA(cudaEventRecord(t0.e, st));
+  am_index* idx = nullptr;
+  AM_TRY(am_knn_build_dev(dX.p, N, d, 1, st, &idx));
+  const int qs = am_knn_query_dev(idx, dX.p, (int)N, k, 0, ids.p, dist.p, st);
+  am_knn_free(idx);
+  AM_TRY(qs);
+  AM_CUDA(cudaEventRecord(t1.e, st));
+  return AM_OK;
+}
+
 }  // namespace am
 
 using namespace am;
@@ -512,57 +529,27 @@ extern "C" int am_spectral_plan_create(const float* X, int64_t N, int d, int n_n
   AM_CHECK(block >= 1 && block <= N, "am_spectral_plan_create: block = %d outside [1, N = %lld]", block, (long long)N);
   *out = nullptr;
   AM_TRY(ensure_init());
-  auto* p = new am_spectral_plan();
-  auto fail = [&](int s) {
-    delete p;
-    return s;
-  };
+  std::unique_ptr<am_spectral_plan> p(new am_spectral_plan());
   p->N = N;
   p->k_nn = n_neighbors;
   p->b = block;
   p->ld = (int)round_up((size_t)block, 32);
-  int s = p->st.create();
-  if (s != AM_OK) return fail(s);
+  AM_TRY(p->st.create());
   cudaStream_t st = p->st.s;
-  cudaEvent_t ev[3] = {nullptr, nullptr, nullptr};
-  for (auto& e : ev) {
-    const cudaError_t ce = cudaEventCreate(&e);
-    if (ce != cudaSuccess) {
-      for (auto& f : ev)
-        if (f) cudaEventDestroy(f);
-      return fail(cuda_fail(ce, "cudaEventCreate", __FILE__, __LINE__));
-    }
-  }
-  auto body = [&]() -> int {
-    DevBuf<float> dX, dist;
-    DevBuf<int64_t> ids;
-    AM_TRY(dX.alloc((size_t)N * d));
-    AM_CUDA(cudaMemcpyAsync(dX.p, X, (size_t)N * d * 4, cudaMemcpyHostToDevice, st));
-    AM_TRY(ids.alloc((size_t)N * n_neighbors));
-    AM_TRY(dist.alloc((size_t)N * n_neighbors));
-    AM_CUDA(cudaEventRecord(ev[0], st));
-    {
-      am_index* idx = nullptr;
-      AM_TRY(am_knn_build_dev(dX.p, N, d, 1, st, &idx));
-      const int qs = am_knn_query_dev(idx, dX.p, (int)N, n_neighbors, 0, ids.p, dist.p, st);
-      am_knn_free(idx);
-      AM_TRY(qs);
-    }
-    AM_CUDA(cudaEventRecord(ev[1], st));
-    AM_TRY(knn_csr_build(ids.p, nullptr, N, n_neighbors, st, p->indptr, p->indices, &p->w, &p->dd, nullptr, &p->nnz));
-    AM_TRY(p->s.alloc((size_t)std::max<int64_t>(1, p->nnz)));
-    AM_LAUNCH(sp::normalise_kernel<float>, sp::row_grid(N), 256, 0, st, p->indptr.p, N, p->indices.p, p->w.p, p->dd.p,
-              p->s.p);
-    AM_CUDA(cudaEventRecord(ev[2], st));
-    AM_TRY(sp::init_block(p, seed));
-    AM_CUDA(cudaEventElapsedTime(&p->knn_ms, ev[0], ev[1]));
-    AM_CUDA(cudaEventElapsedTime(&p->graph_ms, ev[1], ev[2]));
-    return AM_OK;
-  };
-  s = body();
-  for (auto& e : ev) cudaEventDestroy(e);
-  if (s != AM_OK) return fail(s);
-  *out = p;
+  Event ev[3];
+  for (auto& e : ev) AM_TRY(e.create());
+  DevBuf<float> dX, dist;
+  DevBuf<int64_t> ids;
+  AM_TRY(knn_self_query(X, N, d, n_neighbors, st, ev[0], ev[1], dX, ids, dist));
+  AM_TRY(knn_csr_build(ids.p, nullptr, N, n_neighbors, st, p->indptr, p->indices, &p->w, &p->dd, nullptr, &p->nnz));
+  AM_TRY(p->s.alloc((size_t)std::max<int64_t>(1, p->nnz)));
+  AM_LAUNCH(sp::normalise_kernel<float>, sp::row_grid(N), 256, 0, st, p->indptr.p, N, p->indices.p, p->w.p, p->dd.p,
+            p->s.p);
+  AM_CUDA(cudaEventRecord(ev[2].e, st));
+  AM_TRY(sp::init_block(p.get(), seed));
+  AM_TRY(add_elapsed_ms(p->knn_ms, ev[0], ev[1]));
+  AM_TRY(add_elapsed_ms(p->graph_ms, ev[1], ev[2]));
+  *out = p.release();
   return AM_OK;
 }
 
@@ -583,34 +570,27 @@ extern "C" int am_spectral_plan_create_csr(const int64_t* indptr, const int32_t*
              "positive", (long long)e);
   *out = nullptr;
   AM_TRY(ensure_init());
-  auto* p = new am_spectral_plan();
+  std::unique_ptr<am_spectral_plan> p(new am_spectral_plan());
   p->N = N;
   p->b = block;
   p->ld = (int)round_up((size_t)block, 32);
   p->nnz = nnz;
-  auto body = [&]() -> int {
-    AM_TRY(p->st.create());
-    cudaStream_t st = p->st.s;
-    DevBuf<double> w;
-    AM_TRY(p->indptr.alloc((size_t)N + 1));
-    AM_TRY(p->indices.alloc((size_t)nnz));
-    AM_TRY(w.alloc((size_t)nnz));
-    AM_TRY(p->s.alloc((size_t)nnz));
-    AM_TRY(p->dd.alloc((size_t)N));
-    AM_CUDA(cudaMemcpyAsync(p->indptr.p, indptr, ((size_t)N + 1) * 8, cudaMemcpyHostToDevice, st));
-    AM_CUDA(cudaMemcpyAsync(p->indices.p, indices, (size_t)nnz * 4, cudaMemcpyHostToDevice, st));
-    AM_CUDA(cudaMemcpyAsync(w.p, weights, (size_t)nnz * 8, cudaMemcpyHostToDevice, st));
-    AM_LAUNCH(sp::degree_kernel, sp::row_grid(N), 256, 0, st, p->indptr.p, N, w.p, p->dd.p);
-    AM_LAUNCH(sp::normalise_kernel<double>, sp::row_grid(N), 256, 0, st, p->indptr.p, N, p->indices.p, w.p, p->dd.p,
-              p->s.p);
-    return sp::init_block(p, seed);  // synchronises before w is freed
-  };
-  const int s = body();
-  if (s != AM_OK) {
-    delete p;
-    return s;
-  }
-  *out = p;
+  AM_TRY(p->st.create());
+  cudaStream_t st = p->st.s;
+  DevBuf<double> w;
+  AM_TRY(p->indptr.alloc((size_t)N + 1));
+  AM_TRY(p->indices.alloc((size_t)nnz));
+  AM_TRY(w.alloc((size_t)nnz));
+  AM_TRY(p->s.alloc((size_t)nnz));
+  AM_TRY(p->dd.alloc((size_t)N));
+  AM_CUDA(cudaMemcpyAsync(p->indptr.p, indptr, ((size_t)N + 1) * 8, cudaMemcpyHostToDevice, st));
+  AM_CUDA(cudaMemcpyAsync(p->indices.p, indices, (size_t)nnz * 4, cudaMemcpyHostToDevice, st));
+  AM_CUDA(cudaMemcpyAsync(w.p, weights, (size_t)nnz * 8, cudaMemcpyHostToDevice, st));
+  AM_LAUNCH(sp::degree_kernel, sp::row_grid(N), 256, 0, st, p->indptr.p, N, w.p, p->dd.p);
+  AM_LAUNCH(sp::normalise_kernel<double>, sp::row_grid(N), 256, 0, st, p->indptr.p, N, p->indices.p, w.p, p->dd.p,
+            p->s.p);
+  AM_TRY(sp::init_block(p.get(), seed));  // synchronises before w is freed
+  *out = p.release();
   return AM_OK;
 }
 

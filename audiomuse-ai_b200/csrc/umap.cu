@@ -21,6 +21,7 @@
 
 #include <algorithm>
 #include <cmath>
+#include <memory>
 
 struct am_umap_plan {
   int64_t N = 0;
@@ -273,80 +274,58 @@ extern "C" int am_umap_plan_create(const float* X, int64_t N, int d, int n_neigh
   AM_CHECK(n_epochs >= 1, "am_umap_plan_create: n_epochs = %d must be positive", n_epochs);
   *out = nullptr;
   AM_TRY(ensure_init());
-  auto* p = new am_umap_plan();
+  std::unique_ptr<am_umap_plan> p(new am_umap_plan());
   p->N = N;
   p->k = n_neighbors;
   p->n_epochs = n_epochs;
-  cudaEvent_t ev[3] = {nullptr, nullptr, nullptr};
-  auto body = [&]() -> int {
-    AM_TRY(p->st.create());
-    for (auto& e : ev) AM_CUDA(cudaEventCreate(&e));
-    cudaStream_t st = p->st.s;
-    const int k = n_neighbors;
-    DevBuf<float> dX, kdist;
-    DevBuf<int64_t> kids, ids, u_ptr, off;
-    DevBuf<double> dist, row_sum, total, memb, u_w, wmax;
-    DevBuf<int32_t> u_idx;
-    DevBuf<int> cnt;
-    AM_TRY(dX.alloc((size_t)N * d));
-    AM_CUDA(cudaMemcpyAsync(dX.p, X, (size_t)N * d * 4, cudaMemcpyHostToDevice, st));
-    AM_TRY(kids.alloc((size_t)N * k));
-    AM_TRY(kdist.alloc((size_t)N * k));
-    AM_CUDA(cudaEventRecord(ev[0], st));
-    {
-      am_index* idx = nullptr;
-      AM_TRY(am_knn_build_dev(dX.p, N, d, 1, st, &idx));
-      const int qs = am_knn_query_dev(idx, dX.p, (int)N, k, 0, kids.p, kdist.p, st);
-      am_knn_free(idx);
-      AM_TRY(qs);
-    }
-    AM_CUDA(cudaEventRecord(ev[1], st));
-    AM_TRY(ids.alloc((size_t)N * k));
-    AM_TRY(dist.alloc((size_t)N * k));
-    AM_TRY(row_sum.alloc((size_t)N));
-    AM_TRY(total.alloc(1));
-    AM_TRY(memb.alloc((size_t)N * k));
-    AM_TRY(p->rho.alloc((size_t)N));
-    AM_TRY(p->sigma.alloc((size_t)N));
-    AM_LAUNCH(um::self_first_kernel, um::warp_rows_grid(N), 256, 0, st, dX.p, N, d, kids.p, k, ids.p, dist.p,
-              row_sum.p);
-    AM_LAUNCH(um::sum_kernel, 1, 1024, 0, st, row_sum.p, N, total.p);
-    AM_LAUNCH(um::smooth_knn_kernel, (unsigned)((N + 127) / 128), 128, 0, st, ids.p, dist.p, row_sum.p, total.p, N, k,
-              p->rho.p, p->sigma.p, memb.p);
-    int64_t u_nnz = 0;
-    AM_TRY(knn_csr_build(ids.p, memb.p, N, k, st, u_ptr, u_idx, nullptr, nullptr, &u_w, &u_nnz));
-    AM_TRY(wmax.alloc(1));
-    AM_TRY(cnt.alloc((size_t)N));
-    AM_TRY(p->indptr.alloc((size_t)N + 1));
-    AM_LAUNCH(um::max_kernel, 1, 1024, 0, st, u_w.p, u_nnz, wmax.p);
-    AM_LAUNCH(um::prune_count_kernel, um::warp_rows_grid(N), 256, 0, st, u_ptr.p, N, u_w.p, wmax.p, n_epochs, cnt.p);
-    AM_TRY(csr_scan(cnt.p, N, p->indptr.p, st));
-    AM_CUDA(cudaMemcpyAsync(&p->nnz, p->indptr.p + N, 8, cudaMemcpyDeviceToHost, st));
-    AM_CUDA(cudaStreamSynchronize(st));
-    const size_t m = (size_t)std::max<int64_t>(1, p->nnz);
-    AM_TRY(p->indices.alloc(m));
-    AM_TRY(p->w.alloc(m));
-    AM_TRY(p->eps.alloc(m));
-    AM_TRY(p->next_s.alloc(m));
-    AM_TRY(p->next_n.alloc(m));
-    AM_TRY(p->Y0.alloc((size_t)N * 2));
-    AM_TRY(p->Y1.alloc((size_t)N * 2));
-    AM_LAUNCH(um::prune_copy_kernel, um::warp_rows_grid(N), 256, 0, st, u_ptr.p, u_idx.p, u_w.p, N, wmax.p, n_epochs,
-              p->indptr.p, p->indices.p, p->w.p, p->eps.p);
-    AM_CUDA(cudaEventRecord(ev[2], st));
-    AM_CUDA(cudaStreamSynchronize(st));
-    AM_CUDA(cudaEventElapsedTime(&p->knn_ms, ev[0], ev[1]));
-    AM_CUDA(cudaEventElapsedTime(&p->graph_ms, ev[1], ev[2]));
-    return AM_OK;
-  };
-  const int s = body();
-  for (auto& e : ev)
-    if (e) cudaEventDestroy(e);
-  if (s != AM_OK) {
-    delete p;
-    return s;
-  }
-  *out = p;
+  AM_TRY(p->st.create());
+  Event ev[3];
+  for (auto& e : ev) AM_TRY(e.create());
+  cudaStream_t st = p->st.s;
+  const int k = n_neighbors;
+  DevBuf<float> dX, kdist;
+  DevBuf<int64_t> kids, ids, u_ptr;
+  DevBuf<double> dist, row_sum, total, memb, u_w, wmax;
+  DevBuf<int32_t> u_idx;
+  DevBuf<int> cnt;
+  AM_TRY(knn_self_query(X, N, d, k, st, ev[0], ev[1], dX, kids, kdist));
+  AM_TRY(ids.alloc((size_t)N * k));
+  AM_TRY(dist.alloc((size_t)N * k));
+  AM_TRY(row_sum.alloc((size_t)N));
+  AM_TRY(total.alloc(1));
+  AM_TRY(memb.alloc((size_t)N * k));
+  AM_TRY(p->rho.alloc((size_t)N));
+  AM_TRY(p->sigma.alloc((size_t)N));
+  AM_LAUNCH(um::self_first_kernel, um::warp_rows_grid(N), 256, 0, st, dX.p, N, d, kids.p, k, ids.p, dist.p,
+            row_sum.p);
+  AM_LAUNCH(um::sum_kernel, 1, 1024, 0, st, row_sum.p, N, total.p);
+  AM_LAUNCH(um::smooth_knn_kernel, (unsigned)((N + 127) / 128), 128, 0, st, ids.p, dist.p, row_sum.p, total.p, N, k,
+            p->rho.p, p->sigma.p, memb.p);
+  int64_t u_nnz = 0;
+  AM_TRY(knn_csr_build(ids.p, memb.p, N, k, st, u_ptr, u_idx, nullptr, nullptr, &u_w, &u_nnz));
+  AM_TRY(wmax.alloc(1));
+  AM_TRY(cnt.alloc((size_t)N));
+  AM_TRY(p->indptr.alloc((size_t)N + 1));
+  AM_LAUNCH(um::max_kernel, 1, 1024, 0, st, u_w.p, u_nnz, wmax.p);
+  AM_LAUNCH(um::prune_count_kernel, um::warp_rows_grid(N), 256, 0, st, u_ptr.p, N, u_w.p, wmax.p, n_epochs, cnt.p);
+  AM_TRY(csr_scan(cnt.p, N, p->indptr.p, st));
+  AM_CUDA(cudaMemcpyAsync(&p->nnz, p->indptr.p + N, 8, cudaMemcpyDeviceToHost, st));
+  AM_CUDA(cudaStreamSynchronize(st));
+  const size_t m = (size_t)std::max<int64_t>(1, p->nnz);
+  AM_TRY(p->indices.alloc(m));
+  AM_TRY(p->w.alloc(m));
+  AM_TRY(p->eps.alloc(m));
+  AM_TRY(p->next_s.alloc(m));
+  AM_TRY(p->next_n.alloc(m));
+  AM_TRY(p->Y0.alloc((size_t)N * 2));
+  AM_TRY(p->Y1.alloc((size_t)N * 2));
+  AM_LAUNCH(um::prune_copy_kernel, um::warp_rows_grid(N), 256, 0, st, u_ptr.p, u_idx.p, u_w.p, N, wmax.p, n_epochs,
+            p->indptr.p, p->indices.p, p->w.p, p->eps.p);
+  AM_CUDA(cudaEventRecord(ev[2].e, st));
+  AM_CUDA(cudaStreamSynchronize(st));
+  AM_TRY(add_elapsed_ms(p->knn_ms, ev[0], ev[1]));
+  AM_TRY(add_elapsed_ms(p->graph_ms, ev[1], ev[2]));
+  *out = p.release();
   return AM_OK;
 }
 
@@ -387,33 +366,27 @@ extern "C" int am_umap_plan_layout(am_umap_plan* p, float* emb, int epochs, doub
            "am_umap_plan_layout: need finite a > 0, b > 0, gamma >= 0, neg_rate > 0 and alpha0");
   cudaStream_t st = p->st.s;
   const int64_t N = p->N;
-  cudaEvent_t ev[2] = {nullptr, nullptr};
-  auto body = [&]() -> int {
-    for (auto& e : ev) AM_CUDA(cudaEventCreate(&e));
-    AM_CUDA(cudaMemcpyAsync(p->Y0.p, emb, (size_t)N * 8, cudaMemcpyHostToDevice, st));
-    if (p->nnz > 0)
-      AM_LAUNCH(um::schedule_init_kernel, (unsigned)std::min<int64_t>((p->nnz + 255) / 256, (int64_t)sm_count() * 8),
-                256, 0, st, p->eps.p, p->nnz, neg_rate, p->next_s.p, p->next_n.p);
-    AM_CUDA(cudaEventRecord(ev[0], st));
-    float* cur = p->Y0.p;
-    float* nxt = p->Y1.p;
-    for (int n = 0; n < epochs; ++n) {
-      const double alpha = alpha0 * (1.0 - (double)n / (double)p->n_epochs);
-      AM_LAUNCH(um::layout_epoch_kernel, um::warp_rows_grid(N), 256, 0, st, p->indptr.p, p->indices.p, p->eps.p,
-                p->next_s.p, p->next_n.p, N, reinterpret_cast<const float2*>(cur), reinterpret_cast<float2*>(nxt), a,
-                b, gamma, alpha, neg_rate, n, seed);
-      std::swap(cur, nxt);
-    }
-    AM_CUDA(cudaEventRecord(ev[1], st));
-    AM_CUDA(cudaMemcpyAsync(emb, cur, (size_t)N * 8, cudaMemcpyDeviceToHost, st));
-    AM_CUDA(cudaStreamSynchronize(st));
-    AM_CUDA(cudaEventElapsedTime(&p->layout_ms, ev[0], ev[1]));
-    return AM_OK;
-  };
-  const int s = body();
-  for (auto& e : ev)
-    if (e) cudaEventDestroy(e);
-  return s;
+  Event ev[2];
+  for (auto& e : ev) AM_TRY(e.create());
+  AM_CUDA(cudaMemcpyAsync(p->Y0.p, emb, (size_t)N * 8, cudaMemcpyHostToDevice, st));
+  if (p->nnz > 0)
+    AM_LAUNCH(um::schedule_init_kernel, (unsigned)std::min<int64_t>((p->nnz + 255) / 256, (int64_t)sm_count() * 8),
+              256, 0, st, p->eps.p, p->nnz, neg_rate, p->next_s.p, p->next_n.p);
+  AM_CUDA(cudaEventRecord(ev[0].e, st));
+  float* cur = p->Y0.p;
+  float* nxt = p->Y1.p;
+  for (int n = 0; n < epochs; ++n) {
+    const double alpha = alpha0 * (1.0 - (double)n / (double)p->n_epochs);
+    AM_LAUNCH(um::layout_epoch_kernel, um::warp_rows_grid(N), 256, 0, st, p->indptr.p, p->indices.p, p->eps.p,
+              p->next_s.p, p->next_n.p, N, reinterpret_cast<const float2*>(cur), reinterpret_cast<float2*>(nxt), a, b,
+              gamma, alpha, neg_rate, n, seed);
+    std::swap(cur, nxt);
+  }
+  AM_CUDA(cudaEventRecord(ev[1].e, st));
+  AM_CUDA(cudaMemcpyAsync(emb, cur, (size_t)N * 8, cudaMemcpyDeviceToHost, st));
+  AM_CUDA(cudaStreamSynchronize(st));
+  p->layout_ms = 0.f;  // the latest layout's time, not a sum over calls
+  return add_elapsed_ms(p->layout_ms, ev[0], ev[1]);
 }
 
 extern "C" void am_umap_plan_free(am_umap_plan* p) {
