@@ -33,22 +33,17 @@ extern "C" AM_API int am_debug_block(int path, int B, int H, int W, int cin_p, i
                                      const float* b1, const float* wd, const float* bd, const uint16_t* W2,
                                      const float* b2, uint16_t* Y, uint16_t* E_out, uint16_t* D_out, int* info) {
   using namespace am;
-  AM_CHECK(path == 0 || path == 1, "am_debug_block: path %d", path);
+  AM_CHECK(path >= 0 && path <= 2, "am_debug_block: path %d", path);
   AM_CHECK(B > 0 && H > 0 && W > 0 && (stride == 1 || stride == 2), "am_debug_block: bad shape");
   AM_CHECK(cin_p > 0 && cmid_p > 0 && cout_p > 0 && cin_p % 16 == 0 && cmid_p % 16 == 0 && cout_p % 16 == 0,
            "am_debug_block: channel counts must be positive multiples of 16");
   AM_CHECK(has_expand || cin_p == cmid_p, "am_debug_block: a block without expansion has cin_p == cmid_p");
   AM_CHECK(!residual || (stride == 1 && cin_p == cout_p), "am_debug_block: a residual needs stride 1, cin_p == cout_p");
-  AM_CHECK(X && wd && bd && W2 && b2 && Y && info && (!has_expand || (W1 && b1)), "am_debug_block: NULL operand");
-  AM_TRY(ensure_init());
-  const int Ho = (H - 1) / stride + 1, Wo = (W - 1) / stride + 1;
-  const size_t n_x = (size_t)B * H * W * cin_p, n_e = (size_t)B * H * W * cmid_p;
-  const size_t n_d = (size_t)B * Ho * Wo * cmid_p, n_y = (size_t)B * Ho * Wo * cout_p;
-  const std::vector<float> h_wd(wd, wd + (size_t)9 * cmid_p), h_bd(bd, bd + cmid_p);
+  AM_CHECK(info, "am_debug_block: NULL info");
 
   fused::Plan pl;
   fused::BlockDesc d{};
-  if (path == 0) {  // the plan first: a rejected shape launches nothing
+  if (path != 1) {  // the plan first: a rejected shape launches nothing
     d.H = H;
     d.W = W;
     d.cin_p = cin_p;
@@ -58,7 +53,18 @@ extern "C" AM_API int am_debug_block(int path, int B, int H, int W, int cin_p, i
     d.has_expand = has_expand ? 1 : 0;
     d.residual = residual ? 1 : 0;
     AM_CHECK(fused::plan(d, &pl), "am_debug_block: the fused kernel does not take this block");
+    if (path == 2) {
+      *info = pl.tile_h;
+      return AM_OK;
+    }
   }
+
+  AM_CHECK(X && wd && bd && W2 && b2 && Y && (!has_expand || (W1 && b1)), "am_debug_block: NULL operand");
+  AM_TRY(ensure_init());
+  const int Ho = (H - 1) / stride + 1, Wo = (W - 1) / stride + 1;
+  const size_t n_x = (size_t)B * H * W * cin_p, n_e = (size_t)B * H * W * cmid_p;
+  const size_t n_d = (size_t)B * Ho * Wo * cmid_p, n_y = (size_t)B * Ho * Wo * cout_p;
+  const std::vector<float> h_wd(wd, wd + (size_t)9 * cmid_p), h_bd(bd, bd + cmid_p);
 
   DevBuf<__nv_bfloat16> dX, dW1, dW2, dE, dD, dY;
   DevBuf<float> db1, dwd, dbd, db2, dparams;

@@ -1,29 +1,35 @@
 // Fused inverted-residual block on sm_90a: [1x1 expand + ReLU6] -> 3x3 depthwise + ReLU6 -> 1x1 project [+ residual]
 // in one kernel, so the expanded tensor (6x the block width) never goes to HBM.
 //
-// Persistent, warp-specialised CTA of three warpgroups (tma_pipeline.cuh), each CTA looping over 8 x 8 output tiles:
-//   warpgroup 0   TMA producer (one elected lane): per tile the input halo (10 x 10 pixels at stride 1, 17 x 17 at
-//                 stride 2) through a 4-D NHWC tensor map as K-major 128-byte-swizzled bf16 rows, zero filled outside
-//                 the image and past cin_p; per 64-channel chunk of the expansion, into a ring of as many stages as fit
-//                 (up to 4): the W1 and W2 chunks (2-D maps, zero filled past cmid_p / cout_p) or, without an expansion
-//                 conv, the input's channel chunk itself, and the chunk's depthwise weights and biases and expansion
-//                 bias in one bulk copy (packed per chunk at model load, pack_params).  The next tile's halo and first
-//                 chunks load while the consumers finish the current tile.
+// Persistent, warp-specialised CTA of three warpgroups (tma_pipeline.cuh), each CTA looping over output tiles 8 mel
+// columns wide and 8 time rows high, or 16 (the tall tile) for a stride-1 block with cout_p <= 128 whose ring stays
+// as deep (plan()); the height is a kernel parameter, chosen outside every K loop:
+//   warpgroup 0   TMA producer (one elected lane): per tile the input halo (10 x 10 pixels at stride 1, 18 x 10 for
+//                 the tall tile, 17 x 17 at stride 2) through a 4-D NHWC tensor map as K-major 128-byte-swizzled
+//                 bf16 rows, zero filled outside the image and past cin_p; per 64-channel chunk of the expansion, into
+//                 a ring of as many stages as fit (up to 4): the W1 and W2 chunks (2-D maps, zero filled past cmid_p /
+//                 cout_p) or, without an expansion conv, the input's channel chunk itself, and the chunk's depthwise
+//                 weights and biases and expansion bias in one bulk copy (packed per chunk at model load,
+//                 pack_params).  The next tile's halo and first chunks load while the consumers finish the current
+//                 tile.
 //   warpgroups 1, 2   consumers, sharing one tile; per chunk:
 //     expansion   transposed, E^T = W1 chunk . halo^T, so the halo pixels are the MMA's N: each warpgroup one
 //                 contiguous run of 8-pixel atoms (wgmma m64n152k16 / m64n144k16 at stride 2, m64n56k16 / m64n48k16
-//                 at stride 1); fp32 accumulators -> + bias, ReLU6 -> bf16, stored back pixel-major by stmatrix
+//                 at stride 1, m64n96k16 / m64n88k16 for the tall tile's 184 halo rows); fp32 accumulators -> + bias,
+//                 ReLU6 -> bf16, stored back pixel-major by stmatrix
 //                 .trans into the halo tile E [halo pixels x 64, 16-byte groups XOR-swizzled by pixel] (pixels
 //                 outside the image are zero: the depthwise pads with 0, and relu6(bias) need not be);
 //     depthwise   3 x 3 taps from E in fp32 (a thread = 2 channels of one output column, walking its input rows) +
-//                 bias, ReLU6 -> bf16, written as the K-major swizzled A operand [64 pixels x 64 channels] of
-//     projection  wgmma m64n(Cout / 2)k16 into register accumulators, one half of the output columns per warpgroup
-//                 (Cout <= 256), accumulated over the chunks in ascending order.
+//                 bias, ReLU6 -> bf16, written as the K-major swizzled A operand [tile pixels x 64 channels] of
+//     projection  wgmma into register accumulators, accumulated over the chunks in ascending order: for an 8 x 8
+//                 tile m64n(Cout / 2)k16, one half of the output columns per warpgroup (Cout <= 256); for a tall
+//                 tile m64n(Cout)k16, 64 of A's 128 rows per warpgroup (Cout <= 128).
 //   With two or more stages the chunks overlap: chunk c + 1's expansion MMAs are issued before chunk c's depthwise and
 //   run under it (they write only registers), and its epilogue refills E after chunk c's projection.  Two named
 //   barriers per chunk order E and the A operand between the consumer warpgroups; both retire their projection before
 //   the first, so one A buffer serves.
-// Epilogue: + bias (+ the block input for a residual block) -> bf16, straight from the registers.
+// Epilogue: + bias (+ the block input for a residual block) -> bf16, straight from the registers; every bias and
+// residual value is loaded before the first store.
 // Rounding follows the layer-by-layer path: the expansion and the depthwise output are rounded to bf16, every sum is
 // fp32, in the same order for every element.
 #include "fused_block.cuh"
@@ -38,7 +44,8 @@ namespace fused {
 
 using namespace ptx;
 
-constexpr int kTile = 8;        // output tile edge: 64 pixels = one m64 projection
+constexpr int kTile = 8;        // output tile width (mel columns), and the height of the square tile: 64 pixels
+constexpr int kTallTile = 16;   // height (time rows) of the tall tile at stride 1: 128 pixels
 constexpr int kChunk = 64;      // expansion channels per pass = one 128-byte swizzle row of projection K
 constexpr int kMaxCout = 256;
 constexpr int kMaxStages = 4;
@@ -50,9 +57,18 @@ constexpr int kParamRows = 9 + 1 + 1;
 constexpr uint32_t kDwBytes = kParamRows * kChunk * 4;
 using Ring = pipe::Ring<kMaxStages>;
 
+// the input halo of a tile th output rows high: halo(S) pixels wide, halo_h high, halo_px pixels
 __host__ __device__ constexpr int halo(int S) { return (kTile - 1) * S + 3; }
-__host__ __device__ constexpr int halo_px(int S) { return halo(S) * halo(S); }
-__host__ __device__ constexpr int halo_rows(int S) { return (halo_px(S) + 63) / 64 * 64; }
+__host__ __device__ constexpr int halo_h(int S, int th) { return (th - 1) * S + 3; }
+__host__ __device__ constexpr int halo_px(int S, int th) { return halo_h(S, th) * halo(S); }
+// shared-memory rows of one 64-channel block of the halo: the 8 x 8 tile's rounded to 64, the tall tile's to whole
+// 8-pixel atoms (184 for 180 pixels: at 192 block 2 of the shipped student would lose a ring stage)
+__host__ __device__ constexpr int halo_rows(int S, int th) {
+  return th == kTile ? (halo_px(S, th) + 63) / 64 * 64 : (halo_px(S, th) + 7) / 8 * 8;
+}
+// the expansion's split of the halo pixels, rounded up to whole 8-pixel atoms, between the two consumer warpgroups
+__host__ __device__ constexpr int en0(int px) { return ((px + 7) / 8 + 1) / 2 * 8; }
+__host__ __device__ constexpr int en1(int px) { return (px + 7) / 8 * 8 - en0(px); }
 
 constexpr uint32_t round1k(uint32_t v) { return (v + 1023u) & ~1023u; }
 
@@ -68,16 +84,19 @@ __device__ __forceinline__ uint32_t sw128(uint32_t row, uint32_t chunk) {
 // Shared memory: the ring of per-chunk stages, then the kernel's own region (offsets from its start).
 //   stage (expand):     [W1 chunk: kbx x 64 rows x 128 B][W2 chunk: n2 rows x 128 B][depthwise params]
 //   stage (no expand):  [input chunk: halo pixels x 128 B][W2 chunk][depthwise params]
-//   own region:         [input halo: kbx x HR rows x 128 B][projection A: 64 x 128 B][E: halo pixels x 128 B][2 barriers]
+//   own region:         [input halo: kbx x hr rows x 128 B][projection A: tile pixels x 128 B][E: halo pixels x 128 B]
+//                       [2 barriers]
 struct Layout {
   uint32_t stage, w2, dw;     // stage bytes, offsets of W2 and the depthwise params inside a stage
   uint32_t xs, a2, e, bars, extra;
+  int hr;                     // halo_rows of the tile
+  int th;                     // output rows of a tile: kTile, or kTallTile at stride 1
   int stages;
   size_t smem;
 };
 
-static Layout layout(int S, bool has_expand, int cin_p, int cout_p, int stages) {
-  const uint32_t hr = (uint32_t)halo_rows(S), hpx = (uint32_t)halo_px(S);
+static Layout layout(int S, int th, bool has_expand, int cin_p, int cout_p, int stages) {
+  const uint32_t hr = (uint32_t)halo_rows(S, th), hpx = (uint32_t)halo_px(S, th);
   const uint32_t kbx = has_expand ? (uint32_t)((cin_p + 63) / 64) : 0u;
   const uint32_t n2 = (uint32_t)((cout_p + 63) / 64 * 64);
   Layout l;
@@ -86,9 +105,11 @@ static Layout layout(int S, bool has_expand, int cin_p, int cout_p, int stages) 
   l.stage = round1k(l.dw + kDwBytes);
   l.xs = 0;
   l.a2 = l.xs + kbx * hr * 128;
-  l.e = l.a2 + kTile * kTile * 128;
+  l.e = l.a2 + (uint32_t)(th * kTile * 128);
   l.bars = l.e + (has_expand ? hpx * 128 : 0u);
   l.extra = l.bars + 2 * sizeof(uint64_t);
+  l.hr = (int)hr;
+  l.th = th;
   l.stages = stages;
   l.smem = Ring::smem_bytes(l.stage, stages, l.extra);
   return l;
@@ -142,7 +163,11 @@ __global__ void __launch_bounds__(pipe::kThreads, 1)
 fused_block_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_w1,
                    const __grid_constant__ CUtensorMap map_w2, const Args a) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  constexpr int HALO = halo(S), HPX = halo_px(S), HR = halo_rows(S);
+  constexpr int HALO = halo(S);  // halo pixels per row, for both tile heights
+  constexpr int PX8 = halo_px(S, kTile), PXT = halo_px(S, kTallTile);
+  // The tile height is a kernel parameter, so the choice is uniform across the CTA; stride 2 takes 8 x 8 tiles only.
+  const bool tall = S == 1 && a.l.th == kTallTile;
+  const int hpx = tall ? PXT : PX8, hr = a.l.hr;
   Ring ring(smem_raw, a.l.stage, a.l.stages, a.l.extra);
   uint8_t* own = ring.extra();
   uint8_t* xs = own + a.l.xs;
@@ -172,17 +197,17 @@ fused_block_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_const
       uint32_t xs_phase = 0;
       for (int tile = blockIdx.x; tile < a.num_tiles; tile += gridDim.x) {
         const int b = tile / per_img, ty = (tile % per_img) / a.tiles_x, tx = tile % a.tiles_x;
-        const int gy0 = ty * kTile * S - 1, gx0 = tx * kTile * S - 1;  // image position of halo pixel (0, 0)
+        const int gy0 = ty * a.l.th * S - 1, gx0 = tx * kTile * S - 1;  // image position of halo pixel (0, 0)
         if (kExpand) {
           clk.lap(kIssue);
           mbar_wait(xs_empty, xs_phase ^ 1);
           clk.lap(kHaloWait);
-          mbar_expect_tx(xs_full, (uint32_t)(kbx * HPX * 128));
-          for (int kb = 0; kb < kbx; ++kb) tma_load_4d(xs + kb * HR * 128, &map_x, xs_full, kb * 64, gx0, gy0, b);
+          mbar_expect_tx(xs_full, (uint32_t)(kbx * hpx * 128));
+          for (int kb = 0; kb < kbx; ++kb) tma_load_4d(xs + kb * hr * 128, &map_x, xs_full, kb * 64, gx0, gy0, b);
           xs_phase ^= 1;
         }
         for (int c0 = 0; c0 < a.cmid_p; c0 += kChunk) {
-          const uint32_t tx_bytes = (kExpand ? (uint32_t)kbx * kChunk * 128 : (uint32_t)HPX * 128) +
+          const uint32_t tx_bytes = (kExpand ? (uint32_t)kbx * kChunk * 128 : (uint32_t)hpx * 128) +
                                     (uint32_t)n2_blocks * 64 * 128 + kDwBytes;
           clk.lap(kIssue);
           const Ring::Slot s = ring.acquire(tx_bytes);
@@ -213,31 +238,45 @@ fused_block_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_const
   // cannot hold both, so there the expansion waits for chunk c's projection and the stage it frees.
   const bool ahead = a.l.stages > 1;
 
+  // Calls f(std::integral_constant<int, tile height>), so that the code for each tile height has its sizes as
+  // compile-time constants; the choice is made once, outside every K loop.
+  auto with_tile = [&](auto f) {
+    if constexpr (S == 1) {
+      if (tall) return f(std::integral_constant<int, kTallTile>{});
+    }
+    return f(std::integral_constant<int, kTile>{});
+  };
+
   // The expansion runs transposed, E^T [64 channels x halo pixels] = W1 chunk . halo^T: the stage's W1 chunk (64
   // K-major rows) is the A operand and the halo rows are B, so the halo pixels are the MMA's wide dimension.  The
-  // pixels, rounded up to whole 8-row atoms, split between the warpgroups as evenly as whole atoms allow: 152 + 144 at
-  // stride 2, 56 + 48 at stride 1.  Halo rows past HPX are stale and give accumulator columns that are never stored.
-  constexpr int kEN0 = ((HPX + 7) / 8 + 1) / 2 * 8;  // pixels of warpgroup 0
-  constexpr int kEN1 = (HPX + 7) / 8 * 8 - kEN0;     // pixels of warpgroup 1, from kEN0 on
-  // the projection: each warpgroup one half of the output columns, [wg half, (wg + 1) half)
+  // pixels, rounded up to whole 8-row atoms, split between the warpgroups as evenly as whole atoms allow (en0 / en1):
+  // 152 + 144 at stride 2, 56 + 48 at stride 1, 96 + 88 for the tall tile.  Halo rows past the halo's pixels are stale
+  // and give accumulator columns that are never stored.
+  // The projection: an 8 x 8 tile gives each warpgroup all 64 rows of A and one half of the output columns,
+  // [wg half, (wg + 1) half); a tall tile gives each warpgroup 64 of A's 128 rows and all cout_p (<= 128) columns.
   const int half = a.cout_p / 2;
+  const int proj_n = tall ? a.cout_p : half;       // columns of this warpgroup's projection MMA
+  const int proj_col = tall ? 0 : wg * half;       // its first output column
+  const int proj_row = tall ? 64 * wg : 0;         // its first row of A (output pixel of the tile)
 
   // the first MMA of every expansion and of every tile's projection overwrites (scale_d = 0)
-  float acc1[kEN0 / 2];  // expansion: channels 16 warp + lane / 4 (+ 8) of pixels p0 + 8 j + 2 quad (+ 1)
-  float acc2[kMaxCout / 4];  // projection: output columns wg half + 8 j + 2 quad (+ 1), j < half / 8
+  constexpr int kAcc1 = en0(S == 1 ? PXT : PX8) / 2;  // the widest expansion of the kernel's tile heights
+  float acc1[kAcc1];  // expansion: channels 16 warp + lane / 4 (+ 8) of pixels p0 + 8 j + 2 quad (+ 1)
+  float acc2[kMaxCout / 4];  // projection: output columns proj_col + 8 j + 2 quad (+ 1), j < proj_n / 8
 #pragma unroll
-  for (int i = 0; i < kEN0 / 2; ++i) acc1[i] = 0.f;
+  for (int i = 0; i < kAcc1; ++i) acc1[i] = 0.f;
 #pragma unroll
   for (int i = 0; i < kMaxCout / 4; ++i) acc2[i] = 0.f;
 
   // acc1 = W1 chunk . this warpgroup's halo rows^T, issued and committed, not waited for
   // (the width is chosen outside the K loop, so that each warpgroup's MMAs form one straight run ptxas can batch)
   auto expand_issue = [&](const uint8_t* stage) {
-    const uint32_t w1 = smem_u32(stage), px = smem_u32(xs) + (uint32_t)(wg * kEN0 * 128);
-    auto issue = [&](auto width) {
+    const uint32_t w1 = smem_u32(stage);
+    auto issue = [&](auto width, int p0) {
+      const uint32_t px = smem_u32(xs) + (uint32_t)(p0 * 128);
       for (int kb = 0; kb < kbx; ++kb) {
         const uint64_t da = make_smem_desc(w1 + (uint32_t)(kb * kChunk * 128));
-        const uint64_t db = make_smem_desc(px + (uint32_t)(kb * HR * 128));
+        const uint64_t db = make_smem_desc(px + (uint32_t)(kb * hr * 128));
         const int ksteps = min(4, (a.cin_p - kb * 64) / 16);
         for (int ks = 0; ks < ksteps; ++ks)
           wgmma_into<decltype(width)::value>(acc1, da + (uint64_t)(ks * 2), db + (uint64_t)(ks * 2),
@@ -245,33 +284,39 @@ fused_block_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_const
       }
     };
     wgmma_fence();
-    if (wg == 0) issue(std::integral_constant<int, kEN0>{});
-    else issue(std::integral_constant<int, kEN1>{});
+    with_tile([&](auto th) {
+      constexpr int PX = halo_px(S, decltype(th)::value);
+      if (wg == 0) issue(std::integral_constant<int, en0(PX)>{}, 0);
+      else issue(std::integral_constant<int, en1(PX)>{}, en0(PX));
+    });
     wgmma_commit();
   };
   // Bit 2 j + k of this thread's mask: halo pixel p0 + 8 j + 2 quad + k of its warpgroup lies inside the image.  It
   // depends on the tile only, so it is computed once per tile rather than in every chunk's epilogue.  The pixels'
-  // halo coordinates do not depend on the tile; the empty asm keeps the compiler from hoisting all 2 x kEN0 / 4 of
+  // halo coordinates do not depend on the tile; the empty asm keeps the compiler from hoisting all 2 x en0 / 4 of
   // them out of the tile loop, where they would not fit in the registers the chunk loop leaves.
   auto inside_mask = [&](int gy0, int gx0) {
-    int p0 = wg * kEN0 + 2 * quad;
-    asm volatile("" : "+r"(p0));
-    uint64_t m = 0;
+    return with_tile([&](auto th) {
+      constexpr int EN0 = en0(halo_px(S, decltype(th)::value));
+      int p0 = wg * EN0 + 2 * quad;
+      asm volatile("" : "+r"(p0));
+      uint64_t m = 0;
 #pragma unroll
-    for (int j = 0; j < kEN0 / 8; ++j)
+      for (int j = 0; j < EN0 / 8; ++j)
 #pragma unroll
-      for (int k = 0; k < 2; ++k) {
-        const int p = p0 + 8 * j + k;
-        const int gy = gy0 + p / HALO, gx = gx0 + p % HALO;
-        if (gy >= 0 && gy < a.H && gx >= 0 && gx < a.W) m |= 1ull << (2 * j + k);
-      }
-    return m;
+        for (int k = 0; k < 2; ++k) {
+          const int p = p0 + 8 * j + k;
+          const int gy = gy0 + p / HALO, gx = gx0 + p % HALO;
+          if (gy >= 0 && gy < a.H && gx >= 0 && gx < a.W) m |= 1ull << (2 * j + k);
+        }
+      return m;
+    });
   };
   // E pixels of this warpgroup = relu6(acc1 + b1), zero outside the image and past the chunk's channels.  A thread's
   // bf16 pair (channel r + 8 h, pixels 8 j + 2 quad, + 1) is one register of the 8 x 8 fragment (pixel group j,
   // channel group 2 warp + h); stmatrix .trans writes the fragments back pixel-major, each pixel's 8 channels one
-  // 16-byte group at e_off, so E keeps the layout the depthwise reads.  The pixel groups past HPX's last whole atom
-  // (warpgroup 1's last one) store element by element, stopping at HPX.
+  // 16-byte group at e_off, so E keeps the layout the depthwise reads.  The pixel groups past the halo's last whole
+  // atom (warpgroup 1's last one) store element by element, stopping at the halo's last pixel.
   auto expand_epilogue = [&](const uint8_t* stage, int nch, uint64_t inside) {
     reg_fence(acc1);
     const float* b1 = reinterpret_cast<const float*>(stage + a.l.dw) + 10 * kChunk;
@@ -289,10 +334,11 @@ fused_block_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_const
                                                      relu6f(acc1[4 * j + 2 * h + 1] + bias[h]));
       return *reinterpret_cast<const uint32_t*>(&v) & mask;
     };
-    auto store = [&](auto wgc) {
-      constexpr int P0 = decltype(wgc)::value * kEN0;
-      constexpr int NG = (decltype(wgc)::value ? kEN1 : kEN0) / 8;  // pixel groups of this warpgroup
-      constexpr int NFULL = (HPX - P0) / 8 < NG ? (HPX - P0) / 8 : NG;  // those entirely below HPX
+    auto store = [&](auto wgc, auto th) {
+      constexpr int HPX = halo_px(S, decltype(th)::value);
+      constexpr int P0 = decltype(wgc)::value * en0(HPX);
+      constexpr int NG = (decltype(wgc)::value ? en1(HPX) : en0(HPX)) / 8;  // pixel groups of this warpgroup
+      constexpr int NFULL = (HPX - P0) / 8 < NG ? (HPX - P0) / 8 : NG;     // those entirely below HPX
       // lane 8 i + k addresses row k of matrix i: pixel group j + i / 2, channel group 2 warp + i % 2
       const int mi = lane >> 3;
       const uint32_t e_base = smem_u32(e_own);
@@ -319,15 +365,17 @@ fused_block_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_const
           }
         }
     };
-    if (wg == 0) store(std::integral_constant<int, 0>{});
-    else store(std::integral_constant<int, 1>{});
+    with_tile([&](auto th) {
+      if (wg == 0) store(std::integral_constant<int, 0>{}, th);
+      else store(std::integral_constant<int, 1>{}, th);
+    });
   };
 
   PhaseClock clk;
   uint32_t xs_phase = 0;
   for (int tile = blockIdx.x; tile < a.num_tiles; tile += gridDim.x) {
     const int b = tile / per_img, ty = (tile % per_img) / a.tiles_x, tx = tile % a.tiles_x;
-    const int oy0 = ty * kTile, ox0 = tx * kTile;
+    const int oy0 = ty * a.l.th, ox0 = tx * kTile;
     const int gy0 = oy0 * S - 1, gx0 = ox0 * S - 1;
     const uint64_t inside = kExpand ? inside_mask(gy0, gx0) : 0;
     if (kExpand) {
@@ -364,25 +412,34 @@ fused_block_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_const
 
       // depthwise: a thread = one channel pair (2 cp, 2 cp + 1) of one output column ox, a warp = all 64 channels of
       // that column, so every E load and A store of a warp is one 128-byte pixel row (conflict-free under the XOR
-      // swizzles).  The thread walks the column's HALO input rows top to bottom, converts each of the row's 3 taps once
-      // and adds it into every output row that uses it; per output the order stays bias, then dy and dx ascending.
-      {
+      // swizzles).  The thread walks the column's input rows top to bottom, converts each of the row's 3 taps once and
+      // adds it into every output row that uses it; per output the order stays bias, then dy and dx ascending.  The
+      // 8 x 8 tile keeps its 8 output rows and stores them at the end; the tall tile stores each of its 16 rows as
+      // soon as its last tap is in, so only about 3 rows of accumulators are live.
+      with_tile([&](auto th) {
+        constexpr int TH = decltype(th)::value, HH = halo_h(S, TH);
         const int ox = ct >> 5, cp = lane, g = cp >> 2;
-        uint32_t out[kTile] = {};  // bf16 pairs of output rows 0 .. 7; lanes past the chunk's channels write zeros
+        // A row 8 oy + ox: its swizzle depends on ox only (sw128 takes the row mod 8)
+        uint8_t* arow = a2 + sw128(ox, g) + 4 * (cp & 3);
+        auto put = [&](int oy, uint32_t v) { *reinterpret_cast<uint32_t*>(arow + oy * kTile * 128) = v; };
         if (2 * cp < nch) {
           float2 w[9];
 #pragma unroll
           for (int t = 0; t < 9; ++t) w[t] = *reinterpret_cast<const float2*>(dwp + t * kChunk + 2 * cp);
           const float2 bias = *reinterpret_cast<const float2*>(dwp + 9 * kChunk + 2 * cp);
-          float2 acc[kTile];
+          float2 acc[TH];
 #pragma unroll
-          for (int oy = 0; oy < kTile; ++oy) acc[oy] = bias;
+          for (int oy = 0; oy < TH; ++oy) acc[oy] = bias;
+          auto out = [&](int oy) {  // bf16 pair of output row oy
+            const __nv_bfloat162 o = __floats2bfloat162_rn(relu6f(acc[oy].x), relu6f(acc[oy].y));
+            return *reinterpret_cast<const uint32_t*>(&o);
+          };
           // halo pixel ox * S + d (d = iy * HALO + dx) is at col[d & 7] + 64 d: its swizzle depends on d only mod 8
           const __nv_bfloat16* col[8];
 #pragma unroll
           for (int k = 0; k < 8; ++k) col[k] = e + ox * S * 64 + ((g ^ ((ox * S + k) & 7)) << 3) + 2 * (cp & 3);
 #pragma unroll
-          for (int iy = 0; iy < HALO; ++iy) {
+          for (int iy = 0; iy < HH; ++iy) {
             float2 v[3];
 #pragma unroll
             for (int dx = 0; dx < 3; ++dx) {
@@ -391,7 +448,7 @@ fused_block_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_const
             }
 #pragma unroll
             for (int dy = 0; dy < 3; ++dy) {  // output row oy takes input row iy as its tap row dy
-              if (iy < dy || (iy - dy) % S != 0 || (iy - dy) / S >= kTile) continue;
+              if (iy < dy || (iy - dy) % S != 0 || (iy - dy) / S >= TH) continue;
               const int oy = (iy - dy) / S;
 #pragma unroll
               for (int dx = 0; dx < 3; ++dx) {
@@ -399,35 +456,38 @@ fused_block_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_const
                 acc[oy].y = fmaf(v[dx].y, w[dy * 3 + dx].y, acc[oy].y);
               }
             }
+            if constexpr (TH != kTile) {  // stride 1: input row iy is output row iy - 2's last tap row
+              if (iy >= 2) put(iy - 2, out(iy - 2));
+            }
           }
+          if constexpr (TH == kTile) {
 #pragma unroll
-          for (int oy = 0; oy < kTile; ++oy) {
-            const __nv_bfloat162 o = __floats2bfloat162_rn(relu6f(acc[oy].x), relu6f(acc[oy].y));
-            out[oy] = *reinterpret_cast<const uint32_t*>(&o);
+            for (int oy = 0; oy < TH; ++oy) put(oy, out(oy));
           }
+        } else {  // a lane past the chunk's channels writes zeros
+#pragma unroll
+          for (int oy = 0; oy < TH; ++oy) put(oy, 0u);
         }
-        // A row 8 oy + ox: its swizzle depends on ox only (sw128 takes the row mod 8)
-        uint8_t* arow = a2 + sw128(ox, g) + 4 * (cp & 3);
-#pragma unroll
-        for (int oy = 0; oy < kTile; ++oy) *reinterpret_cast<uint32_t*>(arow + oy * kTile * 128) = out[oy];
-      }
+      });
       fence_proxy_async();  // generic-proxy writes of A -> visible to the wgmma (async proxy) reads
       clk.lap(kDepthwise);
       // A is complete, and both warpgroups are done reading E
       named_bar_sync(kConsumerBar, pipe::kConsumerThreads);
       clk.lap(kBarrier);
 
-      // projection: acc2 += A2 [64 x nch] . W2_chunk rows [wg half, (wg + 1) half)^T, one MMA of width half per k step
+      // projection: acc2 += A2 rows [proj_row, + 64) . W2_chunk rows [proj_col, + proj_n)^T, one MMA of width proj_n
+      // per k step
       wgmma_fence();
       {
-        const uint64_t da = make_smem_desc(smem_u32(a2));
-        const uint64_t db = make_smem_desc(smem_u32(sp) + a.l.w2 + (uint32_t)(wg * half * 128));
+        const uint64_t da = make_smem_desc(smem_u32(a2) + (uint32_t)(proj_row * 128));
+        const uint64_t db = make_smem_desc(smem_u32(sp) + a.l.w2 + (uint32_t)(proj_col * 128));
         auto project = [&](auto width) {
           for (int ks = 0; ks < nch / 16; ++ks)
             wgmma_into<decltype(width)::value>(acc2, da + (uint64_t)(ks * 2), db + (uint64_t)(ks * 2),
                                                (c0 | ks) ? 1u : 0u);
         };
-        switch (half) {  // cout_p is a multiple of 16 and at most kMaxCout (plan())
+        // cout_p is a multiple of 16 and at most kMaxCout, and at most 128 for a tall tile (plan())
+        switch (proj_n) {
           case 8: project(std::integral_constant<int, 8>{}); break;
           case 16: project(std::integral_constant<int, 16>{}); break;
           case 24: project(std::integral_constant<int, 24>{}); break;
@@ -469,25 +529,49 @@ fused_block_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_const
       }
     }
 
-    // epilogue: + bias (+ block input) -> bf16
+    // epilogue: + bias (+ block input) -> bf16.  A thread holds pixels proj_row + 16 warp + lane / 4 (+ 8) of the tile,
+    // columns proj_col + 8 j + 2 quad (+ 1).  Every bias and residual value is loaded before the first store: as far as
+    // the compiler knows Y may alias b2 and X, so a load placed after a store would wait for it, one global-load
+    // latency per column pair.
+    {
+      constexpr int J = kMaxCout / 16;  // column groups of 8 a warpgroup holds at most
+      bool in[2];
+      int64_t pix[2];
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int px = warp * 16 + (lane >> 2) + 8 * h;
-      const int oy = oy0 + (px >> 3), ox = ox0 + (px & 7);
-      if (oy >= a.Ho || ox >= a.Wo) continue;
-      const int64_t pix = ((int64_t)b * a.Ho + oy) * a.Wo + ox;
+      for (int h = 0; h < 2; ++h) {
+        const int px = proj_row + warp * 16 + (lane >> 2) + 8 * h;
+        const int oy = oy0 + (px >> 3), ox = ox0 + (px & 7);
+        in[h] = oy < a.Ho && ox < a.Wo;
+        pix[h] = ((int64_t)b * a.Ho + oy) * a.Wo + ox;
+      }
+      float2 bias[J];
+      uint32_t res[2][J];  // bf16 pairs of the block input (stride 1, cin_p == cout_p) at the same pixel
 #pragma unroll
-      for (int j = 0; j < kMaxCout / 16; ++j) {
-        if (8 * j >= half) break;
-        const int n = wg * half + 8 * j + 2 * quad;
-        float f0 = acc2[4 * j + 2 * h] + __ldg(&a.b2[n]);
-        float f1 = acc2[4 * j + 2 * h + 1] + __ldg(&a.b2[n + 1]);
-        if (a.residual) {  // stride 1, cin_p == cout_p: the block input at the same pixel
-          const float2 r = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(a.X + pix * a.cin_p + n));
-          f0 += r.x;
-          f1 += r.y;
+      for (int j = 0; j < J; ++j) {
+        bias[j] = make_float2(0.f, 0.f);
+        res[0][j] = res[1][j] = 0u;
+        if (8 * j >= proj_n) continue;
+        const int n = proj_col + 8 * j + 2 * quad;
+        bias[j] = make_float2(__ldg(&a.b2[n]), __ldg(&a.b2[n + 1]));
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+          if (a.residual && in[h]) res[h][j] = *reinterpret_cast<const uint32_t*>(a.X + pix[h] * a.cin_p + n);
+      }
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        if (!in[h]) continue;
+#pragma unroll
+        for (int j = 0; j < J; ++j) {
+          if (8 * j >= proj_n) break;
+          const int n = proj_col + 8 * j + 2 * quad;
+          float f0 = acc2[4 * j + 2 * h] + bias[j].x;
+          float f1 = acc2[4 * j + 2 * h + 1] + bias[j].y;
+          if (a.residual) {
+            f0 += __uint_as_float(res[h][j] << 16);
+            f1 += __uint_as_float(res[h][j] & 0xffff0000u);
+          }
+          *reinterpret_cast<__nv_bfloat162*>(a.Y + pix[h] * a.cout_p + n) = __floats2bfloat162_rn(f0, f1);
         }
-        *reinterpret_cast<__nv_bfloat162*>(a.Y + pix * a.cout_p + n) = __floats2bfloat162_rn(f0, f1);
       }
     }
     clk.lap(kEpilogue);
@@ -502,7 +586,7 @@ fused_block_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_const
 // one-stage layout is never larger for blocks with an expansion (E holds only the halo pixels, not 64-row blocks), and
 // at most 48 bytes larger for the no-expansion blocks, whose working set is far below the limit.
 static bool fits(const BlockDesc& d) {
-  const size_t hr = (size_t)halo_rows(d.stride);
+  const size_t hr = (size_t)halo_rows(d.stride, kTile);
   const size_t kbx = d.has_expand ? (size_t)((d.cin_p + 63) / 64) : 0;
   const size_t n2 = (size_t)((d.cout_p + 63) / 64 * 64);
   const size_t set = kbx * hr * 128 + kbx * kChunk * 128 + n2 * 128 + 64 * 128 + hr * 128;
@@ -515,9 +599,23 @@ bool plan(const BlockDesc& d, Plan* out) {
   if (!d.has_expand && d.cin_p != d.cmid_p) return false;
   if (d.residual && (d.stride != 1 || d.cin_p != d.cout_p)) return false;
   if (!fits(d)) return false;
-  Layout l = layout(d.stride, d.has_expand != 0, d.cin_p, d.cout_p, kMaxStages);
-  for (int s = kMaxStages - 1; s >= 1 && l.smem > kSmemMax; --s) l = layout(d.stride, d.has_expand != 0, d.cin_p, d.cout_p, s);
+  auto deepest = [&](int th) {  // the layout with as many ring stages as fit
+    Layout l = layout(d.stride, th, d.has_expand != 0, d.cin_p, d.cout_p, kMaxStages);
+    for (int s = kMaxStages - 1; s >= 1 && l.smem > kSmemMax; --s)
+      l = layout(d.stride, th, d.has_expand != 0, d.cin_p, d.cout_p, s);
+    return l;
+  };
+  Layout l = deepest(kTile);
+  // The tall tile halves the per-pixel share of each chunk's fixed costs (barriers, ring and halo waits, MMA issue)
+  // and runs the expansion over 184 halo pixels per 128 outputs instead of 104 per 64.  It needs stride 1, cout_p <=
+  // 128 so that one warpgroup's projection over all the columns keeps 64 accumulator registers, and as deep a ring as
+  // the 8 x 8 tile: a shallower ring would stall the pipeline more than the tile saves.
+  if (d.stride == 1 && d.cout_p <= 128) {
+    const Layout t = deepest(kTallTile);
+    if (t.smem <= kSmemMax && t.stages == l.stages) l = t;
+  }
   out->stages = l.stages;
+  out->tile_h = l.th;
   out->smem_bytes = l.smem;
   return out->smem_bytes <= kSmemMax;
 }
@@ -574,7 +672,9 @@ int run(const BlockDesc& d, const Plan& p, const __nv_bfloat16* X, const __nv_bf
   a.W = d.W;
   a.Ho = (d.H - 1) / d.stride + 1;  // 3 x 3, pad 1
   a.Wo = (d.W - 1) / d.stride + 1;
-  a.tiles_y = (a.Ho + kTile - 1) / kTile;
+  AM_CHECK(p.tile_h == kTile || (p.tile_h == kTallTile && d.stride == 1 && d.cout_p <= 128),
+           "fused block: plan does not match the block");
+  a.tiles_y = (a.Ho + p.tile_h - 1) / p.tile_h;
   a.tiles_x = (a.Wo + kTile - 1) / kTile;
   const int64_t tiles = (int64_t)B * a.tiles_y * a.tiles_x;
   AM_CHECK(tiles < ((int64_t)1 << 31), "fused block: %lld tiles is too many for one launch", (long long)tiles);
@@ -583,13 +683,12 @@ int run(const BlockDesc& d, const Plan& p, const __nv_bfloat16* X, const __nv_bf
   a.cmid_p = d.cmid_p;
   a.cout_p = d.cout_p;
   a.residual = d.residual;
-  const Layout l = layout(d.stride, d.has_expand != 0, d.cin_p, d.cout_p, p.stages);
+  const Layout l = layout(d.stride, p.tile_h, d.has_expand != 0, d.cin_p, d.cout_p, p.stages);
   AM_CHECK(l.smem == p.smem_bytes, "fused block: plan does not match the block");
   a.l = l;
 
   CUtensorMap mx, m1, m2;
-  const int hl = halo(d.stride);
-  AM_TRY(gemm::encode_map_nhwc_bf16(&mx, X, B, d.H, d.W, d.cin_p, hl, hl, true));
+  AM_TRY(gemm::encode_map_nhwc_bf16(&mx, X, B, d.H, d.W, d.cin_p, halo(d.stride), halo_h(d.stride, p.tile_h), true));
   AM_TRY(gemm::encode_map_bf16(&m2, W2, d.cmid_p, d.cout_p, d.cmid_p, (d.cout_p + 63) / 64 * 64));
   if (d.has_expand) AM_TRY(gemm::encode_map_bf16(&m1, W1, d.cin_p, d.cmid_p, d.cin_p, kChunk));
   else m1 = m2;  // unused

@@ -18,6 +18,7 @@ struct BlockDesc {
 struct Plan {
   size_t smem_bytes = 0;
   int stages = 1;  // depth of the per-chunk weight ring: as many stages as fit, up to 4
+  int tile_h = 8;  // output rows (time) of a tile, 8 columns wide: 8, or 16 at stride 1 where the ring stays as deep
 };
 
 // false when the block does not fit the kernel (Cout > 256, shared memory)

@@ -28,7 +28,10 @@ AM_API int am_probe_pipe(int op, int warps, int iters, double* cycles_per_warp_i
  *           *info = the ring depth of the plan.
  *   path 1: layer by layer through the encoder's GEMM and depthwise dispatch; *info = the depthwise kernel (0 strip,
  *           1 row, 2 fp32 generic).  E_out [B, H, W, cmid_p] and D_out [B, Ho, Wo, cmid_p] (may be NULL) receive the
- *           expanded and depthwise tensors. */
+ *           expanded and depthwise tensors.
+ *   path 2: the fused kernel's plan only, on the host (no device, no operand is read: they may be NULL);
+ *           *info = the output rows (time) of its tiles, 8 or 16 (tiles are 8 columns wide).  A block it rejects is
+ *           an error. */
 AM_API int am_debug_block(int path, int B, int H, int W, int cin_p, int cmid_p, int cout_p, int stride, int has_expand,
                           int residual, const uint16_t* X, const uint16_t* W1, const float* b1, const float* wd,
                           const float* bd, const uint16_t* W2, const float* b2, uint16_t* Y, uint16_t* E_out,

@@ -18,22 +18,23 @@ from audiomuse_ai_b200 import clap_analyzer as ca, weights  # noqa: E402
 
 WINDOWS, T, STEPS = 256, 1001, 3
 PEAK_TFLOPS, PEAK_TBS = 989.0, 3.35
-# (H, W, cin_p, cmid_p or None without expansion, cout_p, stride) of the blocks that fuse, alpha 3, T = 1001
-BLOCKS = [(501, 64, 144, None, 80, 1), (501, 64, 80, 432, 80, 2), (251, 32, 80, 416, 80, 1),
-          (251, 32, 80, 400, 144, 2), (126, 16, 144, 768, 144, 1)]
+# (H, W, cin_p, cmid_p or None without expansion, cout_p, stride, tile height) of the blocks that fuse, alpha 3,
+# T = 1001; the plan gives blocks 0 and 2 tall (16 x 8) tiles
+BLOCKS = [(501, 64, 144, None, 80, 1, 16), (501, 64, 80, 432, 80, 2, 8), (251, 32, 80, 416, 80, 1, 16),
+          (251, 32, 80, 400, 144, 2, 8), (126, 16, 144, 768, 144, 1, 8)]
 
 
-def per_window(H, W, cin_p, cmid_p, cout_p, S):
-    """(issued MMA FLOP, compulsory HBM bytes) of one window: 8 x 8 output tiles, the expansion over the halo pixels
-    rounded up to 8-pixel atoms (its N) with the K steps of 16 past cin_p skipped, the projection over cout_p columns
-    (two halves of cout_p / 2)."""
+def per_window(H, W, cin_p, cmid_p, cout_p, S, th):
+    """(issued MMA FLOP, compulsory HBM bytes) of one window: th x 8 output tiles, the expansion over the halo pixels
+    ((th - 1) S + 3 rows of 7 S + 3, 184 per 128 outputs for the tall tile) rounded up to 8-pixel atoms (its N) with
+    the K steps of 16 past cin_p skipped, the projection over the tile's pixels and cout_p columns."""
     Ho, Wo = (H - 1) // S + 1, (W - 1) // S + 1
-    tiles = math.ceil(Ho / 8) * math.ceil(Wo / 8)
-    hp = math.ceil(((7 * S + 3) ** 2) / 8) * 8
+    tiles = math.ceil(Ho / th) * math.ceil(Wo / 8)
+    hp = math.ceil((((th - 1) * S + 3) * (7 * S + 3)) / 8) * 8
     cm = cmid_p or cin_p
     chunks = math.ceil(cm / 64)
     expand = 0 if cmid_p is None else 2 * hp * 64 * chunks * cin_p
-    project = 2 * 64 * cout_p * cm
+    project = 2 * th * 8 * cout_p * cm
     return tiles * (expand + project), 2 * (H * W * cin_p + Ho * Wo * cout_p)
 
 
