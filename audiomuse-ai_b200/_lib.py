@@ -56,6 +56,7 @@ class SimilarCfg(C.Structure):
 
 
 ALCHEMY_MAX_N, ALCHEMY_MAX_CANDIDATES = 600, 3000   # AM_ALCHEMY_MAX_N, AM_ALCHEMY_MAX_CANDIDATES
+KMEANS_BATCH_MAX_KD, KMEANS_BATCH_MAX_ROWS = 24576, 1 << 20   # AM_KMEANS_BATCH_MAX_KD, AM_KMEANS_BATCH_MAX_ROWS
 
 
 _vp, _i, _i64, _f, _u64, _sz = C.c_void_p, C.c_int, C.c_int64, C.c_float, C.c_uint64, C.c_size_t
@@ -121,6 +122,7 @@ SIGNATURES = {
     "am_knn_get_vectors": (_i, [_vp, _vp, _i, _vp]),
     "am_knn_query_dev": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _vp]),
     "am_kmeans_fit": (_i, [_vp, _i64, _i, _i, _i, _i, _f, _u64, _vp, _vp, _vp, _P(_f), _P(_i)]),
+    "am_kmeans_fit_batch": (_i, [_vp, _vp, _i64, _vp, _vp, _i, _i, _i, _f, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "am_pca_moments": (_i, [_vp, _i64, _i, _vp, _vp]),
     "am_pca_project": (_i, [_vp, _i64, _i, _vp, _vp, _i, _vp]),
     "am_dbscan": (_i, [_vp, _i64, _i, C.c_double, _i, _vp, _P(_i)]),

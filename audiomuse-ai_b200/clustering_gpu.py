@@ -6,7 +6,8 @@
     get_clustering_model('kmeans', {'n_clusters': k}, use_gpu)          :338-404
 
 cuML is replaced by am_kmeans_fit (k-means++ D^2 seeding, n_init restarts, Lloyd with sklearn's
-tol rule).  The reference silently falls back to sklearn when the GPU path raises (:130-148);
+tol rule).  kmeans_fit_batch fits many small problems at once (am_kmeans_fit_batch: one CTA per (problem, init), the
+same definition and seeds as am_kmeans_fit), for the clustering task's batches of iterations.  The reference silently falls back to sklearn when the GPU path raises (:130-148);
 here that fallback exists only when ``B200_ALLOW_SKLEARN_FALLBACK=1`` (default: fail loudly,
 so a missing CUDA library can never masquerade as the GPU path).
 
@@ -71,6 +72,70 @@ def kmeans_fit(X, k, n_init=10, max_iter=300, tol=1e-4, seed=0, init_centers=Non
                                  int(seed) & 0xFFFFFFFFFFFFFFFF, None if init is None else _lib.ptr(init),
                                  _lib.ptr(centers), _lib.ptr(labels), C.byref(inertia), C.byref(n_iter)))
     return centers, labels, float(inertia.value), int(n_iter.value)
+
+
+def kmeans_batch_serves(N, d, k):
+    """True when am_kmeans_fit_batch holds the shape (centres and sums in one CTA's shared memory); larger problems
+    go to am_kmeans_fit"""
+    return N <= _lib.KMEANS_BATCH_MAX_ROWS and max(k, 8) * (d + 1) <= _lib.KMEANS_BATCH_MAX_KD
+
+
+def kmeans_fit_batch(problems, k, n_init=10, max_iter=300, tol=1e-4, seeds=0, intermediates=False):
+    """Many independent k-means fits at once.  problems: a sequence of [N_p, d_p] arrays; k and seeds: one value for
+    every problem or one per problem.  -> one (centers f32[k, d], labels i32[N], inertia, n_iter) per problem, each
+    kmeans_fit(problem, k, n_init, max_iter, tol, seed)'s definition; with intermediates, a fifth entry: the k-means++
+    rows i32[n_init, k] (None for a problem am_kmeans_fit serves).  Problems am_kmeans_fit_batch holds run together
+    on the device (am_kmeans_fit_batch); the others one by one through kmeans_fit.  Every input is checked, with
+    scikit-learn's ValueError wording, before any device work."""
+    Xs = [_finite_f32(X) for X in problems]
+    P = len(Xs)
+    ks = [int(k)] * P if np.ndim(k) == 0 else [int(v) for v in k]
+    sd = [int(seeds)] * P if np.ndim(seeds) == 0 else [int(v) for v in seeds]
+    if len(ks) != P or len(sd) != P:
+        raise ValueError(f"k and seeds need one value per problem ({P})")
+    for X, kk in zip(Xs, ks):
+        N, d = X.shape
+        if d < 1:
+            raise ValueError(f"Found array with 0 feature(s) (shape={X.shape}) while a minimum of 1 is required "
+                             "by KMeans.")
+        if kk < 1:
+            raise ValueError(f"The 'n_clusters' parameter of KMeans must be an int in the range [1, inf). Got {kk} "
+                             "instead.")
+        if N < kk:
+            raise ValueError(f"n_samples={N} should be >= n_clusters={kk}.")
+    if n_init < 1 or max_iter < 1:
+        raise ValueError("n_init and max_iter must be >= 1")
+    out = [None] * P
+    batch = [p for p in range(P) if kmeans_batch_serves(Xs[p].shape[0], Xs[p].shape[1], ks[p])]
+    for p in range(P):
+        if p not in batch:
+            r = kmeans_fit(Xs[p], ks[p], n_init=n_init, max_iter=max_iter, tol=tol, seed=sd[p])
+            out[p] = r + (None,) if intermediates else r
+    if not batch:
+        return out
+    ns = np.array([Xs[p].shape[0] for p in batch], np.int64)
+    ds = np.array([Xs[p].shape[1] for p in batch], np.int32)
+    kb = np.array([ks[p] for p in batch], np.int32)
+    row_off = np.concatenate([[0], np.cumsum(ns)]).astype(np.int64)
+    cen_off = np.concatenate([[0], np.cumsum(kb.astype(np.int64) * ds)]).astype(np.int64)
+    kpp_off = np.concatenate([[0], np.cumsum(kb.astype(np.int64) * n_init)]).astype(np.int64)
+    rows = np.ascontiguousarray(np.concatenate([Xs[p].ravel() for p in batch]))
+    seeds_u = np.array([sd[p] & 0xFFFFFFFFFFFFFFFF for p in batch], np.uint64)
+    centers = np.empty(int(cen_off[-1]), np.float32)
+    labels = np.empty(int(row_off[-1]), np.int32)
+    inertia = np.empty(len(batch), np.float32)
+    n_iter = np.empty(len(batch), np.int32)
+    kpp = np.empty(int(kpp_off[-1]), np.int32) if intermediates else None
+    lib = _lib.load()
+    _lib.check(lib.am_kmeans_fit_batch(_lib.ptr(rows), _lib.ptr(row_off), int(row_off[-1]), _lib.ptr(ds), _lib.ptr(kb),
+                                       len(batch), int(n_init), int(max_iter), float(tol), _lib.ptr(seeds_u),
+                                       _lib.ptr(centers), _lib.ptr(cen_off), _lib.ptr(labels), _lib.ptr(inertia),
+                                       _lib.ptr(n_iter), None if kpp is None else _lib.ptr(kpp)))
+    for i, p in enumerate(batch):
+        r = (centers[cen_off[i]:cen_off[i + 1]].reshape(kb[i], ds[i]).copy(),
+             labels[row_off[i]:row_off[i + 1]].copy(), float(inertia[i]), int(n_iter[i]))
+        out[p] = r + (kpp[kpp_off[i]:kpp_off[i + 1]].reshape(n_init, kb[i]).copy(),) if intermediates else r
+    return out
 
 
 class GPUKMeans:

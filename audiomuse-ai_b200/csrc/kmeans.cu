@@ -15,6 +15,7 @@
 #include "common.cuh"
 #include "gemm_wgmma.cuh"
 #include "host_call.cuh"
+#include "kmeans_common.cuh"
 #include "kmeans_tc.cuh"
 
 #include <algorithm>
@@ -26,9 +27,7 @@ __global__ void center_norms_kernel(const float* __restrict__ C, int k, int d, f
   const int j = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
   if (j >= k) return;
-  float acc = 0.f;
-  for (int i = lane; i < d; i += 32) acc = fmaf(C[(int64_t)j * d + i], C[(int64_t)j * d + i], acc);
-  acc = warp_sum(acc);
+  const float acc = warp_sq_norm(C + (int64_t)j * d, d, lane);
   if (lane == 0) cn[j] = acc;
 }
 
@@ -45,9 +44,7 @@ assign_kernel(const float* __restrict__ X, int64_t N, int d, const float* __rest
     const float* x = X + row * d;
     float best = INFINITY;
     int best_j = 0;
-    float xn = 0.f;
-    for (int i = lane; i < d; i += 32) xn = fmaf(x[i], x[i], xn);
-    xn = warp_sum(xn);
+    const float xn = warp_sq_norm(x, d, lane);
     for (int j = 0; j < k; ++j) exact_argmin<1, 1>(x, d, C, cn, k, lane, j, best, best_j);
     if (lane == 0) {
       labels[row] = best_j;
@@ -162,20 +159,15 @@ pp_update_kernel(const float* __restrict__ X, int64_t N, int d, const float* __r
                  float* __restrict__ mind2, double* __restrict__ block_sums) {
   __shared__ double s_part[8];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const int64_t base = (int64_t)blockIdx.x * 1024;
+  const int64_t base = (int64_t)blockIdx.x * kKppBlock;
   double part = 0.0;
-  for (int r = warp; r < 1024; r += 8) {
+  for (int r = warp; r < kKppBlock; r += 8) {
     const int64_t row = base + r;
     if (row >= N) break;
-    const float* x = X + row * d;
-    float acc = 0.f;
-    for (int i = lane; i < d; i += 32) {
-      const float df = x[i] - __ldg(&c[i]);
-      acc = fmaf(df, df, acc);
-    }
-    acc = warp_sum(acc);
+    float acc[1];
+    d2_chains<1>(X + row * d, c, 0, 1, d, lane, acc);
     if (lane == 0) {
-      const float m = first ? acc : fminf(mind2[row], acc);
+      const float m = first ? acc[0] : fminf(mind2[row], acc[0]);
       mind2[row] = m;
       part += (double)m;
     }
@@ -191,41 +183,24 @@ pp_update_kernel(const float* __restrict__ X, int64_t N, int d, const float* __r
 
 // greedy k-means++ (sklearn's _kmeans_plusplus): for each of L candidate rows, the potential
 // sum_i min(mind2[i], ||x_i - c_l||^2); per-block partial sums -> block_pot[block][L]
-constexpr int kMaxTrials = 8;
 __global__ void __launch_bounds__(256)
 pp_trial_kernel(const float* __restrict__ X, int64_t N, int d, const float* __restrict__ cand, int L,
                 const float* __restrict__ mind2, double* __restrict__ block_pot) {
   __shared__ double s_part[8][kMaxTrials];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const int64_t base = (int64_t)blockIdx.x * 1024;
+  const int64_t base = (int64_t)blockIdx.x * kKppBlock;
   double part[kMaxTrials];
 #pragma unroll
   for (int l = 0; l < kMaxTrials; ++l) part[l] = 0.0;
-  for (int r = warp; r < 1024; r += 8) {
+  for (int r = warp; r < kKppBlock; r += 8) {
     const int64_t row = base + r;
     if (row >= N) break;
-    const float* x = X + row * d;
     float acc[kMaxTrials];
-#pragma unroll
-    for (int l = 0; l < kMaxTrials; ++l) acc[l] = 0.f;
-    for (int i = lane; i < d; i += 32) {
-      const float xv = x[i];
-#pragma unroll
-      for (int l = 0; l < kMaxTrials; ++l) {
-        if (l < L) {
-          const float df = xv - __ldg(&cand[(int64_t)l * d + i]);
-          acc[l] = fmaf(df, df, acc[l]);
-        }
-      }
-    }
+    d2_chains<kMaxTrials>(X + row * d, cand, d, L, d, lane, acc);
     const float m = mind2[row];
 #pragma unroll
-    for (int l = 0; l < kMaxTrials; ++l) {
-      if (l < L) {
-        const float v = warp_sum(acc[l]);
-        part[l] += (double)fminf(m, v);
-      }
-    }
+    for (int l = 0; l < kMaxTrials; ++l)
+      if (l < L) part[l] += (double)fminf(m, acc[l]);
   }
   if (lane == 0) {
 #pragma unroll
@@ -238,17 +213,6 @@ pp_trial_kernel(const float* __restrict__ X, int64_t N, int d, const float* __re
     block_pot[(int64_t)blockIdx.x * kMaxTrials + threadIdx.x] = t;
   }
 }
-
-struct SplitMix {
-  uint64_t s;
-  uint64_t next() {
-    uint64_t z = (s += 0x9e3779b97f4a7c15ull);
-    z = (z ^ (z >> 30)) * 0xbf58476d1ce4e5b9ull;
-    z = (z ^ (z >> 27)) * 0x94d049bb133111ebull;
-    return z ^ (z >> 31);
-  }
-  double uniform() { return (double)(next() >> 11) * (1.0 / 9007199254740992.0); }
-};
 
 static int launch_accumulate(const float* X, int64_t N, int d, const int32_t* labels, int k, float* sums,
                              cudaStream_t st) {
@@ -367,14 +331,8 @@ static int scaled_tolerance(const float* X, int64_t N, int d, float tol, cudaStr
   std::vector<double> hm((size_t)2 * d);
   AM_CUDA(cudaMemcpyAsync(hm.data(), mom.p, hm.size() * 8, cudaMemcpyDeviceToHost, st));
   AM_CUDA(cudaStreamSynchronize(st));
-  double var_mean = 0.0;
   mean.resize((size_t)d);
-  for (int c = 0; c < d; ++c) {
-    const double mu = hm[c] / N;
-    var_mean += hm[d + c] / N - mu * mu;
-    mean[(size_t)c] = (float)mu;
-  }
-  *tol_abs = var_mean / d * tol;
+  *tol_abs = kmeans_tol_abs(hm.data(), hm.data() + d, N, d, tol, mean.data());
   return AM_OK;
 }
 
@@ -382,10 +340,10 @@ static int scaled_tolerance(const float* X, int64_t N, int d, float tol, cudaStr
 // mind2 f32[N], bsum f64[nblk], cand f32[kMaxTrials, d], bpot f64[nblk, kMaxTrials] (nblk 1024-row blocks)
 static int kmeanspp_seed(const float* X, int64_t N, int d, int k, SplitMix& rng, float* C, float* mind2,
                          double* bsum, float* cand, double* bpot, cudaStream_t st) {
-  const int64_t nblk = (N + 1023) / 1024;
+  const int64_t nblk = (N + kKppBlock - 1) / kKppBlock;
   std::vector<double> hbs(nblk), hpot((size_t)nblk * kMaxTrials);
-  std::vector<float> hblock(1024);
-  const int L = std::min(kMaxTrials, 2 + (int)std::log((double)k));
+  std::vector<float> hblock(kKppBlock);
+  const int L = kpp_trials(k);
   int64_t pick = std::min<int64_t>((int64_t)(rng.uniform() * N), N - 1);
   AM_CUDA(cudaMemcpyAsync(C, X + (size_t)pick * d, (size_t)d * 4, cudaMemcpyDeviceToDevice, st));
   AM_LAUNCH(pp_update_kernel, (unsigned)nblk, 256, 0, st, X, N, d, C, 1, mind2, bsum);
@@ -397,20 +355,10 @@ static int kmeanspp_seed(const float* X, int64_t N, int d, int k, SplitMix& rng,
     int64_t cand_row[kMaxTrials];
     for (int l = 0; l < L; ++l) {
       double r = rng.uniform() * total;
-      int64_t b = 0;
-      for (; b < nblk - 1; ++b) {
-        if (r < hbs[b]) break;
-        r -= hbs[b];
-      }
-      const int64_t b0 = b * 1024, cnt = std::min<int64_t>(1024, N - b0);
+      const int64_t b0 = kpp_scan(hbs.data(), nblk, r) * kKppBlock, cnt = std::min<int64_t>(kKppBlock, N - b0);
       AM_CUDA(cudaMemcpyAsync(hblock.data(), mind2 + b0, cnt * 4, cudaMemcpyDeviceToHost, st));
       AM_CUDA(cudaStreamSynchronize(st));
-      int64_t o = 0;
-      for (; o < cnt - 1; ++o) {
-        if (r < hblock[o]) break;
-        r -= hblock[o];
-      }
-      cand_row[l] = b0 + o;
+      cand_row[l] = b0 + kpp_scan(hblock.data(), cnt, r);
       AM_CUDA(cudaMemcpyAsync(cand + (size_t)l * d, X + (size_t)cand_row[l] * d, (size_t)d * 4,
                               cudaMemcpyDeviceToDevice, st));
     }
@@ -468,7 +416,7 @@ static int lloyd(am_kmeans_plan& step, int max_iter, double tol_abs, float* C, i
       std::vector<int64_t> order((size_t)N);
       for (int64_t i = 0; i < N; ++i) order[(size_t)i] = i;
       std::partial_sort(order.begin(), order.begin() + (int64_t)empty.size(), order.end(), [&](int64_t a, int64_t b) {
-        return hdist[(size_t)a] > hdist[(size_t)b] || (hdist[(size_t)a] == hdist[(size_t)b] && a < b);
+        return relocate_before(hdist[(size_t)a], a, hdist[(size_t)b], b);
       });
       AM_TRY(far_dev.alloc(empty.size()));
       AM_TRY(empty_dev.alloc(empty.size()));
@@ -497,7 +445,7 @@ extern "C" int am_kmeans_fit(const float* X, int64_t N, int d, int k, int n_init
   AM_CHECK(max_iter > 0 && n_init > 0, "am_kmeans_fit: max_iter and n_init must be positive");
   cudaStream_t st;
   AM_TRY(HostCall::thread_stream(&st));
-  const int64_t nblk = (N + 1023) / 1024;
+  const int64_t nblk = (N + kKppBlock - 1) / kKppBlock;
   HostCall call(st, 0, HostCall::Memory::Owned);
   float *dX, *dC, *dBestC, *sums, *counts, *dist, *mind2, *cand, *dmean;
   int32_t *dL, *dBestL;
@@ -528,7 +476,7 @@ extern "C" int am_kmeans_fit(const float* X, int64_t N, int d, int k, int n_init
   am_kmeans_plan step{dX, N, d, k};
   AM_TRY(step.create(kmeans_use_tensor_cores(N, d, k, KMeansUse::kFit), st));
 
-  SplitMix rng{seed ^ 0x5851f42d4c957f2dull};
+  SplitMix rng{seed ^ kKmeansSeedMix};
   double best_inertia = INFINITY;
   int best_iters = 0;
   for (int run = 0; run < (init_centers ? 1 : n_init); ++run) {

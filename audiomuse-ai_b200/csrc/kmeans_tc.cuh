@@ -15,8 +15,15 @@ bool kmeans_use_tensor_cores(int64_t N, int d, int k, KMeansUse use);
 // The exact fp32 argmin of row x over centres j0 + kStep u, u < NC (those >= k skipped), by a whole warp: each lane
 // takes features lane, lane + 32, ... with fmaf, one warp_sum tree per centre, v_j = cn_j - 2 x.c_j, and a strict "<"
 // in increasing j (the lowest index wins ties).  assign_kernel and recheck_kernel both decide with it, which is why a
-// row the tensor-core step rechecks gets the CUDA-core label.
-template <int NC, int kStep>
+// row the tensor-core step rechecks gets the CUDA-core label.  kLdg = false reads C with plain loads, for
+// centres in shared memory or written by the same kernel (kmeans_batch.cu); the arithmetic is the same.
+template <bool kLdg>
+__device__ __forceinline__ float ld_centre(const float* p) {
+  if constexpr (kLdg) return __ldg(p);
+  else return *p;
+}
+
+template <int NC, int kStep, bool kLdg = true>
 __device__ __forceinline__ void exact_argmin(const float* x, int d, const float* C, const float* cn, int k, int lane,
                                              int j0, float& best, int& best_j) {
   float acc[NC] = {};
@@ -27,7 +34,7 @@ __device__ __forceinline__ void exact_argmin(const float* x, int d, const float*
 #pragma unroll
     for (int u = 0; u < NC; ++u) {
       const int j = j0 + kStep * u;
-      if (j < k) acc[u] = fmaf(xv, __ldg(NC == 1 ? &c0[i] : &C[(int64_t)j * d + i]), acc[u]);
+      if (j < k) acc[u] = fmaf(xv, ld_centre<kLdg>(NC == 1 ? &c0[i] : &C[(int64_t)j * d + i]), acc[u]);
     }
   }
   float b = best;

@@ -160,7 +160,7 @@ def apply(clap=None, voyager_manager=None, clustering=None, allow_sklearn_fallba
           clustering_helper=None, song_alchemy=None, app_map=None, artist_gmm_manager=None,
           gaussian_mixture=None, radius_walk=None, path_manager=None, app_path=None, analysis=None, alchemy=None,
           app_alchemy=None, similar=None, app_voyager=None, sonic_fingerprint=None,
-          gmm_all_covariance_types: bool = False, clap_text=None) -> None:
+          gmm_all_covariance_types: bool = False, clap_text=None, clustering_batch=None) -> None:
     """clap / voyager_manager / clustering / clustering_helper: the reference's already imported tasks.* modules (pass
     only the ones to patch).  allow_sklearn_fallback keeps the reference's contract that a failing GPU k-means silently
     falls back to scikit-learn (tasks/clustering_gpu.py:130-148); this repository's own tests run with it off so a
@@ -197,7 +197,13 @@ def apply(clap=None, voyager_manager=None, clustering=None, allow_sklearn_fallba
     embeddings and get_text_embeddings_batch run on the device while the tokenizer, get_text_embedding and
     search_by_text stay the reference's.  With clap= as well, the installed unload_clap_model and is_clap_model_loaded
     also close and clear the module's _text_session (and its tokenizer, as the reference's unload does), so the idle
-    unload timer frees the text model too."""
+    unload timer frees the text model too.  clustering_batch (the reference's tasks.clustering) gets
+    clustering_batch.make_run_clustering_batch_task as run_clustering_batch_task: RQ resolves
+    'tasks.clustering.run_clustering_batch_task' by name when a batch job runs (clustering.py:884-887), and the drop-in
+    fits a batch's k-means iterations in one device pass.  It builds the reference's GPUKMeans, so clustering= must
+    be passed too."""
+    if clustering_batch is not None and clustering is None:
+        raise ValueError("clustering_batch= builds the device GPUKMeans that clustering= installs: pass both")
     if gmm_all_covariance_types and gaussian_mixture is None:
         raise ValueError("gmm_all_covariance_types= selects the class installed by gaussian_mixture=: pass both")
     if analysis is not None:
@@ -258,6 +264,11 @@ def apply(clap=None, voyager_manager=None, clustering=None, allow_sklearn_fallba
         clustering.GPUPCA = b200_cg.GPUPCA
         clustering.GPUSpectralClustering = b200_cg.GPUSpectralClustering
         clustering.check_gpu_available = b200_cg.check_gpu_available
+    if clustering_batch is not None:
+        from . import clustering_batch as b200_cb
+
+        clustering_batch.run_clustering_batch_task = b200_cb.make_run_clustering_batch_task(
+            clustering_batch, sys.modules[clustering_batch._perform_single_clustering_iteration.__module__])
     if gaussian_mixture is not None:
         from . import clustering_gpu as b200_cg
 

@@ -358,6 +358,25 @@ AM_API int am_kmeans_fit(const float* X, int64_t N, int d, int k, int n_init, in
 AM_API int am_kmeans_assign_dev(const float* X_dev, int64_t N, int d, const float* centers_dev, int k,
                          int32_t* labels_dev, float* sums_dev, float* counts_dev,
                          float* inertia_dev, void* stream);
+/* Many small k-means fits at once: the clustering task's RQ batches (tasks/clustering.py:175-227, one
+ * KMeans(k, init='k-means++', n_init=10) per iteration through tasks/clustering_helper.py:261-335).  Problem p has
+ * N_p = row_offsets[p + 1] - row_offsets[p] rows of dims[p] features, packed row-major after problem p - 1's
+ * (row_offsets i64[n_problems + 1] from 0 to n_rows), k = ks[p] and seed seeds[p].  Each problem's centres
+ * f32[k, d] land at centers + center_offsets[p] (center_offsets i64[n_problems + 1], steps of k * d), its labels i32 at
+ * labels + row_offsets[p], inertia f32[p] and n_iter i32[p]; kpp_rows (optional) receives the k-means++ rows,
+ * i32[n_init, k] per problem, problem after problem.  Every problem's result is am_kmeans_fit's definition with the
+ * same seed (column-mean shift, sklearn's tolerance, greedy k-means++ on the same SplitMix draws, Lloyd with
+ * sklearn's empty-cluster rule, the first init with the strictly lowest inertia), computed by one CTA per
+ * (problem, init) with every reduction in a fixed order: deterministic, and independent of the other problems of
+ * the batch.  Limits per problem: 1 <= k <= N <= AM_KMEANS_BATCH_MAX_ROWS, d >= 1 and
+ * max(k, 8) * (d + 1) <= AM_KMEANS_BATCH_MAX_KD (centres and sums in shared memory); AM_ERR_INVALID beyond them, as for
+ * NaN / inf rows.  am_kmeans_fit serves larger problems. */
+#define AM_KMEANS_BATCH_MAX_KD 24576
+#define AM_KMEANS_BATCH_MAX_ROWS 1048576
+AM_API int am_kmeans_fit_batch(const float* rows, const int64_t* row_offsets, int64_t n_rows, const int32_t* dims,
+                               const int32_t* ks, int n_problems, int n_init, int max_iter, float tol,
+                               const uint64_t* seeds, float* centers, const int64_t* center_offsets, int32_t* labels,
+                               float* inertia, int32_t* n_iter, int32_t* kpp_rows);
 
 /* ------------------------------------------------------------------ PCA / DBSCAN (SURVEY 8(f4))
  * Replace cuml.decomposition.PCA / cuml.cluster.DBSCAN behind GPUPCA / GPUDBSCAN (tasks/clustering_gpu.py:151-278);
